@@ -29,10 +29,17 @@ constexpr int BLOCK_K = 64;          // 64 bf16 = one 128-byte swizzle span
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;        // 16 KiB
 constexpr int NUM_THREADS = 384;
 constexpr int CS_MAX = 1024;         // DGRAD column sums are gathered in shared memory: N <= CS_MAX
-// operand ring depth per tile width: the ring fills ~192 KB of the 227 KB of shared memory
-constexpr int gemm_stages(int bn) { return bn == 256 ? 4 : bn == 128 ? 6 : 8; }
-constexpr int smem_bytes(int bn) {
-  return gemm_stages(bn) * (A_STAGE_BYTES + bn * BLOCK_K * 2) + CS_MAX * 4 + 256 /*barriers*/ + 1024 /*align*/;
+// TS: the bf16 output tile is staged in shared memory (BN / 64 blocks of [128 rows x 64 cols], 128-byte swizzle)
+// and written by TMA bulk stores, which leave coalesced full lines and run while the next tile's main loop does.
+// The staging tile takes the place of ring stages: 64 KB at BN = 256 leaves room for 3 stages.
+constexpr int staging_bytes(int bn, bool ts) { return ts ? BLOCK_M * bn * 2 : 0; }
+// operand ring depth per tile width: the ring and the staging tile fill up to ~210 KB of the 227 KB of shared memory
+constexpr int gemm_stages(int bn, bool ts) {
+  return ts ? (bn == 256 ? 3 : bn == 128 ? 5 : 8) : (bn == 256 ? 4 : bn == 128 ? 6 : 8);
+}
+constexpr int smem_bytes(int bn, bool ts) {
+  return gemm_stages(bn, ts) * (A_STAGE_BYTES + bn * BLOCK_K * 2) + staging_bytes(bn, ts) + CS_MAX * 4 +
+         256 /*barriers*/ + 1024 /*align*/;
 }
 
 struct GemmParams {
@@ -57,11 +64,11 @@ struct GemmParams {
 
 // Accumulator fragment of wgmma m64nBN (per consumer thread): acc[4i + 2h + e] is row 16*warp + lane/4 + 8h,
 // column 8i + 2*(lane%4) + e of the warpgroup's 64 x BN tile.
-template <int MODE, int BN>
+template <int MODE, int BN, bool TS>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-               const GemmParams p) {
-  constexpr int STAGES = gemm_stages(BN);
+               const __grid_constant__ CUtensorMap tmap_c, const GemmParams p) {
+  constexpr int STAGES = gemm_stages(BN, TS);
   constexpr int B_STAGE = BN * BLOCK_K * 2;
   constexpr bool kWgrad = (MODE == MNRF_GEMM_WGRAD);
   constexpr int NACC = BN / 2;
@@ -69,7 +76,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_b + STAGES * B_STAGE);   // [STAGES]
+  uint8_t* smem_c = smem_b + STAGES * B_STAGE;                                   // TS: output staging tile
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_c + staging_bytes(BN, TS));  // [STAGES]
   uint64_t* empty_bar = full_bar + STAGES;                                       // [STAGES]
   float* cs_s = reinterpret_cast<float*>(empty_bar + STAGES);                    // [CS_MAX] DGRAD column sums
 
@@ -82,6 +90,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_b);
+    if (TS) prefetch_tmap(&tmap_c);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 8);     // one arrival per consumer warp
@@ -187,6 +196,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         }
         continue;
       }
+      if (TS) {
+        // the previous tile's bulk stores must have finished reading the staging rows of this warpgroup
+        if ((threadIdx.x & 127) == 0) tma_store_wait_read<0>();
+        named_bar_sync(2 + c, 128);
+      }
+      const uint32_t c_row = smem_u32(smem_c) + r_in * 128 + (cq << 1);   // TS: this thread's staging row (h = 0)
       int64_t rows[2];
       bool row_ok[2];
       float rv[2] = {0.f, 0.f};
@@ -255,10 +270,16 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           }
         }
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
-          if (row_ok[h])
+        for (int h = 0; h < 2; ++h) {
+          if (TS) {
+            // [128 x 64] block i / 8, row r_in + 8h, 16-byte chunk (i % 8) ^ (row % 8), byte 2 * cq
+            st_shared_u32(c_row + h * (8 * 128) + (i >> 3) * (BLOCK_M * 128) + (((i & 7) ^ ((lane >> 2) & 7)) << 4),
+                          pack_bf16(v[h][0], v[h][1]));
+          } else if (row_ok[h]) {
             *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + rows[h] * p.ldc + col) =
                 pack_bf16(v[h][0], v[h][1]);
+          }
+        }
         if (MODE == MNRF_GEMM_FWD && p.act == MNRF_ACT_RELU && p.maskbits && (i & 3) == 3) {
           // one 32-column mask word per row: the four lanes of a quad hold its 32 bits between them
 #pragma unroll
@@ -270,7 +291,20 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           }
         }
       }
+      if (TS) {
+        // TMA clips the rows past M
+        fence_proxy_async();                    // generic-proxy writes -> visible to the bulk store (async proxy)
+        named_bar_sync(2 + c, 128);
+        if ((threadIdx.x & 127) == 0) {   // one thread per warpgroup issues its bulk stores
+#pragma unroll
+          for (int j = 0; j < BN / 64; ++j)
+            tma_store_2d(&tmap_c, smem_c + j * (BLOCK_M * 128) + c * (64 * 128), ncol0 + 64 * j,
+                         (int)((int64_t)m_blk * BLOCK_M + 64 * c));
+          tma_store_commit();
+        }
+      }
     }
+    if (TS && (threadIdx.x & 127) == 0) tma_store_wait_all();
     if (do_cs) {
       named_bar_sync(1, 2 * 128);               // both consumer warpgroups are done with the shared sums
       for (int i = threadIdx.x - 128; i < p.n; i += 2 * 128) atomicAdd(p.colsum + i, cs_s[i]);
@@ -350,7 +384,10 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
     MNRF_CHECK(d->ldc % 2 == 0 && ((uintptr_t)out % 8) == 0, "mnrf_gemm(tc): fp32 output must be 8-byte aligned");
   }
 
-  CUtensorMap ta, tb;
+  // The bf16 output goes through the staged bulk store when its tiles are whole 128-byte swizzle spans and TMA can
+  // address it (16-byte aligned base and row pitch); otherwise the epilogue stores from registers.
+  const bool ts = d->mode != MNRF_GEMM_WGRAD && block_n >= 64 && ((uintptr_t)out % 16) == 0 && d->ldc % 8 == 0;
+  CUtensorMap ta, tb, tc;
   if (d->mode != MNRF_GEMM_WGRAD) {
     if (make_tmap(&ta, a, d->m, d->k, d->lda, BLOCK_K, BLOCK_M)) return 1;
     if (make_tmap(&tb, b, d->n, d->k, d->ldb, BLOCK_K, block_n)) return 1;
@@ -359,15 +396,20 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
     if (make_tmap(&ta, a, d->k, d->m, d->lda, 64, BLOCK_K)) return 1;
     if (make_tmap(&tb, b, d->k, d->n, d->ldb, 64, BLOCK_K)) return 1;
   }
+  if (ts) {
+    if (make_tmap(&tc, out, d->m, d->n, d->ldc, 64, 64)) return 1;
+  } else {
+    tc = tb;   // not read
+  }
   const int total_tiles = p.num_m_blocks * p.num_n_blocks * p.num_splits;
   const int grid = std::min(total_tiles, workers);
   if (grid == 0) return 0;
-#define MNRF_LAUNCH_TC2(MODE_, BN_)                                                                   \
+#define MNRF_LAUNCH_TC3(MODE_, BN_, TS_)                                                              \
   do {                                                                                                \
     static bool attr_set = false;                                                                     \
-    constexpr int kSmem = smem_bytes(BN_);                                                            \
+    constexpr int kSmem = smem_bytes(BN_, TS_);                                                       \
     static_assert(kSmem <= 232448, "shared memory budget");                                           \
-    auto kern = gemm_tc_kernel<MODE_, BN_>;                                                           \
+    auto kern = gemm_tc_kernel<MODE_, BN_, TS_>;                                                      \
     if (!attr_set) {                                                                                  \
       MNRF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));      \
       attr_set = true;                                                                                \
@@ -379,7 +421,12 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                                  \
     attr[0].val.programmaticStreamSerializationAllowed = 1;                                           \
     cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;                                           \
-    MNRF_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, p));                                             \
+    MNRF_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, tc, p));                                         \
+  } while (0)
+#define MNRF_LAUNCH_TC2(MODE_, BN_)                                                                   \
+  do {                                                                                                \
+    if (ts) MNRF_LAUNCH_TC3(MODE_, BN_, MODE_ != MNRF_GEMM_WGRAD && BN_ >= 64);                       \
+    else MNRF_LAUNCH_TC3(MODE_, BN_, false);                                                          \
   } while (0)
 #define MNRF_LAUNCH_TC(MODE_)                                                                         \
   do {                                                                                                \

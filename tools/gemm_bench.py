@@ -3,7 +3,8 @@
   python tools/gemm_bench.py [--rows 1048576]
 
 Prints ms / TFLOP/s / GB/s per (mode, N, K, features) so epilogue features can be costed in
-isolation (each timing: 20 launches after 3 warm-ups, inputs larger than L2).
+isolation (each timing: 20 launches after 3 warm-ups, inputs larger than L2), and beside each GEMM the rate of
+torch.matmul (cuBLAS, bf16 output) on the same operands as a yardstick of what the card attains at that shape.
 """
 import argparse
 import os
@@ -87,7 +88,10 @@ def main():
   torch.manual_seed(0)
   if args.bottleneck:
     return bottleneck(dev, args.rows // 2)
-  for (M, N, K) in [(args.rows, 256, 256), (args.rows, 256, 512), (args.rows // 2, 1024, 1024)]:
+  # the PropMLP trunk, the NerfMLP trunk and its skip layer (K = 1536: FWD and the [1536, 1024] WGRAD; its DGRAD
+  # output is 1536 wide, past the fused column sums' limit, and runs split at the concat in the model)
+  for (M, N, K) in [(args.rows, 256, 256), (args.rows, 256, 512), (args.rows // 2, 1024, 1024),
+                    (args.rows // 2, 1024, 1536)]:
     x = (torch.randn(M, K, device=dev) * 0.5).bfloat16()
     w_nk = (torch.randn(N, K, device=dev) * 0.05).bfloat16()
     w_kn = w_nk.t().contiguous()
@@ -101,21 +105,26 @@ def main():
     cs = torch.zeros(K, device=dev)
     flops = 2.0 * M * N * K
 
-    def report(name, ms, nbytes):
+    def report(name, ms, nbytes, torch_ms=None):
+      ref = f'  torch.matmul {flops / torch_ms / 1e9:7.1f} TFLOP/s' if torch_ms else ''
       print(f'M={M} N={N} K={K} {name:28s} {ms:7.3f} ms  {flops / ms / 1e9:7.1f} TFLOP/s  '
-            f'{nbytes / ms / 1e6:7.1f} GB/s', flush=True)
+            f'{nbytes / ms / 1e6:7.1f} GB/s{ref}', flush=True)
 
+    t_fwd = timeit(lambda: torch.matmul(x, w_nk.t(), out=y))
     ms = timeit(lambda: ops.gemm(L.GEMM_FWD, x, w_nk, y, m=M, n=N, k=K, act=L.ACT_RELU, bias=bias,
                                  maskbits=bits))
-    report('fwd bias+relu+bits', ms, 2.0 * M * (N + K))
-    ms = timeit(lambda: ops.gemm(L.GEMM_DGRAD, dy, w_kn, dx, m=M, n=K, k=N))
-    report('dgrad plain', ms, 2.0 * M * (N + K))
-    ms = timeit(lambda: ops.gemm(L.GEMM_DGRAD, dy, w_kn, dx, m=M, n=K, k=N, maskbits=xbits))
-    report('dgrad bits', ms, 2.0 * M * (N + K))
-    ms = timeit(lambda: ops.gemm(L.GEMM_DGRAD, dy, w_kn, dx, m=M, n=K, k=N, maskbits=xbits, colsum=cs))
-    report('dgrad bits+colsum', ms, 2.0 * M * (N + K))
+    report('fwd bias+relu+bits', ms, 2.0 * M * (N + K), t_fwd)
+    if K <= 1024:
+      t_dgrad = timeit(lambda: torch.matmul(dy, w_kn.t(), out=dx))
+      ms = timeit(lambda: ops.gemm(L.GEMM_DGRAD, dy, w_kn, dx, m=M, n=K, k=N))
+      report('dgrad plain', ms, 2.0 * M * (N + K), t_dgrad)
+      ms = timeit(lambda: ops.gemm(L.GEMM_DGRAD, dy, w_kn, dx, m=M, n=K, k=N, maskbits=xbits))
+      report('dgrad bits', ms, 2.0 * M * (N + K), t_dgrad)
+      ms = timeit(lambda: ops.gemm(L.GEMM_DGRAD, dy, w_kn, dx, m=M, n=K, k=N, maskbits=xbits, colsum=cs))
+      report('dgrad bits+colsum', ms, 2.0 * M * (N + K), t_dgrad)
+    t_wgrad = timeit(lambda: torch.matmul(x.t(), dy))     # the [K, N] output is too small for its dtype to matter
     ms = timeit(lambda: ops.gemm(L.GEMM_WGRAD, x, dy, dw, m=K, n=N, k=M))
-    report('wgrad', ms, 2.0 * M * (N + K))
+    report('wgrad', ms, 2.0 * M * (N + K), t_wgrad)
     ms = timeit(lambda: ops.colsum(dy, N, cs[:N] if N <= K else torch.zeros(N, device=dev)))
     report('colsum kernel', ms, 2.0 * M * N)
     del x, y, dy, dx, bits, xbits
