@@ -29,17 +29,19 @@ constexpr int BLOCK_K = 64;          // 64 bf16 = one 128-byte swizzle span
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;        // 16 KiB
 constexpr int NUM_THREADS = 384;
 constexpr int CS_MAX = 1024;         // DGRAD column sums are gathered in shared memory: N <= CS_MAX
-// TS: the bf16 output tile is staged in shared memory (BN / 64 blocks of [128 rows x 64 cols], 128-byte swizzle)
-// and written by TMA bulk stores, which leave coalesced full lines and run while the next tile's main loop does.
-// The staging tile takes the place of ring stages: 64 KB at BN = 256 leaves room for 3 stages.
-constexpr int staging_bytes(int bn, bool ts) { return ts ? BLOCK_M * bn * 2 : 0; }
-// operand ring depth per tile width: the ring and the staging tile fill up to ~210 KB of the 227 KB of shared memory
-constexpr int gemm_stages(int bn, bool ts) {
-  return ts ? (bn == 256 ? 3 : bn == 128 ? 5 : 8) : (bn == 256 ? 4 : bn == 128 ? 6 : 8);
+// operand ring depth per tile width: 192 KB of the 227 KB of shared memory
+constexpr int gemm_stages(int bn) { return bn == 256 ? 4 : bn == 128 ? 6 : 8; }
+// TS: the bf16 output is staged in shared memory and written by TMA bulk stores, which leave coalesced full lines
+// and run while the epilogue and the next tile's main loop do.  Each consumer warpgroup stages its 64 x BN tile one
+// [64 rows x 64 cols] block (8 KB, 128-byte swizzle) at a time through a ring of staging blocks: two where the
+// tile has an even number of blocks and the shared memory has room (FWD: DGRAD holds the column sums), else one.
+constexpr int STAGING_BLOCK_BYTES = 64 * 128;
+constexpr int staging_blocks(int mode, int bn, bool ts) {
+  return !ts ? 0 : (mode == MNRF_GEMM_FWD && bn >= 128) ? 2 : 1;
 }
-constexpr int smem_bytes(int bn, bool ts) {
-  return gemm_stages(bn, ts) * (A_STAGE_BYTES + bn * BLOCK_K * 2) + staging_bytes(bn, ts) + CS_MAX * 4 +
-         256 /*barriers*/ + 1024 /*align*/;
+constexpr int smem_bytes(int mode, int bn, bool ts) {
+  return gemm_stages(bn) * (A_STAGE_BYTES + bn * BLOCK_K * 2) + 2 * staging_blocks(mode, bn, ts) * STAGING_BLOCK_BYTES +
+         (mode == MNRF_GEMM_DGRAD ? CS_MAX * 4 : 0) + 256 /*barriers*/ + 1024 /*align*/;
 }
 
 struct GemmParams {
@@ -68,16 +70,18 @@ template <int MODE, int BN, bool TS>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const __grid_constant__ CUtensorMap tmap_c, const GemmParams p) {
-  constexpr int STAGES = gemm_stages(BN, TS);
+  constexpr int STAGES = gemm_stages(BN);
   constexpr int B_STAGE = BN * BLOCK_K * 2;
   constexpr bool kWgrad = (MODE == MNRF_GEMM_WGRAD);
   constexpr int NACC = BN / 2;
+  constexpr int SB = staging_blocks(MODE, BN, TS);
+  static_assert(SB < 2 || (BN / 64) % 2 == 0, "block j of every tile must use staging block j % SB");
   extern __shared__ uint8_t smem_dyn[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
-  uint8_t* smem_c = smem_b + STAGES * B_STAGE;                                   // TS: output staging tile
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_c + staging_bytes(BN, TS));  // [STAGES]
+  uint8_t* smem_c = smem_b + STAGES * B_STAGE;                                   // TS: [2 warpgroups][SB] blocks
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_c + 2 * SB * STAGING_BLOCK_BYTES);  // [STAGES]
   uint64_t* empty_bar = full_bar + STAGES;                                       // [STAGES]
   float* cs_s = reinterpret_cast<float*>(empty_bar + STAGES);                    // [CS_MAX] DGRAD column sums
 
@@ -196,12 +200,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         }
         continue;
       }
-      if (TS) {
-        // the previous tile's bulk stores must have finished reading the staging rows of this warpgroup
-        if ((threadIdx.x & 127) == 0) tma_store_wait_read<0>();
-        named_bar_sync(2 + c, 128);
-      }
-      const uint32_t c_row = smem_u32(smem_c) + r_in * 128 + (cq << 1);   // TS: this thread's staging row (h = 0)
+      const bool leader = (threadIdx.x & 127) == 0;   // TS: issues and waits on the warpgroup's bulk stores
+      // TS: this thread's row (h = 0) in the warpgroup's first staging block
+      const uint32_t c_row = smem_u32(smem_c) + c * (SB * STAGING_BLOCK_BYTES) + (r_in - 64 * c) * 128 + (cq << 1);
       int64_t rows[2];
       bool row_ok[2];
       float rv[2] = {0.f, 0.f};
@@ -216,9 +217,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         }
       }
       uint32_t bits[2] = {0u, 0u};
+      uint32_t mw[2] = {0u, 0u};                // DGRAD mask bits: the rows' words of the current 32 columns
 #pragma unroll
       for (int i = 0; i < BN / 8; ++i) {
         const int col = ncol0 + 8 * i + cq;
+        if (TS && SB == 1 && (i & 7) == 0) {
+          // the previous bulk store must have finished reading the staging block
+          if (leader) tma_store_wait_read<0>();
+          named_bar_sync(2 + c, 128);
+        }
+        if (MODE == MNRF_GEMM_DGRAD && p.maskbits && (i & 3) == 0) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) mw[h] = row_ok[h] ? __ldg(mrow[h] + (col >> 5)) : 0u;
+        }
         float v[2][2];
 #pragma unroll
         for (int h = 0; h < 2; ++h) { v[h][0] = acc[4 * i + 2 * h]; v[h][1] = acc[4 * i + 2 * h + 1]; }
@@ -244,9 +255,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           for (int h = 0; h < 2; ++h) {
             if (p.rowv) { v[h][0] += rv[h] * cv.x; v[h][1] += rv[h] * cv.y; }
             if (p.maskbits) {
-              const uint32_t wd = row_ok[h] ? __ldg(mrow[h] + (col >> 5)) : 0u;
-              if (!((wd >> (col & 31)) & 1u)) v[h][0] = 0.f;
-              if (!((wd >> ((col + 1) & 31)) & 1u)) v[h][1] = 0.f;
+              if (!((mw[h] >> (col & 31)) & 1u)) v[h][0] = 0.f;
+              if (!((mw[h] >> ((col + 1) & 31)) & 1u)) v[h][1] = 0.f;
             } else if (p.mask && row_ok[h]) {
               const uint32_t mm = __ldg(reinterpret_cast<const unsigned int*>(p.mask + rows[h] * p.ldmask + col));
               if (!(bf16_lo(mm) > 0.f)) v[h][0] = 0.f;
@@ -259,21 +269,24 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
             }
           }
           if (do_cs) {
-            // column sums over the warp's 16 rows (rows past M hold zeros: zero-filled A tile, rv = 0)
-            float s0 = v[0][0] + v[1][0], s1 = v[0][1] + v[1][1];
-#pragma unroll
-            for (int o = 4; o < 32; o <<= 1) {
-              s0 += __shfl_xor_sync(0xffffffffu, s0, o);
-              s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-            }
-            if (lane < 4) { atomicAdd(cs_s + col, s0); atomicAdd(cs_s + col + 1, s1); }
+            // column sums over the warp's 16 rows (rows past M hold zeros: zero-filled A tile, rv = 0).  The first
+            // butterfly step swaps halves: lane bit 2 keeps column col + bit 2, so the two columns share the
+            // remaining steps and one atomic.  Each sum is added in the same pairwise order as a butterfly per column.
+            const bool hi = (lane >> 2) & 1;
+            const float s0 = v[0][0] + v[1][0], s1 = v[0][1] + v[1][1];
+            float t = (hi ? s1 : s0) + __shfl_xor_sync(0xffffffffu, hi ? s0 : s1, 4);
+            t += __shfl_xor_sync(0xffffffffu, t, 8);
+            t += __shfl_xor_sync(0xffffffffu, t, 16);
+            if (lane < 8) atomicAdd(cs_s + col + hi, t);
           }
         }
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           if (TS) {
-            // [128 x 64] block i / 8, row r_in + 8h, 16-byte chunk (i % 8) ^ (row % 8), byte 2 * cq
-            st_shared_u32(c_row + h * (8 * 128) + (i >> 3) * (BLOCK_M * 128) + (((i & 7) ^ ((lane >> 2) & 7)) << 4),
+            // staging block (i / 8) % SB (SB is 1 or 2), row r_in - 64c + 8h, 16-byte chunk (i % 8) ^ (row % 8),
+            // byte 2 * cq
+            st_shared_u32(c_row + ((i >> 3) & (SB - 1)) * STAGING_BLOCK_BYTES + h * (8 * 128) +
+                              (((i & 7) ^ ((lane >> 2) & 7)) << 4),
                           pack_bf16(v[h][0], v[h][1]));
           } else if (row_ok[h]) {
             *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + rows[h] * p.ldc + col) =
@@ -290,17 +303,16 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
             bits[h] = 0u;
           }
         }
-      }
-      if (TS) {
-        // TMA clips the rows past M
-        fence_proxy_async();                    // generic-proxy writes -> visible to the bulk store (async proxy)
-        named_bar_sync(2 + c, 128);
-        if ((threadIdx.x & 127) == 0) {   // one thread per warpgroup issues its bulk stores
-#pragma unroll
-          for (int j = 0; j < BN / 64; ++j)
-            tma_store_2d(&tmap_c, smem_c + j * (BLOCK_M * 128) + c * (64 * 128), ncol0 + 64 * j,
+        if (TS && (i & 7) == 7) {
+          fence_proxy_async();                  // generic-proxy writes -> visible to the bulk store (async proxy)
+          // SB = 2: the store of the previous block, in the staging block that the next block overwrites, has been read
+          if (SB == 2 && leader) tma_store_wait_read<0>();
+          named_bar_sync(2 + c, 128);
+          if (leader) {                         // TMA clips the rows past M
+            tma_store_2d(&tmap_c, smem_c + (c * SB + ((i >> 3) & (SB - 1))) * STAGING_BLOCK_BYTES, ncol0 + 8 * (i & ~7),
                          (int)((int64_t)m_blk * BLOCK_M + 64 * c));
-          tma_store_commit();
+            tma_store_commit();
+          }
         }
       }
     }
@@ -407,7 +419,7 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
 #define MNRF_LAUNCH_TC3(MODE_, BN_, TS_)                                                              \
   do {                                                                                                \
     static bool attr_set = false;                                                                     \
-    constexpr int kSmem = smem_bytes(BN_, TS_);                                                       \
+    constexpr int kSmem = smem_bytes(MODE_, BN_, TS_);                                                \
     static_assert(kSmem <= 232448, "shared memory budget");                                           \
     auto kern = gemm_tc_kernel<MODE_, BN_, TS_>;                                                      \
     if (!attr_set) {                                                                                  \
