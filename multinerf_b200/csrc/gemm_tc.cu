@@ -28,20 +28,27 @@ constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;          // 64 bf16 = one 128-byte swizzle span
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;        // 16 KiB
 constexpr int NUM_THREADS = 384;
-constexpr int CS_MAX = 1024;         // DGRAD column sums are gathered in shared memory: N <= CS_MAX
+constexpr int CS_MAX = 1024;         // widest output the fused DGRAD column sums are offered for
 // operand ring depth per tile width: 192 KB of the 227 KB of shared memory
 constexpr int gemm_stages(int bn) { return bn == 256 ? 4 : bn == 128 ? 6 : 8; }
 // TS: the bf16 output is staged in shared memory and written by TMA bulk stores, which leave coalesced full lines
 // and run while the epilogue and the next tile's main loop do.  Each consumer warpgroup stages its 64 x BN tile one
 // [64 rows x 64 cols] block (8 KB, 128-byte swizzle) at a time through a ring of staging blocks: two where the
-// tile has an even number of blocks and the shared memory has room (FWD: DGRAD holds the column sums), else one.
+// tile has an even number of blocks and the shared memory has room (FWD: DGRAD holds column sums and mask words),
+// else one.
 constexpr int STAGING_BLOCK_BYTES = 64 * 128;
 constexpr int staging_blocks(int mode, int bn, bool ts) {
   return !ts ? 0 : (mode == MNRF_GEMM_FWD && bn >= 128) ? 2 : 1;
 }
+// DGRAD: mask words per row of a tile's TMA-loaded mask block.  A box row must be a multiple of 16 bytes and start
+// 16-byte aligned, so tiles narrower than 128 columns load their mask words in the epilogue instead.
+constexpr int mask_words(int bn) { return bn >= 128 ? bn / 32 : 0; }
+constexpr int MASK_BUFS = 2;         // mask blocks in flight: the producer loads tile t+1's during tile t's epilogue
+// DGRAD: per-consumer-warp column sums [8][BN] fp32, then MASK_BUFS mask blocks [128 rows][mask_words] uint32
+constexpr int dgrad_smem_bytes(int bn) { return 8 * bn * 4 + MASK_BUFS * BLOCK_M * mask_words(bn) * 4; }
 constexpr int smem_bytes(int mode, int bn, bool ts) {
   return gemm_stages(bn) * (A_STAGE_BYTES + bn * BLOCK_K * 2) + 2 * staging_blocks(mode, bn, ts) * STAGING_BLOCK_BYTES +
-         (mode == MNRF_GEMM_DGRAD ? CS_MAX * 4 : 0) + 256 /*barriers*/ + 1024 /*align*/;
+         (mode == MNRF_GEMM_DGRAD ? dgrad_smem_bytes(bn) : 0) + 256 /*barriers*/ + 1024 /*align*/;
 }
 
 struct GemmParams {
@@ -57,6 +64,7 @@ struct GemmParams {
   uint32_t* maskbits;         // FWD+ReLU: written (1 bit per output, word = 32 columns); DGRAD: read
   int64_t ldmaskbits;         // in 32-bit words
   int64_t mask_mod;           // > 0: mask row = output row mod mask_mod
+  int mask_tma;               // DGRAD: the producer loads each tile's mask words by TMA (else the epilogue's __ldg)
   const __nv_bfloat16* addend;  // DGRAD: out += addend[M, ldadd] (second contribution to a shared input)
   int64_t ldadd;
   float* colsum;              // DGRAD: colsum[N] += column sums of the output (bias gradient of the
@@ -69,40 +77,54 @@ struct GemmParams {
 template <int MODE, int BN, bool TS>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-               const __grid_constant__ CUtensorMap tmap_c, const GemmParams p) {
+               const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_m,
+               const GemmParams p) {
   constexpr int STAGES = gemm_stages(BN);
   constexpr int B_STAGE = BN * BLOCK_K * 2;
   constexpr bool kWgrad = (MODE == MNRF_GEMM_WGRAD);
+  constexpr bool kDgrad = (MODE == MNRF_GEMM_DGRAD);
   constexpr int NACC = BN / 2;
   constexpr int SB = staging_blocks(MODE, BN, TS);
+  constexpr int MW = mask_words(BN);
   static_assert(SB < 2 || (BN / 64) % 2 == 0, "block j of every tile must use staging block j % SB");
   extern __shared__ uint8_t smem_dyn[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
   uint8_t* smem_c = smem_b + STAGES * B_STAGE;                                   // TS: [2 warpgroups][SB] blocks
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_c + 2 * SB * STAGING_BLOCK_BYTES);  // [STAGES]
+  // DGRAD: column sums of the current n-block, one private [BN] slice per consumer warp, then the mask blocks
+  // (offsets stay multiples of 128 bytes, as TMA destinations need)
+  float* cs_s = reinterpret_cast<float*>(smem_c + 2 * SB * STAGING_BLOCK_BYTES);  // [8][BN]
+  uint32_t* mask_s = reinterpret_cast<uint32_t*>(cs_s + (kDgrad ? 8 * BN : 0));   // [MASK_BUFS][BLOCK_M][MW]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(mask_s + (kDgrad ? MASK_BUFS * BLOCK_M * MW : 0));  // [STAGES]
   uint64_t* empty_bar = full_bar + STAGES;                                       // [STAGES]
-  float* cs_s = reinterpret_cast<float*>(empty_bar + STAGES);                    // [CS_MAX] DGRAD column sums
+  uint64_t* mask_full = empty_bar + STAGES;                                      // [MASK_BUFS]
+  uint64_t* mask_empty = mask_full + MASK_BUFS;                                  // [MASK_BUFS]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int wg = threadIdx.x >> 7;
   const int total_tiles = p.num_m_blocks * p.num_n_blocks * p.num_splits;
-  const bool do_cs = MODE == MNRF_GEMM_DGRAD && p.colsum != nullptr;
+  const bool do_cs = kDgrad && p.colsum != nullptr;
+  const bool mask_tma = kDgrad && p.mask_tma;
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_b);
     if (TS) prefetch_tmap(&tmap_c);
+    if (mask_tma) prefetch_tmap(&tmap_m);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 8);     // one arrival per consumer warp
     }
+    for (int i = 0; i < MASK_BUFS; ++i) {
+      mbar_init(&mask_full[i], 1);
+      mbar_init(&mask_empty[i], 8);
+    }
     fence_barrier_init();
   }
   if (do_cs)
-    for (int i = threadIdx.x; i < p.n; i += NUM_THREADS) cs_s[i] = 0.f;
+    for (int i = threadIdx.x; i < 8 * BN; i += NUM_THREADS) cs_s[i] = 0.f;
   __syncthreads();
   // Programmatic dependent launch: nothing above touched global memory, everything below may.
   pdl_launch_dependents();
@@ -114,13 +136,23 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     if (threadIdx.x == 0) {
       const uint32_t stage_bytes = A_STAGE_BYTES + B_STAGE;
       uint32_t stage = 0, phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      for (int tile = blockIdx.x, it = 0; tile < total_tiles; tile += gridDim.x, ++it) {
         const int n_blk = tile % p.num_n_blocks;
         const int rest = tile / p.num_n_blocks;
         const int m_blk = rest % p.num_m_blocks;
         const int split = rest / p.num_m_blocks;
         const int kb0 = split * p.kblocks_per_split;
         const int kb1 = min(p.num_k_blocks, kb0 + p.kblocks_per_split);
+        if (mask_tma) {
+          // the tile's [128 rows x MW words] of mask bits; with mask_mod (a multiple of 128) the tile's rows map to
+          // 128 consecutive mask rows.  Rows past the end are zero-filled.
+          const int mb = it % MASK_BUFS;
+          mbar_wait(&mask_empty[mb], ((it / MASK_BUFS) & 1) ^ 1, 4);
+          mbar_expect_tx(&mask_full[mb], BLOCK_M * MW * 4);
+          const int64_t r0 = (int64_t)m_blk * BLOCK_M;
+          tma_load_2d(mask_s + mb * (BLOCK_M * MW), &tmap_m, &mask_full[mb], n_blk * (BN / 32),
+                      (int)(p.mask_mod > 0 ? r0 % p.mask_mod : r0));
+        }
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1, 1);
           mbar_expect_tx(&full_bar[stage], stage_bytes);
@@ -152,7 +184,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     const int cq = 2 * (lane & 3);
     uint32_t stage = 0, phase = 0;
     float acc[NACC];
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    // DGRAD: this warp's column-sum slice, at the column pair of lanes 0-7 after the butterfly below
+    const uint32_t cs_lane = smem_u32(cs_s) + ((warp - 4) * BN + cq + ((lane >> 2) & 1)) * 4;
+    for (int tile = blockIdx.x, it = 0; tile < total_tiles; tile += gridDim.x, ++it) {
       const int n_blk = tile % p.num_n_blocks;
       const int rest = tile / p.num_n_blocks;
       const int m_blk = rest % p.num_m_blocks;
@@ -213,9 +247,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         row_ok[h] = rows[h] < p.m;
         if (MODE == MNRF_GEMM_DGRAD && row_ok[h]) {
           if (p.rowv) rv[h] = p.rowv[rows[h]];
-          if (p.maskbits) mrow[h] = p.maskbits + (p.mask_mod > 0 ? rows[h] % p.mask_mod : rows[h]) * p.ldmaskbits;
+          if (p.maskbits && !mask_tma)
+            mrow[h] = p.maskbits + (p.mask_mod > 0 ? rows[h] % p.mask_mod : rows[h]) * p.ldmaskbits;
         }
       }
+      // mask_tma: this thread's row (h = 0) of the tile's mask block, once the producer's load has landed
+      const uint32_t m_row = smem_u32(mask_s) + ((it % MASK_BUFS) * BLOCK_M + r_in) * (MW * 4);
+      if (mask_tma) mbar_wait(&mask_full[it % MASK_BUFS], (it / MASK_BUFS) & 1, 5);
       uint32_t bits[2] = {0u, 0u};
       uint32_t mw[2] = {0u, 0u};                // DGRAD mask bits: the rows' words of the current 32 columns
 #pragma unroll
@@ -228,7 +266,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         }
         if (MODE == MNRF_GEMM_DGRAD && p.maskbits && (i & 3) == 0) {
 #pragma unroll
-          for (int h = 0; h < 2; ++h) mw[h] = row_ok[h] ? __ldg(mrow[h] + (col >> 5)) : 0u;
+          for (int h = 0; h < 2; ++h)
+            mw[h] = mask_tma ? ld_shared_u32(m_row + (8 * h * MW + (i >> 2)) * 4)
+                             : row_ok[h] ? __ldg(mrow[h] + (col >> 5)) : 0u;
         }
         float v[2][2];
 #pragma unroll
@@ -271,13 +311,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           if (do_cs) {
             // column sums over the warp's 16 rows (rows past M hold zeros: zero-filled A tile, rv = 0).  The first
             // butterfly step swaps halves: lane bit 2 keeps column col + bit 2, so the two columns share the
-            // remaining steps and one atomic.  Each sum is added in the same pairwise order as a butterfly per column.
+            // remaining steps and one slice word.  Each sum is added in the same pairwise order as a butterfly per
+            // column.  Lanes 0-7 own 8 distinct words of the warp's own slice: a plain load and store.
             const bool hi = (lane >> 2) & 1;
             const float s0 = v[0][0] + v[1][0], s1 = v[0][1] + v[1][1];
             float t = (hi ? s1 : s0) + __shfl_xor_sync(0xffffffffu, hi ? s0 : s1, 4);
             t += __shfl_xor_sync(0xffffffffu, t, 8);
             t += __shfl_xor_sync(0xffffffffu, t, 16);
-            if (lane < 8) atomicAdd(cs_s + col + hi, t);
+            if (lane < 8) {
+              const uint32_t a = cs_lane + 8 * i * 4;
+              st_shared_u32(a, __float_as_uint(__uint_as_float(ld_shared_u32(a)) + t));
+            }
           }
         }
 #pragma unroll
@@ -315,12 +359,28 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           }
         }
       }
+      if (mask_tma) {                           // this warp has read its mask words: the buffer may be refilled
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&mask_empty[it % MASK_BUFS]);
+      }
+      const int next = tile + (int)gridDim.x;
+      if (do_cs && (next >= total_tiles || next % p.num_n_blocks != n_blk)) {
+        // the n-block's sums are complete: add the eight slices in warp order, one global reduction per column,
+        // and clear the slices for the next n-block
+        named_bar_sync(1, 2 * 128);
+        for (int j = threadIdx.x - 128; j < BN; j += 2 * 128) {
+          float s = 0.f;
+#pragma unroll
+          for (int sw = 0; sw < 8; ++sw) {
+            s += cs_s[sw * BN + j];
+            cs_s[sw * BN + j] = 0.f;
+          }
+          atomicAdd(p.colsum + ncol0 + j, s);
+        }
+        named_bar_sync(1, 2 * 128);
+      }
     }
     if (TS && (threadIdx.x & 127) == 0) tma_store_wait_all();
-    if (do_cs) {
-      named_bar_sync(1, 2 * 128);               // both consumer warpgroups are done with the shared sums
-      for (int i = threadIdx.x - 128; i < p.n; i += 2 * 128) atomicAdd(p.colsum + i, cs_s[i]);
-    }
   }
 }
 
@@ -413,6 +473,17 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
   } else {
     tc = tb;   // not read
   }
+  // DGRAD mask bits go through TMA when the tile is at least 128 columns wide and the mask rows of a 128-row tile
+  // are 128 consecutive rows of a TMA-addressable array (16-byte aligned base and row pitch); otherwise the
+  // epilogue loads them itself.
+  CUtensorMap tm = tb;   // not read unless p.mask_tma
+  p.mask_tma = d->mode == MNRF_GEMM_DGRAD && maskbits && mask_words(block_n) > 0 && d->ldmaskbits % 4 == 0 &&
+               ((uintptr_t)maskbits % 16) == 0 && (d->mask_mod == 0 || d->mask_mod % BLOCK_M == 0);
+  if (p.mask_tma &&
+      make_tmap(&tm, maskbits, d->mask_mod > 0 ? d->mask_mod : d->m, d->n / 32, d->ldmaskbits,
+                mask_words(block_n), BLOCK_M, CU_TENSOR_MAP_DATA_TYPE_UINT32, 4,
+                CU_TENSOR_MAP_SWIZZLE_NONE))
+    return 1;
   const int total_tiles = p.num_m_blocks * p.num_n_blocks * p.num_splits;
   const int grid = std::min(total_tiles, workers);
   if (grid == 0) return 0;
@@ -433,7 +504,7 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                                  \
     attr[0].val.programmaticStreamSerializationAllowed = 1;                                           \
     cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;                                           \
-    MNRF_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, tc, p));                                         \
+    MNRF_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, tc, tm, p));                                     \
   } while (0)
 #define MNRF_LAUNCH_TC2(MODE_, BN_)                                                                   \
   do {                                                                                                \

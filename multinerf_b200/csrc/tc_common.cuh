@@ -83,6 +83,11 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
 __device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
   asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
 __device__ __forceinline__ void named_bar_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
@@ -151,17 +156,20 @@ inline EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// 2-D bf16 tensor [rows, cols] (cols contiguous, row pitch ld elements), box = [box_cols, box_rows].
+// 2-D tensor [rows, cols] (cols contiguous, row pitch ld elements), box = [box_cols, box_rows]; bf16 with the
+// 128-byte swizzle unless told otherwise.
 inline int make_tmap(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int64_t ld,
-                     int box_cols, int box_rows) {
+                     int box_cols, int box_rows,
+                     CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, int elem_bytes = 2,
+                     CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   EncodeTiledFn fn = get_encode_fn();
   MNRF_CHECK(fn, "cuTensorMapEncodeTiled is not available from the driver");
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * elem_bytes};
   cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+  CUresult r = fn(map, dtype, 2, const_cast<void*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   MNRF_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d): rows=%lld cols=%lld ld=%lld box=%dx%d base=%p",
              (int)r, (long long)rows, (long long)cols, (long long)ld, box_cols, box_rows, base);
