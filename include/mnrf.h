@@ -303,6 +303,44 @@ int mnrf_composite_bwd(const mnrf_loss_desc* d, const float* raw_density, const 
                        const float* sdist_fine, const float* weights_fine,
                        float* d_raw_density, float* d_raw_rgb, float* d_rgb_scale /* [B,3] or NULL */,
                        float* d_raw_diffuse, float* d_raw_tint, float* stats, mnrf_stream stream);
+/* Same, with a per-ray 0/1 weight on the data loss (data_loss_type 'robustnerf', train_utils.py:104-108):
+ * the data-loss value and its gradient of ray r are multiplied by data_mask[r] ([B] fp32); the mse stat
+ * (stats[1]) stays unmasked.  data_mask == NULL is mnrf_composite_bwd. */
+int mnrf_composite_bwd_masked(const mnrf_loss_desc* d, const float* raw_density, const float* raw_rgb,
+                              const float* density_noise, const float* sdist, const float* directions,
+                              const float* near, const float* far, const float* bg_rgb,
+                              const float* rgb_scale, const float* raw_diffuse, const float* raw_tint,
+                              const float* extra_dw, const float* target_rgb,
+                              const float* lossmult, const float* inv_denom,
+                              const float* sdist_fine, const float* weights_fine, const float* data_mask,
+                              float* d_raw_density, float* d_raw_rgb, float* d_rgb_scale,
+                              float* d_raw_diffuse, float* d_raw_tint, float* stats, mnrf_stream stream);
+
+/* ---- RobustNeRF mask and inlier threshold (robustnerf.py:8-115) ------------------------------
+ * mnrf_robust_mask: one CTA per patch; rays are patch-major [num_rays / p^2, p, p].
+ *   rgb, target [B,3]; threshold: device scalar (the previous step's loss_threshold; strict "<")
+ *   mask [B] fp32 0/1 (all ones when enable == 0); error_per_pixel [B] = mean over the 3 channels of
+ *   (rgb - target)^2, rounded as ((r0 + r1) + r2) / 3
+ *   stats (optional): stats[1..4] += per-rank means of is_inlier_loss, has_inlier_neighbors,
+ *   is_inlier_patch, mask (only mask when enable == 0); needs `counts`, a uint32[5] workspace that is
+ *   zero before the first launch and that every launch leaves zero.
+ * Requires p*p <= 1024, num_rays a multiple of p*p, and (enable) inner_patch_size <= p, odd filter_size <= p.
+ * Comparisons on neighbourhood / patch means use fl32(count / size) > fl32(1 - quantile); see csrc/robust.cu
+ * for the tie rule of the box filter.
+ * mnrf_quantile: out[0] = jnp.quantile(x[0:n], q) ('linear'), computed in fp32 as
+ *   qn = q * (n - 1), lo = floor(qn), hi = ceil(qn), w = qn - lo, x_(lo) * (1 - w) + x_(hi) * w
+ * (x_(i) = i-th smallest); NaN if any x is NaN.  One CTA, no workspace; 1 <= n < 2^24. */
+typedef struct {
+  int32_t num_rays;
+  int32_t patch_size, inner_patch_size, filter_size;
+  int32_t enable;
+  float smoothed_thresh;    /* fl32(1 - robustnerf_smoothed_inlier_quantile) */
+  float patch_thresh;       /* fl32(1 - robustnerf_inner_patch_inlier_quantile) */
+} mnrf_robust_desc;
+
+int mnrf_robust_mask(const mnrf_robust_desc* d, const float* rgb, const float* target, const float* threshold,
+                     float* mask, float* error_per_pixel, uint32_t* counts, float* stats, mnrf_stream stream);
+int mnrf_quantile(int32_t n, float q, const float* x, float* out, mnrf_stream stream);
 
 /* ---- Ref-NeRF per-sample stage ---------------------------------------------------------------
  * Between the spatial trunk and the directional MLP: normals_pred / normals = -l2_normalize(.)

@@ -17,7 +17,7 @@ COMMON = ['-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC', '--expt-relax
 SOURCES = {
     'lib.cu': [], 'sampling.cu': ['-fmad=false'], 'encode.cu': ['-fmad=false'],
     'composite.cu': ['-fmad=false'], 'heads.cu': [], 'gemm_tc.cu': [], 'chain.cu': [], 'gemm_ref.cu': [],
-    'refnerf.cu': [], 'camera.cu': ['-fmad=false'],
+    'refnerf.cu': [], 'camera.cu': ['-fmad=false'], 'robust.cu': ['-fmad=false'],
 }
 
 

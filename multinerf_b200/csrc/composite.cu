@@ -239,6 +239,7 @@ composite_bwd_kernel(mnrf_loss_desc L, const float* __restrict__ raw_density,
                      const float* __restrict__ extra_dw, const float* __restrict__ target_rgb,
                      const float* __restrict__ lossmult, const float* __restrict__ inv_denom_p,
                      const float* __restrict__ sdist_fine, const float* __restrict__ weights_fine,
+                     const float* __restrict__ data_mask,
                      float* __restrict__ d_raw_density, float* __restrict__ d_raw_rgb,
                      float* __restrict__ d_rgb_scale, float* __restrict__ d_raw_diffuse,
                      float* __restrict__ d_raw_tint, float* __restrict__ stats) {
@@ -293,6 +294,11 @@ composite_bwd_kernel(mnrf_loss_desc L, const float* __restrict__ raw_density,
         float sc = 1.f / (1e-3f + clip);
         lv = rc * rc * sc * sc;
         g = v < 1.f ? 2.f * rc * sc * sc : 0.f;
+      }
+      if (data_mask) {                                // robustnerf: resid_sq * mask (a constant for autodiff)
+        const float m = data_mask[ray];
+        lv *= m;
+        g *= m;
       }
       dpx[ch] = L.data_mult * lm * g * inv_denom;
       if (lane == 0) {
@@ -494,17 +500,15 @@ extern "C" int mnrf_composite_fwd(const mnrf_composite_desc* d, const float* raw
   return 0;
 }
 
-extern "C" int mnrf_composite_bwd(const mnrf_loss_desc* d, const float* raw_density,
-                                  const float* raw_rgb, const float* density_noise,
-                                  const float* sdist, const float* directions, const float* near,
-                                  const float* far, const float* bg_rgb, const float* rgb_scale,
-                                  const float* raw_diffuse, const float* raw_tint, const float* extra_dw,
-                                  const float* target_rgb,
-                                  const float* lossmult, const float* inv_denom,
-                                  const float* sdist_fine, const float* weights_fine,
-                                  float* d_raw_density, float* d_raw_rgb, float* d_rgb_scale,
-                                  float* d_raw_diffuse, float* d_raw_tint, float* stats,
-                                  mnrf_stream stream) {
+// mnrf_composite_bwd and mnrf_composite_bwd_masked share this body (data_mask == NULL: no mask).
+static int composite_bwd_launch(const mnrf_loss_desc* d, const float* raw_density, const float* raw_rgb,
+                                const float* density_noise, const float* sdist, const float* directions,
+                                const float* near, const float* far, const float* bg_rgb, const float* rgb_scale,
+                                const float* raw_diffuse, const float* raw_tint, const float* extra_dw,
+                                const float* target_rgb, const float* lossmult, const float* inv_denom,
+                                const float* sdist_fine, const float* weights_fine, const float* data_mask,
+                                float* d_raw_density, float* d_raw_rgb, float* d_rgb_scale,
+                                float* d_raw_diffuse, float* d_raw_tint, float* stats, mnrf_stream stream) {
   using namespace mnrf;
   MNRF_CHECK(d->c.rgb_mode == 0 || (raw_rgb && raw_diffuse && d_raw_diffuse && (!raw_tint || d_raw_tint)),
              "mnrf_composite_bwd: rgb_mode 1 needs raw_diffuse / d_raw_diffuse (and d_raw_tint with raw_tint)");
@@ -525,8 +529,43 @@ extern "C" int mnrf_composite_bwd(const mnrf_loss_desc* d, const float* raw_dens
   if (blocks > maxb) blocks = maxb;
   MNRF_DISPATCH_CH(d->c.num_samples, (composite_bwd_kernel<CH><<<blocks, nw * 32, smem, (cudaStream_t)stream>>>(
       *d, raw_density, raw_rgb, density_noise, sdist, directions, near, far, bg_rgb, rgb_scale, raw_diffuse,
-      raw_tint, extra_dw, target_rgb, lossmult, inv_denom, sdist_fine, weights_fine, d_raw_density, d_raw_rgb,
-      d_rgb_scale, d_raw_diffuse, d_raw_tint, stats)));
+      raw_tint, extra_dw, target_rgb, lossmult, inv_denom, sdist_fine, weights_fine, data_mask, d_raw_density,
+      d_raw_rgb, d_rgb_scale, d_raw_diffuse, d_raw_tint, stats)));
   MNRF_LAUNCH_CHECK();
   return 0;
+}
+
+extern "C" int mnrf_composite_bwd(const mnrf_loss_desc* d, const float* raw_density,
+                                  const float* raw_rgb, const float* density_noise,
+                                  const float* sdist, const float* directions, const float* near,
+                                  const float* far, const float* bg_rgb, const float* rgb_scale,
+                                  const float* raw_diffuse, const float* raw_tint, const float* extra_dw,
+                                  const float* target_rgb,
+                                  const float* lossmult, const float* inv_denom,
+                                  const float* sdist_fine, const float* weights_fine,
+                                  float* d_raw_density, float* d_raw_rgb, float* d_rgb_scale,
+                                  float* d_raw_diffuse, float* d_raw_tint, float* stats,
+                                  mnrf_stream stream) {
+  return composite_bwd_launch(d, raw_density, raw_rgb, density_noise, sdist, directions, near, far, bg_rgb,
+                              rgb_scale, raw_diffuse, raw_tint, extra_dw, target_rgb, lossmult, inv_denom,
+                              sdist_fine, weights_fine, nullptr, d_raw_density, d_raw_rgb, d_rgb_scale,
+                              d_raw_diffuse, d_raw_tint, stats, stream);
+}
+
+extern "C" int mnrf_composite_bwd_masked(const mnrf_loss_desc* d, const float* raw_density,
+                                         const float* raw_rgb, const float* density_noise,
+                                         const float* sdist, const float* directions, const float* near,
+                                         const float* far, const float* bg_rgb, const float* rgb_scale,
+                                         const float* raw_diffuse, const float* raw_tint, const float* extra_dw,
+                                         const float* target_rgb,
+                                         const float* lossmult, const float* inv_denom,
+                                         const float* sdist_fine, const float* weights_fine,
+                                         const float* data_mask,
+                                         float* d_raw_density, float* d_raw_rgb, float* d_rgb_scale,
+                                         float* d_raw_diffuse, float* d_raw_tint, float* stats,
+                                         mnrf_stream stream) {
+  return composite_bwd_launch(d, raw_density, raw_rgb, density_noise, sdist, directions, near, far, bg_rgb,
+                              rgb_scale, raw_diffuse, raw_tint, extra_dw, target_rgb, lossmult, inv_denom,
+                              sdist_fine, weights_fine, data_mask, d_raw_density, d_raw_rgb, d_rgb_scale,
+                              d_raw_diffuse, d_raw_tint, stats, stream);
 }

@@ -55,6 +55,12 @@ class LossDesc(C.Structure):
               ('lossmult_channels', C.c_int32)]
 
 
+class RobustDesc(C.Structure):
+  _fields_ = [('num_rays', C.c_int32), ('patch_size', C.c_int32), ('inner_patch_size', C.c_int32),
+              ('filter_size', C.c_int32), ('enable', C.c_int32), ('smoothed_thresh', C.c_float),
+              ('patch_thresh', C.c_float)]
+
+
 class RefdirDesc(C.Structure):
   _fields_ = [('M', C.c_int64), ('num_samples', C.c_int32), ('use_pred_normals', C.c_int32),
               ('use_density_normals', C.c_int32), ('use_reflections', C.c_int32), ('use_ide', C.c_int32),
@@ -128,6 +134,9 @@ _SIGNATURES = {
     'mnrf_colsum': (C.c_int, [C.c_int64, C.c_int32, _P, C.c_int64, _P, _P]),
     'mnrf_composite_fwd': (C.c_int, [C.POINTER(CompositeDesc)] + [_P] * 18),
     'mnrf_composite_bwd': (C.c_int, [C.POINTER(LossDesc)] + [_P] * 24),
+    'mnrf_composite_bwd_masked': (C.c_int, [C.POINTER(LossDesc)] + [_P] * 25),
+    'mnrf_robust_mask': (C.c_int, [C.POINTER(RobustDesc)] + [_P] * 8),
+    'mnrf_quantile': (C.c_int, [C.c_int32, C.c_float, _P, _P, _P]),
     'mnrf_encode_tangent': (C.c_int, [C.POINTER(EncodeDesc)] + [_P] * 9 + [C.c_int32, _P]),
     'mnrf_refdir_fwd': (C.c_int, [C.POINTER(RefdirDesc)] + [_P] * 10 + [C.c_float, C.c_float, C.c_int32, _P, _P]),
     'mnrf_refdir_bwd': (C.c_int, [C.POINTER(RefdirDesc)] + [_P] * 8 + [C.c_int32, C.c_float, C.c_float, C.c_int32] +

@@ -278,7 +278,10 @@ def composite_bwd(raw_density, raw_rgb, sdist, directions, near, far, target_rgb
                   inv_denom, stats, *, cfg, loss_type, charb_padding, data_mult, distortion_mult,
                   interlevel_mult, sdist_fine=None, weights_fine=None, density_noise=None,
                   bg_rgb=None, rgb_scale=None, d_raw_density=None, d_raw_rgb=None, d_rgb_scale=None,
-                  raw_diffuse=None, raw_tint=None, extra_dw=None, d_raw_diffuse=None, d_raw_tint=None):
+                  raw_diffuse=None, raw_tint=None, extra_dw=None, d_raw_diffuse=None, d_raw_tint=None,
+                  data_mask=None):
+  """Losses + compositing backward of one level; `data_mask` [B] (optional) weights each ray's data loss
+  (robustnerf) through mnrf_composite_bwd_masked."""
   lib = L.load()
   B, S = raw_density.shape
   dev = raw_density.device
@@ -291,16 +294,57 @@ def composite_bwd(raw_density, raw_rgb, sdist, directions, near, far, target_rgb
   if raw_rgb is not None and d_raw_rgb is None:
     d_raw_rgb = torch.empty(B, S, 3, device=dev)
   _count()
-  L.check(lib.mnrf_composite_bwd(C.byref(d), L.ptr(_f32(raw_density)), L.ptr(_f32(raw_rgb)),
-                                 L.ptr(_f32(density_noise)), L.ptr(_f32(sdist)),
-                                 L.ptr(_f32(directions)), L.ptr(_f32(near)), L.ptr(_f32(far)),
-                                 L.ptr(_f32(bg_rgb)), L.ptr(_f32(rgb_scale)), L.ptr(_f32(raw_diffuse)),
-                                 L.ptr(_f32(raw_tint)), L.ptr(_f32(extra_dw)), L.ptr(_f32(target_rgb)),
-                                 L.ptr(_f32(lossmult)), L.ptr(_f32(inv_denom)),
-                                 L.ptr(_f32(sdist_fine)), L.ptr(_f32(weights_fine)),
-                                 L.ptr(d_raw_density), L.ptr(d_raw_rgb), L.ptr(d_rgb_scale),
-                                 L.ptr(d_raw_diffuse), L.ptr(d_raw_tint), L.ptr(stats), L.stream_ptr()))
+  head = (C.byref(d), L.ptr(_f32(raw_density)), L.ptr(_f32(raw_rgb)), L.ptr(_f32(density_noise)),
+          L.ptr(_f32(sdist)), L.ptr(_f32(directions)), L.ptr(_f32(near)), L.ptr(_f32(far)), L.ptr(_f32(bg_rgb)),
+          L.ptr(_f32(rgb_scale)), L.ptr(_f32(raw_diffuse)), L.ptr(_f32(raw_tint)), L.ptr(_f32(extra_dw)),
+          L.ptr(_f32(target_rgb)), L.ptr(_f32(lossmult)), L.ptr(_f32(inv_denom)), L.ptr(_f32(sdist_fine)),
+          L.ptr(_f32(weights_fine)))
+  tail = (L.ptr(d_raw_density), L.ptr(d_raw_rgb), L.ptr(d_rgb_scale), L.ptr(d_raw_diffuse), L.ptr(d_raw_tint),
+          L.ptr(stats), L.stream_ptr())
+  if data_mask is not None:
+    assert data_mask.numel() == B
+    L.check(lib.mnrf_composite_bwd_masked(*head, L.ptr(_f32(data_mask)), *tail))
+  else:
+    L.check(lib.mnrf_composite_bwd(*head, *tail))
   return d_raw_density, d_raw_rgb
+
+
+def robust_desc(num_rays, *, patch_size, inner_patch_size, filter_size, smoothed_inlier_quantile,
+                inner_patch_inlier_quantile, enable):
+  """mnrf_robust_desc of robustnerf.py's hyperparameters (the two thresholds are fl32(1 - quantile))."""
+  return L.RobustDesc(int(num_rays), int(patch_size), int(inner_patch_size), int(filter_size), int(bool(enable)),
+                      1.0 - float(smoothed_inlier_quantile), 1.0 - float(inner_patch_inlier_quantile))
+
+
+def robust_mask(rgb, target, threshold, desc, *, mask=None, error=None, counts=None, stats=None):
+  """robustnerf.robustnerf_mask for patch-major rays: returns (mask [B], error_per_pixel [B]).
+  `threshold` is a device scalar; with `stats` (a row of >= 5 floats), stats[1:5] += the per-rank means of
+  is_inlier_loss, has_inlier_neighbors, is_inlier_patch and mask, using `counts` (int32[5], zero, left zero)."""
+  lib = L.load()
+  B = rgb.shape[0]
+  assert desc.num_rays == B and rgb.shape == (B, 3) and target.shape == (B, 3) and threshold.numel() == 1
+  if mask is None:
+    mask = torch.empty(B, device=rgb.device)
+  if error is None:
+    error = torch.empty(B, device=rgb.device)
+  if stats is not None:
+    assert counts is not None and counts.dtype == torch.int32 and counts.numel() >= 5
+    assert stats.is_contiguous() and stats.numel() >= 5
+  _count()
+  L.check(lib.mnrf_robust_mask(C.byref(desc), L.ptr(_f32(rgb)), L.ptr(_f32(target)), L.ptr(_f32(threshold)),
+                               L.ptr(mask), L.ptr(error), L.ptr(counts), L.ptr(stats), L.stream_ptr()))
+  return mask, error
+
+
+def quantile(x, q, out=None):
+  """out[0] = jnp.quantile(x, q) (method 'linear') of a flat fp32 tensor, on the device (one CTA)."""
+  lib = L.load()
+  x = _f32(x.reshape(-1))
+  if out is None:
+    out = torch.empty(1, device=x.device)
+  _count()
+  L.check(lib.mnrf_quantile(x.numel(), float(q), L.ptr(x), L.ptr(out), L.stream_ptr()))
+  return out
 
 
 def clip_adam(params, grads, mu, nu, scratch, *, step, lr, beta1, beta2, eps, grad_max_val,

@@ -25,7 +25,9 @@ class SyntheticScene:
   """Infinite iterator of utils.Batch for a procedurally defined scene.
 
   rays: utils.Pixels when `cast_rays_in_train_step` (the cameras are in `.cameras`), else utils.Rays
-  generated on the device by camera_utils.cast_ray_batch; rgb: [B, 3] analytic colours."""
+  generated on the device by camera_utils.cast_ray_batch; rgb: [B, 3] analytic colours.  With
+  `config.patch_size` p > 1 a batch is B // p^2 whole p x p patches, rays in [patch, y, x] order, each patch
+  from one camera (as Dataset._next_train draws them)."""
 
   def __init__(self, config, n_cameras=24, width=96, height=72, focal=90.0, radius=3.0, seed=0,
                device='cuda', rank=0, world=1):
@@ -67,11 +69,28 @@ class SyntheticScene:
 
   def pixels(self):
     B = self.batch
+    p = max(self.config.patch_size, 1)
+    if p > 1:
+      return self._patch_pixels(p)
     meta = lambda v: np.full((B, 1), v, np.float32)
     return utils.Pixels(pix_x_int=self.rng.integers(0, self.width, B).astype(np.int32),
                         pix_y_int=self.rng.integers(0, self.height, B).astype(np.int32),
                         lossmult=meta(1.0), near=meta(self.config.near), far=meta(self.config.far),
                         cam_idx=self.rng.integers(0, self.size, (B, 1)).astype(np.int32))
+
+  def _patch_pixels(self, p):
+    n = self.batch // (p * p)
+    if n < 1:
+      raise ValueError(f'Patch size {p}^2 too large for per-process batch size {self.batch}')
+    x0 = self.rng.integers(0, self.width - p + 1, (n, 1, 1))
+    y0 = self.rng.integers(0, self.height - p + 1, (n, 1, 1))
+    cam = self.rng.integers(0, self.size, (n, 1, 1))
+    dx, dy = camera_utils.pixel_coordinates(p, p)          # [y, x]
+    flat = lambda a: np.ascontiguousarray(np.broadcast_to(a, (n, p, p)).reshape(-1)).astype(np.int32)
+    B = n * p * p
+    meta = lambda v: np.full((B, 1), v, np.float32)
+    return utils.Pixels(pix_x_int=flat(x0 + dx), pix_y_int=flat(y0 + dy), lossmult=meta(1.0),
+                        near=meta(self.config.near), far=meta(self.config.far), cam_idx=flat(cam)[:, None])
 
   def __iter__(self):
     return self
@@ -197,6 +216,8 @@ def train(bundle, dataset, seed=20200823, log=print, use_graph=False, test_datas
   reset_stats, train_start = True, time.time()
   total_time = total_steps = 0
   train_frac = 0.0
+  robust = config.data_loss_type == 'robustnerf'
+  loss_threshold = 1.0                               # train.py:109; not checkpointed, a resumed run restarts here
   gc.disable()
   try:
     for step, batch in zip(range(init_step, num_steps + 1), dataset):
@@ -204,7 +225,9 @@ def train(bundle, dataset, seed=20200823, log=print, use_graph=False, test_datas
         stats_buffer, train_start, reset_stats = [], time.time(), False
       learning_rate = lr_fn(step)
       train_frac = float(np.clip((step - 1) / max(1, config.max_steps - 1), 0, 1))
-      state, stats, gen = train_pstep(gen, state, batch, cameras, train_frac, 1.0)
+      state, stats, gen = train_pstep(gen, state, batch, cameras, train_frac, loss_threshold)
+      if robust and config.enable_robustnerf_loss:
+        loss_threshold = stats.device_loss_threshold()   # train.py:128-129, stays on the device
       stats_buffer.append(stats)
       if step % config.gc_every == 0:
         gc.collect()
@@ -225,6 +248,9 @@ def train(bundle, dataset, seed=20200823, log=print, use_graph=False, test_datas
         for k in mats[0]['losses']:
           if enabled.get(k, True):
             series['losses/' + k] = [m['losses'][k] for m in mats]
+        for k in train_utils.ROBUST_STAT_NAMES:
+          if k in mats[0]:
+            series[k] = [m[k] for m in mats]
         for i in range(len(mats[0]['psnrs'])):           # vector statistics split per level (train.py:160-166)
           series[f'psnrs/{i}'] = [float(m['psnrs'][i]) for m in mats]
           series[f'mses/{i}'] = [float(m['mses'][i]) for m in mats]

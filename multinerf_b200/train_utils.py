@@ -54,6 +54,26 @@ class TrainState:
 
 
 STAT_NAMES = ('data', 'mse', 'distortion', 'interlevel')
+# the robustnerf row of the stats tail (after the level rows): the next loss threshold, then the means of the mask
+ROBUST_STAT_NAMES = ('loss_threshold', 'is_inlier_loss', 'has_inlier_neighbors', 'is_inlier_patch', 'mask')
+ROBUST_MAX_PATCH_PIXELS = 1024
+
+
+def check_robust_config(config, rays_per_rank=None):
+  """The limits of data_loss_type 'robustnerf' on this path (ValueError, like a reference trace-time error)."""
+  p = config.patch_size
+  if p < 1 or p * p > ROBUST_MAX_PATCH_PIXELS:
+    raise ValueError(f'robustnerf: patch_size {p} needs 1 <= patch_size^2 <= {ROBUST_MAX_PATCH_PIXELS}')
+  if not config.enable_robustnerf_loss:
+    return
+  if config.robustnerf_inner_patch_size > p:
+    raise ValueError('patch_size must be larger than robustnerf_inner_patch_size '
+                     f'({p} < {config.robustnerf_inner_patch_size}).')
+  f = config.robustnerf_smoothed_filter_size
+  if f < 1 or f % 2 == 0 or f > p:
+    raise ValueError(f'robustnerf_smoothed_filter_size {f} must be odd and at most patch_size {p}')
+  if rays_per_rank is not None and rays_per_rank % (p * p) != 0:
+    raise ValueError(f'robustnerf: {rays_per_rank} rays per process is not a multiple of patch_size^2 = {p * p}')
 
 
 def _anneal(mcfg, train_frac):
@@ -77,8 +97,11 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
   """
   mcfg = model.mcfg
   camtype = getattr(dataset, 'camtype', camera_utils.ProjectionType.PERSPECTIVE)
-  if config.data_loss_type not in ('mse', 'charb', 'rawnerf'):
+  if config.data_loss_type not in ('mse', 'charb', 'rawnerf', 'robustnerf'):
     raise NotImplementedError(f'data_loss_type {config.data_loss_type!r}')
+  robust = config.data_loss_type == 'robustnerf'
+  if robust:
+    check_robust_config(config, config.batch_size // _world()[0])
   if use_graph and (mcfg.near_anneal_rate is not None or
                     mcfg.bg_intensity_range[0] != mcfg.bg_intensity_range[1] or
                     any(p.cfg.bottleneck_noise > 0 for p in model.plans.values())):
@@ -91,20 +114,29 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
       raise ValueError(f'weight_decay_mults: unknown parameter subtree {key!r}')
     decay_views.append((parts[0], parts[1] if len(parts) == 2 else None, float(mult)))
   dev = model.device
-  if mcfg.num_levels * 8 > models.Params.STATS_TAIL:
-    raise ValueError(f'num_levels {mcfg.num_levels} > {models.Params.STATS_TAIL // 8}')
+  stat_rows = mcfg.num_levels + (1 if robust else 0)
+  if stat_rows * 8 > models.Params.STATS_TAIL:
+    raise ValueError(f'num_levels {mcfg.num_levels} > {models.Params.STATS_TAIL // 8 - (1 if robust else 0)}')
 
   def stats_view(params):
     # the loss accumulators ride in the tail of the flat gradient buffer: one collective per step
     return params.stats_tail[:mcfg.num_levels * 8].view(mcfg.num_levels, 8)
+
+  def stats_rows(params):
+    # level rows, then (robustnerf) its own row: [loss_threshold, is_inlier_loss, has_inlier_neighbors,
+    # is_inlier_patch, mask, 0, 0, 0]
+    return params.stats_tail[:stat_rows * 8].view(stat_rows, 8)
   scratch = torch.zeros(4, device=dev)
-  dyn = torch.zeros(4, device=dev)               # lr, 1-b1^t, 1-b2^t, annealing exponent: ONE H2D copy per step
+  # lr, 1-b1^t, 1-b2^t, annealing exponent, robustnerf loss threshold: ONE H2D copy per step
+  dyn = torch.zeros(5, device=dev)
   # Pinned staging ring for the per-step scalars: the host may run several graph replays ahead of the
   # device, so a slot is rewritten only after the H2D copy that last read it has completed (event).
   DYN_SLOTS = 8
-  dyn_host = [torch.zeros(4).pin_memory() for _ in range(DYN_SLOTS)]
+  dyn_host = [torch.zeros(5).pin_memory() for _ in range(DYN_SLOTS)]
   dyn_events = [None] * DYN_SLOTS
   anneal_dev = dyn[3:4]
+  threshold_dev = dyn[4:5]
+  robust_counts = torch.zeros(5, dtype=torch.int32, device=dev) if robust else None   # left zero by every launch
   G = {'state': 0, 'fb': None, 'opt': None, 'rays': None, 'target': None, 'jitter': None,
        'noise': None, 'launches': 0}
   import os
@@ -148,11 +180,13 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
     params, states, rays = ctx['params'], ctx['states'], ctx['rays']
     st, fine, n = states[i], states[-1], len(states)
     is_fine = i == n - 1
+    data_mult = config.data_loss_mult if is_fine else config.data_coarse_loss_mult
+    data_mask = robust_level(ctx, st, is_fine) if robust and (is_fine or data_mult != 0) else None
     ops.composite_bwd(
         st.raw_density, st.raw_rgb, st.sdist, rays.directions, rays.near_flat, rays.far_flat,
         ctx['target'], ctx['lossmult'], ctx['inv_denom'], ctx['stats'][i], cfg=st.comp_cfg,
-        loss_type=config.data_loss_type, charb_padding=config.charb_padding,
-        data_mult=config.data_loss_mult if is_fine else config.data_coarse_loss_mult,
+        loss_type='mse' if robust else config.data_loss_type, charb_padding=config.charb_padding,
+        data_mult=data_mult, data_mask=data_mask,
         distortion_mult=config.distortion_loss_mult if is_fine else 0.0,
         interlevel_mult=0.0 if is_fine else config.interlevel_loss_mult,
         sdist_fine=None if is_fine else fine.sdist,
@@ -169,6 +203,25 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
       params.seg('exposure_scaling_offsets', params.grads).view(-1, 3).index_add_(0, eidx, g)
     model._mlp_backward(st, model.mlps[st.mname], rays=rays, impl=impl, loss_mults=st.loss_mults,
                         stats=ctx['stats'][i])
+
+  def robust_level(ctx, st, is_fine):
+    """robustnerf_mask of this level's pixels (train_utils.py:104-108) against the threshold in `threshold_dev`;
+    the final level also writes the stats row: its mask means and the quantile that is the next threshold."""
+    B = ctx['target'].shape[0]
+    p = config.patch_size
+    if not config.enable_robustnerf_loss and B % (p * p) != 0:
+      p = 1                        # the mask is all ones: any grouping of the rays into patches gives it
+    desc = ops.robust_desc(B, patch_size=p, inner_patch_size=config.robustnerf_inner_patch_size,
+                           filter_size=config.robustnerf_smoothed_filter_size,
+                           smoothed_inlier_quantile=config.robustnerf_smoothed_inlier_quantile,
+                           inner_patch_inlier_quantile=config.robustnerf_inner_patch_inlier_quantile,
+                           enable=config.enable_robustnerf_loss)
+    row = stats_rows(ctx['params'])[-1] if is_fine else None
+    mask, err = ops.robust_mask(st.comp['rgb'], ctx['target'], threshold_dev, desc,
+                                counts=robust_counts if is_fine else None, stats=row)
+    if is_fine:
+      ops.quantile(err, config.robustnerf_inlier_quantile, out=row[0:1])
+    return mask
 
   def split_level(n_levels, world):
     """Level after whose backward the first gradient segment is final (None: exchange everything at the end)."""
@@ -235,7 +288,7 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
     for mlp in model.mlps.values():
       mlp.repack()
 
-  def set_dyn(step, lr, anneal=1.0):
+  def set_dyn(step, lr, anneal=1.0, threshold=1.0):
     slot = G['dyn_slot'] = (G.get('dyn_slot', -1) + 1) % DYN_SLOTS
     if dyn_events[slot] is not None:
       dyn_events[slot].synchronize()
@@ -244,6 +297,7 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
     h[1] = 1.0 - config.adam_beta1 ** step
     h[2] = 1.0 - config.adam_beta2 ** step
     h[3] = anneal
+    h[4] = threshold
     dyn.copy_(h, non_blocking=True)
     if dyn_events[slot] is None:
       dyn_events[slot] = torch.cuda.Event()
@@ -283,7 +337,17 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
       out['density_noise'] = G['noise']
     return out
 
+  def stage_threshold(loss_threshold, in_dyn):
+    """Puts the robustnerf threshold in `threshold_dev` without a host sync: a device tensor by a device copy, a
+    Python float in the pinned `dyn` copy (in_dyn: set_dyn already carried it) or by a fill."""
+    if torch.is_tensor(loss_threshold):
+      threshold_dev.copy_(loss_threshold.reshape(1), non_blocking=True)
+    elif not in_dyn:
+      threshold_dev.fill_(float(loss_threshold))
+
   def train_step(rng, state, batch, cameras, train_frac, loss_threshold=1.0):
+    """`loss_threshold`: robustnerf inlier threshold of this step (train.py:109-129), a Python float or a 0-d
+    device tensor such as the previous step's `stats.device_loss_threshold()`."""
     world, _ = _world()
     params = state.params
     if model.params is not params:
@@ -299,6 +363,8 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
       rays = camera_utils.cast_ray_batch(cameras, rays, camtype, device=dev)
     rays = rays if hasattr(rays, 'radii_flat') else model._prep_rays(rays)
     B = rays.origins.shape[0]
+    if robust:
+      check_robust_config(config, B)
     target = torch.as_tensor(batch.rgb).to(dev, torch.float32).reshape(B, -1)[:, :3].contiguous()
     sched = model.level_schedule(train_frac)[2]
     n = len(sched)
@@ -308,15 +374,20 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
                              config.lr_delay_steps, config.lr_delay_mult)
     if not use_graph or G['state'] == 0:
       # eager step (also the warm-up that allocates every buffer before a capture)
+      if robust:
+        stage_threshold(loss_threshold, in_dyn=False)
       fwd_bwd(draw_randomness(rng, B, sched) if use_graph else rng, rays, target, train_frac, None, world)
       optim(grad_scale, params.step, lr, None)
       G['state'] = 1 if use_graph else 0
       G['B'] = B
-      return state, LazyStats(stats_view(params).clone(), n, grad_scale), rng
+      return state, LazyStats(stats_rows(params).clone(), n, grad_scale, robust_cfg), rng
     if G['B'] != B:
       raise ValueError(f'graph mode needs a fixed batch size ({G["B"]} rays per rank), got {B}')
     rand = draw_randomness(rng, B, sched)
-    set_dyn(params.step, lr, _anneal(mcfg, train_frac))
+    host_thr = float(loss_threshold) if robust and not torch.is_tensor(loss_threshold) else 1.0
+    set_dyn(params.step, lr, _anneal(mcfg, train_frac), host_thr)
+    if robust:
+      stage_threshold(loss_threshold, in_dyn=True)
     if G['state'] == 1:
       # capture: inputs live in static buffers from now on
       import dataclasses
@@ -388,8 +459,9 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
         allreduce_flat_(params, world)
       G['opt'].replay()
     ops.LAUNCHES += G['launches']
-    return state, LazyStats(stats_view(params).clone(), n, grad_scale), rng
+    return state, LazyStats(stats_rows(params).clone(), n, grad_scale, robust_cfg), rng
 
+  robust_cfg = {'enable': bool(config.enable_robustnerf_loss)} if robust else None
   train_step.graph_info = G
   return train_step
 
@@ -399,12 +471,25 @@ class LazyStats(dict):
   snapshot of the shared accumulator, so stats kept across steps stay distinct (train.py averages the
   print window)."""
 
-  def __init__(self, buf, n, scale=1.0):
+  def __init__(self, buf, n, scale=1.0, robust=None):
     super().__init__()
-    self._buf, self._n, self._scale = buf, n, scale
+    self._buf, self._n, self._scale, self._robust = buf, n, scale, robust
+
+  def device_loss_threshold(self):
+    """robustnerf: this step's next loss threshold as a 0-d device tensor, already the mean over processes
+    (train.py:129), for the next train_step without a host round trip."""
+    if self._robust is None:
+      raise KeyError('loss_threshold: data_loss_type is not robustnerf')
+    t = self._buf[-1, 0]
+    return t if self._scale == 1.0 else t * self._scale
 
   def materialize(self):
     b = self._buf.detach().cpu() * self._scale       # pmean of the per-rank stats: SUM all-reduce x 1/world
+    if self._robust is not None:
+      r, b = b[-1], b[:-1]
+      names = ROBUST_STAT_NAMES if self._robust['enable'] else ('loss_threshold', 'mask')
+      for k in names:
+        self[k] = float(r[ROBUST_STAT_NAMES.index(k)])
     mses = b[:, 1].clone()
     losses = {'data': float(b[:, 0].sum()), 'interlevel': float(b[:, 3].sum()),
               'distortion': float(b[:, 2].sum()), 'orientation': float(b[:, 4].sum()),
