@@ -415,6 +415,22 @@ int mnrf_pixels_to_rays(const mnrf_camera_desc* d, const int32_t* pix_x, const i
                         float* origins, float* directions, float* viewdirs, float* radii,
                         float* imageplane, mnrf_stream stream);
 
+/* camera_utils.cast_spherical_rays (camera_utils.py:716-763): an equirectangular 360-degree panorama of
+ * height x width pixels, the render_camtype = 'pano' path of datasets.py:486-492.  Computed in fp64 as the
+ * reference does: grid nodes theta = linspace(0, 2 pi, width + 1), phi = linspace(0, pi, height + 1) (numpy's
+ * rounding: node k = k * (stop / n), the last node exactly stop); pixel (x, y) looks along node (x, y),
+ * R [-sin(phi) sin(theta), cos(phi), sin(phi) cos(theta)] with R = camtoworld[:3, :3], not normalised;
+ * radii from the differences to nodes (x+1, y) and (x, y+1) as in mnrf_pixels_to_rays; origins = the
+ * camera position; imageplane = 0.  viewdirs = directions.
+ * Outputs are [height * width, 3|3|3|1|2] fp32, row-major with y outer; 64-bit ray indices. */
+typedef struct {
+  int32_t height, width;
+  double camtoworld[12];      /* [3, 4] row-major, by value: no device copy of the pose */
+} mnrf_spherical_desc;
+
+int mnrf_spherical_rays(const mnrf_spherical_desc* d, float* origins, float* directions, float* viewdirs,
+                        float* radii, float* imageplane, mnrf_stream stream);
+
 /* ---- optimizer ---------------------------------------------------------------------------
  * train_utils.clip_gradients (train_utils.py:200-218: value clip, then global-norm clip with
  * eps in the denominator), nan_to_num (:328) and optax.adam on one flat fp32 parameter

@@ -2,7 +2,8 @@
 
 `cast_ray_batch(cameras, pixels, camtype)` and `pixels_to_rays(...)` keep the reference's names,
 argument meaning and return order (camera_utils.py:522-688); the work is one launch of
-`mnrf_pixels_to_rays` (csrc/camera.cu).  The small host helpers (`intrinsic_matrix`,
+`mnrf_pixels_to_rays` (csrc/camera.cu).  `cast_spherical_rays(...)` (camera_utils.py:716-763) is one
+launch of `mnrf_spherical_rays`.  The small host helpers (`intrinsic_matrix`,
 `get_pixtocam`, `pixel_coordinates`) are the reference's one-liners in numpy.
 """
 import enum
@@ -43,13 +44,17 @@ def _dev(x, dtype, device):
 _checked = False
 
 
-def _launch(pix_x, pix_y, cam_idx, pixtocams, camtoworlds, distortion_params, pixtocam_ndc, camtype):
-  """All inputs flat on the device; returns the five [B, n] fp32 outputs."""
+def _load():
   global _checked
   if not _checked:
     L.require_device()          # queries device properties: once, not per launch
     _checked = True
-  lib = L.load()
+  return L.load()
+
+
+def _launch(pix_x, pix_y, cam_idx, pixtocams, camtoworlds, distortion_params, pixtocam_ndc, camtype):
+  """All inputs flat on the device; returns the five [B, n] fp32 outputs."""
+  lib = _load()
   B = pix_x.shape[0]
   dev = pix_x.device
   if isinstance(camtype, str):
@@ -122,6 +127,28 @@ def cast_ray_batch(cameras, pixels, camtype=ProjectionType.PERSPECTIVE, device='
   return utils.Rays(origins=rs(o), directions=rs(d), viewdirs=rs(v), radii=rs(r), imageplane=rs(ip),
                     lossmult=pixels.lossmult, near=pixels.near, far=pixels.far, cam_idx=pixels.cam_idx,
                     exposure_idx=pixels.exposure_idx, exposure_values=pixels.exposure_values)
+
+
+def cast_spherical_rays(camtoworld, height, width, near, far, device='cuda'):
+  """camera_utils.py:716-763: an equirectangular 360-degree panorama from the pose `camtoworld` ([3, 4] or
+  [4, 4], numpy or torch).  Returns utils.Rays of [height, width, n] CUDA tensors: fp32 fields and int32
+  `cam_idx` (0); `imageplane` is 0, `lossmult` 1, no exposure fields.  The rays are computed in float64 from
+  the pose as given, like the reference's `xnp=np` path, and rounded to fp32 once."""
+  height, width = int(height), int(width)
+  if height < 1 or width < 1:
+    raise ValueError(f'panorama size must be at least 1 x 1, got {height} x {width}')
+  c2w = np.asarray(camtoworld.detach().cpu() if isinstance(camtoworld, torch.Tensor) else camtoworld, np.float64)
+  if c2w.shape not in ((3, 4), (4, 4)):
+    raise ValueError(f'camtoworld must be [3, 4] or [4, 4], got {list(c2w.shape)}')
+  lib = _load()
+  d = L.SphericalDesc(height, width, (L.C.c_double * 12)(*c2w[:3, :4].reshape(-1)))
+  out = [torch.empty(height, width, n, device=device, dtype=torch.float32) for n in (3, 3, 3, 1, 2)]
+  from . import ops
+  ops._count()
+  L.check(lib.mnrf_spherical_rays(L.C.byref(d), *[L.ptr(t) for t in out], L.stream_ptr()))
+  full = lambda v, dtype: torch.full((height, width, 1), v, device=device, dtype=dtype)
+  return utils.Rays(*out, lossmult=full(1., torch.float32), near=full(near, torch.float32),
+                    far=full(far, torch.float32), cam_idx=full(0, torch.int32))
 
 
 # ------------------------------------------------------------------------------------------------

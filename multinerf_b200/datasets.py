@@ -9,7 +9,8 @@ Differences from the reference's host pipeline:
   * the reference's loader thread also casts the rays with numpy (datasets.py:452-455); here the thread only
     draws PIXELS (coordinates, camera indices, colours) and `__next__` turns them into rays with ONE
     launch of `mnrf_pixels_to_rays` on the device (or hands the pixels to the train step when
-    `cast_rays_in_train_step` is set) -- there is no CPU ray-casting path;
+    `cast_rays_in_train_step` is set) -- there is no CPU ray-casting path; a panorama
+    (`render_camtype='pano'`) is queued as its camera index and cast by `mnrf_spherical_rays`;
   * one process per GPU: every process draws `batch_size // world_size` rays from its own numpy
     stream (the reference seeds `20201473 + host_id`, train.py:47), nothing is re-sharded afterwards.
 
@@ -267,7 +268,12 @@ class Dataset(threading.Thread, metaclass=abc.ABCMeta):
     return utils.Batch(**batch)
 
   def _finish(self, batch):
-    """Device half: pixels -> rays (one kernel launch), unless the train step does it itself."""
+    """Device half: pixels -> rays (one kernel launch), unless the train step does it itself.  A panorama's
+    host item is its camera index alone: the whole panorama is cast on the device (datasets.py:488-492)."""
+    if not isinstance(batch, utils.Batch):
+      rays = camera_utils.cast_spherical_rays(self.camtoworlds[batch], self.height, self.width, self.near,
+                                              self.far, device=self.device)
+      return utils.Batch(rays=rays)
     if isinstance(batch.rays, utils.Rays):
       return batch
     if self._cast_rays_in_train_step and self.split == utils.DataSplit.TRAIN:
@@ -300,7 +306,7 @@ class Dataset(threading.Thread, metaclass=abc.ABCMeta):
 
   def _host_image_batch(self, cam_idx):
     if self._render_spherical:
-      raise NotImplementedError('spherical (pano) render cameras')
+      return cam_idx
     pix_x, pix_y = camera_utils.pixel_coordinates(self.width, self.height)
     return self._make_pixel_batch(pix_x, pix_y, cam_idx)
 

@@ -77,6 +77,10 @@ class CameraDesc(C.Structure):
               ('ndc_p12', C.c_float), ('ndc_near', C.c_float)]
 
 
+class SphericalDesc(C.Structure):
+  _fields_ = [('height', C.c_int32), ('width', C.c_int32), ('camtoworld', C.c_double * 12)]
+
+
 class PackItem(C.Structure):
   _fields_ = [('master', C.c_void_p), ('w_nk', C.c_void_p), ('w_kn', C.c_void_p), ('in_pad', C.c_int32),
               ('out', C.c_int32), ('tile0', C.c_int32), ('reserved', C.c_int32)]
@@ -143,6 +147,7 @@ _SIGNATURES = {
                         [_P] * 8),
     'mnrf_outer_mask': (C.c_int, [C.c_int64, C.c_int32, C.c_int64, _P, _P, _P, C.c_int64, _P, C.c_int64, _P]),
     'mnrf_pixels_to_rays': (C.c_int, [C.POINTER(CameraDesc)] + [_P] * 11),
+    'mnrf_spherical_rays': (C.c_int, [C.POINTER(SphericalDesc)] + [_P] * 6),
     'mnrf_clip_adam': (C.c_int, [C.POINTER(AdamDesc)] + [_P] * 6),
     'mnrf_clip_adam_dyn': (C.c_int, [C.POINTER(AdamDesc)] + [_P] * 7),
     'mnrf_pack_weights': (C.c_int, [C.c_int32, C.c_int32, _P, _P, _P, _P]),
