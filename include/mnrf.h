@@ -379,6 +379,24 @@ int mnrf_refdir_bwd(const mnrf_refdir_desc* d, const float* ide_mat, const int32
                     const float* d_raw_density, const float* d_raw_diffuse, const float* d_raw_tint,
                     float* d_grad_pred, float* d_raw_rough, float* d_raw_grad_density,
                     float* stats, mnrf_stream stream);
+/* Colourless form of the stage, for an MLP with disable_rgb (a proposal MLP) whose normals only feed
+ * the losses and the renderings: the normals, extra_dw and the loss adjoint of mnrf_refdir_fwd/bwd,
+ * with no direction encoding.  grad_pred [M, 3] (with normals_pred / d_grad_pred) and
+ * raw_grad_density [3, M] (with normals / d_raw_grad_density) may each be NULL, not both.
+ * viewdirs [M / num_samples, 3] are read only for the orientation loss; weights and stats only when a
+ * multiplier is > 0 (stats[4], stats[5] as above).  head_grads (optional, bf16 [M, ld_head_grads]):
+ * the backward writes [d_raw_density | d_grad_pred] to its columns 0..3 and leaves the others alone, so
+ * a zero-filled [M, 64] buffer is the A operand of one dgrad GEMM into the trunk against the K-major
+ * [w_density | W_grad_pred | 0]. */
+int mnrf_normals_fwd(int64_t M, int32_t num_samples, const float* grad_pred, const float* raw_grad_density,
+                     const float* viewdirs, float* normals_pred, float* normals, float orient_mult,
+                     float prednorm_mult, int32_t orient_on_pred, float* extra_dw /* [M] or NULL */,
+                     mnrf_stream stream);
+int mnrf_normals_bwd(int64_t M, int32_t num_samples, const float* grad_pred, const float* raw_grad_density,
+                     const float* viewdirs, const float* weights, float orient_mult, float prednorm_mult,
+                     int32_t orient_on_pred, const float* d_raw_density, float* d_grad_pred,
+                     float* d_raw_grad_density, mnrf_bf16* head_grads, int64_t ld_head_grads, float* stats,
+                     mnrf_stream stream);
 /* out[r, n] bf16 = maskbit(r mod mask_mod, n) ? rowv[r] * colv[n] : 0 -- the first dY of the
  * density-normal (tangent) backward chain. */
 int mnrf_outer_mask(int64_t rows, int32_t n, int64_t mask_mod, const float* rowv, const float* colv,

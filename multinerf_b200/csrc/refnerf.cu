@@ -293,6 +293,118 @@ refdir_bwd_kernel(RefDesc d, RefLoss L, const float* __restrict__ ide_mat, const
   }
 }
 
+// Colourless form of the stage: an MLP with disable_rgb (a proposal MLP) whose normals feed only the
+// orientation / predicted-normal losses and the renderings.  Same normals and loss arithmetic as
+// refdir_fwd/bwd, no direction encoding.  Kept apart from those kernels so that the Ref-NeRF stage's code
+// (and its bits) stay as they are.  A NULL grad_pred / raw_grad_density switches that normal off.
+__global__ void __launch_bounds__(128)
+normals_fwd_kernel(int64_t M, int S, const float* __restrict__ grad_pred,
+                   const float* __restrict__ raw_grad_density /* [3, M] */, const float* __restrict__ viewdirs,
+                   float* __restrict__ normals_pred, float* __restrict__ normals, RefLoss L,
+                   float* __restrict__ extra_dw) {
+  for (int64_t m = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; m < M; m += (int64_t)gridDim.x * blockDim.x) {
+    float np_[3] = {0.f, 0.f, 0.f}, nd[3] = {0.f, 0.f, 0.f}, s;
+    bool cl;
+    if (grad_pred) {
+      const float g[3] = {grad_pred[m * 3], grad_pred[m * 3 + 1], grad_pred[m * 3 + 2]};
+      neg_normalize(g, np_, s, cl);
+      normals_pred[m * 3] = np_[0]; normals_pred[m * 3 + 1] = np_[1]; normals_pred[m * 3 + 2] = np_[2];
+    }
+    if (raw_grad_density) {
+      const float g[3] = {raw_grad_density[m], raw_grad_density[M + m], raw_grad_density[2 * M + m]};
+      neg_normalize(g, nd, s, cl);
+      normals[m * 3] = nd[0]; normals[m * 3 + 1] = nd[1]; normals[m * 3 + 2] = nd[2];
+    }
+    if (extra_dw) {
+      float dw = 0.f;
+      if (L.orient_mult > 0.f) {
+        const int ray = (int)(m / S);
+        // selected by value, not through a pointer into the two arrays (which would put them on the stack)
+        const bool op = L.orient_on_pred;
+        float pm = fminf(0.f, -((op ? np_[0] : nd[0]) * viewdirs[ray * 3] + (op ? np_[1] : nd[1]) * viewdirs[ray * 3 + 1] +
+                                (op ? np_[2] : nd[2]) * viewdirs[ray * 3 + 2]));
+        dw += L.orient_mult * pm * pm;
+      }
+      if (L.prednorm_mult > 0.f) dw += L.prednorm_mult * (1.f - (nd[0] * np_[0] + nd[1] * np_[1] + nd[2] * np_[2]));
+      extra_dw[m] = dw;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(128)
+normals_bwd_kernel(int64_t M, int S, RefLoss L, const float* __restrict__ grad_pred,
+                   const float* __restrict__ raw_grad_density, const float* __restrict__ viewdirs,
+                   const float* __restrict__ weights, const float* __restrict__ d_raw_density,
+                   float* __restrict__ d_grad_pred, float* __restrict__ d_raw_grad_density /* [3, M] */,
+                   __nv_bfloat16* __restrict__ head_grads, int64_t ld_head_grads,
+                   float* __restrict__ stats /* [4]=orientation, [5]=pred normals */) {
+  float st_or = 0.f, st_pn = 0.f;
+  for (int64_t m = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; m < M; m += (int64_t)gridDim.x * blockDim.x) {
+    float np_[3] = {0.f, 0.f, 0.f}, nd[3] = {0.f, 0.f, 0.f}, s_p = 1.f, s_d = 1.f;
+    bool cl_p = false, cl_d = false;
+    if (grad_pred) {
+      const float g[3] = {grad_pred[m * 3], grad_pred[m * 3 + 1], grad_pred[m * 3 + 2]};
+      neg_normalize(g, np_, s_p, cl_p);
+    }
+    if (raw_grad_density) {
+      const float g[3] = {raw_grad_density[m], raw_grad_density[M + m], raw_grad_density[2 * M + m]};
+      neg_normalize(g, nd, s_d, cl_d);
+    }
+    float a_p[3] = {0.f, 0.f, 0.f}, a_d[3] = {0.f, 0.f, 0.f};
+    if (L.orient_mult > 0.f || L.prednorm_mult > 0.f) {
+      const float w = weights[m];
+      if (L.orient_mult > 0.f) {
+        const int ray = (int)(m / S);
+        const float v[3] = {viewdirs[ray * 3], viewdirs[ray * 3 + 1], viewdirs[ray * 3 + 2]};
+        const bool op = L.orient_on_pred;
+        float p = -((op ? np_[0] : nd[0]) * v[0] + (op ? np_[1] : nd[1]) * v[1] + (op ? np_[2] : nd[2]) * v[2]);
+        float pm = fminf(0.f, p);
+        st_or += L.orient_mult * w * pm * pm;
+        if (p < 0.f) {
+#pragma unroll
+          for (int i = 0; i < 3; ++i) {
+            const float a = L.orient_mult * w * 2.f * p * (-v[i]);
+            if (op) a_p[i] += a; else a_d[i] += a;
+          }
+        }
+      }
+      if (L.prednorm_mult > 0.f) {
+        float dot = nd[0] * np_[0] + nd[1] * np_[1] + nd[2] * np_[2];
+        st_pn += L.prednorm_mult * w * (1.f - dot);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+          a_p[i] += -L.prednorm_mult * w * nd[i];
+          a_d[i] += -L.prednorm_mult * w * np_[i];
+        }
+      }
+    }
+    float dgp[3] = {0.f, 0.f, 0.f};
+    if (grad_pred) {
+      neg_normalize_bwd(np_, s_p, cl_p, a_p, dgp);
+      d_grad_pred[m * 3] = dgp[0]; d_grad_pred[m * 3 + 1] = dgp[1]; d_grad_pred[m * 3 + 2] = dgp[2];
+    }
+    if (raw_grad_density) {
+      float dg[3];
+      neg_normalize_bwd(nd, s_d, cl_d, a_d, dg);
+      d_raw_grad_density[m] = dg[0]; d_raw_grad_density[M + m] = dg[1]; d_raw_grad_density[2 * M + m] = dg[2];
+    }
+    if (head_grads) {
+      // [d raw_density | d grad_pred]: the A operand of the dgrad GEMM into the trunk against [w_density | W_grad_pred]
+      __nv_bfloat16* hs = head_grads + m * ld_head_grads;
+      *reinterpret_cast<uint32_t*>(hs) = pack_bf16(d_raw_density[m], dgp[0]);
+      *reinterpret_cast<uint32_t*>(hs + 2) = pack_bf16(dgp[1], dgp[2]);
+    }
+  }
+  if (stats) {
+    st_or = warp_sum(st_or);
+    st_pn = warp_sum(st_pn);
+    if ((threadIdx.x & 31) == 0) {
+      if (st_or != 0.f) atomicAdd(&stats[4], st_or);
+      if (st_pn != 0.f) atomicAdd(&stats[5], st_pn);
+    }
+  }
+}
+
 // out[r, n] (bf16) = mask(r mod mod, n) ? rowv[r] * colv[n] : 0     (start of the tangent backward chain)
 __global__ void outer_mask_kernel(int64_t R, int N, int64_t mod, const float* __restrict__ rowv,
                                   const float* __restrict__ colv, const uint32_t* __restrict__ maskbits,
@@ -376,6 +488,54 @@ extern "C" int mnrf_outer_mask(int64_t rows, int32_t n, int64_t mask_mod, const 
   int blocks = (int)std::min<int64_t>((total + 255) / 256, (int64_t)mnrf_num_sms() * 16);
   outer_mask_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(rows, n, mask_mod, rowv, colv, maskbits, ldmaskbits,
                                                             reinterpret_cast<__nv_bfloat16*>(out), ldo);
+  MNRF_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int mnrf_normals_fwd(int64_t M, int32_t num_samples, const float* grad_pred, const float* raw_grad_density,
+                                const float* viewdirs, float* normals_pred, float* normals, float orient_mult,
+                                float prednorm_mult, int32_t orient_on_pred, float* extra_dw, mnrf_stream stream) {
+  using namespace mnrf;
+  if (M == 0) return 0;
+  MNRF_CHECK(grad_pred || raw_grad_density, "mnrf_normals_fwd: no normals to compute");
+  MNRF_CHECK(!grad_pred == !normals_pred && !raw_grad_density == !normals, "mnrf_normals_fwd: null pointer");
+  MNRF_CHECK(!extra_dw || !(orient_mult > 0.f) || (viewdirs && (orient_on_pred ? grad_pred : raw_grad_density)),
+             "Normals cannot be None if orientation loss is on.");
+  MNRF_CHECK(!extra_dw || !(prednorm_mult > 0.f) || (grad_pred && raw_grad_density),
+             "Predicted normals and gradient normals cannot be None if predicted normal loss is on.");
+  MNRF_CHECK(num_samples > 0, "mnrf_normals_fwd: num_samples must be positive");
+  int blocks = (int)std::min<int64_t>((M + 127) / 128, (int64_t)mnrf_num_sms() * 16);
+  normals_fwd_kernel<<<blocks, 128, 0, (cudaStream_t)stream>>>(
+      M, num_samples, grad_pred, raw_grad_density, viewdirs, normals_pred, normals,
+      RefLoss{orient_mult, prednorm_mult, orient_on_pred}, extra_dw);
+  MNRF_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int mnrf_normals_bwd(int64_t M, int32_t num_samples, const float* grad_pred, const float* raw_grad_density,
+                                const float* viewdirs, const float* weights, float orient_mult, float prednorm_mult,
+                                int32_t orient_on_pred, const float* d_raw_density, float* d_grad_pred,
+                                float* d_raw_grad_density, mnrf_bf16* head_grads, int64_t ld_head_grads,
+                                float* stats, mnrf_stream stream) {
+  using namespace mnrf;
+  if (M == 0) return 0;
+  MNRF_CHECK(grad_pred || raw_grad_density, "mnrf_normals_bwd: no normals to differentiate");
+  MNRF_CHECK(!grad_pred == !d_grad_pred && !raw_grad_density == !d_raw_grad_density, "mnrf_normals_bwd: null pointer");
+  const bool losses = orient_mult > 0.f || prednorm_mult > 0.f;
+  MNRF_CHECK(!losses || (weights && stats), "mnrf_normals_bwd: the losses need weights and a stats row");
+  MNRF_CHECK(!(orient_mult > 0.f) || (viewdirs && (orient_on_pred ? grad_pred : raw_grad_density)),
+             "Normals cannot be None if orientation loss is on.");
+  MNRF_CHECK(!(prednorm_mult > 0.f) || (grad_pred && raw_grad_density),
+             "Predicted normals and gradient normals cannot be None if predicted normal loss is on.");
+  MNRF_CHECK(!head_grads || (grad_pred && d_raw_density && ld_head_grads >= 4 && ld_head_grads % 2 == 0 &&
+                             (reinterpret_cast<uintptr_t>(head_grads) & 3) == 0),
+             "mnrf_normals_bwd: head_grads needs grad_pred, d_raw_density and 4 aligned columns");
+  MNRF_CHECK(num_samples > 0, "mnrf_normals_bwd: num_samples must be positive");
+  int blocks = (int)std::min<int64_t>((M + 127) / 128, (int64_t)mnrf_num_sms() * 16);
+  normals_bwd_kernel<<<blocks, 128, 0, (cudaStream_t)stream>>>(
+      M, num_samples, RefLoss{orient_mult, prednorm_mult, orient_on_pred}, grad_pred, raw_grad_density, viewdirs,
+      weights, d_raw_density, d_grad_pred, d_raw_grad_density, reinterpret_cast<__nv_bfloat16*>(head_grads),
+      ld_head_grads, losses ? stats : nullptr);
   MNRF_LAUNCH_CHECK();
   return 0;
 }

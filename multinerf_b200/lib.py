@@ -145,7 +145,10 @@ _SIGNATURES = {
     'mnrf_refdir_fwd': (C.c_int, [C.POINTER(RefdirDesc)] + [_P] * 10 + [C.c_float, C.c_float, C.c_int32, _P, _P]),
     'mnrf_refdir_bwd': (C.c_int, [C.POINTER(RefdirDesc)] + [_P] * 8 + [C.c_int32, C.c_float, C.c_float, C.c_int32] +
                         [_P] * 8),
-    'mnrf_outer_mask': (C.c_int, [C.c_int64, C.c_int32, C.c_int64, _P, _P, _P, C.c_int64, _P, C.c_int64, _P]),
+    'mnrf_normals_fwd': (C.c_int, [C.c_int64, C.c_int32] + [_P] * 5 + [C.c_float, C.c_float, C.c_int32, _P, _P]),
+    'mnrf_normals_bwd': (C.c_int, [C.c_int64, C.c_int32] + [_P] * 4 + [C.c_float, C.c_float, C.c_int32] + [_P] * 4 +
+                         [C.c_int64, _P, _P]),
+    'mnrf_outer_mask': (C.c_int,[C.c_int64, C.c_int32, C.c_int64, _P, _P, _P, C.c_int64, _P, C.c_int64, _P]),
     'mnrf_pixels_to_rays': (C.c_int, [C.POINTER(CameraDesc)] + [_P] * 11),
     'mnrf_spherical_rays': (C.c_int, [C.POINTER(SphericalDesc)] + [_P] * 6),
     'mnrf_clip_adam': (C.c_int, [C.POINTER(AdamDesc)] + [_P] * 6),

@@ -98,8 +98,11 @@ class MLPPlan:
     self.has_rgb = not cfg.disable_rgb
     self.use_viewdirs = use_viewdirs
     self.ref_stage = False
-    if (self.pred_normals or self.density_normals) and not self.has_rgb:
-      raise NotImplementedError('normals on an MLP with disable_rgb (no consumer on the CUDA path)')
+    # normals of a colourless MLP feed only the orientation / predicted-normal losses and the renderings
+    # (csrc/refnerf.cu normals_fwd/bwd)
+    self.normals_stage = (self.pred_normals or self.density_normals) and not self.has_rgb
+    # K of the trunk-top dgrad GEMM of such an MLP with predicted normals: [d raw_density | d grad_pred | 0]
+    self.normals_head_cols = 64 if (self.normals_stage and self.pred_normals) else 0
     if self.has_rgb:
       if not use_viewdirs:
         raise NotImplementedError('use_viewdirs=False with rgb is not wired into the CUDA path')
@@ -208,13 +211,16 @@ class MLPDevice:
     if getattr(self, 'colv_density', None) is None:
       self.colv_density = torch.zeros(d.in_pad, device=self.device)
     self.colv_density.copy_(self.w_nk[d.name][0])
-    if plan.ref_stage:
+    if plan.ref_stage or plan.normals_head_cols:
       # [x_pad, vin_pad] K-major B operand of the trunk-entry dgrad:  [ W_bottleneck | head weights ]
+      # (colourless MLP with predicted normals: [x_pad, 64] = [ w_density | W_grad_pred | 0 ])
       bt = plan.one('bottleneck')
-      bw = bt.out_dim
+      bw = bt.out_dim if plan.ref_stage else 0
       if not hasattr(self, 'wcat_kn'):
-        self.wcat_kn = torch.zeros(plan.x_pad, plan.vin_pad, device=self.device, dtype=torch.bfloat16)
-      self.wcat_kn[:, :bw] = self.w_kn[bt.name]
+        cols = plan.vin_pad if plan.ref_stage else plan.normals_head_cols
+        self.wcat_kn = torch.zeros(plan.x_pad, cols, device=self.device, dtype=torch.bfloat16)
+      if plan.ref_stage:
+        self.wcat_kn[:, :bw] = self.w_kn[bt.name]
       for role, (c0, n) in plan.HEAD_SLOTS.items():
         sp = plan.one(role)
         if sp is not None:
@@ -504,6 +510,12 @@ class Model:
         if cfg.enable_pred_roughness:
           st.roughness = torch.empty(M, device=dev)
         st.extra_dw = torch.empty(B, S, device=dev)
+    if plan.normals_stage:
+      if plan.pred_normals:
+        st.heads['grad_pred'] = torch.empty(M, 3, device=dev)
+        st.d_heads['grad_pred'] = torch.empty(M, 3, device=dev)
+        st.normals_pred = torch.empty(M, 3, device=dev)
+      st.extra_dw = torch.empty(B, S, device=dev)
     st.bwd = None   # backward scratch, allocated on first backward
     st.keep_acts = True     # False: render-only pass, the chained trunk skips activation / mask stores
     self._levels[key] = st
@@ -567,6 +579,13 @@ class Model:
         t = st.tacts[i]
       st.t_last = t
       ops.head_fwd(t, mlp.w_nk[d.name], None, 1, d.in_pad, raw=st.rgd.view(3 * M, 1))
+    if plan.normals_stage:
+      gp = plan.one('grad_pred')
+      if gp is not None:
+        ops.head_fwd(x, mlp.w_nk[gp.name], mlp.b(gp), gp.out_dim, gp.in_pad, raw=st.heads['grad_pred'])
+      om, pm, on_pred = loss_mults if loss_mults is not None else (0.0, 0.0, True)
+      ops.normals_fwd(M, S, st.heads.get('grad_pred'), st.rgd if plan.density_normals else None, rays.viewdirs,
+                      st.normals_pred, st.normals, om, pm, on_pred, st.extra_dw if loss_mults is not None else None)
     if not plan.has_rgb:
       return
     for role in ('grad_pred', 'diffuse', 'tint', 'roughness'):
@@ -636,7 +655,7 @@ class Model:
         if sp.in_pad == W + plan.Fpad:          # skip layer: [hidden | features] against [W | Fpad] weight columns
           ly.update(n_stream=nf, stream_col0=0, stream_kb0=W // 64)
       last = i == len(trunk) - 1
-      if st.keep_acts or (last and (plan.has_rgb or plan.last_has_feat)):
+      if st.keep_acts or (last and (plan.has_rgb or plan.last_has_feat or plan.pred_normals)):
         ly['out'] = st.acts[i][:, :W]
       if st.keep_acts:
         ly['maskbits'] = st.bits[i]
@@ -752,8 +771,9 @@ class Model:
           st.bneck_noise = rng['bottleneck_noise'][i].to(dev).reshape(B * lv['S'], bwid)
         else:
           st.bneck_noise = torch.randn(B * lv['S'], bwid, device=dev, generator=rng)
-      st.loss_mults = self.level_loss_mults(loss_config, i, B) if (loss_config is not None and
-                                                                   mlp.plan.ref_stage) else None
+      # levels of an MLP without normals skip the normal losses (the reference raises there instead)
+      st.loss_mults = self.level_loss_mults(loss_config, i, B) if (
+          loss_config is not None and (mlp.plan.ref_stage or mlp.plan.normals_stage)) else None
       if st.loss_mults is not None:
         om, pm, on_pred = st.loss_mults
         if (om > 0 and ((on_pred and not mlp.plan.pred_normals) or (not on_pred and not mlp.plan.density_normals))):
@@ -869,6 +889,8 @@ class Model:
         bw_.dv = [torch.empty(M, Wv, device=dev, dtype=bf) for _ in range(2)]
         bw_.d_vin = torch.empty(M, plan.vin_pad, device=dev, dtype=bf)
         bw_.d_vin_skip = torch.empty(M, plan.vin_pad, device=dev, dtype=bf) if plan.view_concat_after else None
+      # zero-filled once: the normals backward writes only its first four columns
+      bw_.dhead = torch.zeros(M, plan.normals_head_cols, device=dev, dtype=bf) if plan.normals_head_cols else None
       if plan.density_normals:
         bw_.h = [torch.empty(3 * M, W, device=dev, dtype=bf) for _ in range(2)]
       st.bwd = bw_
@@ -961,8 +983,24 @@ class Model:
         self.params.seg('Embed_0', self.params.grads).view(self.mcfg.num_glo_embeddings, -1).index_add_(
             0, rays.cam_idx[:, 0].long(), d_glo)
     else:
-      ops.head_bwd(x_last, mlp.w_nk[d.name], d_raw_density, 1, d.in_pad, dx=dy, relu_mask=True,
-                   dw=mlp.W(d, g), db=mlp.b(d, g), dxsum=None if side else mlp.b(trunk[-1], g))
+      if plan.normals_stage:
+        om, pm, on_pred = loss_mults if loss_mults is not None else (0.0, 0.0, True)
+        ops.normals_bwd(M, st.S, st.heads.get('grad_pred'), st.rgd if plan.density_normals else None,
+                        rays.viewdirs, st.comp['weights'], om, pm, on_pred, st.d_raw_density,
+                        st.d_heads.get('grad_pred'), st.d_rgd if plan.density_normals else None,
+                        head_grads=sc.dhead, stats=stats)
+      if plan.normals_head_cols:
+        # d x_last = relu'(x_last) * ([d raw_density | d grad_pred] @ [w_density | W_grad_pred]^T), with the bias
+        # gradient of the last trunk layer from the same epilogue
+        ops.gemm(L.GEMM_DGRAD, sc.dhead, mlp.wcat_kn, dy, m=M, n=W, k=plan.normals_head_cols,
+                 maskbits=st.bits[-1], colsum=None if side else mlp.b(trunk[-1], g), impl=impl)
+        gp = plan.one('grad_pred')
+        ops.head_bwd(x_last, mlp.w_nk[d.name], d_raw_density, 1, d.in_pad, dx=None, dw=mlp.W(d, g), db=mlp.b(d, g))
+        ops.head_bwd(x_last, mlp.w_nk[gp.name], st.d_heads['grad_pred'], gp.out_dim, gp.in_pad, dx=None,
+                     dw=mlp.W(gp, g), db=mlp.b(gp, g))
+      else:
+        ops.head_bwd(x_last, mlp.w_nk[d.name], d_raw_density, 1, d.in_pad, dx=dy, relu_mask=True,
+                     dw=mlp.W(d, g), db=mlp.b(d, g), dxsum=None if side else mlp.b(trunk[-1], g))
     if plan.density_normals:
       # adjoint of the tangent chain: H_last = relu'(x_last) * (d_rgd (x) w_density), three streams
       hcur, hoth = sc.h[0], sc.h[1]

@@ -423,6 +423,29 @@ def refdir_bwd(desc, ide_mat, ide_ml, grad_pred, raw_rough, raw_grad_density, vi
                               L.ptr(d_raw_rough), L.ptr(d_raw_grad_density), L.ptr(stats), L.stream_ptr()))
 
 
+def normals_fwd(M, S, grad_pred, raw_grad_density, viewdirs, normals_pred, normals, orient_mult=0.0,
+                prednorm_mult=0.0, orient_on_pred=True, extra_dw=None):
+  """Colourless normals stage (include/mnrf.h mnrf_normals_fwd): normals of an MLP without a colour branch."""
+  lib = L.load()
+  _count()
+  L.check(lib.mnrf_normals_fwd(M, S, L.ptr(_f32(grad_pred)), L.ptr(_f32(raw_grad_density)), L.ptr(_f32(viewdirs)),
+                               L.ptr(_f32(normals_pred)), L.ptr(_f32(normals)), float(orient_mult),
+                               float(prednorm_mult), int(orient_on_pred), L.ptr(_f32(extra_dw)), L.stream_ptr()))
+
+
+def normals_bwd(M, S, grad_pred, raw_grad_density, viewdirs, weights, orient_mult, prednorm_mult, orient_on_pred,
+                d_raw_density, d_grad_pred, d_raw_grad_density, head_grads=None, stats=None):
+  lib = L.load()
+  if head_grads is not None:
+    assert head_grads.dtype == torch.bfloat16 and head_grads.stride(1) == 1
+  _count()
+  L.check(lib.mnrf_normals_bwd(M, S, L.ptr(_f32(grad_pred)), L.ptr(_f32(raw_grad_density)), L.ptr(_f32(viewdirs)),
+                               L.ptr(_f32(weights)), float(orient_mult), float(prednorm_mult), int(orient_on_pred),
+                               L.ptr(_f32(d_raw_density)), L.ptr(_f32(d_grad_pred)), L.ptr(_f32(d_raw_grad_density)),
+                               L.ptr(head_grads), head_grads.stride(0) if head_grads is not None else 0,
+                               L.ptr(stats), L.stream_ptr()))
+
+
 def outer_mask(rowv, colv, maskbits, out, *, rows, n, mask_mod=0):
   lib = L.load()
   _count()
