@@ -67,6 +67,116 @@ struct RefLoss {
   int orient_on_pred;                 // orientation_loss_target == 'normals_pred'
 };
 
+// The normals and normal-loss arithmetic shared by the Ref-NeRF stage (refdir_*) and the colourless stage
+// (normals_*).  Both stages must produce the same bits for the same inputs, so each piece exists once.
+
+// One sample's normals_pred (p) and normals (d), zero when off, with the norms they were divided by
+// and whether those norms were clamped.
+struct Normals {
+  float p[3], d[3];
+  float s_p, s_d;
+  bool cl_p, cl_d;
+};
+
+__device__ __forceinline__ void load_viewdir(const float* __restrict__ viewdirs, int S, int64_t m, float v[3]) {
+  const int ray = (int)(m / S);
+  v[0] = viewdirs[ray * 3]; v[1] = viewdirs[ray * 3 + 1]; v[2] = viewdirs[ray * 3 + 2];
+}
+
+// normals_pred = -l2_normalize(grad_pred), normals = -l2_normalize(raw_grad_density); each is stored when its
+// output pointer is given
+__device__ __forceinline__ Normals load_normals(int64_t M, int64_t m, bool use_p, bool use_d,
+                                                const float* __restrict__ grad_pred,
+                                                const float* __restrict__ raw_grad_density /* [3, M] */,
+                                                float* __restrict__ normals_pred, float* __restrict__ normals) {
+  Normals n{{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}, 1.f, 1.f, false, false};
+  if (use_p) {
+    const float g[3] = {grad_pred[m * 3], grad_pred[m * 3 + 1], grad_pred[m * 3 + 2]};
+    neg_normalize(g, n.p, n.s_p, n.cl_p);
+    if (normals_pred) { normals_pred[m * 3] = n.p[0]; normals_pred[m * 3 + 1] = n.p[1]; normals_pred[m * 3 + 2] = n.p[2]; }
+  }
+  if (use_d) {
+    const float g[3] = {raw_grad_density[m], raw_grad_density[M + m], raw_grad_density[2 * M + m]};
+    neg_normalize(g, n.d, n.s_d, n.cl_d);
+    if (normals) { normals[m * 3] = n.d[0]; normals[m * 3 + 1] = n.d[1]; normals[m * 3 + 2] = n.d[2]; }
+  }
+  return n;
+}
+
+// -(n . v) for the normal the orientation loss reads.  Selected by value, not through a pointer into the two
+// arrays (which would put them on the stack).
+__device__ __forceinline__ float orient_p(const Normals& n, bool op, const float v[3]) {
+  return -((op ? n.p[0] : n.d[0]) * v[0] + (op ? n.p[1] : n.d[1]) * v[1] + (op ? n.p[2] : n.d[2]) * v[2]);
+}
+
+// d(orientation + predicted-normal loss)/d(weight of this sample): pure forward quantities
+__device__ __forceinline__ float loss_dw(const Normals& n, const float v[3], const RefLoss& L) {
+  float dw = 0.f;
+  if (L.orient_mult > 0.f) {
+    float pm = fminf(0.f, orient_p(n, L.orient_on_pred, v));
+    dw += L.orient_mult * pm * pm;
+  }
+  if (L.prednorm_mult > 0.f) dw += L.prednorm_mult * (1.f - (n.d[0] * n.p[0] + n.d[1] * n.p[1] + n.d[2] * n.p[2]));
+  return dw;
+}
+
+// The two losses at weight w: values added to st_or / st_pn, adjoints with respect to the normals to a_p / a_d
+// (the weights are differentiated through extra_dw)
+__device__ __forceinline__ void loss_bwd(const Normals& n, const float v[3], float w, const RefLoss& L, float a_p[3],
+                                         float a_d[3], float& st_or, float& st_pn) {
+  if (L.orient_mult > 0.f) {
+    const bool op = L.orient_on_pred;
+    float p = orient_p(n, op, v);
+    float pm = fminf(0.f, p);
+    st_or += L.orient_mult * w * pm * pm;
+    if (p < 0.f) {
+      // a += t * -v, fused explicitly: with the destination chosen by a branch the compiler does not always
+      // contract a product that both adds share
+      const float t = L.orient_mult * w * 2.f * p;
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+        if (op) a_p[i] = fmaf(t, -v[i], a_p[i]); else a_d[i] = fmaf(t, -v[i], a_d[i]);
+      }
+    }
+  }
+  if (L.prednorm_mult > 0.f) {
+    float dot = n.d[0] * n.p[0] + n.d[1] * n.p[1] + n.d[2] * n.p[2];
+    st_pn += L.prednorm_mult * w * (1.f - dot);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+      a_p[i] += -L.prednorm_mult * w * n.d[i];
+      a_d[i] += -L.prednorm_mult * w * n.p[i];
+    }
+  }
+}
+
+// Adjoint of load_normals: stores d grad_pred and d raw_grad_density [3, M] of the enabled normals and returns
+// d grad_pred (zero when off) in dgp
+__device__ __forceinline__ void normals_adjoint(const Normals& n, bool use_p, bool use_d, int64_t M, int64_t m,
+                                                const float a_p[3], const float a_d[3], float* __restrict__ d_grad_pred,
+                                                float* __restrict__ d_raw_grad_density, float dgp[3]) {
+  dgp[0] = dgp[1] = dgp[2] = 0.f;
+  if (use_p) {
+    neg_normalize_bwd(n.p, n.s_p, n.cl_p, a_p, dgp);
+    d_grad_pred[m * 3] = dgp[0]; d_grad_pred[m * 3 + 1] = dgp[1]; d_grad_pred[m * 3 + 2] = dgp[2];
+  }
+  if (use_d) {
+    float dg[3];
+    neg_normalize_bwd(n.d, n.s_d, n.cl_d, a_d, dg);
+    d_raw_grad_density[m] = dg[0]; d_raw_grad_density[M + m] = dg[1]; d_raw_grad_density[2 * M + m] = dg[2];
+  }
+}
+
+// stats[4] += orientation loss, stats[5] += predicted-normal loss, one atomic per warp
+__device__ __forceinline__ void add_loss_stats(float st_or, float st_pn, float* stats) {
+  st_or = warp_sum(st_or);
+  st_pn = warp_sum(st_pn);
+  if ((threadIdx.x & 31) == 0) {
+    if (st_or != 0.f) atomicAdd(&stats[4], st_or);
+    if (st_pn != 0.f) atomicAdd(&stats[5], st_pn);
+  }
+}
+
 __global__ void __launch_bounds__(128)
 refdir_fwd_kernel(RefDesc d, const float* __restrict__ ide_mat, const int* __restrict__ ide_ml, int ide_n,
                   const float* __restrict__ grad_pred, const float* __restrict__ raw_rough,
@@ -76,37 +186,18 @@ refdir_fwd_kernel(RefDesc d, const float* __restrict__ ide_mat, const int* __res
   __shared__ IdeTab tab;
   if (d.use_ide) load_tab(&tab, ide_mat, ide_ml, ide_n, (1 << (d.deg_view - 1)) + 1);
   for (int64_t m = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; m < d.M; m += (int64_t)gridDim.x * blockDim.x) {
-    const int ray = (int)(m / d.S);
-    const float v[3] = {viewdirs[ray * 3], viewdirs[ray * 3 + 1], viewdirs[ray * 3 + 2]};
-    float np_[3] = {0.f, 0.f, 0.f}, nd[3] = {0.f, 0.f, 0.f}, s;
-    bool cl;
-    if (d.use_pred_normals) {
-      const float g[3] = {grad_pred[m * 3], grad_pred[m * 3 + 1], grad_pred[m * 3 + 2]};
-      neg_normalize(g, np_, s, cl);
-      normals_pred[m * 3] = np_[0]; normals_pred[m * 3 + 1] = np_[1]; normals_pred[m * 3 + 2] = np_[2];
-    }
-    if (d.use_density_normals) {
-      const float g[3] = {raw_grad_density[m], raw_grad_density[d.M + m], raw_grad_density[2 * d.M + m]};
-      neg_normalize(g, nd, s, cl);
-      normals[m * 3] = nd[0]; normals[m * 3 + 1] = nd[1]; normals[m * 3 + 2] = nd[2];
-    }
-    const float* n = d.use_pred_normals ? np_ : nd;
+    float v[3];
+    load_viewdir(viewdirs, d.S, m, v);
+    const Normals nrm = load_normals(d.M, m, d.use_pred_normals, d.use_density_normals, grad_pred, raw_grad_density,
+                                     normals_pred, normals);
+    const bool up = d.use_pred_normals;
+    const float n[3] = {up ? nrm.p[0] : nrm.d[0], up ? nrm.p[1] : nrm.d[1], up ? nrm.p[2] : nrm.d[2]};
     float kappa = 0.f;
     if (d.use_roughness) {
       kappa = softplus_f(raw_rough[m] + d.roughness_bias);
       roughness[m] = kappa;
     }
-    if (extra_dw) {
-      // d(orientation + predicted-normal loss)/d(weight of this sample): pure forward quantities
-      float dw = 0.f;
-      if (L.orient_mult > 0.f) {
-        const float* no = L.orient_on_pred ? np_ : nd;
-        float pm = fminf(0.f, -(no[0] * v[0] + no[1] * v[1] + no[2] * v[2]));
-        dw += L.orient_mult * pm * pm;
-      }
-      if (L.prednorm_mult > 0.f) dw += L.prednorm_mult * (1.f - (nd[0] * np_[0] + nd[1] * np_[1] + nd[2] * np_[2]));
-      extra_dw[m] = dw;
-    }
+    if (extra_dw) extra_dw[m] = loss_dw(nrm, v, L);
     const float ndv = n[0] * v[0] + n[1] * v[1] + n[2] * v[2];
     float dir[3] = {v[0], v[1], v[2]};
     if (d.use_reflections) {
@@ -161,19 +252,12 @@ refdir_bwd_kernel(RefDesc d, RefLoss L, const float* __restrict__ ide_mat, const
   if (d.use_ide) load_tab(&tab, ide_mat, ide_ml, ide_n, (1 << (d.deg_view - 1)) + 1);
   float st_or = 0.f, st_pn = 0.f;
   for (int64_t m = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; m < d.M; m += (int64_t)gridDim.x * blockDim.x) {
-    const int ray = (int)(m / d.S);
-    const float v[3] = {viewdirs[ray * 3], viewdirs[ray * 3 + 1], viewdirs[ray * 3 + 2]};
-    float np_[3] = {0.f, 0.f, 0.f}, nd[3] = {0.f, 0.f, 0.f}, s_p = 1.f, s_d = 1.f;
-    bool cl_p = false, cl_d = false;
-    if (d.use_pred_normals) {
-      const float g[3] = {grad_pred[m * 3], grad_pred[m * 3 + 1], grad_pred[m * 3 + 2]};
-      neg_normalize(g, np_, s_p, cl_p);
-    }
-    if (d.use_density_normals) {
-      const float g[3] = {raw_grad_density[m], raw_grad_density[d.M + m], raw_grad_density[2 * d.M + m]};
-      neg_normalize(g, nd, s_d, cl_d);
-    }
-    const float* n = d.use_pred_normals ? np_ : nd;
+    float v[3];
+    load_viewdir(viewdirs, d.S, m, v);
+    const Normals nrm = load_normals(d.M, m, d.use_pred_normals, d.use_density_normals, grad_pred, raw_grad_density,
+                                     nullptr, nullptr);
+    const bool up = d.use_pred_normals;
+    const float n[3] = {up ? nrm.p[0] : nrm.d[0], up ? nrm.p[1] : nrm.d[1], up ? nrm.p[2] : nrm.d[2]};
     float kappa = 0.f, rin = 0.f;
     if (d.use_roughness) { rin = raw_rough[m] + d.roughness_bias; kappa = softplus_f(rin); }
     const float ndv = n[0] * v[0] + n[1] * v[1] + n[2] * v[2];
@@ -238,45 +322,15 @@ refdir_bwd_kernel(RefDesc d, RefLoss L, const float* __restrict__ ide_mat, const
     float a_p[3] = {0.f, 0.f, 0.f}, a_d[3] = {0.f, 0.f, 0.f};
     if (d.use_pred_normals) { a_p[0] = a_n[0]; a_p[1] = a_n[1]; a_p[2] = a_n[2]; }
     else { a_d[0] = a_n[0]; a_d[1] = a_n[1]; a_d[2] = a_n[2]; }
-    // ---- losses on the normals (weights are differentiated through extra_dw)
-    const float w = weights[m];
-    if (L.orient_mult > 0.f) {
-      const float* no = L.orient_on_pred ? np_ : nd;
-      float* ao = L.orient_on_pred ? a_p : a_d;
-      float p = -(no[0] * v[0] + no[1] * v[1] + no[2] * v[2]);
-      float pm = fminf(0.f, p);
-      st_or += L.orient_mult * w * pm * pm;
-      if (p < 0.f) {
-#pragma unroll
-        for (int i = 0; i < 3; ++i) ao[i] += L.orient_mult * w * 2.f * p * (-v[i]);
-      }
-    }
-    if (L.prednorm_mult > 0.f) {
-      float dot = nd[0] * np_[0] + nd[1] * np_[1] + nd[2] * np_[2];
-      st_pn += L.prednorm_mult * w * (1.f - dot);
-#pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        a_p[i] += -L.prednorm_mult * w * nd[i];
-        a_d[i] += -L.prednorm_mult * w * np_[i];
-      }
-    }
+    loss_bwd(nrm, v, weights[m], L, a_p, a_d, st_or, st_pn);
     float hg[11];                        // head gradients, in the column order of Wcat (models.py layout)
 #pragma unroll
     for (int i = 0; i < 11; ++i) hg[i] = 0.f;
     hg[0] = d_raw_density ? d_raw_density[m] : 0.f;
-    if (d.use_pred_normals) {
-      float dg[3];
-      neg_normalize_bwd(np_, s_p, cl_p, a_p, dg);
-      d_grad_pred[m * 3] = dg[0]; d_grad_pred[m * 3 + 1] = dg[1]; d_grad_pred[m * 3 + 2] = dg[2];
-      hg[1] = dg[0]; hg[2] = dg[1]; hg[3] = dg[2];
-    }
+    normals_adjoint(nrm, d.use_pred_normals, d.use_density_normals, d.M, m, a_p, a_d, d_grad_pred, d_raw_grad_density,
+                    hg + 1);
     if (d_raw_diffuse) { hg[4] = d_raw_diffuse[m * 3]; hg[5] = d_raw_diffuse[m * 3 + 1]; hg[6] = d_raw_diffuse[m * 3 + 2]; }
     if (d_raw_tint) { hg[7] = d_raw_tint[m * 3]; hg[8] = d_raw_tint[m * 3 + 1]; hg[9] = d_raw_tint[m * 3 + 2]; }
-    if (d.use_density_normals) {
-      float dg[3];
-      neg_normalize_bwd(nd, s_d, cl_d, a_d, dg);
-      d_raw_grad_density[m] = dg[0]; d_raw_grad_density[d.M + m] = dg[1]; d_raw_grad_density[2 * d.M + m] = dg[2];
-    }
     if (d.use_roughness) { hg[10] = dkappa * sigmoid_f(rin); d_raw_rough[m] = hg[10]; }
     // the consumed direction-encoding gradient columns are re-used for the head gradients: together
     // with the bottleneck gradient in columns [0, col0) they form the A operand of one dgrad GEMM
@@ -285,48 +339,25 @@ refdir_bwd_kernel(RefDesc d, RefLoss L, const float* __restrict__ ide_mat, const
     for (int i = 0; i < 11; ++i) hs[i] = __float2bfloat16(hg[i]);
     for (int i = 11; d.col0 + i < d.col_end; ++i) hs[i] = __float2bfloat16(0.f);
   }
-  st_or = warp_sum(st_or);
-  st_pn = warp_sum(st_pn);
-  if ((threadIdx.x & 31) == 0) {
-    if (st_or != 0.f) atomicAdd(&stats[4], st_or);
-    if (st_pn != 0.f) atomicAdd(&stats[5], st_pn);
-  }
+  add_loss_stats(st_or, st_pn, stats);
 }
 
 // Colourless form of the stage: an MLP with disable_rgb (a proposal MLP) whose normals feed only the
-// orientation / predicted-normal losses and the renderings.  Same normals and loss arithmetic as
-// refdir_fwd/bwd, no direction encoding.  Kept apart from those kernels so that the Ref-NeRF stage's code
-// (and its bits) stay as they are.  A NULL grad_pred / raw_grad_density switches that normal off.
+// orientation / predicted-normal losses and the renderings.  The normals and loss pieces of refdir_fwd/bwd, no
+// direction encoding.  A NULL grad_pred / raw_grad_density switches that normal off, and viewdirs / weights are
+// read only when a loss needs them.
 __global__ void __launch_bounds__(128)
 normals_fwd_kernel(int64_t M, int S, const float* __restrict__ grad_pred,
                    const float* __restrict__ raw_grad_density /* [3, M] */, const float* __restrict__ viewdirs,
                    float* __restrict__ normals_pred, float* __restrict__ normals, RefLoss L,
                    float* __restrict__ extra_dw) {
   for (int64_t m = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; m < M; m += (int64_t)gridDim.x * blockDim.x) {
-    float np_[3] = {0.f, 0.f, 0.f}, nd[3] = {0.f, 0.f, 0.f}, s;
-    bool cl;
-    if (grad_pred) {
-      const float g[3] = {grad_pred[m * 3], grad_pred[m * 3 + 1], grad_pred[m * 3 + 2]};
-      neg_normalize(g, np_, s, cl);
-      normals_pred[m * 3] = np_[0]; normals_pred[m * 3 + 1] = np_[1]; normals_pred[m * 3 + 2] = np_[2];
-    }
-    if (raw_grad_density) {
-      const float g[3] = {raw_grad_density[m], raw_grad_density[M + m], raw_grad_density[2 * M + m]};
-      neg_normalize(g, nd, s, cl);
-      normals[m * 3] = nd[0]; normals[m * 3 + 1] = nd[1]; normals[m * 3 + 2] = nd[2];
-    }
+    const Normals nrm = load_normals(M, m, grad_pred != nullptr, raw_grad_density != nullptr, grad_pred,
+                                     raw_grad_density, normals_pred, normals);
     if (extra_dw) {
-      float dw = 0.f;
-      if (L.orient_mult > 0.f) {
-        const int ray = (int)(m / S);
-        // selected by value, not through a pointer into the two arrays (which would put them on the stack)
-        const bool op = L.orient_on_pred;
-        float pm = fminf(0.f, -((op ? np_[0] : nd[0]) * viewdirs[ray * 3] + (op ? np_[1] : nd[1]) * viewdirs[ray * 3 + 1] +
-                                (op ? np_[2] : nd[2]) * viewdirs[ray * 3 + 2]));
-        dw += L.orient_mult * pm * pm;
-      }
-      if (L.prednorm_mult > 0.f) dw += L.prednorm_mult * (1.f - (nd[0] * np_[0] + nd[1] * np_[1] + nd[2] * np_[2]));
-      extra_dw[m] = dw;
+      float v[3] = {0.f, 0.f, 0.f};
+      if (L.orient_mult > 0.f) load_viewdir(viewdirs, S, m, v);
+      extra_dw[m] = loss_dw(nrm, v, L);
     }
   }
 }
@@ -340,54 +371,17 @@ normals_bwd_kernel(int64_t M, int S, RefLoss L, const float* __restrict__ grad_p
                    float* __restrict__ stats /* [4]=orientation, [5]=pred normals */) {
   float st_or = 0.f, st_pn = 0.f;
   for (int64_t m = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; m < M; m += (int64_t)gridDim.x * blockDim.x) {
-    float np_[3] = {0.f, 0.f, 0.f}, nd[3] = {0.f, 0.f, 0.f}, s_p = 1.f, s_d = 1.f;
-    bool cl_p = false, cl_d = false;
-    if (grad_pred) {
-      const float g[3] = {grad_pred[m * 3], grad_pred[m * 3 + 1], grad_pred[m * 3 + 2]};
-      neg_normalize(g, np_, s_p, cl_p);
-    }
-    if (raw_grad_density) {
-      const float g[3] = {raw_grad_density[m], raw_grad_density[M + m], raw_grad_density[2 * M + m]};
-      neg_normalize(g, nd, s_d, cl_d);
-    }
+    const bool use_p = grad_pred != nullptr, use_d = raw_grad_density != nullptr;
+    const Normals nrm = load_normals(M, m, use_p, use_d, grad_pred, raw_grad_density, nullptr, nullptr);
     float a_p[3] = {0.f, 0.f, 0.f}, a_d[3] = {0.f, 0.f, 0.f};
     if (L.orient_mult > 0.f || L.prednorm_mult > 0.f) {
-      const float w = weights[m];
-      if (L.orient_mult > 0.f) {
-        const int ray = (int)(m / S);
-        const float v[3] = {viewdirs[ray * 3], viewdirs[ray * 3 + 1], viewdirs[ray * 3 + 2]};
-        const bool op = L.orient_on_pred;
-        float p = -((op ? np_[0] : nd[0]) * v[0] + (op ? np_[1] : nd[1]) * v[1] + (op ? np_[2] : nd[2]) * v[2]);
-        float pm = fminf(0.f, p);
-        st_or += L.orient_mult * w * pm * pm;
-        if (p < 0.f) {
-#pragma unroll
-          for (int i = 0; i < 3; ++i) {
-            const float a = L.orient_mult * w * 2.f * p * (-v[i]);
-            if (op) a_p[i] += a; else a_d[i] += a;
-          }
-        }
-      }
-      if (L.prednorm_mult > 0.f) {
-        float dot = nd[0] * np_[0] + nd[1] * np_[1] + nd[2] * np_[2];
-        st_pn += L.prednorm_mult * w * (1.f - dot);
-#pragma unroll
-        for (int i = 0; i < 3; ++i) {
-          a_p[i] += -L.prednorm_mult * w * nd[i];
-          a_d[i] += -L.prednorm_mult * w * np_[i];
-        }
-      }
+      const float w = weights[m];      // issued before the ray index's division, which hides its latency
+      float v[3] = {0.f, 0.f, 0.f};
+      if (L.orient_mult > 0.f) load_viewdir(viewdirs, S, m, v);
+      loss_bwd(nrm, v, w, L, a_p, a_d, st_or, st_pn);
     }
-    float dgp[3] = {0.f, 0.f, 0.f};
-    if (grad_pred) {
-      neg_normalize_bwd(np_, s_p, cl_p, a_p, dgp);
-      d_grad_pred[m * 3] = dgp[0]; d_grad_pred[m * 3 + 1] = dgp[1]; d_grad_pred[m * 3 + 2] = dgp[2];
-    }
-    if (raw_grad_density) {
-      float dg[3];
-      neg_normalize_bwd(nd, s_d, cl_d, a_d, dg);
-      d_raw_grad_density[m] = dg[0]; d_raw_grad_density[M + m] = dg[1]; d_raw_grad_density[2 * M + m] = dg[2];
-    }
+    float dgp[3];
+    normals_adjoint(nrm, use_p, use_d, M, m, a_p, a_d, d_grad_pred, d_raw_grad_density, dgp);
     if (head_grads) {
       // [d raw_density | d grad_pred]: the A operand of the dgrad GEMM into the trunk against [w_density | W_grad_pred]
       __nv_bfloat16* hs = head_grads + m * ld_head_grads;
@@ -395,14 +389,7 @@ normals_bwd_kernel(int64_t M, int S, RefLoss L, const float* __restrict__ grad_p
       *reinterpret_cast<uint32_t*>(hs + 2) = pack_bf16(dgp[1], dgp[2]);
     }
   }
-  if (stats) {
-    st_or = warp_sum(st_or);
-    st_pn = warp_sum(st_pn);
-    if ((threadIdx.x & 31) == 0) {
-      if (st_or != 0.f) atomicAdd(&stats[4], st_or);
-      if (st_pn != 0.f) atomicAdd(&stats[5], st_pn);
-    }
-  }
+  if (stats) add_loss_stats(st_or, st_pn, stats);
 }
 
 // out[r, n] (bf16) = mask(r mod mod, n) ? rowv[r] * colv[n] : 0     (start of the tangent backward chain)

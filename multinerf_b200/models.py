@@ -240,6 +240,11 @@ class LevelState:
   pass
 
 
+def _loss_args(loss_mults):
+  """(orient_mult, prednorm_mult, orient_on_pred) of the normals kernels: both losses off without loss_mults."""
+  return loss_mults if loss_mults is not None else (0.0, 0.0, True)
+
+
 class Params:
   """`variables`: flat fp32 parameter/gradient/Adam buffers + per-module views."""
 
@@ -499,22 +504,16 @@ class Model:
         st.vin = torch.empty(M, plan.vin_pad, device=dev, dtype=bf)
       st.raw_rgb = torch.empty(B, S, 3, device=dev)
       st.d_raw_rgb = torch.empty(B, S, 3, device=dev)
-      for role in ('grad_pred', 'diffuse', 'tint', 'roughness'):
-        sp = plan.one(role)
-        if sp is not None:
-          st.heads[role] = torch.empty(M, sp.out_dim, device=dev)
-          st.d_heads[role] = torch.empty(M, sp.out_dim, device=dev)
-      if plan.ref_stage:
-        if plan.pred_normals:
-          st.normals_pred = torch.empty(M, 3, device=dev)
-        if cfg.enable_pred_roughness:
-          st.roughness = torch.empty(M, device=dev)
-        st.extra_dw = torch.empty(B, S, device=dev)
-    if plan.normals_stage:
+    for role in ('grad_pred', 'diffuse', 'tint', 'roughness'):
+      sp = plan.one(role)
+      if sp is not None:
+        st.heads[role] = torch.empty(M, sp.out_dim, device=dev)
+        st.d_heads[role] = torch.empty(M, sp.out_dim, device=dev)
+    if plan.ref_stage or plan.normals_stage:
       if plan.pred_normals:
-        st.heads['grad_pred'] = torch.empty(M, 3, device=dev)
-        st.d_heads['grad_pred'] = torch.empty(M, 3, device=dev)
         st.normals_pred = torch.empty(M, 3, device=dev)
+      if plan.ref_stage and cfg.enable_pred_roughness:
+        st.roughness = torch.empty(M, device=dev)
       st.extra_dw = torch.empty(B, S, device=dev)
     st.bwd = None   # backward scratch, allocated on first backward
     st.keep_acts = True     # False: render-only pass, the chained trunk skips activation / mask stores
@@ -536,7 +535,8 @@ class Model:
   # ------------------------------------------------------------------ forward
   def _mlp_forward(self, st: LevelState, mlp: MLPDevice, rays, impl=0, loss_mults=None):
     """loss_mults = (orientation, predicted-normal) multipliers of this level divided by the number
-    of rays, + orientation target flag: when given, the Ref-NeRF stage also emits d(loss)/d(weights)."""
+    of rays, + orientation target flag: when given, the normals stage (Ref-NeRF or colourless) also emits
+    d(loss)/d(weights)."""
     plan = mlp.plan
     cfg = plan.cfg
     B, S = st.B, st.S
@@ -579,19 +579,17 @@ class Model:
         t = st.tacts[i]
       st.t_last = t
       ops.head_fwd(t, mlp.w_nk[d.name], None, 1, d.in_pad, raw=st.rgd.view(3 * M, 1))
-    if plan.normals_stage:
-      gp = plan.one('grad_pred')
-      if gp is not None:
-        ops.head_fwd(x, mlp.w_nk[gp.name], mlp.b(gp), gp.out_dim, gp.in_pad, raw=st.heads['grad_pred'])
-      om, pm, on_pred = loss_mults if loss_mults is not None else (0.0, 0.0, True)
-      ops.normals_fwd(M, S, st.heads.get('grad_pred'), st.rgd if plan.density_normals else None, rays.viewdirs,
-                      st.normals_pred, st.normals, om, pm, on_pred, st.extra_dw if loss_mults is not None else None)
-    if not plan.has_rgb:
-      return
     for role in ('grad_pred', 'diffuse', 'tint', 'roughness'):
       sp = plan.one(role)
       if sp is not None:
         ops.head_fwd(x, mlp.w_nk[sp.name], mlp.b(sp), sp.out_dim, sp.in_pad, raw=st.heads[role])
+    om, pm, on_pred = _loss_args(loss_mults)
+    extra_dw = st.extra_dw if loss_mults is not None else None
+    if plan.normals_stage:
+      ops.normals_fwd(M, S, st.heads.get('grad_pred'), st.rgd if plan.density_normals else None, rays.viewdirs,
+                      st.normals_pred, st.normals, om, pm, on_pred, extra_dw)
+    if not plan.has_rgb:
+      return
     bt = plan.one('bottleneck')
     ops.gemm(L.GEMM_FWD, x, mlp.w_nk[bt.name], st.vin[:, :bt.out_dim], m=M, n=bt.out_dim,
              k=bt.in_pad, act=L.ACT_NONE, bias=mlp.b(bt), impl=impl)
@@ -602,11 +600,9 @@ class Model:
       desc = self._refdir_desc(st, plan)
       desc.ld = st.vin.stride(0)
       mat, ml, _ = mlp.ide_tables() if cfg.use_directional_enc else (None, None, 0)
-      om, pm, on_pred = loss_mults if loss_mults is not None else (0.0, 0.0, True)
       ops.refdir_fwd(desc, mat, ml, st.heads.get('grad_pred'), st.heads.get('roughness'),
                      st.rgd if plan.density_normals else None, rays.viewdirs, st.normals_pred, st.normals,
-                     st.roughness, st.vin, om, pm, on_pred,
-                     st.extra_dw if loss_mults is not None else None)
+                     st.roughness, st.vin, om, pm, on_pred, extra_dw)
     else:
       ops.viewdir_enc(rays.viewdirs, S, cfg.deg_view, st.vin, bt.out_dim, plan.vin_pad)
     if plan.glo_features > 0:
@@ -864,6 +860,15 @@ class Model:
     return self(rng, rays, train_frac, compute_extras, zero_glo)
 
   # ------------------------------------------------------------------ backward
+  def _narrow_heads_bwd(self, st: LevelState, mlp: MLPDevice):
+    """Parameter gradients of the narrow heads (x^T d_raw), accumulated into mlp.grads."""
+    g = mlp.grads
+    for role in ('grad_pred', 'diffuse', 'tint', 'roughness'):
+      sp = mlp.plan.one(role)
+      if sp is not None:
+        ops.head_bwd(st.x_last, mlp.w_nk[sp.name], st.d_heads[role], sp.out_dim, sp.in_pad, dx=None,
+                     dw=mlp.W(sp, g), db=mlp.b(sp, g))
+
   def _mlp_backward(self, st: LevelState, mlp: MLPDevice, rays=None, impl=0, loss_mults=None, stats=None):
     """Accumulates parameter gradients of one level into mlp.grads (fp32).
 
@@ -903,6 +908,7 @@ class Model:
     x_last = st.x_last
     dy = sc.dy[0]
     d_raw_density = st.d_raw_density.view(M, 1)
+    om, pm, on_pred = _loss_args(loss_mults)
     if plan.has_rgb:
       r = plan.one('rgb')
       views = plan.by_role('view')
@@ -939,18 +945,12 @@ class Model:
         desc = self._refdir_desc(st, plan)
         desc.ld = st.vin.stride(0)
         mat, ml, _ = mlp.ide_tables() if cfg.use_directional_enc else (None, None, 0)
-        om, pm, on_pred = loss_mults if loss_mults is not None else (0.0, 0.0, True)
         ops.refdir_bwd(desc, mat, ml, st.heads.get('grad_pred'), st.heads.get('roughness'),
                        st.rgd if plan.density_normals else None, rays.viewdirs, st.comp['weights'], sc.d_vin,
                        om, pm, on_pred, st.d_raw_density, st.d_heads.get('diffuse'), st.d_heads.get('tint'),
                        st.d_heads.get('grad_pred'), st.d_heads.get('roughness').view(M) if 'roughness' in st.d_heads else None,
                        st.d_rgd if plan.density_normals else None, stats)
-        # parameter gradients of the narrow heads (x^T d_raw)
-        for role in ('grad_pred', 'diffuse', 'tint', 'roughness'):
-          sp = plan.one(role)
-          if sp is not None:
-            ops.head_bwd(x_last, mlp.w_nk[sp.name], st.d_heads[role], sp.out_dim, sp.in_pad, dx=None,
-                         dw=mlp.W(sp, g), db=mlp.b(sp, g))
+        self._narrow_heads_bwd(st, mlp)
         # bottleneck dW + db, and the Dense(1) density head's dW from the same x_last tiles
         ops.gemm_wgrad(x_last, sc.d_vin[:, :bw], mlp.W(bt, g), m=bt.in_pad, n=bw, k=M, bsum=mlp.b(bt, g),
                        side_w=st.d_raw_density.view(M), side_aw=mlp.W(d, g).view(-1), impl=impl)
@@ -984,7 +984,6 @@ class Model:
             0, rays.cam_idx[:, 0].long(), d_glo)
     else:
       if plan.normals_stage:
-        om, pm, on_pred = loss_mults if loss_mults is not None else (0.0, 0.0, True)
         ops.normals_bwd(M, st.S, st.heads.get('grad_pred'), st.rgd if plan.density_normals else None,
                         rays.viewdirs, st.comp['weights'], om, pm, on_pred, st.d_raw_density,
                         st.d_heads.get('grad_pred'), st.d_rgd if plan.density_normals else None,
@@ -994,10 +993,8 @@ class Model:
         # gradient of the last trunk layer from the same epilogue
         ops.gemm(L.GEMM_DGRAD, sc.dhead, mlp.wcat_kn, dy, m=M, n=W, k=plan.normals_head_cols,
                  maskbits=st.bits[-1], colsum=None if side else mlp.b(trunk[-1], g), impl=impl)
-        gp = plan.one('grad_pred')
         ops.head_bwd(x_last, mlp.w_nk[d.name], d_raw_density, 1, d.in_pad, dx=None, dw=mlp.W(d, g), db=mlp.b(d, g))
-        ops.head_bwd(x_last, mlp.w_nk[gp.name], st.d_heads['grad_pred'], gp.out_dim, gp.in_pad, dx=None,
-                     dw=mlp.W(gp, g), db=mlp.b(gp, g))
+        self._narrow_heads_bwd(st, mlp)
       else:
         ops.head_bwd(x_last, mlp.w_nk[d.name], d_raw_density, 1, d.in_pad, dx=dy, relu_mask=True,
                      dw=mlp.W(d, g), db=mlp.b(d, g), dxsum=None if side else mlp.b(trunk[-1], g))

@@ -641,6 +641,55 @@ def test_refdir_stage_vs_oracle_autograd(ops, mode):
   close(hs[:, 10], d_rr.cpu().to(torch.bfloat16).float(), atol=0, rtol=0, msg='head slab roughness')
 
 
+@pytest.mark.parametrize('on_pred', [True, False])
+def test_normals_stage_matches_refdir_stage(ops, on_pred):
+  """The colourless stage (mnrf_normals_fwd/bwd) and the Ref-NeRF stage share their normals and normal-loss
+  arithmetic: with a zero direction-encoding gradient both give the same bits."""
+  rng = np.random.default_rng(43)
+  B, S = 37, 8
+  M = B * S
+  v = rng.normal(size=(B, 3)).astype(np.float32)
+  v /= np.linalg.norm(v, axis=-1, keepdims=True)
+  vt = torch.tensor(v).cuda()
+  gp = torch.tensor(rng.normal(size=(M, 3)).astype(np.float32))
+  rgd = torch.tensor(rng.normal(size=(3, M)).astype(np.float32) * 30.0)
+  gp[0] = 0.0          # clamped norms
+  rgd[:, 1] = 0.0
+  gp, rgd = gp.cuda(), rgd.cuda()
+  w = torch.tensor(rng.uniform(0, 0.2, M).astype(np.float32)).cuda()
+  drd = torch.tensor(rng.normal(size=M).astype(np.float32)).cuda()
+  om, pm = 0.1 / B, 3e-4 / B
+  col0, ld = 64, 128
+  desc = ops.refdir_desc(M, S, use_pred_normals=True, use_density_normals=True, use_reflections=False,
+                         use_ide=False, use_n_dot_v=False, use_roughness=False, deg_view=4, ide_n=0,
+                         roughness_bias=0.0, ld=ld, col0=col0, col_end=ld)
+  outs = []
+  for stage in ('refdir', 'normals'):
+    npd, nd_, edw = torch.empty(M, 3, device='cuda'), torch.empty(M, 3, device='cuda'), torch.empty(M, device='cuda')
+    d_gp, d_rgd = torch.empty(M, 3, device='cuda'), torch.empty(3, M, device='cuda')
+    stats = torch.zeros(8, device='cuda')
+    if stage == 'refdir':
+      slab = torch.empty(M, ld, dtype=torch.bfloat16, device='cuda')
+      ops.refdir_fwd(desc, None, None, gp, None, rgd, vt, npd, nd_, None, slab, om, pm, on_pred, edw)
+      d_slab = torch.zeros(M, ld, dtype=torch.bfloat16, device='cuda')
+      ops.refdir_bwd(desc, None, None, gp, None, rgd, vt, w, d_slab, om, pm, on_pred, drd, None, None, d_gp, None,
+                     d_rgd, stats)
+      heads = d_slab[:, col0:col0 + 4]
+    else:
+      ops.normals_fwd(M, S, gp, rgd, vt, npd, nd_, om, pm, on_pred, edw)
+      head_grads = torch.zeros(M, 64, dtype=torch.bfloat16, device='cuda')
+      ops.normals_bwd(M, S, gp, rgd, vt, w, om, pm, on_pred, drd, d_gp, d_rgd, head_grads=head_grads, stats=stats)
+      heads = head_grads[:, :4]
+    outs.append(dict(normals_pred=npd, normals=nd_, extra_dw=edw, d_grad_pred=d_gp, d_raw_grad_density=d_rgd,
+                     heads=heads, stats=stats[4:6]))
+  torch.cuda.synchronize()
+  ref, got = outs
+  assert (ref['extra_dw'] > 0).any() and (ref['stats'] > 0).all()
+  for k in ('normals_pred', 'normals', 'extra_dw', 'd_grad_pred', 'd_raw_grad_density', 'heads'):
+    assert torch.equal(got[k], ref[k]), k
+  close(got['stats'].cpu(), ref['stats'].cpu(), atol=0, rtol=1e-6, msg='loss stats')
+
+
 def test_outer_mask_and_gemm_mask_mod_addend(ops):
   from multinerf_b200 import lib as L
   rng = np.random.default_rng(51)
