@@ -102,7 +102,9 @@ int mnrf_encode(const mnrf_encode_desc* d, const float* sdist, const float* orig
                 float* tdist_out, mnrf_stream stream);
 /* Same, plus the tangent features d(feature)/d(mean_x|y|z) as three stacked bf16 blocks
  * tfeat[dir*B*S + m, ld_tfeat] (input of the forward-mode density-normal chain that replaces
- * vmap(value_and_grad(predict_density)), models.py:473-492).  Contraction is not supported here. */
+ * vmap(value_and_grad(predict_density)), models.py:473-492).  The derivative is taken with respect to
+ * the world-space mean: with warp_contract it runs through the contraction, including the dependence of
+ * the warped covariance J Sigma J^T on the mean (coord.track_linearize, coord.py:39-60). */
 int mnrf_encode_tangent(const mnrf_encode_desc* d, const float* sdist, const float* origins,
                         const float* directions, const float* radii, const float* near,
                         const float* far, const float* basis, mnrf_bf16* feat_bf16,

@@ -80,10 +80,44 @@ __device__ __forceinline__ void contract_gauss(Gauss& g) {
   for (int i = 0; i < 3; ++i) g.mean[i] = scale * x[i];
 }
 
-// smem: basis[3K] (block) | per warp: tdist[S+1] | gauss[S][13] | lift_mean[K] | lift_var[K] |
-//       row[feat_cols] bf16
-constexpr int kGaussStride = 13;   // 12 floats (mean 3 + cov 9), padded against bank conflicts
+// Tangent rows through the contraction.  z = s x and Sigma' = J Sigma J^T.  With r = |x|, xh = x / r and
+// P = xh xh^T, outside the unit ball J = s (I - P) + q P with s = 2/r - 1/r^2 and q = 1/r^2 (inside: J = I).
+// For a basis vector b write beta = xh.b, b_t = b - beta xh, u = J b = s b_t + q beta xh and v = Sigma u
+// (pre-warp Sigma), gamma = xh.v, v_t = v - gamma xh.  The lifted mean and variance move with world axis a as
+//   d(b.z)/dx_a          = u_a
+//   d(b^T Sigma' b)/dx_a = 2 [ xh_a (s_r (b_t.v) + q_r beta gamma) + s_r (beta (v_t)_a + gamma (b_t)_a) ]
+// with s_r = ds/dr = -2 (r - 1) / r^3 (which is also (q - s) / r, the factor of dP/dx) and q_r = -2 / r^3, both 0
+// inside the ball.  Every term there is of the size of the result: written with c = 2/r^4 - 2/r^3 in
+// J = s I + c x x^T instead, the terms grow with r against their sum and fp32 loses the variance term from
+// |x| ~ 1e3 on.  Phase A keeps xh (0 inside the ball), the pre-warp Sigma (6 unique entries) and (s, q, s_r, q_r)
+// beside the warped Gaussian.
+struct ContractTerms {
+  float xh[3], cov[6], s, q, s_r, q_r;
+};
 
+__device__ __forceinline__ void contract_terms(const Gauss& g, ContractTerms& t) {
+  const float x0 = g.mean[0], x1 = g.mean[1], x2 = g.mean[2];
+  t.cov[0] = g.cov[0][0]; t.cov[1] = g.cov[0][1]; t.cov[2] = g.cov[0][2];
+  t.cov[3] = g.cov[1][1]; t.cov[4] = g.cov[1][2]; t.cov[5] = g.cov[2][2];
+  const float m = fmaxf(kEps, x0 * x0 + x1 * x1 + x2 * x2);
+  t.xh[0] = t.xh[1] = t.xh[2] = 0.f;
+  t.s = 1.f; t.q = 1.f; t.s_r = 0.f; t.q_r = 0.f;
+  if (m <= 1.f) return;
+  const float r = sqrtf(m);
+  const float ir = 1.f / r;
+  t.xh[0] = x0 * ir; t.xh[1] = x1 * ir; t.xh[2] = x2 * ir;
+  t.s = 2.f / r - 1.f / m;
+  t.q = 1.f / m;
+  t.q_r = -2.f / (m * r);
+  t.s_r = (r - 1.f) * t.q_r;
+}
+
+// smem: basis[3K] (block) | per warp: tdist[S+1] | gauss[S][stride] | lift_mean[K] | lift_var[K] |
+//       (Contract: d lift_mean[3][K] | d lift_var[3][K]) | row[feat_cols] bf16 | 3 tangent rows
+constexpr int kGaussStride = 13;   // 12 floats (mean 3 + cov 9), padded against bank conflicts
+constexpr int kContractStride = 25;   // + xh 3, pre-warp cov 6, (s, q, s_r, q_r) 4: odd against bank conflicts
+
+template <bool Contract>
 __global__ void __launch_bounds__(256)
 encode_kernel(mnrf_encode_desc d, const float* __restrict__ sdist,
               const float* __restrict__ origins, const float* __restrict__ directions,
@@ -96,12 +130,15 @@ encode_kernel(mnrf_encode_desc d, const float* __restrict__ sdist,
   const int S = d.num_samples, K = d.basis_k, L = d.max_deg - d.min_deg, KL = K * L;
   float* sb = reinterpret_cast<float*>(smem_raw);                 // basis [K][3]
   const int row_bytes = ((d.feat_cols * 2 + 15) / 16) * 16;
-  const int per_warp_f = (S + 1) + S * kGaussStride + 2 * K;
+  constexpr int stride = Contract ? kContractStride : kGaussStride;
+  const int per_warp_f = (S + 1) + S * stride + (Contract ? 8 : 2) * K;
   float* wbase = sb + 3 * K + (size_t)wib * per_warp_f;
   float* tds = wbase;
   float* gs = tds + (S + 1);
-  float* lm = gs + S * kGaussStride;
+  float* lm = gs + S * stride;
   float* lv = lm + K;
+  float* dlm = lv + K;         // Contract only: [dir][K]
+  float* dlv = dlm + 3 * K;
   unsigned char* rows = smem_raw + (((size_t)(3 * K + nw * per_warp_f) * 4 + 15) / 16) * 16;
   const int rows_per_warp = tfeat ? 4 : 1;        // feature row + three tangent rows
   __nv_bfloat16* row = reinterpret_cast<__nv_bfloat16*>(rows + (size_t)wib * rows_per_warp * row_bytes);
@@ -132,8 +169,17 @@ encode_kernel(mnrf_encode_desc d, const float* __restrict__ sdist,
     for (int s = lane; s < S; s += 32) {
       Gauss g;
       cast_one(d.ray_shape, tds[s], tds[s + 1], o, dv, radius, g);
+      float* gp = gs + s * stride;
+      if (Contract) {
+        ContractTerms t;
+        contract_terms(g, t);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) gp[12 + i] = t.xh[i];
+#pragma unroll
+        for (int i = 0; i < 6; ++i) gp[15 + i] = t.cov[i];
+        gp[21] = t.s; gp[22] = t.q; gp[23] = t.s_r; gp[24] = t.q_r;
+      }
       if (d.warp_contract) contract_gauss(g);
-      float* gp = gs + s * kGaussStride;
       gp[0] = g.mean[0]; gp[1] = g.mean[1]; gp[2] = g.mean[2];
 #pragma unroll
       for (int i = 0; i < 3; ++i)
@@ -143,7 +189,7 @@ encode_kernel(mnrf_encode_desc d, const float* __restrict__ sdist,
     __syncwarp();
     // phase B: per sample, lift onto the basis and emit the 2*K*L features
     for (int s = 0; s < S; ++s) {
-      const float* gp = gs + s * kGaussStride;
+      const float* gp = gs + s * stride;
       for (int k = lane; k < K; k += 32) {
         float b0 = sb[k * 3 + 0], b1 = sb[k * 3 + 1], b2 = sb[k * 3 + 2];
         lm[k] = gp[0] * b0 + gp[1] * b1 + gp[2] * b2;
@@ -151,6 +197,33 @@ encode_kernel(mnrf_encode_desc d, const float* __restrict__ sdist,
         float c1 = gp[6] * b0 + gp[7] * b1 + gp[8] * b2;
         float c2 = gp[9] * b0 + gp[10] * b1 + gp[11] * b2;
         lv[k] = d.disable_integration ? 0.f : (b0 * c0 + b1 * c1 + b2 * c2);
+        if (Contract) {
+          const float b[3] = {b0, b1, b2};
+          const float* xh = gp + 12;
+          const float* cv = gp + 15;                 // xx xy xz yy yz zz
+          const float sj = gp[21], qj = gp[22], s_r = gp[23], q_r = gp[24];
+          const float beta = xh[0] * b0 + xh[1] * b1 + xh[2] * b2;
+          float bt[3], u[3], v[3], vt[3];
+#pragma unroll
+          for (int i = 0; i < 3; ++i) {
+            bt[i] = b[i] - beta * xh[i];
+            u[i] = sj * bt[i] + (qj * beta) * xh[i];
+          }
+          v[0] = cv[0] * u[0] + cv[1] * u[1] + cv[2] * u[2];
+          v[1] = cv[1] * u[0] + cv[3] * u[1] + cv[4] * u[2];
+          v[2] = cv[2] * u[0] + cv[4] * u[1] + cv[5] * u[2];
+          const float gamma = xh[0] * v[0] + xh[1] * v[1] + xh[2] * v[2];
+#pragma unroll
+          for (int i = 0; i < 3; ++i) vt[i] = v[i] - gamma * xh[i];
+          const float btv = bt[0] * v[0] + bt[1] * v[1] + bt[2] * v[2];
+          const float radial = s_r * btv + q_r * (beta * gamma);
+#pragma unroll
+          for (int a = 0; a < 3; ++a) {
+            dlm[a * K + k] = u[a];
+            dlv[a * K + k] = d.disable_integration ? 0.f
+                                                   : 2.f * (xh[a] * radial + s_r * (beta * vt[a] + gamma * bt[a]));
+          }
+        }
       }
       __syncwarp();
       const size_t m = (size_t)ray * S + s;
@@ -168,11 +241,22 @@ encode_kernel(mnrf_encode_desc d, const float* __restrict__ sdist,
           safe_sincos_fast(y + 1.57079637050628662109375f, s1, c1);
           fs = e * s0;
           fc = e * s1;
+          if (Contract) {
+            // d feature = e cos(y) sc d lift_mean - 1/2 sc^2 feature d lift_var
+            const float esc = e * sc, hsc2 = 0.5f * (sc * sc);
 #pragma unroll
-          for (int dir = 0; dir < 3; ++dir) {
-            const float bk = sb[k * 3 + dir] * sc * e;
-            trow[dir * trow_elems + f] = __float2bfloat16(c0 * bk);
-            trow[dir * trow_elems + KL + f] = __float2bfloat16(c1 * bk);
+            for (int dir = 0; dir < 3; ++dir) {
+              const float dm = dlm[dir * K + k] * esc, dvar = dlv[dir * K + k] * hsc2;
+              trow[dir * trow_elems + f] = __float2bfloat16(c0 * dm - fs * dvar);
+              trow[dir * trow_elems + KL + f] = __float2bfloat16(c1 * dm - fc * dvar);
+            }
+          } else {
+#pragma unroll
+            for (int dir = 0; dir < 3; ++dir) {
+              const float bk = sb[k * 3 + dir] * sc * e;
+              trow[dir * trow_elems + f] = __float2bfloat16(c0 * bk);
+              trow[dir * trow_elems + KL + f] = __float2bfloat16(c1 * bk);
+            }
           }
         } else {
           fs = e * safe_sin_fast(y);
@@ -421,7 +505,6 @@ static int encode_impl(const mnrf_encode_desc* d, const float* sdist, const floa
   using namespace mnrf;
   if (d && d->num_rays == 0) return 0;            // nothing to do (and empty tensors carry null pointers)
   if (tfeat) {
-    MNRF_CHECK(!d->warp_contract, "mnrf_encode_tangent: density normals with a contraction warp are not supported");
     MNRF_CHECK(ld_tfeat >= d->feat_cols && ld_tfeat % 8 == 0 && ((uintptr_t)tfeat % 16) == 0,
                "mnrf_encode_tangent: tangent rows must be 16-byte aligned");
   }
@@ -467,12 +550,15 @@ static int encode_impl(const mnrf_encode_desc* d, const float* sdist, const floa
     MNRF_LAUNCH_CHECK();
     return 0;
   }
-  size_t smem = (((size_t)(3 * d->basis_k + nw * ((d->num_samples + 1) + d->num_samples * kGaussStride +
-                                                   2 * d->basis_k)) * 4 + 15) / 16) * 16 +
+  const bool contract = d->warp_contract != 0;
+  const int stride = contract ? kContractStride : kGaussStride;
+  size_t smem = (((size_t)(3 * d->basis_k + nw * ((d->num_samples + 1) + d->num_samples * stride +
+                                                   (contract ? 8 : 2) * d->basis_k)) * 4 + 15) / 16) * 16 +
                 (size_t)nw * row_bytes * (tfeat ? 4 : 1);
   MNRF_CHECK(smem <= 200 * 1024, "mnrf_encode: shared memory %zu too large", smem);
-  MNRF_CUDA(cudaFuncSetAttribute(encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  encode_kernel<<<blocks, nw * 32, smem, (cudaStream_t)stream>>>(
+  auto kernel = contract ? encode_kernel<true> : encode_kernel<false>;
+  MNRF_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kernel<<<blocks, nw * 32, smem, (cudaStream_t)stream>>>(
       *d, sdist, origins, directions, radii, near, far, basis,
       reinterpret_cast<__nv_bfloat16*>(feat_bf16), feat_f32, tdist_out,
       reinterpret_cast<__nv_bfloat16*>(tfeat), ld_tfeat);

@@ -61,8 +61,6 @@ class MLPPlan:
     self.cfg = cfg
     self.density_normals = not cfg.disable_density_normals
     self.pred_normals = cfg.enable_pred_normals
-    if self.density_normals and cfg.warp_fn is not None:
-      raise NotImplementedError('density normals through a contraction warp')
     self.basis = np.ascontiguousarray(
         geopoly.generate_basis(cfg.basis_shape, cfg.basis_subdivisions), dtype=np.float32)
     self.K = self.basis.shape[0]

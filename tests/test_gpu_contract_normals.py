@@ -1,0 +1,369 @@
+"""Density normals through the scene contraction (`warp_fn = contract` with `disable_density_normals = False`):
+the tangent rows of csrc/encode.cu with warp_contract, and the normals, normal losses and Ref-NeRF stage of
+360-style models built on them, against the CPU oracle.  Needs an H100.
+
+Reference: internal/models.py:441-492 (vmap(value_and_grad(predict_density)) with respect to the world-space
+mean, through coord.track_linearize(contract, ...), coord.py:39-60).
+"""
+import numpy as np
+import pytest
+import torch
+
+from oracle import o_coord, o_models, o_render, o_train
+from util import close
+from test_gpu_model import mini360, oracle_rays, synth_rays, torch_tree
+from test_gpu_prop_normals import _bases, _grad_report
+
+pytestmark = pytest.mark.gpu
+
+
+@pytest.fixture(scope='module')
+def mods():
+  from multinerf_b200 import lib, models, train_utils
+  lib.require_device()
+  return models, train_utils
+
+
+# ------------------------------------------------------------------ kernel
+
+def _tangent_reference(means, covs, basis_t, maxdeg, mean_term_only=False):
+  """d(IPE feature)/d(world mean) by torch autograd in fp64, [3, B, S, F]."""
+  m = means.detach().clone().requires_grad_(True)
+  if mean_term_only:
+    jac = o_coord.contract_jacobian(m).detach()
+    z, c = o_coord.contract(m), jac @ covs @ jac.transpose(-1, -2)
+  else:
+    z, c = o_coord.track_linearize_contract(m, covs)
+  lm, lv = o_coord.lift_and_diagonalize(z, c, basis_t)
+  enc = o_coord.integrated_pos_enc(lm, lv, 0, maxdeg)
+  jac = torch.stack([torch.autograd.grad(enc[..., f].sum(), m, retain_graph=True)[0]
+                     for f in range(enc.shape[-1])], -1)
+  return jac.permute(2, 0, 1, 3), enc.detach()
+
+
+@pytest.mark.parametrize('rshape,no_integration,far', [('cone', False, False), ('cylinder', False, False),
+                                                       ('cone', True, False), ('cone', False, True)])
+def test_encode_tangent_through_contraction(mods, rshape, no_integration, far):
+  from multinerf_b200 import geopoly, ops
+  rng = np.random.default_rng(71)
+  B, S = 48, 16
+  # maxdeg 8 and cones 0.01-0.03 wide: the degrees where exp(-sc^2 var / 2) turns over, and with them the
+  # covariance term, carry weight against the bound's 2e-4 * max|d feature| floor
+  maxdeg = 8
+  o = torch.tensor(rng.uniform(-1, 1, (B, 3)).astype(np.float32))
+  d = rng.normal(size=(B, 3))
+  d = torch.tensor((d / np.linalg.norm(d, axis=-1, keepdims=True) * rng.uniform(0.8, 1.2, (B, 1))).astype(np.float32))
+  radii = torch.tensor(rng.uniform(0.01, 0.03, (B, 1)).astype(np.float32))
+  if far:
+    # an unbounded capture's ray: reciprocal distances out to 1e6, 1 - s log-uniform so that the samples reach
+    # |x| ~ 1e5, where the contraction's Jacobian is ~1e-10 and the variance term's parts span many decades
+    raydist, near, farv_ = 'reciprocal', 0.2, 1e6
+    sdist = torch.tensor(np.sort(1 - 10 ** rng.uniform(-6.5, 0, (B, S + 1)), -1).astype(np.float32))
+  else:
+    raydist, near, farv_ = None, 0.05, 4.0
+    sdist = torch.tensor(np.sort(rng.uniform(0, 1, (B, S + 1)).astype(np.float32), -1))
+  nearv, farv = torch.full((B, 1), near), torch.full((B, 1), farv_)
+  basis = torch.tensor(geopoly.generate_basis('octahedron', 1), dtype=torch.float32)
+  _, s_to_t = o_coord.construct_ray_warps(raydist, nearv, farv)
+  means, covs = o_render.cast_rays(s_to_t(sdist).double(), o.double(), d.double(), radii.double(), rshape,
+                                   diag=False)
+  mag = means.norm(dim=-1)
+  assert float((mag < 1).float().mean()) > 0.02 and float((mag > 1).float().mean()) > 0.5
+  if far:
+    assert float((mag > 1e4).float().mean()) > 0.1
+  if no_integration:
+    covs = torch.zeros_like(covs)
+  ref, enc = _tangent_reference(means, covs, basis.double().T.contiguous(), maxdeg)
+  F = ref.shape[-1]
+  M = B * S
+  feat = torch.empty(M, 128, dtype=torch.bfloat16, device='cuda')
+  tfeat = torch.empty(3 * M, 128, dtype=torch.bfloat16, device='cuda')
+  ops.encode(sdist.cuda(), o.cuda(), d.cuda(), radii[:, 0].contiguous().cuda(), nearv[:, 0].contiguous().cuda(),
+             farv[:, 0].contiguous().cuda(), basis.cuda(), min_deg=0, max_deg=maxdeg, raydist_fn=raydist,
+             ray_shape=rshape, warp_contract=True, disable_integration=no_integration, feat=feat, feat_cols=128, tfeat=tfeat)
+  got = tfeat.float().cpu().view(3, B, S, 128)[..., :F].double()
+
+  def bad_fraction(r):     # the bound of test_encode_tangent_features
+    scale = float(r.abs().max())
+    return float(((got - r).abs() > 1e-2 * r.abs() + 2e-4 * scale).float().mean())
+
+  def bad_fraction_far(r):  # the same bound with each sample's own scale, on the samples beyond |x| = 100
+    scale = r.abs().amax(dim=(0, 3), keepdim=True)
+    return float(((got - r).abs() > 1e-2 * r.abs() + 2e-4 * scale)[:, mag > 100].float().mean())
+  assert bad_fraction(ref) < 2e-3, bad_fraction(ref)
+  if far:
+    assert bad_fraction_far(ref) < 2e-3, bad_fraction_far(ref)
+  close(feat.float().cpu().view(B, S, 128)[..., :F], enc.float().to(torch.bfloat16).float(), atol=8e-3, rtol=0,
+        msg='features')
+  if not no_integration:
+    ref_mean, _ = _tangent_reference(means, covs, basis.double().T.contiguous(), maxdeg, mean_term_only=True)
+    assert bad_fraction(ref_mean) > 2e-2, bad_fraction(ref_mean)
+    if far:
+      assert bad_fraction_far(ref_mean) > 2e-2, bad_fraction_far(ref_mean)
+
+
+# ------------------------------------------------------------------ model
+
+def mini360_normals(refnerf=False):
+  """mini360 (reciprocal ray distances, contraction on both MLPs) with density and predicted normals on both
+  MLPs and both normal losses; refnerf: the NerfMLP also reflects the view direction, with the integrated
+  directional encoding and a predicted roughness."""
+  b = mini360()
+  for mlp in (b.prop_mlp, b.nerf_mlp):
+    mlp.disable_density_normals, mlp.enable_pred_normals = False, True
+  if refnerf:
+    n = b.nerf_mlp
+    n.use_reflections = n.use_directional_enc = n.enable_pred_roughness = True
+  c = b.config
+  c.orientation_loss_mult, c.orientation_coarse_loss_mult, c.orientation_loss_target = 0.1, 0.01, 'normals_pred'
+  c.predicted_normal_loss_mult, c.predicted_normal_coarse_loss_mult = 3e-4, 3e-5
+  c.grad_max_norm = c.grad_max_val = 0.0
+  return b
+
+
+# Where the bf16 arithmetic itself moves a quantity by more than the fixed bounds, the bound is derived from how
+# far the oracle's own bf16 evaluation lies from its fp32 one on the same inputs: the tensor-core path rounds at
+# other points than the oracle's bf16 emulation, so each may sit on either side of the fp32 value.
+SENSITIVITY = 2.5
+
+
+def _normals_errors(got, ref):
+  """(fraction of unit-length reference normals with cosine > 0.98, per-sample max abs error of the normals whose
+  raw gradient is under the eps clamp of l2_normalize)."""
+  unit = ref.norm(dim=-1) > 0.999
+  cos = (got * ref).sum(-1)[unit]
+  return float((cos > 0.98).float().mean()), (got - ref).abs().amax(-1)[~unit]
+
+
+def _check_normals(got, ref, what, inherent=None):
+  """Unit-length reference normals by cosine; those whose raw gradient is under the eps clamp (shorter than 1,
+  common far out where |J| ~ 1/|x|^2) by absolute error: there the normal is the raw gradient times
+  1/sqrt(eps) ~ 2900, so a bf16 chain's absolute error in a tiny gradient shows at that scale.  `inherent`: the
+  same errors of the oracle's fp32 normals against its bf16 ones, which widen the bounds."""
+  miss, atol = 0.03, 0.05
+  if inherent is not None:
+    frac_i, err_i = inherent
+    miss = max(miss, SENSITIVITY * (1.0 - frac_i))
+    if err_i.numel():
+      atol = max(atol, SENSITIVITY * float(torch.quantile(err_i, 0.97)))
+  frac, err = _normals_errors(got, ref)
+  assert frac > 1.0 - miss, (what, frac, miss)
+  if err.numel():
+    assert float((err < atol).float().mean()) > 0.97, (what, err.numel(), float(err.max()), atol)
+
+
+def _fp32_normals(params, bundle, model, orays, mname, sdist):
+  """The oracle's fp32 density normals at the samples `sdist` of one level."""
+  cfg = bundle.prop_mlp if mname == 'PropMLP_0' else bundle.nerf_mlp
+  _, s_to_t = o_coord.construct_ray_warps(bundle.model.raydist_fn, orays.near, orays.far)
+  gauss = o_render.cast_rays(s_to_t(sdist), orays.origins, orays.directions, orays.radii, bundle.model.ray_shape,
+                             diag=False)
+  out = o_models.mlp_apply(params[mname], cfg, model.plans[mname].basis, gauss, viewdirs=orays.viewdirs, bf16=False)
+  return out['normals'].detach()
+
+
+def _forward_vs_oracle(models, bundle, rays, rand, seed, dens_lim, pix_atol, derived=False):
+  from multinerf_b200 import ops
+  B = rays.origins.shape[0]
+  model, _ = models.construct_model(seed, rays, bundle)
+  params = torch_tree(model.export_flax())
+  rend_o, hist_o = o_models.model_apply(params, bundle, _bases(model), oracle_rays(rays), 0.5, True, rand=rand,
+                                        bf16=True)
+  rend_o = [{k: v.detach() for k, v in r.items()} for r in rend_o]
+  hist_o = [{k: (v.detach() if v is not None else None) for k, v in h.items()} for h in hist_o]
+  r = model._prep_rays(rays)
+  pred = bundle.nerf_mlp.enable_pred_normals
+  n_clamped = 0
+  for i, st in enumerate(model.forward_levels(rand, r, 0.5, True, True)):
+    # sample positions of level i pinned to the oracle's: one level's MLP and normals stage in isolation
+    st.sdist.copy_(hist_o[i]['sdist'].cuda())
+    model._mlp_forward(st, model.mlps[st.mname], r)
+    comp = ops.composite_fwd(st.raw_density, st.raw_rgb, st.sdist, r.directions, r.near_flat, r.far_flat,
+                             cfg=st.comp_cfg, raw_diffuse=st.heads.get('diffuse'), raw_tint=st.heads.get('tint'),
+                             want_samples=True, want_extras=True)
+    torch.cuda.synchronize()
+    Sx = st.S
+    err = (comp['density'].cpu() - hist_o[i]['density']).abs() / (1.0 + hist_o[i]['density'].abs())
+    assert float(err.max()) < dens_lim[0] and float(err.mean()) < dens_lim[1], (i, float(err.max()), float(err.mean()))
+    close(comp['weights'], hist_o[i]['weights'], atol=2e-2, rtol=0, msg=f'weights level {i}')
+    close(comp['rgb'], rend_o[i]['rgb'], atol=pix_atol, rtol=0, msg=f'pixel level {i}')
+    inherent = None
+    if derived:
+      inherent = _normals_errors(_fp32_normals(params, bundle, model, oracle_rays(rays), st.mname, hist_o[i]['sdist']),
+                                 hist_o[i]['normals'])
+      print(f'level {i}: oracle fp32 vs bf16 normals {inherent[0]:.4f}, clamped '
+            f'{float(inherent[1].max()) if inherent[1].numel() else 0.0:.3f}; GPU vs oracle bf16 normals '
+            f'{_normals_errors(st.normals.cpu().view(B, Sx, 3), hist_o[i]["normals"])[0]:.4f}')
+    _check_normals(st.normals.cpu().view(B, Sx, 3), hist_o[i]['normals'], f'normals level {i}', inherent)
+    n_clamped += int((hist_o[i]['normals'].norm(dim=-1) < 0.999).sum())
+    if pred:
+      _check_normals(st.normals_pred.cpu().view(B, Sx, 3), hist_o[i]['normals_pred'], f'normals_pred level {i}')
+  print(f'samples under the eps clamp: {n_clamped}')
+  rend, hist = model(rand, rays, 0.5, True)
+  torch.cuda.synchronize()
+  for i in range(len(hist)):
+    assert 'normals' in rend[i] and hist[i]['normals'] is not None and hist[i]['raw_grad_density'] is not None, i
+  close(rend[-1]['rgb'], rend_o[-1]['rgb'], atol=3e-2, rtol=0, msg='final pixel end-to-end')
+
+
+def _oracle_sensitivity(grads_a, grads_b):
+  """Per leaf (rel, cos) of two oracle gradient sets."""
+  out = {}
+  for k, b in grads_b.items():
+    a, b = grads_a[k].double().flatten(), b.double().flatten()
+    if float(b.norm()) > 0.0:
+      out[k] = (float((a - b).norm() / b.norm()), float((a @ b) / (a.norm() * b.norm()).clamp(min=1e-30)))
+  return out
+
+
+def _train_step_vs_oracle(models, train_utils, bundle, rays, rand, target, seed, lim, derived=False):
+  from multinerf_b200 import utils
+  model, variables = models.construct_model(seed, rays, bundle)
+  params0 = torch_tree(model.export_flax())
+  opt0 = {'count': 0, 'mu': {}, 'nu': {}}
+  _, _, stats_o, grads_o = o_train.train_step(params0, opt0, bundle, _bases(model), oracle_rays(rays),
+                                              torch.tensor(target), 0.5, rand=rand, bf16=True)
+  step_fn = train_utils.create_train_step(model, bundle.config)
+  state = train_utils.TrainState(variables)
+  state, stats, _ = step_fn(rand, state, utils.Batch(rays=rays, rgb=target), None, 0.5)
+  torch.cuda.synchronize()
+  stats.materialize()
+  close(stats['mses'], stats_o['mses'].detach(), atol=2e-3, rtol=3e-2, msg='mses')
+  sens, stats_32 = {}, None
+  if derived:
+    _, _, stats_32, grads_32 = o_train.train_step(params0, opt0, bundle, _bases(model), oracle_rays(rays),
+                                                  torch.tensor(target), 0.5, rand=rand, bf16=False)
+    sens = _oracle_sensitivity(grads_o, grads_32)
+  seen = 0
+  for k in ('orientation', 'predicted_normals'):
+    if k in stats_o['losses'] and float(stats_o['losses'][k].detach()) != 0.0:
+      lo = float(stats_o['losses'][k].detach())
+      rel = 0.05
+      if stats_32 is not None:
+        rel = max(rel, SENSITIVITY * abs(float(stats_32['losses'][k].detach()) - lo) / abs(lo))
+      assert abs(stats['losses'][k] - lo) < rel * abs(lo) + 1e-7, (k, stats['losses'][k], lo, rel)
+      seen += 1
+  assert seen > 0
+  report = _grad_report(model, grads_o, leaves=('kernel', 'bias'))
+  worst = sorted(report.items(), key=lambda kv: -kv[1][0])[:6]
+  print(f'worst leaves (rel, cos): {worst}')
+  if sens:
+    print('oracle bf16 vs fp32 at those leaves:', {k[:2] + (k[2],): tuple(round(x, 4) for x in sens.get(k, (0, 1)))
+                                                   for k, _ in worst})
+
+  def bound(k):
+    rel_i, cos_i = sens.get(k, (0.0, 1.0))
+    return max(lim[0], SENSITIVITY * rel_i), min(lim[1], 1.0 - SENSITIVITY * (1.0 - cos_i))
+  bad = {k: (v, bound(k)) for k, v in report.items() if not (v[0] < bound(k)[0] and v[1] > bound(k)[1])}
+  assert not bad, (bad, worst)
+
+
+def _mini_case(bundle, B, seed):
+  rays, rng = synth_rays(seed, B, 0.2, 1e6)
+  S = [bundle.model.num_prop_samples] * (bundle.model.num_levels - 1) + [bundle.model.num_nerf_samples]
+  rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, 1 if bundle.model.single_jitter else s)).astype(np.float32))
+                     for s in S]}
+  target = rng.uniform(0, 1, (B, 3)).astype(np.float32)
+  return rays, rand, target
+
+
+@pytest.mark.parametrize('refnerf', [False, True])
+def test_forward_vs_oracle(mods, refnerf):
+  models, _ = mods
+  bundle = mini360_normals(refnerf)
+  rays, rand, _ = _mini_case(bundle, 128, 150)
+  _forward_vs_oracle(models, bundle, rays, rand, 151, (0.08, 4e-3), 1.5e-2)
+
+
+@pytest.mark.parametrize('target', ['normals_pred', 'normals'])
+def test_train_step_vs_oracle(mods, target):
+  models, train_utils = mods
+  bundle = mini360_normals()
+  bundle.config.orientation_loss_target = target
+  # the PropMLP's gradient then comes from the normal losses alone: the tangent rows through the contraction
+  # and their adjoint are not hidden behind the interlevel loss
+  bundle.config.interlevel_loss_mult = 0.0
+  rays, rand, target_rgb = _mini_case(bundle, 128, 160)
+  # orientation on the density normals: the loss's gradient runs through the samples under the eps clamp, where
+  # it is scaled by 1/sqrt(eps); there the oracle's bf16 and fp32 evaluations already differ at the density head
+  _train_step_vs_oracle(models, train_utils, bundle, rays, rand, target_rgb, 161, (0.2, 0.98),
+                        derived=target == 'normals')
+
+
+def fullwidth360_normals():
+  """360.gin as shipped with density normals on both MLPs and the orientation loss on them."""
+  from multinerf_b200 import configs
+  b = configs.bundle_360()
+  b.prop_mlp.disable_density_normals = b.nerf_mlp.disable_density_normals = False
+  b.config.orientation_loss_mult, b.config.orientation_coarse_loss_mult = 0.1, 0.01
+  b.config.orientation_loss_target = 'normals'
+  b.config.grad_max_norm = b.config.grad_max_val = 0.0
+  return b
+
+
+def test_fullwidth_forward_vs_oracle(mods):
+  from test_gpu_fullwidth import _case
+  models, _ = mods
+  _, rays, _, rand, _, _ = _case('360')
+  _forward_vs_oracle(models, fullwidth360_normals(), rays, rand, 40, (0.1, 5e-3), 1.5e-2, derived=True)
+
+
+def test_fullwidth_train_step_vs_oracle(mods):
+  from test_gpu_fullwidth import _case
+  models, train_utils = mods
+  _, rays, target, rand, _, _ = _case('360')
+  _train_step_vs_oracle(models, train_utils, fullwidth360_normals(), rays, rand, target, 41, (0.3, 0.95),
+                        derived=True)
+
+
+def test_cuda_graph_matches_eager(mods):
+  models, train_utils = mods
+  from multinerf_b200 import utils
+  bundle = mini360_normals()
+  B, steps = 192, 5
+  rng = np.random.default_rng(93)
+  batches = []
+  for _ in range(steps):
+    rays, _ = synth_rays(int(rng.integers(1 << 30)), B, 0.2, 1e6)
+    rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B,)).astype(np.float32)) for _ in range(3)]}
+    batches.append((rays, rng.uniform(0, 1, (B, 3)).astype(np.float32), rand))
+  results = []
+  for use_graph in [False, True]:
+    model, variables = models.construct_model(8, batches[0][0], bundle)
+    step_fn = train_utils.create_train_step(model, bundle.config, use_graph=use_graph)
+    state = train_utils.TrainState(variables)
+    losses, orient = [], []
+    for i, (rays, tgt, rand) in enumerate(batches):
+      state, stats, _ = step_fn(rand, state, utils.Batch(rays=rays, rgb=tgt), None, i / 10.0)
+      s = stats.materialize()
+      losses.append(s['loss'])
+      orient.append(s['losses']['orientation'])
+    torch.cuda.synchronize()
+    results.append((losses, orient, variables.flat.clone()))
+    if use_graph:
+      assert step_fn.graph_info['state'] == 2, step_fn.graph_info['state']
+  (l0, o0, p0), (l1, o1, p1) = results
+  for a, b in zip(l0 + o0, l1 + o1):
+    assert abs(a - b) < 2e-3 * max(1.0, abs(a)), (l0, l1, o0, o1)
+  assert float((p0 - p1).norm() / p0.norm()) < 2e-3
+
+
+def test_render_image_normals_chunked_equals_direct_call(mods):
+  models, train_utils = mods
+  from test_gpu_render import _image_rays
+  bundle = mini360_normals()
+  H, W = 29, 41
+  bundle.config.render_chunk_size = 256
+  bundle.config.vis_num_rays = 8
+  rays = _image_rays(H, W, focal=40.0)          # origin inside the unit ball, near 0.2, far 1e6
+  model, state, render_eval_pfn, _, _ = train_utils.setup_model(bundle, 3)
+  out = models.render_image(lambda rng, r: render_eval_pfn(state.params, 1.0, None, r), rays, None, bundle,
+                            verbose=False)
+  flat = rays.map(lambda a: a.reshape(H * W, -1))
+  rend, hist = model(None, flat, 1.0, True)
+  torch.cuda.synchronize()
+  for i, r in enumerate(rend):
+    assert 'normals' in r and 'normals_pred' in r and hist[i]['normals'] is not None, i
+    assert torch.isfinite(r['normals']).all() and torch.isfinite(r['normals_pred']).all()
+  for k in ('rgb', 'acc', 'normals', 'normals_pred'):
+    assert torch.equal(out[k].reshape(rend[-1][k].shape), rend[-1][k]), k
