@@ -183,8 +183,10 @@ int mnrf_gemm_wgrad(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16
  * `w` is K-major [256, ldw] bf16: the forward operand w_nk [out, in_pad] or the dgrad operand
  * w_kn [in_pad(first 256 rows used), out].
  *   FWD: out = relu(acc + bias) (bf16), maskbits written (1 bit per output, as mnrf_gemm);
- *        head_w/head_b/head_out (optional): head_out[m] = <bf16(out_last[m, :]), head_w> + head_b[0],
- *        the Dense(1) density head of models.py:460 computed in the last layer's epilogue.
+ *        head_w/head_b/head_out (optional): head_out[m, o] = <bf16(out_last[m, :]), head_w[o, :]> + head_b[o]
+ *        for o < head_n, computed in the last layer's epilogue: the Dense(1) density head of models.py:460
+ *        (head_n = 1), or that head stacked with the Dense(3) rgb head of a view-independent model
+ *        (use_viewdirs = False, models.py:584; head_n = 4, head_out [m, 4] = [raw_density | raw_rgb]).
  *   BWD: out = acc masked by maskbits (read; NULL = no mask); colsum[256] += column sums of out (the
  *        bias gradient of the layer whose activation the mask came from).
  * `out` may be NULL (FWD only: the activation is not needed later).  m is any row count; rows past m
@@ -214,9 +216,11 @@ typedef struct {
   int64_t m;                  /* sample rows */
   const mnrf_bf16* stream;    /* [m, ldstream] bf16 */
   int64_t ldstream;
-  const float* head_w;        /* [256] fp32 or NULL */
-  const float* head_b;        /* device scalar or NULL */
-  float* head_out;            /* [m] fp32 */
+  const float* head_w;        /* [head_n, 256] fp32 or NULL */
+  const float* head_b;        /* [head_n] fp32 or NULL */
+  float* head_out;            /* [m, head_n] fp32 */
+  int32_t head_n;             /* 1 or 4 (0 reads as 1) */
+  int32_t reserved;
   mnrf_chain_layer layer[MNRF_CHAIN_MAX_LAYERS];
 } mnrf_chain_desc;
 
@@ -229,12 +233,17 @@ int mnrf_mlp_chain_max_layers(void);
  * provided -- the trunk adds the density term through mnrf_gemm's rowv/colv),
  * dW[K, n_out] += (the fp32 master layout [in, out]), db[n_out] += (fp32 atomics);
  * dxsum[K] += column sums of dX (optional: bias gradient of the layer that produced X).
+ * 0 < dw_split < n_out splits dW between two master matrices: outputs [0, dw_split) go to
+ * dw [K, dw_split], outputs [dw_split, n_out) to dw2 [K, n_out - dw_split] (the density and rgb heads
+ * of a view-independent model run as one stacked head; their weights live apart).  dx_cols (0: K) limits dX and
+ * dxsum to the first dx_cols columns (a head reading [hidden | features] needs the gradient of the hidden part only).
  */
 int mnrf_head_fwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx,
                   const mnrf_bf16* w, const float* b, float* raw, mnrf_stream stream);
 int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx,
                   const mnrf_bf16* w, const float* draw, mnrf_bf16* dx, int64_t lddx,
-                  int32_t relu_mask, float* dw, float* db, float* dxsum, mnrf_stream stream);
+                  int32_t relu_mask, float* dw, float* dw2, int32_t dw_split, float* db, float* dxsum,
+                  int32_t dx_cols, mnrf_stream stream);
 
 /* Column sums of a bf16 matrix into fp32 (bias gradients): out[N] += sum_m x[m, :]. */
 int mnrf_colsum(int64_t m, int32_t n, const mnrf_bf16* x, int64_t ldx, float* out,
@@ -244,7 +253,9 @@ int mnrf_colsum(int64_t m, int32_t n, const mnrf_bf16* x, int64_t ldx, float* ou
  * Forward: density activation (models.py:506) + rgb activation/padding (models.py:584-602)
  * + render.compute_alpha_weights (render.py:130-151) + render.volumetric_rendering
  * (render.py:154-213).  One warp owns one ray.
- *   raw_density [B,S]; raw_rgb [B,S,3] or NULL (PropMLP: disable_rgb -> rgb = 0)
+ *   raw_density [B,S]; raw_rgb [B,S,3] or NULL (PropMLP: disable_rgb -> rgb = 0); ld_density / ld_rgb
+ *   are the floats between consecutive samples of raw_density / raw_rgb and of their gradients (0: 1 and 3),
+ *   so a stacked head's [B*S, 4] output is read and its gradient written in place (ld 4 for both)
  *   density_noise optional [B,S] N(0,1) draws (models.py:462-464)
  *   sdist [B,S+1]; directions [B,3]; near/far [B]; bg: scalar or NULL->bg_rgb [B,3]
  *   rgb_scale optional [B,3]: per-ray colour scale applied to the sample colours (RawNeRF
@@ -264,6 +275,7 @@ typedef struct {
   int32_t rgb_mode;         /* 0: colour = act(raw_rgb); 1: diffuse + specular (models.py:588-599):
                                clip(linear_to_srgb(tint * act(raw_rgb) + sigmoid(raw_diffuse - log 3)), 0, 1),
                                tint = sigmoid(raw_tint) or 0.5 when raw_tint is NULL */
+  int32_t ld_density, ld_rgb;
 } mnrf_composite_desc;
 
 int mnrf_composite_fwd(const mnrf_composite_desc* d, const float* raw_density,
@@ -389,16 +401,18 @@ int mnrf_refdir_bwd(const mnrf_refdir_desc* d, const float* ide_mat, const int32
  * multiplier is > 0 (stats[4], stats[5] as above).  head_grads (optional, bf16 [M, ld_head_grads]):
  * the backward writes [d_raw_density | d_grad_pred] to its columns 0..3 and leaves the others alone, so
  * a zero-filled [M, 64] buffer is the A operand of one dgrad GEMM into the trunk against the K-major
- * [w_density | W_grad_pred | 0]. */
+ * [w_density | W_grad_pred | 0].  d_raw_rgb (optional, with head_grads: the rgb head of a view-independent
+ * model on the same trunk) goes to columns 4..6, against [w_density | W_grad_pred | W_rgb | 0].  Sample m of
+ * d_raw_density / d_raw_rgb is at m * ld_raw (0 reads as 1). */
 int mnrf_normals_fwd(int64_t M, int32_t num_samples, const float* grad_pred, const float* raw_grad_density,
                      const float* viewdirs, float* normals_pred, float* normals, float orient_mult,
                      float prednorm_mult, int32_t orient_on_pred, float* extra_dw /* [M] or NULL */,
                      mnrf_stream stream);
 int mnrf_normals_bwd(int64_t M, int32_t num_samples, const float* grad_pred, const float* raw_grad_density,
                      const float* viewdirs, const float* weights, float orient_mult, float prednorm_mult,
-                     int32_t orient_on_pred, const float* d_raw_density, float* d_grad_pred,
-                     float* d_raw_grad_density, mnrf_bf16* head_grads, int64_t ld_head_grads, float* stats,
-                     mnrf_stream stream);
+                     int32_t orient_on_pred, const float* d_raw_density, const float* d_raw_rgb, int64_t ld_raw,
+                     float* d_grad_pred, float* d_raw_grad_density, mnrf_bf16* head_grads, int64_t ld_head_grads,
+                     float* stats, mnrf_stream stream);
 /* out[r, n] bf16 = maskbit(r mod mask_mod, n) ? rowv[r] * colv[n] : 0 -- the first dY of the
  * density-normal (tangent) backward chain. */
 int mnrf_outer_mask(int64_t rows, int32_t n, int64_t mask_mod, const float* rowv, const float* colv,

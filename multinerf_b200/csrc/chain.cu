@@ -62,9 +62,9 @@ struct ChainParams {
   int64_t m;
   int64_t num_units;
   ChainLayer layer[CH_MAX_LAYERS];
-  const float* head_w;      // FWD: Dense(1) on the last layer's output (density head), fp32 copy of the bf16 row
-  const float* head_b;
-  float* head_out;
+  const float* head_w;      // FWD: [NH][256] narrow head on the last layer's output, fp32 copy of the bf16 rows
+  const float* head_b;      //   (NH = 1: the density head; 4: density + rgb of a view-independent model)
+  float* head_out;          // [m][NH]
 };
 
 // two fp32 -> packed bf16x2 with ReLU in the conversion (one instruction for both lanes)
@@ -76,7 +76,8 @@ __device__ __forceinline__ uint32_t pack_bf16_relu(float lo, float hi) {
 
 // MODE 0: forward  -- epilogue = + bias, ReLU, 1-bit masks out, bf16 activation to smem (+ HBM), density head
 // MODE 1: backward -- epilogue = x ReLU mask (bits in), bias-gradient column sums, bf16 gradient to smem + HBM
-template <int MODE>
+// NH: outputs of the forward head (1 or 4)
+template <int MODE, int NH>
 __global__ void __launch_bounds__(CH_THREADS, 1)
 mlp_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainParams p) {
   extern __shared__ uint8_t smem_dyn[];
@@ -184,7 +185,9 @@ mlp_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainParams p) {
           row_ok[h] = rows[h] < p.m;
         }
         uint32_t bits[2] = {0u, 0u};
-        float hdot[2] = {0.f, 0.f};
+        float hdot[NH][2];
+#pragma unroll
+        for (int o = 0; o < NH; ++o) hdot[o][0] = hdot[o][1] = 0.f;
 #pragma unroll
         for (int i = 0; i < CH_W / 8; ++i) {
           const int col = 8 * i + cq;
@@ -204,10 +207,13 @@ mlp_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainParams p) {
               o[h] = pack_bf16_relu(v[h][0], v[h][1]);
             }
             if (do_head) {
-              // Dense(1) on the bf16-rounded activation, fp32 accumulate (what the head kernel computes)
-              const float2 hw = __ldg(reinterpret_cast<const float2*>(p.head_w + col));
+              // Dense(NH) on the bf16-rounded activation, fp32 accumulate (what the head kernel computes)
 #pragma unroll
-              for (int h = 0; h < 2; ++h) hdot[h] += bf16_lo(o[h]) * hw.x + bf16_hi(o[h]) * hw.y;
+              for (int oo = 0; oo < NH; ++oo) {
+                const float2 hw = __ldg(reinterpret_cast<const float2*>(p.head_w + oo * CH_W + col));
+#pragma unroll
+                for (int h = 0; h < 2; ++h) hdot[oo][h] += bf16_lo(o[h]) * hw.x + bf16_hi(o[h]) * hw.y;
+              }
             }
           } else {
 #pragma unroll
@@ -258,11 +264,14 @@ mlp_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainParams p) {
         }
         if (do_head) {
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            hdot[h] += __shfl_xor_sync(0xffffffffu, hdot[h], 1);
-            hdot[h] += __shfl_xor_sync(0xffffffffu, hdot[h], 2);
-            if ((lane & 3) == 0 && row_ok[h]) p.head_out[rows[h]] = hdot[h] + (p.head_b ? __ldg(p.head_b) : 0.f);
-          }
+          for (int oo = 0; oo < NH; ++oo)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              hdot[oo][h] += __shfl_xor_sync(0xffffffffu, hdot[oo][h], 1);
+              hdot[oo][h] += __shfl_xor_sync(0xffffffffu, hdot[oo][h], 2);
+              if ((lane & 3) == 0 && row_ok[h])
+                p.head_out[rows[h] * NH + oo] = hdot[oo][h] + (p.head_b ? __ldg(p.head_b + oo) : 0.f);
+            }
         }
       }
     }
@@ -335,8 +344,10 @@ extern "C" int mnrf_mlp_chain(const mnrf_chain_desc* d, mnrf_stream stream_) {
     if (make_tmap(&maps.stream, d->stream, d->m, d->stream_cols, d->ldstream, 64, CH_ROWS)) return 1;
   }
   p.head_w = d->head_w; p.head_b = d->head_b; p.head_out = d->head_out;
+  const int head_n = d->head_n ? d->head_n : 1;
   if (d->head_w) MNRF_CHECK(d->mode == MNRF_CHAIN_FWD && d->head_out && ((uintptr_t)d->head_w % 16) == 0,
                             "mnrf_mlp_chain: the head is a forward output (16-byte aligned weights)");
+  MNRF_CHECK(head_n == 1 || (head_n == 4 && d->head_w), "mnrf_mlp_chain: head_n must be 1 or 4, got %d", head_n);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)std::min<int64_t>(p.num_units, sms)); cfg.blockDim = dim3(CH_THREADS);
   cfg.dynamicSmemBytes = CH_SMEM; cfg.stream = stream;
@@ -344,14 +355,19 @@ extern "C" int mnrf_mlp_chain(const mnrf_chain_desc* d, mnrf_stream stream_) {
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  if (d->mode == MNRF_CHAIN_FWD) {
+  if (d->mode == MNRF_CHAIN_FWD && head_n == 4) {
+    static bool set4 = false;
+    auto kern = mlp_chain_kernel<0, 4>;
+    if (!set4) { MNRF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, CH_SMEM)); set4 = true; }
+    MNRF_CUDA(cudaLaunchKernelEx(&cfg, kern, maps, p));
+  } else if (d->mode == MNRF_CHAIN_FWD) {
     static bool set0 = false;
-    auto kern = mlp_chain_kernel<0>;
+    auto kern = mlp_chain_kernel<0, 1>;
     if (!set0) { MNRF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, CH_SMEM)); set0 = true; }
     MNRF_CUDA(cudaLaunchKernelEx(&cfg, kern, maps, p));
   } else {
     static bool set1 = false;
-    auto kern = mlp_chain_kernel<1>;
+    auto kern = mlp_chain_kernel<1, 1>;
     if (!set1) { MNRF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, CH_SMEM)); set1 = true; }
     MNRF_CUDA(cudaLaunchKernelEx(&cfg, kern, maps, p));
   }

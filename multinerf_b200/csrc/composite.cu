@@ -60,6 +60,10 @@ __device__ __forceinline__ float rgb_act_grad(int kind, float z) {
   return s * (1.f - s);
 }
 
+// floats between consecutive samples of raw_density / raw_rgb and of their gradients (mnrf.h)
+__device__ __forceinline__ size_t ld_density(const mnrf_composite_desc& d) { return d.ld_density ? d.ld_density : 1; }
+__device__ __forceinline__ size_t ld_rgb(const mnrf_composite_desc& d) { return d.ld_rgb ? d.ld_rgb : 3; }
+
 template <int CH>
 __device__ __forceinline__ void ray_forward(const mnrf_composite_desc& d, int ray, int lane,
                                             const float* __restrict__ raw_density,
@@ -77,7 +81,7 @@ __device__ __forceinline__ void ray_forward(const mnrf_composite_desc& d, int ra
   for (int j = 0; j < CH; ++j) {
     int s = lane * CH + j;
     bool ok = s < S;
-    float raw = ok ? raw_density[(size_t)ray * S + s] : 0.f;
+    float raw = ok ? raw_density[((size_t)ray * S + s) * ld_density(d)] : 0.f;
     if (density_noise && ok) raw += d.density_noise * density_noise[(size_t)ray * S + s];
     float din = raw + d.density_bias;
     st.dens_in[j] = din;
@@ -93,7 +97,7 @@ __device__ __forceinline__ void ray_forward(const mnrf_composite_desc& d, int ra
       float z = 0.f, c = 0.f, zd = 0.f, zt = 0.f;
       if (raw_rgb && ok) {
         const size_t ci = ((size_t)ray * S + s) * 3 + ch;
-        z = d.rgb_premult * raw_rgb[ci] + d.rgb_bias;
+        z = d.rgb_premult * raw_rgb[((size_t)ray * S + s) * ld_rgb(d) + ch] + d.rgb_bias;
         if (d.rgb_mode == 1) {
           zd = raw_diffuse[ci];
           if (raw_tint) zt = raw_tint[ci];
@@ -427,11 +431,12 @@ composite_bwd_kernel(mnrf_loss_desc L, const float* __restrict__ raw_density,
         if (isinf(st.a[j])) da = 0.f;
         else da = g[j] * expf(-st.a[j]) * st.T[j] - after;
         float dd = da * st.delta[j] * sigmoid_f(st.dens_in[j]);
-        d_raw_density[(size_t)ray * S + s] = dd;
+        d_raw_density[((size_t)ray * S + s) * ld_density(d)] = dd;
         if (d_raw_rgb) {
 #pragma unroll
           for (int ch = 0; ch < 3; ++ch) {
             const size_t ci = ((size_t)ray * S + s) * 3 + ch;
+            const size_t ri = ((size_t)ray * S + s) * ld_rgb(d) + ch;
             // dL/d(colour before padding and scale)
             const float gc = dpx[ch] * st.w[j] * st.sc[ch] * (1.f + 2.f * d.rgb_padding);
             const float da = rgb_act_grad(d.rgb_act, st.z[j][ch]) * d.rgb_premult;
@@ -442,11 +447,11 @@ composite_bwd_kernel(mnrf_loss_desc L, const float* __restrict__ raw_density,
               const float lin = t * a + dl;
               const float sr = lin2srgb(lin);
               const float glin = (sr > 0.f && sr < 1.f) ? gc * lin2srgb_grad(lin) : 0.f;
-              d_raw_rgb[ci] = glin * t * da;
+              d_raw_rgb[ri] = glin * t * da;
               d_raw_diffuse[ci] = glin * dl * (1.f - dl);
               if (d_raw_tint) d_raw_tint[ci] = raw_tint ? glin * a * t * (1.f - t) : 0.f;
             } else {
-              d_raw_rgb[ci] = gc * da;
+              d_raw_rgb[ri] = gc * da;
             }
           }
         }

@@ -50,14 +50,19 @@ head_fwd_kernel(int64_t M, int K, int n_out, const __nv_bfloat16* __restrict__ x
   }
 }
 
+// element (k, o) of dW in the fp32 master layout: outputs [0, split) in dw [K, split], the rest in dw2 (mnrf.h)
+__device__ __forceinline__ float* dw_at(float* dw, float* dw2, int split, int n_out, int k, int o) {
+  return o < split ? dw + (size_t)k * split + o : dw2 + (size_t)k * (n_out - split) + (o - split);
+}
+
 // dx[m,k] = relu'(x[m,k]) * sum_o draw[m,o] w[o,k];  dw[k,o] += sum_m draw[m,o] x[m,k];  db[o] += sum_m draw[m,o]
 template <int N_OUT, int kMaxChunks>
 __global__ void __launch_bounds__(256)
 head_bwd_kernel(int64_t M, int K, const __nv_bfloat16* __restrict__ x, int64_t ldx,
                 const __nv_bfloat16* __restrict__ w, const float* __restrict__ draw,
                 __nv_bfloat16* __restrict__ dx, int64_t lddx, int relu_mask,
-                float* __restrict__ dw, float* __restrict__ db, float* __restrict__ dxsum,
-                int64_t rows_per_block) {
+                float* __restrict__ dw, float* __restrict__ dw2, int dw_split, float* __restrict__ db,
+                float* __restrict__ dxsum, int dx_cols, int64_t rows_per_block) {
   extern __shared__ __align__(16) unsigned char smraw[];
   constexpr int n_out = N_OUT;
   float* sdw = reinterpret_cast<float*>(smraw);                                   // [n_out][K] fp32
@@ -113,7 +118,7 @@ head_bwd_kernel(int64_t M, int K, const __nv_bfloat16* __restrict__ x, int64_t l
 #pragma unroll
           for (int e = 0; e < 8; ++e) racc[o][q][e] += g[o] * xe[e];
         }
-        if (dxr) {
+        if (dxr && c * 8 < dx_cols) {
           if (relu_mask) {
 #pragma unroll
             for (int e = 0; e < 8; ++e) de[e] = xe[e] > 0.f ? de[e] : 0.f;
@@ -149,7 +154,7 @@ head_bwd_kernel(int64_t M, int K, const __nv_bfloat16* __restrict__ x, int64_t l
     __syncthreads();
     if (dw) for (int i = threadIdx.x; i < n_out * K; i += blockDim.x) {
       int o = i / K, k = i - o * K;
-      atomicAdd(&dw[(size_t)k * n_out + o], sdw[i]);
+      atomicAdd(dw_at(dw, dw2, dw_split, n_out, k, o), sdw[i]);
     }
     __syncthreads();
     for (int i = threadIdx.x; i < K; i += blockDim.x) sdw[i] = 0.f;
@@ -163,14 +168,14 @@ head_bwd_kernel(int64_t M, int K, const __nv_bfloat16* __restrict__ x, int64_t l
       }
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < K; i += blockDim.x) atomicAdd(&dxsum[i], sdw[i]);
+    for (int i = threadIdx.x; i < dx_cols; i += blockDim.x) atomicAdd(&dxsum[i], sdw[i]);
     return;
   }
   __syncthreads();
   // dw is in the master layout [K, n_out] (row-major), the staging buffer is [n_out][K]
   if (dw) for (int i = threadIdx.x; i < n_out * K; i += blockDim.x) {
     int o = i / K, k = i - o * K;
-    atomicAdd(&dw[(size_t)k * n_out + o], sdw[i]);
+    atomicAdd(dw_at(dw, dw2, dw_split, n_out, k, o), sdw[i]);
   }
 }
 
@@ -230,8 +235,8 @@ __global__ void __launch_bounds__(256)
 head_bwd_sub_kernel(int64_t M, const __nv_bfloat16* __restrict__ x, int64_t ldx,
                     const __nv_bfloat16* __restrict__ w, const float* __restrict__ draw,
                     __nv_bfloat16* __restrict__ dx, int64_t lddx, int relu_mask,
-                    float* __restrict__ dw, float* __restrict__ db, float* __restrict__ dxsum,
-                    int64_t rows_per_block) {
+                    float* __restrict__ dw, float* __restrict__ dw2, int dw_split, float* __restrict__ db,
+                    float* __restrict__ dxsum, int dx_cols, int64_t rows_per_block) {
   constexpr int K = LPR * 8, RW = 32 / LPR;
   __shared__ float sdw[N_OUT * K];
   __shared__ float sxs[K];
@@ -288,7 +293,7 @@ head_bwd_sub_kernel(int64_t M, const __nv_bfloat16* __restrict__ x, int64_t ldx,
         }
         if (c == 0) dbacc[o] += g[u][o];
       }
-      if (dx && row < m_end) {
+      if (dx && row < m_end && c * 8 < dx_cols) {
         if (relu_mask) {
 #pragma unroll
           for (int e = 0; e < 8; ++e) de[e] = xe[e] > 0.f ? de[e] : 0.f;
@@ -316,9 +321,9 @@ head_bwd_sub_kernel(int64_t M, const __nv_bfloat16* __restrict__ x, int64_t ldx,
   // dw is in the master layout [K, n_out] (row-major), the staging buffer is [n_out][K]
   if (dw) for (int i = threadIdx.x; i < N_OUT * K; i += blockDim.x) {
     const int o = i / K, k = i - o * K;
-    atomicAdd(&dw[(size_t)k * N_OUT + o], sdw[i]);
+    atomicAdd(dw_at(dw, dw2, dw_split, N_OUT, k, o), sdw[i]);
   }
-  if (dxsum) for (int i = threadIdx.x; i < K; i += blockDim.x) atomicAdd(&dxsum[i], sxs[i]);
+  if (dxsum) for (int i = threadIdx.x; i < dx_cols; i += blockDim.x) atomicAdd(&dxsum[i], sxs[i]);
 }
 
 // out[n] += sum_m x[m, n]
@@ -486,7 +491,8 @@ extern "C" int mnrf_head_fwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf1
 
 extern "C" int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx,
                              const mnrf_bf16* w, const float* draw, mnrf_bf16* dx, int64_t lddx,
-                             int32_t relu_mask, float* dw, float* db, float* dxsum, mnrf_stream stream) {
+                             int32_t relu_mask, float* dw, float* dw2, int32_t dw_split, float* db, float* dxsum,
+                             int32_t dx_cols, mnrf_stream stream) {
   using namespace mnrf;
   if (m == 0) return 0;
   MNRF_CHECK(x && w && draw, "mnrf_head_bwd: null pointer");
@@ -494,6 +500,10 @@ extern "C" int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf1
   MNRF_CHECK(n_out >= 1 && n_out <= kMaxHead, "mnrf_head_bwd: n_out %d not in [1,4]", n_out);
   MNRF_CHECK(k % 8 == 0 && k <= 1536 && ldx % 8 == 0 && (!dx || lddx % 8 == 0),
              "mnrf_head_bwd: K must be a multiple of 8 and <= 1536");
+  if (dw_split <= 0 || dw_split >= n_out) dw_split = n_out;
+  if (dx_cols <= 0) dx_cols = k;
+  MNRF_CHECK(dx_cols <= k && dx_cols % 8 == 0, "mnrf_head_bwd: dx_cols must be a multiple of 8 and <= K");
+  MNRF_CHECK(dw_split == n_out || (dw && dw2), "mnrf_head_bwd: a split weight gradient needs dw and dw2");
   if (m == 0) return 0;
   if ((k == 256 || k == 128 || k == 64) && ((uintptr_t)w % 16) == 0) {
     // rows of one / half / a quarter of a warp's 16-byte chunks (see head_bwd_sub_kernel)
@@ -504,7 +514,7 @@ extern "C" int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf1
 #define MNRF_HBS(NO, LPR_)                                                                              \
   head_bwd_sub_kernel<NO, LPR_, 4><<<blocks_s, 256, 0, (cudaStream_t)stream>>>(                         \
       m, reinterpret_cast<const __nv_bfloat16*>(x), ldx, reinterpret_cast<const __nv_bfloat16*>(w), draw, \
-      reinterpret_cast<__nv_bfloat16*>(dx), lddx, relu_mask, dw, db, dxsum, rpb_s)
+      reinterpret_cast<__nv_bfloat16*>(dx), lddx, relu_mask, dw, dw2, dw_split, db, dxsum, dx_cols, rpb_s)
 #define MNRF_HBS_N(NO) do { if (k == 256) MNRF_HBS(NO, 32); else if (k == 128) MNRF_HBS(NO, 16); else MNRF_HBS(NO, 8); } while (0)
     switch (n_out) {
       case 1: MNRF_HBS_N(1); break;
@@ -523,7 +533,7 @@ extern "C" int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf1
 #define MNRF_HB(NO, CK)                                                                         \
   head_bwd_kernel<NO, CK><<<blocks, 256, smem, (cudaStream_t)stream>>>(                         \
       m, k, reinterpret_cast<const __nv_bfloat16*>(x), ldx, reinterpret_cast<const __nv_bfloat16*>(w), \
-      draw, reinterpret_cast<__nv_bfloat16*>(dx), lddx, relu_mask, dw, db, dxsum, rpb)
+      draw, reinterpret_cast<__nv_bfloat16*>(dx), lddx, relu_mask, dw, dw2, dw_split, db, dxsum, dx_cols, rpb)
 #define MNRF_HB_N(NO)                                      \
   do {                                                     \
     if (chunks <= 1) MNRF_HB(NO, 1);                       \

@@ -366,7 +366,7 @@ __global__ void __launch_bounds__(128)
 normals_bwd_kernel(int64_t M, int S, RefLoss L, const float* __restrict__ grad_pred,
                    const float* __restrict__ raw_grad_density, const float* __restrict__ viewdirs,
                    const float* __restrict__ weights, const float* __restrict__ d_raw_density,
-                   float* __restrict__ d_grad_pred, float* __restrict__ d_raw_grad_density /* [3, M] */,
+                   const float* __restrict__ d_raw_rgb, int64_t ld_raw, float* __restrict__ d_grad_pred, float* __restrict__ d_raw_grad_density /* [3, M] */,
                    __nv_bfloat16* __restrict__ head_grads, int64_t ld_head_grads,
                    float* __restrict__ stats /* [4]=orientation, [5]=pred normals */) {
   float st_or = 0.f, st_pn = 0.f;
@@ -385,8 +385,14 @@ normals_bwd_kernel(int64_t M, int S, RefLoss L, const float* __restrict__ grad_p
     if (head_grads) {
       // [d raw_density | d grad_pred]: the A operand of the dgrad GEMM into the trunk against [w_density | W_grad_pred]
       __nv_bfloat16* hs = head_grads + m * ld_head_grads;
-      *reinterpret_cast<uint32_t*>(hs) = pack_bf16(d_raw_density[m], dgp[0]);
+      *reinterpret_cast<uint32_t*>(hs) = pack_bf16(d_raw_density[m * ld_raw], dgp[0]);
       *reinterpret_cast<uint32_t*>(hs + 2) = pack_bf16(dgp[1], dgp[2]);
+      if (d_raw_rgb) {
+        // [.. | d raw_rgb]: the rgb head of a view-independent model reads the same trunk output
+        const float* g = d_raw_rgb + m * ld_raw;
+        *reinterpret_cast<uint32_t*>(hs + 4) = pack_bf16(g[0], g[1]);
+        *reinterpret_cast<uint32_t*>(hs + 6) = pack_bf16(g[2], 0.f);
+      }
     }
   }
   if (stats) add_loss_stats(st_or, st_pn, stats);
@@ -501,9 +507,9 @@ extern "C" int mnrf_normals_fwd(int64_t M, int32_t num_samples, const float* gra
 
 extern "C" int mnrf_normals_bwd(int64_t M, int32_t num_samples, const float* grad_pred, const float* raw_grad_density,
                                 const float* viewdirs, const float* weights, float orient_mult, float prednorm_mult,
-                                int32_t orient_on_pred, const float* d_raw_density, float* d_grad_pred,
-                                float* d_raw_grad_density, mnrf_bf16* head_grads, int64_t ld_head_grads,
-                                float* stats, mnrf_stream stream) {
+                                int32_t orient_on_pred, const float* d_raw_density, const float* d_raw_rgb,
+                                int64_t ld_raw, float* d_grad_pred, float* d_raw_grad_density, mnrf_bf16* head_grads,
+                                int64_t ld_head_grads, float* stats, mnrf_stream stream) {
   using namespace mnrf;
   if (M == 0) return 0;
   MNRF_CHECK(grad_pred || raw_grad_density, "mnrf_normals_bwd: no normals to differentiate");
@@ -517,11 +523,14 @@ extern "C" int mnrf_normals_bwd(int64_t M, int32_t num_samples, const float* gra
   MNRF_CHECK(!head_grads || (grad_pred && d_raw_density && ld_head_grads >= 4 && ld_head_grads % 2 == 0 &&
                              (reinterpret_cast<uintptr_t>(head_grads) & 3) == 0),
              "mnrf_normals_bwd: head_grads needs grad_pred, d_raw_density and 4 aligned columns");
+  MNRF_CHECK(!d_raw_rgb || (head_grads && ld_head_grads >= 8), "mnrf_normals_bwd: d_raw_rgb needs 8 head_grads columns");
+  if (ld_raw <= 0) ld_raw = 1;
   MNRF_CHECK(num_samples > 0, "mnrf_normals_bwd: num_samples must be positive");
   int blocks = (int)std::min<int64_t>((M + 127) / 128, (int64_t)mnrf_num_sms() * 16);
   normals_bwd_kernel<<<blocks, 128, 0, (cudaStream_t)stream>>>(
       M, num_samples, RefLoss{orient_mult, prednorm_mult, orient_on_pred}, grad_pred, raw_grad_density, viewdirs,
-      weights, d_raw_density, d_grad_pred, d_raw_grad_density, reinterpret_cast<__nv_bfloat16*>(head_grads),
+      weights, d_raw_density, d_raw_rgb, ld_raw, d_grad_pred, d_raw_grad_density,
+      reinterpret_cast<__nv_bfloat16*>(head_grads),
       ld_head_grads, losses ? stats : nullptr);
   MNRF_LAUNCH_CHECK();
   return 0;

@@ -45,7 +45,7 @@ class CompositeDesc(C.Structure):
               ('opaque_background', C.c_int32), ('density_bias', C.c_float),
               ('density_noise', C.c_float), ('rgb_act', C.c_int32), ('rgb_premult', C.c_float),
               ('rgb_bias', C.c_float), ('rgb_padding', C.c_float), ('bg_const', C.c_float),
-              ('rgb_mode', C.c_int32)]
+              ('rgb_mode', C.c_int32), ('ld_density', C.c_int32), ('ld_rgb', C.c_int32)]
 
 
 class LossDesc(C.Structure):
@@ -100,7 +100,8 @@ class ChainLayer(C.Structure):
 class ChainDesc(C.Structure):
   _fields_ = [('mode', C.c_int32), ('num_layers', C.c_int32), ('width', C.c_int32), ('stream_cols', C.c_int32),
               ('m', C.c_int64), ('stream', C.c_void_p), ('ldstream', C.c_int64), ('head_w', C.c_void_p),
-              ('head_b', C.c_void_p), ('head_out', C.c_void_p), ('layer', ChainLayer * CHAIN_MAX_LAYERS)]
+              ('head_b', C.c_void_p), ('head_out', C.c_void_p), ('head_n', C.c_int32), ('reserved', C.c_int32),
+              ('layer', ChainLayer * CHAIN_MAX_LAYERS)]
 
 
 class AdamDesc(C.Structure):
@@ -134,7 +135,7 @@ _SIGNATURES = {
     'mnrf_mlp_chain_max_layers': (C.c_int, []),
     'mnrf_head_fwd': (C.c_int, [C.c_int64, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P, _P, _P]),
     'mnrf_head_bwd': (C.c_int, [C.c_int64, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P, _P,
-                                C.c_int64, C.c_int32, _P, _P, _P, _P]),
+                                C.c_int64, C.c_int32, _P, _P, C.c_int32, _P, _P, C.c_int32, _P]),
     'mnrf_colsum': (C.c_int, [C.c_int64, C.c_int32, _P, C.c_int64, _P, _P]),
     'mnrf_composite_fwd': (C.c_int, [C.POINTER(CompositeDesc)] + [_P] * 18),
     'mnrf_composite_bwd': (C.c_int, [C.POINTER(LossDesc)] + [_P] * 24),
@@ -146,7 +147,8 @@ _SIGNATURES = {
     'mnrf_refdir_bwd': (C.c_int, [C.POINTER(RefdirDesc)] + [_P] * 8 + [C.c_int32, C.c_float, C.c_float, C.c_int32] +
                         [_P] * 8),
     'mnrf_normals_fwd': (C.c_int, [C.c_int64, C.c_int32] + [_P] * 5 + [C.c_float, C.c_float, C.c_int32, _P, _P]),
-    'mnrf_normals_bwd': (C.c_int, [C.c_int64, C.c_int32] + [_P] * 4 + [C.c_float, C.c_float, C.c_int32] + [_P] * 4 +
+    'mnrf_normals_bwd': (C.c_int, [C.c_int64, C.c_int32] + [_P] * 4 + [C.c_float, C.c_float, C.c_int32] + [_P] * 2 +
+                         [C.c_int64] + [_P] * 3 +
                          [C.c_int64, _P, _P]),
     'mnrf_outer_mask': (C.c_int,[C.c_int64, C.c_int32, C.c_int64, _P, _P, _P, C.c_int64, _P, C.c_int64, _P]),
     'mnrf_pixels_to_rays': (C.c_int, [C.POINTER(CameraDesc)] + [_P] * 11),

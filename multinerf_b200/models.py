@@ -95,16 +95,30 @@ class MLPPlan:
       add('grad_pred', x_dim, x_pad, 3, True, rm=rmx)
     self.has_rgb = not cfg.disable_rgb
     self.use_viewdirs = use_viewdirs
+    # view-independent colour (models.py:512,584): rgb = act(Dense(3)(x)) on the trunk output, no view branch.  The
+    # rgb head runs stacked with the density head as one 4-output head: raw [M, 4] = [raw_density | raw_rgb]
+    self.rgb_on_trunk = self.has_rgb and not use_viewdirs
     self.ref_stage = False
-    # normals of a colourless MLP feed only the orientation / predicted-normal losses and the renderings
-    # (csrc/refnerf.cu normals_fwd/bwd)
-    self.normals_stage = (self.pred_normals or self.density_normals) and not self.has_rgb
-    # K of the trunk-top dgrad GEMM of such an MLP with predicted normals: [d raw_density | d grad_pred | 0]
+    # normals of an MLP without a view branch feed only the orientation / predicted-normal losses and the
+    # renderings (csrc/refnerf.cu normals_fwd/bwd)
+    self.normals_stage = (self.pred_normals or self.density_normals) and (not self.has_rgb or self.rgb_on_trunk)
+    # K of the trunk-top dgrad GEMM of such an MLP with predicted normals: [d raw_density | d grad_pred (| d raw_rgb)
+    # | 0]
     self.normals_head_cols = 64 if (self.normals_stage and self.pred_normals) else 0
-    if self.has_rgb:
-      if not use_viewdirs:
-        raise NotImplementedError('use_viewdirs=False with rgb is not wired into the CUDA path')
+    if self.rgb_on_trunk:
+      if cfg.use_diffuse_color:
+        raise ValueError('use_viewdirs=False with use_diffuse_color: the reference reads raw_rgb_diffuse, which it '
+                         'creates only with view directions (internal/models.py:591)')
+      # Ref-NeRF heads and encodings are not created without view directions (models.py:512); normals still run
+      add('rgb', x_dim, x_pad, cfg.num_rgb_channels, True, rm=rmx)
+    elif self.has_rgb:
       if cfg.bottleneck_width <= 0:
+        if not cfg.use_reflections:
+          raise ValueError('bottleneck_width = 0 needs use_reflections: the reference reads bottleneck.shape to '
+                           'broadcast the view encoding (internal/models.py:552-554)')
+        if glo_features > 0:
+          raise ValueError('bottleneck_width = 0 with num_glo_features > 0: the reference reads bottleneck.shape to '
+                           'broadcast the GLO vector (internal/models.py:567-568)')
         raise NotImplementedError('bottleneck_width == 0 is not supported (models.py:536-554)')
       if cfg.use_diffuse_color:
         add('diffuse', x_dim, x_pad, 3, True, rm=rmx)
@@ -158,8 +172,12 @@ class MLPPlan:
       sp.w_off = off
       off += sp.in_pad * sp.out_dim
       off = (off + 3) // 4 * 4
+      if self.rgb_on_trunk and sp.role == 'rgb':
+        # the density head's bias block holds [b_density | b_rgb]: the stacked head's bias and bias gradient
+        sp.b_off = self.one('density', specs).b_off + 1
+        continue
       sp.b_off = off
-      off += sp.out_dim
+      off += 4 if (self.rgb_on_trunk and sp.role == 'density') else sp.out_dim
       off = (off + 3) // 4 * 4
     self.specs = specs
     self.flat_size = off
@@ -168,8 +186,8 @@ class MLPPlan:
   def by_role(self, role):
     return [sp for sp in self.specs if sp.role == role]
 
-  def one(self, role):
-    r = self.by_role(role)
+  def one(self, role, specs=None):
+    r = [sp for sp in (self.specs if specs is None else specs) if sp.role == role]
     return r[0] if r else None
 
 
@@ -182,7 +200,14 @@ class MLPDevice:
     self.device = device
     self.basis = torch.tensor(plan.basis, device=device)
     self.w_nk, self.w_kn, self.colv = {}, {}, {}
+    if plan.rgb_on_trunk:
+      # [w_density; W_rgb]: the density and rgb heads of a view-independent model as one 4-output head
+      d, r = plan.one('density'), plan.one('rgb')
+      self.w_head = torch.zeros(4, d.in_pad, device=device, dtype=torch.bfloat16)
+      self.w_nk[d.name], self.w_nk[r.name] = self.w_head[:1], self.w_head[1:]
     for sp in plan.specs:
+      if sp.name in self.w_nk:
+        continue
       self.w_nk[sp.name] = torch.zeros(sp.out_dim, sp.in_pad, device=device, dtype=torch.bfloat16)
       if not sp.head:
         self.w_kn[sp.name] = torch.zeros(sp.in_pad, sp.out_dim, device=device, dtype=torch.bfloat16)
@@ -206,9 +231,16 @@ class MLPDevice:
     d = plan.one('density')
     # bf16-rounded, as the fwd used.  Updated IN PLACE: captured CUDA graphs hold this pointer
     # (DGRAD colv / outer_mask), so the tensor must never be re-allocated.
-    if getattr(self, 'colv_density', None) is None:
-      self.colv_density = torch.zeros(d.in_pad, device=self.device)
-    self.colv_density.copy_(self.w_nk[d.name][0])
+    if plan.rgb_on_trunk:
+      # fp32 rows of the stacked head (the chained trunk's epilogue head); row 0 is colv_density
+      if getattr(self, 'colv_head', None) is None:
+        self.colv_head = torch.zeros(4, d.in_pad, device=self.device)
+        self.colv_density = self.colv_head[0]
+      self.colv_head.copy_(self.w_head)
+    else:
+      if getattr(self, 'colv_density', None) is None:
+        self.colv_density = torch.zeros(d.in_pad, device=self.device)
+      self.colv_density.copy_(self.w_nk[d.name][0])
     if plan.ref_stage or plan.normals_head_cols:
       # [x_pad, vin_pad] K-major B operand of the trunk-entry dgrad:  [ W_bottleneck | head weights ]
       # (colourless MLP with predicted normals: [x_pad, 64] = [ w_density | W_grad_pred | 0 ])
@@ -219,7 +251,9 @@ class MLPDevice:
         self.wcat_kn = torch.zeros(plan.x_pad, cols, device=self.device, dtype=torch.bfloat16)
       if plan.ref_stage:
         self.wcat_kn[:, :bw] = self.w_kn[bt.name]
-      for role, (c0, n) in plan.HEAD_SLOTS.items():
+      # a view-independent model's rgb head takes the diffuse slot (it has no diffuse head, MLPPlan)
+      slots = dict(plan.HEAD_SLOTS, rgb=plan.HEAD_SLOTS['diffuse']) if plan.rgb_on_trunk else plan.HEAD_SLOTS
+      for role, (c0, n) in slots.items():
         sp = plan.one(role)
         if sp is not None:
           self.wcat_kn[:, bw + c0:bw + c0 + n] = self.w_nk[sp.name].t()
@@ -490,7 +524,13 @@ class Model:
       st.rgd = torch.empty(3, M, device=dev)
       st.d_rgd = torch.empty(3, M, device=dev)
       st.normals = torch.empty(M, 3, device=dev)
-    if plan.has_rgb:
+    if plan.rgb_on_trunk:
+      # the stacked head's output and its gradient, [M, 4] = [density | rgb]: compositing reads and writes them in
+      # place through sample strides
+      st.raw4, st.d_raw4 = torch.empty(M, 4, device=dev), torch.empty(M, 4, device=dev)
+      st.raw_density, st.raw_rgb = st.raw4.view(B, S, 4)[..., 0], st.raw4.view(B, S, 4)[..., 1:]
+      st.d_raw_density, st.d_raw_rgb = st.d_raw4.view(B, S, 4)[..., 0], st.d_raw4.view(B, S, 4)[..., 1:]
+    elif plan.has_rgb:
       Wv = cfg.net_width_viewdirs
       nv = cfg.net_depth_viewdirs
       st.vacts = [torch.empty(M, Wv + plan.vin_pad if i in plan.view_concat_after else Wv, device=dev, dtype=bf)
@@ -556,14 +596,16 @@ class Model:
       # the whole trunk (+ the Dense(1) density head when it reads the plain 256-wide output) in ONE launch
       ops.mlp_chain(self._chain_fwd_desc(st, mlp))
       x = st.acts[-1]
-      if plan.last_has_feat:
-        ops.head_fwd(x, mlp.w_nk[d.name], mlp.b(d), 1, d.in_pad, raw=st.raw_density.view(M, 1))
     else:
       for i, sp in enumerate(trunk):
         ops.gemm(L.GEMM_FWD, x, mlp.w_nk[sp.name], st.acts[i][:, :W], m=M, n=W, k=sp.in_pad, act=L.ACT_RELU,
                  bias=mlp.b(sp), maskbits=st.bits[i], impl=impl)
         x = st.acts[i]          # full width (incl. concatenated features) feeds the next layer
-      ops.head_fwd(x, mlp.w_nk[d.name], mlp.b(d), 1, d.in_pad, raw=st.raw_density.view(M, 1))
+    if not chained or plan.last_has_feat:
+      if plan.rgb_on_trunk:     # density + rgb in one pass over the trunk output (bias block [b_density | b_rgb])
+        ops.head_fwd(x, mlp.w_head, mlp.b(d), 4, d.in_pad, raw=st.raw4)
+      else:
+        ops.head_fwd(x, mlp.w_nk[d.name], mlp.b(d), 1, d.in_pad, raw=st.raw_density.view(M, 1))
     st.x_last = x
     if plan.density_normals:
       # raw_grad_density = d raw_density / d mean by forward mode (replaces vmap(value_and_grad),
@@ -586,7 +628,7 @@ class Model:
     if plan.normals_stage:
       ops.normals_fwd(M, S, st.heads.get('grad_pred'), st.rgd if plan.density_normals else None, rays.viewdirs,
                       st.normals_pred, st.normals, om, pm, on_pred, extra_dw)
-    if not plan.has_rgb:
+    if not plan.has_rgb or plan.rgb_on_trunk:
       return
     bt = plan.one('bottleneck')
     ops.gemm(L.GEMM_FWD, x, mlp.w_nk[bt.name], st.vin[:, :bt.out_dim], m=M, n=bt.out_dim,
@@ -649,7 +691,8 @@ class Model:
         if sp.in_pad == W + plan.Fpad:          # skip layer: [hidden | features] against [W | Fpad] weight columns
           ly.update(n_stream=nf, stream_col0=0, stream_kb0=W // 64)
       last = i == len(trunk) - 1
-      if st.keep_acts or (last and (plan.has_rgb or plan.last_has_feat or plan.pred_normals)):
+      if st.keep_acts or (last and ((plan.has_rgb and not plan.rgb_on_trunk) or plan.last_has_feat or
+                                    plan.pred_normals)):
         ly['out'] = st.acts[i][:, :W]
       if st.keep_acts:
         ly['maskbits'] = st.bits[i]
@@ -657,7 +700,10 @@ class Model:
     head = {}
     if not plan.last_has_feat:
       dsp = plan.one('density')
-      head = dict(head_w=mlp.colv_density, head_b=mlp.b(dsp), head_out=st.raw_density.view(M))
+      if plan.rgb_on_trunk:
+        head = dict(head_w=mlp.colv_head, head_b=mlp.b(dsp), head_out=st.raw4, head_n=4)
+      else:
+        head = dict(head_w=mlp.colv_density, head_b=mlp.b(dsp), head_out=st.raw_density.view(M))
     cache[key] = ops.chain_desc(L.CHAIN_FWD, M, layers, stream=st.feat, stream_cols=plan.Fpad, **head)
     return cache[key]
 
@@ -759,7 +805,7 @@ class Model:
       if m.num_glo_features > 0 and not lv['is_prop'] and not zero_glo:
         st.glo_vec = self.params.seg('Embed_0').view(m.num_glo_embeddings, -1)[rays.cam_idx[:, 0].long()]
       st.bneck_noise = None
-      if mlp.plan.cfg.bottleneck_noise > 0 and rng is not None and mlp.plan.has_rgb:
+      if mlp.plan.cfg.bottleneck_noise > 0 and rng is not None and mlp.plan.one('bottleneck') is not None:
         bwid = mlp.plan.cfg.bottleneck_width
         if isinstance(rng, dict):
           st.bneck_noise = rng['bottleneck_noise'][i].to(dev).reshape(B * lv['S'], bwid)
@@ -887,7 +933,7 @@ class Model:
       # per-layer gradient buffers when the dgrad chain runs as one launch (its wgrads come after)
       n_dy = cfg.net_depth if self._use_chain(plan, M, impl) else 2
       bw_.dy = [torch.empty(M, W, device=dev, dtype=bf) for _ in range(n_dy)]
-      if plan.has_rgb:
+      if plan.has_rgb and not plan.rgb_on_trunk:
         Wv = cfg.net_width_viewdirs
         bw_.dv = [torch.empty(M, Wv, device=dev, dtype=bf) for _ in range(2)]
         bw_.d_vin = torch.empty(M, plan.vin_pad, device=dev, dtype=bf)
@@ -907,8 +953,8 @@ class Model:
     dy = sc.dy[0]
     d_raw_density = st.d_raw_density.view(M, 1)
     om, pm, on_pred = _loss_args(loss_mults)
-    if plan.has_rgb:
-      r = plan.one('rgb')
+    r = plan.one('rgb')
+    if plan.has_rgb and not plan.rgb_on_trunk:
       views = plan.by_role('view')
       Wv = cfg.net_width_viewdirs
       bt = plan.one('bottleneck')
@@ -985,17 +1031,30 @@ class Model:
         ops.normals_bwd(M, st.S, st.heads.get('grad_pred'), st.rgd if plan.density_normals else None,
                         rays.viewdirs, st.comp['weights'], om, pm, on_pred, st.d_raw_density,
                         st.d_heads.get('grad_pred'), st.d_rgd if plan.density_normals else None,
-                        head_grads=sc.dhead, stats=stats)
+                        head_grads=sc.dhead, stats=stats,
+                        d_raw_rgb=st.d_raw_rgb if (plan.rgb_on_trunk and sc.dhead is not None) else None)
       if plan.normals_head_cols:
-        # d x_last = relu'(x_last) * ([d raw_density | d grad_pred] @ [w_density | W_grad_pred]^T), with the bias
-        # gradient of the last trunk layer from the same epilogue
+        # d x_last = relu'(x_last) * ([d raw_density | d grad_pred (| d raw_rgb)] @ [w_density | W_grad_pred
+        # (| W_rgb)]^T), with the bias gradient of the last trunk layer from the same epilogue
         ops.gemm(L.GEMM_DGRAD, sc.dhead, mlp.wcat_kn, dy, m=M, n=W, k=plan.normals_head_cols,
                  maskbits=st.bits[-1], colsum=None if side else mlp.b(trunk[-1], g), impl=impl)
-        ops.head_bwd(x_last, mlp.w_nk[d.name], d_raw_density, 1, d.in_pad, dx=None, dw=mlp.W(d, g), db=mlp.b(d, g))
+        if plan.rgb_on_trunk:
+          ops.head_bwd(x_last, mlp.w_head, st.d_raw4, 4, d.in_pad, dx=None, dw=mlp.W(d, g), dw2=mlp.W(r, g),
+                       dw_split=1, db=mlp.b(d, g))
+        else:
+          ops.head_bwd(x_last, mlp.w_nk[d.name], d_raw_density, 1, d.in_pad, dx=None, dw=mlp.W(d, g),
+                       db=mlp.b(d, g))
         self._narrow_heads_bwd(st, mlp)
+      elif plan.rgb_on_trunk:
+        # both heads' input gradient, weight gradients (split between the two master matrices) and bias gradients
+        # [b_density | b_rgb] in one pass
+        ops.head_bwd(x_last, mlp.w_head, st.d_raw4, 4, d.in_pad, dx=dy, relu_mask=True, dw=mlp.W(d, g),
+                     dw2=mlp.W(r, g), dw_split=1, db=mlp.b(d, g), dxsum=None if side else mlp.b(trunk[-1], g),
+                     dx_cols=W)       # features after a skip are constants: dy holds the hidden columns only
       else:
         ops.head_bwd(x_last, mlp.w_nk[d.name], d_raw_density, 1, d.in_pad, dx=dy, relu_mask=True,
-                     dw=mlp.W(d, g), db=mlp.b(d, g), dxsum=None if side else mlp.b(trunk[-1], g))
+                     dw=mlp.W(d, g), db=mlp.b(d, g), dxsum=None if side else mlp.b(trunk[-1], g),
+                     dx_cols=W)       # a trunk ending on a skip layer: dy holds the hidden columns only
     if plan.density_normals:
       # adjoint of the tangent chain: H_last = relu'(x_last) * (d_rgd (x) w_density), three streams
       hcur, hoth = sc.h[0], sc.h[1]

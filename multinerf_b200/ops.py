@@ -29,6 +29,20 @@ def _f32(t):
   return t
 
 
+def _sample_ld(t, channels):
+  """Floats between consecutive samples of an fp32 per-sample tensor: [B, S] (channels 0) or [B, S, channels] with a
+  unit channel stride, whose samples are evenly spaced -- a contiguous tensor, or a column view of a stacked head's
+  [B*S, 4] output."""
+  if t is None:
+    return 0
+  assert t.dtype == torch.float32
+  ld = t.stride(-1) if channels == 0 else t.stride(-2)
+  assert channels == 0 or t.stride(-1) == 1
+  assert all(t.stride(i) == ld * math.prod(t.shape[i + 1:len(t.shape) - (1 if channels else 0)])
+             for i in range(t.dim() - (2 if channels else 1))), 'samples must be evenly spaced'
+  return ld
+
+
 def u_grid(num_samples, randomized):
   """Host-side u grid of stepfun.sample (stepfun.py:190-209): (u_base[S] fp32, max_jitter)."""
   eps = EPS
@@ -165,8 +179,9 @@ def gemm_wgrad(x, dy, out, *, m, n, k, bsum=None, side_w=None, side_aw=None, imp
   return out
 
 
-def chain_desc(mode, m, layers, *, stream=None, stream_cols=0, head_w=None, head_b=None, head_out=None):
-  """Descriptor of one layer-chained launch (include/mnrf.h mnrf_chain_desc).  layers: list of dicts with
+def chain_desc(mode, m, layers, *, stream=None, stream_cols=0, head_w=None, head_b=None, head_out=None, head_n=1):
+  """Descriptor of one layer-chained launch (include/mnrf.h mnrf_chain_desc).  head_w [head_n, 256] fp32, head_out
+  [m, head_n]: the narrow head of the last layer's epilogue (head_n 1 or 4).  layers: list of dicts with
   w [256, ldw] bf16, optional bias / maskbits / colsum / out, n_stream, stream_col0, stream_kb0, n_res, res_kb0.
   The tensors must outlive the descriptor (the caller keeps them: level-state / weight buffers)."""
   d = L.ChainDesc()
@@ -175,7 +190,8 @@ def chain_desc(mode, m, layers, *, stream=None, stream_cols=0, head_w=None, head
     assert stream.dtype == torch.bfloat16 and stream.stride(1) == 1
     d.stream, d.ldstream = stream.data_ptr(), stream.stride(0)
   if head_w is not None:
-    d.head_w, d.head_out = head_w.data_ptr(), head_out.data_ptr()
+    assert head_w.is_contiguous() and head_w.numel() == head_n * 256 and head_out.is_contiguous()
+    d.head_w, d.head_out, d.head_n = head_w.data_ptr(), head_out.data_ptr(), head_n
     d.head_b = head_b.data_ptr() if head_b is not None else None
   flops = 0.0
   for j, ly in enumerate(layers):
@@ -226,13 +242,17 @@ def head_fwd(x, w_nk, bias, n_out, k, raw=None):
   return raw
 
 
-def head_bwd(x, w_nk, draw, n_out, k, dx=None, relu_mask=False, dw=None, db=None, dxsum=None):
+def head_bwd(x, w_nk, draw, n_out, k, dx=None, relu_mask=False, dw=None, db=None, dxsum=None, dw2=None, dw_split=0,
+             dx_cols=0):
+  """dw2 / dw_split: outputs [dw_split, n_out) put their weight gradient in dw2; dx_cols: dx and dxsum cover the
+  first dx_cols columns only (include/mnrf.h)."""
   lib = L.load()
   M = x.shape[0]
   _count()
   L.check(lib.mnrf_head_bwd(M, k, n_out, L.ptr(x), x.stride(0), L.ptr(w_nk), L.ptr(_f32(draw)),
                             L.ptr(dx), dx.stride(0) if dx is not None else 0, int(relu_mask),
-                            L.ptr(dw), L.ptr(db), L.ptr(dxsum), L.stream_ptr()))
+                            L.ptr(dw), L.ptr(dw2), int(dw_split), L.ptr(db), L.ptr(dxsum), int(dx_cols),
+                            L.stream_ptr()))
 
 
 def colsum(x, n, out):
@@ -258,6 +278,7 @@ def composite_fwd(raw_density, raw_rgb, sdist, directions, near, far, *, cfg, de
   B, S = raw_density.shape
   dev = raw_density.device
   d = _cdesc(B, S, **cfg)
+  d.ld_density, d.ld_rgb = _sample_ld(raw_density, 0), _sample_ld(raw_rgb, 3)
   weights = torch.empty(B, S, device=dev)
   rgb = torch.empty(B, 3, device=dev)
   dens = torch.empty(B, S, device=dev) if want_samples else None
@@ -265,7 +286,7 @@ def composite_fwd(raw_density, raw_rgb, sdist, directions, near, far, *, cfg, de
   acc = torch.empty(B, device=dev) if want_extras else None
   dist = torch.empty(B, 4, device=dev) if want_extras else None
   _count()
-  L.check(lib.mnrf_composite_fwd(C.byref(d), L.ptr(_f32(raw_density)), L.ptr(_f32(raw_rgb)),
+  L.check(lib.mnrf_composite_fwd(C.byref(d), L.ptr(raw_density), L.ptr(raw_rgb),
                                  L.ptr(_f32(density_noise)), L.ptr(_f32(sdist)),
                                  L.ptr(_f32(directions)), L.ptr(_f32(near)), L.ptr(_f32(far)),
                                  L.ptr(_f32(bg_rgb)), L.ptr(_f32(rgb_scale)), L.ptr(_f32(raw_diffuse)),
@@ -293,8 +314,11 @@ def composite_bwd(raw_density, raw_rgb, sdist, directions, near, far, target_rgb
     d_raw_density = torch.empty(B, S, device=dev)
   if raw_rgb is not None and d_raw_rgb is None:
     d_raw_rgb = torch.empty(B, S, 3, device=dev)
+  # the gradients share the raw values' sample spacing (one pair of strides in the descriptor)
+  d.c.ld_density, d.c.ld_rgb = _sample_ld(raw_density, 0), _sample_ld(raw_rgb, 3)
+  assert _sample_ld(d_raw_density, 0) == d.c.ld_density and (raw_rgb is None or _sample_ld(d_raw_rgb, 3) == d.c.ld_rgb)
   _count()
-  head = (C.byref(d), L.ptr(_f32(raw_density)), L.ptr(_f32(raw_rgb)), L.ptr(_f32(density_noise)),
+  head = (C.byref(d), L.ptr(raw_density), L.ptr(raw_rgb), L.ptr(_f32(density_noise)),
           L.ptr(_f32(sdist)), L.ptr(_f32(directions)), L.ptr(_f32(near)), L.ptr(_f32(far)), L.ptr(_f32(bg_rgb)),
           L.ptr(_f32(rgb_scale)), L.ptr(_f32(raw_diffuse)), L.ptr(_f32(raw_tint)), L.ptr(_f32(extra_dw)),
           L.ptr(_f32(target_rgb)), L.ptr(_f32(lossmult)), L.ptr(_f32(inv_denom)), L.ptr(_f32(sdist_fine)),
@@ -434,14 +458,18 @@ def normals_fwd(M, S, grad_pred, raw_grad_density, viewdirs, normals_pred, norma
 
 
 def normals_bwd(M, S, grad_pred, raw_grad_density, viewdirs, weights, orient_mult, prednorm_mult, orient_on_pred,
-                d_raw_density, d_grad_pred, d_raw_grad_density, head_grads=None, stats=None):
+                d_raw_density, d_grad_pred, d_raw_grad_density, head_grads=None, stats=None, d_raw_rgb=None):
+  """d_raw_rgb (with head_grads): the gradient of an rgb head on the same trunk, written to head_grads[:, 4:7]."""
   lib = L.load()
+  ld_raw = _sample_ld(d_raw_density, 0)
+  assert d_raw_rgb is None or _sample_ld(d_raw_rgb, 3) == ld_raw
   if head_grads is not None:
     assert head_grads.dtype == torch.bfloat16 and head_grads.stride(1) == 1
   _count()
   L.check(lib.mnrf_normals_bwd(M, S, L.ptr(_f32(grad_pred)), L.ptr(_f32(raw_grad_density)), L.ptr(_f32(viewdirs)),
                                L.ptr(_f32(weights)), float(orient_mult), float(prednorm_mult), int(orient_on_pred),
-                               L.ptr(_f32(d_raw_density)), L.ptr(_f32(d_grad_pred)), L.ptr(_f32(d_raw_grad_density)),
+                               L.ptr(d_raw_density), L.ptr(d_raw_rgb), ld_raw, L.ptr(_f32(d_grad_pred)),
+                               L.ptr(_f32(d_raw_grad_density)),
                                L.ptr(head_grads), head_grads.stride(0) if head_grads is not None else 0,
                                L.ptr(stats), L.stream_ptr()))
 
