@@ -12,6 +12,7 @@ There is no CPU path: constructing a Model without an H100 raises.
 """
 import dataclasses
 import math
+import os
 from typing import Any, Dict, List, Optional
 
 import numpy as np
@@ -87,7 +88,7 @@ class MLPPlan:
         x_dim, x_pad, x_has_feat = W + self.F, W + self.Fpad, True
       else:
         x_dim, x_pad, x_has_feat = W, W, False
-    self.last_has_feat = x_has_feat
+    self.last_has_feat = x_has_feat       # the heads read [hidden | features] after a skip layer
     self.x_dim, self.x_pad = x_dim, x_pad
     rmx = np.concatenate([np.arange(W), W + np.arange(self.F)]) if x_has_feat else None
     add('density', x_dim, x_pad, 1, True, rm=rmx)
@@ -95,23 +96,23 @@ class MLPPlan:
       add('grad_pred', x_dim, x_pad, 3, True, rm=rmx)
     self.has_rgb = not cfg.disable_rgb
     self.use_viewdirs = use_viewdirs
-    # view-independent colour (models.py:512,584): rgb = act(Dense(3)(x)) on the trunk output, no view branch.  The
-    # rgb head runs stacked with the density head as one 4-output head: raw [M, 4] = [raw_density | raw_rgb]
-    self.rgb_on_trunk = self.has_rgb and not use_viewdirs
+    # What sits on top of the trunk, decided here once (every other site reads `top`, `ref_stage`, `slab_cols`):
+    #   'view':    bottleneck -> Ref-NeRF stage (`ref_stage`) or direction encoding -> GLO -> view MLP -> rgb head
+    #   'density': the Dense(1) density head
+    #   'stacked': view-independent colour (models.py:512,584), rgb = act(Dense(3)(x)) on the trunk output.  The rgb
+    #              head runs stacked with the density head as one 4-output head: raw [M, 4] = [raw_density | raw_rgb]
+    # each with the narrow heads on the trunk output; without a view branch, normals feed only the orientation /
+    # predicted-normal losses and the renderings through the colourless normals stage (csrc/refnerf.cu normals_*)
+    self.top = ('view' if use_viewdirs else 'stacked') if self.has_rgb else 'density'
+    self.head_n = 4 if self.top == 'stacked' else 1
     self.ref_stage = False
-    # normals of an MLP without a view branch feed only the orientation / predicted-normal losses and the
-    # renderings (csrc/refnerf.cu normals_fwd/bwd)
-    self.normals_stage = (self.pred_normals or self.density_normals) and (not self.has_rgb or self.rgb_on_trunk)
-    # K of the trunk-top dgrad GEMM of such an MLP with predicted normals: [d raw_density | d grad_pred (| d raw_rgb)
-    # | 0]
-    self.normals_head_cols = 64 if (self.normals_stage and self.pred_normals) else 0
-    if self.rgb_on_trunk:
+    if self.top == 'stacked':
       if cfg.use_diffuse_color:
         raise ValueError('use_viewdirs=False with use_diffuse_color: the reference reads raw_rgb_diffuse, which it '
                          'creates only with view directions (internal/models.py:591)')
       # Ref-NeRF heads and encodings are not created without view directions (models.py:512); normals still run
       add('rgb', x_dim, x_pad, cfg.num_rgb_channels, True, rm=rmx)
-    elif self.has_rgb:
+    elif self.top == 'view':
       if cfg.bottleneck_width <= 0:
         if not cfg.use_reflections:
           raise ValueError('bottleneck_width = 0 needs use_reflections: the reference reads bottleneck.shape to '
@@ -167,21 +168,41 @@ class MLPPlan:
       if cfg.net_depth_viewdirs == 0:
         raise NotImplementedError('net_depth_viewdirs == 0')
       add('rgb', v_dim, v_pad, cfg.num_rgb_channels, True, rm=rmv)
+      # columns of d vin the first view layer's dgrad writes: the Ref-NeRF stage and GLO read past the bottleneck
+      self.d_vin_cols = vin_pad if (self.ref_stage or glo_features > 0) else bw
     off = 0
     for sp in specs:
       sp.w_off = off
       off += sp.in_pad * sp.out_dim
       off = (off + 3) // 4 * 4
-      if self.rgb_on_trunk and sp.role == 'rgb':
+      if self.top == 'stacked' and sp.role == 'rgb':
         # the density head's bias block holds [b_density | b_rgb]: the stacked head's bias and bias gradient
         sp.b_off = self.one('density', specs).b_off + 1
         continue
       sp.b_off = off
-      off += 4 if (self.rgb_on_trunk and sp.role == 'density') else sp.out_dim
+      off += self.head_n if sp.role == 'density' else sp.out_dim
       off = (off + 3) // 4 * 4
     self.specs = specs
     self.flat_size = off
     self.num_params = sum(sp.in_dim * sp.out_dim + sp.out_dim for sp in specs)
+    self.narrow = [sp for sp in specs if sp.role in ('grad_pred', 'diffuse', 'tint', 'roughness')]
+    # the colourless normals stage (normals of an MLP without a view branch); either normals stage takes the losses
+    self.normals_stage = self.top != 'view' and (self.pred_normals or self.density_normals)
+    self.has_normals_stage = self.ref_stage or self.normals_stage
+    # Width of the head-gradient slab that ONE dgrad GEMM runs against `MLPDevice.wcat_kn` at the top of the trunk:
+    # [d bottleneck | Ref-NeRF head gradients] with the Ref-NeRF stage, [d raw_density | d grad_pred (| d raw_rgb) |
+    # 0] in the colourless normals stage with predicted normals, no slab otherwise.  `slab_heads` are the
+    # (head, first slab column) pairs; a view-independent rgb head takes the diffuse slot (it has no diffuse head).
+    if self.ref_stage:
+      self.slab_cols, c0, slots = self.vin_pad, self.cfg.bottleneck_width, self.HEAD_SLOTS
+    else:
+      self.slab_cols = 64 if (self.normals_stage and self.pred_normals) else 0
+      c0, slots = 0, dict(self.HEAD_SLOTS, rgb=self.HEAD_SLOTS['diffuse'])
+    self.slab_heads = [(sp, c0 + slots[sp.role][0]) for sp in specs if self.slab_cols and sp.role in slots]
+
+  # names kept for the layout tests and tools that read them
+  rgb_on_trunk = property(lambda self: self.top == 'stacked')
+  normals_head_cols = property(lambda self: 0 if self.ref_stage else self.slab_cols)
 
   def by_role(self, role):
     return [sp for sp in self.specs if sp.role == role]
@@ -192,25 +213,45 @@ class MLPPlan:
 
 
 class MLPDevice:
-  """Device state of one MLP: fp32 master slice, bf16 shadows, gradient views."""
+  """Device state of one MLP: fp32 master slice, bf16 shadows, gradient views.
+
+  Every buffer is allocated here and only filled afterwards: captured CUDA graphs hold these pointers."""
 
   def __init__(self, plan: MLPPlan, master, grads, device):
     self.plan = plan
     self.master, self.grads = master, grads           # views into the global flat buffers
     self.device = device
     self.basis = torch.tensor(plan.basis, device=device)
-    self.w_nk, self.w_kn, self.colv = {}, {}, {}
-    if plan.rgb_on_trunk:
-      # [w_density; W_rgb]: the density and rgb heads of a view-independent model as one 4-output head
-      d, r = plan.one('density'), plan.one('rgb')
-      self.w_head = torch.zeros(4, d.in_pad, device=device, dtype=torch.bfloat16)
-      self.w_nk[d.name], self.w_nk[r.name] = self.w_head[:1], self.w_head[1:]
+    self.w_nk, self.w_kn = {}, {}
+    d = plan.one('density')
+    # [head_n, x_pad]: the density head, or [w_density; W_rgb], the density and rgb heads of a view-independent
+    # model as one 4-output head
+    self.w_head = torch.zeros(plan.head_n, d.in_pad, device=device, dtype=torch.bfloat16)
+    self.w_nk[d.name] = self.w_head[:1]
+    if plan.top == 'stacked':
+      self.w_nk[plan.one('rgb').name] = self.w_head[1:]
     for sp in plan.specs:
       if sp.name in self.w_nk:
         continue
       self.w_nk[sp.name] = torch.zeros(sp.out_dim, sp.in_pad, device=device, dtype=torch.bfloat16)
       if not sp.head:
         self.w_kn[sp.name] = torch.zeros(sp.in_pad, sp.out_dim, device=device, dtype=torch.bfloat16)
+    self._pack_table = ops.pack_table([(self.W(sp), self.w_nk[sp.name], self.w_kn.get(sp.name))
+                                       for sp in plan.specs], self.device)
+    # fp32 rows of the density (or stacked) head, bf16-rounded as the fwd used: the chained trunk's epilogue head,
+    # and row 0, colv_density, for DGRAD colv / outer_mask
+    self.colv_head = torch.zeros(plan.head_n, d.in_pad, device=device)
+    self.colv_density = self.colv_head[0]
+    # [x_pad, slab_cols] K-major B operand of the trunk-top dgrad: [ W_bottleneck | head weights ] with the Ref-NeRF
+    # stage, [ w_density | W_grad_pred (| W_rgb) | 0 ] in the colourless normals stage
+    self.wcat_kn = (torch.zeros(plan.x_pad, plan.slab_cols, device=device, dtype=torch.bfloat16)
+                    if plan.slab_cols else None)
+    self.ide = None
+    if plan.cfg.use_directional_enc:
+      from . import ref_utils
+      m, l, mat = ref_utils.ide_tables(plan.cfg.deg_view)
+      self.ide = (torch.tensor(mat, dtype=torch.float32, device=device).contiguous(),
+                  torch.tensor(np.stack([m, l]), dtype=torch.int32, device=device).contiguous(), len(m))
     self.repack()
 
   def W(self, s, buf=None):
@@ -222,54 +263,61 @@ class MLPDevice:
     return buf[s.b_off:s.b_off + s.out_dim]
 
   def repack(self):
-    """fp32 master -> bf16 operand layouts (after init and after every optimizer step)."""
+    """fp32 master -> bf16 operand layouts (after init and after every optimizer step), in place."""
     plan = self.plan
-    if getattr(self, '_pack_table', None) is None:      # buffers never move: build the device table once
-      self._pack_table = ops.pack_table([(self.W(sp), self.w_nk[sp.name], self.w_kn.get(sp.name))
-                                         for sp in plan.specs], self.device)
     ops.pack_weights_batched(self._pack_table)
-    d = plan.one('density')
-    # bf16-rounded, as the fwd used.  Updated IN PLACE: captured CUDA graphs hold this pointer
-    # (DGRAD colv / outer_mask), so the tensor must never be re-allocated.
-    if plan.rgb_on_trunk:
-      # fp32 rows of the stacked head (the chained trunk's epilogue head); row 0 is colv_density
-      if getattr(self, 'colv_head', None) is None:
-        self.colv_head = torch.zeros(4, d.in_pad, device=self.device)
-        self.colv_density = self.colv_head[0]
-      self.colv_head.copy_(self.w_head)
-    else:
-      if getattr(self, 'colv_density', None) is None:
-        self.colv_density = torch.zeros(d.in_pad, device=self.device)
-      self.colv_density.copy_(self.w_nk[d.name][0])
-    if plan.ref_stage or plan.normals_head_cols:
-      # [x_pad, vin_pad] K-major B operand of the trunk-entry dgrad:  [ W_bottleneck | head weights ]
-      # (colourless MLP with predicted normals: [x_pad, 64] = [ w_density | W_grad_pred | 0 ])
+    self.colv_head.copy_(self.w_head)
+    if plan.ref_stage:
       bt = plan.one('bottleneck')
-      bw = bt.out_dim if plan.ref_stage else 0
-      if not hasattr(self, 'wcat_kn'):
-        cols = plan.vin_pad if plan.ref_stage else plan.normals_head_cols
-        self.wcat_kn = torch.zeros(plan.x_pad, cols, device=self.device, dtype=torch.bfloat16)
-      if plan.ref_stage:
-        self.wcat_kn[:, :bw] = self.w_kn[bt.name]
-      # a view-independent model's rgb head takes the diffuse slot (it has no diffuse head, MLPPlan)
-      slots = dict(plan.HEAD_SLOTS, rgb=plan.HEAD_SLOTS['diffuse']) if plan.rgb_on_trunk else plan.HEAD_SLOTS
-      for role, (c0, n) in slots.items():
-        sp = plan.one(role)
-        if sp is not None:
-          self.wcat_kn[:, bw + c0:bw + c0 + n] = self.w_nk[sp.name].t()
-
-  def ide_tables(self):
-    if not hasattr(self, '_ide'):
-      from . import ref_utils
-      m, l, mat = ref_utils.ide_tables(self.plan.cfg.deg_view)
-      self._ide = (torch.tensor(mat, dtype=torch.float32, device=self.device).contiguous(),
-                   torch.tensor(np.stack([m, l]), dtype=torch.int32, device=self.device).contiguous(), len(m))
-    return self._ide
+      self.wcat_kn[:, :bt.out_dim] = self.w_kn[bt.name]
+    for sp, c0 in plan.slab_heads:
+      self.wcat_kn[:, c0:c0 + sp.out_dim] = self.w_nk[sp.name].t()
 
 
 class LevelState:
-  """Per-level device buffers kept from forward for the backward pass."""
-  pass
+  """Per-level device buffers kept from forward for the backward pass.  Model._level_state allocates them once per
+  (level, module, shape): captured CUDA graphs hold their pointers.  Buffers of absent stages stay None."""
+
+  def __init__(self, B, S, mname):
+    self.B, self.S, self.M, self.mname = B, S, B * S, mname     # M: rows (samples) of the level
+    self.sdist = None
+    # trunk activations, features (+ their copies into later skip layers) and ReLU masks; tangent streams
+    self.acts, self.feat, self.feat_copies, self.bits = [], None, [], []
+    self.tacts, self.tfeat, self.tfeat_copies, self.rgd, self.d_rgd = [], None, [], None, None
+    # raw_head / d_raw_head [M, head_n]: the density (or stacked [density | rgb]) head's output and gradient, of which
+    # raw_density (and a stacked raw_rgb) are views
+    self.raw_head = self.d_raw_head = self.raw_density = self.d_raw_density = self.raw_rgb = self.d_raw_rgb = None
+    self.heads, self.d_heads = {}, {}          # narrow heads by role
+    self.normals = self.normals_pred = self.roughness = self.extra_dw = None
+    self.vacts, self.vbits, self.vin = [], [], None
+    self.x_last = self.t_last = self.v_last = None   # inputs of the last trunk layer / tangent stream / view layer
+    self.bwd = None         # BwdScratch, allocated on the first backward
+    self.keep_acts = True   # False: render-only pass, the chained trunk skips activation / mask stores
+    self.chain = {}         # chain descriptors (Model.bind drops them)
+    # set per call by Model.forward_levels
+    self.lv, self.is_prop, self.glo_vec, self.bneck_noise, self.loss_mults = None, False, None, None, None
+    self.noise = self.comp_cfg = self.bg_rgb = self.comp = self.rgb_scale = None
+    self.d_rgb_scale = None   # gradient of rgb_scale, allocated on first use (train_utils)
+
+
+class BwdScratch:
+  """Gradient buffers of one level's backward, allocated on its first backward."""
+
+  def __init__(self, plan, M, chained, dev):
+    cfg, bf = plan.cfg, torch.bfloat16
+    # trunk: per-layer gradient buffers when the dgrad chain runs as one launch (its wgrads come after), else two
+    self.dy = [torch.empty(M, cfg.net_width, device=dev, dtype=bf) for _ in range(cfg.net_depth if chained else 2)]
+    self.dv = self.d_vin = self.d_vin_skip = self.dhead = self.h = None
+    if plan.top == 'view':
+      self.dv = [torch.empty(M, cfg.net_width_viewdirs, device=dev, dtype=bf) for _ in range(2)]
+      self.d_vin = torch.empty(M, plan.vin_pad, device=dev, dtype=bf)
+      # the view layer after a skip also consumed vin
+      self.d_vin_skip = torch.empty(M, plan.vin_pad, device=dev, dtype=bf) if plan.view_concat_after else None
+    elif plan.slab_cols:
+      # zero-filled once: the normals backward writes only its first four (seven) columns
+      self.dhead = torch.zeros(M, plan.slab_cols, device=dev, dtype=bf)
+    if plan.density_normals:
+      self.h = [torch.empty(3 * M, cfg.net_width, device=dev, dtype=bf) for _ in range(2)]    # tangent adjoints
 
 
 def _loss_args(loss_mults):
@@ -410,37 +458,29 @@ class Model:
     self.mlps = {n: MLPDevice(p, params.seg(n), params.seg(n, params.grads), self.device)
                  for n, p in self.plans.items()}
     for st in self._levels.values():        # cached chain descriptors point into the previous buffers
-      st.__dict__.pop('_chain', None)
+      st.chain.clear()
+
+  def _export(self, buf):
+    """`buf` (the flat parameters or their gradients) as the reference's flax tree (numpy), without padding rows."""
+    out = {}
+    for mname, plan in self.plans.items():
+      mlp, seg = self.mlps[mname], self.params.seg(mname, buf)
+      out[mname] = {}
+      for s in plan.specs:
+        Wp = mlp.W(s, seg).detach().cpu().numpy()
+        rows = s.row_map if s.row_map is not None else np.arange(s.in_dim)
+        out[mname][s.name] = {'kernel': Wp[rows].copy(), 'bias': mlp.b(s, seg).detach().cpu().numpy().copy()}
+    for name in self.extra_params:
+      out[name] = {'embedding': self.params.seg(name, buf).detach().cpu().numpy().reshape(
+          self.mcfg.num_glo_embeddings, -1).copy()}
+    return out
 
   def export_flax(self):
     """Parameters as the reference's flax tree (numpy), dropping the padding rows."""
-    out = {}
-    for mname, plan in self.plans.items():
-      mlp = self.mlps[mname]
-      out[mname] = {}
-      for s in plan.specs:
-        Wp = mlp.W(s).detach().cpu().numpy()
-        rows = s.row_map if s.row_map is not None else np.arange(s.in_dim)
-        out[mname][s.name] = {'kernel': Wp[rows].copy(), 'bias': mlp.b(s).detach().cpu().numpy().copy()}
-    for name in self.extra_params:
-      out[name] = {'embedding': self.params.seg(name).detach().cpu().numpy().reshape(
-          self.mcfg.num_glo_embeddings, -1).copy()}
-    return out
+    return self._export(self.params.flat)
 
   def export_grads_flax(self):
-    out = {}
-    for mname, plan in self.plans.items():
-      mlp = self.mlps[mname]
-      out[mname] = {}
-      for s in plan.specs:
-        Wp = mlp.W(s, mlp.grads).detach().cpu().numpy()
-        rows = s.row_map if s.row_map is not None else np.arange(s.in_dim)
-        out[mname][s.name] = {'kernel': Wp[rows].copy(),
-                              'bias': mlp.b(s, mlp.grads).detach().cpu().numpy().copy()}
-    for name in self.extra_params:
-      out[name] = {'embedding': self.params.seg(name, self.params.grads).detach().cpu().numpy().reshape(
-          self.mcfg.num_glo_embeddings, -1).copy()}
-    return out
+    return self._export(self.params.grads)
 
   # ------------------------------------------------------------------ schedule
   def level_schedule(self, train_frac):
@@ -487,16 +527,14 @@ class Model:
     # an image) must not free them
     key = (key, mname, B, S)
     st = self._levels.get(key)
-    plan = self.plans[mname]
     if st is not None:
       return st
-    st = LevelState()
-    st.B, st.S, st.mname = B, S, mname
-    M = B * S
-    dev = self.device
+    plan = self.plans[mname]
     cfg = plan.cfg
     W = cfg.net_width
-    bf = torch.bfloat16
+    M = B * S
+    dev, bf = self.device, torch.bfloat16
+    st = LevelState(B, S, mname)
     st.sdist = torch.empty(B, S + 1, device=dev)
 
     def trunk_buffers(rows):
@@ -512,25 +550,20 @@ class Model:
       return acts, feat, copies
     st.acts, st.feat, st.feat_copies = trunk_buffers(M)
     st.bits = [torch.empty(M, W // 32, device=dev, dtype=torch.int32) for _ in range(cfg.net_depth)]
-    st.raw_density = torch.empty(B, S, device=dev)
-    st.d_raw_density = torch.empty(B, S, device=dev)
-    st.raw_rgb = st.d_raw_rgb = None
-    st.heads, st.d_heads = {}, {}
-    st.extra_dw = None
-    st.normals = st.normals_pred = st.roughness = None
     if plan.density_normals:
       # forward-mode tangents d(.)/d(mean_x|y|z), three stacked streams of M rows
       st.tacts, st.tfeat, st.tfeat_copies = trunk_buffers(3 * M)
       st.rgd = torch.empty(3, M, device=dev)
       st.d_rgd = torch.empty(3, M, device=dev)
       st.normals = torch.empty(M, 3, device=dev)
-    if plan.rgb_on_trunk:
-      # the stacked head's output and its gradient, [M, 4] = [density | rgb]: compositing reads and writes them in
-      # place through sample strides
-      st.raw4, st.d_raw4 = torch.empty(M, 4, device=dev), torch.empty(M, 4, device=dev)
-      st.raw_density, st.raw_rgb = st.raw4.view(B, S, 4)[..., 0], st.raw4.view(B, S, 4)[..., 1:]
-      st.d_raw_density, st.d_raw_rgb = st.d_raw4.view(B, S, 4)[..., 0], st.d_raw4.view(B, S, 4)[..., 1:]
-    elif plan.has_rgb:
+    # the head's output and its gradient, [M, head_n] (stacked: [density | rgb]): compositing reads and writes them
+    # in place through sample strides
+    st.raw_head, st.d_raw_head = torch.empty(M, plan.head_n, device=dev), torch.empty(M, plan.head_n, device=dev)
+    st.raw_density = st.raw_head.view(B, S, plan.head_n)[..., 0]
+    st.d_raw_density = st.d_raw_head.view(B, S, plan.head_n)[..., 0]
+    if plan.top == 'stacked':
+      st.raw_rgb, st.d_raw_rgb = st.raw_head.view(B, S, 4)[..., 1:], st.d_raw_head.view(B, S, 4)[..., 1:]
+    elif plan.top == 'view':
       Wv = cfg.net_width_viewdirs
       nv = cfg.net_depth_viewdirs
       st.vacts = [torch.empty(M, Wv + plan.vin_pad if i in plan.view_concat_after else Wv, device=dev, dtype=bf)
@@ -542,33 +575,29 @@ class Model:
         st.vin = torch.empty(M, plan.vin_pad, device=dev, dtype=bf)
       st.raw_rgb = torch.empty(B, S, 3, device=dev)
       st.d_raw_rgb = torch.empty(B, S, 3, device=dev)
-    for role in ('grad_pred', 'diffuse', 'tint', 'roughness'):
-      sp = plan.one(role)
-      if sp is not None:
-        st.heads[role] = torch.empty(M, sp.out_dim, device=dev)
-        st.d_heads[role] = torch.empty(M, sp.out_dim, device=dev)
-    if plan.ref_stage or plan.normals_stage:
+    for sp in plan.narrow:
+      st.heads[sp.role] = torch.empty(M, sp.out_dim, device=dev)
+      st.d_heads[sp.role] = torch.empty(M, sp.out_dim, device=dev)
+    if plan.has_normals_stage:
       if plan.pred_normals:
         st.normals_pred = torch.empty(M, 3, device=dev)
       if plan.ref_stage and cfg.enable_pred_roughness:
         st.roughness = torch.empty(M, device=dev)
       st.extra_dw = torch.empty(B, S, device=dev)
-    st.bwd = None   # backward scratch, allocated on first backward
-    st.keep_acts = True     # False: render-only pass, the chained trunk skips activation / mask stores
     self._levels[key] = st
     return st
 
-  def _refdir_desc(self, st, plan):
+  def _refdir_args(self, st, mlp, rays):
+    """The leading arguments of ops.refdir_fwd / refdir_bwd: descriptor, IDE tables and the stage's inputs."""
+    plan = mlp.plan
     cfg = plan.cfg
-    bw = cfg.bottleneck_width
-    ide_n = self.mlps[st.mname].ide_tables()[2] if cfg.use_directional_enc else 0
-    return ops.refdir_desc(
-        st.B * st.S, st.S, use_pred_normals=plan.pred_normals, use_density_normals=plan.density_normals,
+    mat, ml, ide_n = mlp.ide or (None, None, 0)
+    desc = ops.refdir_desc(
+        st.M, st.S, use_pred_normals=plan.pred_normals, use_density_normals=plan.density_normals,
         use_reflections=cfg.use_reflections, use_ide=cfg.use_directional_enc, use_n_dot_v=cfg.use_n_dot_v,
         use_roughness=cfg.enable_pred_roughness, deg_view=cfg.deg_view, ide_n=ide_n,
-        roughness_bias=cfg.roughness_bias, ld=0, col0=bw, col_end=plan.vin_pad)
-
-  # NB: with GLO the slab's zero-fill would also clear the GLO columns; they are written after it.
+        roughness_bias=cfg.roughness_bias, ld=st.vin.stride(0), col0=cfg.bottleneck_width, col_end=plan.vin_pad)
+    return desc, mat, ml, st.heads.get('grad_pred'), st.heads.get('roughness'), st.rgd, rays.viewdirs
 
   # ------------------------------------------------------------------ forward
   def _mlp_forward(self, st: LevelState, mlp: MLPDevice, rays, impl=0, loss_mults=None):
@@ -576,77 +605,83 @@ class Model:
     of rays, + orientation target flag: when given, the normals stage (Ref-NeRF or colourless) also emits
     d(loss)/d(weights)."""
     plan = mlp.plan
+    self._trunk_fwd(st, mlp, rays, impl)
+    if plan.density_normals:
+      self._tangent_fwd(st, mlp, impl)
+    for sp in plan.narrow:
+      ops.head_fwd(st.x_last, mlp.w_nk[sp.name], mlp.b(sp), sp.out_dim, sp.in_pad, raw=st.heads[sp.role])
+    # (orientation, predicted-normal, target flag, d(loss)/d(weights) output) of the normals stage
+    normals_args = _loss_args(loss_mults) + (st.extra_dw if loss_mults is not None else None,)
+    if plan.normals_stage:
+      ops.normals_fwd(st.M, st.S, st.heads.get('grad_pred'), st.rgd, rays.viewdirs, st.normals_pred,
+                      st.normals, *normals_args)
+    if plan.top == 'view':
+      self._view_fwd(st, mlp, rays, impl, normals_args)
+
+  def _trunk_fwd(self, st, mlp, rays, impl):
+    """Encoding, the trunk (one chained launch, or one GEMM per layer) and the density (or stacked) head."""
+    plan = mlp.plan
     cfg = plan.cfg
-    B, S = st.B, st.S
-    M = B * S
     W = cfg.net_width
     m = self.mcfg
     ops.encode(st.sdist, rays.origins, rays.directions, rays.radii_flat, rays.near_flat,
                rays.far_flat, mlp.basis, min_deg=cfg.min_deg_point, max_deg=cfg.max_deg_point,
                raydist_fn=m.raydist_fn, ray_shape=m.ray_shape, warp_contract=cfg.warp_fn == 'contract',
-               disable_integration=m.disable_integration, feat=st.feat, feat_cols=plan.Fpad,
-               tfeat=st.tfeat if plan.density_normals else None)
+               disable_integration=m.disable_integration, feat=st.feat, feat_cols=plan.Fpad, tfeat=st.tfeat)
     for c in st.feat_copies:
       c.copy_(st.feat)
     x = st.feat
-    trunk = plan.by_role('trunk')
-    d = plan.one('density')
-    chained = self._use_chain(plan, M, impl)
+    chained = self._use_chain(plan, st.M, impl)
     if chained:
-      # the whole trunk (+ the Dense(1) density head when it reads the plain 256-wide output) in ONE launch
+      # the whole trunk (+ the density head when it reads the plain 256-wide output) in ONE launch
       ops.mlp_chain(self._chain_fwd_desc(st, mlp))
       x = st.acts[-1]
     else:
-      for i, sp in enumerate(trunk):
-        ops.gemm(L.GEMM_FWD, x, mlp.w_nk[sp.name], st.acts[i][:, :W], m=M, n=W, k=sp.in_pad, act=L.ACT_RELU,
+      for i, sp in enumerate(plan.by_role('trunk')):
+        ops.gemm(L.GEMM_FWD, x, mlp.w_nk[sp.name], st.acts[i][:, :W], m=st.M, n=W, k=sp.in_pad, act=L.ACT_RELU,
                  bias=mlp.b(sp), maskbits=st.bits[i], impl=impl)
         x = st.acts[i]          # full width (incl. concatenated features) feeds the next layer
     if not chained or plan.last_has_feat:
-      if plan.rgb_on_trunk:     # density + rgb in one pass over the trunk output (bias block [b_density | b_rgb])
-        ops.head_fwd(x, mlp.w_head, mlp.b(d), 4, d.in_pad, raw=st.raw4)
-      else:
-        ops.head_fwd(x, mlp.w_nk[d.name], mlp.b(d), 1, d.in_pad, raw=st.raw_density.view(M, 1))
+      # stacked: density + rgb in one pass over the trunk output (bias block [b_density | b_rgb])
+      d = plan.one('density')
+      ops.head_fwd(x, mlp.w_head, mlp.b(d), plan.head_n, d.in_pad, raw=st.raw_head)
     st.x_last = x
-    if plan.density_normals:
-      # raw_grad_density = d raw_density / d mean by forward mode (replaces vmap(value_and_grad),
-      # models.py:473-492): tangents see the same weights, no bias, and the primal's ReLU masks
-      for c in st.tfeat_copies:
-        c.copy_(st.tfeat)
-      t = st.tfeat
-      for i, sp in enumerate(trunk):
-        ops.gemm(L.GEMM_DGRAD, t, mlp.w_nk[sp.name], st.tacts[i][:, :W], m=3 * M, n=W, k=sp.in_pad,
-                 maskbits=st.bits[i], mask_mod=M, impl=impl)
-        t = st.tacts[i]
-      st.t_last = t
-      ops.head_fwd(t, mlp.w_nk[d.name], None, 1, d.in_pad, raw=st.rgd.view(3 * M, 1))
-    for role in ('grad_pred', 'diffuse', 'tint', 'roughness'):
-      sp = plan.one(role)
-      if sp is not None:
-        ops.head_fwd(x, mlp.w_nk[sp.name], mlp.b(sp), sp.out_dim, sp.in_pad, raw=st.heads[role])
-    om, pm, on_pred = _loss_args(loss_mults)
-    extra_dw = st.extra_dw if loss_mults is not None else None
-    if plan.normals_stage:
-      ops.normals_fwd(M, S, st.heads.get('grad_pred'), st.rgd if plan.density_normals else None, rays.viewdirs,
-                      st.normals_pred, st.normals, om, pm, on_pred, extra_dw)
-    if not plan.has_rgb or plan.rgb_on_trunk:
-      return
+
+  def _tangent_fwd(self, st, mlp, impl):
+    """raw_grad_density = d raw_density / d mean by forward mode (replaces vmap(value_and_grad),
+    models.py:473-492): tangents see the same weights, no bias, and the primal's ReLU masks."""
+    plan = mlp.plan
+    W = plan.cfg.net_width
+    for c in st.tfeat_copies:
+      c.copy_(st.tfeat)
+    t = st.tfeat
+    for i, sp in enumerate(plan.by_role('trunk')):
+      ops.gemm(L.GEMM_DGRAD, t, mlp.w_nk[sp.name], st.tacts[i][:, :W], m=3 * st.M, n=W, k=sp.in_pad,
+               maskbits=st.bits[i], mask_mod=st.M, impl=impl)
+      t = st.tacts[i]
+    st.t_last = t
+    d = plan.one('density')
+    ops.head_fwd(t, mlp.w_nk[d.name], None, 1, d.in_pad, raw=st.rgd.view(3 * st.M, 1))
+
+  def _view_fwd(self, st, mlp, rays, impl, normals_args):
+    """Bottleneck, Ref-NeRF stage or direction encoding, GLO, view MLP and rgb head."""
+    plan = mlp.plan
+    cfg = plan.cfg
+    B, S = st.B, st.S
     bt = plan.one('bottleneck')
-    ops.gemm(L.GEMM_FWD, x, mlp.w_nk[bt.name], st.vin[:, :bt.out_dim], m=M, n=bt.out_dim,
+    ops.gemm(L.GEMM_FWD, st.x_last, mlp.w_nk[bt.name], st.vin[:, :bt.out_dim], m=st.M, n=bt.out_dim,
              k=bt.in_pad, act=L.ACT_NONE, bias=mlp.b(bt), impl=impl)
-    if cfg.bottleneck_noise > 0 and getattr(st, 'bneck_noise', None) is not None:
+    if st.bneck_noise is not None:
       # models.py:529-533 (regulariser, unused by the shipped configs): plain elementwise add
       st.vin[:, :bt.out_dim].add_((cfg.bottleneck_noise * st.bneck_noise).to(torch.bfloat16))
     if plan.ref_stage:
-      desc = self._refdir_desc(st, plan)
-      desc.ld = st.vin.stride(0)
-      mat, ml, _ = mlp.ide_tables() if cfg.use_directional_enc else (None, None, 0)
-      ops.refdir_fwd(desc, mat, ml, st.heads.get('grad_pred'), st.heads.get('roughness'),
-                     st.rgd if plan.density_normals else None, rays.viewdirs, st.normals_pred, st.normals,
-                     st.roughness, st.vin, om, pm, on_pred, extra_dw)
+      ops.refdir_fwd(*self._refdir_args(st, mlp, rays), st.normals_pred, st.normals, st.roughness, st.vin,
+                     *normals_args)
     else:
       ops.viewdir_enc(rays.viewdirs, S, cfg.deg_view, st.vin, bt.out_dim, plan.vin_pad)
     if plan.glo_features > 0:
-      # GLO vector of the ray's camera, broadcast over the samples (models.py:565-569)
+      # GLO vector of the ray's camera, broadcast over the samples (models.py:565-569).  Written after the Ref-NeRF
+      # stage: its slab zero-fill would also clear the GLO columns.
       g0 = plan.glo_col0
       st.vin.view(B, S, st.vin.stride(0))[:, :, g0:g0 + plan.glo_features] = \
           (st.glo_vec if st.glo_vec is not None else torch.zeros(B, plan.glo_features, device=st.vin.device)
@@ -654,17 +689,16 @@ class Model:
     v = st.vin
     for i, sp in enumerate(plan.by_role('view')):
       Wv = sp.out_dim
-      ops.gemm(L.GEMM_FWD, v, mlp.w_nk[sp.name], st.vacts[i][:, :Wv], m=M, n=Wv, k=sp.in_pad,
+      ops.gemm(L.GEMM_FWD, v, mlp.w_nk[sp.name], st.vacts[i][:, :Wv], m=st.M, n=Wv, k=sp.in_pad,
                act=L.ACT_RELU, bias=mlp.b(sp), maskbits=st.vbits[i], impl=impl)
       v = st.vacts[i]
     st.v_last = v
     r = plan.one('rgb')
-    ops.head_fwd(v, mlp.w_nk[r.name], mlp.b(r), r.out_dim, r.in_pad, raw=st.raw_rgb.view(M, 3))
+    ops.head_fwd(v, mlp.w_nk[r.name], mlp.b(r), r.out_dim, r.in_pad, raw=st.raw_rgb.view(st.M, 3))
 
   # ------------------------------------------------------------------ layer-chained 256-wide trunks
   def _use_chain(self, plan, M, impl=0):
     """One persistent launch per trunk (csrc/chain.cu) when every trunk layer is 256 wide."""
-    import os
     if impl != 0 or os.environ.get('MNRF_CHAIN', '1') == '0':
       return False
     cfg = plan.cfg
@@ -673,14 +707,14 @@ class Model:
 
   def _chain_fwd_desc(self, st, mlp):
     key = ('fwd', st.keep_acts)
-    cache = st.__dict__.setdefault('_chain', {})
-    if key in cache:
-      return cache[key]
+    if key in st.chain:
+      return st.chain[key]
     plan = mlp.plan
     W = plan.cfg.net_width
-    M = st.B * st.S
     nf = plan.Fpad // 64
     trunk = plan.by_role('trunk')
+    # the trunk output is read outside the chain: by the view branch, by heads after a skip, by the narrow heads
+    out_read = plan.top == 'view' or plan.last_has_feat or bool(plan.narrow)
     layers = []
     for i, sp in enumerate(trunk):
       ly = dict(w=mlp.w_nk[sp.name], bias=mlp.b(sp))
@@ -690,44 +724,33 @@ class Model:
         ly.update(n_res=W // 64, res_kb0=0)
         if sp.in_pad == W + plan.Fpad:          # skip layer: [hidden | features] against [W | Fpad] weight columns
           ly.update(n_stream=nf, stream_col0=0, stream_kb0=W // 64)
-      last = i == len(trunk) - 1
-      if st.keep_acts or (last and ((plan.has_rgb and not plan.rgb_on_trunk) or plan.last_has_feat or
-                                    plan.pred_normals)):
+      if st.keep_acts or (i == len(trunk) - 1 and out_read):
         ly['out'] = st.acts[i][:, :W]
       if st.keep_acts:
         ly['maskbits'] = st.bits[i]
       layers.append(ly)
     head = {}
     if not plan.last_has_feat:
-      dsp = plan.one('density')
-      if plan.rgb_on_trunk:
-        head = dict(head_w=mlp.colv_head, head_b=mlp.b(dsp), head_out=st.raw4, head_n=4)
-      else:
-        head = dict(head_w=mlp.colv_density, head_b=mlp.b(dsp), head_out=st.raw_density.view(M))
-    cache[key] = ops.chain_desc(L.CHAIN_FWD, M, layers, stream=st.feat, stream_cols=plan.Fpad, **head)
-    return cache[key]
+      head = dict(head_w=mlp.colv_head, head_b=mlp.b(plan.one('density')), head_out=st.raw_head, head_n=plan.head_n)
+    st.chain[key] = ops.chain_desc(L.CHAIN_FWD, st.M, layers, stream=st.feat, stream_cols=plan.Fpad, **head)
+    return st.chain[key]
 
   def _chain_bwd_desc(self, st, mlp, dyl):
     """dyl[i] = gradient w.r.t. the (pre-activation-masked) output of trunk layer i; dyl[-1] is the input."""
-    cache = st.__dict__.setdefault('_chain', {})
-    if 'bwd' in cache:
-      return cache['bwd']
-    plan = mlp.plan
-    W = plan.cfg.net_width
-    M = st.B * st.S
-    trunk = plan.by_role('trunk')
-    g = mlp.grads
+    if 'bwd' in st.chain:
+      return st.chain['bwd']
+    W = mlp.plan.cfg.net_width
+    trunk = mlp.plan.by_role('trunk')
     layers = []
     for j, i in enumerate(range(len(trunk) - 1, 0, -1)):
-      sp = trunk[i]
-      ly = dict(w=mlp.w_kn[sp.name], maskbits=st.bits[i - 1], out=dyl[i - 1])
+      ly = dict(w=mlp.w_kn[trunk[i].name], maskbits=st.bits[i - 1], out=dyl[i - 1])
       if j == 0:
         ly.update(n_stream=W // 64, stream_col0=0, stream_kb0=0)
       else:
         ly.update(n_res=W // 64, res_kb0=0)
       layers.append(ly)
-    cache['bwd'] = ops.chain_desc(L.CHAIN_BWD, M, layers, stream=dyl[-1], stream_cols=W)
-    return cache['bwd']
+    st.chain['bwd'] = ops.chain_desc(L.CHAIN_BWD, st.M, layers, stream=dyl[-1], stream_cols=W)
+    return st.chain['bwd']
 
   def _prep_rays(self, rays):
     r = utils.to_device_flat(rays, self.device)
@@ -779,6 +802,12 @@ class Model:
       if len(self._init_hist) < 8 and not torch.cuda.is_current_stream_capturing():
         self._init_hist[ck] = init
     sdist_prev, w_prev = init
+
+    def draw(key, i, shape, sample):
+      # level i's draw: from an explicit dict of draws, or `sample` (torch.rand / randn) from the generator
+      if isinstance(rng, dict):
+        return rng[key][i].to(dev).reshape(shape).contiguous()
+      return sample(shape, device=dev, generator=rng)
     states = []
     for i, lv in enumerate(sched):
       mname = 'NerfMLP_0' if (m.single_mlp or not lv['is_prop']) else 'PropMLP_0'
@@ -790,12 +819,7 @@ class Model:
       st.keep_acts = loss_config is not None or mlp.plan.density_normals
       jit = None
       if rng is not None:
-        if isinstance(rng, dict):
-          jit = rng['jitter'][i].to(dev).contiguous()
-          jit = jit.reshape(B) if m.single_jitter else jit.reshape(B, lv['S'])
-        else:
-          shape = (B,) if m.single_jitter else (B, lv['S'])
-          jit = torch.rand(shape, device=dev, generator=rng)
+        jit = draw('jitter', i, (B,) if m.single_jitter else (B, lv['S']), torch.rand)
       u_base, max_jitter = self._u(lv['S'], jit is not None)
       ops.sample_level(sdist_prev, w_prev, lv['S'], dilation=lv['dilation'],
                        use_dilation=lv['use_dilation'], domain=(s_near, s_far), anneal=lv['anneal'],
@@ -805,15 +829,11 @@ class Model:
       if m.num_glo_features > 0 and not lv['is_prop'] and not zero_glo:
         st.glo_vec = self.params.seg('Embed_0').view(m.num_glo_embeddings, -1)[rays.cam_idx[:, 0].long()]
       st.bneck_noise = None
-      if mlp.plan.cfg.bottleneck_noise > 0 and rng is not None and mlp.plan.one('bottleneck') is not None:
-        bwid = mlp.plan.cfg.bottleneck_width
-        if isinstance(rng, dict):
-          st.bneck_noise = rng['bottleneck_noise'][i].to(dev).reshape(B * lv['S'], bwid)
-        else:
-          st.bneck_noise = torch.randn(B * lv['S'], bwid, device=dev, generator=rng)
+      if mlp.plan.cfg.bottleneck_noise > 0 and rng is not None and mlp.plan.top == 'view':
+        st.bneck_noise = draw('bottleneck_noise', i, (B * lv['S'], mlp.plan.cfg.bottleneck_width), torch.randn)
       # levels of an MLP without normals skip the normal losses (the reference raises there instead)
       st.loss_mults = self.level_loss_mults(loss_config, i, B) if (
-          loss_config is not None and (mlp.plan.ref_stage or mlp.plan.normals_stage)) else None
+          loss_config is not None and mlp.plan.has_normals_stage) else None
       if st.loss_mults is not None:
         om, pm, on_pred = st.loss_mults
         if (om > 0 and ((on_pred and not mlp.plan.pred_normals) or (not on_pred and not mlp.plan.density_normals))):
@@ -824,10 +844,7 @@ class Model:
       self._mlp_forward(st, mlp, rays, impl=impl, loss_mults=st.loss_mults)
       st.noise = None
       if mlp.plan.cfg.density_noise > 0 and rng is not None:
-        if isinstance(rng, dict):
-          st.noise = rng['density_noise'][i].to(dev).reshape(B, lv['S']).contiguous()
-        else:
-          st.noise = torch.randn(B, lv['S'], device=dev, generator=rng)
+        st.noise = draw('density_noise', i, (B, lv['S']), torch.randn)
       st.comp_cfg = self._comp_cfg(mlp.plan.cfg)
       # background colour (models.py:240-254): constant, midpoint (rng=None) or per-ray uniform draws
       lo, hi = m.bg_intensity_range
@@ -836,11 +853,7 @@ class Model:
         if rng is None:
           st.comp_cfg['bg_const'] = (lo + hi) / 2
         else:
-          if isinstance(rng, dict):
-            ub = rng['bg'][i].to(dev).reshape(B, 3)
-          else:
-            ub = torch.rand(B, 3, device=dev, generator=rng)
-          st.bg_rgb = (lo + (hi - lo) * ub).contiguous()
+          st.bg_rgb = (lo + (hi - lo) * draw('bg', i, (B, 3), torch.rand)).contiguous()
       st.comp = ops.composite_fwd(st.raw_density, st.raw_rgb, st.sdist, rays.directions,
                                   rays.near_flat, rays.far_flat, cfg=st.comp_cfg,
                                   density_noise=st.noise, bg_rgb=st.bg_rgb,
@@ -904,15 +917,6 @@ class Model:
     return self(rng, rays, train_frac, compute_extras, zero_glo)
 
   # ------------------------------------------------------------------ backward
-  def _narrow_heads_bwd(self, st: LevelState, mlp: MLPDevice):
-    """Parameter gradients of the narrow heads (x^T d_raw), accumulated into mlp.grads."""
-    g = mlp.grads
-    for role in ('grad_pred', 'diffuse', 'tint', 'roughness'):
-      sp = mlp.plan.one(role)
-      if sp is not None:
-        ops.head_bwd(st.x_last, mlp.w_nk[sp.name], st.d_heads[role], sp.out_dim, sp.in_pad, dx=None,
-                     dw=mlp.W(sp, g), db=mlp.b(sp, g))
-
   def _mlp_backward(self, st: LevelState, mlp: MLPDevice, rays=None, impl=0, loss_mults=None, stats=None):
     """Accumulates parameter gradients of one level into mlp.grads (fp32).
 
@@ -923,171 +927,165 @@ class Model:
     separate pass over the activation.
     """
     plan = mlp.plan
-    cfg = plan.cfg
-    M = st.B * st.S
-    W = cfg.net_width
-    dev = self.device
-    bf = torch.bfloat16
+    trunk = plan.by_role('trunk')
+    # the trunk's input-gradient chain runs as one launch; its bias gradients then come from its weight-gradient
+    # GEMMs, so the top of the trunk does not sum the last layer's
+    chained = self._use_chain(plan, st.M, impl) and len(trunk) > 1
     if st.bwd is None:
-      bw_ = LevelState()
-      # per-layer gradient buffers when the dgrad chain runs as one launch (its wgrads come after)
-      n_dy = cfg.net_depth if self._use_chain(plan, M, impl) else 2
-      bw_.dy = [torch.empty(M, W, device=dev, dtype=bf) for _ in range(n_dy)]
-      if plan.has_rgb and not plan.rgb_on_trunk:
-        Wv = cfg.net_width_viewdirs
-        bw_.dv = [torch.empty(M, Wv, device=dev, dtype=bf) for _ in range(2)]
-        bw_.d_vin = torch.empty(M, plan.vin_pad, device=dev, dtype=bf)
-        bw_.d_vin_skip = torch.empty(M, plan.vin_pad, device=dev, dtype=bf) if plan.view_concat_after else None
-      # zero-filled once: the normals backward writes only its first four columns
-      bw_.dhead = torch.zeros(M, plan.normals_head_cols, device=dev, dtype=bf) if plan.normals_head_cols else None
-      if plan.density_normals:
-        bw_.h = [torch.empty(3 * M, W, device=dev, dtype=bf) for _ in range(2)]
-      st.bwd = bw_
-    sc = st.bwd
+      st.bwd = BwdScratch(plan, st.M, chained, self.device)
+    colsum = None if chained else mlp.b(trunk[-1], mlp.grads)
+    lm = _loss_args(loss_mults)
+    if plan.top == 'view':
+      self._view_bwd(st, mlp, rays, impl, lm, stats, colsum)
+    else:
+      self._heads_bwd(st, mlp, rays, impl, lm, stats, colsum)
+    if plan.density_normals:
+      self._tangent_bwd(st, mlp, impl)
+    self._trunk_bwd(st, mlp, impl, chained)
+
+  def _slab_dgrad(self, st, mlp, slab, colsum, impl):
+    """d x_last = relu'(x_last) * (slab @ wcat_kn^T): one dgrad over the head-gradient slab, with the bias gradient
+    of the last trunk layer (`colsum`) from the same epilogue."""
+    ops.gemm(L.GEMM_DGRAD, slab, mlp.wcat_kn, st.bwd.dy[0], m=st.M, n=mlp.plan.cfg.net_width,
+             k=mlp.plan.slab_cols, maskbits=st.bits[-1], colsum=colsum, impl=impl)
+
+  def _heads_bwd(self, st, mlp, rays, impl, lm, stats, colsum):
+    """Top of a trunk without a view branch: colourless normals stage, density (or stacked) and narrow heads."""
+    plan = mlp.plan
+    sc, g = st.bwd, mlp.grads
+    d = plan.one('density')
+    if plan.normals_stage:
+      ops.normals_bwd(st.M, st.S, st.heads.get('grad_pred'), st.rgd, rays.viewdirs, st.comp['weights'], *lm,
+                      st.d_raw_density, st.d_heads.get('grad_pred'), st.d_rgd, head_grads=sc.dhead, stats=stats,
+                      d_raw_rgb=st.d_raw_rgb if sc.dhead is not None else None)
+    # the stacked head splits its weight gradient between the two heads' master matrices
+    split = dict(dw2=mlp.W(plan.one('rgb'), g), dw_split=1) if plan.top == 'stacked' else {}
+    if plan.slab_cols:
+      # d x_last against [w_density | W_grad_pred (| W_rgb)]; the heads' weight and bias gradients follow
+      self._slab_dgrad(st, mlp, sc.dhead, colsum, impl)
+      ops.head_bwd(st.x_last, mlp.w_head, st.d_raw_head, plan.head_n, d.in_pad, dx=None, dw=mlp.W(d, g),
+                   db=mlp.b(d, g), **split)
+      self._narrow_heads_bwd(st, mlp)
+    else:
+      # input gradient, weight gradients and bias gradients ([b_density | b_rgb]) in one pass.  Features after a
+      # skip are constants: dy holds the hidden columns only
+      ops.head_bwd(st.x_last, mlp.w_head, st.d_raw_head, plan.head_n, d.in_pad, dx=sc.dy[0], relu_mask=True,
+                   dw=mlp.W(d, g), db=mlp.b(d, g), dxsum=colsum, dx_cols=plan.cfg.net_width, **split)
+
+  def _narrow_heads_bwd(self, st: LevelState, mlp: MLPDevice):
+    """Parameter gradients of the narrow heads (x^T d_raw), accumulated into mlp.grads."""
     g = mlp.grads
-    # bias gradients of the trunk come from its weight-gradient GEMMs when its dgrad chain is one launch
-    side = self._use_chain(plan, M, impl) and len(plan.by_role('trunk')) > 1
+    for sp in mlp.plan.narrow:
+      ops.head_bwd(st.x_last, mlp.w_nk[sp.name], st.d_heads[sp.role], sp.out_dim, sp.in_pad, dx=None,
+                   dw=mlp.W(sp, g), db=mlp.b(sp, g))
+
+  def _view_mlp_bwd(self, st, mlp, impl):
+    """rgb head and view MLP backward; returns the gradient of the first view layer's output and the skip layer's
+    contribution to d vin (None without a skip)."""
+    plan = mlp.plan
+    sc, g = st.bwd, mlp.grads
+    views, r = plan.by_role('view'), plan.one('rgb')
+    Wv = plan.cfg.net_width_viewdirs
+    dcur = sc.dv[0]
+    ops.head_bwd(st.v_last, mlp.w_nk[r.name], st.d_raw_rgb.view(st.M, 3), r.out_dim, r.in_pad, dx=dcur,
+                 relu_mask=True, dw=mlp.W(r, g), db=mlp.b(r, g), dxsum=mlp.b(views[-1], g))
+    skip = None
+    for i in range(len(views) - 1, -1, -1):
+      sp = views[i]
+      xin = st.vin if i == 0 else st.vacts[i - 1]
+      ops.gemm(L.GEMM_WGRAD, xin, dcur, mlp.W(sp, g), m=sp.in_pad, n=Wv, k=st.M, impl=impl)
+      if i > 0:
+        if (i - 1) in plan.view_concat_after:
+          # this layer also consumed vin (skip concat): its second gradient contribution
+          ops.gemm(L.GEMM_DGRAD, dcur, mlp.w_kn[sp.name][Wv:], sc.d_vin_skip, m=st.M, n=plan.vin_pad, k=Wv,
+                   impl=impl)
+          skip = sc.d_vin_skip
+        nxt = sc.dv[1] if dcur is sc.dv[0] else sc.dv[0]
+        ops.gemm(L.GEMM_DGRAD, dcur, mlp.w_kn[sp.name], nxt, m=st.M, n=Wv, k=Wv,
+                 maskbits=st.vbits[i - 1], colsum=mlp.b(views[i - 1], g), impl=impl)
+        dcur = nxt
+    return dcur, skip
+
+  def _view_bwd(self, st, mlp, rays, impl, lm, stats, colsum):
+    """Top of a trunk with a view branch: view MLP, GLO, Ref-NeRF stage or direction encoding, bottleneck."""
+    plan = mlp.plan
+    sc, g = st.bwd, mlp.grads
+    bt, d = plan.one('bottleneck'), plan.one('density')
+    bw = bt.out_dim
+    dcur, skip = self._view_mlp_bwd(st, mlp, impl)
+    # d vin = dcur * Wv0^T: [ d bottleneck (| d direction encoding | d n.v) (| d GLO) ] (no activation on vin)
+    n = plan.d_vin_cols
+    ops.gemm(L.GEMM_DGRAD, dcur, mlp.w_kn[plan.by_role('view')[0].name], sc.d_vin[:, :n], m=st.M, n=n,
+             k=plan.cfg.net_width_viewdirs, addend=skip[:, :n] if skip is not None else None, impl=impl)
+    if st.glo_vec is not None:
+      # the GLO columns of vin, summed over the samples; read before the Ref-NeRF stage re-uses the slab columns
+      g0 = plan.glo_col0
+      d_glo = sc.d_vin.view(st.B, st.S, plan.vin_pad)[:, :, g0:g0 + plan.glo_features].float().sum(1)
+      self.params.seg('Embed_0', self.params.grads).view(self.mcfg.num_glo_embeddings, -1).index_add_(
+          0, rays.cam_idx[:, 0].long(), d_glo)
+    if plan.ref_stage:
+      ops.refdir_bwd(*self._refdir_args(st, mlp, rays), st.comp['weights'], sc.d_vin, *lm, st.d_raw_density,
+                     st.d_heads.get('diffuse'), st.d_heads.get('tint'), st.d_heads.get('grad_pred'),
+                     st.d_heads['roughness'].view(st.M) if 'roughness' in st.d_heads else None, st.d_rgd, stats)
+      self._narrow_heads_bwd(st, mlp)
+    # bottleneck dW + db, and the Dense(1) density head's dW from the same x_last tiles (models.py:460,527)
+    ops.gemm_wgrad(st.x_last, sc.d_vin[:, :bw], mlp.W(bt, g), m=bt.in_pad, n=bw, k=st.M, bsum=mlp.b(bt, g),
+                   side_w=st.d_raw_density.view(st.M), side_aw=mlp.W(d, g).view(-1), impl=impl)
+    if plan.ref_stage:
+      # d x_last = relu'(x_last) * ([d bottleneck | head gradients] @ [W_b | w_heads]^T)
+      self._slab_dgrad(st, mlp, sc.d_vin, colsum, impl)
+    else:
+      # d x_last = (dbott * Wb^T + d_raw_density (x) w_density) * relu'(x_last)
+      ops.gemm(L.GEMM_DGRAD, sc.d_vin[:, :bw], mlp.w_kn[bt.name], sc.dy[0], m=st.M, n=plan.cfg.net_width, k=bw,
+               rowv=st.d_raw_density.view(st.M), colv=mlp.colv_density, maskbits=st.bits[-1], colsum=colsum,
+               impl=impl)
+    # bias gradient of the density head: a plain sum of d_raw_density
+    mlp.b(d, g).add_(st.d_raw_density.sum())
+
+  def _tangent_bwd(self, st, mlp, impl):
+    """Adjoint of the tangent chain: H_last = relu'(x_last) * (d_rgd (x) w_density), three streams."""
+    plan = mlp.plan
+    sc, g = st.bwd, mlp.grads
+    W = plan.cfg.net_width
     d = plan.one('density')
     trunk = plan.by_role('trunk')
-    x_last = st.x_last
-    dy = sc.dy[0]
-    d_raw_density = st.d_raw_density.view(M, 1)
-    om, pm, on_pred = _loss_args(loss_mults)
-    r = plan.one('rgb')
-    if plan.has_rgb and not plan.rgb_on_trunk:
-      views = plan.by_role('view')
-      Wv = cfg.net_width_viewdirs
-      bt = plan.one('bottleneck')
-      bw = bt.out_dim
-      dcur = sc.dv[0]
-      ops.head_bwd(st.v_last, mlp.w_nk[r.name], st.d_raw_rgb.view(M, 3), r.out_dim, r.in_pad, dx=dcur,
-                   relu_mask=True, dw=mlp.W(r, g), db=mlp.b(r, g), dxsum=mlp.b(views[-1], g))
-      have_skip_grad = False
-      for i in range(len(views) - 1, -1, -1):
-        sp = views[i]
-        xin = st.vin if i == 0 else st.vacts[i - 1]
-        ops.gemm(L.GEMM_WGRAD, xin, dcur, mlp.W(sp, g), m=sp.in_pad, n=Wv, k=M, impl=impl)
-        if i > 0:
-          if (i - 1) in plan.view_concat_after:
-            # this layer also consumed vin (skip concat): its second gradient contribution
-            ops.gemm(L.GEMM_DGRAD, dcur, mlp.w_kn[sp.name][Wv:], sc.d_vin_skip, m=M, n=plan.vin_pad, k=Wv,
-                     impl=impl)
-            have_skip_grad = True
-          nxt = sc.dv[1] if dcur is sc.dv[0] else sc.dv[0]
-          ops.gemm(L.GEMM_DGRAD, dcur, mlp.w_kn[sp.name], nxt, m=M, n=Wv, k=Wv,
-                   maskbits=st.vbits[i - 1], colsum=mlp.b(views[i - 1], g), impl=impl)
-          dcur = nxt
-      s0 = views[0]
-      if plan.ref_stage:
-        # full d vin: [ d bottleneck | d direction encoding (| d n.v) ]
-        ops.gemm(L.GEMM_DGRAD, dcur, mlp.w_kn[s0.name], sc.d_vin, m=M, n=plan.vin_pad, k=Wv,
-                 addend=sc.d_vin_skip if have_skip_grad else None, impl=impl)
-        d_glo_ref = None
-        if plan.glo_features > 0 and st.glo_vec is not None:     # before the slab columns are re-used
-          g0 = plan.glo_col0
-          d_glo_ref = sc.d_vin.view(st.B, st.S, plan.vin_pad)[:, :, g0:g0 + plan.glo_features].float().sum(1)
-        desc = self._refdir_desc(st, plan)
-        desc.ld = st.vin.stride(0)
-        mat, ml, _ = mlp.ide_tables() if cfg.use_directional_enc else (None, None, 0)
-        ops.refdir_bwd(desc, mat, ml, st.heads.get('grad_pred'), st.heads.get('roughness'),
-                       st.rgd if plan.density_normals else None, rays.viewdirs, st.comp['weights'], sc.d_vin,
-                       om, pm, on_pred, st.d_raw_density, st.d_heads.get('diffuse'), st.d_heads.get('tint'),
-                       st.d_heads.get('grad_pred'), st.d_heads.get('roughness').view(M) if 'roughness' in st.d_heads else None,
-                       st.d_rgd if plan.density_normals else None, stats)
-        self._narrow_heads_bwd(st, mlp)
-        # bottleneck dW + db, and the Dense(1) density head's dW from the same x_last tiles
-        ops.gemm_wgrad(x_last, sc.d_vin[:, :bw], mlp.W(bt, g), m=bt.in_pad, n=bw, k=M, bsum=mlp.b(bt, g),
-                       side_w=st.d_raw_density.view(M), side_aw=mlp.W(d, g).view(-1), impl=impl)
-        # d x_last = relu'(x_last) * ([d bottleneck | head gradients] @ [W_b | w_heads]^T)
-        ops.gemm(L.GEMM_DGRAD, sc.d_vin, mlp.wcat_kn, dy, m=M, n=W, k=plan.vin_pad,
-                 maskbits=st.bits[-1], colsum=None if side else mlp.b(trunk[-1], g), impl=impl)
-      else:
-        dbott = sc.d_vin[:, :bw]
-        # d vin[:, :bw] = dcur * Wv0[:bw, :]^T  (no activation on the bottleneck)
-        if plan.glo_features > 0:
-          # the GLO columns of vin carry gradient too: full-width dgrad, then sum over the samples
-          ops.gemm(L.GEMM_DGRAD, dcur, mlp.w_kn[s0.name], sc.d_vin, m=M, n=plan.vin_pad, k=Wv,
-                   addend=sc.d_vin_skip if have_skip_grad else None, impl=impl)
-        else:
-          ops.gemm(L.GEMM_DGRAD, dcur, mlp.w_kn[s0.name], dbott, m=M, n=bw, k=Wv,
-                   addend=sc.d_vin_skip[:, :bw] if have_skip_grad else None, impl=impl)
-        # bottleneck dW + db, and the Dense(1) density head's dW from the same x_last tiles (models.py:460,527)
-        ops.gemm_wgrad(x_last, dbott, mlp.W(bt, g), m=bt.in_pad, n=bw, k=M, bsum=mlp.b(bt, g),
-                       side_w=st.d_raw_density.view(M), side_aw=mlp.W(d, g).view(-1), impl=impl)
-        # d x_last = (dbott * Wb^T + d_raw_density (x) w_density) * relu'(x_last)
-        ops.gemm(L.GEMM_DGRAD, dbott, mlp.w_kn[bt.name], dy, m=M, n=W, k=bw,
-                 rowv=st.d_raw_density.view(M), colv=mlp.colv_density, maskbits=st.bits[-1],
-                 colsum=None if side else mlp.b(trunk[-1], g), impl=impl)
-      # bias gradient of the density head: a plain sum of d_raw_density
-      mlp.b(d, g).add_(st.d_raw_density.sum())
-      if plan.glo_features > 0 and st.glo_vec is not None:
-        g0 = plan.glo_col0
-        d_glo = d_glo_ref if plan.ref_stage else \
-            sc.d_vin.view(st.B, st.S, plan.vin_pad)[:, :, g0:g0 + plan.glo_features].float().sum(1)
-        self.params.seg('Embed_0', self.params.grads).view(self.mcfg.num_glo_embeddings, -1).index_add_(
-            0, rays.cam_idx[:, 0].long(), d_glo)
-    else:
-      if plan.normals_stage:
-        ops.normals_bwd(M, st.S, st.heads.get('grad_pred'), st.rgd if plan.density_normals else None,
-                        rays.viewdirs, st.comp['weights'], om, pm, on_pred, st.d_raw_density,
-                        st.d_heads.get('grad_pred'), st.d_rgd if plan.density_normals else None,
-                        head_grads=sc.dhead, stats=stats,
-                        d_raw_rgb=st.d_raw_rgb if (plan.rgb_on_trunk and sc.dhead is not None) else None)
-      if plan.normals_head_cols:
-        # d x_last = relu'(x_last) * ([d raw_density | d grad_pred (| d raw_rgb)] @ [w_density | W_grad_pred
-        # (| W_rgb)]^T), with the bias gradient of the last trunk layer from the same epilogue
-        ops.gemm(L.GEMM_DGRAD, sc.dhead, mlp.wcat_kn, dy, m=M, n=W, k=plan.normals_head_cols,
-                 maskbits=st.bits[-1], colsum=None if side else mlp.b(trunk[-1], g), impl=impl)
-        if plan.rgb_on_trunk:
-          ops.head_bwd(x_last, mlp.w_head, st.d_raw4, 4, d.in_pad, dx=None, dw=mlp.W(d, g), dw2=mlp.W(r, g),
-                       dw_split=1, db=mlp.b(d, g))
-        else:
-          ops.head_bwd(x_last, mlp.w_nk[d.name], d_raw_density, 1, d.in_pad, dx=None, dw=mlp.W(d, g),
-                       db=mlp.b(d, g))
-        self._narrow_heads_bwd(st, mlp)
-      elif plan.rgb_on_trunk:
-        # both heads' input gradient, weight gradients (split between the two master matrices) and bias gradients
-        # [b_density | b_rgb] in one pass
-        ops.head_bwd(x_last, mlp.w_head, st.d_raw4, 4, d.in_pad, dx=dy, relu_mask=True, dw=mlp.W(d, g),
-                     dw2=mlp.W(r, g), dw_split=1, db=mlp.b(d, g), dxsum=None if side else mlp.b(trunk[-1], g),
-                     dx_cols=W)       # features after a skip are constants: dy holds the hidden columns only
-      else:
-        ops.head_bwd(x_last, mlp.w_nk[d.name], d_raw_density, 1, d.in_pad, dx=dy, relu_mask=True,
-                     dw=mlp.W(d, g), db=mlp.b(d, g), dxsum=None if side else mlp.b(trunk[-1], g),
-                     dx_cols=W)       # a trunk ending on a skip layer: dy holds the hidden columns only
-    if plan.density_normals:
-      # adjoint of the tangent chain: H_last = relu'(x_last) * (d_rgd (x) w_density), three streams
-      hcur, hoth = sc.h[0], sc.h[1]
-      ops.outer_mask(st.d_rgd.view(3 * M), mlp.colv_density, st.bits[-1], hcur, rows=3 * M, n=W, mask_mod=M)
-      ops.head_bwd(st.t_last, mlp.w_nk[d.name], st.d_rgd.view(3 * M, 1), 1, d.in_pad, dx=None,
-                   dw=mlp.W(d, g), db=None)
-      for i in range(len(trunk) - 1, -1, -1):
-        sp = trunk[i]
-        tin = st.tfeat if i == 0 else st.tacts[i - 1]
-        ops.gemm(L.GEMM_WGRAD, tin, hcur, mlp.W(sp, g), m=sp.in_pad, n=W, k=3 * M, impl=impl)
-        if i > 0:
-          ops.gemm(L.GEMM_DGRAD, hcur, mlp.w_kn[sp.name], hoth, m=3 * M, n=W, k=W,
-                   maskbits=st.bits[i - 1], mask_mod=M, impl=impl)
-          hcur, hoth = hoth, hcur
-    if self._use_chain(plan, M, impl) and len(trunk) > 1:
-      # dyl[i] = d loss / d (output of trunk layer i); dyl[-1] was produced above (sc.dy[0])
-      nl = len(trunk)
-      dyl = [sc.dy[nl - 1 - i] for i in range(nl)]        # dyl[nl-1] is sc.dy[0]
-      ops.mlp_chain(self._chain_bwd_desc(st, mlp, dyl))
-      for i in range(nl - 1, -1, -1):
-        sp = trunk[i]
-        xin = st.feat if i == 0 else st.acts[i - 1]
-        ops.gemm_wgrad(xin, dyl[i], mlp.W(sp, g), m=sp.in_pad, n=W, k=M, bsum=mlp.b(sp, g), impl=impl)
-      return
-    cur, other = sc.dy[0], sc.dy[1]
+    hcur, hoth = sc.h[0], sc.h[1]
+    ops.outer_mask(st.d_rgd.view(3 * st.M), mlp.colv_density, st.bits[-1], hcur, rows=3 * st.M, n=W, mask_mod=st.M)
+    ops.head_bwd(st.t_last, mlp.w_nk[d.name], st.d_rgd.view(3 * st.M, 1), 1, d.in_pad, dx=None,
+                 dw=mlp.W(d, g), db=None)
     for i in range(len(trunk) - 1, -1, -1):
       sp = trunk[i]
+      tin = st.tfeat if i == 0 else st.tacts[i - 1]
+      ops.gemm(L.GEMM_WGRAD, tin, hcur, mlp.W(sp, g), m=sp.in_pad, n=W, k=3 * st.M, impl=impl)
+      if i > 0:
+        ops.gemm(L.GEMM_DGRAD, hcur, mlp.w_kn[sp.name], hoth, m=3 * st.M, n=W, k=W,
+                 maskbits=st.bits[i - 1], mask_mod=st.M, impl=impl)
+        hcur, hoth = hoth, hcur
+
+  def _trunk_bwd(self, st, mlp, impl, chained):
+    """Trunk backward from dy[0] = d loss / d (output of the last trunk layer)."""
+    sc, g = st.bwd, mlp.grads
+    W = mlp.plan.cfg.net_width
+    trunk = mlp.plan.by_role('trunk')
+    nl = len(trunk)
+    if chained:
+      # dyl[i] = d loss / d (output of trunk layer i); dyl[nl-1] is sc.dy[0], produced at the top of the trunk
+      dyl = [sc.dy[nl - 1 - i] for i in range(nl)]
+      ops.mlp_chain(self._chain_bwd_desc(st, mlp, dyl))
+      for i in range(nl - 1, -1, -1):
+        xin = st.feat if i == 0 else st.acts[i - 1]
+        ops.gemm_wgrad(xin, dyl[i], mlp.W(trunk[i], g), m=trunk[i].in_pad, n=W, k=st.M, bsum=mlp.b(trunk[i], g),
+                       impl=impl)
+      return
+    cur, other = sc.dy[0], sc.dy[1]
+    for i in range(nl - 1, -1, -1):
+      sp = trunk[i]
       xin = st.feat if i == 0 else st.acts[i - 1]
-      ops.gemm(L.GEMM_WGRAD, xin, cur, mlp.W(sp, g), m=sp.in_pad, n=W, k=M, impl=impl)
+      ops.gemm(L.GEMM_WGRAD, xin, cur, mlp.W(sp, g), m=sp.in_pad, n=W, k=st.M, impl=impl)
       if i > 0:
         # only the hidden part of the input carries gradient (features are constants:
         # stop_gradient(sdist), models.py:200-201)
-        ops.gemm(L.GEMM_DGRAD, cur, mlp.w_kn[sp.name], other, m=M, n=W, k=W,
+        ops.gemm(L.GEMM_DGRAD, cur, mlp.w_kn[sp.name], other, m=st.M, n=W, k=W,
                  maskbits=st.bits[i - 1], colsum=mlp.b(trunk[i - 1], g), impl=impl)
         cur, other = other, cur
 

@@ -273,7 +273,7 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
   def _d_scale_buf(st):
     if st.rgb_scale is None:
       return None
-    if getattr(st, 'd_rgb_scale', None) is None or st.d_rgb_scale.shape[0] != st.B:
+    if st.d_rgb_scale is None or st.d_rgb_scale.shape[0] != st.B:
       st.d_rgb_scale = torch.empty(st.B, 3, device=dev)
     return st.d_rgb_scale
 
