@@ -157,9 +157,10 @@ int mnrf_gemm(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, c
               const float* rowv, const float* colv, const mnrf_bf16* mask, uint32_t* maskbits,
               float* colsum, const mnrf_bf16* addend, void* out, mnrf_stream stream);
 
-/* Weight gradient with side sums computed from the operand tiles the main loop stages (the epilogue warps
- * are idle there), so the bias gradient and the gradient of a Dense(1) head on the same activation cost no
- * extra pass over HBM:
+/* Weight gradient with side sums computed from the operand tiles the main loop stages (by the three warps of
+ * the producer warpgroup that issue no loads), so the bias gradient and the gradient of a Dense(1) head on the
+ * same activation cost no extra pass over HBM; one launch (impl = 1, the SIMT reference, runs them as separate
+ * passes).  They do cost shared-memory bandwidth the MMAs use (DESIGN.md section 3):
  *   out[Mo,N] += A[R,Mo]^T B[R,N]                       (as mnrf_gemm, mode MNRF_GEMM_WGRAD; A = X, B = dY)
  *   bsum[N]   += sum_r B[r, :]                          (optional: bias gradient of the layer)
  *   side_aw[Mo] += sum_r side_w[r] * A[r, :]            (optional: dW of a Dense(1) head reading X, with

@@ -8,7 +8,8 @@ namespace mnrf {
 
 int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
                    const float* rowv, const float* colv, const mnrf_bf16* mask, uint32_t* maskbits,
-                   float* colsum, const mnrf_bf16* addend, void* out, cudaStream_t stream);
+                   float* colsum, const mnrf_bf16* addend, void* out, cudaStream_t stream, float* bsum,
+                   const float* side_w, float* side_aw);
 
 __device__ __forceinline__ float ldbf(const __nv_bfloat16* p) { return __bfloat162float(*p); }
 
@@ -88,7 +89,8 @@ extern "C" int mnrf_gemm(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf
   cudaStream_t s = (cudaStream_t)stream;
   if (colsum) MNRF_CHECK(d->mode == MNRF_GEMM_DGRAD, "mnrf_gemm: colsum is a DGRAD output");
   if (addend) MNRF_CHECK(d->mode == MNRF_GEMM_DGRAD, "mnrf_gemm: addend is a DGRAD input");
-  if (d->impl == 0) return gemm_tc_launch(d, a, b, bias, rowv, colv, mask, maskbits, colsum, addend, out, s);
+  if (d->impl == 0)
+    return gemm_tc_launch(d, a, b, bias, rowv, colv, mask, maskbits, colsum, addend, out, s, nullptr, nullptr, nullptr);
   dim3 block(16, 16);
   if (d->mode != MNRF_GEMM_WGRAD) {
     dim3 grid((d->n + 15) / 16, (unsigned)((d->m + 15) / 16));
@@ -125,8 +127,10 @@ extern "C" int mnrf_gemm_wgrad(const mnrf_gemm_desc* d, const mnrf_bf16* a, cons
   MNRF_CHECK(d && a && b && out, "mnrf_gemm_wgrad: null pointer");
   MNRF_CHECK(d->mode == MNRF_GEMM_WGRAD, "mnrf_gemm_wgrad: mode must be MNRF_GEMM_WGRAD");
   MNRF_CHECK((side_w == nullptr) == (side_aw == nullptr), "mnrf_gemm_wgrad: side_w and side_aw come together");
-  // the weight gradient (tensor-core or SIMT reference kernel), then the side sums as separate passes over the
-  // same operands
+  // tensor cores: one launch, the side sums taken from the operand tiles the main loop stages
+  if (d->impl == 0) return gemm_tc_launch(d, a, b, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, out,
+                                          (cudaStream_t)stream, bsum, side_w, side_aw);
+  // SIMT reference: the weight gradient, then the side sums as separate passes over the same operands
   if (int rc = mnrf_gemm(d, a, b, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, out, stream)) return rc;
   if (bsum)
     if (int rc = mnrf_colsum(d->k, d->n, b, d->ldb, bsum, stream)) return rc;

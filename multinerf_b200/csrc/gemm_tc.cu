@@ -4,7 +4,8 @@
 // jax.value_and_grad derives from them (train_utils.py:316-317).
 //
 //   warpgroup 0   : TMA producer (one thread) -- cp.async.bulk.tensor.2d into an operand ring of 128 x 64 A and
-//                   BN x 64 B k-blocks; gives its registers up (setmaxnreg) to
+//                   BN x 64 B k-blocks; WGRAD with side sums: warps 1-3 sum the staged tiles (bias gradient,
+//                   Dense(1) head gradient) while the consumers multiply them; gives its registers up (setmaxnreg) to
 //   warpgroups 1-2: consumers -- each issues wgmma m64nBNk16 for 64 of the tile's 128 rows, keeps the fp32
 //                   accumulators in registers and runs the epilogue from them: bias/ReLU/mask bits | rank-1 term,
 //                   mask, addend, column sums | fp32 vector reductions.
@@ -46,9 +47,13 @@ constexpr int mask_words(int bn) { return bn >= 128 ? bn / 32 : 0; }
 constexpr int MASK_BUFS = 2;         // mask blocks in flight: the producer loads tile t+1's during tile t's epilogue
 // DGRAD: per-consumer-warp column sums [8][BN] fp32, then MASK_BUFS mask blocks [128 rows][mask_words] uint32
 constexpr int dgrad_smem_bytes(int bn) { return 8 * bn * 4 + MASK_BUFS * BLOCK_M * mask_words(bn) * 4; }
-constexpr int smem_bytes(int mode, int bn, bool ts) {
+// WGRAD side sums: warps 1-3 of the producer warpgroup, 8 columns (one 16-byte chunk) per thread, whose partial sums
+// meet in an fp32 scratch of [96 threads][8] once per tile
+constexpr int SIDE_SCRATCH = 96 * 8;
+constexpr int smem_bytes(int mode, int bn, bool ts, bool side) {
   return gemm_stages(bn) * (A_STAGE_BYTES + bn * BLOCK_K * 2) + 2 * staging_blocks(mode, bn, ts) * STAGING_BLOCK_BYTES +
-         (mode == MNRF_GEMM_DGRAD ? dgrad_smem_bytes(bn) : 0) + 256 /*barriers*/ + 1024 /*align*/;
+         (mode == MNRF_GEMM_DGRAD ? dgrad_smem_bytes(bn) : 0) + (side ? SIDE_SCRATCH * 4 : 0) + 256 /*barriers*/ +
+         1024 /*align*/;
 }
 
 struct GemmParams {
@@ -69,12 +74,103 @@ struct GemmParams {
   int64_t ldadd;
   float* colsum;              // DGRAD: colsum[N] += column sums of the output (bias gradient of the
                               // layer that produced the masking activation)
+  float* bsum;                // WGRAD side sums (optional): bsum[N] += sum_r B[r, :]
+  const float* side_w;        //   and side_aw[Mo] += sum_r side_w[r] * A[r, :]
+  float* side_aw;
   void* out;
 };
 
+// WGRAD side sums of one operand, run by NT threads of the producer warpgroup (t = 0..NT-1) beside the consumers:
+//   B (WEIGHTED = false): out = bsum,    out[n_blk * BN + col]  += sum_r B[r, col]
+//   A (WEIGHTED = true):  out = side_aw, out[m_blk * 128 + col] += sum_r side_w[r] A[r, col]
+// Tile (m_blk, n_blk) sums, of every k-block it stages, the B rows r % num_m_blocks == m_blk and the A rows
+// r % num_n_blocks == n_blk: every row of every (n-block, k-block) B tile and (m-block, k-block) A tile is summed
+// once across the grid, and each stage costs the same few shared-memory reads.  (Summing whole k-blocks on every
+// num_m_blocks-th stage instead holds those stages for longer than the MMAs take: under the wgmma traffic a shared
+// load here takes a few hundred cycles.)  The threads wait on every stage as the consumers do and release it once
+// read (empty_bar counts their warps).  MN-major stage layout: atoms of [64 r x 64 mn], the 16-byte chunk c of row r
+// at chunk c ^ (r & 7).  Thread t owns the 8 columns of chunk t % CHUNKS, in fp32 registers (this warpgroup runs at 40
+// registers a thread), and flushes them once per tile through `scratch`: the row groups meet there and one reduction
+// per column leaves.  Rows past R are zero-filled by TMA; side_w is read as 0 there.
+template <int STAGES, int STAGE_BYTES, int CHUNKS, int NT, bool WEIGHTED>
+__device__ __forceinline__ void wgrad_side_sums(const GemmParams& p, int t, uint32_t ring, uint64_t* full_bar,
+                                                uint64_t* empty_bar, uint32_t scratch) {
+  constexpr int G = NT / CHUNKS;                     // row groups
+  constexpr int COLS = CHUNKS * 8;
+  static_assert(NT % CHUNKS == 0 && NT % 32 == 0, "side-sum warps tile the chunks");
+  const int lane = t & 31;
+  const int c = t % CHUNKS, g0 = t / CHUNKS;
+  // chunk c in row 0 of a stage: the ring is 1024-byte aligned, so the swizzle is an XOR on address bits 4-6
+  ring += (c >> 3) * (BLOCK_K * 128) + ((c & 7) << 4);
+  const int total_tiles = p.num_m_blocks * p.num_n_blocks * p.num_splits;
+  const int every = WEIGHTED ? p.num_n_blocks : p.num_m_blocks;
+  const int step = every * G;                        // row stride of a thread
+  uint32_t slot = 0;                                 // k-blocks consumed: stage slot % STAGES
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const int n_blk = tile % p.num_n_blocks;
+    const int rest = tile / p.num_n_blocks;
+    const int m_blk = rest % p.num_m_blocks;
+    const int split = rest / p.num_m_blocks;
+    const int kb0 = split * p.kblocks_per_split;
+    const int kb1 = min(p.num_k_blocks, kb0 + p.kblocks_per_split);
+    const int own = WEIGHTED ? n_blk : m_blk;        // first row of each k-block this tile sums
+    float acc[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[e] = 0.f;
+    for (int kb = kb0; kb < kb1; ++kb, ++slot) {
+      float wlo = 0.f, whi = 0.f;                    // A: side_w of the k-block's 64 rows, two per lane
+      if (WEIGHTED) {
+        const int r0 = kb * BLOCK_K + lane;
+        if (r0 < p.k) wlo = __ldg(p.side_w + r0);
+        if (r0 + 32 < p.k) whi = __ldg(p.side_w + r0 + 32);
+      }
+      mbar_wait(&full_bar[slot % STAGES], (slot / STAGES) & 1, 6);
+      const uint32_t base = ring + (slot % STAGES) * STAGE_BYTES;
+      // the same trip count on every lane (the weights come by shuffle); B one row at a time, A two: deeper
+      // unrolling spills
+#pragma unroll(WEIGHTED ? 2 : 1)
+      for (int r0 = own; r0 < BLOCK_K; r0 += step) {
+        const int r = r0 + every * g0;
+        float w = 1.f;                               // B: fma with 1 is the plain sum
+        if (WEIGHTED) {                              // (the source lane's value cannot depend on this lane's r)
+          const float wl = __shfl_sync(0xffffffffu, wlo, r & 31), wh = __shfl_sync(0xffffffffu, whi, r & 31);
+          w = r < 32 ? wl : wh;
+        }
+        if (r < BLOCK_K) {
+          const uint4 v = ld_shared_v4((base + r * 128) ^ ((r & 7) << 4));
+          const uint32_t u[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            acc[2 * q] = fmaf(w, bf16_lo(u[q]), acc[2 * q]);
+            acc[2 * q + 1] = fmaf(w, bf16_hi(u[q]), acc[2 * q + 1]);
+          }
+        }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[slot % STAGES]);
+    }
+    if (own < BLOCK_K && kb0 < kb1) {                // the same on all NT threads
+      // thread t's partials at t * 8: row group g of column col sits at g * COLS + col
+      if (NT > 32) named_bar_sync(4, NT); else __syncwarp();   // the previous flush has read the scratch
+#pragma unroll
+      for (int e = 0; e < 8; ++e) st_shared_u32(scratch + (t * 8 + e) * 4, __float_as_uint(acc[e]));
+      if (NT > 32) named_bar_sync(4, NT); else __syncwarp();
+      const int64_t col0 = WEIGHTED ? (int64_t)m_blk * BLOCK_M : (int64_t)n_blk * COLS;
+      float* out = WEIGHTED ? p.side_aw : p.bsum;
+      for (int col = t; col < COLS; col += NT) {
+        if (WEIGHTED && col0 + col >= p.m) break;    // columns past Mo are never written
+        float sum = 0.f;
+#pragma unroll
+        for (int g = 0; g < G; ++g) sum += __uint_as_float(ld_shared_u32(scratch + (g * COLS + col) * 4));
+        atomicAdd(out + col0 + col, sum);
+      }
+    }
+  }
+}
+
 // Accumulator fragment of wgmma m64nBN (per consumer thread): acc[4i + 2h + e] is row 16*warp + lane/4 + 8h,
 // column 8i + 2*(lane%4) + e of the warpgroup's 64 x BN tile.
-template <int MODE, int BN, bool TS>
+template <int MODE, int BN, bool TS, bool SIDE>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_m,
@@ -87,6 +183,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   constexpr int SB = staging_blocks(MODE, BN, TS);
   constexpr int MW = mask_words(BN);
   static_assert(SB < 2 || (BN / 64) % 2 == 0, "block j of every tile must use staging block j % SB");
+  static_assert(!SIDE || kWgrad, "side sums are a WGRAD feature");
   extern __shared__ uint8_t smem_dyn[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
@@ -95,7 +192,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   // DGRAD: column sums of the current n-block, one private [BN] slice per consumer warp, then the mask blocks
   // (offsets stay multiples of 128 bytes, as TMA destinations need)
   float* cs_s = reinterpret_cast<float*>(smem_c + 2 * SB * STAGING_BLOCK_BYTES);  // [8][BN]
-  uint32_t* mask_s = reinterpret_cast<uint32_t*>(cs_s + (kDgrad ? 8 * BN : 0));   // [MASK_BUFS][BLOCK_M][MW]
+  float* side_s = cs_s;                                                          // WGRAD: [SIDE_SCRATCH]
+  uint32_t* mask_s = reinterpret_cast<uint32_t*>(cs_s + (kDgrad ? 8 * BN : SIDE ? SIDE_SCRATCH : 0));  // [MASK_BUFS][BLOCK_M][MW]
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(mask_s + (kDgrad ? MASK_BUFS * BLOCK_M * MW : 0));  // [STAGES]
   uint64_t* empty_bar = full_bar + STAGES;                                       // [STAGES]
   uint64_t* mask_full = empty_bar + STAGES;                                      // [MASK_BUFS]
@@ -115,7 +213,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     if (mask_tma) prefetch_tmap(&tmap_m);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 8);     // one arrival per consumer warp
+      // one arrival per consumer warp and side-sum warp
+      mbar_init(&empty_bar[i], 8 + (!SIDE ? 0 : !p.side_aw ? 3 : p.bsum ? 3 : 2));
     }
     for (int i = 0; i < MASK_BUFS; ++i) {
       mbar_init(&mask_full[i], 1);
@@ -173,6 +272,20 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
+      }
+    } else if (SIDE && warp > 0) {
+      // ===================== WGRAD side sums =====================
+      // bsum alone: warps 1-3.  With side_aw, whose A rows of every k-block are all read when N is one tile wide
+      // (the bottleneck): warp 1 bsum, warps 2-3 side_aw.
+      const uint32_t scratch = smem_u32(side_s);
+      if (!p.side_aw) {
+        wgrad_side_sums<STAGES, B_STAGE, BN / 8, 96, false>(p, threadIdx.x - 32, smem_u32(smem_b), full_bar, empty_bar,
+                                                            scratch);
+      } else if (warp >= 2) {
+        wgrad_side_sums<STAGES, A_STAGE_BYTES, BLOCK_M / 8, 64, true>(p, threadIdx.x - 64, smem_u32(smem_a), full_bar,
+                                                                      empty_bar, scratch + 32 * 8 * 4);
+      } else if (p.bsum) {
+        wgrad_side_sums<STAGES, B_STAGE, BN / 8, 32, false>(p, lane, smem_u32(smem_b), full_bar, empty_bar, scratch);
       }
     }
   } else {
@@ -394,7 +507,8 @@ static int pick_block_n(int n) {
 
 int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
                    const float* rowv, const float* colv, const mnrf_bf16* mask, uint32_t* maskbits,
-                   float* colsum, const mnrf_bf16* addend, void* out, cudaStream_t stream) {
+                   float* colsum, const mnrf_bf16* addend, void* out, cudaStream_t stream, float* bsum,
+                   const float* side_w, float* side_aw) {
   // K-major modes: the reduction index is the contiguous one and layers are padded to 64.  WGRAD reduces
   // over the sample rows, any count: the last 64-row block is zero-filled by TMA past the tensor's end.
   MNRF_CHECK(d->mode == MNRF_GEMM_WGRAD || d->k % BLOCK_K == 0,
@@ -424,6 +538,10 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
   p.colsum = colsum;
   if (colsum) MNRF_CHECK(d->mode == MNRF_GEMM_DGRAD && d->n <= CS_MAX,
                          "mnrf_gemm(tc): colsum is a DGRAD output of at most %d columns", CS_MAX);
+  const bool side = bsum != nullptr || side_aw != nullptr;
+  if (side) MNRF_CHECK(d->mode == MNRF_GEMM_WGRAD && (side_w == nullptr) == (side_aw == nullptr),
+                       "mnrf_gemm(tc): side sums are WGRAD outputs; side_w and side_aw come together");
+  p.bsum = bsum; p.side_w = side_w; p.side_aw = side_aw;
   if (maskbits) {
     MNRF_CHECK(d->mode != MNRF_GEMM_WGRAD, "mnrf_gemm(tc): maskbits make no sense for WGRAD");
     MNRF_CHECK(d->n % 32 == 0 && block_n % 32 == 0 && d->ldmaskbits * 32 >= d->n,
@@ -487,12 +605,12 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
   const int total_tiles = p.num_m_blocks * p.num_n_blocks * p.num_splits;
   const int grid = std::min(total_tiles, workers);
   if (grid == 0) return 0;
-#define MNRF_LAUNCH_TC3(MODE_, BN_, TS_)                                                              \
+#define MNRF_LAUNCH_TC3(MODE_, BN_, TS_, SIDE_)                                                       \
   do {                                                                                                \
     static bool attr_set = false;                                                                     \
-    constexpr int kSmem = smem_bytes(MODE_, BN_, TS_);                                                \
+    constexpr int kSmem = smem_bytes(MODE_, BN_, TS_, SIDE_);                                         \
     static_assert(kSmem <= 232448, "shared memory budget");                                           \
-    auto kern = gemm_tc_kernel<MODE_, BN_, TS_>;                                                      \
+    auto kern = gemm_tc_kernel<MODE_, BN_, TS_, SIDE_>;                                               \
     if (!attr_set) {                                                                                  \
       MNRF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));      \
       attr_set = true;                                                                                \
@@ -508,8 +626,9 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
   } while (0)
 #define MNRF_LAUNCH_TC2(MODE_, BN_)                                                                   \
   do {                                                                                                \
-    if (ts) MNRF_LAUNCH_TC3(MODE_, BN_, MODE_ != MNRF_GEMM_WGRAD && BN_ >= 64);                       \
-    else MNRF_LAUNCH_TC3(MODE_, BN_, false);                                                          \
+    if (side) MNRF_LAUNCH_TC3(MODE_, BN_, false, MODE_ == MNRF_GEMM_WGRAD && BN_ >= 64);              \
+    else if (ts) MNRF_LAUNCH_TC3(MODE_, BN_, MODE_ != MNRF_GEMM_WGRAD && BN_ >= 64, false);           \
+    else MNRF_LAUNCH_TC3(MODE_, BN_, false, false);                                                   \
   } while (0)
 #define MNRF_LAUNCH_TC(MODE_)                                                                         \
   do {                                                                                                \

@@ -920,36 +920,31 @@ class Model:
   def _mlp_backward(self, st: LevelState, mlp: MLPDevice, rays=None, impl=0, loss_mults=None, stats=None):
     """Accumulates parameter gradients of one level into mlp.grads (fp32).
 
-    Bias gradients are column sums of the dY buffers.  For the 1024-wide layers the dgrad epilogue that PRODUCES
-    the dY sums them (`colsum`, no extra pass).  For chained 256-wide trunks, whose dY come out of the chain kernel,
-    `ops.gemm_wgrad` (`bsum`) sums them in a separate pass over dY after the weight-gradient GEMM; the
-    bottleneck's weight gradient likewise adds the Dense(1) density head's weight gradient (`side_aw`) in a
-    separate pass over the activation.
+    The bias gradient of a trunk layer, and of the bottleneck, is the column sum of its weight-gradient GEMM's B
+    operand (the stored bf16 dY): `ops.gemm_wgrad` (`bsum`) takes it from the tiles the GEMM stages, with no
+    extra pass over HBM.
     """
     plan = mlp.plan
     trunk = plan.by_role('trunk')
-    # the trunk's input-gradient chain runs as one launch; its bias gradients then come from its weight-gradient
-    # GEMMs, so the top of the trunk does not sum the last layer's
+    # the trunk's input-gradient chain runs as one launch
     chained = self._use_chain(plan, st.M, impl) and len(trunk) > 1
     if st.bwd is None:
       st.bwd = BwdScratch(plan, st.M, chained, self.device)
-    colsum = None if chained else mlp.b(trunk[-1], mlp.grads)
     lm = _loss_args(loss_mults)
     if plan.top == 'view':
-      self._view_bwd(st, mlp, rays, impl, lm, stats, colsum)
+      self._view_bwd(st, mlp, rays, impl, lm, stats)
     else:
-      self._heads_bwd(st, mlp, rays, impl, lm, stats, colsum)
+      self._heads_bwd(st, mlp, rays, impl, lm, stats)
     if plan.density_normals:
       self._tangent_bwd(st, mlp, impl)
     self._trunk_bwd(st, mlp, impl, chained)
 
-  def _slab_dgrad(self, st, mlp, slab, colsum, impl):
-    """d x_last = relu'(x_last) * (slab @ wcat_kn^T): one dgrad over the head-gradient slab, with the bias gradient
-    of the last trunk layer (`colsum`) from the same epilogue."""
+  def _slab_dgrad(self, st, mlp, slab, impl):
+    """d x_last = relu'(x_last) * (slab @ wcat_kn^T): one dgrad over the head-gradient slab."""
     ops.gemm(L.GEMM_DGRAD, slab, mlp.wcat_kn, st.bwd.dy[0], m=st.M, n=mlp.plan.cfg.net_width,
-             k=mlp.plan.slab_cols, maskbits=st.bits[-1], colsum=colsum, impl=impl)
+             k=mlp.plan.slab_cols, maskbits=st.bits[-1], impl=impl)
 
-  def _heads_bwd(self, st, mlp, rays, impl, lm, stats, colsum):
+  def _heads_bwd(self, st, mlp, rays, impl, lm, stats):
     """Top of a trunk without a view branch: colourless normals stage, density (or stacked) and narrow heads."""
     plan = mlp.plan
     sc, g = st.bwd, mlp.grads
@@ -962,7 +957,7 @@ class Model:
     split = dict(dw2=mlp.W(plan.one('rgb'), g), dw_split=1) if plan.top == 'stacked' else {}
     if plan.slab_cols:
       # d x_last against [w_density | W_grad_pred (| W_rgb)]; the heads' weight and bias gradients follow
-      self._slab_dgrad(st, mlp, sc.dhead, colsum, impl)
+      self._slab_dgrad(st, mlp, sc.dhead, impl)
       ops.head_bwd(st.x_last, mlp.w_head, st.d_raw_head, plan.head_n, d.in_pad, dx=None, dw=mlp.W(d, g),
                    db=mlp.b(d, g), **split)
       self._narrow_heads_bwd(st, mlp)
@@ -970,7 +965,7 @@ class Model:
       # input gradient, weight gradients and bias gradients ([b_density | b_rgb]) in one pass.  Features after a
       # skip are constants: dy holds the hidden columns only
       ops.head_bwd(st.x_last, mlp.w_head, st.d_raw_head, plan.head_n, d.in_pad, dx=sc.dy[0], relu_mask=True,
-                   dw=mlp.W(d, g), db=mlp.b(d, g), dxsum=colsum, dx_cols=plan.cfg.net_width, **split)
+                   dw=mlp.W(d, g), db=mlp.b(d, g), dx_cols=plan.cfg.net_width, **split)
 
   def _narrow_heads_bwd(self, st: LevelState, mlp: MLPDevice):
     """Parameter gradients of the narrow heads (x^T d_raw), accumulated into mlp.grads."""
@@ -1006,7 +1001,7 @@ class Model:
         dcur = nxt
     return dcur, skip
 
-  def _view_bwd(self, st, mlp, rays, impl, lm, stats, colsum):
+  def _view_bwd(self, st, mlp, rays, impl, lm, stats):
     """Top of a trunk with a view branch: view MLP, GLO, Ref-NeRF stage or direction encoding, bottleneck."""
     plan = mlp.plan
     sc, g = st.bwd, mlp.grads
@@ -1028,17 +1023,18 @@ class Model:
                      st.d_heads.get('diffuse'), st.d_heads.get('tint'), st.d_heads.get('grad_pred'),
                      st.d_heads['roughness'].view(st.M) if 'roughness' in st.d_heads else None, st.d_rgd, stats)
       self._narrow_heads_bwd(st, mlp)
-    # bottleneck dW + db, and the Dense(1) density head's dW from the same x_last tiles (models.py:460,527)
-    ops.gemm_wgrad(st.x_last, sc.d_vin[:, :bw], mlp.W(bt, g), m=bt.in_pad, n=bw, k=st.M, bsum=mlp.b(bt, g),
-                   side_w=st.d_raw_density.view(st.M), side_aw=mlp.W(d, g).view(-1), impl=impl)
+    # bottleneck dW + db (models.py:527), then the Dense(1) density head's dW (models.py:460) in a pass of its own:
+    # summed inside the GEMM, the weighted x_last tiles take more shared-memory bandwidth from the MMAs than the
+    # pass takes HBM time (DESIGN.md section 3)
+    ops.gemm_wgrad(st.x_last, sc.d_vin[:, :bw], mlp.W(bt, g), m=bt.in_pad, n=bw, k=st.M, bsum=mlp.b(bt, g), impl=impl)
+    ops.head_bwd(st.x_last, st.x_last, st.d_raw_density.view(st.M, 1), 1, bt.in_pad, dw=mlp.W(d, g).view(-1, 1))
     if plan.ref_stage:
       # d x_last = relu'(x_last) * ([d bottleneck | head gradients] @ [W_b | w_heads]^T)
-      self._slab_dgrad(st, mlp, sc.d_vin, colsum, impl)
+      self._slab_dgrad(st, mlp, sc.d_vin, impl)
     else:
       # d x_last = (dbott * Wb^T + d_raw_density (x) w_density) * relu'(x_last)
       ops.gemm(L.GEMM_DGRAD, sc.d_vin[:, :bw], mlp.w_kn[bt.name], sc.dy[0], m=st.M, n=plan.cfg.net_width, k=bw,
-               rowv=st.d_raw_density.view(st.M), colv=mlp.colv_density, maskbits=st.bits[-1], colsum=colsum,
-               impl=impl)
+               rowv=st.d_raw_density.view(st.M), colv=mlp.colv_density, maskbits=st.bits[-1], impl=impl)
     # bias gradient of the density head: a plain sum of d_raw_density
     mlp.b(d, g).add_(st.d_raw_density.sum())
 
@@ -1081,12 +1077,11 @@ class Model:
     for i in range(nl - 1, -1, -1):
       sp = trunk[i]
       xin = st.feat if i == 0 else st.acts[i - 1]
-      ops.gemm(L.GEMM_WGRAD, xin, cur, mlp.W(sp, g), m=sp.in_pad, n=W, k=st.M, impl=impl)
+      ops.gemm_wgrad(xin, cur, mlp.W(sp, g), m=sp.in_pad, n=W, k=st.M, bsum=mlp.b(sp, g), impl=impl)
       if i > 0:
         # only the hidden part of the input carries gradient (features are constants:
         # stop_gradient(sdist), models.py:200-201)
-        ops.gemm(L.GEMM_DGRAD, cur, mlp.w_kn[sp.name], other, m=st.M, n=W, k=W,
-                 maskbits=st.bits[i - 1], colsum=mlp.b(trunk[i - 1], g), impl=impl)
+        ops.gemm(L.GEMM_DGRAD, cur, mlp.w_kn[sp.name], other, m=st.M, n=W, k=W, maskbits=st.bits[i - 1], impl=impl)
         cur, other = other, cur
 
 

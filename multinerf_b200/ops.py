@@ -167,15 +167,23 @@ def gemm_wgrad(x, dy, out, *, m, n, k, bsum=None, side_w=None, side_aw=None, imp
   """dW[m, n] += x[k, m]^T dy[k, n], plus (optional) bsum[n] += column sums of dy (the layer's bias gradient) and
   side_aw[m] += sum_r side_w[r] x[r, m] (weight gradient of a Dense(1) head on x) -- include/mnrf.h.
 
-  The same three launches as mnrf_gemm_wgrad, issued one by one so that each is counted and only the GEMM is
-  timed in GEMM_EVENTS."""
+  One launch on the tensor-core path: the side sums come from the operand tiles the GEMM stages (the SIMT reference,
+  impl=1, adds them in separate passes)."""
+  lib = L.load()
   assert x.stride(-1) == 1 and dy.stride(-1) == 1 and out.stride(-1) == 1
   assert (side_w is None) == (side_aw is None)
-  gemm(L.GEMM_WGRAD, x, dy, out, m=m, n=n, k=k, impl=impl)
-  if bsum is not None:
-    colsum(dy[:k], n, bsum)
-  if side_aw is not None:
-    head_bwd(x[:k], x[:k], _f32(side_w).view(-1, 1), 1, m, dw=side_aw.view(-1, 1))
+  d = L.GemmDesc(L.GEMM_WGRAD, L.ACT_NONE, m, n, k, x.stride(0), dy.stride(0), out.stride(0), 0, 0, 0, 0, impl)
+  _count()
+  ev = None
+  if GEMM_EVENTS is not None:
+    ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+    ev[0].record()
+  L.check(lib.mnrf_gemm_wgrad(C.byref(d), L.ptr(x), L.ptr(dy), L.ptr(bsum),
+                              L.ptr(_f32(side_w)), L.ptr(side_aw), L.ptr(out),
+                              L.stream_ptr()))
+  if ev is not None:
+    ev[1].record()
+    GEMM_EVENTS.append((ev[0], ev[1], 2.0 * m * n * k))
   return out
 
 

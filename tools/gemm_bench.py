@@ -1,6 +1,6 @@
 """Micro-benchmark of mnrf_gemm on the shapes of the 360 config (run on an H100).
 
-  python tools/gemm_bench.py [--rows 1048576]
+  python tools/gemm_bench.py [--rows 1048576] [--bottleneck | --side_sums]
 
 Prints ms / TFLOP/s / GB/s per (mode, N, K, features) so epilogue features can be costed in
 isolation (each timing: 20 launches after 3 warm-ups, inputs larger than L2), and beside each GEMM the rate of
@@ -78,16 +78,59 @@ def bottleneck(dev, M):
           f'{2.0 * Mh * K * (2 if with_dx else 1) / ms / 1e6:7.1f} GB/s', flush=True)
 
 
+def side_sums(dev, rows):
+  """The weight-gradient GEMM with and without the side sums it takes from its staged operand tiles (bias gradient
+  `bsum`, Dense(1) head gradient `side_aw`), at the 360.gin shapes: the NerfMLP trunk [1024, 1024] at rows / 2, the
+  PropMLP trunk [512 | 256, 256] at `rows`, the bottleneck [1024, 256] with both sums; and the 1024-wide DGRAD with
+  mask bits only against mask bits plus column sums."""
+  def line(name, ms, flops, base_ms=None):
+    rel = f'  {100.0 * (ms / base_ms - 1):+5.1f} % vs plain' if base_ms else ''
+    print(f'{name:52s} {ms * 1e3:8.1f} us  {flops / ms / 1e9:7.1f} TFLOP/s{rel}', flush=True)
+  for (M, K, N, head) in [(rows // 2, 1024, 1024, False), (rows, 512, 256, False), (rows, 256, 256, False),
+                          (rows // 2, 1024, 256, True)]:
+    x = (torch.randn(M, K, device=dev) * 0.5).bfloat16()
+    dy = (torch.randn(M, N, device=dev) * 0.1).bfloat16()
+    dw = torch.zeros(K, N, device=dev)
+    db = torch.zeros(N, device=dev)
+    w = torch.randn(M, device=dev)
+    aw = torch.zeros(K, device=dev)
+    fl = 2.0 * M * N * K
+    tag = f'R={M} wgrad [{K},{N}]'
+    base = timeit(lambda: ops.gemm(L.GEMM_WGRAD, x, dy, dw, m=K, n=N, k=M))
+    line(f'{tag} plain', base, fl)
+    ms = timeit(lambda: ops.gemm_wgrad(x, dy, dw, m=K, n=N, k=M, bsum=db))
+    line(f'{tag} + bsum', ms, fl, base)
+    if head:
+      ms = timeit(lambda: ops.gemm_wgrad(x, dy, dw, m=K, n=N, k=M, bsum=db, side_w=w, side_aw=aw))
+      line(f'{tag} + bsum + side_aw', ms, fl, base)
+    del x, dy
+  M, W = rows // 2, 1024
+  dy = (torch.randn(M, W, device=dev) * 0.1).bfloat16()
+  w_kn = (torch.randn(W, W, device=dev) * 0.05).bfloat16()
+  dx = torch.empty(M, W, device=dev, dtype=torch.bfloat16)
+  bits = torch.randint(-2**31, 2**31 - 1, (M, W // 32), device=dev, dtype=torch.int32)
+  cs = torch.zeros(W, device=dev)
+  fl = 2.0 * M * W * W
+  base = timeit(lambda: ops.gemm(L.GEMM_DGRAD, dy, w_kn, dx, m=M, n=W, k=W, maskbits=bits))
+  line(f'R={M} dgrad [{W},{W}] bits', base, fl)
+  ms = timeit(lambda: ops.gemm(L.GEMM_DGRAD, dy, w_kn, dx, m=M, n=W, k=W, maskbits=bits, colsum=cs))
+  line(f'R={M} dgrad [{W},{W}] bits + colsum', ms, fl, base)
+
+
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--rows', type=int, default=1 << 20)
   ap.add_argument('--bottleneck', action='store_true',
                   help='only the NerfMLP bottleneck shapes of 360.gin (1024 <-> 256 at 524288 rows)')
+  ap.add_argument('--side_sums', action='store_true',
+                  help='only the weight-gradient side sums (with / without) and the DGRAD column sums')
   args = ap.parse_args()
   dev = torch.device('cuda:0')
   torch.manual_seed(0)
   if args.bottleneck:
     return bottleneck(dev, args.rows // 2)
+  if args.side_sums:
+    return side_sums(dev, args.rows)
   # the PropMLP trunk, the NerfMLP trunk and its skip layer (K = 1536: FWD and the [1536, 1024] WGRAD; its DGRAD
   # output is 1536 wide, past the fused column sums' limit, and runs split at the concat in the model)
   for (M, N, K) in [(args.rows, 256, 256), (args.rows, 256, 512), (args.rows // 2, 1024, 1024),
