@@ -305,11 +305,19 @@ composite_bwd_kernel(mnrf_loss_desc L, const float* __restrict__ raw_density,
         g *= m;
       }
       dpx[ch] = L.data_mult * lm * g * inv_denom;
+      // d pixel / d scale = sum_s w_s c_unscaled_s = (sum_s w_s c_s) / scale.  A zero scale (RawNeRF exposure
+      // value times 1 + offset) leaves no scaled colour to divide: sum the unscaled colours again (warp-uniform).
+      float wcu = 0.f;
+      if (d_rgb_scale && st.sc[ch] == 0.f && raw_rgb) {
+#pragma unroll
+        for (int j = 0; j < CH; ++j)
+          wcu += st.w[j] * colour_fwd(d, st.z[j][ch], st.zd[j][ch], st.zt[j][ch], raw_tint != nullptr);
+        wcu = warp_sum(wcu);
+      }
       if (lane == 0) {
         st_data += L.data_mult * lm * lv * inv_denom;
         st_mse += lm * resid * resid * inv_denom;
-        // d pixel / d scale = sum_s w_s c_unscaled_s = (sum_s w_s c_s) / scale
-        if (d_rgb_scale) d_rgb_scale[ray * 3 + ch] = st.sc[ch] != 0.f ? dpx[ch] * wc[ch] / st.sc[ch] : 0.f;
+        if (d_rgb_scale) d_rgb_scale[ray * 3 + ch] = st.sc[ch] != 0.f ? dpx[ch] * wc[ch] / st.sc[ch] : dpx[ch] * wcu;
       }
     }
 
