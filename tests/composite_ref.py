@@ -169,3 +169,24 @@ def cdf_at(t_aug, cdf, t):
   for i in range(t.shape[1]):
     out[:, i] = o_math.interp(t[:, i:i + 1].contiguous(), t_aug, cdf)[:, 0]
   return out
+
+
+# the plain compositing descriptor of the kernel-parity tests (a reciprocal-distance level with an opaque background)
+CFG = dict(raydist_fn='reciprocal', opaque_background=True, density_bias=-1.0, density_noise=0.0,
+           rgb_activation='sigmoid', rgb_premultiplier=1.0, rgb_bias=0.0, rgb_padding=0.001, bg_const=1.0)
+
+
+def oracle_composite(raw_d, raw_rgb, sdist, d, near, far, cfg, extras=False):
+  """The oracle's compositing of one level without the optional inputs: (weights, renderings, density, rgb)."""
+  _, s_to_t = o_coord.construct_ray_warps(cfg['raydist_fn'], near, far)
+  tdist = s_to_t(sdist)
+  density = torch.nn.functional.softplus(raw_d + cfg['density_bias'])
+  if raw_rgb is None:
+    rgb = torch.zeros(raw_d.shape + (3,))
+  else:
+    z = cfg['rgb_premultiplier'] * raw_rgb + cfg['rgb_bias']
+    act = torch.sigmoid(z) if cfg['rgb_activation'] == 'sigmoid' else o_math.safe_exp(z)
+    rgb = act * (1 + 2 * cfg['rgb_padding']) - cfg['rgb_padding']
+  w = o_render.compute_alpha_weights(density, tdist, d, opaque_background=cfg['opaque_background'])[0]
+  r = o_render.volumetric_rendering(rgb, w, tdist, cfg['bg_const'], far, extras)
+  return w, r, density, rgb

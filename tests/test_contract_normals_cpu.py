@@ -13,8 +13,8 @@ import pytest
 import torch
 
 from multinerf_b200.models import MLPPlan
+from model_golden import TOL, load, rand_of
 from oracle import o_coord, o_models, o_train
-from test_oracle_model_golden import TOL, load, rand_of
 from util import close
 
 TAG = 'minicontractnormals'

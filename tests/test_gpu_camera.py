@@ -94,7 +94,7 @@ def test_train_step_with_device_ray_generation():
   """Config.cast_rays_in_train_step (train_utils.py:266-268): a step fed with utils.Pixels + cameras
   equals the step fed with the rays those pixels generate."""
   from multinerf_b200 import camera_utils, models, train_utils, utils
-  from test_gpu_model import mini360
+  from model_parity import mini360
   p2c, poses, dist, ndc = _cameras('dist')
   B = 256
   rng = np.random.default_rng(5)

@@ -173,7 +173,7 @@ def test_model_chain_matches_per_layer_path():
   the 2^11-frequency IPE features amplify that, so only a loose bound holds there (the same sensitivity shows
   in the oracle comparison of Dense_0, test_gpu_fullwidth.py)."""
   from multinerf_b200 import configs, lib, models, train_utils, utils
-  from test_gpu_model import synth_rays
+  from model_parity import synth_rays
   lib.require_device()
   for which, tol in (('blender1', 5e-3), ('360', 0.2)):
     grads = []

@@ -9,10 +9,11 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import o_coord, o_models, o_render, o_train
+from model_parity import (fullwidth_case, graph_matches_eager, grad_report, image_rays, mini360, mlp_leaves,
+                          oracle_rays, oracle_step, pinned_forward, synth_case, synth_rays, torch_tree, train_step,
+                          worst)
+from oracle import o_coord, o_models, o_render
 from util import close
-from test_gpu_model import mini360, oracle_rays, synth_rays, torch_tree
-from test_gpu_prop_normals import _bases, _grad_report
 
 pytestmark = pytest.mark.gpu
 
@@ -163,41 +164,27 @@ def _fp32_normals(params, bundle, model, orays, mname, sdist):
 
 
 def _forward_vs_oracle(models, bundle, rays, rand, seed, dens_lim, pix_atol, derived=False):
-  from multinerf_b200 import ops
   B = rays.origins.shape[0]
   model, _ = models.construct_model(seed, rays, bundle)
   params = torch_tree(model.export_flax())
-  rend_o, hist_o = o_models.model_apply(params, bundle, _bases(model), oracle_rays(rays), 0.5, True, rand=rand,
-                                        bf16=True)
-  rend_o = [{k: v.detach() for k, v in r.items()} for r in rend_o]
-  hist_o = [{k: (v.detach() if v is not None else None) for k, v in h.items()} for h in hist_o]
-  r = model._prep_rays(rays)
   pred = bundle.nerf_mlp.enable_pred_normals
   n_clamped = 0
-  for i, st in enumerate(model.forward_levels(rand, r, 0.5, True, True)):
-    # sample positions of level i pinned to the oracle's: one level's MLP and normals stage in isolation
-    st.sdist.copy_(hist_o[i]['sdist'].cuda())
-    model._mlp_forward(st, model.mlps[st.mname], r)
-    comp = ops.composite_fwd(st.raw_density, st.raw_rgb, st.sdist, r.directions, r.near_flat, r.far_flat,
-                             cfg=st.comp_cfg, raw_diffuse=st.heads.get('diffuse'), raw_tint=st.heads.get('tint'),
-                             want_samples=True, want_extras=True)
-    torch.cuda.synchronize()
-    Sx = st.S
-    err = (comp['density'].cpu() - hist_o[i]['density']).abs() / (1.0 + hist_o[i]['density'].abs())
-    assert float(err.max()) < dens_lim[0] and float(err.mean()) < dens_lim[1], (i, float(err.max()), float(err.mean()))
-    close(comp['weights'], hist_o[i]['weights'], atol=2e-2, rtol=0, msg=f'weights level {i}')
-    close(comp['rgb'], rend_o[i]['rgb'], atol=pix_atol, rtol=0, msg=f'pixel level {i}')
+
+  def normals(i, st, h):
+    nonlocal n_clamped
     inherent = None
     if derived:
-      inherent = _normals_errors(_fp32_normals(params, bundle, model, oracle_rays(rays), st.mname, hist_o[i]['sdist']),
-                                 hist_o[i]['normals'])
+      inherent = _normals_errors(_fp32_normals(params, bundle, model, oracle_rays(rays), st.mname, h['sdist']),
+                                 h['normals'])
       print(f'level {i}: oracle fp32 vs bf16 normals {inherent[0]:.4f}, clamped '
             f'{float(inherent[1].max()) if inherent[1].numel() else 0.0:.3f}; GPU vs oracle bf16 normals '
-            f'{_normals_errors(st.normals.cpu().view(B, Sx, 3), hist_o[i]["normals"])[0]:.4f}')
-    _check_normals(st.normals.cpu().view(B, Sx, 3), hist_o[i]['normals'], f'normals level {i}', inherent)
-    n_clamped += int((hist_o[i]['normals'].norm(dim=-1) < 0.999).sum())
+            f'{_normals_errors(st.normals.cpu().view(B, st.S, 3), h["normals"])[0]:.4f}')
+    _check_normals(st.normals.cpu().view(B, st.S, 3), h['normals'], f'normals level {i}', inherent)
+    n_clamped += int((h['normals'].norm(dim=-1) < 0.999).sum())
     if pred:
-      _check_normals(st.normals_pred.cpu().view(B, Sx, 3), hist_o[i]['normals_pred'], f'normals_pred level {i}')
+      _check_normals(st.normals_pred.cpu().view(B, st.S, 3), h['normals_pred'], f'normals_pred level {i}')
+  # sample positions of each level pinned to the oracle's: one level's MLP and normals stage in isolation
+  rend_o, _ = pinned_forward(model, bundle, rays, rand, dens=dens_lim, pixel=pix_atol, level=normals)
   print(f'samples under the eps clamp: {n_clamped}')
   rend, hist = model(rand, rays, 0.5, True)
   torch.cuda.synchronize()
@@ -217,23 +204,14 @@ def _oracle_sensitivity(grads_a, grads_b):
 
 
 def _train_step_vs_oracle(models, train_utils, bundle, rays, rand, target, seed, lim, derived=False):
-  from multinerf_b200 import utils
   model, variables = models.construct_model(seed, rays, bundle)
-  params0 = torch_tree(model.export_flax())
-  opt0 = {'count': 0, 'mu': {}, 'nu': {}}
-  _, _, stats_o, grads_o = o_train.train_step(params0, opt0, bundle, _bases(model), oracle_rays(rays),
-                                              torch.tensor(target), 0.5, rand=rand, bf16=True)
-  step_fn = train_utils.create_train_step(model, bundle.config)
-  state = train_utils.TrainState(variables)
-  state, stats, _ = step_fn(rand, state, utils.Batch(rays=rays, rgb=target), None, 0.5)
-  torch.cuda.synchronize()
-  stats.materialize()
+  t = train_step(model, variables, bundle, rays, target, rand, 0.5)
+  stats, stats_o = t.stats, t.stats_o
   close(stats['mses'], stats_o['mses'].detach(), atol=2e-3, rtol=3e-2, msg='mses')
   sens, stats_32 = {}, None
   if derived:
-    _, _, stats_32, grads_32 = o_train.train_step(params0, opt0, bundle, _bases(model), oracle_rays(rays),
-                                                  torch.tensor(target), 0.5, rand=rand, bf16=False)
-    sens = _oracle_sensitivity(grads_o, grads_32)
+    _, _, stats_32, grads_32 = oracle_step(t.params0, model, bundle, rays, target, rand, 0.5, bf16=False)
+    sens = _oracle_sensitivity(t.grads_o, grads_32)
   seen = 0
   for k in ('orientation', 'predicted_normals'):
     if k in stats_o['losses'] and float(stats_o['losses'][k].detach()) != 0.0:
@@ -244,34 +222,25 @@ def _train_step_vs_oracle(models, train_utils, bundle, rays, rand, target, seed,
       assert abs(stats['losses'][k] - lo) < rel * abs(lo) + 1e-7, (k, stats['losses'][k], lo, rel)
       seen += 1
   assert seen > 0
-  report = _grad_report(model, grads_o, leaves=('kernel', 'bias'))
-  worst = sorted(report.items(), key=lambda kv: -kv[1][0])[:6]
-  print(f'worst leaves (rel, cos): {worst}')
+  report, zero = grad_report(model, t.grads_o, mlp_leaves(model, ('kernel', 'bias')))
+  assert not any(zero.values()), zero
+  print(f'worst leaves (rel, cos): {worst(report)}')
   if sens:
     print('oracle bf16 vs fp32 at those leaves:', {k[:2] + (k[2],): tuple(round(x, 4) for x in sens.get(k, (0, 1)))
-                                                   for k, _ in worst})
+                                                   for k, _ in worst(report)})
 
   def bound(k):
     rel_i, cos_i = sens.get(k, (0.0, 1.0))
     return max(lim[0], SENSITIVITY * rel_i), min(lim[1], 1.0 - SENSITIVITY * (1.0 - cos_i))
   bad = {k: (v, bound(k)) for k, v in report.items() if not (v[0] < bound(k)[0] and v[1] > bound(k)[1])}
-  assert not bad, (bad, worst)
-
-
-def _mini_case(bundle, B, seed):
-  rays, rng = synth_rays(seed, B, 0.2, 1e6)
-  S = [bundle.model.num_prop_samples] * (bundle.model.num_levels - 1) + [bundle.model.num_nerf_samples]
-  rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, 1 if bundle.model.single_jitter else s)).astype(np.float32))
-                     for s in S]}
-  target = rng.uniform(0, 1, (B, 3)).astype(np.float32)
-  return rays, rand, target
+  assert not bad, (bad, worst(report))
 
 
 @pytest.mark.parametrize('refnerf', [False, True])
 def test_forward_vs_oracle(mods, refnerf):
   models, _ = mods
   bundle = mini360_normals(refnerf)
-  rays, rand, _ = _mini_case(bundle, 128, 150)
+  rays, rand, _ = synth_case(bundle, 128, 150, 0.2, 1e6)
   _forward_vs_oracle(models, bundle, rays, rand, 151, (0.08, 4e-3), 1.5e-2)
 
 
@@ -283,7 +252,7 @@ def test_train_step_vs_oracle(mods, target):
   # the PropMLP's gradient then comes from the normal losses alone: the tangent rows through the contraction
   # and their adjoint are not hidden behind the interlevel loss
   bundle.config.interlevel_loss_mult = 0.0
-  rays, rand, target_rgb = _mini_case(bundle, 128, 160)
+  rays, rand, target_rgb = synth_case(bundle, 128, 160, 0.2, 1e6)
   # orientation on the density normals: the loss's gradient runs through the samples under the eps clamp, where
   # it is scaled by 1/sqrt(eps); there the oracle's bf16 and fp32 evaluations already differ at the density head
   _train_step_vs_oracle(models, train_utils, bundle, rays, rand, target_rgb, 161, (0.2, 0.98),
@@ -302,24 +271,20 @@ def fullwidth360_normals():
 
 
 def test_fullwidth_forward_vs_oracle(mods):
-  from test_gpu_fullwidth import _case
   models, _ = mods
-  _, rays, _, rand, _, _ = _case('360')
+  _, rays, _, rand, _, _ = fullwidth_case('360')
   _forward_vs_oracle(models, fullwidth360_normals(), rays, rand, 40, (0.1, 5e-3), 1.5e-2, derived=True)
 
 
 def test_fullwidth_train_step_vs_oracle(mods):
-  from test_gpu_fullwidth import _case
   models, train_utils = mods
-  _, rays, target, rand, _, _ = _case('360')
+  _, rays, target, rand, _, _ = fullwidth_case('360')
   _train_step_vs_oracle(models, train_utils, fullwidth360_normals(), rays, rand, target, 41, (0.3, 0.95),
                         derived=True)
 
 
 def test_cuda_graph_matches_eager(mods):
   models, train_utils = mods
-  from multinerf_b200 import utils
-  bundle = mini360_normals()
   B, steps = 192, 5
   rng = np.random.default_rng(93)
   batches = []
@@ -327,35 +292,17 @@ def test_cuda_graph_matches_eager(mods):
     rays, _ = synth_rays(int(rng.integers(1 << 30)), B, 0.2, 1e6)
     rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B,)).astype(np.float32)) for _ in range(3)]}
     batches.append((rays, rng.uniform(0, 1, (B, 3)).astype(np.float32), rand))
-  results = []
-  for use_graph in [False, True]:
-    model, variables = models.construct_model(8, batches[0][0], bundle)
-    step_fn = train_utils.create_train_step(model, bundle.config, use_graph=use_graph)
-    state = train_utils.TrainState(variables)
-    losses, orient = [], []
-    for i, (rays, tgt, rand) in enumerate(batches):
-      state, stats, _ = step_fn(rand, state, utils.Batch(rays=rays, rgb=tgt), None, i / 10.0)
-      s = stats.materialize()
-      losses.append(s['loss'])
-      orient.append(s['losses']['orientation'])
-    torch.cuda.synchronize()
-    results.append((losses, orient, variables.flat.clone()))
-    if use_graph:
-      assert step_fn.graph_info['state'] == 2, step_fn.graph_info['state']
-  (l0, o0, p0), (l1, o1, p1) = results
-  for a, b in zip(l0 + o0, l1 + o1):
-    assert abs(a - b) < 2e-3 * max(1.0, abs(a)), (l0, l1, o0, o1)
-  assert float((p0 - p1).norm() / p0.norm()) < 2e-3
+  graph_matches_eager(models, train_utils, mini360_normals(), batches, 8,
+                      extra=lambda stats: stats['losses']['orientation'])
 
 
 def test_render_image_normals_chunked_equals_direct_call(mods):
   models, train_utils = mods
-  from test_gpu_render import _image_rays
   bundle = mini360_normals()
   H, W = 29, 41
   bundle.config.render_chunk_size = 256
   bundle.config.vis_num_rays = 8
-  rays = _image_rays(H, W, focal=40.0)          # origin inside the unit ball, near 0.2, far 1e6
+  rays = image_rays(H, W, focal=40.0)          # origin inside the unit ball, near 0.2, far 1e6
   model, state, render_eval_pfn, _, _ = train_utils.setup_model(bundle, 3)
   out = models.render_image(lambda rng, r: render_eval_pfn(state.params, 1.0, None, r), rays, None, bundle,
                             verbose=False)

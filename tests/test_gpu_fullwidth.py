@@ -12,9 +12,8 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import o_models, o_train
+from model_parity import beyond, fullwidth_case, grad_report, mlp_leaves, pinned_forward, train_step, worst
 from util import close
-from test_gpu_model import oracle_rays, synth_rays, torch_tree
 
 pytestmark = pytest.mark.gpu
 
@@ -26,93 +25,29 @@ def mods():
   return models, train_utils
 
 
-def _case(which):
-  """(bundle, rays, target, rand, train_frac) for one BASELINE config at its stated widths."""
-  from multinerf_b200 import configs, utils
-  f = np.float32
-  if which == '360':
-    bundle = configs.bundle_360()
-    B = 256
-    rays, rng = synth_rays(31, B, 0.2, 1e6)
-    S = [64, 64, 32]
-    rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, 1)).astype(f)) for _ in S]}
-  elif which == 'refnerf':
-    bundle = configs.bundle_blender_refnerf()
-    B = 128
-    rays, rng = synth_rays(32, B, 2.0, 6.0, unit_cube=False)
-    S = [128, 128]
-    rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, s)).astype(f)) for s in S]}
-  else:
-    bundle = configs.bundle_llff_raw()
-    B = 128
-    rng = np.random.default_rng(33)
-    o = np.concatenate([rng.uniform(-1, 1, (B, 2)), -np.ones((B, 1))], -1)
-    d = np.concatenate([rng.uniform(-.5, .5, (B, 2)), 2 * np.ones((B, 1))], -1)
-    v = d / np.linalg.norm(d, axis=-1, keepdims=True)
-    eidx = rng.integers(0, 4, (B, 1)).astype(np.int32)
-    lossmult = np.eye(3, dtype=f)[rng.integers(0, 3, B)]           # Bayer mask: one channel per ray
-    rays = utils.Rays(origins=o.astype(f), directions=d.astype(f), viewdirs=v.astype(f),
-                      radii=rng.uniform(1e-3, 2e-3, (B, 1)).astype(f), imageplane=np.zeros((B, 2), f),
-                      lossmult=lossmult, near=np.zeros((B, 1), f), far=np.ones((B, 1), f),
-                      cam_idx=np.zeros((B, 1), np.int32), exposure_idx=eidx,
-                      exposure_values=(2.0 ** -eidx).astype(f))
-    S = [128, 128]
-    rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, s)).astype(f)) for s in S],
-            'density_noise': [torch.tensor(rng.normal(size=(B, s)).astype(f)) for s in S]}
-  target = (rng.uniform(0, 1, (B, 3)) ** (2 if which == 'raw' else 1)).astype(f)
-  return bundle, rays, target, rand, B, S
-
-
 @pytest.mark.parametrize('which', ['360', 'refnerf', 'raw'])
 def test_fullwidth_forward_vs_oracle(mods, which):
   models, _ = mods
-  from multinerf_b200 import ops
-  bundle, rays, target, rand, B, S = _case(which)
+  bundle, rays, target, rand, B, S = fullwidth_case(which)
   model, variables = models.construct_model(40, rays, bundle)
   if which == 'raw':
     tree = model.export_flax()
     tree['exposure_scaling_offsets']['embedding'] = \
         np.random.default_rng(5).normal(size=(1000, 3)).astype(np.float32) * 0.1
     variables = model.init(flax_params=tree)
-  params = torch_tree(model.export_flax())
-  bases = {'nerf': model.plans['NerfMLP_0'].basis,
-           'prop': model.plans.get('PropMLP_0', model.plans['NerfMLP_0']).basis}
-  orays = oracle_rays(rays)
-  rend_o, hist_o = o_models.model_apply(params, bundle, bases, orays, 0.5, True, rand=rand, bf16=True)
-  rend_o = [{k: v.detach() for k, v in r.items()} for r in rend_o]
-  hist_o = [{k: (v.detach() if v is not None else None) for k, v in h.items()} for h in hist_o]
-  r = model._prep_rays(rays)
-  states = model.forward_levels(rand, r, 0.5, True, True)
-  torch.cuda.synchronize()
-  close(states[0].sdist, hist_o[0]['sdist'], atol=1e-6, rtol=1e-6, msg='level-0 sdist')
-  rgb_scale = states[-1].rgb_scale
-  for i, st in enumerate(states):
-    # the sample positions of level i pinned to the oracle's: compares one level's chain in isolation
-    st.sdist.copy_(hist_o[i]['sdist'].cuda())
-    model._mlp_forward(st, model.mlps[st.mname], r)
-    comp = ops.composite_fwd(st.raw_density, st.raw_rgb, st.sdist, r.directions, r.near_flat, r.far_flat,
-                             cfg=st.comp_cfg, density_noise=st.noise,
-                             rgb_scale=rgb_scale if st.raw_rgb is not None else None,
-                             raw_diffuse=st.heads.get('diffuse'), raw_tint=st.heads.get('tint'),
-                             want_samples=True, want_extras=True)
-    torch.cuda.synchronize()
-    dens_o, dens = hist_o[i]['density'], comp['density'].cpu()
-    err = (dens - dens_o).abs() / (1.0 + dens_o.abs())
-    # bf16 tensor-core MLP (8 x 1024-wide layers) vs the bf16-emulating oracle
-    assert float(err.max()) < 0.1 and float(err.mean()) < 5e-3, (which, i, float(err.max()), float(err.mean()))
-    close(comp['weights'], hist_o[i]['weights'], atol=2e-2, rtol=0, msg=f'{which} weights level {i}')
-    close(comp['rgb'], rend_o[i]['rgb'], atol=1.5e-2, rtol=0, msg=f'{which} pixel level {i}')
-    close(comp['acc'], rend_o[i]['acc'], atol=1e-2, rtol=0, msg=f'{which} acc level {i}')
-    if st.raw_rgb is not None:
-      close(comp['rgb_samples'], hist_o[i]['rgb'], atol=4e-2, rtol=0, msg=f'{which} rgb samples level {i}')
+
+  def normals(i, st, h):
     if which == 'refnerf':
-      Sx = st.S
       # unit vectors from a bf16 head: a handful of samples with a tiny raw gradient are ill-conditioned
-      ne = (st.normals_pred.cpu().view(B, Sx, 3) - hist_o[i]['normals_pred']).abs()
+      ne = (st.normals_pred.cpu().view(B, st.S, 3) - h['normals_pred']).abs()
       assert float((ne < 3e-2).float().mean()) > 0.999 and float(ne.max()) < 0.15, (float(ne.max()),)
-      cosn = (st.normals.cpu().view(B, Sx, 3) * hist_o[i]['normals']).sum(-1)
+      cosn = (st.normals.cpu().view(B, st.S, 3) * h['normals']).sum(-1)
       assert float((cosn > 0.98).float().mean()) > 0.97, float((cosn > 0.98).float().mean())
-      close(st.roughness.cpu().view(B, Sx, 1), hist_o[i]['roughness'], atol=2e-2, rtol=0, msg='roughness')
+      close(st.roughness.cpu().view(B, st.S, 1), h['roughness'], atol=2e-2, rtol=0, msg='roughness')
+  # the sample positions of each level pinned to the oracle's: compares one level's chain in isolation; bf16
+  # tensor-core MLP (8 x 1024-wide layers) vs the bf16-emulating oracle
+  rend_o, _ = pinned_forward(model, bundle, rays, rand, dens=(0.1, 5e-3), pixel=1.5e-2, acc=1e-2, samples=4e-2,
+                             level=normals)
   # end to end through Model.__call__ (sample positions drift with the bf16-level differences upstream)
   rend, hist = model(rand, rays, 0.5, True)
   close(rend[-1]['rgb'], rend_o[-1]['rgb'], atol=3e-2, rtol=0, msg=f'{which} final pixel end-to-end')
@@ -121,9 +56,8 @@ def test_fullwidth_forward_vs_oracle(mods, which):
 
 @pytest.mark.parametrize('which', ['360', 'refnerf', 'raw'])
 def test_fullwidth_train_step_vs_oracle(mods, which):
-  models, train_utils = mods
-  from multinerf_b200 import utils
-  bundle, rays, target, rand, B, S = _case(which)
+  models, _ = mods
+  bundle, rays, target, rand, B, S = fullwidth_case(which)
   bundle.config.grad_max_norm = 0.0        # raw Adam update; clipping has its own tests
   bundle.config.grad_max_val = 0.0
   model, variables = models.construct_model(41, rays, bundle)
@@ -132,17 +66,8 @@ def test_fullwidth_train_step_vs_oracle(mods, which):
     tree['exposure_scaling_offsets']['embedding'] = \
         np.random.default_rng(6).normal(size=(1000, 3)).astype(np.float32) * 0.1
     variables = model.init(flax_params=tree)
-  params0 = torch_tree(model.export_flax())
-  bases = {'nerf': model.plans['NerfMLP_0'].basis,
-           'prop': model.plans.get('PropMLP_0', model.plans['NerfMLP_0']).basis}
-  opt0 = {'count': 0, 'mu': {}, 'nu': {}}
-  new_o, opt_o, stats_o, grads_o = o_train.train_step(params0, opt0, bundle, bases, oracle_rays(rays),
-                                                      torch.tensor(target), 0.5, rand=rand, bf16=True)
-  step_fn = train_utils.create_train_step(model, bundle.config)
-  state = train_utils.TrainState(variables)
-  state, stats, _ = step_fn(rand, state, utils.Batch(rays=rays, rgb=target), None, 0.5)
-  torch.cuda.synchronize()
-  stats.materialize()
+  t = train_step(model, variables, bundle, rays, target, rand, 0.5)
+  stats, stats_o = t.stats, t.stats_o
   # per-level mse, PSNR and loss of the train step against the oracle's (tools/psnr_parity.py prints the same
   # comparison), asserted with an order of magnitude of head-room over bf16 rounding
   close(stats['mses'], stats_o['mses'].detach(), atol=1e-6, rtol=2e-3, msg=f'{which} mses')
@@ -154,43 +79,32 @@ def test_fullwidth_train_step_vs_oracle(mods, which):
     if k in stats_o['losses'] and float(stats_o['losses'][k].detach()) != 0.0:
       v = float(stats_o['losses'][k].detach())
       assert abs(stats['losses'][k] - v) < 0.05 * abs(v) + 1e-7, (k, stats['losses'][k], v)
+  heads = [(m, sp.name) for m in model.plans for sp in model.plans[m].specs if sp.out_dim <= 4]
+  keys = mlp_leaves(model, ('kernel', 'bias'))
+  report, zero = grad_report(model, t.grads_o, [k for k in keys if k[2] == 'kernel' or k[:2] not in heads])
+  assert not any(zero.values()), zero
   g = model.export_grads_flax()
-  report = {}
-  for mname in model.plans:
-    plan = model.plans[mname]
-    for sp in plan.specs:
-      lname = sp.name
-      ka = torch.tensor(g[mname][lname]['kernel']).double().flatten()
-      kb = grads_o[(mname, lname, 'kernel')].double().flatten()
-      if float(kb.norm()) == 0.0:
-        assert float(ka.norm()) == 0.0, (mname, lname)
-        continue
-      rel = float((ka - kb).norm() / kb.norm())
-      cos = float((ka @ kb) / (ka.norm() * kb.norm()).clamp(min=1e-30))
-      report[(mname, lname, 'kernel')] = (round(rel, 3), round(cos, 4))
-      ba = torch.tensor(g[mname][lname]['bias']).double().flatten()
-      bb = grads_o[(mname, lname, 'bias')].double().flatten()
-      if sp.out_dim <= 4:
-        # a head's bias gradient is a plain sum of the per-sample gradients: it cancels to (nearly) nothing,
-        # so its error is measured against the size of the same head's kernel-gradient entries
-        scale = max(float(bb.abs().max()), float(kb.abs().max()))
-        report[(mname, lname, 'bias')] = (round(float((ba - bb).abs().max()) / scale, 3), 1.0)
-      else:
-        report[(mname, lname, 'bias')] = (round(float((ba - bb).norm() / bb.norm().clamp(min=1e-12)), 3),
-                                   round(float((ba @ bb) / (ba.norm() * bb.norm()).clamp(min=1e-30)), 4))
+  for mname, lname in heads:
+    if (mname, lname, 'kernel') in zero:
+      continue
+    # a head's bias gradient is a plain sum of the per-sample gradients: it cancels to (nearly) nothing,
+    # so its error is measured against the size of the same head's kernel-gradient entries
+    ba = torch.tensor(g[mname][lname]['bias']).double()
+    bb, kb = t.grads_o[(mname, lname, 'bias')].double(), t.grads_o[(mname, lname, 'kernel')].double()
+    scale = max(float(bb.abs().max()), float(kb.abs().max()))
+    report[(mname, lname, 'bias')] = (round(float((ba - bb).abs().max()) / scale, 3), 1.0)
+  report = {k: report[k] for k in keys if k in report}
   # dY travels between layers in bf16 on both sides with different rounding points, and every ReLU whose
   # pre-activation sits within bf16 noise of zero may flip: the error grows with depth and is largest at
   # Dense_0 (the worst leaves are printed below).
   # Ref-NeRF adds the bf16 tangent chain and an 8-layer view MLP.
   lim = {'360': (0.2, 0.98), 'refnerf': (0.3, 0.95), 'raw': (0.1, 0.995)}[which]
-  worst = sorted(report.items(), key=lambda kv: -kv[1][0])[:6]
-  print(f'[fullwidth {which}] worst leaves (rel, cos): {worst}')
-  bad = {k: v for k, v in report.items() if not (v[0] < lim[0] and v[1] > lim[1])}
-  assert not bad, (bad, worst)
+  print(f'[fullwidth {which}] worst leaves (rel, cos): {worst(report)}')
+  bad = beyond(report, *lim)
+  assert not bad, (bad, worst(report))
   if which == 'raw':
-    a = torch.tensor(g['exposure_scaling_offsets']['embedding']).double().flatten()
-    b = grads_o[('exposure_scaling_offsets', 'embedding')].double().flatten()
-    assert float((a - b).norm() / b.norm()) < 0.05 and float(b.norm()) > 0
+    r, z = grad_report(model, t.grads_o, [('exposure_scaling_offsets', 'embedding')])
+    assert not z and r[('exposure_scaling_offsets', 'embedding')][0] < 0.05, (r, z)
 
 
 def test_fullwidth_cta_pair_kernels_ran(mods):

@@ -10,8 +10,9 @@ import numpy as np
 import pytest
 import torch
 
+from composite_ref import CFG, oracle_composite
 from oracle import o_coord, o_math, o_render, o_stepfun
-from util import close
+from util import close, kernel_rays
 
 pytestmark = pytest.mark.gpu
 
@@ -81,14 +82,6 @@ def test_sample_level_deterministic_and_errors(ops):
     ops.sample_level(t, w, 1)
 
 
-def _rays(rng, b, unit_cube=True):
-  o = rng.uniform(-1, 1, (b, 3)).astype(np.float32)
-  d = rng.normal(size=(b, 3)).astype(np.float32)
-  d = (d / np.linalg.norm(d, axis=-1, keepdims=True) * rng.uniform(0.8, 1.2, (b, 1))).astype(np.float32)
-  radii = rng.uniform(5e-4, 1e-3, (b, 1)).astype(np.float32)
-  return torch.tensor(o), torch.tensor(d), torch.tensor(radii)
-
-
 @pytest.mark.parametrize('name,shape,sub,maxdeg,raydist,near,far,contract,rshape', [
     ('360', 'icosahedron', 2, 12, 'reciprocal', 0.2, 1e6, True, 'cone'),
     ('blender', 'octahedron', 1, 16, None, 2.0, 6.0, False, 'cone'),
@@ -98,7 +91,7 @@ def test_encode_vs_oracle(ops, name, shape, sub, maxdeg, raydist, near, far, con
   from multinerf_b200 import geopoly
   rng = np.random.default_rng(7)
   B, S = 96, 32
-  o, d, radii = _rays(rng, B)
+  o, d, radii = kernel_rays(rng, B)
   sdist = torch.tensor(np.sort(rng.uniform(0, 1, (B, S + 1)).astype(np.float32), -1))
   sdist[:, 0], sdist[:, -1] = 0, 1
   nearv, farv = torch.full((B, 1), near), torch.full((B, 1), far)
@@ -155,25 +148,6 @@ def test_viewdir_enc(ops):
   assert (got[:, :, 283:] == 0).all() and (got[:, :, :256] == 7).all()
 
 
-CFG = dict(raydist_fn='reciprocal', opaque_background=True, density_bias=-1.0, density_noise=0.0,
-           rgb_activation='sigmoid', rgb_premultiplier=1.0, rgb_bias=0.0, rgb_padding=0.001, bg_const=1.0)
-
-
-def _oracle_composite(raw_d, raw_rgb, sdist, d, near, far, cfg, extras=False):
-  _, s_to_t = o_coord.construct_ray_warps(cfg['raydist_fn'], near, far)
-  tdist = s_to_t(sdist)
-  density = torch.nn.functional.softplus(raw_d + cfg['density_bias'])
-  if raw_rgb is None:
-    rgb = torch.zeros(raw_d.shape + (3,))
-  else:
-    z = cfg['rgb_premultiplier'] * raw_rgb + cfg['rgb_bias']
-    act = torch.sigmoid(z) if cfg['rgb_activation'] == 'sigmoid' else o_math.safe_exp(z)
-    rgb = act * (1 + 2 * cfg['rgb_padding']) - cfg['rgb_padding']
-  w = o_render.compute_alpha_weights(density, tdist, d, opaque_background=cfg['opaque_background'])[0]
-  r = o_render.volumetric_rendering(rgb, w, tdist, cfg['bg_const'], far, extras)
-  return w, r, density, rgb
-
-
 @pytest.mark.parametrize('S,opaque,raydist,near,far,act', [
     (32, True, 'reciprocal', 0.2, 1e6, 'sigmoid'), (64, True, 'reciprocal', 0.2, 1e6, 'sigmoid'),
     (128, False, None, 2.0, 6.0, 'sigmoid'), (48, False, None, 0.0, 1.0, 'safe_exp')])
@@ -182,7 +156,7 @@ def test_composite_fwd_vs_oracle(ops, S, opaque, raydist, near, far, act):
   B = 130
   cfg = dict(CFG, raydist_fn=raydist, opaque_background=opaque, rgb_activation=act,
              rgb_bias=-5.0 if act == 'safe_exp' else 0.0, rgb_padding=0.0 if act == 'safe_exp' else 0.001)
-  _, d, _ = _rays(rng, B)
+  _, d, _ = kernel_rays(rng, B)
   sdist = torch.tensor(np.sort(rng.uniform(0, 1, (B, S + 1)).astype(np.float32), -1))
   sdist[:, 0], sdist[:, -1] = 0, 1
   raw_d = torch.tensor(rng.normal(size=(B, S)).astype(np.float32) * 3)
@@ -190,7 +164,7 @@ def test_composite_fwd_vs_oracle(ops, S, opaque, raydist, near, far, act):
   raw_d[1] = 30
   raw_rgb = torch.tensor(rng.normal(size=(B, S, 3)).astype(np.float32))
   nearv, farv = torch.full((B, 1), near), torch.full((B, 1), far)
-  w_o, r_o, dens_o, rgb_o = _oracle_composite(raw_d, raw_rgb, sdist, d, nearv, farv, cfg, extras=True)
+  w_o, r_o, dens_o, rgb_o = oracle_composite(raw_d, raw_rgb, sdist, d, nearv, farv, cfg, extras=True)
   out = ops.composite_fwd(raw_d.cuda(), raw_rgb.cuda(), sdist.cuda(), d.cuda(), nearv[:, 0].contiguous().cuda(),
                           farv[:, 0].contiguous().cuda(), cfg=cfg, want_samples=True, want_extras=True)
   close(out['density'], dens_o, msg='density')
@@ -207,7 +181,7 @@ def test_composite_fwd_vs_oracle(ops, S, opaque, raydist, near, far, act):
     rel = ((dist[:, 1 + i] - ref).abs() / ref.abs().clamp(min=1e-6))
     assert (rel < 1e-3).float().mean() > 0.97, (k, rel.max())
   # PropMLP levels: rgb = 0
-  w_o2, r_o2, _, _ = _oracle_composite(raw_d, None, sdist, d, nearv, farv, cfg)
+  w_o2, r_o2, _, _ = oracle_composite(raw_d, None, sdist, d, nearv, farv, cfg)
   out2 = ops.composite_fwd(raw_d.cuda(), None, sdist.cuda(), d.cuda(), nearv[:, 0].contiguous().cuda(),
                            farv[:, 0].contiguous().cuda(), cfg=cfg)
   close(out2['rgb'], r_o2['rgb'], msg='prop pixel')
@@ -220,7 +194,7 @@ def test_composite_bwd_vs_oracle_autograd(ops, level, loss_type, S):
   rng = np.random.default_rng(11)
   B, Sf = 70, 32
   cfg = dict(CFG)
-  _, d, _ = _rays(rng, B)
+  _, d, _ = kernel_rays(rng, B)
 
   def mk_sdist(n):
     s = torch.tensor(np.sort(rng.uniform(0, 1, (B, n + 1)).astype(np.float32), -1))
@@ -246,7 +220,7 @@ def test_composite_bwd_vs_oracle_autograd(ops, level, loss_type, S):
     data_loss_mult = 1.0
     interlevel_loss_mult = 1.0
     distortion_loss_mult = 0.01
-  w_o, r_o, _, _ = _oracle_composite(raw_d, raw_rgb, sdist, d, nearv, farv, cfg)
+  w_o, r_o, _, _ = oracle_composite(raw_d, raw_rgb, sdist, d, nearv, farv, cfg)
   lm = lossmult.expand(B, 3)
   data, st = o_train.compute_data_loss(target, [r_o], lm, Cfg)   # single level -> data_loss_mult
   data_mult = 1.0
@@ -516,7 +490,7 @@ def test_composite_diffuse_specular_mode(ops):
   rng = np.random.default_rng(31)
   B, S = 50, 32
   cfg = dict(CFG, raydist_fn=None, opaque_background=False, density_bias=0.5, rgb_mode=1)
-  _, d, _ = _rays(rng, B)
+  _, d, _ = kernel_rays(rng, B)
   sdist = torch.tensor(np.sort(rng.uniform(0, 1, (B, S + 1)).astype(np.float32), -1))
   nearv, farv = torch.full((B, 1), 2.0), torch.full((B, 1), 6.0)
   leaves = [torch.tensor(rng.normal(size=sh).astype(np.float32) * sc, requires_grad=True)
@@ -718,7 +692,7 @@ def test_encode_tangent_features(ops):
   from multinerf_b200 import geopoly
   rng = np.random.default_rng(61)
   B, S, maxdeg = 40, 16, 16
-  o, d, radii = _rays(rng, B)
+  o, d, radii = kernel_rays(rng, B)
   o = o * 3
   sdist = torch.tensor(np.sort(rng.uniform(0, 1, (B, S + 1)).astype(np.float32), -1))
   nearv, farv = torch.full((B, 1), 2.0), torch.full((B, 1), 6.0)

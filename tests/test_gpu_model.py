@@ -6,72 +6,18 @@ bf16-rounded weights and bf16-rounded layer inputs (fp32 accumulation) -- see
 oracle/o_models.py `bf16=True`.  Achieved errors are asserted with explicit tolerances.
 """
 import copy
-import math
 
 import numpy as np
 import pytest
 import torch
 
+from model_parity import (bases, beyond, graph_matches_eager, grad_report, level_jitter, mini360, mini_refnerf,
+                          mlp_leaves, oracle_rays, pinned_forward, plumbing_blender, raw_rays, synth_rays, torch_tree,
+                          train_step)
 from oracle import o_models, o_train
 from util import close
 
 pytestmark = pytest.mark.gpu
-
-
-def synth_rays(seed, B, near, far, unit_cube=True, radius=4.0):
-  from multinerf_b200 import utils
-  rng = np.random.default_rng(seed)
-  if unit_cube:
-    o = rng.uniform(-1, 1, (B, 3))
-    d = rng.normal(size=(B, 3))
-    d /= np.linalg.norm(d, axis=-1, keepdims=True)
-  else:   # cameras on a sphere looking at the origin (tests/render_test.py:137-143 style)
-    o = rng.normal(size=(B, 3))
-    o = o / np.linalg.norm(o, axis=-1, keepdims=True) * radius
-    d = -o / radius + rng.normal(size=(B, 3)) * 0.1
-    d /= np.linalg.norm(d, axis=-1, keepdims=True)
-  v = d.copy()
-  d = d * rng.uniform(0.8, 1.2, (B, 1))
-  f = np.float32
-  return utils.Rays(origins=o.astype(f), directions=d.astype(f), viewdirs=v.astype(f),
-                    radii=rng.uniform(5e-4, 1e-3, (B, 1)).astype(f),
-                    imageplane=np.zeros((B, 2), f), lossmult=np.ones((B, 1), f),
-                    near=np.full((B, 1), near, f), far=np.full((B, 1), far, f),
-                    cam_idx=np.zeros((B, 1), np.int32)), rng
-
-
-def mini360():
-  from multinerf_b200 import configs
-  b = configs.bundle_360()
-  b.model.num_prop_samples = 32
-  b.model.num_nerf_samples = 16
-  b.prop_mlp.net_depth, b.prop_mlp.net_width = 2, 64
-  b.nerf_mlp.net_depth, b.nerf_mlp.net_width = 6, 128
-  b.nerf_mlp.bottleneck_width, b.nerf_mlp.net_width_viewdirs = 64, 64
-  return b
-
-
-def plumbing_blender():
-  from multinerf_b200 import configs
-  b = configs.bundle_blender_256()
-  b.model.num_levels = 1
-  b.model.num_nerf_samples = 32
-  return b
-
-
-def torch_tree(tree):
-  return {k: (torch_tree(v) if isinstance(v, dict) else torch.tensor(v)) for k, v in tree.items()}
-
-
-class TRays:
-  pass
-
-
-def oracle_rays(rays):
-  r = TRays()
-  for k, v in rays.__dict__.items():
-    setattr(r, k, None if v is None else torch.tensor(np.asarray(v)))
-  return r
 
 
 @pytest.fixture(scope='module')
@@ -99,44 +45,15 @@ def test_model_forward_vs_oracle(mods, which):
   near, far = (2.0, 6.0) if which == 'plumbing' else (0.2, 1e6)
   rays, rng = synth_rays(0 if which == 'plumbing' else 1, B, near, far, unit_cube=which != 'plumbing')
   model, variables = models.construct_model(2, rays, bundle)
-  params = torch_tree(model.export_flax())
-  bases = {'nerf': model.plans['NerfMLP_0'].basis,
-           'prop': model.plans.get('PropMLP_0', model.plans['NerfMLP_0']).basis}
-  orays = oracle_rays(rays)
-  sched = model.level_schedule(0.5)[2]
   for randomized in [False, True]:
-    rand = None
-    if randomized:
-      rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, 1)).astype(np.float32)) for _ in sched]}
-    with torch.no_grad():
-      rend_o, hist_o, dbg_o = o_models.model_apply(params, bundle, bases, orays, 0.5, True, rand=rand,
-                                                   bf16=True, return_debug=True)
+    rand = level_jitter(rng, bundle, B) if randomized else None
     rend, hist = model(rand, rays, 0.5, True)
     torch.cuda.synchronize()
-    # level 0 resamples the trivial [0,1] histogram: identical inputs on both sides
-    close(hist[0]['sdist'], hist_o[0]['sdist'], atol=1e-6, rtol=1e-6, msg='level-0 sdist')
-    # per-level check with the sample positions pinned to the oracle's
-    B_, lv_states = B, model.forward_levels(rand, model._prep_rays(rays), 0.5, True, True)
-    r = model._prep_rays(rays)
-    from multinerf_b200 import ops
-    for i, st in enumerate(lv_states):
-      st.sdist.copy_(hist_o[i]['sdist'].cuda())
-      model._mlp_forward(st, model.mlps[st.mname], r)
-      comp = ops.composite_fwd(st.raw_density, st.raw_rgb, st.sdist, r.directions, r.near_flat, r.far_flat,
-                               cfg=st.comp_cfg, want_samples=True, want_extras=True)
-      torch.cuda.synchronize()
-      dens_o, dens = hist_o[i]['density'], comp['density'].cpu()
-      # bf16 tensor-core MLP vs bf16-emulating oracle: state the achieved error
-      err = (dens - dens_o).abs() / (1.0 + dens_o.abs())
-      assert float(err.max()) < 0.08 and float(err.mean()) < 4e-3, (i, float(err.max()), float(err.mean()))
-      close(comp['weights'], hist_o[i]['weights'], atol=2e-2, rtol=0, msg=f'weights level {i}')
-      close(comp['rgb'], rend_o[i]['rgb'], atol=1e-2, rtol=0, msg=f'pixel level {i}')
-      if st.raw_rgb is not None:
-        close(comp['rgb_samples'], hist_o[i]['rgb'], atol=3e-2, rtol=0, msg=f'rgb samples level {i}')
-      close(comp['acc'], rend_o[i]['acc'], atol=1e-2, rtol=0, msg=f'acc level {i}')
+    # bf16 tensor-core MLP vs bf16-emulating oracle: state the achieved error
+    rend_o, _ = pinned_forward(model, bundle, rays, rand, dens=(0.08, 4e-3), pixel=1e-2, acc=1e-2, samples=3e-2)
     # end to end (sample positions drift with the bf16-level differences of earlier levels)
     close(rend[-1]['rgb'], rend_o[-1]['rgb'], atol=2e-2, rtol=0, msg='final pixel end-to-end')
-    assert rend[-1]['rgb'].shape == (B, 3) and hist[-1]['weights'].shape == (B, sched[-1]['S'])
+    assert rend[-1]['rgb'].shape == (B, 3) and hist[-1]['weights'].shape == (B, bundle.model.num_nerf_samples)
     for k in ['acc', 'distance_mean', 'distance_median', 'distance_percentile_5', 'distance_percentile_95',
               'ray_sdist', 'ray_weights', 'ray_rgbs']:
       assert k in rend[-1]
@@ -144,8 +61,7 @@ def test_model_forward_vs_oracle(mods, which):
 
 @pytest.mark.parametrize('which,impl', [('mini360', 1), ('mini360', 0), ('plumbing', 0)])
 def test_train_step_vs_oracle(mods, which, impl):
-  models, train_utils = mods
-  from multinerf_b200 import utils
+  models, _ = mods
   bundle = plumbing_blender() if which == 'plumbing' else mini360()
   bundle.config.grad_max_norm = 0.0      # compare raw Adam first; clipping is covered below
   B = 64 if which == 'plumbing' else 160
@@ -153,49 +69,26 @@ def test_train_step_vs_oracle(mods, which, impl):
   rays, rng = synth_rays(3, B, near, far, unit_cube=which != 'plumbing')
   target = rng.uniform(0, 1, (B, 3)).astype(np.float32)
   model, variables = models.construct_model(4, rays, bundle)
-  params0 = torch_tree(model.export_flax())
-  bases = {'nerf': model.plans['NerfMLP_0'].basis,
-           'prop': model.plans.get('PropMLP_0', model.plans['NerfMLP_0']).basis}
-  sched = model.level_schedule(0.5)[2]
-  rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, 1)).astype(np.float32)) for _ in sched]}
-  # oracle step (bf16-emulated forward, fp32 autograd)
-  opt0 = {'count': 0, 'mu': {}, 'nu': {}}
-  new_o, opt_o, stats_o, grads_o = o_train.train_step(params0, opt0, bundle, bases, oracle_rays(rays),
-                                                      torch.tensor(target), 0.5, rand=rand, bf16=True)
-  step_fn = train_utils.create_train_step(model, bundle.config, impl=impl)
-  state = train_utils.TrainState(variables)
-  batch = utils.Batch(rays=rays, rgb=target)
-  state, stats, _ = step_fn(rand, state, batch, None, 0.5)
-  torch.cuda.synchronize()
-  stats.materialize()
-  close(stats['mses'], stats_o['mses'].detach(), atol=2e-3, rtol=2e-2, msg='mses')
-  assert abs(stats['loss'] - float(stats_o['loss'].detach())) < 2e-2 * max(1.0, abs(float(stats_o['loss'].detach())))
-  g = model.export_grads_flax()
-  worst = 0.0
-  for mname in g:
-    for lname in g[mname]:
-      for leaf in ['kernel', 'bias']:
-        a = torch.tensor(g[mname][lname][leaf]).double().flatten()
-        b = grads_o[(mname, lname, leaf)].double().flatten()
-        if float(b.norm()) == 0.0:            # module unused by this config (e.g. PropMLP at 1 level)
-          assert float(a.norm()) == 0.0, (mname, lname, leaf)
-          continue
-        denom = b.norm().clamp(min=1e-12)
-        rel = float((a - b).norm() / denom)
-        cos = float((a @ b) / (a.norm() * b.norm()).clamp(min=1e-30))
-        worst = max(worst, rel)
-        # dY travels between layers in bf16 on both sides (different rounding points): the deepest
-        # backward path (Dense_0) accumulates the most
-        assert rel < 0.12 and cos > 0.993, (mname, lname, leaf, rel, cos)
+  t = train_step(model, variables, bundle, rays, target, level_jitter(rng, bundle, B), 0.5, impl=impl)
+  close(t.stats['mses'], t.stats_o['mses'].detach(), atol=2e-3, rtol=2e-2, msg='mses')
+  lo = float(t.stats_o['loss'].detach())
+  assert abs(t.stats['loss'] - lo) < 2e-2 * max(1.0, abs(lo)), (t.stats['loss'], lo)
+  report, zero = grad_report(model, t.grads_o, mlp_leaves(model, ('kernel', 'bias')))
+  # a module unused by the config (e.g. PropMLP at 1 level) gets no gradient on either side
+  assert not any(zero.values()), zero
+  # dY travels between layers in bf16 on both sides (different rounding points): the deepest
+  # backward path (Dense_0) accumulates the most
+  assert not beyond(report, 0.12, 0.993), beyond(report, 0.12, 0.993)
   # parameters after one Adam step (first step moves every weight by ~lr regardless of scale)
   newp = model.export_flax()
   lr = o_train.lr_at(0, bundle.config)
   for mname in newp:
     for lname in newp[mname]:
       a = torch.tensor(newp[mname][lname]['kernel'])
-      b = new_o[mname][lname]['kernel']
+      b = t.new_o[mname][lname]['kernel']
+      p0 = t.params0[mname][lname]['kernel']
       assert float((a - b).abs().max()) <= 2.1 * lr, (mname, lname)
-      agree = ((a - params0[mname][lname]['kernel']).sign() == (b - params0[mname][lname]['kernel']).sign())
+      agree = ((a - p0).sign() == (b - p0).sign())
       assert float(agree.float().mean()) > 0.95, (mname, lname, float(agree.float().mean()))
 
 
@@ -203,36 +96,12 @@ def test_cuda_graph_train_step_matches_eager(mods):
   """The captured two-graph step (forward+backward | clip+Adam+repack) must track the eager step
   while train_frac, the learning rate, the Adam bias corrections and the jitter change per step."""
   models, train_utils = mods
-  from multinerf_b200 import utils
-  bundle = mini360()
-  B = 256
-  rays, rng = synth_rays(5, B, 0.2, 1e6)
-  sched_n = 3
-  steps = 5
+  B, steps = 256, 5
+  _, rng = synth_rays(5, B, 0.2, 1e6)
   batches = [(synth_rays(10 + i, B, 0.2, 1e6)[0], rng.uniform(0, 1, (B, 3)).astype(np.float32)) for i in range(steps)]
-  rands = [{'jitter': [torch.tensor(rng.uniform(0, 1, (B,)).astype(np.float32)) for _ in range(sched_n)]}
+  rands = [{'jitter': [torch.tensor(rng.uniform(0, 1, (B,)).astype(np.float32)) for _ in range(3)]}
            for _ in range(steps)]
-  results = []
-  for use_graph in [False, True]:
-    model, variables = models.construct_model(6, rays, bundle)
-    step_fn = train_utils.create_train_step(model, bundle.config, use_graph=use_graph)
-    state = train_utils.TrainState(variables)
-    losses = []
-    for i in range(steps):
-      r, tgt = batches[i]
-      state, stats, _ = step_fn(rands[i], state, utils.Batch(rays=r, rgb=tgt), None, i / 10.0)
-      losses.append(stats.materialize()['loss'])
-    torch.cuda.synchronize()
-    results.append((losses, variables.flat.clone(), variables.step))
-    if use_graph:
-      assert step_fn.graph_info['state'] == 2 and step_fn.graph_info['launches'] > 20
-  (l0, p0, s0), (l1, p1, s1) = results
-  assert s0 == s1 == steps
-  for a, b in zip(l0, l1):
-    assert abs(a - b) < 2e-3 * max(1.0, abs(a)), (l0, l1)
-  # fp32 atomics make the two runs differ in the last bits only
-  rel = float((p0 - p1).norm() / p0.norm())
-  assert rel < 2e-3, rel
+  graph_matches_eager(models, train_utils, mini360(), [b + (r,) for b, r in zip(batches, rands)], 6)
 
 
 def test_cuda_graph_gradients_track_eager_with_moving_weights(mods):
@@ -291,150 +160,77 @@ def test_rawnerf_train_step_vs_oracle(mods):
   """BASELINE config 4 (llff_raw.gin) at reduced size: single MLP for both levels, cylinder rays,
   safe_exp colours, per-sample jitter, density noise, exposure scaling with learned offsets, Bayer
   lossmult, rawnerf loss, coarse data loss, value + norm clipping."""
-  models, train_utils = mods
-  from multinerf_b200 import configs, utils
+  models, _ = mods
+  from multinerf_b200 import configs
   bundle = configs.bundle_llff_raw()
   bundle.model.num_prop_samples = bundle.model.num_nerf_samples = 32
   bundle.nerf_mlp.net_width, bundle.nerf_mlp.bottleneck_width, bundle.nerf_mlp.net_width_viewdirs = 128, 64, 64
   bundle.config.grad_max_norm = 0.0
   bundle.config.grad_max_val = 0.0
   B, S = 192, 32
-  rng = np.random.default_rng(21)
   f = np.float32
-  o = np.concatenate([rng.uniform(-1, 1, (B, 2)), -np.ones((B, 1))], -1)
-  d = np.concatenate([rng.uniform(-.5, .5, (B, 2)), 2 * np.ones((B, 1))], -1)
-  v = d / np.linalg.norm(d, axis=-1, keepdims=True)
-  eidx = rng.integers(0, 4, (B, 1)).astype(np.int32)
-  lossmult = np.eye(3, dtype=f)[rng.integers(0, 3, B)]           # Bayer mask: one channel per ray
-  rays = utils.Rays(origins=o.astype(f), directions=d.astype(f), viewdirs=v.astype(f),
-                    radii=rng.uniform(1e-3, 2e-3, (B, 1)).astype(f), imageplane=np.zeros((B, 2), f),
-                    lossmult=lossmult, near=np.zeros((B, 1), f), far=np.ones((B, 1), f),
-                    cam_idx=np.zeros((B, 1), np.int32), exposure_idx=eidx,
-                    exposure_values=(2.0 ** -eidx).astype(f))
+  rng = np.random.default_rng(21)
+  rays = raw_rays(rng, B)
   target = (rng.uniform(0, 1, (B, 3)) ** 2).astype(f)
   model, variables = models.construct_model(8, rays, bundle)
   tree = model.export_flax()
   tree['exposure_scaling_offsets']['embedding'] = rng.normal(size=(1000, 3)).astype(f) * 0.1
   variables = model.init(flax_params=tree)
-  params0 = torch_tree(model.export_flax())
-  bases = {'nerf': model.plans['NerfMLP_0'].basis, 'prop': model.plans['NerfMLP_0'].basis}
   rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, S)).astype(f)) for _ in range(2)],
           'density_noise': [torch.tensor(rng.normal(size=(B, S)).astype(f)) for _ in range(2)]}
-  opt0 = {'count': 0, 'mu': {}, 'nu': {}}
-  new_o, opt_o, stats_o, grads_o = o_train.train_step(params0, opt0, bundle, bases, oracle_rays(rays),
-                                                      torch.tensor(target), 0.3, rand=rand, bf16=True)
-  step_fn = train_utils.create_train_step(model, bundle.config)
-  state = train_utils.TrainState(variables)
-  state, stats, _ = step_fn(rand, state, utils.Batch(rays=rays, rgb=target), None, 0.3)
-  torch.cuda.synchronize()
-  stats.materialize()
-  close(stats['mses'], stats_o['mses'].detach(), atol=2e-3, rtol=3e-2, msg='mses')
-  lo = float(stats_o['loss'].detach())
-  assert abs(stats['loss'] - lo) < 3e-2 * max(1.0, abs(lo)), (stats['loss'], lo)
-  g = model.export_grads_flax()
-  a = torch.tensor(g['exposure_scaling_offsets']['embedding']).double().flatten()
-  b = grads_o[('exposure_scaling_offsets', 'embedding')].double().flatten()
-  assert float((a - b).norm() / b.norm()) < 0.05 and float(b.norm()) > 0, float((a - b).norm() / b.norm())
-  assert float(a.reshape(-1, 3)[0].abs().max()) == 0.0      # index 0 is pinned (mask = idx > 0)
-  for lname in g['NerfMLP_0']:
-    a = torch.tensor(g['NerfMLP_0'][lname]['kernel']).double().flatten()
-    b = grads_o[('NerfMLP_0', lname, 'kernel')].double().flatten()
-    rel = float((a - b).norm() / b.norm().clamp(min=1e-12))
-    cos = float((a @ b) / (a.norm() * b.norm()).clamp(min=1e-30))
-    assert rel < 0.15 and cos > 0.99, (lname, rel, cos)
-
-
-def mini_refnerf():
-  from multinerf_b200 import configs
-  b = configs.Bundle()
-  c, m, n = b.config, b.model, b.nerf_mlp
-  c.data_loss_type, c.distortion_loss_mult, c.interlevel_loss_mult, c.data_coarse_loss_mult = 'mse', 0.0, 0.0, 0.1
-  c.orientation_loss_mult, c.orientation_coarse_loss_mult = 0.1, 0.01
-  c.predicted_normal_loss_mult, c.predicted_normal_coarse_loss_mult = 3e-4, 3e-5
-  c.adam_eps, c.near, c.far = 1e-8, 2.0, 6.0
-  m.num_levels, m.single_mlp, m.num_prop_samples, m.num_nerf_samples = 2, True, 16, 16
-  m.anneal_slope, m.dilation_multiplier, m.dilation_bias, m.single_jitter, m.resample_padding = 0., 0., 0., False, 0.01
-  n.net_depth, n.net_width, n.net_depth_viewdirs, n.net_width_viewdirs = 6, 128, 6, 64
-  n.basis_shape, n.basis_subdivisions, n.disable_density_normals, n.enable_pred_normals = 'octahedron', 1, False, True
-  n.use_directional_enc = n.use_reflections = n.enable_pred_roughness = True
-  n.use_diffuse_color = n.use_specular_tint = n.use_n_dot_v = True
-  n.deg_view, n.bottleneck_width, n.density_bias, n.max_deg_point = 5, 64, 0.5, 16
-  return b
+  t = train_step(model, variables, bundle, rays, target, rand, 0.3)
+  close(t.stats['mses'], t.stats_o['mses'].detach(), atol=2e-3, rtol=3e-2, msg='mses')
+  lo = float(t.stats_o['loss'].detach())
+  assert abs(t.stats['loss'] - lo) < 3e-2 * max(1.0, abs(lo)), (t.stats['loss'], lo)
+  exposure = ('exposure_scaling_offsets', 'embedding')
+  report, zero = grad_report(model, t.grads_o, [exposure] + mlp_leaves(model, modules=['NerfMLP_0']))
+  assert not zero, zero
+  assert report.pop(exposure)[0] < 0.05
+  a = model.export_grads_flax()['exposure_scaling_offsets']['embedding']
+  assert float(np.abs(a.reshape(-1, 3)[0]).max()) == 0.0      # index 0 is pinned (mask = idx > 0)
+  assert not beyond(report, 0.15, 0.99), beyond(report, 0.15, 0.99)
 
 
 def test_refnerf_forward_and_train_step_vs_oracle(mods):
   """BASELINE config 3 (blender_refnerf.gin) at reduced size: IDE of reflected directions, predicted
   and density-gradient normals (forward-mode tangent chain), diffuse + tinted specular colour,
   n.v, 6-layer view MLP with a skip connection, orientation + predicted-normal losses."""
-  models, train_utils = mods
-  from multinerf_b200 import utils
+  models, _ = mods
   bundle = mini_refnerf()
   bundle.config.grad_max_norm = 0.0
   B, S = 96, 16
   rays, rng = synth_rays(7, B, 2.0, 6.0, unit_cube=False)
   target = rng.uniform(0, 1, (B, 3)).astype(np.float32)
   model, variables = models.construct_model(9, rays, bundle)
-  params0 = torch_tree(model.export_flax())
-  bases = {'nerf': model.plans['NerfMLP_0'].basis, 'prop': model.plans['NerfMLP_0'].basis}
-  rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, S)).astype(np.float32)) for _ in range(2)]}
-  orays = oracle_rays(rays)
-  # ---- forward (sample positions pinned to the oracle's per level)
-  rend_o, hist_o = o_models.model_apply(params0, bundle, bases, orays, 0.5, True, rand=rand, bf16=True)
-  rend_o = [{k: v.detach() for k, v in r.items()} for r in rend_o]
-  hist_o = [{k: (v.detach() if v is not None else None) for k, v in h.items()} for h in hist_o]
-  r = model._prep_rays(rays)
-  from multinerf_b200 import ops
-  states = model.forward_levels(rand, r, 0.5, True, True)
-  for i, st in enumerate(states):
-    st.sdist.copy_(hist_o[i]['sdist'].cuda())
-    model._mlp_forward(st, model.mlps[st.mname], r)
-    comp = ops.composite_fwd(st.raw_density, st.raw_rgb, st.sdist, r.directions, r.near_flat, r.far_flat,
-                             cfg=st.comp_cfg, raw_diffuse=st.heads.get('diffuse'), raw_tint=st.heads.get('tint'),
-                             want_samples=True, want_extras=True)
-    torch.cuda.synchronize()
-    err = (comp['density'].cpu() - hist_o[i]['density']).abs() / (1.0 + hist_o[i]['density'].abs())
-    assert float(err.max()) < 0.08 and float(err.mean()) < 4e-3, (i, float(err.max()), float(err.mean()))
-    close(st.normals_pred.cpu().view(B, S, 3), hist_o[i]['normals_pred'], atol=3e-2, rtol=0, msg='normals_pred')
+  rand = level_jitter(rng, bundle, B)
+
+  def normals(i, st, h):
+    close(st.normals_pred.cpu().view(B, S, 3), h['normals_pred'], atol=3e-2, rtol=0, msg='normals_pred')
     # density normals: bf16 tangent chain vs fp32 autograd of the bf16-emulated forward
-    cosn = (st.normals.cpu().view(B, S, 3) * hist_o[i]['normals']).sum(-1)
+    cosn = (st.normals.cpu().view(B, S, 3) * h['normals']).sum(-1)
     assert float((cosn > 0.98).float().mean()) > 0.97, float((cosn > 0.98).float().mean())
-    close(st.roughness.cpu().view(B, S, 1), hist_o[i]['roughness'], atol=2e-2, rtol=0, msg='roughness')
-    close(comp['rgb_samples'], hist_o[i]['rgb'], atol=4e-2, rtol=0, msg=f'rgb samples level {i}')
-    close(comp['rgb'], rend_o[i]['rgb'], atol=1.5e-2, rtol=0, msg=f'pixel level {i}')
+    close(st.roughness.cpu().view(B, S, 1), h['roughness'], atol=2e-2, rtol=0, msg='roughness')
+  rend_o, _ = pinned_forward(model, bundle, rays, rand, dens=(0.08, 4e-3), pixel=1.5e-2, samples=4e-2, level=normals)
   rend, hist = model(rand, rays, 0.5, True)
   for k in ['normals', 'normals_pred', 'roughness']:
     assert k in rend[-1] and hist[-1][k] is not None
   close(rend[-1]['rgb'], rend_o[-1]['rgb'], atol=3e-2, rtol=0, msg='final pixel end-to-end')
   # ---- one train step
-  opt0 = {'count': 0, 'mu': {}, 'nu': {}}
-  new_o, opt_o, stats_o, grads_o = o_train.train_step(params0, opt0, bundle, bases, orays, torch.tensor(target), 0.5,
-                                                      rand=rand, bf16=True)
-  step_fn = train_utils.create_train_step(model, bundle.config)
-  state = train_utils.TrainState(variables)
-  state, stats, _ = step_fn(rand, state, utils.Batch(rays=rays, rgb=target), None, 0.5)
-  torch.cuda.synchronize()
-  stats.materialize()
-  close(stats['mses'], stats_o['mses'].detach(), atol=2e-3, rtol=3e-2, msg='mses')
+  t = train_step(model, variables, bundle, rays, target, rand, 0.5)
+  close(t.stats['mses'], t.stats_o['mses'].detach(), atol=2e-3, rtol=3e-2, msg='mses')
   for k in ['orientation', 'predicted_normals']:
-    lo = float(stats_o['losses'][k].detach())
-    assert abs(stats['losses'][k] - lo) < 0.05 * abs(lo) + 1e-7, (k, stats['losses'][k], lo)
-  g = model.export_grads_flax()
-  report = {}
-  for lname in g['NerfMLP_0']:
-    a = torch.tensor(g['NerfMLP_0'][lname]['kernel']).double().flatten()
-    b = grads_o[('NerfMLP_0', lname, 'kernel')].double().flatten()
-    rel = float((a - b).norm() / b.norm().clamp(min=1e-12))
-    cos = float((a @ b) / (a.norm() * b.norm()).clamp(min=1e-30))
-    report[lname] = (round(rel, 3), round(cos, 4))
-  bad = {k: v for k, v in report.items() if not (v[0] < 0.2 and v[1] > 0.98)}
+    lo = float(t.stats_o['losses'][k].detach())
+    assert abs(t.stats['losses'][k] - lo) < 0.05 * abs(lo) + 1e-7, (k, t.stats['losses'][k], lo)
+  report, zero = grad_report(model, t.grads_o, mlp_leaves(model, modules=['NerfMLP_0']))
+  assert not zero, zero
+  bad = beyond(report, 0.2, 0.98)
   assert not bad, (bad, report)
 
 
 def test_weight_decay_random_background_and_bottleneck_noise(mods):
   """Smaller switches of the path: weight_decay_mults (train_utils.py:304-309), random background
   colours (models.py:240-254) and bottleneck noise (models.py:529-533) against the oracle."""
-  models, train_utils = mods
-  from multinerf_b200 import utils
+  models, _ = mods
   bundle = mini360()
   bundle.config.grad_max_norm = 0.0
   bundle.config.weight_decay_mults = {'NerfMLP_0': 1e-3, 'PropMLP_0/Dense_0': 1e-2}
@@ -444,37 +240,26 @@ def test_weight_decay_random_background_and_bottleneck_noise(mods):
   rays, rng = synth_rays(13, B, 0.2, 1e6)
   target = rng.uniform(0, 1, (B, 3)).astype(np.float32)
   model, variables = models.construct_model(14, rays, bundle)
-  params0 = torch_tree(model.export_flax())
-  bases = {'nerf': model.plans['NerfMLP_0'].basis, 'prop': model.plans['PropMLP_0'].basis}
   S = [32, 32, 16]
   rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, 1)).astype(np.float32)) for _ in S],
           'bg': [torch.tensor(rng.uniform(0, 1, (B, 3)).astype(np.float32)) for _ in S],
           'bottleneck_noise': [torch.tensor(rng.normal(size=(B, s, 64)).astype(np.float32)) for s in S]}
   # deterministic render: midpoint background
-  rend_o, _ = o_models.model_apply(params0, bundle, bases, oracle_rays(rays), 0.5, False, rand=None, bf16=True)
+  rend_o, _ = o_models.model_apply(torch_tree(model.export_flax()), bundle, bases(model), oracle_rays(rays), 0.5,
+                                   False, rand=None, bf16=True)
   rend, _ = model(None, rays, 0.5, False)
   close(rend[0]['rgb'], rend_o[0]['rgb'].detach(), atol=1e-2, rtol=0, msg='midpoint background')
-  opt0 = {'count': 0, 'mu': {}, 'nu': {}}
-  new_o, opt_o, stats_o, grads_o = o_train.train_step(params0, opt0, bundle, bases, oracle_rays(rays),
-                                                      torch.tensor(target), 0.5, rand=rand, bf16=True)
-  step_fn = train_utils.create_train_step(model, bundle.config, use_graph=True)   # falls back to eager
-  state = train_utils.TrainState(variables)
-  state, stats, _ = step_fn(rand, state, utils.Batch(rays=rays, rgb=target), None, 0.5)
-  torch.cuda.synchronize()
-  stats.materialize()
-  close(stats['mses'], stats_o['mses'].detach(), atol=3e-3, rtol=3e-2, msg='mses (random bg)')
-  g = model.export_grads_flax()
-  for mname, lname in [('NerfMLP_0', 'Dense_3'), ('PropMLP_0', 'Dense_0'), ('PropMLP_0', 'Dense_1')]:
-    a = torch.tensor(g[mname][lname]['kernel']).double().flatten()
-    b = grads_o[(mname, lname, 'kernel')].double().flatten()
-    assert float((a - b).norm() / b.norm()) < 0.15, (mname, lname, float((a - b).norm() / b.norm()))
+  t = train_step(model, variables, bundle, rays, target, rand, 0.5, use_graph=True)   # falls back to eager
+  close(t.stats['mses'], t.stats_o['mses'].detach(), atol=3e-3, rtol=3e-2, msg='mses (random bg)')
+  keys = [('NerfMLP_0', 'Dense_3', 'kernel'), ('PropMLP_0', 'Dense_0', 'kernel'), ('PropMLP_0', 'Dense_1', 'kernel')]
+  report, zero = grad_report(model, t.grads_o, keys)
+  assert not zero and all(rel < 0.15 for rel, _ in report.values()), (report, zero)
 
 
 def test_glo_embeddings_vs_oracle(mods):
   """configs/360_glo4.gin at reduced size: per-camera GLO vectors appended to the view-MLP input
   (models.py:101-110,565-569), their gradient scattered back into the embedding table."""
-  models, train_utils = mods
-  from multinerf_b200 import utils
+  models, _ = mods
   bundle = mini360()
   bundle.config.grad_max_norm = 0.0
   bundle.model.num_glo_features = 4
@@ -487,27 +272,17 @@ def test_glo_embeddings_vs_oracle(mods):
   params0 = torch_tree(model.export_flax())
   assert params0['Embed_0']['embedding'].shape == (16, 4)
   assert params0['NerfMLP_0']['Dense_8']['kernel'].shape[0] == 64 + 27 + 4
-  bases = {'nerf': model.plans['NerfMLP_0'].basis, 'prop': model.plans['PropMLP_0'].basis}
-  rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, 1)).astype(np.float32)) for _ in range(3)]}
+  rand = level_jitter(rng, bundle, B)
   orays = oracle_rays(rays)
-  orays.cam_idx = torch.tensor(rays.cam_idx)
   # zero_glo=True (construct/eval default) vs False
   for zero_glo in [True, False]:
-    rend_o, _ = o_models.model_apply(params0, bundle, bases, orays, 0.5, False, rand=rand, zero_glo=zero_glo, bf16=True)
+    rend_o, _ = o_models.model_apply(params0, bundle, bases(model), orays, 0.5, False, rand=rand, zero_glo=zero_glo,
+                                     bf16=True)
     rend, _ = model(rand, rays, 0.5, False, zero_glo=zero_glo)
     close(rend[-1]['rgb'], rend_o[-1]['rgb'].detach(), atol=2e-2, rtol=0, msg=f'pixel zero_glo={zero_glo}')
-  opt0 = {'count': 0, 'mu': {}, 'nu': {}}
-  new_o, opt_o, stats_o, grads_o = o_train.train_step(params0, opt0, bundle, bases, orays, torch.tensor(target), 0.5,
-                                                      rand=rand, bf16=True)
-  step_fn = train_utils.create_train_step(model, bundle.config)
-  state = train_utils.TrainState(variables)
-  state, stats, _ = step_fn(rand, state, utils.Batch(rays=rays, rgb=target), None, 0.5)
-  torch.cuda.synchronize()
-  g = model.export_grads_flax()
-  a = torch.tensor(g['Embed_0']['embedding']).double().flatten()
-  b = grads_o[('Embed_0', 'embedding')].double().flatten()
-  rel = float((a - b).norm() / b.norm())
-  assert float(b.norm()) > 0 and rel < 0.15, rel
+  t = train_step(model, variables, bundle, rays, target, rand, 0.5)
+  report, zero = grad_report(model, t.grads_o, [('Embed_0', 'embedding')])
+  assert not zero and report[('Embed_0', 'embedding')][0] < 0.15, (report, zero)
 
 
 def test_full_size_properties(mods):
@@ -679,8 +454,7 @@ def test_config_variants_vs_oracle(mods, name):
   """Model / Config switches away from the shipped 360.gin values, each against the oracle: rendered
   pixels and level-0 sample positions of a randomized forward pass, then loss, per-level MSEs and the
   direction of every layer's gradient for one train step."""
-  models, train_utils = mods
-  from multinerf_b200 import utils
+  models, _ = mods
   bundle = _variant(name)
   bundle.config.grad_max_norm = 0.0
   B = 96
@@ -688,42 +462,23 @@ def test_config_variants_vs_oracle(mods, name):
   rays, rng = synth_rays(31, B, near, far)
   target = rng.uniform(0, 1, (B, 3)).astype(np.float32)
   model, variables = models.construct_model(6, rays, bundle)
-  params0 = torch_tree(model.export_flax())
-  bases = {'nerf': model.plans['NerfMLP_0'].basis,
-           'prop': model.plans.get('PropMLP_0', model.plans['NerfMLP_0']).basis}
-  sched = model.level_schedule(0.5)[2]
-  width = lambda lv: 1 if bundle.model.single_jitter else lv['S']
-  rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, width(lv))).astype(np.float32)) for lv in sched]}
+  rand = level_jitter(rng, bundle, B)
   with torch.no_grad():
-    rend_o, hist_o = o_models.model_apply(params0, bundle, bases, oracle_rays(rays), 0.5, True, rand=rand, bf16=True)
+    rend_o, hist_o = o_models.model_apply(torch_tree(model.export_flax()), bundle, bases(model), oracle_rays(rays),
+                                          0.5, True, rand=rand, bf16=True)
   rend, hist = model(rand, rays, 0.5, True)
   torch.cuda.synchronize()
   assert len(rend) == bundle.model.num_levels
   close(hist[0]['sdist'], hist_o[0]['sdist'], atol=1e-6, rtol=1e-6, msg='level-0 sdist')
   close(rend[-1]['rgb'], rend_o[-1]['rgb'], atol=2e-2, rtol=0, msg='final pixel')
   close(rend[-1]['acc'], rend_o[-1]['acc'], atol=2e-2, rtol=0, msg='final acc')
-  opt0 = {'count': 0, 'mu': {}, 'nu': {}}
-  _, _, stats_o, grads_o = o_train.train_step(params0, opt0, bundle, bases, oracle_rays(rays), torch.tensor(target),
-                                              0.5, rand=rand, bf16=True)
-  step_fn = train_utils.create_train_step(model, bundle.config)
-  state = train_utils.TrainState(variables)
-  state, stats, _ = step_fn(rand, state, utils.Batch(rays=rays, rgb=target), None, 0.5)
-  torch.cuda.synchronize()
-  stats.materialize()
-  close(stats['mses'], stats_o['mses'].detach(), atol=2e-3, rtol=3e-2, msg='mses')
-  lo = float(stats_o['loss'].detach())
-  assert abs(stats['loss'] - lo) < 3e-2 * max(1.0, abs(lo)), (stats['loss'], lo)
-  g = model.export_grads_flax()
-  for mname in g:
-    for lname in g[mname]:
-      a = torch.tensor(g[mname][lname]['kernel']).double().flatten()
-      b = grads_o[(mname, lname, 'kernel')].double().flatten()
-      if float(b.norm()) == 0.0:
-        assert float(a.norm()) == 0.0, (mname, lname)
-        continue
-      cos = float((a @ b) / (a.norm() * b.norm()).clamp(min=1e-30))
-      rel = float((a - b).norm() / b.norm())
-      assert cos > 0.98 and rel < 0.25, (name, mname, lname, cos, rel)
+  t = train_step(model, variables, bundle, rays, target, rand, 0.5)
+  close(t.stats['mses'], t.stats_o['mses'].detach(), atol=2e-3, rtol=3e-2, msg='mses')
+  lo = float(t.stats_o['loss'].detach())
+  assert abs(t.stats['loss'] - lo) < 3e-2 * max(1.0, abs(lo)), (t.stats['loss'], lo)
+  report, zero = grad_report(model, t.grads_o, mlp_leaves(model))
+  assert not any(zero.values()), zero
+  assert not beyond(report, 0.25, 0.98), (name, beyond(report, 0.25, 0.98))
 
 
 def _refnerf_variant(name):
@@ -750,48 +505,28 @@ def _refnerf_variant(name):
 def test_refnerf_variants_vs_oracle(mods, name):
   """Ref-NeRF switches one at a time (models.py:473-604): which normals feed the reflection and the
   orientation loss, IDE vs plain PE of the (reflected) direction, the colour-composition terms."""
-  models, train_utils = mods
-  from multinerf_b200 import utils
+  models, _ = mods
   bundle = _refnerf_variant(name)
   bundle.config.grad_max_norm = 0.0
-  B, S = 96, 16
+  B = 96
   rays, rng = synth_rays(17, B, 2.0, 6.0, unit_cube=False)
   target = rng.uniform(0, 1, (B, 3)).astype(np.float32)
   model, variables = models.construct_model(5, rays, bundle)
-  params0 = torch_tree(model.export_flax())
-  bases = {'nerf': model.plans['NerfMLP_0'].basis, 'prop': model.plans['NerfMLP_0'].basis}
-  rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, S)).astype(np.float32)) for _ in range(2)]}
-  orays = oracle_rays(rays)
-  rend_o, hist_o = o_models.model_apply(params0, bundle, bases, orays, 0.5, True, rand=rand, bf16=True)
+  rand = level_jitter(rng, bundle, B)
+  rend_o, hist_o = o_models.model_apply(torch_tree(model.export_flax()), bundle, bases(model), oracle_rays(rays), 0.5,
+                                        True, rand=rand, bf16=True)
   rend, hist = model(rand, rays, 0.5, True)
   torch.cuda.synchronize()
   close(rend[-1]['rgb'], rend_o[-1]['rgb'].detach(), atol=3e-2, rtol=0, msg='final pixel')
-  opt0 = {'count': 0, 'mu': {}, 'nu': {}}
-  _, _, stats_o, grads_o = o_train.train_step(params0, opt0, bundle, bases, orays, torch.tensor(target), 0.5,
-                                              rand=rand, bf16=True)
-  step_fn = train_utils.create_train_step(model, bundle.config)
-  state = train_utils.TrainState(variables)
-  state, stats, _ = step_fn(rand, state, utils.Batch(rays=rays, rgb=target), None, 0.5)
-  torch.cuda.synchronize()
-  stats.materialize()
-  close(stats['mses'], stats_o['mses'].detach(), atol=2e-3, rtol=3e-2, msg='mses')
-  lo = float(stats_o['losses']['orientation'].detach())
-  assert abs(stats['losses']['orientation'] - lo) < 0.05 * abs(lo) + 1e-7, (stats['losses']['orientation'], lo)
-  g = model.export_grads_flax()
-  bad = {}
-  for lname in g['NerfMLP_0']:
-    a = torch.tensor(g['NerfMLP_0'][lname]['kernel']).double().flatten()
-    b = grads_o[('NerfMLP_0', lname, 'kernel')].double().flatten()
-    if float(b.norm()) == 0.0:
-      assert float(a.norm()) == 0.0, lname
-      continue
-    rel = float((a - b).norm() / b.norm())
-    cos = float((a @ b) / (a.norm() * b.norm()).clamp(min=1e-30))
-    # with density-gradient normals alone, every colour gradient reaches the first layers through the
-    # bf16 forward-mode tangent streams as well: measured 0.24 / 0.971 on Dense_0
-    lim_rel, lim_cos = (0.3, 0.96) if name == 'density_normals_only' else (0.25, 0.98)
-    if not (rel < lim_rel and cos > lim_cos):
-      bad[lname] = (round(rel, 3), round(cos, 4))
+  t = train_step(model, variables, bundle, rays, target, rand, 0.5)
+  close(t.stats['mses'], t.stats_o['mses'].detach(), atol=2e-3, rtol=3e-2, msg='mses')
+  lo = float(t.stats_o['losses']['orientation'].detach())
+  assert abs(t.stats['losses']['orientation'] - lo) < 0.05 * abs(lo) + 1e-7, (t.stats['losses']['orientation'], lo)
+  report, zero = grad_report(model, t.grads_o, mlp_leaves(model, modules=['NerfMLP_0']))
+  assert not any(zero.values()), zero
+  # with density-gradient normals alone, every colour gradient reaches the first layers through the
+  # bf16 forward-mode tangent streams as well: measured 0.24 / 0.971 on Dense_0
+  bad = beyond(report, 0.3, 0.96) if name == 'density_normals_only' else beyond(report, 0.25, 0.98)
   assert not bad, bad
   if name == 'reflections_with_plain_pe':
     broken = _refnerf_variant(name)
@@ -801,34 +536,24 @@ def test_refnerf_variants_vs_oracle(mods, name):
 
 
 def _family(name, rng, B):
-  """(bundle, rays, per-level jitter width) of a reduced-size model family with per-step varying inputs."""
-  from multinerf_b200 import configs, utils
-  f = np.float32
+  """(bundle, rays) of a reduced-size model family with per-step varying inputs."""
+  from multinerf_b200 import configs
   if name == 'rawnerf':
     bundle = configs.bundle_llff_raw()
     bundle.model.num_prop_samples = bundle.model.num_nerf_samples = 32
     bundle.nerf_mlp.net_width, bundle.nerf_mlp.bottleneck_width, bundle.nerf_mlp.net_width_viewdirs = 128, 64, 64
     bundle.nerf_mlp.density_noise = 0.0           # the graph path refreshes jitter only from a generator or dict
-    o = np.concatenate([rng.uniform(-1, 1, (B, 2)), -np.ones((B, 1))], -1)
-    d = np.concatenate([rng.uniform(-.5, .5, (B, 2)), 2 * np.ones((B, 1))], -1)
-    eidx = rng.integers(0, 4, (B, 1)).astype(np.int32)
-    rays = utils.Rays(origins=o.astype(f), directions=d.astype(f),
-                      viewdirs=(d / np.linalg.norm(d, axis=-1, keepdims=True)).astype(f),
-                      radii=rng.uniform(1e-3, 2e-3, (B, 1)).astype(f), imageplane=np.zeros((B, 2), f),
-                      lossmult=np.eye(3, dtype=f)[rng.integers(0, 3, B)], near=np.zeros((B, 1), f),
-                      far=np.ones((B, 1), f), cam_idx=np.zeros((B, 1), np.int32), exposure_idx=eidx,
-                      exposure_values=(2.0 ** -eidx).astype(f))
-    return bundle, rays, [32, 32]
+    return bundle, raw_rays(rng, B, radii_first=True)
   if name == 'refnerf':
     bundle = mini_refnerf()
     rays, _ = synth_rays(int(rng.integers(1 << 30)), B, 2.0, 6.0, unit_cube=False)
-    return bundle, rays, [16, 16]
+    return bundle, rays
   if name == 'glo':
     bundle = mini360()
     bundle.model.num_glo_features, bundle.model.num_glo_embeddings = 4, 16
     rays, _ = synth_rays(int(rng.integers(1 << 30)), B, 0.2, 1e6)
     rays.cam_idx = rng.integers(0, 16, (B, 1)).astype(np.int32)
-    return bundle, rays, [1, 1, 1]
+    return bundle, rays
   raise KeyError(name)
 
 
@@ -838,28 +563,11 @@ def test_cuda_graph_matches_eager_other_families(mods, family):
   Ref-NeRF tangent chain and reflection stage): five steps with changing rays, targets, jitter,
   train_frac and learning rate track the eager run."""
   models, train_utils = mods
-  from multinerf_b200 import utils
   B, steps = 192, 5
   rng = np.random.default_rng(77)
   batches = []
   for _ in range(steps):
-    bundle, rays, widths = _family(family, rng, B)
-    rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, w)).astype(np.float32)) for w in widths]}
+    bundle, rays = _family(family, rng, B)
+    rand = level_jitter(rng, bundle, B)
     batches.append((rays, rng.uniform(0, 1, (B, 3)).astype(np.float32), rand))
-  results = []
-  for use_graph in [False, True]:
-    model, variables = models.construct_model(6, batches[0][0], bundle)
-    step_fn = train_utils.create_train_step(model, bundle.config, use_graph=use_graph)
-    state = train_utils.TrainState(variables)
-    losses = []
-    for i, (rays, tgt, rand) in enumerate(batches):
-      state, stats, _ = step_fn(rand, state, utils.Batch(rays=rays, rgb=tgt), None, i / 10.0)
-      losses.append(stats.materialize()['loss'])
-    torch.cuda.synchronize()
-    results.append((losses, variables.flat.clone()))
-    if use_graph:
-      assert step_fn.graph_info['state'] == 2, step_fn.graph_info['state']
-  (l0, p0), (l1, p1) = results
-  for a, b in zip(l0, l1):
-    assert abs(a - b) < 2e-3 * max(1.0, abs(a)), (l0, l1)
-  assert float((p0 - p1).norm() / p0.norm()) < 2e-3
+  graph_matches_eager(models, train_utils, bundle, batches, 6)

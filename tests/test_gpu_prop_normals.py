@@ -9,9 +9,10 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import o_models, o_train
+from model_parity import (bases, check_train_step, graph_matches_eager, image_rays, oracle_rays, pinned_forward,
+                          synth_case, synth_rays, torch_tree)
+from oracle import o_models
 from util import close
-from test_gpu_model import oracle_rays, synth_rays, torch_tree
 
 pytestmark = pytest.mark.gpu
 
@@ -56,43 +57,21 @@ def fullwidth_normals(pred=False):
   return b
 
 
-def _bases(model):
-  return {'nerf': model.plans['NerfMLP_0'].basis, 'prop': model.plans['PropMLP_0'].basis}
-
-
 def _forward_vs_oracle(models, bundle, B, seed, dens_lim, pix_atol):
-  from multinerf_b200 import ops
-  rays, rng = synth_rays(seed, B, 2.0, 6.0, unit_cube=False)
+  rays, rand, _ = synth_case(bundle, B, seed, 2.0, 6.0, unit_cube=False)
   S = [bundle.model.num_prop_samples] * (bundle.model.num_levels - 1) + [bundle.model.num_nerf_samples]
-  rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, 1 if bundle.model.single_jitter else s)).astype(np.float32))
-                     for s in S]}
   model, _ = models.construct_model(seed + 1, rays, bundle)
-  params = torch_tree(model.export_flax())
-  rend_o, hist_o = o_models.model_apply(params, bundle, _bases(model), oracle_rays(rays), 0.5, True, rand=rand,
-                                        bf16=True)
-  rend_o = [{k: v.detach() for k, v in r.items()} for r in rend_o]
-  hist_o = [{k: (v.detach() if v is not None else None) for k, v in h.items()} for h in hist_o]
-  r = model._prep_rays(rays)
   pred = bundle.prop_mlp.enable_pred_normals
-  for i, st in enumerate(model.forward_levels(rand, r, 0.5, True, True)):
-    # sample positions of level i pinned to the oracle's: one level's MLP and normals stage in isolation
-    st.sdist.copy_(hist_o[i]['sdist'].cuda())
-    model._mlp_forward(st, model.mlps[st.mname], r)
-    comp = ops.composite_fwd(st.raw_density, st.raw_rgb, st.sdist, r.directions, r.near_flat, r.far_flat,
-                             cfg=st.comp_cfg, raw_diffuse=st.heads.get('diffuse'), raw_tint=st.heads.get('tint'),
-                             want_samples=True, want_extras=True)
-    torch.cuda.synchronize()
-    Sx = st.S
-    err = (comp['density'].cpu() - hist_o[i]['density']).abs() / (1.0 + hist_o[i]['density'].abs())
-    assert float(err.max()) < dens_lim[0] and float(err.mean()) < dens_lim[1], (i, float(err.max()), float(err.mean()))
-    close(comp['weights'], hist_o[i]['weights'], atol=2e-2, rtol=0, msg=f'weights level {i}')
-    close(comp['rgb'], rend_o[i]['rgb'], atol=pix_atol, rtol=0, msg=f'pixel level {i}')
+
+  def normals(i, st, h):
     # density normals: bf16 tangent chain vs fp32 autograd of the bf16-emulated forward (Ref-NeRF test's bound)
-    cosn = (st.normals.cpu().view(B, Sx, 3) * hist_o[i]['normals']).sum(-1)
+    cosn = (st.normals.cpu().view(B, st.S, 3) * h['normals']).sum(-1)
     assert float((cosn > 0.98).float().mean()) > 0.97, (i, float((cosn > 0.98).float().mean()))
     if pred:
-      cosp = (st.normals_pred.cpu().view(B, Sx, 3) * hist_o[i]['normals_pred']).sum(-1)
+      cosp = (st.normals_pred.cpu().view(B, st.S, 3) * h['normals_pred']).sum(-1)
       assert float((cosp > 0.98).float().mean()) > 0.97, (i, float((cosp > 0.98).float().mean()))
+  # sample positions of each level pinned to the oracle's: one level's MLP and normals stage in isolation
+  rend_o, _ = pinned_forward(model, bundle, rays, rand, dens=dens_lim, pixel=pix_atol, level=normals)
   rend, hist = model(rand, rays, 0.5, True)
   torch.cuda.synchronize()
   keys = ('normals', 'normals_pred') if pred else ('normals',)
@@ -103,52 +82,6 @@ def _forward_vs_oracle(models, bundle, B, seed, dens_lim, pix_atol):
     assert hist[i]['raw_grad_density'].shape == (B, S[i], 3)
     assert (hist[i]['grad_pred'] is not None) == pred
   close(rend[-1]['rgb'], rend_o[-1]['rgb'], atol=3e-2, rtol=0, msg='final pixel end-to-end')
-
-
-def _grad_report(model, grads_o, leaves=('kernel',)):
-  g = model.export_grads_flax()
-  report = {}
-  for mname, plan in model.plans.items():
-    for sp in plan.specs:
-      for leaf in leaves:
-        a = torch.tensor(g[mname][sp.name][leaf]).double().flatten()
-        b = grads_o[(mname, sp.name, leaf)].double().flatten()
-        if float(b.norm()) == 0.0:
-          assert float(a.norm()) == 0.0, (mname, sp.name, leaf)
-          continue
-        report[(mname, sp.name, leaf)] = (round(float((a - b).norm() / b.norm()), 3),
-                                          round(float((a @ b) / (a.norm() * b.norm()).clamp(min=1e-30)), 4))
-  return report
-
-
-def _train_step_vs_oracle(models, train_utils, bundle, B, seed, lim):
-  from multinerf_b200 import utils
-  rays, rng = synth_rays(seed, B, 2.0, 6.0, unit_cube=False)
-  S = [bundle.model.num_prop_samples] * (bundle.model.num_levels - 1) + [bundle.model.num_nerf_samples]
-  rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, 1 if bundle.model.single_jitter else s)).astype(np.float32))
-                     for s in S]}
-  target = rng.uniform(0, 1, (B, 3)).astype(np.float32)
-  model, variables = models.construct_model(seed + 1, rays, bundle)
-  params0 = torch_tree(model.export_flax())
-  opt0 = {'count': 0, 'mu': {}, 'nu': {}}
-  _, _, stats_o, grads_o = o_train.train_step(params0, opt0, bundle, _bases(model), oracle_rays(rays),
-                                              torch.tensor(target), 0.5, rand=rand, bf16=True)
-  step_fn = train_utils.create_train_step(model, bundle.config)
-  state = train_utils.TrainState(variables)
-  state, stats, _ = step_fn(rand, state, utils.Batch(rays=rays, rgb=target), None, 0.5)
-  torch.cuda.synchronize()
-  stats.materialize()
-  close(stats['mses'], stats_o['mses'].detach(), atol=2e-3, rtol=3e-2, msg='mses')
-  for k in ('orientation', 'predicted_normals'):
-    if k in stats_o['losses']:
-      lo = float(stats_o['losses'][k].detach())
-      assert abs(stats['losses'][k] - lo) < 0.05 * abs(lo) + 1e-7, (k, stats['losses'][k], lo)
-  report = _grad_report(model, grads_o)
-  assert any(k[0] == 'PropMLP_0' for k in report) and any(k[0] == 'NerfMLP_0' for k in report)
-  worst = sorted(report.items(), key=lambda kv: -kv[1][0])[:6]
-  print(f'worst leaves (rel, cos): {worst}')
-  bad = {k: v for k, v in report.items() if not (v[0] < lim[0] and v[1] > lim[1])}
-  assert not bad, (bad, worst)
 
 
 def test_construction_and_flax_tree(mods):
@@ -170,7 +103,7 @@ def test_construction_and_flax_tree(mods):
       assert names[-1] == f'Dense_{depth}'
     # the oracle's flax-style MLP consumes exactly this tree (a missing or extra Dense raises there)
     rays, _ = synth_rays(0, 4, 2.0, 6.0, unit_cube=False)
-    o_models.model_apply(torch_tree(tree), bundle, _bases(model), oracle_rays(rays), 0.5, False)
+    o_models.model_apply(torch_tree(tree), bundle, bases(model), oracle_rays(rays), 0.5, False)
   # PropMLP: grad_pred adds one Dense(3) on the 256-wide trunk output
   shipped = models.Model(configs.bundle_blender_256()).num_params()
   b = configs.bundle_blender_256()
@@ -190,7 +123,7 @@ def test_train_step_vs_oracle(mods, target):
   # the PropMLP's gradient then comes from the normal losses alone: the new stage, its adjoint and the tangent
   # adjoint are not hidden behind the interlevel loss
   bundle.config.interlevel_loss_mult = 0.0
-  _train_step_vs_oracle(models, train_utils, bundle, 96, 60, (0.2, 0.98))
+  check_train_step(models, train_utils, bundle, 96, 60, (0.2, 0.98))
 
 
 def test_fullwidth_forward_vs_oracle(mods):
@@ -202,13 +135,11 @@ def test_fullwidth_forward_vs_oracle(mods):
 def test_fullwidth_train_step_vs_oracle(mods, pred):
   # pred: the 256-wide PropMLP's trunk-top dgrad against [w_density | W_grad_pred] feeds the chained dgrad launch
   models, train_utils = mods
-  _train_step_vs_oracle(models, train_utils, fullwidth_normals(pred), 128, 80, (0.3, 0.95))
+  check_train_step(models, train_utils, fullwidth_normals(pred), 128, 80, (0.3, 0.95))
 
 
 def test_cuda_graph_matches_eager(mods):
   models, train_utils = mods
-  from multinerf_b200 import utils
-  bundle = mini_prop_normals()
   B, steps = 192, 5
   rng = np.random.default_rng(91)
   batches = []
@@ -216,25 +147,8 @@ def test_cuda_graph_matches_eager(mods):
     rays, _ = synth_rays(int(rng.integers(1 << 30)), B, 2.0, 6.0, unit_cube=False)
     rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B,)).astype(np.float32)) for _ in range(2)]}
     batches.append((rays, rng.uniform(0, 1, (B, 3)).astype(np.float32), rand))
-  results = []
-  for use_graph in [False, True]:
-    model, variables = models.construct_model(6, batches[0][0], bundle)
-    step_fn = train_utils.create_train_step(model, bundle.config, use_graph=use_graph)
-    state = train_utils.TrainState(variables)
-    losses, orient = [], []
-    for i, (rays, tgt, rand) in enumerate(batches):
-      state, stats, _ = step_fn(rand, state, utils.Batch(rays=rays, rgb=tgt), None, i / 10.0)
-      s = stats.materialize()
-      losses.append(s['loss'])
-      orient.append(s['losses']['orientation'])
-    torch.cuda.synchronize()
-    results.append((losses, orient, variables.flat.clone()))
-    if use_graph:
-      assert step_fn.graph_info['state'] == 2, step_fn.graph_info['state']
-  (l0, o0, p0), (l1, o1, p1) = results
-  for a, b in zip(l0 + o0, l1 + o1):
-    assert abs(a - b) < 2e-3 * max(1.0, abs(a)), (l0, l1, o0, o1)
-  assert float((p0 - p1).norm() / p0.norm()) < 2e-3
+  graph_matches_eager(models, train_utils, mini_prop_normals(), batches, 6,
+                      extra=lambda stats: stats['losses']['orientation'])
 
 
 def test_render_image_normals_chunked_equals_direct_call(mods):
@@ -242,13 +156,12 @@ def test_render_image_normals_chunked_equals_direct_call(mods):
   bit for bit.  The PropMLP is 256 wide with predicted normals only, so its trunk runs as one chained launch
   that must still store the last layer's output for the grad_pred head."""
   models, train_utils = mods
-  from test_gpu_render import _image_rays
   bundle = mini_prop_normals()
   bundle.prop_mlp.net_width, bundle.prop_mlp.disable_density_normals = 256, True
   H, W = 29, 41
   bundle.config.render_chunk_size = 256
   bundle.config.vis_num_rays = 8
-  rays = _image_rays(H, W, focal=40.0)
+  rays = image_rays(H, W, focal=40.0)
   rays.origins[...] = np.array([0.0, 0.0, 4.0], np.float32)
   rays.near[...], rays.far[...] = 2.0, 6.0
   model, state, render_eval_pfn, _, _ = train_utils.setup_model(bundle, 3)
@@ -265,7 +178,7 @@ def test_render_image_normals_chunked_equals_direct_call(mods):
     assert torch.equal(out[k].reshape(rend[-1][k].shape), rend[-1][k]), k
   # the proposal level's normals against the oracle's (deterministic call)
   params = torch_tree(model.export_flax())
-  rend_o, hist_o = o_models.model_apply(params, bundle, _bases(model), oracle_rays(flat), 1.0, True, rand=None,
+  rend_o, hist_o = o_models.model_apply(params, bundle, bases(model), oracle_rays(flat), 1.0, True, rand=None,
                                         bf16=True)
   cosp = (hist[0]['normals_pred'].cpu() * hist_o[0]['normals_pred']).sum(-1)
   assert float((cosp > 0.98).float().mean()) > 0.97, float((cosp > 0.98).float().mean())

@@ -2,28 +2,14 @@
 train_utils.py:377-396 render_eval_pfn): a chunked image render must equal one direct
 Model.__call__ on the same rays, keep the reference's output keys/shapes, and agree with the oracle.
 Needs an H100.  The N-GPU all-gather variant is tools/render_check.py (needs torchrun)."""
-import numpy as np
 import pytest
 import torch
 
+from model_parity import bases, image_rays, mini360, oracle_rays, torch_tree
 from oracle import o_models
 from util import close
-from test_gpu_model import mini360, oracle_rays, torch_tree
 
 pytestmark = pytest.mark.gpu
-
-
-def _image_rays(H, W, focal=120.0):
-  from multinerf_b200 import utils
-  f = np.float32
-  ys, xs = np.meshgrid(np.arange(H), np.arange(W), indexing='ij')
-  d = np.stack([(xs - W / 2) / focal, (ys - H / 2) / focal, -np.ones_like(xs, dtype=np.float64)], -1)
-  v = d / np.linalg.norm(d, axis=-1, keepdims=True)
-  o = np.broadcast_to(np.array([0.5, 0.5, 0.3]), d.shape)
-  return utils.Rays(origins=o.astype(f), directions=d.astype(f), viewdirs=v.astype(f),
-                    radii=np.full((H, W, 1), 7e-4, f), imageplane=np.zeros((H, W, 2), f),
-                    lossmult=np.ones((H, W, 1), f), near=np.full((H, W, 1), 0.2, f),
-                    far=np.full((H, W, 1), 1e6, f), cam_idx=np.zeros((H, W, 1), np.int32))
 
 
 @pytest.mark.parametrize('which', ['mini360', 'full360'])
@@ -34,7 +20,7 @@ def test_render_image_equals_direct_call(which):
   H, W = (37, 53) if which == 'mini360' else (48, 64)          # 1961 rays: ragged last chunk | 3072 rays
   bundle.config.render_chunk_size = 512 if which == 'mini360' else 1024
   bundle.config.vis_num_rays = 8
-  rays = _image_rays(H, W)
+  rays = image_rays(H, W)
   model, state, render_eval_pfn, _, _ = train_utils.setup_model(bundle, 3)
   render_fn = lambda rng, r: render_eval_pfn(state.params, 1.0, None, r)
   out = models.render_image(render_fn, rays, None, bundle, verbose=False)
@@ -67,14 +53,13 @@ def test_render_image_vs_oracle():
   bundle = mini360()
   H, W = 12, 20
   bundle.config.render_chunk_size = 100
-  rays = _image_rays(H, W, focal=30.0)
+  rays = image_rays(H, W, focal=30.0)
   model, state, render_eval_pfn, _, _ = train_utils.setup_model(bundle, 5)
   out = models.render_image(lambda rng, r: render_eval_pfn(state.params, 1.0, None, r), rays, None, bundle,
                             verbose=False)
-  params = torch_tree(model.export_flax())
-  bases = {'nerf': model.plans['NerfMLP_0'].basis, 'prop': model.plans['PropMLP_0'].basis}
   flat = rays.map(lambda a: a.reshape(H * W, -1))
   with torch.no_grad():
-    rend_o, _ = o_models.model_apply(params, bundle, bases, oracle_rays(flat), 1.0, True, rand=None, bf16=True)
+    rend_o, _ = o_models.model_apply(torch_tree(model.export_flax()), bundle, bases(model), oracle_rays(flat), 1.0,
+                                     True, rand=None, bf16=True)
   close(out['rgb'].reshape(H * W, 3), rend_o[-1]['rgb'], atol=2e-2, rtol=0, msg='rendered image vs oracle')
   close(out['acc'].reshape(H * W), rend_o[-1]['acc'], atol=2e-2, rtol=0, msg='acc vs oracle')

@@ -6,10 +6,11 @@ import numpy as np
 import pytest
 import torch
 
+from composite_ref import CFG, oracle_composite
+from model_parity import (bases, beyond, grad_report, mini360, mlp_leaves, oracle_rays, synth_rays, torch_tree,
+                          train_loop_bundle, train_step)
 from oracle import o_robust, o_train
-from util import close, golden
-from test_gpu_kernels import CFG, _oracle_composite, _rays
-from test_gpu_model import mini360, oracle_rays, synth_rays, torch_tree
+from util import close, golden, kernel_rays
 
 pytestmark = pytest.mark.gpu
 
@@ -162,7 +163,7 @@ def test_masked_composite_bwd(mods, S):
   rng = np.random.default_rng(5 + S)
   B = 96
   cfg = dict(CFG)
-  _, d, _ = _rays(rng, B)
+  _, d, _ = kernel_rays(rng, B)
   s = torch.tensor(np.sort(rng.uniform(0, 1, (B, S + 1)).astype(np.float32), -1))
   s[:, 0], s[:, -1] = 0, 1
   raw_d = torch.tensor(rng.normal(size=(B, S)).astype(np.float32) * 2, requires_grad=True)
@@ -171,7 +172,7 @@ def test_masked_composite_bwd(mods, S):
   target = torch.tensor(rng.uniform(0, 1, (B, 3)).astype(np.float32))
   mask = torch.tensor((rng.uniform(size=B) < 0.6).astype(np.float32))
   # oracle: resid_sq * mask with the mask a constant (train_utils.py:104-111), distortion on top
-  w_o, r_o, _, _ = _oracle_composite(raw_d, raw_rgb, s, d, nearv, farv, cfg)
+  w_o, r_o, _, _ = oracle_composite(raw_d, raw_rgb, s, d, nearv, farv, cfg)
   resid_sq = (r_o['rgb'] - target) ** 2
   data = (resid_sq * mask[:, None]).sum() / (3 * B)
   extra = 0.01 * o_train.o_stepfun.lossfun_distortion(s, w_o).mean()
@@ -209,11 +210,9 @@ def _robust_bundle(p=8, inner=4):
 
 def _oracle_errors(bundle, model, rays, target, rand, train_frac):
   from oracle import o_models
-  params = torch_tree(model.export_flax())
-  bases = {'nerf': model.plans['NerfMLP_0'].basis, 'prop': model.plans['PropMLP_0'].basis}
   with torch.no_grad():
-    rend, _ = o_models.model_apply(params, bundle, bases, oracle_rays(rays), train_frac, False, rand=rand,
-                                   zero_glo=False, bf16=True)
+    rend, _ = o_models.model_apply(torch_tree(model.export_flax()), bundle, bases(model), oracle_rays(rays),
+                                   train_frac, False, rand=rand, zero_glo=False, bf16=True)
   return ((rend[-1]['rgb'] - torch.tensor(target)) ** 2).mean(-1)
 
 
@@ -227,42 +226,19 @@ def _gap_threshold(err, lo_q, hi_q):
   return float(np.float32(np.sqrt(e[k] * e[k + 1])))
 
 
-def _grad_report(model, grads_o):
-  g = model.export_grads_flax()
-  for mname in g:
-    for lname in g[mname]:
-      for leaf in ['kernel', 'bias']:
-        a = torch.tensor(g[mname][lname][leaf]).double().flatten()
-        b = grads_o[(mname, lname, leaf)].double().flatten()
-        if float(b.norm()) == 0.0:
-          assert float(a.norm()) == 0.0, (mname, lname, leaf)
-          continue
-        yield (mname, lname, leaf), float((a - b).norm() / b.norm().clamp(min=1e-12)), \
-            float((a @ b) / (a.norm() * b.norm()).clamp(min=1e-30))
-
-
 def test_mini_train_step_vs_oracle(mods):
   models, _, train_utils = mods
-  from multinerf_b200 import utils
   bundle = _robust_bundle()
   bundle.config.grad_max_norm = 0.0
   B = 4 * 64                                     # 4 patches of 8 x 8
   rays, rng = synth_rays(13, B, 0.2, 1e6)
   target = rng.uniform(0, 1, (B, 3)).astype(np.float32)
   model, variables = models.construct_model(14, rays, bundle)
-  params0 = torch_tree(model.export_flax())
-  bases = {'nerf': model.plans['NerfMLP_0'].basis, 'prop': model.plans['PropMLP_0'].basis}
   rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, 1)).astype(np.float32)) for _ in range(3)]}
   thr = _gap_threshold(_oracle_errors(bundle, model, rays, target, rand, 0.5), 0.3, 0.6)
-  new_o, _, stats_o, grads_o = o_robust.train_step(params0, {'count': 0, 'mu': {}, 'nu': {}}, bundle, bases,
-                                                   oracle_rays(rays), torch.tensor(target), 0.5, rand=rand,
-                                                   bf16=True, loss_threshold=thr)
+  t = train_step(model, variables, bundle, rays, target, rand, 0.5, oracle=o_robust.train_step, loss_threshold=thr)
+  stats, stats_o = t.stats, t.stats_o
   assert 0.1 < float(stats_o['mask']) < 0.9, float(stats_o['mask'])
-  step_fn = train_utils.create_train_step(model, bundle.config)
-  state = train_utils.TrainState(variables)
-  state, stats, _ = step_fn(rand, state, utils.Batch(rays=rays, rgb=target), None, 0.5, thr)
-  torch.cuda.synchronize()
-  stats.materialize()
   for k in train_utils.ROBUST_STAT_NAMES:
     tol = 0.02 if k == 'loss_threshold' else 0.01
     assert abs(stats[k] - float(stats_o[k])) <= tol * max(abs(float(stats_o[k])), 1e-3), \
@@ -270,8 +246,9 @@ def test_mini_train_step_vs_oracle(mods):
   close(stats['mses'], stats_o['mses'].detach(), atol=2e-3, rtol=2e-2, msg='mses')
   lo = float(stats_o['loss'].detach())
   assert abs(stats['loss'] - lo) < 2e-2 * max(1.0, abs(lo)), (stats['loss'], lo)
-  for key, rel, cos in _grad_report(model, grads_o):
-    assert rel < 0.12 and cos > 0.993, (key, rel, cos)
+  report, zero = grad_report(model, t.grads_o, mlp_leaves(model, ('kernel', 'bias')))
+  assert not any(zero.values()), zero
+  assert not beyond(report, 0.12, 0.993), beyond(report, 0.12, 0.993)
 
 
 def test_graph_replay_with_device_threshold_tracks_eager(mods):
@@ -353,35 +330,27 @@ def test_fullwidth_360_robustnerf_step_vs_oracle(mods):
   target = rng.uniform(0, 1, (B, 3)).astype(np.float32)
   rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, 1)).astype(np.float32)) for _ in range(3)]}
   model, variables = models.construct_model(52, rays, bundle)
-  params0 = torch_tree(model.export_flax())
-  bases = {'nerf': model.plans['NerfMLP_0'].basis, 'prop': model.plans['PropMLP_0'].basis}
   thr = _gap_threshold(_oracle_errors(bundle, model, rays, target, rand, 0.5), 0.3, 0.6)
-  _, _, stats_o, grads_o = o_robust.train_step(params0, {'count': 0, 'mu': {}, 'nu': {}}, bundle, bases,
-                                               oracle_rays(rays), torch.tensor(target), 0.5, rand=rand, bf16=True,
-                                               loss_threshold=thr)
+  t = train_step(model, variables, bundle, rays, target, rand, 0.5, oracle=o_robust.train_step, loss_threshold=thr)
+  stats, stats_o = t.stats, t.stats_o
   assert 0.1 < float(stats_o['mask']) < 0.9, float(stats_o['mask'])
-  step_fn = train_utils.create_train_step(model, c)
-  state = train_utils.TrainState(variables)
-  state, stats, _ = step_fn(rand, state, utils.Batch(rays=rays, rgb=target), None, 0.5, thr)
-  torch.cuda.synchronize()
-  stats.materialize()
   close(stats['mses'], stats_o['mses'].detach(), atol=1e-6, rtol=2e-3, msg='mses')
   lo = float(stats_o['loss'].detach())
   assert abs(stats['loss'] - lo) < 3e-3 * max(1.0, abs(lo)), (stats['loss'], lo)
   assert abs(stats['mask'] - float(stats_o['mask'])) < 0.01, (stats['mask'], float(stats_o['mask']))
+  report, zero = grad_report(model, t.grads_o, mlp_leaves(model, ('kernel', 'bias')))
+  assert not any(zero.values()), zero
   # a head's bias gradient is a plain sum that cancels to nearly nothing (test_gpu_fullwidth.py measures it
   # against its kernel's scale): trunk leaves and kernels are held to the 360.gin bound
   head = {(m, sp.name) for m in model.plans for sp in model.plans[m].specs if sp.out_dim <= 4}
-  bad = {k: (rel, cos) for k, rel, cos in _grad_report(model, grads_o)
-         if not (rel < 0.2 and cos > 0.98) and not (k[2] == 'bias' and k[:2] in head)}
+  bad = {k: v for k, v in beyond(report, 0.2, 0.98).items() if not (k[2] == 'bias' and k[:2] in head)}
   assert not bad, bad
 
 
 def test_train_loop_feeds_threshold_back_and_logs_robust_stats(mods, monkeypatch):
   _, _, train_utils = mods
   from multinerf_b200 import train_loop
-  from test_gpu_train_loop import _bundle
-  b = _bundle(6, cast=True)
+  b = train_loop_bundle(6, cast=True)
   c = b.config
   c.data_loss_type, c.patch_size, c.enable_robustnerf_loss = 'robustnerf', 16, True
   c.robustnerf_inlier_quantile, c.print_every = 0.8, 3

@@ -15,8 +15,7 @@ import pytest
 import torch
 
 from oracle import o_spherical
-from test_spherical_cpu import POSES, SIZES, write_nerfpp_scene
-from util import golden
+from util import POSES, SIZES, golden, write_nerfpp_scene
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -8,24 +8,15 @@ import numpy as np
 import pytest
 import torch
 
+from model_parity import plumbing_blender, train_loop_bundle
+
 pytestmark = pytest.mark.gpu
-
-
-def _bundle(steps, ckpt=None, cast=False):
-  from test_gpu_model import mini360
-  b = mini360()
-  c = b.config
-  c.batch_size, c.max_steps, c.print_every = 2048, steps, 20
-  c.lr_init, c.lr_final, c.lr_delay_steps = 5e-3, 5e-4, 20
-  c.checkpoint_every, c.checkpoint_dir = 60, ckpt
-  c.cast_rays_in_train_step = cast
-  return b
 
 
 def test_training_reduces_loss_and_logs_reference_fields():
   from multinerf_b200 import train_loop
   lines = []
-  b = _bundle(160, cast=True)
+  b = train_loop_bundle(160, cast=True)
   model, state, hist = train_loop.train(b, train_loop.SyntheticScene(b.config), log=lines.append)
   assert state.step == 160 and hist[-1]['step'] == 160
   first, last = hist[0], hist[-1]
@@ -43,15 +34,15 @@ def test_checkpoint_resume(tmp_path):
   from multinerf_b200 import checkpoints, train_loop
   ck = str(tmp_path / 'ckpt')
   # uninterrupted: 120 steps
-  b = _bundle(120)
+  b = train_loop_bundle(120)
   model_a, state_a, _ = train_loop.train(b, train_loop.SyntheticScene(b.config, seed=3), log=lambda s: None)
   # interrupted at 60 (checkpoint_every), then resumed to 120 with a dataset continuing the same stream
-  b1 = _bundle(120, ckpt=ck)
+  b1 = train_loop_bundle(120, ckpt=ck)
   b1.config.early_exit_steps = 60
   ds = train_loop.SyntheticScene(b1.config, seed=3)
   train_loop.train(b1, ds, log=lambda s: None)
   assert checkpoints.latest_checkpoint(ck).endswith('checkpoint_60')
-  b2 = _bundle(120, ckpt=ck)
+  b2 = train_loop_bundle(120, ckpt=ck)
   model_b, state_b, hist_b = train_loop.train(b2, ds, log=lambda s: None)
   assert state_b.step == 120 and hist_b[0]['step'] == 61
   pa, pb = state_a.params.flat, state_b.params.flat
@@ -62,7 +53,6 @@ def test_checkpoint_resume(tmp_path):
   assert blob['step'] == 120 and set(blob['params_tree']) == {'NerfMLP_0', 'PropMLP_0'}
   assert blob['params_tree']['NerfMLP_0']['Dense_0']['kernel'].shape[1] == 128
   with pytest.raises(ValueError):
-    from test_gpu_model import plumbing_blender
     from multinerf_b200 import train_utils
     other = plumbing_blender()
     m2, st2, *_ = train_utils.setup_model(other, 0)

@@ -8,10 +8,10 @@ import numpy as np
 import pytest
 import torch
 
+from model_parity import (bases, check_train_step, graph_matches_eager, oracle_rays, pinned_forward, synth_case,
+                          synth_rays, torch_tree)
 from oracle import o_models
 from util import close
-from test_gpu_model import oracle_rays, synth_rays, torch_tree
-from test_gpu_prop_normals import _train_step_vs_oracle
 
 pytestmark = pytest.mark.gpu
 
@@ -52,46 +52,19 @@ def fullwidth_view_independent(name):
   return b
 
 
-def _rays_for(bundle, seed, B):
-  if bundle.model.raydist_fn is None or bundle.config.far < 100:
-    return synth_rays(seed, B, 2.0, 6.0, unit_cube=False)
-  return synth_rays(seed, B, 0.2, 1e6)
-
-
-def _bases(model):
-  return {'nerf': model.plans['NerfMLP_0'].basis, 'prop': model.plans['PropMLP_0'].basis}
-
-
 def _forward_vs_oracle(models, bundle, B, seed, dens_lim, pix_atol):
-  from multinerf_b200 import ops
-  rays, rng = _rays_for(bundle, seed, B)
-  S = [bundle.model.num_prop_samples] * (bundle.model.num_levels - 1) + [bundle.model.num_nerf_samples]
-  rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B, 1 if bundle.model.single_jitter else s)).astype(np.float32))
-                     for s in S]}
+  if bundle.model.raydist_fn is None or bundle.config.far < 100:
+    rays, rand, _ = synth_case(bundle, B, seed, 2.0, 6.0, unit_cube=False)
+  else:
+    rays, rand, _ = synth_case(bundle, B, seed, 0.2, 1e6)
   model, _ = models.construct_model(seed + 1, rays, bundle)
   assert model.plans['NerfMLP_0'].rgb_on_trunk
-  params = torch_tree(model.export_flax())
-  rend_o, hist_o = o_models.model_apply(params, bundle, _bases(model), oracle_rays(rays), 0.5, True, rand=rand,
-                                        bf16=True)
-  hist_o = [{k: (v.detach() if v is not None else None) for k, v in h.items()} for h in hist_o]
-  r = model._prep_rays(rays)
-  for i, st in enumerate(model.forward_levels(rand, r, 0.5, True, True)):
-    # sample positions pinned to the oracle's: each level's MLP and heads in isolation
-    st.sdist.copy_(hist_o[i]['sdist'].cuda())
-    model._mlp_forward(st, model.mlps[st.mname], r)
-    comp = ops.composite_fwd(st.raw_density, st.raw_rgb, st.sdist, r.directions, r.near_flat, r.far_flat,
-                             cfg=st.comp_cfg, want_samples=True, want_extras=True)
-    torch.cuda.synchronize()
-    err = (comp['density'].cpu() - hist_o[i]['density']).abs() / (1.0 + hist_o[i]['density'].abs())
-    assert float(err.max()) < dens_lim[0] and float(err.mean()) < dens_lim[1], (i, float(err.max()), float(err.mean()))
-    close(comp['weights'], hist_o[i]['weights'], atol=2e-2, rtol=0, msg=f'weights level {i}')
-    if st.raw_rgb is not None:
-      close(comp['rgb_samples'], hist_o[i]['rgb'], atol=pix_atol, rtol=0, msg=f'sample colours level {i}')
-    close(comp['rgb'], rend_o[i]['rgb'].detach(), atol=pix_atol, rtol=0, msg=f'pixel level {i}')
+  # sample positions pinned to the oracle's: each level's MLP and heads in isolation
+  rend_o, _ = pinned_forward(model, bundle, rays, rand, dens=dens_lim, pixel=pix_atol, samples=pix_atol)
   rend, hist = model(rand, rays, 0.5, True)
   torch.cuda.synchronize()
   assert all('roughness' not in r_ for r_ in rend)
-  close(rend[-1]['rgb'], rend_o[-1]['rgb'].detach(), atol=3e-2, rtol=0, msg='final pixel end-to-end')
+  close(rend[-1]['rgb'], rend_o[-1]['rgb'], atol=3e-2, rtol=0, msg='final pixel end-to-end')
   return model
 
 
@@ -116,7 +89,7 @@ def test_construction_and_flax_tree(mods):
       for k, v in tree[mname].items():
         assert np.array_equal(v['kernel'], t2[mname][k]['kernel']) and np.array_equal(v['bias'], t2[mname][k]['bias'])
     rays, _ = synth_rays(0, 4, 2.0, 6.0, unit_cube=False)
-    o_models.model_apply(torch_tree(tree), bundle, _bases(model), oracle_rays(rays), 0.5, False)
+    o_models.model_apply(torch_tree(tree), bundle, bases(model), oracle_rays(rays), 0.5, False)
 
 
 @pytest.mark.parametrize('normals', [False, True])
@@ -129,7 +102,7 @@ def test_forward_vs_oracle(mods, normals):
 def test_train_step_vs_oracle(mods, normals):
   models, train_utils = mods
   bundle = mini_view_independent(normals)
-  _train_step_vs_oracle(models, train_utils, bundle, 96, 20, (0.2, 0.98))
+  check_train_step(models, train_utils, bundle, 96, 20, (0.2, 0.98))
   # GLO vectors feed no layer without view directions: their gradient is zero, as in the reference
   model, variables = models.construct_model(3, synth_rays(0, 8, 2.0, 6.0, unit_cube=False)[0], bundle)
   from multinerf_b200 import utils
@@ -157,7 +130,7 @@ def test_fullwidth_train_step_vs_oracle(mods, name):
   # stacked mnrf_head_fwd / mnrf_head_bwd at K = 1024.  Bounds of the shipped full-width train-step tests.
   models, train_utils = mods
   lim = (0.3, 0.95) if name == 'blender_256' else (0.2, 0.98)
-  _train_step_vs_oracle(models, train_utils, fullwidth_view_independent(name), 128, 40, lim)
+  check_train_step(models, train_utils, fullwidth_view_independent(name), 128, 40, lim)
 
 
 def test_colourless_trunk_ending_on_skip_train_step_vs_oracle(mods):
@@ -167,7 +140,7 @@ def test_colourless_trunk_ending_on_skip_train_step_vs_oracle(mods):
   bundle = mini_view_independent(normals=False, glo=False)
   bundle.prop_mlp.net_depth = 5
   assert models.MLPPlan(bundle.prop_mlp).last_has_feat
-  _train_step_vs_oracle(models, train_utils, bundle, 96, 25, (0.2, 0.98))
+  check_train_step(models, train_utils, bundle, 96, 25, (0.2, 0.98))
 
 
 def test_chained_trunk_matches_per_layer(mods, monkeypatch):
@@ -202,8 +175,6 @@ def test_chained_trunk_matches_per_layer(mods, monkeypatch):
 
 def test_cuda_graph_matches_eager(mods):
   models, train_utils = mods
-  from multinerf_b200 import utils
-  bundle = mini_view_independent()
   B, steps = 192, 5
   rng = np.random.default_rng(33)
   batches = []
@@ -211,23 +182,7 @@ def test_cuda_graph_matches_eager(mods):
     rays, _ = synth_rays(int(rng.integers(1 << 30)), B, 2.0, 6.0, unit_cube=False)
     rand = {'jitter': [torch.tensor(rng.uniform(0, 1, (B,)).astype(np.float32)) for _ in range(2)]}
     batches.append((rays, rng.uniform(0, 1, (B, 3)).astype(np.float32), rand))
-  results = []
-  for use_graph in [False, True]:
-    model, variables = models.construct_model(6, batches[0][0], bundle)
-    step_fn = train_utils.create_train_step(model, bundle.config, use_graph=use_graph)
-    state = train_utils.TrainState(variables)
-    losses = []
-    for i, (rays, tgt, rand) in enumerate(batches):
-      state, stats, _ = step_fn(rand, state, utils.Batch(rays=rays, rgb=tgt), None, i / 10.0)
-      losses.append(stats.materialize()['loss'])
-    torch.cuda.synchronize()
-    results.append((losses, variables.flat.clone()))
-    if use_graph:
-      assert step_fn.graph_info['state'] == 2, step_fn.graph_info['state']
-  (l0, p0), (l1, p1) = results
-  for a, b in zip(l0, l1):
-    assert abs(a - b) < 2e-3 * max(1.0, abs(a)), (l0, l1)
-  assert float((p0 - p1).norm() / p0.norm()) < 2e-3
+  graph_matches_eager(models, train_utils, mini_view_independent(), batches, 6)
 
 
 @pytest.mark.parametrize('M', [512, 1000, 16384])

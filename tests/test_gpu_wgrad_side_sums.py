@@ -93,7 +93,7 @@ def test_model_bias_gradients_are_column_sums_of_stored_dy(ops, monkeypatch):
   """One backward of every level of the full-width 360.gin model: the bias gradient of each trunk layer and of the
   bottleneck is the fp64 column sum of the bf16 dY its weight-gradient GEMM reads."""
   from multinerf_b200 import configs, models
-  from test_gpu_model import synth_rays
+  from model_parity import synth_rays
   bundle = configs.bundle_360()
   B = 256
   rays, _ = synth_rays(3, B, 0.2, 1e6)

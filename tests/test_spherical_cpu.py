@@ -11,12 +11,10 @@ import pytest
 import torch
 
 from oracle import o_spherical
-from util import golden
+from util import POSES, SIZES, golden, write_nerfpp_scene
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 G = golden('spherical')
-SIZES = [tuple(int(v) for v in s) for s in G['sizes']]
-POSES = ['rot', 'rot_f32', 'skew']
 
 
 @pytest.mark.parametrize('pose', POSES)
@@ -72,27 +70,6 @@ def test_cast_spherical_rays_rejects_bad_sizes_before_any_launch():
       camera_utils.cast_spherical_rays(pose, h, w, 0.2, 1e6)
   with pytest.raises(ValueError, match=r'\[3, 4\] or \[4, 4\]'):
     camera_utils.cast_spherical_rays(pose[:, :3], 4, 8, 0.2, 1e6)
-
-
-def write_nerfpp_scene(root, rng, n_train=3, n_test=2, n_path=4, height=6, width=10):
-  """A scene in NeRF++'s layout (datasets.py:720-764): <split>/{pose,intrinsics}/*.txt and, outside
-  camera_path/, <split>/rgb/*.png.  Poses are random rotations and positions."""
-  from PIL import Image
-  for split, n in (('train', n_train), ('test', n_test), ('camera_path', n_path)):
-    for i in range(n):
-      m = np.eye(4)
-      m[:3, :3] = np.linalg.qr(rng.normal(size=(3, 3)))[0]
-      m[:3, 3] = rng.normal(size=3)
-      K = np.eye(4)
-      K[0, 0] = K[1, 1] = 37.5
-      K[0, 2], K[1, 2] = width / 2, height / 2
-      for d, mat in (('pose', m), ('intrinsics', K)):
-        os.makedirs(os.path.join(root, split, d), exist_ok=True)
-        np.savetxt(os.path.join(root, split, d, f'{i:03d}.txt'), mat.reshape(1, 16))
-      if split != 'camera_path':
-        os.makedirs(os.path.join(root, split, 'rgb'), exist_ok=True)
-        img = rng.integers(0, 256, (height, width, 3), dtype=np.uint8)
-        Image.fromarray(img).save(os.path.join(root, split, 'rgb', f'{i:03d}.png'))
 
 
 def test_pano_render_path_dataset_constructs(tmp_path):

@@ -7,8 +7,8 @@ import torch
 
 from multinerf_b200 import configs
 from multinerf_b200.models import MLPPlan
+from model_golden import TOL, load, rand_of
 from oracle import o_models, o_train
-from test_oracle_model_golden import TOL, load, rand_of
 from util import close
 
 TAG = 'miniviewindep'

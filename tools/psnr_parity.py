@@ -1,6 +1,6 @@
 """Per-level PSNR of one train step, CUDA path vs the CPU oracle, on identical rays, weights and random draws
 (BASELINE.json: "PSNR parity"; SURVEY.md 8d asks for the agreement of train.py's printed PSNRs).  Runs the three
-BASELINE model families at their stated widths (the cases of tests/test_gpu_fullwidth.py) and prints what is measured.
+BASELINE model families at their stated widths (tests/model_parity.py `fullwidth_case`) and prints what is measured.
 
   python tools/psnr_parity.py            # needs an H100
 """
@@ -14,35 +14,25 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, 'tests'))
-from oracle import o_train                                   # noqa: E402  (test infrastructure: the checker)
-from test_gpu_fullwidth import _case                         # noqa: E402
-from test_gpu_model import oracle_rays, torch_tree           # noqa: E402
+from model_parity import fullwidth_case, train_step              # noqa: E402  (test infrastructure: the checker)
 
 
 def main():
-  from multinerf_b200 import lib, models, train_utils, utils
+  from multinerf_b200 import lib, models
   lib.require_device()
   print('# per-level PSNR = -10 log10(mse) of one train step (image.py:28-30, train_utils.py:337-338): CUDA path vs oracle')
   print('# (oracle = torch-CPU restatement with bf16-rounded weights and layer inputs, fp32 accumulate), identical rays,')
   print('# weights, jitter and noise draws; 360.gin on 256 rays, blender_refnerf.gin and llff_raw.gin on 128 rays')
   for which in ('360', 'refnerf', 'raw'):
-    bundle, rays, target, rand, B, S = _case(which)
+    bundle, rays, target, rand, B, S = fullwidth_case(which)
     model, variables = models.construct_model(41, rays, bundle)
     if which == 'raw':
       tree = model.export_flax()
       tree['exposure_scaling_offsets']['embedding'] = \
           np.random.default_rng(6).normal(size=(1000, 3)).astype(np.float32) * 0.1
       variables = model.init(flax_params=tree)
-    params0 = torch_tree(model.export_flax())
-    bases = {'nerf': model.plans['NerfMLP_0'].basis,
-             'prop': model.plans.get('PropMLP_0', model.plans['NerfMLP_0']).basis}
-    _, _, stats_o, _ = o_train.train_step(params0, {'count': 0, 'mu': {}, 'nu': {}}, bundle, bases, oracle_rays(rays),
-                                          torch.tensor(target), 0.5, rand=rand, bf16=True)
-    step_fn = train_utils.create_train_step(model, bundle.config)
-    state = train_utils.TrainState(variables)
-    state, stats, _ = step_fn(rand, state, utils.Batch(rays=rays, rgb=target), None, 0.5)
-    torch.cuda.synchronize()
-    stats.materialize()
+    t = train_step(model, variables, bundle, rays, target, rand, 0.5)
+    stats, stats_o = t.stats, t.stats_o
     mo = stats_o['mses'].detach().double()
     mk = stats['mses'].double()
     po = -10.0 / math.log(10.0) * torch.log(mo)
