@@ -238,13 +238,16 @@ int mnrf_mlp_chain_max_layers(void);
  * dw [K, dw_split], outputs [dw_split, n_out) to dw2 [K, n_out - dw_split] (the density and rgb heads
  * of a view-independent model run as one stacked head; their weights live apart).  dx_cols (0: K) limits dX and
  * dxsum to the first dx_cols columns (a head reading [hidden | features] needs the gradient of the hidden part only).
+ * dx2 (optional, needs dx_cols < K): dx2[M, K - dx_cols] (bf16, row pitch lddx2) receives the input gradient of
+ * columns [dx_cols, K), never relu-masked and not summed into dxsum -- the rgb head of a view MLP that ends on a
+ * skip layer reads [hidden | view input], and the second part is its contribution to the view input's gradient.
  */
 int mnrf_head_fwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx,
                   const mnrf_bf16* w, const float* b, float* raw, mnrf_stream stream);
 int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx,
                   const mnrf_bf16* w, const float* draw, mnrf_bf16* dx, int64_t lddx,
                   int32_t relu_mask, float* dw, float* dw2, int32_t dw_split, float* db, float* dxsum,
-                  int32_t dx_cols, mnrf_stream stream);
+                  int32_t dx_cols, mnrf_bf16* dx2, int64_t lddx2, mnrf_stream stream);
 
 /* Column sums of a bf16 matrix into fp32 (bias gradients): out[N] += sum_m x[m, :]. */
 int mnrf_colsum(int64_t m, int32_t n, const mnrf_bf16* x, int64_t ldx, float* out,

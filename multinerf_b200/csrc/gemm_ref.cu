@@ -135,7 +135,8 @@ extern "C" int mnrf_gemm_wgrad(const mnrf_gemm_desc* d, const mnrf_bf16* a, cons
   if (bsum)
     if (int rc = mnrf_colsum(d->k, d->n, b, d->ldb, bsum, stream)) return rc;
   if (side_aw)      // side_aw[m] += sum_r side_w[r] * A[r, m]  ==  the dW of a Dense(1) head on A with draw = side_w
-    if (int rc = mnrf_head_bwd(d->k, (int32_t)d->m, 1, a, d->lda, a, side_w, nullptr, 0, 0, side_aw, nullptr, 0, nullptr, nullptr, 0, stream))
+    if (int rc = mnrf_head_bwd(d->k, (int32_t)d->m, 1, a, d->lda, a, side_w, nullptr, 0, 0, side_aw, nullptr, 0,
+                               nullptr, nullptr, 0, nullptr, 0, stream))
       return rc;
   return 0;
 }

@@ -55,14 +55,16 @@ __device__ __forceinline__ float* dw_at(float* dw, float* dw2, int split, int n_
   return o < split ? dw + (size_t)k * split + o : dw2 + (size_t)k * (n_out - split) + (o - split);
 }
 
-// dx[m,k] = relu'(x[m,k]) * sum_o draw[m,o] w[o,k];  dw[k,o] += sum_m draw[m,o] x[m,k];  db[o] += sum_m draw[m,o]
+// dx[m,k] = relu'(x[m,k]) * sum_o draw[m,o] w[o,k] for k < dx_cols;  dx2[m,k-dx_cols] = sum_o draw[m,o] w[o,k] for
+// k >= dx_cols (optional);  dw[k,o] += sum_m draw[m,o] x[m,k];  db[o] += sum_m draw[m,o]
 template <int N_OUT, int kMaxChunks>
 __global__ void __launch_bounds__(256)
 head_bwd_kernel(int64_t M, int K, const __nv_bfloat16* __restrict__ x, int64_t ldx,
                 const __nv_bfloat16* __restrict__ w, const float* __restrict__ draw,
                 __nv_bfloat16* __restrict__ dx, int64_t lddx, int relu_mask,
                 float* __restrict__ dw, float* __restrict__ dw2, int dw_split, float* __restrict__ db,
-                float* __restrict__ dxsum, int dx_cols, int64_t rows_per_block) {
+                float* __restrict__ dxsum, int dx_cols, __nv_bfloat16* __restrict__ dx2, int64_t lddx2,
+                int64_t rows_per_block) {
   extern __shared__ __align__(16) unsigned char smraw[];
   constexpr int n_out = N_OUT;
   float* sdw = reinterpret_cast<float*>(smraw);                                   // [n_out][K] fp32
@@ -95,6 +97,7 @@ head_bwd_kernel(int64_t M, int K, const __nv_bfloat16* __restrict__ x, int64_t l
     for (int o = 0; o < N_OUT; ++o) g[o] = draw[m * n_out + o];
     const uint4* xr = reinterpret_cast<const uint4*>(x + m * ldx);
     uint4* dxr = dx ? reinterpret_cast<uint4*>(dx + m * lddx) : nullptr;
+    __nv_bfloat16* dx2r = dx2 ? dx2 + m * lddx2 : nullptr;
 #pragma unroll
     for (int q = 0; q < kMaxChunks; ++q) {
       int c = lane + 32 * q;
@@ -129,6 +132,12 @@ head_bwd_kernel(int64_t M, int K, const __nv_bfloat16* __restrict__ x, int64_t l
           o4.x = pack_bf16(de[0], de[1]); o4.y = pack_bf16(de[2], de[3]);
           o4.z = pack_bf16(de[4], de[5]); o4.w = pack_bf16(de[6], de[7]);
           dxr[c] = o4;
+        } else if (dx2r && c * 8 >= dx_cols) {
+          // columns past dx_cols: unmasked, not summed (the input tail a skip concatenation appended)
+          uint4 o4;
+          o4.x = pack_bf16(de[0], de[1]); o4.y = pack_bf16(de[2], de[3]);
+          o4.z = pack_bf16(de[4], de[5]); o4.w = pack_bf16(de[6], de[7]);
+          reinterpret_cast<uint4*>(dx2r + (c * 8 - dx_cols))[0] = o4;
         }
       }
     }
@@ -236,7 +245,8 @@ head_bwd_sub_kernel(int64_t M, const __nv_bfloat16* __restrict__ x, int64_t ldx,
                     const __nv_bfloat16* __restrict__ w, const float* __restrict__ draw,
                     __nv_bfloat16* __restrict__ dx, int64_t lddx, int relu_mask,
                     float* __restrict__ dw, float* __restrict__ dw2, int dw_split, float* __restrict__ db,
-                    float* __restrict__ dxsum, int dx_cols, int64_t rows_per_block) {
+                    float* __restrict__ dxsum, int dx_cols, __nv_bfloat16* __restrict__ dx2, int64_t lddx2,
+                    int64_t rows_per_block) {
   constexpr int K = LPR * 8, RW = 32 / LPR;
   __shared__ float sdw[N_OUT * K];
   __shared__ float sxs[K];
@@ -304,6 +314,11 @@ head_bwd_sub_kernel(int64_t M, const __nv_bfloat16* __restrict__ x, int64_t ldx,
         o4.x = pack_bf16(de[0], de[1]); o4.y = pack_bf16(de[2], de[3]);
         o4.z = pack_bf16(de[4], de[5]); o4.w = pack_bf16(de[6], de[7]);
         reinterpret_cast<uint4*>(dx + row * lddx)[c] = o4;
+      } else if (dx2 && row < m_end && c * 8 >= dx_cols) {
+        uint4 o4;
+        o4.x = pack_bf16(de[0], de[1]); o4.y = pack_bf16(de[2], de[3]);
+        o4.z = pack_bf16(de[4], de[5]); o4.w = pack_bf16(de[6], de[7]);
+        reinterpret_cast<uint4*>(dx2 + row * lddx2 + (c * 8 - dx_cols))[0] = o4;
       }
     }
   }
@@ -492,7 +507,7 @@ extern "C" int mnrf_head_fwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf1
 extern "C" int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx,
                              const mnrf_bf16* w, const float* draw, mnrf_bf16* dx, int64_t lddx,
                              int32_t relu_mask, float* dw, float* dw2, int32_t dw_split, float* db, float* dxsum,
-                             int32_t dx_cols, mnrf_stream stream) {
+                             int32_t dx_cols, mnrf_bf16* dx2, int64_t lddx2, mnrf_stream stream) {
   using namespace mnrf;
   if (m == 0) return 0;
   MNRF_CHECK(x && w && draw, "mnrf_head_bwd: null pointer");
@@ -503,6 +518,8 @@ extern "C" int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf1
   if (dw_split <= 0 || dw_split >= n_out) dw_split = n_out;
   if (dx_cols <= 0) dx_cols = k;
   MNRF_CHECK(dx_cols <= k && dx_cols % 8 == 0, "mnrf_head_bwd: dx_cols must be a multiple of 8 and <= K");
+  MNRF_CHECK(!dx2 || (dx_cols < k && lddx2 % 8 == 0 && ((uintptr_t)dx2 % 16) == 0),
+             "mnrf_head_bwd: dx2 needs dx_cols < K, a pitch that is a multiple of 8 and a 16-byte aligned pointer");
   MNRF_CHECK(dw_split == n_out || (dw && dw2), "mnrf_head_bwd: a split weight gradient needs dw and dw2");
   if (m == 0) return 0;
   if ((k == 256 || k == 128 || k == 64) && ((uintptr_t)w % 16) == 0) {
@@ -514,7 +531,8 @@ extern "C" int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf1
 #define MNRF_HBS(NO, LPR_)                                                                              \
   head_bwd_sub_kernel<NO, LPR_, 4><<<blocks_s, 256, 0, (cudaStream_t)stream>>>(                         \
       m, reinterpret_cast<const __nv_bfloat16*>(x), ldx, reinterpret_cast<const __nv_bfloat16*>(w), draw, \
-      reinterpret_cast<__nv_bfloat16*>(dx), lddx, relu_mask, dw, dw2, dw_split, db, dxsum, dx_cols, rpb_s)
+      reinterpret_cast<__nv_bfloat16*>(dx), lddx, relu_mask, dw, dw2, dw_split, db, dxsum, dx_cols,      \
+      reinterpret_cast<__nv_bfloat16*>(dx2), lddx2, rpb_s)
 #define MNRF_HBS_N(NO) do { if (k == 256) MNRF_HBS(NO, 32); else if (k == 128) MNRF_HBS(NO, 16); else MNRF_HBS(NO, 8); } while (0)
     switch (n_out) {
       case 1: MNRF_HBS_N(1); break;
@@ -533,7 +551,8 @@ extern "C" int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf1
 #define MNRF_HB(NO, CK)                                                                         \
   head_bwd_kernel<NO, CK><<<blocks, 256, smem, (cudaStream_t)stream>>>(                         \
       m, k, reinterpret_cast<const __nv_bfloat16*>(x), ldx, reinterpret_cast<const __nv_bfloat16*>(w), \
-      draw, reinterpret_cast<__nv_bfloat16*>(dx), lddx, relu_mask, dw, dw2, dw_split, db, dxsum, dx_cols, rpb)
+      draw, reinterpret_cast<__nv_bfloat16*>(dx), lddx, relu_mask, dw, dw2, dw_split, db, dxsum, dx_cols, \
+      reinterpret_cast<__nv_bfloat16*>(dx2), lddx2, rpb)
 #define MNRF_HB_N(NO)                                      \
   do {                                                     \
     if (chunks <= 1) MNRF_HB(NO, 1);                       \

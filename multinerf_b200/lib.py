@@ -135,7 +135,7 @@ _SIGNATURES = {
     'mnrf_mlp_chain_max_layers': (C.c_int, []),
     'mnrf_head_fwd': (C.c_int, [C.c_int64, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P, _P, _P]),
     'mnrf_head_bwd': (C.c_int, [C.c_int64, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P, _P,
-                                C.c_int64, C.c_int32, _P, _P, C.c_int32, _P, _P, C.c_int32, _P]),
+                                C.c_int64, C.c_int32, _P, _P, C.c_int32, _P, _P, C.c_int32, _P, C.c_int64, _P]),
     'mnrf_colsum': (C.c_int, [C.c_int64, C.c_int32, _P, C.c_int64, _P, _P]),
     'mnrf_composite_fwd': (C.c_int, [C.POINTER(CompositeDesc)] + [_P] * 18),
     'mnrf_composite_bwd': (C.c_int, [C.POINTER(LossDesc)] + [_P] * 24),

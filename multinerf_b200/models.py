@@ -105,7 +105,8 @@ class MLPPlan:
     # predicted-normal losses and the renderings through the colourless normals stage (csrc/refnerf.cu normals_*)
     self.top = ('view' if use_viewdirs else 'stacked') if self.has_rgb else 'density'
     self.head_n = 4 if self.top == 'stacked' else 1
-    self.ref_stage = False
+    self.ref_stage = self.has_bottleneck = False
+    self.enc_col0, self.view_skips, self.rgb_vin, self.vin_partials = 0, [], None, 0
     if self.top == 'stacked':
       if cfg.use_diffuse_color:
         raise ValueError('use_viewdirs=False with use_diffuse_color: the reference reads raw_rgb_diffuse, which it '
@@ -120,7 +121,6 @@ class MLPPlan:
         if glo_features > 0:
           raise ValueError('bottleneck_width = 0 with num_glo_features > 0: the reference reads bottleneck.shape to '
                            'broadcast the GLO vector (internal/models.py:567-568)')
-        raise NotImplementedError('bottleneck_width == 0 is not supported (models.py:536-554)')
       if cfg.use_diffuse_color:
         add('diffuse', x_dim, x_pad, 3, True, rm=rmx)
       if cfg.use_specular_tint:
@@ -134,9 +134,13 @@ class MLPPlan:
         # reference either (ref_utils.py:141-148); every shipped config pairs IDE with reflections
         raise ValueError('use_directional_enc needs use_reflections (per-sample roughness cannot attenuate '
                          'the encoding of a per-ray view direction)')
-      bw = cfg.bottleneck_width
-      self.device_constraints.append(('bottleneck_width', bw))
-      add('bottleneck', x_dim, x_pad, bw, False, L.ACT_NONE, rmx)
+      # without a bottleneck (the Ref-NeRF ablation, models.py:526-537) the view input starts with the encoding
+      bw = max(cfg.bottleneck_width, 0)
+      self.has_bottleneck = bw > 0
+      if self.has_bottleneck:
+        self.device_constraints.append(('bottleneck_width', bw))
+        add('bottleneck', x_dim, x_pad, bw, False, L.ACT_NONE, rmx)
+      self.enc_col0 = bw        # first column of the direction encoding (and of the head gradients in the slab)
       self.ref_stage = (self.pred_normals or self.density_normals or cfg.use_reflections or
                         cfg.use_directional_enc or cfg.use_n_dot_v)
       if cfg.use_directional_enc:
@@ -153,7 +157,7 @@ class MLPPlan:
       Wv = cfg.net_width_viewdirs
       self.device_constraints.append(('net_width_viewdirs', Wv))
       v_dim, v_pad, v_has_in = vin, vin_pad, False
-      self.view_concat_after = []
+      self.view_concat_after = []     # view layers whose output is concatenated with vin
       for i in range(cfg.net_depth_viewdirs):
         rmv = np.concatenate([np.arange(Wv), Wv + np.arange(vin)]) if v_has_in else None
         add('view', v_dim, v_pad, Wv, False, L.ACT_RELU, rmv)
@@ -162,13 +166,18 @@ class MLPPlan:
           v_dim, v_pad, v_has_in = Wv + vin, Wv + vin_pad, True
         else:
           v_dim, v_pad, v_has_in = Wv, Wv, False
-      if len(self.view_concat_after) > 1:
-        raise NotImplementedError('more than one skip connection inside the view MLP')
       rmv = np.concatenate([np.arange(Wv), Wv + np.arange(vin)]) if v_has_in else None
-      if cfg.net_depth_viewdirs == 0:
-        raise NotImplementedError('net_depth_viewdirs == 0')
       add('rgb', v_dim, v_pad, cfg.num_rgb_channels, True, rm=rmv)
-      # columns of d vin the first view layer's dgrad writes: the Ref-NeRF stage and GLO read past the bottleneck
+      # The consumers of vin besides view layer 0, each one contribution to d vin: the view layers after a skip
+      # (`view_skips`, they read [hidden | vin]) and the rgb head, which reads [hidden | vin] when the view MLP ends
+      # on a skip ('tail') or vin itself without a view MLP ('all', models.py:575-585).
+      nv = cfg.net_depth_viewdirs
+      self.view_skips = [i + 1 for i in self.view_concat_after if i + 1 < nv]
+      self.rgb_vin = 'all' if nv == 0 else ('tail' if v_has_in else None)
+      # d vin summed before view layer 0's dgrad adds the last part: ping-pong buffers of the running sum
+      self.vin_partials = len(self.view_skips) + (self.rgb_vin == 'tail')
+      # columns of d vin the first view layer's dgrad (or the rgb head over vin) writes: the Ref-NeRF stage and GLO
+      # read past the bottleneck
       self.d_vin_cols = vin_pad if (self.ref_stage or glo_features > 0) else bw
     off = 0
     for sp in specs:
@@ -194,7 +203,7 @@ class MLPPlan:
     # 0] in the colourless normals stage with predicted normals, no slab otherwise.  `slab_heads` are the
     # (head, first slab column) pairs; a view-independent rgb head takes the diffuse slot (it has no diffuse head).
     if self.ref_stage:
-      self.slab_cols, c0, slots = self.vin_pad, self.cfg.bottleneck_width, self.HEAD_SLOTS
+      self.slab_cols, c0, slots = self.vin_pad, self.enc_col0, self.HEAD_SLOTS
     else:
       self.slab_cols = 64 if (self.normals_stage and self.pred_normals) else 0
       c0, slots = 0, dict(self.HEAD_SLOTS, rgb=self.HEAD_SLOTS['diffuse'])
@@ -267,7 +276,7 @@ class MLPDevice:
     plan = self.plan
     ops.pack_weights_batched(self._pack_table)
     self.colv_head.copy_(self.w_head)
-    if plan.ref_stage:
+    if plan.ref_stage and plan.has_bottleneck:
       bt = plan.one('bottleneck')
       self.wcat_kn[:, :bt.out_dim] = self.w_kn[bt.name]
     for sp, c0 in plan.slab_heads:
@@ -289,7 +298,7 @@ class LevelState:
     self.raw_head = self.d_raw_head = self.raw_density = self.d_raw_density = self.raw_rgb = self.d_raw_rgb = None
     self.heads, self.d_heads = {}, {}          # narrow heads by role
     self.normals = self.normals_pred = self.roughness = self.extra_dw = None
-    self.vacts, self.vbits, self.vin = [], [], None
+    self.vacts, self.vbits, self.vin, self.vin_copies = [], [], None, []     # + copies of vin into later skip layers
     self.x_last = self.t_last = self.v_last = None   # inputs of the last trunk layer / tangent stream / view layer
     self.bwd = None         # BwdScratch, allocated on the first backward
     self.keep_acts = True   # False: render-only pass, the chained trunk skips activation / mask stores
@@ -307,12 +316,15 @@ class BwdScratch:
     cfg, bf = plan.cfg, torch.bfloat16
     # trunk: per-layer gradient buffers when the dgrad chain runs as one launch (its wgrads come after), else two
     self.dy = [torch.empty(M, cfg.net_width, device=dev, dtype=bf) for _ in range(cfg.net_depth if chained else 2)]
-    self.dv = self.d_vin = self.d_vin_skip = self.dhead = self.h = None
+    self.dv = self.d_vin = self.dhead = self.h = None
+    self.d_vin_parts = []
     if plan.top == 'view':
-      self.dv = [torch.empty(M, cfg.net_width_viewdirs, device=dev, dtype=bf) for _ in range(2)]
+      if cfg.net_depth_viewdirs:
+        self.dv = [torch.empty(M, cfg.net_width_viewdirs, device=dev, dtype=bf) for _ in range(2)]
       self.d_vin = torch.empty(M, plan.vin_pad, device=dev, dtype=bf)
-      # the view layer after a skip also consumed vin
-      self.d_vin_skip = torch.empty(M, plan.vin_pad, device=dev, dtype=bf) if plan.view_concat_after else None
+      # running sums of the other consumers' contributions to d vin (view layers after a skip, the rgb head after a
+      # skip), chained through the dgrad addend: two buffers that take turns as addend and output
+      self.d_vin_parts = [torch.empty(M, plan.vin_pad, device=dev, dtype=bf) for _ in range(min(2, plan.vin_partials))]
     elif plan.slab_cols:
       # zero-filled once: the normals backward writes only its first four (seven) columns
       self.dhead = torch.zeros(M, plan.slab_cols, device=dev, dtype=bf)
@@ -569,8 +581,10 @@ class Model:
       st.vacts = [torch.empty(M, Wv + plan.vin_pad if i in plan.view_concat_after else Wv, device=dev, dtype=bf)
                   for i in range(nv)]
       st.vbits = [torch.empty(M, Wv // 32, device=dev, dtype=torch.int32) for _ in range(nv)]
+      # the first layer whose output is concatenated with vin owns the vin columns, later ones get copies
       if plan.view_concat_after:
         st.vin = st.vacts[plan.view_concat_after[0]][:, Wv:]
+        st.vin_copies = [st.vacts[i][:, Wv:] for i in plan.view_concat_after[1:]]
       else:
         st.vin = torch.empty(M, plan.vin_pad, device=dev, dtype=bf)
       st.raw_rgb = torch.empty(B, S, 3, device=dev)
@@ -596,7 +610,7 @@ class Model:
         st.M, st.S, use_pred_normals=plan.pred_normals, use_density_normals=plan.density_normals,
         use_reflections=cfg.use_reflections, use_ide=cfg.use_directional_enc, use_n_dot_v=cfg.use_n_dot_v,
         use_roughness=cfg.enable_pred_roughness, deg_view=cfg.deg_view, ide_n=ide_n,
-        roughness_bias=cfg.roughness_bias, ld=st.vin.stride(0), col0=cfg.bottleneck_width, col_end=plan.vin_pad)
+        roughness_bias=cfg.roughness_bias, ld=st.vin.stride(0), col0=plan.enc_col0, col_end=plan.vin_pad)
     return desc, mat, ml, st.heads.get('grad_pred'), st.heads.get('roughness'), st.rgd, rays.viewdirs
 
   # ------------------------------------------------------------------ forward
@@ -668,24 +682,29 @@ class Model:
     plan = mlp.plan
     cfg = plan.cfg
     B, S = st.B, st.S
-    bt = plan.one('bottleneck')
-    ops.gemm(L.GEMM_FWD, st.x_last, mlp.w_nk[bt.name], st.vin[:, :bt.out_dim], m=st.M, n=bt.out_dim,
-             k=bt.in_pad, act=L.ACT_NONE, bias=mlp.b(bt), impl=impl)
-    if st.bneck_noise is not None:
-      # models.py:529-533 (regulariser, unused by the shipped configs): plain elementwise add
-      st.vin[:, :bt.out_dim].add_((cfg.bottleneck_noise * st.bneck_noise).to(torch.bfloat16))
+    if plan.has_bottleneck:
+      bt = plan.one('bottleneck')
+      ops.gemm(L.GEMM_FWD, st.x_last, mlp.w_nk[bt.name], st.vin[:, :bt.out_dim], m=st.M, n=bt.out_dim,
+               k=bt.in_pad, act=L.ACT_NONE, bias=mlp.b(bt), impl=impl)
+      if st.bneck_noise is not None:
+        # models.py:529-533 (regulariser, unused by the shipped configs): plain elementwise add
+        st.vin[:, :bt.out_dim].add_((cfg.bottleneck_noise * st.bneck_noise).to(torch.bfloat16))
     if plan.ref_stage:
       ops.refdir_fwd(*self._refdir_args(st, mlp, rays), st.normals_pred, st.normals, st.roughness, st.vin,
                      *normals_args)
     else:
-      ops.viewdir_enc(rays.viewdirs, S, cfg.deg_view, st.vin, bt.out_dim, plan.vin_pad)
+      ops.viewdir_enc(rays.viewdirs, S, cfg.deg_view, st.vin, plan.enc_col0, plan.vin_pad)
     if plan.glo_features > 0:
       # GLO vector of the ray's camera, broadcast over the samples (models.py:565-569).  Written after the Ref-NeRF
       # stage: its slab zero-fill would also clear the GLO columns.
       g0 = plan.glo_col0
-      st.vin.view(B, S, st.vin.stride(0))[:, :, g0:g0 + plan.glo_features] = \
+      # (unflatten, not view: a vin owned by a skip layer's buffer is a strided slice of it)
+      st.vin.unflatten(0, (B, S))[:, :, g0:g0 + plan.glo_features] = \
           (st.glo_vec if st.glo_vec is not None else torch.zeros(B, plan.glo_features, device=st.vin.device)
            )[:, None, :].to(torch.bfloat16)
+    # the view layers after the second and later skips read their own copy of the finished vin
+    for c in st.vin_copies:
+      c.copy_(st.vin)
     v = st.vin
     for i, sp in enumerate(plan.by_role('view')):
       Wv = sp.out_dim
@@ -829,7 +848,7 @@ class Model:
       if m.num_glo_features > 0 and not lv['is_prop'] and not zero_glo:
         st.glo_vec = self.params.seg('Embed_0').view(m.num_glo_embeddings, -1)[rays.cam_idx[:, 0].long()]
       st.bneck_noise = None
-      if mlp.plan.cfg.bottleneck_noise > 0 and rng is not None and mlp.plan.top == 'view':
+      if mlp.plan.cfg.bottleneck_noise > 0 and rng is not None and mlp.plan.has_bottleneck:
         st.bneck_noise = draw('bottleneck_noise', i, (B * lv['S'], mlp.plan.cfg.bottleneck_width), torch.randn)
       # levels of an MLP without normals skip the normal losses (the reference raises there instead)
       st.loss_mults = self.level_loss_mults(loss_config, i, B) if (
@@ -975,43 +994,55 @@ class Model:
                    dw=mlp.W(sp, g), db=mlp.b(sp, g))
 
   def _view_mlp_bwd(self, st, mlp, impl):
-    """rgb head and view MLP backward; returns the gradient of the first view layer's output and the skip layer's
-    contribution to d vin (None without a skip)."""
+    """rgb head and view MLP backward into sc.d_vin[:, :d_vin_cols]: [ d bottleneck (| d direction encoding | d n.v)
+    (| d GLO) ] (no activation on vin), the sum of every consumer's contribution."""
     plan = mlp.plan
     sc, g = st.bwd, mlp.grads
     views, r = plan.by_role('view'), plan.one('rgb')
     Wv = plan.cfg.net_width_viewdirs
+    n = plan.d_vin_cols
+    d_rgb = st.d_raw_rgb.view(st.M, 3)
+    if plan.rgb_vin == 'all':
+      # no view MLP: the rgb head reads vin, its input gradient is all of d vin
+      ops.head_bwd(st.vin, mlp.w_nk[r.name], d_rgb, r.out_dim, r.in_pad, dx=sc.d_vin, dw=mlp.W(r, g), db=mlp.b(r, g),
+                   dx_cols=n)
+      return
+    # the running sum of d vin before view layer 0 adds its part: parts[j % 2] holds contributions 0..j
+    parts, j = sc.d_vin_parts, 0
     dcur = sc.dv[0]
-    ops.head_bwd(st.v_last, mlp.w_nk[r.name], st.d_raw_rgb.view(st.M, 3), r.out_dim, r.in_pad, dx=dcur,
-                 relu_mask=True, dw=mlp.W(r, g), db=mlp.b(r, g), dxsum=mlp.b(views[-1], g))
-    skip = None
+    if plan.rgb_vin == 'tail':
+      # a view MLP ending on a skip: the head reads [hidden | vin]; the vin columns' gradient is the first part
+      ops.head_bwd(st.v_last, mlp.w_nk[r.name], d_rgb, r.out_dim, r.in_pad, dx=dcur, relu_mask=True, dw=mlp.W(r, g),
+                   db=mlp.b(r, g), dxsum=mlp.b(views[-1], g), dx_cols=Wv, dx2=parts[0])
+      j = 1
+    else:
+      ops.head_bwd(st.v_last, mlp.w_nk[r.name], d_rgb, r.out_dim, r.in_pad, dx=dcur, relu_mask=True, dw=mlp.W(r, g),
+                   db=mlp.b(r, g), dxsum=mlp.b(views[-1], g))
     for i in range(len(views) - 1, -1, -1):
       sp = views[i]
       xin = st.vin if i == 0 else st.vacts[i - 1]
       ops.gemm(L.GEMM_WGRAD, xin, dcur, mlp.W(sp, g), m=sp.in_pad, n=Wv, k=st.M, impl=impl)
       if i > 0:
-        if (i - 1) in plan.view_concat_after:
-          # this layer also consumed vin (skip concat): its second gradient contribution
-          ops.gemm(L.GEMM_DGRAD, dcur, mlp.w_kn[sp.name][Wv:], sc.d_vin_skip, m=st.M, n=plan.vin_pad, k=Wv,
-                   impl=impl)
-          skip = sc.d_vin_skip
+        if i in plan.view_skips:
+          # this layer also consumed vin (skip concat): its contribution, added to the parts so far
+          ops.gemm(L.GEMM_DGRAD, dcur, mlp.w_kn[sp.name][Wv:], parts[j % 2], m=st.M, n=plan.vin_pad, k=Wv,
+                   addend=parts[(j - 1) % 2] if j else None, impl=impl)
+          j += 1
         nxt = sc.dv[1] if dcur is sc.dv[0] else sc.dv[0]
         ops.gemm(L.GEMM_DGRAD, dcur, mlp.w_kn[sp.name], nxt, m=st.M, n=Wv, k=Wv,
                  maskbits=st.vbits[i - 1], colsum=mlp.b(views[i - 1], g), impl=impl)
         dcur = nxt
-    return dcur, skip
+    # d vin = dcur * Wv0^T (+ the other consumers' parts)
+    ops.gemm(L.GEMM_DGRAD, dcur, mlp.w_kn[views[0].name], sc.d_vin[:, :n], m=st.M, n=n, k=Wv,
+             addend=parts[(j - 1) % 2][:, :n] if j else None, impl=impl)
 
   def _view_bwd(self, st, mlp, rays, impl, lm, stats):
     """Top of a trunk with a view branch: view MLP, GLO, Ref-NeRF stage or direction encoding, bottleneck."""
     plan = mlp.plan
     sc, g = st.bwd, mlp.grads
     bt, d = plan.one('bottleneck'), plan.one('density')
-    bw = bt.out_dim
-    dcur, skip = self._view_mlp_bwd(st, mlp, impl)
-    # d vin = dcur * Wv0^T: [ d bottleneck (| d direction encoding | d n.v) (| d GLO) ] (no activation on vin)
-    n = plan.d_vin_cols
-    ops.gemm(L.GEMM_DGRAD, dcur, mlp.w_kn[plan.by_role('view')[0].name], sc.d_vin[:, :n], m=st.M, n=n,
-             k=plan.cfg.net_width_viewdirs, addend=skip[:, :n] if skip is not None else None, impl=impl)
+    bw = plan.enc_col0
+    self._view_mlp_bwd(st, mlp, impl)
     if st.glo_vec is not None:
       # the GLO columns of vin, summed over the samples; read before the Ref-NeRF stage re-uses the slab columns
       g0 = plan.glo_col0
@@ -1026,10 +1057,13 @@ class Model:
     # bottleneck dW + db (models.py:527), then the Dense(1) density head's dW (models.py:460) in a pass of its own:
     # summed inside the GEMM, the weighted x_last tiles take more shared-memory bandwidth from the MMAs than the
     # pass takes HBM time (DESIGN.md section 3)
-    ops.gemm_wgrad(st.x_last, sc.d_vin[:, :bw], mlp.W(bt, g), m=bt.in_pad, n=bw, k=st.M, bsum=mlp.b(bt, g), impl=impl)
-    ops.head_bwd(st.x_last, st.x_last, st.d_raw_density.view(st.M, 1), 1, bt.in_pad, dw=mlp.W(d, g).view(-1, 1))
+    if plan.has_bottleneck:
+      ops.gemm_wgrad(st.x_last, sc.d_vin[:, :bw], mlp.W(bt, g), m=bt.in_pad, n=bw, k=st.M, bsum=mlp.b(bt, g),
+                     impl=impl)
+    ops.head_bwd(st.x_last, st.x_last, st.d_raw_density.view(st.M, 1), 1, d.in_pad, dw=mlp.W(d, g).view(-1, 1))
     if plan.ref_stage:
-      # d x_last = relu'(x_last) * ([d bottleneck | head gradients] @ [W_b | w_heads]^T)
+      # d x_last = relu'(x_last) * ([d bottleneck | head gradients] @ [W_b | w_heads]^T); without a bottleneck the
+      # slab holds the head gradients only
       self._slab_dgrad(st, mlp, sc.d_vin, impl)
     else:
       # d x_last = (dbott * Wb^T + d_raw_density (x) w_density) * relu'(x_last)

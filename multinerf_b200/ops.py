@@ -251,16 +251,17 @@ def head_fwd(x, w_nk, bias, n_out, k, raw=None):
 
 
 def head_bwd(x, w_nk, draw, n_out, k, dx=None, relu_mask=False, dw=None, db=None, dxsum=None, dw2=None, dw_split=0,
-             dx_cols=0):
+             dx_cols=0, dx2=None):
   """dw2 / dw_split: outputs [dw_split, n_out) put their weight gradient in dw2; dx_cols: dx and dxsum cover the
-  first dx_cols columns only (include/mnrf.h)."""
+  first dx_cols columns only; dx2 [M, k - dx_cols]: the input gradient of the columns past dx_cols, unmasked
+  (include/mnrf.h)."""
   lib = L.load()
   M = x.shape[0]
   _count()
   L.check(lib.mnrf_head_bwd(M, k, n_out, L.ptr(x), x.stride(0), L.ptr(w_nk), L.ptr(_f32(draw)),
                             L.ptr(dx), dx.stride(0) if dx is not None else 0, int(relu_mask),
                             L.ptr(dw), L.ptr(dw2), int(dw_split), L.ptr(db), L.ptr(dxsum), int(dx_cols),
-                            L.stream_ptr()))
+                            L.ptr(dx2), dx2.stride(0) if dx2 is not None else 0, L.stream_ptr()))
 
 
 def colsum(x, n, out):

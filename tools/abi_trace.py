@@ -95,6 +95,13 @@ def _bundles(configs):
     b.prop_mlp.net_depth = 5
     return b
 
+  def view_layout(b, bottleneck=None, depth=None, skip=None):
+    n = b.nerf_mlp
+    n.bottleneck_width = n.bottleneck_width if bottleneck is None else bottleneck
+    n.net_depth_viewdirs = n.net_depth_viewdirs if depth is None else depth
+    n.skip_layer_dir = n.skip_layer_dir if skip is None else skip
+    return b
+
   b360, b256, bref, braw = (configs.bundle_360, configs.bundle_blender_256, configs.bundle_blender_refnerf,
                             configs.bundle_llff_raw)
   return [
@@ -121,6 +128,10 @@ def _bundles(configs):
       ('deep_view', lambda: deep_view(b256()), {}),
       ('single_mlp', lambda: single(b256()), {}),
       ('robustnerf', lambda: robust(b360()), {}),
+      ('refnerf_no_bottleneck', lambda: view_layout(bref(), bottleneck=0), {}),
+      ('view_depth0_360', lambda: view_layout(b360(), depth=0), {}),
+      ('view_depth0_glo', lambda: view_layout(glo(b256()), depth=0), {}),
+      ('view_skips_end_glo', lambda: view_layout(glo(b256()), depth=9, skip=4), {}),
   ]
 
 
