@@ -131,7 +131,9 @@ int mnrf_viewdir_enc(int32_t num_rays, int32_t num_samples, int32_t deg, const f
  * M-tiles are 128 rows; N must be a multiple of 16.
  */
 enum { MNRF_GEMM_FWD = 0, MNRF_GEMM_DGRAD = 1, MNRF_GEMM_WGRAD = 2 };
-enum { MNRF_ACT_NONE = 0, MNRF_ACT_RELU = 1 };
+/* Activations of the Dense layers (MLP.net_activation, models.py:457,578): SOFTPLUS is jax.nn.softplus
+ * (logaddexp(z, 0)), SILU is jax.nn.silu (z * sigmoid(z)).  The two smooth ones run through mnrf_gemm_act. */
+enum { MNRF_ACT_NONE = 0, MNRF_ACT_RELU = 1, MNRF_ACT_SOFTPLUS = 2, MNRF_ACT_SILU = 3 };
 
 typedef struct {
   int32_t mode, act;
@@ -156,6 +158,18 @@ typedef struct {
 int mnrf_gemm(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
               const float* rowv, const float* colv, const mnrf_bf16* mask, uint32_t* maskbits,
               float* colsum, const mnrf_bf16* addend, void* out, mnrf_stream stream);
+
+/* The FWD and DGRAD GEMMs of a layer with a smooth activation, d->act = MNRF_ACT_SOFTPLUS or MNRF_ACT_SILU.  The
+ * backward needs a'(z) (and, for density normals, a''(z)) of the pre-activation z, which the output h = a(z) does
+ * not give back for SiLU, so the forward stores z itself in place of mask bits:
+ *   mode FWD  : out[M,N] = a(z), z = A Bt^T + bias;  z[M, ldz] (optional, bf16) receives z
+ *   mode DGRAD: out[M,N] = a'(z[r]) * (A Bt^T + rowv colv) + addend, with z row r = output row mod d->mask_mod (when
+ *               > 0: the three tangent streams share the primal's z); colsum[N] += column sums of out
+ * rowv/colv, addend and colsum are those of mnrf_gemm; `mask` and `maskbits` have no counterpart here.  N must be a
+ * multiple of 64 and `out` 16-byte aligned with a row pitch that is a multiple of 8 on the tensor-core path (impl 0). */
+int mnrf_gemm_act(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
+                  const float* rowv, const float* colv, float* colsum, const mnrf_bf16* addend, mnrf_bf16* z,
+                  int64_t ldz, void* out, mnrf_stream stream);
 
 /* Weight gradient with side sums computed from the operand tiles the main loop stages (by the three warps of
  * the producer warpgroup that issue no loads), so the bias gradient and the gradient of a Dense(1) head on the
@@ -248,6 +262,13 @@ int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64
                   const mnrf_bf16* w, const float* draw, mnrf_bf16* dx, int64_t lddx,
                   int32_t relu_mask, float* dw, float* dw2, int32_t dw_split, float* db, float* dxsum,
                   int32_t dx_cols, mnrf_bf16* dx2, int64_t lddx2, mnrf_stream stream);
+/* Same, with the derivative of a smooth activation (act = MNRF_ACT_SOFTPLUS | MNRF_ACT_SILU) in place of the ReLU
+ * mask: dx[m, k] *= a'(z[m, k]) for k < dx_cols, z [M, ldz] bf16 the pre-activation of the layer that produced X
+ * (mnrf_gemm_act FWD); ldz a multiple of 8, z 16-byte aligned.  dxsum sums the factored dx. */
+int mnrf_head_bwd_act(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx,
+                      const mnrf_bf16* w, const float* draw, mnrf_bf16* dx, int64_t lddx,
+                      int32_t act, const mnrf_bf16* z, int64_t ldz, float* dw, float* dw2, int32_t dw_split,
+                      float* db, float* dxsum, int32_t dx_cols, mnrf_bf16* dx2, int64_t lddx2, mnrf_stream stream);
 
 /* Column sums of a bf16 matrix into fp32 (bias gradients): out[N] += sum_m x[m, :]. */
 int mnrf_colsum(int64_t m, int32_t n, const mnrf_bf16* x, int64_t ldx, float* out,
@@ -422,6 +443,16 @@ int mnrf_normals_bwd(int64_t M, int32_t num_samples, const float* grad_pred, con
 int mnrf_outer_mask(int64_t rows, int32_t n, int64_t mask_mod, const float* rowv, const float* colv,
                     const uint32_t* maskbits, int64_t ldmaskbits, mnrf_bf16* out, int64_t ldo,
                     mnrf_stream stream);
+/* One trunk layer of the density-normal backward through a smooth activation a (act = MNRF_ACT_SOFTPLUS |
+ * MNRF_ACT_SILU).  With z [M, N] the layer's pre-activation, T = dL/dt and u = t_in W the tangent before the
+ * activation factor (t = a'(z) u), both three stacked streams [3M, N]:
+ *   du[s*M + m, n] = a'(z[m, n]) T[s*M + m, n]                              dL/du, bf16; du may be T (in place)
+ *   g[m, n]        = a''(z[m, n]) sum_s T[s*M + m, n] u[s*M + m, n]          the second-order part of dL/dz, bf16
+ *                    (accumulate != 0: added to g's contents), fp32 arithmetic
+ * N must be a multiple of 8, every pitch a multiple of 8 and every pointer 16-byte aligned. */
+int mnrf_act_tangent_bwd(int64_t M, int32_t n, int32_t act, const mnrf_bf16* z, int64_t ldz, const mnrf_bf16* t_adj,
+                         int64_t ldt, const mnrf_bf16* u, int64_t ldu, mnrf_bf16* du, int64_t lddu, mnrf_bf16* g,
+                         int64_t ldg, int32_t accumulate, mnrf_stream stream);
 
 /* ---- ray generation (the step before the path; SURVEY 8(f) row 1) --------------------------
  * camera_utils.pixels_to_rays (camera_utils.py:522-636) + the camera gather of

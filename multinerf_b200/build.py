@@ -16,7 +16,8 @@ COMMON = ['-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC', '--expt-relax
 # GEMM and reduction kernels keep FMA.
 SOURCES = {
     'lib.cu': [], 'sampling.cu': ['-fmad=false'], 'encode.cu': ['-fmad=false'],
-    'composite.cu': ['-fmad=false'], 'heads.cu': [], 'gemm_tc.cu': [], 'chain.cu': [], 'gemm_ref.cu': [],
+    'composite.cu': ['-fmad=false'], 'heads.cu': [], 'gemm_tc.cu': [], 'gemm_tc_act.cu': [], 'chain.cu': [],
+    'gemm_ref.cu': [],
     'refnerf.cu': [], 'camera.cu': ['-fmad=false'], 'robust.cu': ['-fmad=false'],
 }
 
@@ -28,9 +29,14 @@ def _nvcc():
   raise RuntimeError('nvcc not found')
 
 
+# sources a unit includes besides the shared headers
+INCLUDES = {'gemm_tc_act.cu': ['gemm_tc.cu']}
+
+
 def _stamp(path, flags):
   h = hashlib.sha1()
-  for p in [path, os.path.join(CSRC, 'common.cuh'), os.path.join(CSRC, 'tc_common.cuh'),
+  extra = [os.path.join(CSRC, f) for f in INCLUDES.get(os.path.basename(path), [])]
+  for p in [path] + extra + [os.path.join(CSRC, 'common.cuh'), os.path.join(CSRC, 'tc_common.cuh'),
             os.path.join(CSRC, 'wgmma.cuh'), os.path.join(HERE, '..', 'include', 'mnrf.h')]:
     with open(p, 'rb') as f:
       h.update(f.read())

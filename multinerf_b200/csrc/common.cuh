@@ -71,6 +71,24 @@ __device__ __forceinline__ float softplus_f(float x) {
 }
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.f / (1.f + expf(-x)); }
 
+// Smooth activations of the Dense layers (MNRF_ACT_SOFTPLUS | MNRF_ACT_SILU) and their first two derivatives:
+//   softplus: a = logaddexp(z, 0),  a' = s,                 a'' = s (1 - s)
+//   silu:     a = z s,              a' = s (1 + z (1 - s)),  a'' = s (1 - s) (2 + z (1 - 2 s)),     s = sigmoid(z)
+// They run in GEMM epilogues, once per output element, and their results are rounded to bf16: the hardware
+// exp / log / reciprocal approximations (relative error ~1e-6) keep the epilogue short.
+__device__ __forceinline__ float sigmoid_fast(float z) { return __fdividef(1.f, 1.f + __expf(-z)); }
+__device__ __forceinline__ float act_fwd(int act, float z) {
+  return act == MNRF_ACT_SILU ? z * sigmoid_fast(z) : fmaxf(z, 0.f) + __logf(1.f + __expf(-fabsf(z)));
+}
+__device__ __forceinline__ float act_d1(int act, float z) {
+  const float s = sigmoid_fast(z);
+  return act == MNRF_ACT_SILU ? s * (1.f + z * (1.f - s)) : s;
+}
+__device__ __forceinline__ float act_d2(int act, float z) {
+  const float s = sigmoid_fast(z), q = s * (1.f - s);
+  return act == MNRF_ACT_SILU ? q * (2.f + z * (1.f - 2.f * s)) : q;
+}
+
 // math.safe_sin (math.py:26-38): sin(|x| < 100*pi ? x : x mod 100*pi), Python-style mod.
 __device__ __forceinline__ float safe_sin_f(float x) {
   const float t = 314.159271240234375f;  // fl32(100*pi)

@@ -9,7 +9,7 @@ namespace mnrf {
 int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
                    const float* rowv, const float* colv, const mnrf_bf16* mask, uint32_t* maskbits,
                    float* colsum, const mnrf_bf16* addend, void* out, cudaStream_t stream, float* bsum,
-                   const float* side_w, float* side_aw);
+                   const float* side_w, float* side_aw, mnrf_bf16* z, int64_t ldz);
 
 __device__ __forceinline__ float ldbf(const __nv_bfloat16* p) { return __bfloat162float(*p); }
 
@@ -18,7 +18,8 @@ __global__ void gemm_ref_nt_kernel(mnrf_gemm_desc d, const __nv_bfloat16* __rest
                                    const __nv_bfloat16* __restrict__ b, const float* __restrict__ bias,
                                    const float* __restrict__ rowv, const float* __restrict__ colv,
                                    const __nv_bfloat16* __restrict__ mask, uint32_t* __restrict__ maskbits,
-                                   const __nv_bfloat16* __restrict__ addend, __nv_bfloat16* __restrict__ out) {
+                                   const __nv_bfloat16* __restrict__ addend, __nv_bfloat16* __restrict__ out,
+                                   __nv_bfloat16* __restrict__ z, int64_t ldz) {
   __shared__ float sa[16][17], sb[16][17];
   const int64_t m = (int64_t)blockIdx.y * 16 + threadIdx.y;
   const int n = blockIdx.x * 16 + threadIdx.x;
@@ -39,10 +40,15 @@ __global__ void gemm_ref_nt_kernel(mnrf_gemm_desc d, const __nv_bfloat16* __rest
     if (d.act == MNRF_ACT_RELU) {
       acc = fmaxf(acc, 0.f);
       if (maskbits && acc > 0.f) atomicOr(&maskbits[m * d.ldmaskbits + (n >> 5)], 1u << (n & 31));
+    } else if (d.act == MNRF_ACT_SOFTPLUS || d.act == MNRF_ACT_SILU) {
+      if (z) z[m * ldz + n] = __float2bfloat16(acc);
+      acc = act_fwd(d.act, acc);
     }
   } else {
     if (rowv) acc += rowv[m] * colv[n];
-    if (maskbits) {
+    if (z) {
+      acc *= act_d1(d.act, ldbf(z + (d.mask_mod > 0 ? m % d.mask_mod : m) * ldz + n));
+    } else if (maskbits) {
       const int64_t mrow = d.mask_mod > 0 ? m % d.mask_mod : m;
       if (!((maskbits[mrow * d.ldmaskbits + (n >> 5)] >> (n & 31)) & 1u)) acc = 0.f;
     } else if (mask && !(ldbf(mask + m * d.ldmask + n) > 0.f)) {
@@ -77,9 +83,11 @@ __global__ void gemm_ref_tn_kernel(mnrf_gemm_desc d, const __nv_bfloat16* __rest
 
 }  // namespace mnrf
 
-extern "C" int mnrf_gemm(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
+// mnrf_gemm and mnrf_gemm_act: z (smooth activations) is null for mnrf_gemm
+static int gemm_dispatch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
                          const float* rowv, const float* colv, const mnrf_bf16* mask, uint32_t* maskbits,
-                         float* colsum, const mnrf_bf16* addend, void* out, mnrf_stream stream) {
+                         float* colsum, const mnrf_bf16* addend, mnrf_bf16* z, int64_t ldz, void* out,
+                         mnrf_stream stream) {
   using namespace mnrf;
   if (d && (d->m == 0 || d->n == 0 || d->k == 0)) return 0;   // empty operand: nothing to compute or accumulate
   MNRF_CHECK(d && a && b && out, "mnrf_gemm: null pointer");
@@ -90,7 +98,8 @@ extern "C" int mnrf_gemm(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf
   if (colsum) MNRF_CHECK(d->mode == MNRF_GEMM_DGRAD, "mnrf_gemm: colsum is a DGRAD output");
   if (addend) MNRF_CHECK(d->mode == MNRF_GEMM_DGRAD, "mnrf_gemm: addend is a DGRAD input");
   if (d->impl == 0)
-    return gemm_tc_launch(d, a, b, bias, rowv, colv, mask, maskbits, colsum, addend, out, s, nullptr, nullptr, nullptr);
+    return gemm_tc_launch(d, a, b, bias, rowv, colv, mask, maskbits, colsum, addend, out, s, nullptr, nullptr, nullptr,
+                          z, ldz);
   dim3 block(16, 16);
   if (d->mode != MNRF_GEMM_WGRAD) {
     dim3 grid((d->n + 15) / 16, (unsigned)((d->m + 15) / 16));
@@ -102,7 +111,8 @@ extern "C" int mnrf_gemm(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf
                                                reinterpret_cast<const __nv_bfloat16*>(b), bias, rowv, colv,
                                                reinterpret_cast<const __nv_bfloat16*>(mask), maskbits,
                                                reinterpret_cast<const __nv_bfloat16*>(addend),
-                                               reinterpret_cast<__nv_bfloat16*>(out));
+                                               reinterpret_cast<__nv_bfloat16*>(out),
+                                               reinterpret_cast<__nv_bfloat16*>(z), ldz);
     MNRF_LAUNCH_CHECK();
     if (colsum) {   // reference path: sum the (bf16-rounded) output in a second pass
       if (int rc = mnrf_colsum(d->m, d->n, reinterpret_cast<const mnrf_bf16*>(out), d->ldc, colsum, stream)) return rc;
@@ -120,6 +130,26 @@ extern "C" int mnrf_gemm(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf
   return 0;
 }
 
+extern "C" int mnrf_gemm(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
+                         const float* rowv, const float* colv, const mnrf_bf16* mask, uint32_t* maskbits,
+                         float* colsum, const mnrf_bf16* addend, void* out, mnrf_stream stream) {
+  return gemm_dispatch(d, a, b, bias, rowv, colv, mask, maskbits, colsum, addend, nullptr, 0, out, stream);
+}
+
+extern "C" int mnrf_gemm_act(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
+                             const float* rowv, const float* colv, float* colsum, const mnrf_bf16* addend,
+                             mnrf_bf16* z, int64_t ldz, void* out, mnrf_stream stream) {
+  using namespace mnrf;
+  MNRF_CHECK(d, "mnrf_gemm_act: null pointer");
+  MNRF_CHECK(d->act == MNRF_ACT_SOFTPLUS || d->act == MNRF_ACT_SILU,
+             "mnrf_gemm_act: act %d is not a smooth activation (softplus %d, silu %d)", d->act, MNRF_ACT_SOFTPLUS,
+             MNRF_ACT_SILU);
+  MNRF_CHECK(d->mode == MNRF_GEMM_FWD || d->mode == MNRF_GEMM_DGRAD, "mnrf_gemm_act: FWD or DGRAD only");
+  MNRF_CHECK(d->mode == MNRF_GEMM_FWD || z, "mnrf_gemm_act: the DGRAD needs z");
+  MNRF_CHECK(!z || ldz >= d->n, "mnrf_gemm_act: ldz %lld < N %d", (long long)ldz, d->n);
+  return gemm_dispatch(d, a, b, bias, rowv, colv, nullptr, nullptr, colsum, addend, z, ldz, out, stream);
+}
+
 extern "C" int mnrf_gemm_wgrad(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, float* bsum,
                                const float* side_w, float* side_aw, float* out, mnrf_stream stream) {
   using namespace mnrf;
@@ -129,7 +159,7 @@ extern "C" int mnrf_gemm_wgrad(const mnrf_gemm_desc* d, const mnrf_bf16* a, cons
   MNRF_CHECK((side_w == nullptr) == (side_aw == nullptr), "mnrf_gemm_wgrad: side_w and side_aw come together");
   // tensor cores: one launch, the side sums taken from the operand tiles the main loop stages
   if (d->impl == 0) return gemm_tc_launch(d, a, b, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, out,
-                                          (cudaStream_t)stream, bsum, side_w, side_aw);
+                                          (cudaStream_t)stream, bsum, side_w, side_aw, nullptr, 0);
   // SIMT reference: the weight gradient, then the side sums as separate passes over the same operands
   if (int rc = mnrf_gemm(d, a, b, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, out, stream)) return rc;
   if (bsum)

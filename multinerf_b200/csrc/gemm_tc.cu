@@ -61,11 +61,12 @@ struct GemmParams {
   int64_t m;                  // output rows
   int n, k;                   // output cols, reduction length
   int num_m_blocks, num_n_blocks, num_splits, kblocks_per_split, num_k_blocks;
-  int64_t ldc, ldmask;
+  int64_t ldc, ldmask;        // SMOOTH instances: ldmask is the row pitch of z
   const float* bias;
   const float* rowv;
   const float* colv;
-  const __nv_bfloat16* mask;
+  const __nv_bfloat16* mask;  // SMOOTH instances (a smooth activation has no mask): the pre-activation z, which FWD
+                              // writes (optional) and DGRAD multiplies by a'(z) (row = output row, mod mask_mod if > 0)
   uint32_t* maskbits;         // FWD+ReLU: written (1 bit per output, word = 32 columns); DGRAD: read
   int64_t ldmaskbits;         // in 32-bit words
   int64_t mask_mod;           // > 0: mask row = output row mod mask_mod
@@ -170,7 +171,9 @@ __device__ __forceinline__ void wgrad_side_sums(const GemmParams& p, int t, uint
 
 // Accumulator fragment of wgmma m64nBN (per consumer thread): acc[4i + 2h + e] is row 16*warp + lane/4 + 8h,
 // column 8i + 2*(lane%4) + e of the warpgroup's 64 x BN tile.
-template <int MODE, int BN, bool TS, bool SIDE>
+// SMOOTH: the epilogue of a softplus / SiLU layer (p.act): FWD stores z and applies a(z), DGRAD multiplies by a'(z)
+// where the ReLU instances handle mask bits.  Separate instances, so the ReLU ones keep their code.
+template <int MODE, int BN, bool TS, bool SIDE, bool SMOOTH = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_m,
@@ -184,6 +187,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   constexpr int MW = mask_words(BN);
   static_assert(SB < 2 || (BN / 64) % 2 == 0, "block j of every tile must use staging block j % SB");
   static_assert(!SIDE || kWgrad, "side sums are a WGRAD feature");
+  static_assert(!SMOOTH || (TS && !kWgrad), "smooth activations are FWD / DGRAD epilogues of the staged store");
   extern __shared__ uint8_t smem_dyn[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
@@ -392,7 +396,16 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
 #pragma unroll
             for (int h = 0; h < 2; ++h) { v[h][0] += b.x; v[h][1] += b.y; }
           }
-          if (p.act == MNRF_ACT_RELU) {
+          if constexpr (SMOOTH) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              if (p.mask && row_ok[h])
+                *reinterpret_cast<uint32_t*>(const_cast<__nv_bfloat16*>(p.mask) + rows[h] * p.ldmask + col) =
+                    pack_bf16(v[h][0], v[h][1]);
+              v[h][0] = act_fwd(p.act, v[h][0]);
+              v[h][1] = act_fwd(p.act, v[h][1]);
+            }
+          } else if (p.act == MNRF_ACT_RELU) {
 #pragma unroll
             for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -407,7 +420,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             if (p.rowv) { v[h][0] += rv[h] * cv.x; v[h][1] += rv[h] * cv.y; }
-            if (p.maskbits) {
+            if constexpr (SMOOTH) {
+              if (row_ok[h]) {
+                const int64_t zr = p.mask_mod > 0 ? rows[h] % p.mask_mod : rows[h];
+                const uint32_t zz = __ldg(reinterpret_cast<const unsigned int*>(p.mask + zr * p.ldmask + col));
+                v[h][0] *= act_d1(p.act, bf16_lo(zz));
+                v[h][1] *= act_d1(p.act, bf16_hi(zz));
+              }
+            } else if (p.maskbits) {
               if (!((mw[h] >> (col & 31)) & 1u)) v[h][0] = 0.f;
               if (!((mw[h] >> ((col + 1) & 31)) & 1u)) v[h][1] = 0.f;
             } else if (p.mask && row_ok[h]) {
@@ -498,6 +518,34 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
 }
 
 // ------------------------------------------------------------------------------------ host
+template <int MODE, int BN, bool TS, bool SIDE, bool SMOOTH>
+static int launch_gemm_tc(int grid, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
+                          const CUtensorMap& tm, const GemmParams& p, cudaStream_t stream) {
+  static bool attr_set = false;
+  constexpr int kSmem = smem_bytes(MODE, BN, TS, SIDE);
+  static_assert(kSmem <= 232448, "shared memory budget");
+  auto kern = gemm_tc_kernel<MODE, BN, TS, SIDE, SMOOTH>;
+  if (!attr_set) {
+    MNRF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
+    attr_set = true;
+  }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(NUM_THREADS);
+  cfg.dynamicSmemBytes = kSmem; cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  MNRF_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, tc, tm, p));
+  return 0;
+}
+
+// The SMOOTH instances are compiled in a translation unit of their own (gemm_tc_act.cu): instantiated beside the
+// ReLU ones, they change how nvcc optimises the ReLU DGRAD instances.
+int gemm_tc_smooth_launch(int mode, int block_n, int grid, const CUtensorMap& ta, const CUtensorMap& tb,
+                          const CUtensorMap& tc, const GemmParams& p, cudaStream_t stream);
+
+#ifndef MNRF_GEMM_TC_SMOOTH_UNIT
 static int pick_block_n(int n) {
   const int cands[] = {256, 128, 64, 32, 16};
   for (int c : cands)
@@ -508,7 +556,7 @@ static int pick_block_n(int n) {
 int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
                    const float* rowv, const float* colv, const mnrf_bf16* mask, uint32_t* maskbits,
                    float* colsum, const mnrf_bf16* addend, void* out, cudaStream_t stream, float* bsum,
-                   const float* side_w, float* side_aw) {
+                   const float* side_w, float* side_aw, mnrf_bf16* z, int64_t ldz) {
   // K-major modes: the reduction index is the contiguous one and layers are padded to 64.  WGRAD reduces
   // over the sample rows, any count: the last 64-row block is zero-filled by TMA past the tensor's end.
   MNRF_CHECK(d->mode == MNRF_GEMM_WGRAD || d->k % BLOCK_K == 0,
@@ -547,6 +595,16 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
     MNRF_CHECK(d->n % 32 == 0 && block_n % 32 == 0 && d->ldmaskbits * 32 >= d->n,
                "mnrf_gemm(tc): maskbits need N %% 32 == 0 and ldmaskbits >= N/32");
   }
+  const bool smooth = d->mode != MNRF_GEMM_WGRAD && (d->act == MNRF_ACT_SOFTPLUS || d->act == MNRF_ACT_SILU);
+  if (smooth) {
+    MNRF_CHECK(!maskbits && !mask, "mnrf_gemm(tc): a smooth activation takes z, not a ReLU mask");
+    MNRF_CHECK(d->mode == MNRF_GEMM_FWD || z, "mnrf_gemm(tc): the DGRAD of a smooth activation needs z");
+    MNRF_CHECK(!z || (ldz % 2 == 0 && ((uintptr_t)z % 4) == 0), "mnrf_gemm(tc): z must be 4-byte aligned");
+  }
+  if (smooth) {
+    p.mask = reinterpret_cast<const __nv_bfloat16*>(z);
+    p.ldmask = ldz;
+  }
   if (bias) MNRF_CHECK(((uintptr_t)bias % 8) == 0, "mnrf_gemm(tc): bias must be 8-byte aligned");
   if (colv) MNRF_CHECK(((uintptr_t)colv % 8) == 0, "mnrf_gemm(tc): colv must be 8-byte aligned");
   const int workers = mnrf_num_sms();
@@ -577,6 +635,9 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
   // The bf16 output goes through the staged bulk store when its tiles are whole 128-byte swizzle spans and TMA can
   // address it (16-byte aligned base and row pitch); otherwise the epilogue stores from registers.
   const bool ts = d->mode != MNRF_GEMM_WGRAD && block_n >= 64 && ((uintptr_t)out % 16) == 0 && d->ldc % 8 == 0;
+  // the smooth epilogues exist for the staged store only: every hidden layer is a multiple of 64 wide
+  MNRF_CHECK(!smooth || ts, "mnrf_gemm(tc): a smooth activation needs N %% 64 == 0 and a 16-byte aligned output "
+             "with a row pitch that is a multiple of 8");
   CUtensorMap ta, tb, tc;
   if (d->mode != MNRF_GEMM_WGRAD) {
     if (make_tmap(&ta, a, d->m, d->k, d->lda, BLOCK_K, BLOCK_M)) return 1;
@@ -607,22 +668,7 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
   if (grid == 0) return 0;
 #define MNRF_LAUNCH_TC3(MODE_, BN_, TS_, SIDE_)                                                       \
   do {                                                                                                \
-    static bool attr_set = false;                                                                     \
-    constexpr int kSmem = smem_bytes(MODE_, BN_, TS_, SIDE_);                                         \
-    static_assert(kSmem <= 232448, "shared memory budget");                                           \
-    auto kern = gemm_tc_kernel<MODE_, BN_, TS_, SIDE_>;                                               \
-    if (!attr_set) {                                                                                  \
-      MNRF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));      \
-      attr_set = true;                                                                                \
-    }                                                                                                 \
-    cudaLaunchConfig_t cfg = {};                                                                      \
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(NUM_THREADS);                                       \
-    cfg.dynamicSmemBytes = kSmem; cfg.stream = stream;                                                \
-    cudaLaunchAttribute attr[1];                                                                      \
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                                  \
-    attr[0].val.programmaticStreamSerializationAllowed = 1;                                           \
-    cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;                                           \
-    MNRF_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, tc, tm, p));                                     \
+    if (int rc = launch_gemm_tc<MODE_, BN_, TS_, SIDE_, false>(grid, ta, tb, tc, tm, p, stream)) return rc; \
   } while (0)
 #define MNRF_LAUNCH_TC2(MODE_, BN_)                                                                   \
   do {                                                                                                \
@@ -640,11 +686,14 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
       default: if (MODE_ != MNRF_GEMM_WGRAD) MNRF_LAUNCH_TC2(MODE_, 16); break;                       \
     }                                                                                                 \
   } while (0)
-  if (d->mode == MNRF_GEMM_FWD) MNRF_LAUNCH_TC(MNRF_GEMM_FWD);
+  if (smooth) {
+    if (int rc = gemm_tc_smooth_launch(d->mode, block_n, grid, ta, tb, tc, p, stream)) return rc;
+  } else if (d->mode == MNRF_GEMM_FWD) MNRF_LAUNCH_TC(MNRF_GEMM_FWD);
   else if (d->mode == MNRF_GEMM_DGRAD) MNRF_LAUNCH_TC(MNRF_GEMM_DGRAD);
   else MNRF_LAUNCH_TC(MNRF_GEMM_WGRAD);
   MNRF_LAUNCH_CHECK();
   return 0;
 }
+#endif  // MNRF_GEMM_TC_SMOOTH_UNIT
 
 }  // namespace mnrf

@@ -55,16 +55,16 @@ __device__ __forceinline__ float* dw_at(float* dw, float* dw2, int split, int n_
   return o < split ? dw + (size_t)k * split + o : dw2 + (size_t)k * (n_out - split) + (o - split);
 }
 
-// dx[m,k] = relu'(x[m,k]) * sum_o draw[m,o] w[o,k] for k < dx_cols;  dx2[m,k-dx_cols] = sum_o draw[m,o] w[o,k] for
+// dx[m,k] = relu'(x[m,k]) * sum_o draw[m,o] w[o,k] for k < dx_cols (SMOOTH: a'(z[m,k]) in place of relu'(x[m,k]));  dx2[m,k-dx_cols] = sum_o draw[m,o] w[o,k] for
 // k >= dx_cols (optional);  dw[k,o] += sum_m draw[m,o] x[m,k];  db[o] += sum_m draw[m,o]
-template <int N_OUT, int kMaxChunks>
+template <int N_OUT, int kMaxChunks, bool SMOOTH>
 __global__ void __launch_bounds__(256)
 head_bwd_kernel(int64_t M, int K, const __nv_bfloat16* __restrict__ x, int64_t ldx,
                 const __nv_bfloat16* __restrict__ w, const float* __restrict__ draw,
                 __nv_bfloat16* __restrict__ dx, int64_t lddx, int relu_mask,
                 float* __restrict__ dw, float* __restrict__ dw2, int dw_split, float* __restrict__ db,
                 float* __restrict__ dxsum, int dx_cols, __nv_bfloat16* __restrict__ dx2, int64_t lddx2,
-                int64_t rows_per_block) {
+                int64_t rows_per_block, int act, const __nv_bfloat16* __restrict__ z, int64_t ldz) {
   extern __shared__ __align__(16) unsigned char smraw[];
   constexpr int n_out = N_OUT;
   float* sdw = reinterpret_cast<float*>(smraw);                                   // [n_out][K] fp32
@@ -122,7 +122,15 @@ head_bwd_kernel(int64_t M, int K, const __nv_bfloat16* __restrict__ x, int64_t l
           for (int e = 0; e < 8; ++e) racc[o][q][e] += g[o] * xe[e];
         }
         if (dxr && c * 8 < dx_cols) {
-          if (relu_mask) {
+          if constexpr (SMOOTH) {
+            const uint4 zv = *reinterpret_cast<const uint4*>(z + m * ldz + c * 8);
+            const uint32_t zz[4] = {zv.x, zv.y, zv.z, zv.w};
+#pragma unroll
+            for (int p = 0; p < 4; ++p) {
+              de[2 * p] *= act_d1(act, bf16_lo(zz[p]));
+              de[2 * p + 1] *= act_d1(act, bf16_hi(zz[p]));
+            }
+          } else if (relu_mask) {
 #pragma unroll
             for (int e = 0; e < 8; ++e) de[e] = xe[e] > 0.f ? de[e] : 0.f;
           }
@@ -239,14 +247,14 @@ head_fwd_sub_kernel(int64_t M, int n_out, const __nv_bfloat16* __restrict__ x, i
   }
 }
 
-template <int N_OUT, int LPR, int U>
+template <int N_OUT, int LPR, int U, bool SMOOTH>
 __global__ void __launch_bounds__(256)
 head_bwd_sub_kernel(int64_t M, const __nv_bfloat16* __restrict__ x, int64_t ldx,
                     const __nv_bfloat16* __restrict__ w, const float* __restrict__ draw,
                     __nv_bfloat16* __restrict__ dx, int64_t lddx, int relu_mask,
                     float* __restrict__ dw, float* __restrict__ dw2, int dw_split, float* __restrict__ db,
                     float* __restrict__ dxsum, int dx_cols, __nv_bfloat16* __restrict__ dx2, int64_t lddx2,
-                    int64_t rows_per_block) {
+                    int64_t rows_per_block, int act, const __nv_bfloat16* __restrict__ z, int64_t ldz) {
   constexpr int K = LPR * 8, RW = 32 / LPR;
   __shared__ float sdw[N_OUT * K];
   __shared__ float sxs[K];
@@ -304,7 +312,15 @@ head_bwd_sub_kernel(int64_t M, const __nv_bfloat16* __restrict__ x, int64_t ldx,
         if (c == 0) dbacc[o] += g[u][o];
       }
       if (dx && row < m_end && c * 8 < dx_cols) {
-        if (relu_mask) {
+        if constexpr (SMOOTH) {
+          const uint4 zv = __ldg(reinterpret_cast<const uint4*>(z + row * ldz) + c);
+          const uint32_t zz[4] = {zv.x, zv.y, zv.z, zv.w};
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            de[2 * q] *= act_d1(act, bf16_lo(zz[q]));
+            de[2 * q + 1] *= act_d1(act, bf16_hi(zz[q]));
+          }
+        } else if (relu_mask) {
 #pragma unroll
           for (int e = 0; e < 8; ++e) de[e] = xe[e] > 0.f ? de[e] : 0.f;
         }
@@ -504,11 +520,13 @@ extern "C" int mnrf_head_fwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf1
   return 0;
 }
 
-extern "C" int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx,
-                             const mnrf_bf16* w, const float* draw, mnrf_bf16* dx, int64_t lddx,
-                             int32_t relu_mask, float* dw, float* dw2, int32_t dw_split, float* db, float* dxsum,
-                             int32_t dx_cols, mnrf_bf16* dx2, int64_t lddx2, mnrf_stream stream) {
+// mnrf_head_bwd and mnrf_head_bwd_act: z (the smooth activation's pre-activation) is null for mnrf_head_bwd
+static int head_bwd_impl(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx, const mnrf_bf16* w,
+                         const float* draw, mnrf_bf16* dx, int64_t lddx, int32_t relu_mask, int32_t act,
+                         const mnrf_bf16* z_, int64_t ldz, float* dw, float* dw2, int32_t dw_split, float* db,
+                         float* dxsum, int32_t dx_cols, mnrf_bf16* dx2, int64_t lddx2, mnrf_stream stream) {
   using namespace mnrf;
+  const __nv_bfloat16* z = reinterpret_cast<const __nv_bfloat16*>(z_);
   if (m == 0) return 0;
   MNRF_CHECK(x && w && draw, "mnrf_head_bwd: null pointer");
   MNRF_CHECK(!dxsum || dx, "mnrf_head_bwd: dxsum needs dx");
@@ -528,11 +546,12 @@ extern "C" int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf1
     // in flight (8 warps x 4 x 512 B each) without serialising the flush
     const int blocks_s = (int)std::min<int64_t>((m + 511) / 512, (int64_t)mnrf_num_sms() * 2);
     const int64_t rpb_s = ((m + blocks_s - 1) / blocks_s + 7) / 8 * 8;
-#define MNRF_HBS(NO, LPR_)                                                                              \
-  head_bwd_sub_kernel<NO, LPR_, 4><<<blocks_s, 256, 0, (cudaStream_t)stream>>>(                         \
+#define MNRF_HBS2(NO, LPR_, SM_)                                                                        \
+  head_bwd_sub_kernel<NO, LPR_, 4, SM_><<<blocks_s, 256, 0, (cudaStream_t)stream>>>(                    \
       m, reinterpret_cast<const __nv_bfloat16*>(x), ldx, reinterpret_cast<const __nv_bfloat16*>(w), draw, \
       reinterpret_cast<__nv_bfloat16*>(dx), lddx, relu_mask, dw, dw2, dw_split, db, dxsum, dx_cols,      \
-      reinterpret_cast<__nv_bfloat16*>(dx2), lddx2, rpb_s)
+      reinterpret_cast<__nv_bfloat16*>(dx2), lddx2, rpb_s, act, z, ldz)
+#define MNRF_HBS(NO, LPR_) do { if (z) MNRF_HBS2(NO, LPR_, true); else MNRF_HBS2(NO, LPR_, false); } while (0)
 #define MNRF_HBS_N(NO) do { if (k == 256) MNRF_HBS(NO, 32); else if (k == 128) MNRF_HBS(NO, 16); else MNRF_HBS(NO, 8); } while (0)
     switch (n_out) {
       case 1: MNRF_HBS_N(1); break;
@@ -548,11 +567,12 @@ extern "C" int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf1
   int blocks = (int)std::min<int64_t>((m + 7) / 8, (int64_t)mnrf_num_sms() * 4);
   int64_t rpb = (m + blocks - 1) / blocks;
   const int chunks = (k / 8 + 31) / 32;
-#define MNRF_HB(NO, CK)                                                                         \
-  head_bwd_kernel<NO, CK><<<blocks, 256, smem, (cudaStream_t)stream>>>(                         \
+#define MNRF_HB2(NO, CK, SM_)                                                                   \
+  head_bwd_kernel<NO, CK, SM_><<<blocks, 256, smem, (cudaStream_t)stream>>>(                    \
       m, k, reinterpret_cast<const __nv_bfloat16*>(x), ldx, reinterpret_cast<const __nv_bfloat16*>(w), \
       draw, reinterpret_cast<__nv_bfloat16*>(dx), lddx, relu_mask, dw, dw2, dw_split, db, dxsum, dx_cols, \
-      reinterpret_cast<__nv_bfloat16*>(dx2), lddx2, rpb)
+      reinterpret_cast<__nv_bfloat16*>(dx2), lddx2, rpb, act, z, ldz)
+#define MNRF_HB(NO, CK) do { if (z) MNRF_HB2(NO, CK, true); else MNRF_HB2(NO, CK, false); } while (0)
 #define MNRF_HB_N(NO)                                      \
   do {                                                     \
     if (chunks <= 1) MNRF_HB(NO, 1);                       \
@@ -568,6 +588,28 @@ extern "C" int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf1
   }
   MNRF_LAUNCH_CHECK();
   return 0;
+}
+
+extern "C" int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx,
+                             const mnrf_bf16* w, const float* draw, mnrf_bf16* dx, int64_t lddx,
+                             int32_t relu_mask, float* dw, float* dw2, int32_t dw_split, float* db, float* dxsum,
+                             int32_t dx_cols, mnrf_bf16* dx2, int64_t lddx2, mnrf_stream stream) {
+  return head_bwd_impl(m, k, n_out, x, ldx, w, draw, dx, lddx, relu_mask, MNRF_ACT_NONE, nullptr, 0, dw, dw2, dw_split,
+                       db, dxsum, dx_cols, dx2, lddx2, stream);
+}
+
+extern "C" int mnrf_head_bwd_act(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx,
+                                 const mnrf_bf16* w, const float* draw, mnrf_bf16* dx, int64_t lddx,
+                                 int32_t act, const mnrf_bf16* z, int64_t ldz, float* dw, float* dw2, int32_t dw_split,
+                                 float* db, float* dxsum, int32_t dx_cols, mnrf_bf16* dx2, int64_t lddx2,
+                                 mnrf_stream stream) {
+  using namespace mnrf;
+  MNRF_CHECK(act == MNRF_ACT_SOFTPLUS || act == MNRF_ACT_SILU, "mnrf_head_bwd_act: act %d is not a smooth activation",
+             act);
+  MNRF_CHECK(z && dx && ldz % 8 == 0 && ((uintptr_t)z % 16) == 0,
+             "mnrf_head_bwd_act: needs dx and a 16-byte aligned z with a pitch that is a multiple of 8");
+  return head_bwd_impl(m, k, n_out, x, ldx, w, draw, dx, lddx, 0, act, z, ldz, dw, dw2, dw_split, db, dxsum, dx_cols,
+                       dx2, lddx2, stream);
 }
 
 extern "C" int mnrf_colsum(int64_t m, int32_t n, const mnrf_bf16* x, int64_t ldx, float* out,

@@ -417,6 +417,59 @@ __global__ void outer_mask_kernel(int64_t R, int N, int64_t mod, const float* __
   }
 }
 
+// One trunk layer of the tangent backward through a smooth activation (mnrf.h): per [row, 8 columns] of z,
+//   du_s = a'(z) T_s,   g (+)= a''(z) sum_s T_s u_s        (s = the three tangent streams, rows m, M + m, 2M + m)
+// du may alias T: each thread reads its T chunk of every stream before it writes the same chunk of du.
+__global__ void __launch_bounds__(256)
+act_tangent_bwd_kernel(int64_t M, int N, int act, const __nv_bfloat16* __restrict__ z, int64_t ldz,
+                       const __nv_bfloat16* t_adj, int64_t ldt, const __nv_bfloat16* __restrict__ u, int64_t ldu,
+                       __nv_bfloat16* du, int64_t lddu, __nv_bfloat16* __restrict__ g, int64_t ldg, int accumulate) {
+  const int64_t total = M * (N / 8);
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / (N / 8);
+    const int c8 = (int)(i - r * (N / 8)) * 8;
+    const uint4 zv = __ldg(reinterpret_cast<const uint4*>(z + r * ldz + c8));
+    uint4 tv[3], uv[3];
+#pragma unroll
+    for (int s = 0; s < 3; ++s) {
+      tv[s] = *reinterpret_cast<const uint4*>(t_adj + (s * M + r) * ldt + c8);
+      uv[s] = __ldg(reinterpret_cast<const uint4*>(u + (s * M + r) * ldu + c8));
+    }
+    float zf[8], d1[8], gs[8];
+    const uint32_t zw[4] = {zv.x, zv.y, zv.z, zv.w};
+#pragma unroll
+    for (int q = 0; q < 4; ++q) { zf[2 * q] = bf16_lo(zw[q]); zf[2 * q + 1] = bf16_hi(zw[q]); }
+#pragma unroll
+    for (int e = 0; e < 8; ++e) { d1[e] = act_d1(act, zf[e]); gs[e] = 0.f; }
+#pragma unroll
+    for (int s = 0; s < 3; ++s) {
+      const uint32_t tw[4] = {tv[s].x, tv[s].y, tv[s].z, tv[s].w}, uw[4] = {uv[s].x, uv[s].y, uv[s].z, uv[s].w};
+      uint32_t o[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const float t0 = bf16_lo(tw[q]), t1 = bf16_hi(tw[q]);
+        gs[2 * q] += t0 * bf16_lo(uw[q]);
+        gs[2 * q + 1] += t1 * bf16_hi(uw[q]);
+        o[q] = pack_bf16(d1[2 * q] * t0, d1[2 * q + 1] * t1);
+      }
+      *reinterpret_cast<uint4*>(du + (s * M + r) * lddu + c8) = make_uint4(o[0], o[1], o[2], o[3]);
+    }
+    float prev[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (accumulate) {
+      const uint4 gv = *reinterpret_cast<const uint4*>(g + r * ldg + c8);
+      const uint32_t gw[4] = {gv.x, gv.y, gv.z, gv.w};
+#pragma unroll
+      for (int q = 0; q < 4; ++q) { prev[2 * q] = bf16_lo(gw[q]); prev[2 * q + 1] = bf16_hi(gw[q]); }
+    }
+    uint32_t o[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+      o[q] = pack_bf16(prev[2 * q] + act_d2(act, zf[2 * q]) * gs[2 * q],
+                       prev[2 * q + 1] + act_d2(act, zf[2 * q + 1]) * gs[2 * q + 1]);
+    *reinterpret_cast<uint4*>(g + r * ldg + c8) = make_uint4(o[0], o[1], o[2], o[3]);
+  }
+}
+
 }  // namespace mnrf
 
 extern "C" int mnrf_refdir_fwd(const mnrf_refdir_desc* d, const float* ide_mat, const int32_t* ide_ml,
@@ -532,6 +585,28 @@ extern "C" int mnrf_normals_bwd(int64_t M, int32_t num_samples, const float* gra
       weights, d_raw_density, d_raw_rgb, ld_raw, d_grad_pred, d_raw_grad_density,
       reinterpret_cast<__nv_bfloat16*>(head_grads),
       ld_head_grads, losses ? stats : nullptr);
+  MNRF_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int mnrf_act_tangent_bwd(int64_t M, int32_t n, int32_t act, const mnrf_bf16* z, int64_t ldz,
+                                    const mnrf_bf16* t_adj, int64_t ldt, const mnrf_bf16* u, int64_t ldu, mnrf_bf16* du,
+                                    int64_t lddu, mnrf_bf16* g, int64_t ldg, int32_t accumulate, mnrf_stream stream) {
+  using namespace mnrf;
+  if (M == 0) return 0;
+  MNRF_CHECK(z && t_adj && u && du && g, "mnrf_act_tangent_bwd: null pointer");
+  MNRF_CHECK(act == MNRF_ACT_SOFTPLUS || act == MNRF_ACT_SILU, "mnrf_act_tangent_bwd: act %d is not a smooth activation",
+             act);
+  MNRF_CHECK(n % 8 == 0 && ldz % 8 == 0 && ldt % 8 == 0 && ldu % 8 == 0 && lddu % 8 == 0 && ldg % 8 == 0,
+             "mnrf_act_tangent_bwd: N and every pitch must be multiples of 8");
+  MNRF_CHECK(((uintptr_t)z | (uintptr_t)t_adj | (uintptr_t)u | (uintptr_t)du | (uintptr_t)g) % 16 == 0,
+             "mnrf_act_tangent_bwd: pointers must be 16-byte aligned");
+  const int64_t total = M * (n / 8);
+  const int blocks = (int)std::min<int64_t>((total + 255) / 256, (int64_t)mnrf_num_sms() * 16);
+  act_tangent_bwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(
+      M, n, act, reinterpret_cast<const __nv_bfloat16*>(z), ldz, reinterpret_cast<const __nv_bfloat16*>(t_adj), ldt,
+      reinterpret_cast<const __nv_bfloat16*>(u), ldu, reinterpret_cast<__nv_bfloat16*>(du), lddu,
+      reinterpret_cast<__nv_bfloat16*>(g), ldg, accumulate);
   MNRF_LAUNCH_CHECK();
   return 0;
 }

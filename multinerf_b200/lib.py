@@ -116,7 +116,8 @@ RAY_SHAPE = {'cone': 0, 'cylinder': 1}
 RGB_ACT = {'sigmoid': 0, 'safe_exp': 1}
 LOSS_TYPE = {'mse': 0, 'charb': 1, 'rawnerf': 2}
 GEMM_FWD, GEMM_DGRAD, GEMM_WGRAD = 0, 1, 2
-ACT_NONE, ACT_RELU = 0, 1
+ACT_NONE, ACT_RELU, ACT_SOFTPLUS, ACT_SILU = 0, 1, 2, 3
+SMOOTH_ACTS = (ACT_SOFTPLUS, ACT_SILU)
 
 _P = C.c_void_p
 _SIGNATURES = {
@@ -130,12 +131,16 @@ _SIGNATURES = {
     'mnrf_viewdir_enc': (C.c_int, [C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_int32, C.c_int32,
                                    C.c_int32, _P]),
     'mnrf_gemm': (C.c_int, [C.POINTER(GemmDesc)] + [_P] * 11),
+    'mnrf_gemm_act': (C.c_int, [C.POINTER(GemmDesc)] + [_P] * 8 + [C.c_int64, _P, _P]),
     'mnrf_gemm_wgrad': (C.c_int, [C.POINTER(GemmDesc)] + [_P] * 7),
     'mnrf_mlp_chain': (C.c_int, [C.POINTER(ChainDesc), _P]),
     'mnrf_mlp_chain_max_layers': (C.c_int, []),
     'mnrf_head_fwd': (C.c_int, [C.c_int64, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P, _P, _P]),
     'mnrf_head_bwd': (C.c_int, [C.c_int64, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P, _P,
                                 C.c_int64, C.c_int32, _P, _P, C.c_int32, _P, _P, C.c_int32, _P, C.c_int64, _P]),
+    'mnrf_head_bwd_act': (C.c_int, [C.c_int64, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P, _P, C.c_int64,
+                                    C.c_int32, _P, C.c_int64, _P, _P, C.c_int32, _P, _P, C.c_int32, _P, C.c_int64,
+                                    _P]),
     'mnrf_colsum': (C.c_int, [C.c_int64, C.c_int32, _P, C.c_int64, _P, _P]),
     'mnrf_composite_fwd': (C.c_int, [C.POINTER(CompositeDesc)] + [_P] * 18),
     'mnrf_composite_bwd': (C.c_int, [C.POINTER(LossDesc)] + [_P] * 24),
@@ -151,6 +156,7 @@ _SIGNATURES = {
                          [C.c_int64] + [_P] * 3 +
                          [C.c_int64, _P, _P]),
     'mnrf_outer_mask': (C.c_int,[C.c_int64, C.c_int32, C.c_int64, _P, _P, _P, C.c_int64, _P, C.c_int64, _P]),
+    'mnrf_act_tangent_bwd': (C.c_int, [C.c_int64, C.c_int32, C.c_int32] + [_P, C.c_int64] * 5 + [C.c_int32, _P]),
     'mnrf_pixels_to_rays': (C.c_int, [C.POINTER(CameraDesc)] + [_P] * 11),
     'mnrf_spherical_rays': (C.c_int, [C.POINTER(SphericalDesc)] + [_P] * 6),
     'mnrf_clip_adam': (C.c_int, [C.POINTER(AdamDesc)] + [_P] * 6),

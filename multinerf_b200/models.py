@@ -50,13 +50,28 @@ class MLPPlan:
 
   HEAD_SLOTS = {'density': (0, 1), 'grad_pred': (1, 3), 'diffuse': (4, 3), 'tint': (7, 3),
                 'roughness': (10, 1)}     # column slots of the head-gradient slab (csrc/refnerf.cu)
+  # net_activation (jax.nn.relu | softplus | silu, internal/configs.py:31) -> the Dense layers' activation code
+  ACTIVATIONS = {'relu': L.ACT_RELU, 'softplus': L.ACT_SOFTPLUS, 'silu': L.ACT_SILU}
 
-  def __init__(self, cfg: configs.MLPConfig, use_viewdirs=True, glo_features=0):
+  def __init__(self, cfg: configs.MLPConfig, use_viewdirs=True, glo_features=0, activations=('relu',)):
+    """activations: the net_activation values the caller runs.  A smooth activation changes the per-level buffers
+    (pre-activations instead of mask bits) and the backward schedule (no chained trunk, the second-order pass of the
+    density normals), so a caller opts into it: Model passes every key of ACTIVATIONS; the bare table is the ReLU
+    one."""
     cfg.validate()
     self.glo_features = glo_features
-    if cfg.net_activation != 'relu' or cfg.density_activation != 'softplus' or \
-       cfg.roughness_activation != 'softplus':
-      raise NotImplementedError('CUDA path supports relu trunk / softplus density and roughness')
+    if cfg.net_activation not in self.ACTIVATIONS:
+      raise NotImplementedError(f'net_activation = {cfg.net_activation!r}: the CUDA path runs relu, softplus and silu')
+    if cfg.net_activation not in activations:
+      raise NotImplementedError(f'net_activation = {cfg.net_activation!r}: this plan is built for {", ".join(activations)}'
+                                f' (models.Model runs {", ".join(self.ACTIVATIONS)})')
+    if cfg.density_activation != 'softplus':
+      raise NotImplementedError(f'density_activation = {cfg.density_activation!r}: the CUDA path runs softplus')
+    if cfg.roughness_activation != 'softplus':
+      raise NotImplementedError(f'roughness_activation = {cfg.roughness_activation!r}: the CUDA path runs softplus')
+    # the activation of every trunk and view layer.  ReLU keeps 1-bit masks for the backward; a smooth one keeps the
+    # pre-activation z (bf16), and its density normals add the second-order term a''(z) to the trunk gradient
+    self.act = self.ACTIVATIONS[cfg.net_activation]
     if cfg.num_rgb_channels != 3:
       raise NotImplementedError('num_rgb_channels != 3')
     self.cfg = cfg
@@ -82,7 +97,7 @@ class MLPPlan:
     self.concat_after = []    # trunk layers whose output is concatenated with the features
     for i in range(cfg.net_depth):
       rm = np.concatenate([np.arange(W), W + np.arange(self.F)]) if x_has_feat else None
-      add('trunk', x_dim, x_pad, W, False, L.ACT_RELU, rm)
+      add('trunk', x_dim, x_pad, W, False, self.act, rm)
       if i % cfg.skip_layer == 0 and i > 0:
         self.concat_after.append(i)
         x_dim, x_pad, x_has_feat = W + self.F, W + self.Fpad, True
@@ -160,7 +175,7 @@ class MLPPlan:
       self.view_concat_after = []     # view layers whose output is concatenated with vin
       for i in range(cfg.net_depth_viewdirs):
         rmv = np.concatenate([np.arange(Wv), Wv + np.arange(vin)]) if v_has_in else None
-        add('view', v_dim, v_pad, Wv, False, L.ACT_RELU, rmv)
+        add('view', v_dim, v_pad, Wv, False, self.act, rmv)
         if i % cfg.skip_layer_dir == 0 and i > 0:
           self.view_concat_after.append(i)
           v_dim, v_pad, v_has_in = Wv + vin, Wv + vin_pad, True
@@ -290,15 +305,16 @@ class LevelState:
   def __init__(self, B, S, mname):
     self.B, self.S, self.M, self.mname = B, S, B * S, mname     # M: rows (samples) of the level
     self.sdist = None
-    # trunk activations, features (+ their copies into later skip layers) and ReLU masks; tangent streams
-    self.acts, self.feat, self.feat_copies, self.bits = [], None, [], []
+    # trunk activations, features (+ their copies into later skip layers) and ReLU masks (bits) or, for a smooth
+    # activation, pre-activations (zs); tangent streams
+    self.acts, self.feat, self.feat_copies, self.bits, self.zs = [], None, [], [], []
     self.tacts, self.tfeat, self.tfeat_copies, self.rgd, self.d_rgd = [], None, [], None, None
     # raw_head / d_raw_head [M, head_n]: the density (or stacked [density | rgb]) head's output and gradient, of which
     # raw_density (and a stacked raw_rgb) are views
     self.raw_head = self.d_raw_head = self.raw_density = self.d_raw_density = self.raw_rgb = self.d_raw_rgb = None
     self.heads, self.d_heads = {}, {}          # narrow heads by role
     self.normals = self.normals_pred = self.roughness = self.extra_dw = None
-    self.vacts, self.vbits, self.vin, self.vin_copies = [], [], None, []     # + copies of vin into later skip layers
+    self.vacts, self.vbits, self.vzs, self.vin, self.vin_copies = [], [], [], None, []   # + vin copies for later skips
     self.x_last = self.t_last = self.v_last = None   # inputs of the last trunk layer / tangent stream / view layer
     self.bwd = None         # BwdScratch, allocated on the first backward
     self.keep_acts = True   # False: render-only pass, the chained trunk skips activation / mask stores
@@ -328,8 +344,13 @@ class BwdScratch:
     elif plan.slab_cols:
       # zero-filled once: the normals backward writes only its first four (seven) columns
       self.dhead = torch.zeros(M, plan.slab_cols, device=dev, dtype=bf)
+    self.u = self.g = None
     if plan.density_normals:
       self.h = [torch.empty(3 * M, cfg.net_width, device=dev, dtype=bf) for _ in range(2)]    # tangent adjoints
+      if plan.act != L.ACT_RELU:
+        # the recomputed tangent before the activation factor, u = t_in W, and the second-order term of dL/dz
+        self.u = torch.empty(3 * M, cfg.net_width, device=dev, dtype=bf)
+        self.g = torch.empty(M, cfg.net_width, device=dev, dtype=bf)
 
 
 def _loss_args(loss_mults):
@@ -408,9 +429,12 @@ class Model:
       raise ValueError(f'raydist_fn {m.raydist_fn!r} not supported')
     if not m.stop_level_grad:
       raise NotImplementedError('stop_level_grad=False (gradients through resampling)')
-    self.plans = {'NerfMLP_0': MLPPlan(bundle.nerf_mlp, m.use_viewdirs, glo_features=m.num_glo_features)}
+    # every activation of the CUDA path: this class runs the smooth ones' buffers and backward schedule
+    acts = tuple(MLPPlan.ACTIVATIONS)
+    self.plans = {'NerfMLP_0': MLPPlan(bundle.nerf_mlp, m.use_viewdirs, glo_features=m.num_glo_features,
+                                       activations=acts)}
     if not m.single_mlp:
-      self.plans['PropMLP_0'] = MLPPlan(bundle.prop_mlp, m.use_viewdirs)
+      self.plans['PropMLP_0'] = MLPPlan(bundle.prop_mlp, m.use_viewdirs, activations=acts)
     for pname, plan in self.plans.items():
       for field, val in plan.device_constraints:
         if val % 64 != 0:
@@ -561,7 +585,11 @@ class Model:
         feat, copies = torch.empty(rows, plan.Fpad, device=dev, dtype=bf), []
       return acts, feat, copies
     st.acts, st.feat, st.feat_copies = trunk_buffers(M)
-    st.bits = [torch.empty(M, W // 32, device=dev, dtype=torch.int32) for _ in range(cfg.net_depth)]
+    relu = plan.act == L.ACT_RELU
+    if relu:
+      st.bits = [torch.empty(M, W // 32, device=dev, dtype=torch.int32) for _ in range(cfg.net_depth)]
+    else:
+      st.zs = [torch.empty(M, W, device=dev, dtype=bf) for _ in range(cfg.net_depth)]
     if plan.density_normals:
       # forward-mode tangents d(.)/d(mean_x|y|z), three stacked streams of M rows
       st.tacts, st.tfeat, st.tfeat_copies = trunk_buffers(3 * M)
@@ -580,7 +608,10 @@ class Model:
       nv = cfg.net_depth_viewdirs
       st.vacts = [torch.empty(M, Wv + plan.vin_pad if i in plan.view_concat_after else Wv, device=dev, dtype=bf)
                   for i in range(nv)]
-      st.vbits = [torch.empty(M, Wv // 32, device=dev, dtype=torch.int32) for _ in range(nv)]
+      if relu:
+        st.vbits = [torch.empty(M, Wv // 32, device=dev, dtype=torch.int32) for _ in range(nv)]
+      else:
+        st.vzs = [torch.empty(M, Wv, device=dev, dtype=bf) for _ in range(nv)]
       # the first layer whose output is concatenated with vin owns the vin columns, later ones get copies
       if plan.view_concat_after:
         st.vin = st.vacts[plan.view_concat_after[0]][:, Wv:]
@@ -600,6 +631,22 @@ class Model:
       st.extra_dw = torch.empty(B, S, device=dev)
     self._levels[key] = st
     return st
+
+  @staticmethod
+  def _act_out(plan, st, i, view=False):
+    """What the FWD GEMM of hidden layer i (trunk, or view MLP) keeps for the backward: ReLU mask bits, or the
+    pre-activation z of a smooth activation (not kept by a render-only pass)."""
+    if plan.act == L.ACT_RELU:
+      return dict(act=L.ACT_RELU, maskbits=(st.vbits if view else st.bits)[i])
+    return dict(act=plan.act, z=(st.vzs if view else st.zs)[i] if st.keep_acts else None)
+
+  @staticmethod
+  def _act_grad(plan, st, i, view=False, head=False):
+    """How a DGRAD (or, head=True, a head_bwd) applies the activation derivative of hidden layer i: ReLU mask bits
+    or a'(z)."""
+    if plan.act == L.ACT_RELU:
+      return dict(relu_mask=True) if head else dict(maskbits=(st.vbits if view else st.bits)[i])
+    return dict(act=plan.act, z=(st.vzs if view else st.zs)[i])
 
   def _refdir_args(self, st, mlp, rays):
     """The leading arguments of ops.refdir_fwd / refdir_bwd: descriptor, IDE tables and the stage's inputs."""
@@ -652,8 +699,8 @@ class Model:
       x = st.acts[-1]
     else:
       for i, sp in enumerate(plan.by_role('trunk')):
-        ops.gemm(L.GEMM_FWD, x, mlp.w_nk[sp.name], st.acts[i][:, :W], m=st.M, n=W, k=sp.in_pad, act=L.ACT_RELU,
-                 bias=mlp.b(sp), maskbits=st.bits[i], impl=impl)
+        ops.gemm(L.GEMM_FWD, x, mlp.w_nk[sp.name], st.acts[i][:, :W], m=st.M, n=W, k=sp.in_pad, bias=mlp.b(sp),
+                 impl=impl, **self._act_out(plan, st, i))
         x = st.acts[i]          # full width (incl. concatenated features) feeds the next layer
     if not chained or plan.last_has_feat:
       # stacked: density + rgb in one pass over the trunk output (bias block [b_density | b_rgb])
@@ -663,7 +710,8 @@ class Model:
 
   def _tangent_fwd(self, st, mlp, impl):
     """raw_grad_density = d raw_density / d mean by forward mode (replaces vmap(value_and_grad),
-    models.py:473-492): tangents see the same weights, no bias, and the primal's ReLU masks."""
+    models.py:473-492): tangents see the same weights, no bias, and the primal's activation derivative (ReLU masks,
+    or a'(z))."""
     plan = mlp.plan
     W = plan.cfg.net_width
     for c in st.tfeat_copies:
@@ -671,7 +719,7 @@ class Model:
     t = st.tfeat
     for i, sp in enumerate(plan.by_role('trunk')):
       ops.gemm(L.GEMM_DGRAD, t, mlp.w_nk[sp.name], st.tacts[i][:, :W], m=3 * st.M, n=W, k=sp.in_pad,
-               maskbits=st.bits[i], mask_mod=st.M, impl=impl)
+               mask_mod=st.M, impl=impl, **self._act_grad(plan, st, i))
       t = st.tacts[i]
     st.t_last = t
     d = plan.one('density')
@@ -709,7 +757,7 @@ class Model:
     for i, sp in enumerate(plan.by_role('view')):
       Wv = sp.out_dim
       ops.gemm(L.GEMM_FWD, v, mlp.w_nk[sp.name], st.vacts[i][:, :Wv], m=st.M, n=Wv, k=sp.in_pad,
-               act=L.ACT_RELU, bias=mlp.b(sp), maskbits=st.vbits[i], impl=impl)
+               bias=mlp.b(sp), impl=impl, **self._act_out(plan, st, i, view=True))
       v = st.vacts[i]
     st.v_last = v
     r = plan.one('rgb')
@@ -717,8 +765,8 @@ class Model:
 
   # ------------------------------------------------------------------ layer-chained 256-wide trunks
   def _use_chain(self, plan, M, impl=0):
-    """One persistent launch per trunk (csrc/chain.cu) when every trunk layer is 256 wide."""
-    if impl != 0 or os.environ.get('MNRF_CHAIN', '1') == '0':
+    """One persistent launch per trunk (csrc/chain.cu) when every trunk layer is 256 wide and uses ReLU."""
+    if impl != 0 or os.environ.get('MNRF_CHAIN', '1') == '0' or plan.act != L.ACT_RELU:
       return False
     cfg = plan.cfg
     return (cfg.net_width == 256 and cfg.net_depth <= L.CHAIN_MAX_LAYERS and M >= 512 and
@@ -959,9 +1007,9 @@ class Model:
     self._trunk_bwd(st, mlp, impl, chained)
 
   def _slab_dgrad(self, st, mlp, slab, impl):
-    """d x_last = relu'(x_last) * (slab @ wcat_kn^T): one dgrad over the head-gradient slab."""
+    """d x_last = act'(x_last) * (slab @ wcat_kn^T): one dgrad over the head-gradient slab."""
     ops.gemm(L.GEMM_DGRAD, slab, mlp.wcat_kn, st.bwd.dy[0], m=st.M, n=mlp.plan.cfg.net_width,
-             k=mlp.plan.slab_cols, maskbits=st.bits[-1], impl=impl)
+             k=mlp.plan.slab_cols, impl=impl, **self._act_grad(mlp.plan, st, -1))
 
   def _heads_bwd(self, st, mlp, rays, impl, lm, stats):
     """Top of a trunk without a view branch: colourless normals stage, density (or stacked) and narrow heads."""
@@ -983,8 +1031,8 @@ class Model:
     else:
       # input gradient, weight gradients and bias gradients ([b_density | b_rgb]) in one pass.  Features after a
       # skip are constants: dy holds the hidden columns only
-      ops.head_bwd(st.x_last, mlp.w_head, st.d_raw_head, plan.head_n, d.in_pad, dx=sc.dy[0], relu_mask=True,
-                   dw=mlp.W(d, g), db=mlp.b(d, g), dx_cols=plan.cfg.net_width, **split)
+      ops.head_bwd(st.x_last, mlp.w_head, st.d_raw_head, plan.head_n, d.in_pad, dx=sc.dy[0], dw=mlp.W(d, g),
+                   db=mlp.b(d, g), dx_cols=plan.cfg.net_width, **split, **self._act_grad(plan, st, -1, head=True))
 
   def _narrow_heads_bwd(self, st: LevelState, mlp: MLPDevice):
     """Parameter gradients of the narrow heads (x^T d_raw), accumulated into mlp.grads."""
@@ -1012,12 +1060,12 @@ class Model:
     dcur = sc.dv[0]
     if plan.rgb_vin == 'tail':
       # a view MLP ending on a skip: the head reads [hidden | vin]; the vin columns' gradient is the first part
-      ops.head_bwd(st.v_last, mlp.w_nk[r.name], d_rgb, r.out_dim, r.in_pad, dx=dcur, relu_mask=True, dw=mlp.W(r, g),
-                   db=mlp.b(r, g), dxsum=mlp.b(views[-1], g), dx_cols=Wv, dx2=parts[0])
+      ops.head_bwd(st.v_last, mlp.w_nk[r.name], d_rgb, r.out_dim, r.in_pad, dx=dcur, dw=mlp.W(r, g), db=mlp.b(r, g),
+                   dxsum=mlp.b(views[-1], g), dx_cols=Wv, dx2=parts[0], **self._act_grad(plan, st, -1, True, True))
       j = 1
     else:
-      ops.head_bwd(st.v_last, mlp.w_nk[r.name], d_rgb, r.out_dim, r.in_pad, dx=dcur, relu_mask=True, dw=mlp.W(r, g),
-                   db=mlp.b(r, g), dxsum=mlp.b(views[-1], g))
+      ops.head_bwd(st.v_last, mlp.w_nk[r.name], d_rgb, r.out_dim, r.in_pad, dx=dcur, dw=mlp.W(r, g), db=mlp.b(r, g),
+                   dxsum=mlp.b(views[-1], g), **self._act_grad(plan, st, -1, True, True))
     for i in range(len(views) - 1, -1, -1):
       sp = views[i]
       xin = st.vin if i == 0 else st.vacts[i - 1]
@@ -1029,8 +1077,8 @@ class Model:
                    addend=parts[(j - 1) % 2] if j else None, impl=impl)
           j += 1
         nxt = sc.dv[1] if dcur is sc.dv[0] else sc.dv[0]
-        ops.gemm(L.GEMM_DGRAD, dcur, mlp.w_kn[sp.name], nxt, m=st.M, n=Wv, k=Wv,
-                 maskbits=st.vbits[i - 1], colsum=mlp.b(views[i - 1], g), impl=impl)
+        ops.gemm(L.GEMM_DGRAD, dcur, mlp.w_kn[sp.name], nxt, m=st.M, n=Wv, k=Wv, colsum=mlp.b(views[i - 1], g),
+                 impl=impl, **self._act_grad(plan, st, i - 1, view=True))
         dcur = nxt
     # d vin = dcur * Wv0^T (+ the other consumers' parts)
     ops.gemm(L.GEMM_DGRAD, dcur, mlp.w_kn[views[0].name], sc.d_vin[:, :n], m=st.M, n=n, k=Wv,
@@ -1062,27 +1110,37 @@ class Model:
                      impl=impl)
     ops.head_bwd(st.x_last, st.x_last, st.d_raw_density.view(st.M, 1), 1, d.in_pad, dw=mlp.W(d, g).view(-1, 1))
     if plan.ref_stage:
-      # d x_last = relu'(x_last) * ([d bottleneck | head gradients] @ [W_b | w_heads]^T); without a bottleneck the
+      # d x_last = act'(x_last) * ([d bottleneck | head gradients] @ [W_b | w_heads]^T); without a bottleneck the
       # slab holds the head gradients only
       self._slab_dgrad(st, mlp, sc.d_vin, impl)
     else:
-      # d x_last = (dbott * Wb^T + d_raw_density (x) w_density) * relu'(x_last)
+      # d x_last = (dbott * Wb^T + d_raw_density (x) w_density) * act'(x_last)
       ops.gemm(L.GEMM_DGRAD, sc.d_vin[:, :bw], mlp.w_kn[bt.name], sc.dy[0], m=st.M, n=plan.cfg.net_width, k=bw,
-               rowv=st.d_raw_density.view(st.M), colv=mlp.colv_density, maskbits=st.bits[-1], impl=impl)
+               rowv=st.d_raw_density.view(st.M), colv=mlp.colv_density, impl=impl, **self._act_grad(plan, st, -1))
     # bias gradient of the density head: a plain sum of d_raw_density
     mlp.b(d, g).add_(st.d_raw_density.sum())
 
   def _tangent_bwd(self, st, mlp, impl):
-    """Adjoint of the tangent chain: H_last = relu'(x_last) * (d_rgd (x) w_density), three streams."""
+    """Adjoint of the tangent chain: H_last = relu'(x_last) * (d_rgd (x) w_density), three streams.
+
+    A smooth activation starts the chain with H_last = a'(z_last) * T_last, T_last = d_rgd (x) w_density, and adds the
+    second-order term a''(z_last) * sum_s T_last u_last into the trunk-top gradient dy[0]; its layers below run
+    interleaved with the trunk backward (_trunk_bwd)."""
     plan = mlp.plan
     sc, g = st.bwd, mlp.grads
     W = plan.cfg.net_width
     d = plan.one('density')
     trunk = plan.by_role('trunk')
     hcur, hoth = sc.h[0], sc.h[1]
-    ops.outer_mask(st.d_rgd.view(3 * st.M), mlp.colv_density, st.bits[-1], hcur, rows=3 * st.M, n=W, mask_mod=st.M)
+    relu = plan.act == L.ACT_RELU
+    ops.outer_mask(st.d_rgd.view(3 * st.M), mlp.colv_density, st.bits[-1] if relu else None, hcur, rows=3 * st.M,
+                   n=W, mask_mod=st.M)
+    if not relu:
+      self._tangent_second_order(st, mlp, len(trunk) - 1, hcur, sc.dy[0], impl)
     ops.head_bwd(st.t_last, mlp.w_nk[d.name], st.d_rgd.view(3 * st.M, 1), 1, d.in_pad, dx=None,
                  dw=mlp.W(d, g), db=None)
+    if not relu:
+      return
     for i in range(len(trunk) - 1, -1, -1):
       sp = trunk[i]
       tin = st.tfeat if i == 0 else st.tacts[i - 1]
@@ -1092,11 +1150,25 @@ class Model:
                  maskbits=st.bits[i - 1], mask_mod=st.M, impl=impl)
         hcur, hoth = hoth, hcur
 
+  def _tangent_second_order(self, st, mlp, i, t_adj, g_out, impl):
+    """Trunk layer i of the tangent backward through a smooth activation: t_adj = T_i = dL/dt_i (three streams)
+    becomes dL/du_i = a'(z_i) T_i in place, and g_out receives (dy[0], the trunk-top gradient: is added) the
+    second-order part of dL/dz_i, a''(z_i) sum_s T_i u_i.  u_i = t_{i-1} W_i is not stored by the forward: it is
+    recomputed here from the stored tangent input of the layer (features included after a skip)."""
+    plan = mlp.plan
+    sc, sp = st.bwd, plan.by_role('trunk')[i]
+    tin = st.tfeat if i == 0 else st.tacts[i - 1]
+    ops.gemm(L.GEMM_FWD, tin, mlp.w_nk[sp.name], sc.u, m=3 * st.M, n=plan.cfg.net_width, k=sp.in_pad, impl=impl)
+    ops.act_tangent_bwd(plan.act, st.zs[i], t_adj, sc.u, t_adj, g_out, accumulate=g_out is sc.dy[0])
+
   def _trunk_bwd(self, st, mlp, impl, chained):
-    """Trunk backward from dy[0] = d loss / d (output of the last trunk layer)."""
+    """Trunk backward from dy[0] = d loss / d (output of the last trunk layer).  With density normals through a
+    smooth activation, the tangent chain (sc.h, from _tangent_bwd) runs here too, one layer ahead: its layer i - 1
+    yields the second-order term g that the primal DGRAD into layer i - 1 adds."""
     sc, g = st.bwd, mlp.grads
-    W = mlp.plan.cfg.net_width
-    trunk = mlp.plan.by_role('trunk')
+    plan = mlp.plan
+    W = plan.cfg.net_width
+    trunk = plan.by_role('trunk')
     nl = len(trunk)
     if chained:
       # dyl[i] = d loss / d (output of trunk layer i); dyl[nl-1] is sc.dy[0], produced at the top of the trunk
@@ -1108,14 +1180,25 @@ class Model:
                        impl=impl)
       return
     cur, other = sc.dy[0], sc.dy[1]
+    tangent = plan.density_normals and plan.act != L.ACT_RELU
+    hcur, hoth = sc.h if tangent else (None, None)
     for i in range(nl - 1, -1, -1):
       sp = trunk[i]
       xin = st.feat if i == 0 else st.acts[i - 1]
       ops.gemm_wgrad(xin, cur, mlp.W(sp, g), m=sp.in_pad, n=W, k=st.M, bsum=mlp.b(sp, g), impl=impl)
+      if tangent:
+        tin = st.tfeat if i == 0 else st.tacts[i - 1]
+        ops.gemm(L.GEMM_WGRAD, tin, hcur, mlp.W(sp, g), m=sp.in_pad, n=W, k=3 * st.M, impl=impl)
       if i > 0:
+        if tangent:
+          # T_{i-1} = dL/du_i W_i^T, then dL/du_{i-1} (in place) and the second-order term g of layer i - 1
+          ops.gemm(L.GEMM_DGRAD, hcur, mlp.w_kn[sp.name], hoth, m=3 * st.M, n=W, k=W, impl=impl)
+          self._tangent_second_order(st, mlp, i - 1, hoth, sc.g, impl)
+          hcur, hoth = hoth, hcur
         # only the hidden part of the input carries gradient (features are constants:
         # stop_gradient(sdist), models.py:200-201)
-        ops.gemm(L.GEMM_DGRAD, cur, mlp.w_kn[sp.name], other, m=st.M, n=W, k=W, maskbits=st.bits[i - 1], impl=impl)
+        ops.gemm(L.GEMM_DGRAD, cur, mlp.w_kn[sp.name], other, m=st.M, n=W, k=W, addend=sc.g if tangent else None,
+                 impl=impl, **self._act_grad(plan, st, i - 1))
         cur, other = other, cur
 
 

@@ -139,10 +139,11 @@ def viewdir_enc(viewdirs, num_samples, deg, out, col0, col_end):
 
 
 def gemm(mode, a, b, out, *, m, n, k, act=L.ACT_NONE, bias=None, rowv=None, colv=None, mask=None,
-         maskbits=None, colsum=None, mask_mod=0, addend=None, impl=0):
-  """Dense-layer GEMM (see include/mnrf.h).  a/b/out/mask are 2-D views with unit inner stride."""
+         maskbits=None, colsum=None, mask_mod=0, addend=None, z=None, impl=0):
+  """Dense-layer GEMM (see include/mnrf.h).  a/b/out/mask/z are 2-D views with unit inner stride.  A smooth `act`
+  (L.SMOOTH_ACTS) runs mnrf_gemm_act: FWD writes the pre-activation to z (optional), DGRAD multiplies by a'(z)."""
   lib = L.load()
-  for t in (a, b, out) + ((mask,) if mask is not None else ()):
+  for t in (a, b, out) + tuple(t for t in (mask, z) if t is not None):
     assert t.stride(-1) == 1
   if maskbits is not None:
     assert maskbits.dtype == torch.int32 and maskbits.stride(-1) == 1
@@ -155,8 +156,15 @@ def gemm(mode, a, b, out, *, m, n, k, act=L.ACT_NONE, bias=None, rowv=None, colv
   if GEMM_EVENTS is not None:
     ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
     ev[0].record()
-  L.check(lib.mnrf_gemm(C.byref(d), L.ptr(a), L.ptr(b), L.ptr(bias), L.ptr(rowv), L.ptr(colv),
-                        L.ptr(mask), L.ptr(maskbits), L.ptr(colsum), L.ptr(addend), L.ptr(out), L.stream_ptr()))
+  if act in L.SMOOTH_ACTS and mode != L.GEMM_WGRAD:
+    assert mask is None and maskbits is None and (z is None or z.dtype == torch.bfloat16)
+    L.check(lib.mnrf_gemm_act(C.byref(d), L.ptr(a), L.ptr(b), L.ptr(bias), L.ptr(rowv), L.ptr(colv), L.ptr(colsum),
+                              L.ptr(addend), L.ptr(z), z.stride(0) if z is not None else 0, L.ptr(out),
+                              L.stream_ptr()))
+  else:
+    assert z is None, 'z is the pre-activation of a smooth activation'
+    L.check(lib.mnrf_gemm(C.byref(d), L.ptr(a), L.ptr(b), L.ptr(bias), L.ptr(rowv), L.ptr(colv),
+                          L.ptr(mask), L.ptr(maskbits), L.ptr(colsum), L.ptr(addend), L.ptr(out), L.stream_ptr()))
   if ev is not None:
     ev[1].record()
     GEMM_EVENTS.append((ev[0], ev[1], 2.0 * m * n * k))
@@ -251,13 +259,20 @@ def head_fwd(x, w_nk, bias, n_out, k, raw=None):
 
 
 def head_bwd(x, w_nk, draw, n_out, k, dx=None, relu_mask=False, dw=None, db=None, dxsum=None, dw2=None, dw_split=0,
-             dx_cols=0, dx2=None):
+             dx_cols=0, dx2=None, act=L.ACT_NONE, z=None):
   """dw2 / dw_split: outputs [dw_split, n_out) put their weight gradient in dw2; dx_cols: dx and dxsum cover the
   first dx_cols columns only; dx2 [M, k - dx_cols]: the input gradient of the columns past dx_cols, unmasked
-  (include/mnrf.h)."""
+  (include/mnrf.h).  z (with a smooth `act`, instead of relu_mask): dx *= a'(z), z the pre-activation of x."""
   lib = L.load()
   M = x.shape[0]
   _count()
+  if z is not None:
+    assert not relu_mask and z.dtype == torch.bfloat16 and z.stride(-1) == 1
+    L.check(lib.mnrf_head_bwd_act(M, k, n_out, L.ptr(x), x.stride(0), L.ptr(w_nk), L.ptr(_f32(draw)), L.ptr(dx),
+                                  dx.stride(0), act, L.ptr(z), z.stride(0), L.ptr(dw), L.ptr(dw2), int(dw_split),
+                                  L.ptr(db), L.ptr(dxsum), int(dx_cols), L.ptr(dx2),
+                                  dx2.stride(0) if dx2 is not None else 0, L.stream_ptr()))
+    return
   L.check(lib.mnrf_head_bwd(M, k, n_out, L.ptr(x), x.stride(0), L.ptr(w_nk), L.ptr(_f32(draw)),
                             L.ptr(dx), dx.stride(0) if dx is not None else 0, int(relu_mask),
                             L.ptr(dw), L.ptr(dw2), int(dw_split), L.ptr(db), L.ptr(dxsum), int(dx_cols),
@@ -489,3 +504,17 @@ def outer_mask(rowv, colv, maskbits, out, *, rows, n, mask_mod=0):
   L.check(lib.mnrf_outer_mask(rows, n, mask_mod, L.ptr(_f32(rowv)), L.ptr(_f32(colv)), L.ptr(maskbits),
                               maskbits.stride(0) if maskbits is not None else 0, L.ptr(out), out.stride(0),
                               L.stream_ptr()))
+
+
+def act_tangent_bwd(act, z, t_adj, u, du, g, *, accumulate=False):
+  """One trunk layer of the density-normal backward through a smooth activation (include/mnrf.h): du = a'(z) T per
+  tangent stream, g (+)= a''(z) sum_s T_s u_s.  z, g [M, n]; t_adj, u, du [3M, n] (du may be t_adj); bf16."""
+  lib = L.load()
+  M, n = z.shape
+  for t in (z, t_adj, u, du, g):
+    assert t.dtype == torch.bfloat16 and t.stride(-1) == 1
+  assert t_adj.shape[0] == u.shape[0] == du.shape[0] == 3 * M
+  _count()
+  L.check(lib.mnrf_act_tangent_bwd(M, n, act, L.ptr(z), z.stride(0), L.ptr(t_adj), t_adj.stride(0), L.ptr(u),
+                                   u.stride(0), L.ptr(du), du.stride(0), L.ptr(g), g.stride(0), int(accumulate),
+                                   L.stream_ptr()))
