@@ -127,8 +127,9 @@ int mnrf_viewdir_enc(int32_t num_rays, int32_t num_samples, int32_t deg, const f
  *               (A = dY, Bt = W in [in,out] layout; mask = stored activation; all optional)
  *   mode WGRAD: out[Mo,N] fp32 += A[R,Mo]^T * B[R,N]   (A = X, B = dY, both row-major with
  *               the reduction index R on rows: "MN-major" operands), split over R, fp32 atomics
- * All leading dimensions are in elements.  K (or R) must be a multiple of 64 (16 for R),
- * M-tiles are 128 rows; N must be a multiple of 16.
+ * All leading dimensions are in elements.  FWD / DGRAD: K must be a multiple of 64 and N a multiple
+ * of 16.  WGRAD: R may be any count (the last 64-row reduction block is zero-filled past R) and N a
+ * multiple of 64.  M-tiles are 128 rows; M (Mo) may be any count.
  */
 enum { MNRF_GEMM_FWD = 0, MNRF_GEMM_DGRAD = 1, MNRF_GEMM_WGRAD = 2 };
 /* Activations of the Dense layers (MLP.net_activation, models.py:457,578): SOFTPLUS is jax.nn.softplus
@@ -143,7 +144,8 @@ typedef struct {
   int64_t ldmaskbits; /* row pitch of `maskbits` in 32-bit words */
   int64_t ldadd;      /* row pitch of `addend` */
   int64_t mask_mod;   /* > 0: mask row = output row mod mask_mod (the 3 stacked tangent streams of the
-                         density-normal chain share the primal's ReLU masks); 0: mask row = output row */
+                         density-normal chain share the primal's ReLU masks); 0: mask row = output row.
+                         Applies to `maskbits` and z; a bf16 `mask` with mask_mod > 0 is refused */
   int32_t impl;       /* 0 = wgmma (product path);   1 = SIMT reference kernel (bring-up/tests) */
 } mnrf_gemm_desc;
 
@@ -181,6 +183,25 @@ int mnrf_gemm_act(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* 
  *                                                        side_w = its d(raw output), models.py:460) */
 int mnrf_gemm_wgrad(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, float* bsum,
                     const float* side_w, float* side_aw, float* out, mnrf_stream stream);
+
+/* The kernel instance and launch shape the tensor-core path (impl 0) of mnrf_gemm / mnrf_gemm_act /
+ * mnrf_gemm_wgrad chooses for these arguments, which take the places they have there (z / ldz: mnrf_gemm_act;
+ * bsum / side_w / side_aw: mnrf_gemm_wgrad; null where the call has none).  Host-only: no pointer is dereferenced
+ * and nothing is launched.  Returns nonzero, with the launch's error message, for arguments the launch refuses. */
+typedef struct {
+  int32_t block_n;    /* output tile width BN: 256, 128, 64, 32 or 16 */
+  int32_t staged;     /* 1: the bf16 output goes through shared memory and TMA bulk stores; 0: register stores */
+  int32_t mask_tma;   /* DGRAD mask bits: 1 loaded by TMA with the operands; 0 loaded by the epilogue (or none) */
+  int32_t smooth;     /* softplus / SiLU epilogue (mnrf_gemm_act) */
+  int32_t side;       /* WGRAD side sums (bsum / side_aw) */
+  int32_t splits;     /* reduction splits (WGRAD; 1 otherwise) */
+  int32_t tiles;      /* work items: row blocks x column blocks x splits */
+  int32_t grid;       /* persistent CTAs */
+} mnrf_gemm_instance;
+int mnrf_gemm_plan(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
+                   const float* rowv, const float* colv, const mnrf_bf16* mask, const uint32_t* maskbits,
+                   const float* colsum, const mnrf_bf16* addend, const mnrf_bf16* z, int64_t ldz, const void* out,
+                   const float* bsum, const float* side_w, const float* side_aw, mnrf_gemm_instance* plan);
 
 /* ---- layer-chained 256-wide MLP trunk ------------------------------------------------------
  * ONE persistent launch walks 512-row units of samples through all Dense layers of a 256-wide trunk

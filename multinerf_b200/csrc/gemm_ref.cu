@@ -93,6 +93,8 @@ static int gemm_dispatch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf
   MNRF_CHECK(d && a && b && out, "mnrf_gemm: null pointer");
   MNRF_CHECK(d->mode >= 0 && d->mode <= 2, "mnrf_gemm: unknown mode %d", d->mode);
   MNRF_CHECK((rowv == nullptr) == (colv == nullptr), "mnrf_gemm: rowv and colv come together");
+  // the bf16 mask has a row per output row (mask_mod is for the 1-bit masks and z of the stacked tangent streams)
+  MNRF_CHECK(!mask || d->mask_mod == 0, "mnrf_gemm: mask_mod applies to maskbits and z, not to a bf16 mask");
   if (d->m == 0 || d->n == 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
   if (colsum) MNRF_CHECK(d->mode == MNRF_GEMM_DGRAD, "mnrf_gemm: colsum is a DGRAD output");

@@ -553,43 +553,29 @@ static int pick_block_n(int n) {
   return 0;
 }
 
-int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
-                   const float* rowv, const float* colv, const mnrf_bf16* mask, uint32_t* maskbits,
-                   float* colsum, const mnrf_bf16* addend, void* out, cudaStream_t stream, float* bsum,
-                   const float* side_w, float* side_aw, mnrf_bf16* z, int64_t ldz) {
+// The host-side choices of gemm_tc_launch, after every argument check: tile width, store path, where DGRAD's mask
+// bits come from, instance family, reduction splits and grid.  Dereferences nothing (mnrf_gemm_plan).
+static int gemm_tc_plan(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
+                        const float* colv, const mnrf_bf16* mask, const uint32_t* maskbits, const float* colsum,
+                        const mnrf_bf16* addend, const void* out, const float* bsum, const float* side_w,
+                        const float* side_aw, const mnrf_bf16* z, int64_t ldz, mnrf_gemm_instance* plan) {
   // K-major modes: the reduction index is the contiguous one and layers are padded to 64.  WGRAD reduces
   // over the sample rows, any count: the last 64-row block is zero-filled by TMA past the tensor's end.
   MNRF_CHECK(d->mode == MNRF_GEMM_WGRAD || d->k % BLOCK_K == 0,
              "mnrf_gemm(tc): reduction length %d must be a multiple of %d", d->k, BLOCK_K);
   MNRF_CHECK(d->lda % 8 == 0 && d->ldb % 8 == 0 && ((uintptr_t)a % 16) == 0 && ((uintptr_t)b % 16) == 0,
              "mnrf_gemm(tc): operands must be 16-byte aligned with ld %% 8 == 0");
-  GemmParams p{};
-  p.mode = d->mode; p.act = d->act; p.m = d->m; p.n = d->n; p.k = d->k;
   const int block_n = pick_block_n(d->n);
   MNRF_CHECK(block_n > 0, "mnrf_gemm(tc): N=%d must be a multiple of 16", d->n);
   if (d->mode == MNRF_GEMM_WGRAD)
     MNRF_CHECK(block_n >= 64, "mnrf_gemm(tc): WGRAD needs N %% 64 == 0 (MN-major 128-byte atoms), N=%d", d->n);
-  p.num_m_blocks = (int)((d->m + BLOCK_M - 1) / BLOCK_M);
-  p.num_n_blocks = d->n / block_n;
-  p.num_k_blocks = (d->k + BLOCK_K - 1) / BLOCK_K;
-  p.ldc = d->ldc; p.ldmask = d->ldmask;
-  p.bias = bias; p.rowv = rowv; p.colv = colv;
-  p.mask = reinterpret_cast<const __nv_bfloat16*>(mask);
-  p.out = out;
-  p.maskbits = maskbits;
-  p.ldmaskbits = d->ldmaskbits;
-  p.mask_mod = d->mask_mod;
-  p.addend = reinterpret_cast<const __nv_bfloat16*>(addend);
-  p.ldadd = d->ldadd;
   if (addend) MNRF_CHECK(d->mode == MNRF_GEMM_DGRAD && d->ldadd % 2 == 0 && ((uintptr_t)addend % 4) == 0,
                          "mnrf_gemm(tc): addend is a DGRAD input with 4-byte aligned rows");
-  p.colsum = colsum;
   if (colsum) MNRF_CHECK(d->mode == MNRF_GEMM_DGRAD && d->n <= CS_MAX,
                          "mnrf_gemm(tc): colsum is a DGRAD output of at most %d columns", CS_MAX);
   const bool side = bsum != nullptr || side_aw != nullptr;
   if (side) MNRF_CHECK(d->mode == MNRF_GEMM_WGRAD && (side_w == nullptr) == (side_aw == nullptr),
                        "mnrf_gemm(tc): side sums are WGRAD outputs; side_w and side_aw come together");
-  p.bsum = bsum; p.side_w = side_w; p.side_aw = side_aw;
   if (maskbits) {
     MNRF_CHECK(d->mode != MNRF_GEMM_WGRAD, "mnrf_gemm(tc): maskbits make no sense for WGRAD");
     MNRF_CHECK(d->n % 32 == 0 && block_n % 32 == 0 && d->ldmaskbits * 32 >= d->n,
@@ -601,43 +587,91 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
     MNRF_CHECK(d->mode == MNRF_GEMM_FWD || z, "mnrf_gemm(tc): the DGRAD of a smooth activation needs z");
     MNRF_CHECK(!z || (ldz % 2 == 0 && ((uintptr_t)z % 4) == 0), "mnrf_gemm(tc): z must be 4-byte aligned");
   }
-  if (smooth) {
-    p.mask = reinterpret_cast<const __nv_bfloat16*>(z);
-    p.ldmask = ldz;
-  }
   if (bias) MNRF_CHECK(((uintptr_t)bias % 8) == 0, "mnrf_gemm(tc): bias must be 8-byte aligned");
   if (colv) MNRF_CHECK(((uintptr_t)colv % 8) == 0, "mnrf_gemm(tc): colv must be 8-byte aligned");
   const int workers = mnrf_num_sms();
-  p.num_splits = 1;
+  const int num_m_blocks = (int)((d->m + BLOCK_M - 1) / BLOCK_M);
+  const int num_n_blocks = d->n / block_n;
+  const int num_k_blocks = (d->k + BLOCK_K - 1) / BLOCK_K;
+  int num_splits = 1;
   if (d->mode == MNRF_GEMM_WGRAD) {
     // Split the reduction over the sample rows so that (output tiles x splits) work items fill whole rounds of the
     // workers -- with the FEWEST splits that do: every work item ends in an fp32 reduction pass over its output
     // tile, and for a one-tile weight gradient (PropMLP 256 x 256) those passes all hit the same 256 KB of L2.
-    const int out_tiles = p.num_m_blocks * p.num_n_blocks;
-    const int max_splits = std::min(std::max(1, (2 * workers) / out_tiles), p.num_k_blocks);
+    const int out_tiles = num_m_blocks * num_n_blocks;
+    const int max_splits = std::min(std::max(1, (2 * workers) / out_tiles), num_k_blocks);
     int splits = max_splits;
     for (int sp = 1; sp <= max_splits; ++sp) {
       const int items = out_tiles * sp;
       const int rounds = (items + workers - 1) / workers;
       if (items * 100 >= rounds * workers * 95) { splits = sp; break; }
     }
-    p.num_splits = splits;
+    num_splits = splits;
   }
-  p.kblocks_per_split = (p.num_k_blocks + p.num_splits - 1) / p.num_splits;
-  p.num_splits = (p.num_k_blocks + p.kblocks_per_split - 1) / p.kblocks_per_split;
+  const int kblocks_per_split = (num_k_blocks + num_splits - 1) / num_splits;
+  num_splits = (num_k_blocks + kblocks_per_split - 1) / kblocks_per_split;
   if (d->mode != MNRF_GEMM_WGRAD) {
     MNRF_CHECK(d->ldc % 2 == 0 && ((uintptr_t)out % 4) == 0, "mnrf_gemm(tc): bf16 output must be 4-byte aligned");
     if (mask) MNRF_CHECK(d->ldmask % 2 == 0 && ((uintptr_t)mask % 4) == 0, "mnrf_gemm(tc): mask must be 4-byte aligned");
   } else {
     MNRF_CHECK(d->ldc % 2 == 0 && ((uintptr_t)out % 8) == 0, "mnrf_gemm(tc): fp32 output must be 8-byte aligned");
   }
-
   // The bf16 output goes through the staged bulk store when its tiles are whole 128-byte swizzle spans and TMA can
   // address it (16-byte aligned base and row pitch); otherwise the epilogue stores from registers.
   const bool ts = d->mode != MNRF_GEMM_WGRAD && block_n >= 64 && ((uintptr_t)out % 16) == 0 && d->ldc % 8 == 0;
   // the smooth epilogues exist for the staged store only: every hidden layer is a multiple of 64 wide
   MNRF_CHECK(!smooth || ts, "mnrf_gemm(tc): a smooth activation needs N %% 64 == 0 and a 16-byte aligned output "
              "with a row pitch that is a multiple of 8");
+  // DGRAD mask bits go through TMA when the tile is at least 128 columns wide and the mask rows of a 128-row tile
+  // are 128 consecutive rows of a TMA-addressable array (16-byte aligned base and row pitch); otherwise the
+  // epilogue loads them itself.
+  const bool mask_tma = d->mode == MNRF_GEMM_DGRAD && maskbits && mask_words(block_n) > 0 && d->ldmaskbits % 4 == 0 &&
+                        ((uintptr_t)maskbits % 16) == 0 && (d->mask_mod == 0 || d->mask_mod % BLOCK_M == 0);
+  const int tiles = num_m_blocks * num_n_blocks * num_splits;
+  plan->block_n = block_n;
+  plan->staged = ts;
+  plan->mask_tma = mask_tma;
+  plan->smooth = smooth;
+  plan->side = side;
+  plan->splits = num_splits;
+  plan->tiles = tiles;
+  plan->grid = std::min(tiles, workers);
+  return 0;
+}
+
+int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
+                   const float* rowv, const float* colv, const mnrf_bf16* mask, uint32_t* maskbits,
+                   float* colsum, const mnrf_bf16* addend, void* out, cudaStream_t stream, float* bsum,
+                   const float* side_w, float* side_aw, mnrf_bf16* z, int64_t ldz) {
+  mnrf_gemm_instance plan;
+  if (int rc = gemm_tc_plan(d, a, b, bias, colv, mask, maskbits, colsum, addend, out, bsum, side_w, side_aw, z, ldz,
+                            &plan))
+    return rc;
+  const int block_n = plan.block_n;
+  const bool ts = plan.staged, side = plan.side, smooth = plan.smooth;
+  GemmParams p{};
+  p.mode = d->mode; p.act = d->act; p.m = d->m; p.n = d->n; p.k = d->k;
+  p.num_m_blocks = (int)((d->m + BLOCK_M - 1) / BLOCK_M);
+  p.num_n_blocks = d->n / block_n;
+  p.num_k_blocks = (d->k + BLOCK_K - 1) / BLOCK_K;
+  p.num_splits = plan.splits;
+  p.kblocks_per_split = (p.num_k_blocks + p.num_splits - 1) / p.num_splits;
+  p.ldc = d->ldc; p.ldmask = d->ldmask;
+  p.bias = bias; p.rowv = rowv; p.colv = colv;
+  p.mask = reinterpret_cast<const __nv_bfloat16*>(mask);
+  p.out = out;
+  p.maskbits = maskbits;
+  p.ldmaskbits = d->ldmaskbits;
+  p.mask_mod = d->mask_mod;
+  p.addend = reinterpret_cast<const __nv_bfloat16*>(addend);
+  p.ldadd = d->ldadd;
+  p.colsum = colsum;
+  p.bsum = bsum; p.side_w = side_w; p.side_aw = side_aw;
+  if (smooth) {
+    p.mask = reinterpret_cast<const __nv_bfloat16*>(z);
+    p.ldmask = ldz;
+  }
+  p.mask_tma = plan.mask_tma;
   CUtensorMap ta, tb, tc;
   if (d->mode != MNRF_GEMM_WGRAD) {
     if (make_tmap(&ta, a, d->m, d->k, d->lda, BLOCK_K, BLOCK_M)) return 1;
@@ -652,19 +686,13 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
   } else {
     tc = tb;   // not read
   }
-  // DGRAD mask bits go through TMA when the tile is at least 128 columns wide and the mask rows of a 128-row tile
-  // are 128 consecutive rows of a TMA-addressable array (16-byte aligned base and row pitch); otherwise the
-  // epilogue loads them itself.
   CUtensorMap tm = tb;   // not read unless p.mask_tma
-  p.mask_tma = d->mode == MNRF_GEMM_DGRAD && maskbits && mask_words(block_n) > 0 && d->ldmaskbits % 4 == 0 &&
-               ((uintptr_t)maskbits % 16) == 0 && (d->mask_mod == 0 || d->mask_mod % BLOCK_M == 0);
   if (p.mask_tma &&
       make_tmap(&tm, maskbits, d->mask_mod > 0 ? d->mask_mod : d->m, d->n / 32, d->ldmaskbits,
                 mask_words(block_n), BLOCK_M, CU_TENSOR_MAP_DATA_TYPE_UINT32, 4,
                 CU_TENSOR_MAP_SWIZZLE_NONE))
     return 1;
-  const int total_tiles = p.num_m_blocks * p.num_n_blocks * p.num_splits;
-  const int grid = std::min(total_tiles, workers);
+  const int grid = plan.grid;
   if (grid == 0) return 0;
 #define MNRF_LAUNCH_TC3(MODE_, BN_, TS_, SIDE_)                                                       \
   do {                                                                                                \
@@ -697,3 +725,17 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
 #endif  // MNRF_GEMM_TC_SMOOTH_UNIT
 
 }  // namespace mnrf
+
+#ifndef MNRF_GEMM_TC_SMOOTH_UNIT
+extern "C" int mnrf_gemm_plan(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
+                              const float* rowv, const float* colv, const mnrf_bf16* mask, const uint32_t* maskbits,
+                              const float* colsum, const mnrf_bf16* addend, const mnrf_bf16* z, int64_t ldz,
+                              const void* out, const float* bsum, const float* side_w, const float* side_aw,
+                              mnrf_gemm_instance* plan) {
+  MNRF_CHECK(d && plan, "mnrf_gemm_plan: null pointer");
+  MNRF_CHECK((rowv == nullptr) == (colv == nullptr), "mnrf_gemm: rowv and colv come together");
+  MNRF_CHECK(!mask || d->mask_mod == 0, "mnrf_gemm: mask_mod applies to maskbits and z, not to a bf16 mask");
+  return mnrf::gemm_tc_plan(d, a, b, bias, colv, mask, maskbits, colsum, addend, out, bsum, side_w, side_aw, z, ldz,
+                            plan);
+}
+#endif

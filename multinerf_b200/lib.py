@@ -40,6 +40,11 @@ class GemmDesc(C.Structure):
               ('impl', C.c_int32)]
 
 
+class GemmInstance(C.Structure):
+  _fields_ = [('block_n', C.c_int32), ('staged', C.c_int32), ('mask_tma', C.c_int32), ('smooth', C.c_int32),
+              ('side', C.c_int32), ('splits', C.c_int32), ('tiles', C.c_int32), ('grid', C.c_int32)]
+
+
 class CompositeDesc(C.Structure):
   _fields_ = [('num_rays', C.c_int32), ('num_samples', C.c_int32), ('raydist_fn', C.c_int32),
               ('opaque_background', C.c_int32), ('density_bias', C.c_float),
@@ -133,6 +138,8 @@ _SIGNATURES = {
     'mnrf_gemm': (C.c_int, [C.POINTER(GemmDesc)] + [_P] * 11),
     'mnrf_gemm_act': (C.c_int, [C.POINTER(GemmDesc)] + [_P] * 8 + [C.c_int64, _P, _P]),
     'mnrf_gemm_wgrad': (C.c_int, [C.POINTER(GemmDesc)] + [_P] * 7),
+    'mnrf_gemm_plan': (C.c_int, [C.POINTER(GemmDesc)] + [_P] * 10 + [C.c_int64] + [_P] * 4 +
+                       [C.POINTER(GemmInstance)]),
     'mnrf_mlp_chain': (C.c_int, [C.POINTER(ChainDesc), _P]),
     'mnrf_mlp_chain_max_layers': (C.c_int, []),
     'mnrf_head_fwd': (C.c_int, [C.c_int64, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P, _P, _P]),

@@ -195,6 +195,24 @@ def gemm_wgrad(x, dy, out, *, m, n, k, bsum=None, side_w=None, side_aw=None, imp
   return out
 
 
+def gemm_plan(mode, a, b, out, *, m, n, k, act=L.ACT_NONE, bias=None, rowv=None, colv=None, mask=None,
+              maskbits=None, colsum=None, mask_mod=0, addend=None, z=None, bsum=None, side_w=None, side_aw=None):
+  """The tensor-core instance that gemm (or gemm_wgrad, with bsum / side_w / side_aw) launches for these arguments:
+  a dict of the fields of mnrf_gemm_instance (include/mnrf.h).  Reads only shapes, strides and addresses, so the
+  tensors may live on any device."""
+  lib = L.load()
+  def p(t):
+    return None if t is None else C.c_void_p(t.data_ptr())
+  def ld(t):
+    return t.stride(0) if t is not None else 0
+  d = L.GemmDesc(mode, act, m, n, k, a.stride(0), b.stride(0), out.stride(0), ld(mask), ld(maskbits), ld(addend),
+                 mask_mod, 0)
+  plan = L.GemmInstance()
+  L.check(lib.mnrf_gemm_plan(C.byref(d), p(a), p(b), p(bias), p(rowv), p(colv), p(mask), p(maskbits), p(colsum),
+                             p(addend), p(z), ld(z), p(out), p(bsum), p(side_w), p(side_aw), C.byref(plan)))
+  return {name: int(getattr(plan, name)) for name, _ in L.GemmInstance._fields_}
+
+
 def chain_desc(mode, m, layers, *, stream=None, stream_cols=0, head_w=None, head_b=None, head_out=None, head_n=1):
   """Descriptor of one layer-chained launch (include/mnrf.h mnrf_chain_desc).  head_w [head_n, 256] fp32, head_out
   [m, head_n]: the narrow head of the last layer's epilogue (head_n 1 or 4).  layers: list of dicts with

@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 import torch
 
+from gemm_ref import pack_bits as _pack
 from util import close
 
 pytestmark = pytest.mark.gpu
@@ -20,16 +21,6 @@ def ops():
 
 def _bf(x):
   return torch.tensor(x).to(torch.bfloat16)
-
-
-def _pack(maskb, words_pitch):
-  """[rows, N] bool -> [rows, words_pitch] int32 mask words (bit j of word w <-> column 32w + j), zero padded."""
-  rows, n = maskb.shape
-  words = (maskb.reshape(rows, n // 32, 32).long() << torch.arange(32)).sum(-1)
-  words = torch.where(words >= 2 ** 31, words - 2 ** 32, words).to(torch.int32)
-  out = torch.zeros(rows, words_pitch, dtype=torch.int32)
-  out[:, :n // 32] = words
-  return out
 
 
 # N = 640 and N = 320 run 5 column blocks (of 128 and 64) on 132 SMs, so a CTA's consecutive tiles change column
