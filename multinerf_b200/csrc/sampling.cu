@@ -148,7 +148,9 @@ sample_level_kernel(mnrf_sample_desc d, const float* __restrict__ sdist_prev,
       se = warp_sum(se);
       __syncwarp();
       // cw = [0, min(1, cumsum(w[:-1])), 1]: lane L owns a contiguous chunk (sequential adds
-      // inside it), chunk offsets come from a warp shuffle scan of the chunk sums.
+      // inside it), chunk offsets come from a warp shuffle scan of the chunk sums.  The min keeps
+      // a NaN (all logits -inf, or anneal 0 times log 0) as jnp.minimum does, where fminf would
+      // drop it: the samples of such a ray then collapse onto td[0], as in the reference.
       const int chunk = (nb + 31) / 32;
       const int b0 = lane * chunk;
       float local = 0.f;
@@ -162,7 +164,7 @@ sample_level_kernel(mnrf_sample_desc d, const float* __restrict__ sdist_prev,
       if (lane == 0) run = 0.f;
       for (int i = b0; i < b0 + chunk && i < nb - 1; ++i) {
         run += wd[i];
-        cw[i + 1] = fminf(1.f, run);
+        cw[i + 1] = run > 1.f ? 1.f : run;
       }
       if (lane == 0) { cw[0] = 0.f; cw[nb] = 1.f; }
       __syncwarp();

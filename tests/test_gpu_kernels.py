@@ -11,7 +11,7 @@ import pytest
 import torch
 
 from composite_ref import CFG, oracle_composite
-from oracle import o_coord, o_math, o_render, o_stepfun
+from oracle import o_coord, o_math, o_render
 from util import close, kernel_rays
 
 pytestmark = pytest.mark.gpu
@@ -22,64 +22,6 @@ def ops():
   from multinerf_b200 import lib, ops as _ops
   lib.require_device()
   return _ops
-
-
-def _stepfun(rng, b, n, dup=True):
-  t = np.sort(rng.uniform(0, 1, (b, n + 1)).astype(np.float32), -1)
-  t[:, 0], t[:, -1] = 0, 1
-  if dup:
-    t[::3, n // 2] = t[::3, n // 2 - 1]
-  w = rng.uniform(0, 1, (b, n)).astype(np.float32) ** 3
-  w /= w.sum(-1, keepdims=True)
-  return torch.tensor(t), torch.tensor(w.astype(np.float32))
-
-
-@pytest.mark.parametrize('P,S,dil,single', [(64, 64, 0.0103125, True), (64, 32, 0.0026220703125, True),
-                                            (1, 64, 0.0, True), (128, 128, 0.0, False),
-                                            (37, 17, 0.02, False)])
-def test_sample_level_vs_oracle(ops, P, S, dil, single):
-  rng = np.random.default_rng(P * 1000 + S)
-  B = 257
-  t, w = _stepfun(rng, B, P, dup=P > 4)
-  use_dil = dil > 0
-  anneal, pad = 0.9091, 0.0 if use_dil else 0.01
-  jit = torch.tensor(rng.uniform(0, 1, (B, 1 if single else S)).astype(np.float32))
-  # oracle
-  if use_dil:
-    td, wd = o_stepfun.max_dilate_weights(t, w, dil, domain=(0.0, 1.0), renormalize=True)
-    td, wd = td[..., 1:-1], wd[..., 1:-1]
-  else:
-    td, wd = t, w
-  logits = torch.where(td[..., 1:] > td[..., :-1], anneal * torch.log(wd + pad), torch.tensor(-math.inf))
-  sd_o, idx_o, cw_o = o_stepfun.sample_intervals(jit, td, logits, S, single_jitter=single,
-                                                domain=(0.0, 1.0), return_index=True)
-  # device, end to end
-  sd, dbg = ops.sample_level(t.cuda(), w.cuda(), S, dilation=dil, use_dilation=use_dil, anneal=anneal,
-                             resample_padding=pad, jitter=(jit[:, 0] if single else jit).contiguous().cuda(),
-                             single_jitter=single, want_index=True, want_debug=True)
-  if use_dil:
-    np.testing.assert_array_equal(dbg['tdil'].cpu().numpy(), td.numpy())      # merge == sort: exact
-    close(dbg['wdil'], wd, atol=1e-7, rtol=1e-5, msg='dilated weights')
-  close(dbg['cw'], cw_o, atol=2e-6, rtol=0, msg='cdf')
-  close(sd, sd_o, atol=1e-5, rtol=1e-5, msg='sdist end-to-end')
-  mism = (dbg['idx'].cpu().long() != idx_o)
-  # end to end the CDFs differ by rounding, so an index may flip only where u sits on a knot
-  assert mism.float().mean() < 2e-3, mism.float().mean()
-  # integer contract: same CDF in -> identical interval indices and sdist to 1 ulp
-  sd2, dbg2 = ops.sample_level(t.cuda(), w.cuda(), S, dilation=dil, use_dilation=use_dil, anneal=anneal,
-                               resample_padding=pad, jitter=(jit[:, 0] if single else jit).contiguous().cuda(),
-                               single_jitter=single, cw_in=cw_o.contiguous().cuda(), want_index=True)
-  np.testing.assert_array_equal(dbg2['idx'].cpu().numpy(), idx_o.numpy().astype(np.int32))
-  close(sd2, sd_o, atol=2e-7, rtol=1e-6, msg='sdist with shared cdf')
-
-
-def test_sample_level_deterministic_and_errors(ops):
-  t = torch.tensor([[3.0, 4.0]] * 5).cuda()
-  w = torch.ones(5, 1).cuda()
-  sd = ops.sample_level(t, w, 10, domain=(-math.inf, math.inf))
-  close(sd, np.tile(np.linspace(3, 4, 11, dtype=np.float32), (5, 1)), atol=1e-5)   # stepfun_test.py:579-586
-  with pytest.raises(ValueError):
-    ops.sample_level(t, w, 1)
 
 
 @pytest.mark.parametrize('name,shape,sub,maxdeg,raydist,near,far,contract,rshape', [
