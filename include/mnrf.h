@@ -375,6 +375,20 @@ int mnrf_composite_bwd_masked(const mnrf_loss_desc* d, const float* raw_density,
                               const float* sdist_fine, const float* weights_fine, const float* data_mask,
                               float* d_raw_density, float* d_raw_rgb, float* d_rgb_scale,
                               float* d_raw_diffuse, float* d_raw_tint, float* stats, mnrf_stream stream);
+/* Same as mnrf_composite_bwd_masked (data_mask may be NULL) for one pass of a train step that runs its batch in
+ * several passes: the distortion and interlevel losses are means over `batch_rays` rays (the whole batch,
+ * >= num_rays) instead of the launch's num_rays, so each pass adds its share to stats and every per-sample gradient
+ * equals the one-pass step's.  batch_rays == num_rays is mnrf_composite_bwd_masked. */
+int mnrf_composite_bwd_chunk(const mnrf_loss_desc* d, const float* raw_density, const float* raw_rgb,
+                             const float* density_noise, const float* sdist, const float* directions,
+                             const float* near, const float* far, const float* bg_rgb,
+                             const float* rgb_scale, const float* raw_diffuse, const float* raw_tint,
+                             const float* extra_dw, const float* target_rgb,
+                             const float* lossmult, const float* inv_denom,
+                             const float* sdist_fine, const float* weights_fine, const float* data_mask,
+                             float* d_raw_density, float* d_raw_rgb, float* d_rgb_scale,
+                             float* d_raw_diffuse, float* d_raw_tint, float* stats, int32_t batch_rays,
+                             mnrf_stream stream);
 
 /* ---- RobustNeRF mask and inlier threshold (robustnerf.py:8-115) ------------------------------
  * mnrf_robust_mask: one CTA per patch; rays are patch-major [num_rays / p^2, p, p].
@@ -400,6 +414,11 @@ typedef struct {
 
 int mnrf_robust_mask(const mnrf_robust_desc* d, const float* rgb, const float* target, const float* threshold,
                      float* mask, float* error_per_pixel, uint32_t* counts, float* stats, mnrf_stream stream);
+/* Same for one pass of a batch of batch_rays (>= num_rays) rays: stats[1..4] += count / batch_rays, so the passes
+ * of a step add up to the batch's means.  batch_rays == num_rays is mnrf_robust_mask. */
+int mnrf_robust_mask_chunk(const mnrf_robust_desc* d, const float* rgb, const float* target, const float* threshold,
+                           float* mask, float* error_per_pixel, uint32_t* counts, float* stats, int32_t batch_rays,
+                           mnrf_stream stream);
 int mnrf_quantile(int32_t n, float q, const float* x, float* out, mnrf_stream stream);
 
 /* ---- Ref-NeRF per-sample stage ---------------------------------------------------------------

@@ -41,6 +41,9 @@ class Config:
   print_every: int = 100
   train_render_every: int = 5000
   cast_rays_in_train_step: bool = False
+  # rays per forward/backward pass of a train step, per process (0: the whole per-process batch in one pass); the
+  # passes accumulate into one gradient, so a batch larger than device memory trains at its configured size
+  train_chunk_size: int = 0
   data_loss_type: str = 'charb'
   charb_padding: float = 0.001
   data_loss_mult: float = 1.0

@@ -246,7 +246,7 @@ composite_bwd_kernel(mnrf_loss_desc L, const float* __restrict__ raw_density,
                      const float* __restrict__ data_mask,
                      float* __restrict__ d_raw_density, float* __restrict__ d_raw_rgb,
                      float* __restrict__ d_rgb_scale, float* __restrict__ d_raw_diffuse,
-                     float* __restrict__ d_raw_tint, float* __restrict__ stats) {
+                     float* __restrict__ d_raw_tint, float* __restrict__ stats, int batch_rays) {
   extern __shared__ float smem[];
   const mnrf_composite_desc& d = L.c;
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5, nw = blockDim.x >> 5;
@@ -257,7 +257,9 @@ composite_bwd_kernel(mnrf_loss_desc L, const float* __restrict__ raw_density,
   float* cy = senv + (S + 1);
   float* D = cy + (S + 1);
   const float inv_denom = *inv_denom_p;
-  const float invB = 1.f / (float)d.num_rays;
+  // the distortion and interlevel losses are means over the step's whole batch (batch_rays), of which this launch
+  // may be one pass
+  const float invB = 1.f / (float)batch_rays;
   float st_data = 0.f, st_mse = 0.f, st_dist = 0.f, st_inter = 0.f;
 
   for (int ray = blockIdx.x * nw + wib; ray < d.num_rays; ray += gridDim.x * nw) {
@@ -387,7 +389,7 @@ composite_bwd_kernel(mnrf_loss_desc L, const float* __restrict__ raw_density,
       __syncwarp();
       const float* cf = sdist_fine + (size_t)ray * (Sf + 1);
       const float* wf = weights_fine + (size_t)ray * Sf;
-      const float scale = L.interlevel_mult / ((float)d.num_rays * (float)Sf);
+      const float scale = L.interlevel_mult / ((float)batch_rays * (float)Sf);
       float lossp = 0.f;
       for (int i = lane; i < Sf; i += 32) {
         float t0 = cf[i], t1 = cf[i + 1], w = wf[i];
@@ -513,7 +515,8 @@ extern "C" int mnrf_composite_fwd(const mnrf_composite_desc* d, const float* raw
   return 0;
 }
 
-// mnrf_composite_bwd and mnrf_composite_bwd_masked share this body (data_mask == NULL: no mask).
+// mnrf_composite_bwd, mnrf_composite_bwd_masked and mnrf_composite_bwd_chunk share this body (data_mask == NULL: no
+// mask; batch_rays: the ray count the per-ray means divide by, num_rays unless the launch is one pass of a batch).
 static int composite_bwd_launch(const mnrf_loss_desc* d, const float* raw_density, const float* raw_rgb,
                                 const float* density_noise, const float* sdist, const float* directions,
                                 const float* near, const float* far, const float* bg_rgb, const float* rgb_scale,
@@ -521,7 +524,8 @@ static int composite_bwd_launch(const mnrf_loss_desc* d, const float* raw_densit
                                 const float* target_rgb, const float* lossmult, const float* inv_denom,
                                 const float* sdist_fine, const float* weights_fine, const float* data_mask,
                                 float* d_raw_density, float* d_raw_rgb, float* d_rgb_scale,
-                                float* d_raw_diffuse, float* d_raw_tint, float* stats, mnrf_stream stream) {
+                                float* d_raw_diffuse, float* d_raw_tint, float* stats, int32_t batch_rays,
+                                mnrf_stream stream) {
   using namespace mnrf;
   MNRF_CHECK(d->c.rgb_mode == 0 || (raw_rgb && raw_diffuse && d_raw_diffuse && (!raw_tint || d_raw_tint)),
              "mnrf_composite_bwd: rgb_mode 1 needs raw_diffuse / d_raw_diffuse (and d_raw_tint with raw_tint)");
@@ -534,6 +538,8 @@ static int composite_bwd_launch(const mnrf_loss_desc* d, const float* raw_densit
              "mnrf_composite_bwd: interlevel loss needs the final level's sdist/weights");
   MNRF_CHECK(d->lossmult_channels == 1 || d->lossmult_channels == 3, "lossmult_channels must be 1 or 3");
   MNRF_CHECK(d->loss_type >= 0 && d->loss_type <= 2, "unknown data_loss_type");
+  MNRF_CHECK(batch_rays >= d->c.num_rays, "mnrf_composite_bwd_chunk: batch_rays %d < num_rays %d", batch_rays,
+             d->c.num_rays);
   if (d->c.num_rays == 0) return 0;
   const int nw = 4;
   size_t smem = (size_t)nw * (4 * d->c.num_samples + 6) * sizeof(float);
@@ -543,7 +549,7 @@ static int composite_bwd_launch(const mnrf_loss_desc* d, const float* raw_densit
   MNRF_DISPATCH_CH(d->c.num_samples, (composite_bwd_kernel<CH><<<blocks, nw * 32, smem, (cudaStream_t)stream>>>(
       *d, raw_density, raw_rgb, density_noise, sdist, directions, near, far, bg_rgb, rgb_scale, raw_diffuse,
       raw_tint, extra_dw, target_rgb, lossmult, inv_denom, sdist_fine, weights_fine, data_mask, d_raw_density,
-      d_raw_rgb, d_rgb_scale, d_raw_diffuse, d_raw_tint, stats)));
+      d_raw_rgb, d_rgb_scale, d_raw_diffuse, d_raw_tint, stats, batch_rays)));
   MNRF_LAUNCH_CHECK();
   return 0;
 }
@@ -562,7 +568,7 @@ extern "C" int mnrf_composite_bwd(const mnrf_loss_desc* d, const float* raw_dens
   return composite_bwd_launch(d, raw_density, raw_rgb, density_noise, sdist, directions, near, far, bg_rgb,
                               rgb_scale, raw_diffuse, raw_tint, extra_dw, target_rgb, lossmult, inv_denom,
                               sdist_fine, weights_fine, nullptr, d_raw_density, d_raw_rgb, d_rgb_scale,
-                              d_raw_diffuse, d_raw_tint, stats, stream);
+                              d_raw_diffuse, d_raw_tint, stats, d ? d->c.num_rays : 0, stream);
 }
 
 extern "C" int mnrf_composite_bwd_masked(const mnrf_loss_desc* d, const float* raw_density,
@@ -580,5 +586,23 @@ extern "C" int mnrf_composite_bwd_masked(const mnrf_loss_desc* d, const float* r
   return composite_bwd_launch(d, raw_density, raw_rgb, density_noise, sdist, directions, near, far, bg_rgb,
                               rgb_scale, raw_diffuse, raw_tint, extra_dw, target_rgb, lossmult, inv_denom,
                               sdist_fine, weights_fine, data_mask, d_raw_density, d_raw_rgb, d_rgb_scale,
-                              d_raw_diffuse, d_raw_tint, stats, stream);
+                              d_raw_diffuse, d_raw_tint, stats, d ? d->c.num_rays : 0, stream);
+}
+
+extern "C" int mnrf_composite_bwd_chunk(const mnrf_loss_desc* d, const float* raw_density,
+                                        const float* raw_rgb, const float* density_noise,
+                                        const float* sdist, const float* directions, const float* near,
+                                        const float* far, const float* bg_rgb, const float* rgb_scale,
+                                        const float* raw_diffuse, const float* raw_tint, const float* extra_dw,
+                                        const float* target_rgb,
+                                        const float* lossmult, const float* inv_denom,
+                                        const float* sdist_fine, const float* weights_fine,
+                                        const float* data_mask,
+                                        float* d_raw_density, float* d_raw_rgb, float* d_rgb_scale,
+                                        float* d_raw_diffuse, float* d_raw_tint, float* stats,
+                                        int32_t batch_rays, mnrf_stream stream) {
+  return composite_bwd_launch(d, raw_density, raw_rgb, density_noise, sdist, directions, near, far, bg_rgb,
+                              rgb_scale, raw_diffuse, raw_tint, extra_dw, target_rgb, lossmult, inv_denom,
+                              sdist_fine, weights_fine, data_mask, d_raw_density, d_raw_rgb, d_rgb_scale,
+                              d_raw_diffuse, d_raw_tint, stats, batch_rays, stream);
 }

@@ -22,7 +22,7 @@ constexpr int kMaxPatchPixels = 1024;
 __global__ void __launch_bounds__(1024)
 robust_mask_kernel(mnrf_robust_desc d, const float* __restrict__ rgb, const float* __restrict__ target,
                    const float* __restrict__ threshold, float* __restrict__ mask, float* __restrict__ err_out,
-                   uint32_t* __restrict__ counts, float* __restrict__ stats, int num_rays) {
+                   uint32_t* __restrict__ counts, float* __restrict__ stats, int batch_rays) {
   __shared__ uint8_t inl[kMaxPatchPixels];
   __shared__ uint16_t rowcnt[kMaxPatchPixels];
   const int p = d.patch_size, pp = p * p;
@@ -80,7 +80,7 @@ robust_mask_kernel(mnrf_robust_desc d, const float* __restrict__ rgb, const floa
 
   if (stats == nullptr) return;
   // per-rank means of is_inlier_loss, has_inlier_neighbors, is_inlier_patch, mask: exact integer counts,
-  // then the last CTA divides once and leaves the counters zeroed for the next launch
+  // then the last CTA divides once by the batch's ray count and leaves the counters zeroed for the next launch
   const int c0 = __syncthreads_count(is_inl), c1 = __syncthreads_count(nb);
   const int c2 = __syncthreads_count(in_patch), c3 = __syncthreads_count(live && m);
   if (t == 0) {
@@ -92,7 +92,7 @@ robust_mask_kernel(mnrf_robust_desc d, const float* __restrict__ rgb, const floa
     const uint32_t ticket = atomicAdd(&counts[4], 1u);
     if (ticket == gridDim.x - 1) {
       __threadfence();
-      const float n = (float)num_rays;
+      const float n = (float)batch_rays;
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         const uint32_t c = atomicExch(&counts[k], 0u);
@@ -185,9 +185,10 @@ quantile_kernel(int n, float q, const float* __restrict__ x, float* __restrict__
 
 }  // namespace mnrf
 
-extern "C" int mnrf_robust_mask(const mnrf_robust_desc* d, const float* rgb, const float* target,
-                                const float* threshold, float* mask, float* error_per_pixel, uint32_t* counts,
-                                float* stats, mnrf_stream stream) {
+// mnrf_robust_mask and mnrf_robust_mask_chunk share this body; the mask means divide by batch_rays.
+static int robust_mask_launch(const mnrf_robust_desc* d, const float* rgb, const float* target,
+                              const float* threshold, float* mask, float* error_per_pixel, uint32_t* counts,
+                              float* stats, int32_t batch_rays, mnrf_stream stream) {
   using namespace mnrf;
   MNRF_CHECK(d && rgb && target && threshold && mask && error_per_pixel, "mnrf_robust_mask: null pointer");
   MNRF_CHECK(!stats || counts, "mnrf_robust_mask: stats need the counts workspace");
@@ -202,12 +203,27 @@ extern "C" int mnrf_robust_mask(const mnrf_robust_desc* d, const float* rgb, con
     MNRF_CHECK(d->filter_size >= 1 && d->filter_size % 2 == 1 && d->filter_size <= p,
                "mnrf_robust_mask: filter_size %d must be odd and <= patch_size %d", d->filter_size, p);
   }
+  MNRF_CHECK(batch_rays >= d->num_rays, "mnrf_robust_mask_chunk: batch_rays %d < num_rays %d", batch_rays,
+             d->num_rays);
   if (d->num_rays == 0) return 0;
   const int threads = (p * p + 31) / 32 * 32;
   robust_mask_kernel<<<d->num_rays / (p * p), threads, 0, (cudaStream_t)stream>>>(
-      *d, rgb, target, threshold, mask, error_per_pixel, counts, stats, d->num_rays);
+      *d, rgb, target, threshold, mask, error_per_pixel, counts, stats, batch_rays);
   MNRF_LAUNCH_CHECK();
   return 0;
+}
+
+extern "C" int mnrf_robust_mask(const mnrf_robust_desc* d, const float* rgb, const float* target,
+                                const float* threshold, float* mask, float* error_per_pixel, uint32_t* counts,
+                                float* stats, mnrf_stream stream) {
+  return robust_mask_launch(d, rgb, target, threshold, mask, error_per_pixel, counts, stats, d ? d->num_rays : 0,
+                            stream);
+}
+
+extern "C" int mnrf_robust_mask_chunk(const mnrf_robust_desc* d, const float* rgb, const float* target,
+                                      const float* threshold, float* mask, float* error_per_pixel, uint32_t* counts,
+                                      float* stats, int32_t batch_rays, mnrf_stream stream) {
+  return robust_mask_launch(d, rgb, target, threshold, mask, error_per_pixel, counts, stats, batch_rays, stream);
 }
 
 extern "C" int mnrf_quantile(int32_t n, float q, const float* x, float* out, mnrf_stream stream) {

@@ -152,7 +152,9 @@ _SIGNATURES = {
     'mnrf_composite_fwd': (C.c_int, [C.POINTER(CompositeDesc)] + [_P] * 18),
     'mnrf_composite_bwd': (C.c_int, [C.POINTER(LossDesc)] + [_P] * 24),
     'mnrf_composite_bwd_masked': (C.c_int, [C.POINTER(LossDesc)] + [_P] * 25),
+    'mnrf_composite_bwd_chunk': (C.c_int, [C.POINTER(LossDesc)] + [_P] * 24 + [C.c_int32, _P]),
     'mnrf_robust_mask': (C.c_int, [C.POINTER(RobustDesc)] + [_P] * 8),
+    'mnrf_robust_mask_chunk': (C.c_int, [C.POINTER(RobustDesc)] + [_P] * 7 + [C.c_int32, _P]),
     'mnrf_quantile': (C.c_int, [C.c_int32, C.c_float, _P, _P, _P]),
     'mnrf_encode_tangent': (C.c_int, [C.POINTER(EncodeDesc)] + [_P] * 9 + [C.c_int32, _P]),
     'mnrf_refdir_fwd': (C.c_int, [C.POINTER(RefdirDesc)] + [_P] * 10 + [C.c_float, C.c_float, C.c_int32, _P, _P]),

@@ -837,8 +837,9 @@ class Model:
     return om / B, pm / B, config.orientation_loss_target == 'normals_pred'
 
   def forward_levels(self, rng, rays, train_frac, compute_extras, want_samples, impl=0, anneal_dev=None,
-                     loss_config=None, zero_glo=True):
-    """Runs all levels; returns the list of LevelState (buffers stay valid until the next call)."""
+                     loss_config=None, zero_glo=True, batch_rays=None):
+    """Runs all levels; returns the list of LevelState (buffers stay valid until the next call).  `batch_rays`: the
+    rays are one pass of a train step over that many rays, whose count the per-ray loss multipliers divide by."""
     if self.params is None:
       raise RuntimeError('Model has no parameters: call construct_model()/init() first')
     m = self.mcfg
@@ -899,7 +900,7 @@ class Model:
       if mlp.plan.cfg.bottleneck_noise > 0 and rng is not None and mlp.plan.has_bottleneck:
         st.bneck_noise = draw('bottleneck_noise', i, (B * lv['S'], mlp.plan.cfg.bottleneck_width), torch.randn)
       # levels of an MLP without normals skip the normal losses (the reference raises there instead)
-      st.loss_mults = self.level_loss_mults(loss_config, i, B) if (
+      st.loss_mults = self.level_loss_mults(loss_config, i, batch_rays or B) if (
           loss_config is not None and mlp.plan.has_normals_stage) else None
       if st.loss_mults is not None:
         om, pm, on_pred = st.loss_mults

@@ -342,9 +342,10 @@ def composite_bwd(raw_density, raw_rgb, sdist, directions, near, far, target_rgb
                   interlevel_mult, sdist_fine=None, weights_fine=None, density_noise=None,
                   bg_rgb=None, rgb_scale=None, d_raw_density=None, d_raw_rgb=None, d_rgb_scale=None,
                   raw_diffuse=None, raw_tint=None, extra_dw=None, d_raw_diffuse=None, d_raw_tint=None,
-                  data_mask=None):
+                  data_mask=None, batch_rays=None):
   """Losses + compositing backward of one level; `data_mask` [B] (optional) weights each ray's data loss
-  (robustnerf) through mnrf_composite_bwd_masked."""
+  (robustnerf) through mnrf_composite_bwd_masked.  `batch_rays`: these B rays are one pass of a step over that
+  many rays, which the distortion and interlevel means divide by (mnrf_composite_bwd_chunk)."""
   lib = L.load()
   B, S = raw_density.shape
   dev = raw_density.device
@@ -369,6 +370,9 @@ def composite_bwd(raw_density, raw_rgb, sdist, directions, near, far, target_rgb
           L.ptr(stats), L.stream_ptr())
   if data_mask is not None:
     assert data_mask.numel() == B
+  if batch_rays is not None:
+    L.check(lib.mnrf_composite_bwd_chunk(*head, L.ptr(_f32(data_mask)), *tail[:-1], int(batch_rays), tail[-1]))
+  elif data_mask is not None:
     L.check(lib.mnrf_composite_bwd_masked(*head, L.ptr(_f32(data_mask)), *tail))
   else:
     L.check(lib.mnrf_composite_bwd(*head, *tail))
@@ -382,10 +386,11 @@ def robust_desc(num_rays, *, patch_size, inner_patch_size, filter_size, smoothed
                       1.0 - float(smoothed_inlier_quantile), 1.0 - float(inner_patch_inlier_quantile))
 
 
-def robust_mask(rgb, target, threshold, desc, *, mask=None, error=None, counts=None, stats=None):
+def robust_mask(rgb, target, threshold, desc, *, mask=None, error=None, counts=None, stats=None, batch_rays=None):
   """robustnerf.robustnerf_mask for patch-major rays: returns (mask [B], error_per_pixel [B]).
   `threshold` is a device scalar; with `stats` (a row of >= 5 floats), stats[1:5] += the per-rank means of
-  is_inlier_loss, has_inlier_neighbors, is_inlier_patch and mask, using `counts` (int32[5], zero, left zero)."""
+  is_inlier_loss, has_inlier_neighbors, is_inlier_patch and mask, using `counts` (int32[5], zero, left zero).
+  `batch_rays`: these B rays are one pass of a step over that many rays, and the means divide by it."""
   lib = L.load()
   B = rgb.shape[0]
   assert desc.num_rays == B and rgb.shape == (B, 3) and target.shape == (B, 3) and threshold.numel() == 1
@@ -397,8 +402,12 @@ def robust_mask(rgb, target, threshold, desc, *, mask=None, error=None, counts=N
     assert counts is not None and counts.dtype == torch.int32 and counts.numel() >= 5
     assert stats.is_contiguous() and stats.numel() >= 5
   _count()
-  L.check(lib.mnrf_robust_mask(C.byref(desc), L.ptr(_f32(rgb)), L.ptr(_f32(target)), L.ptr(_f32(threshold)),
-                               L.ptr(mask), L.ptr(error), L.ptr(counts), L.ptr(stats), L.stream_ptr()))
+  args = (C.byref(desc), L.ptr(_f32(rgb)), L.ptr(_f32(target)), L.ptr(_f32(threshold)), L.ptr(mask), L.ptr(error),
+          L.ptr(counts), L.ptr(stats))
+  if batch_rays is not None:
+    L.check(lib.mnrf_robust_mask_chunk(*args, int(batch_rays), L.stream_ptr()))
+  else:
+    L.check(lib.mnrf_robust_mask(*args, L.stream_ptr()))
   return mask, error
 
 

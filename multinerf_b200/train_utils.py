@@ -76,6 +76,30 @@ def check_robust_config(config, rays_per_rank=None):
     raise ValueError(f'robustnerf: {rays_per_rank} rays per process is not a multiple of patch_size^2 = {p * p}')
 
 
+def check_chunk_config(config, rays_per_rank):
+  """The limits of Config.train_chunk_size for a step over `rays_per_rank` rays per process (ValueError)."""
+  c = config.train_chunk_size
+  if c < 0:
+    raise ValueError(f'train_chunk_size {c} must be >= 0 (0: one pass over the whole batch)')
+  if c == 0 or c == rays_per_rank:
+    return
+  if rays_per_rank % c != 0:
+    raise ValueError(f'train_chunk_size {c} does not divide the {rays_per_rank} rays per process')
+  if config.data_loss_type == 'robustnerf' and config.enable_robustnerf_loss and c % (config.patch_size ** 2) != 0:
+    raise ValueError(f'train_chunk_size {c} is not a multiple of patch_size^2 = {config.patch_size ** 2}: a '
+                     'robustnerf patch would straddle two passes')
+
+
+def _ray_rows(rays, lo, hi):
+  """Rows [lo, hi) of flat device rays (every field and the flat near/far/radii): views, no copies."""
+  import dataclasses
+  r = type(rays)(**{f.name: (None if getattr(rays, f.name) is None else getattr(rays, f.name)[lo:hi])
+                    for f in dataclasses.fields(rays)})
+  for extra in ('radii_flat', 'near_flat', 'far_flat'):
+    setattr(r, extra, getattr(rays, extra)[lo:hi])
+  return r
+
+
 def _anneal(mcfg, train_frac):
   if mcfg.anneal_slope > 0:
     sl = mcfg.anneal_slope
@@ -94,6 +118,10 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
   with the NCCL all-reduce between them) after one eager warm-up step; per-step scalars
   (annealing exponent, learning rate, Adam bias corrections) and the jitter draws live in device
   buffers that are refreshed before each replay, so train_frac and the step count may advance.
+
+  With `config.train_chunk_size` C (0 < C < rays per process), the forward and backward passes run on C rays at a
+  time into the same gradients and statistics, and the exchange, clipping and Adam step follow the last pass
+  (passes_fwd_bwd); under use_graph every pass is in one graph.
   """
   mcfg = model.mcfg
   camtype = getattr(dataset, 'camtype', camera_utils.ProjectionType.PERSPECTIVE)
@@ -102,6 +130,7 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
   robust = config.data_loss_type == 'robustnerf'
   if robust:
     check_robust_config(config, config.batch_size // _world()[0])
+  check_chunk_config(config, config.batch_size // _world()[0])
   if use_graph and (mcfg.near_anneal_rate is not None or
                     mcfg.bg_intensity_range[0] != mcfg.bg_intensity_range[1] or
                     any(p.cfg.bottleneck_noise > 0 for p in model.plans.values())):
@@ -160,20 +189,30 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
       first_use.setdefault(mname, i)
     return {i: mname for mname, i in first_use.items() if i > 0}
 
-  def fb_begin(rng, rays, target, train_frac, anneal_ptr):
-    """Zero the gradients, run the forward pass of every level; returns the context of the backward pass."""
-    params = model.params
+  def loss_norm(rays):
+    """The data loss's per-ray weights and 1 / their sum (train_utils.py:72-136), over all of `rays`."""
     lossmult = rays.lossmult
     if config.disable_multiscale_loss:
       lossmult = torch.ones_like(lossmult)
     lm_ch = lossmult.shape[-1]
-    inv_denom = (1.0 / (lossmult.sum() * (3 if lm_ch == 1 else 1))).reshape(1)
-    params.grads_ext.zero_()
+    return lossmult, (1.0 / (lossmult.sum() * (3 if lm_ch == 1 else 1))).reshape(1)
+
+  def fb_begin(rng, rays, target, train_frac, anneal_ptr, whole=None):
+    """Zero the gradients, run the forward pass of every level; returns the context of the backward pass.
+    `whole`: the rays are rows [lo, hi) of a step over whole['B'] rays, whose loss weights and normaliser it carries;
+    the gradients are not zeroed (the step did that before its first pass)."""
+    params = model.params
+    if whole is None:
+      lossmult, inv_denom = loss_norm(rays)
+      params.grads_ext.zero_()
+    else:
+      lossmult, inv_denom = whole['lossmult'][whole['lo']:whole['hi']], whole['inv_denom']
     states = model.forward_levels(rng if config.randomized else None, rays, train_frac,
                                   compute_extras=False, want_samples=False, impl=impl,
-                                  anneal_dev=anneal_ptr, loss_config=config, zero_glo=False)
+                                  anneal_dev=anneal_ptr, loss_config=config, zero_glo=False,
+                                  batch_rays=None if whole is None else whole['B'])
     return dict(params=params, states=states, rays=rays, target=target, lossmult=lossmult, inv_denom=inv_denom,
-                stats=stats_view(params))
+                stats=stats_view(params), whole=whole)
 
   def fb_level(ctx, i):
     """Losses + backward of level i (accumulates parameter gradients)."""
@@ -195,7 +234,8 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
         d_raw_rgb=st.d_raw_rgb, d_rgb_scale=_d_scale_buf(st),
         raw_diffuse=st.heads.get('diffuse'), raw_tint=st.heads.get('tint'),
         extra_dw=st.extra_dw if st.loss_mults is not None else None,
-        d_raw_diffuse=st.d_heads.get('diffuse'), d_raw_tint=st.d_heads.get('tint'))
+        d_raw_diffuse=st.d_heads.get('diffuse'), d_raw_tint=st.d_heads.get('tint'),
+        batch_rays=None if ctx['whole'] is None else ctx['whole']['B'])
     if st.rgb_scale is not None and mcfg.learned_exposure_scaling:
       # d offsets[idx] += [idx > 0] * exposure_values * d_scale   (adjoint of models.py:262-267)
       eidx = rays.exposure_idx[:, 0].long()
@@ -217,15 +257,24 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
                            inner_patch_inlier_quantile=config.robustnerf_inner_patch_inlier_quantile,
                            enable=config.enable_robustnerf_loss)
     row = stats_rows(ctx['params'])[-1] if is_fine else None
+    whole = ctx['whole']
+    if whole is not None:
+      # one pass of a longer step: the final level's errors go to their rows of the batch's buffer, whose quantile
+      # the step takes after its last pass (passes_fwd_bwd); the mask means divide by the batch's ray count
+      mask, _ = ops.robust_mask(st.comp['rgb'], ctx['target'], threshold_dev, desc,
+                                error=whole['err'][whole['lo']:whole['hi']] if is_fine else None,
+                                counts=robust_counts if is_fine else None, stats=row, batch_rays=whole['B'])
+      return mask
     mask, err = ops.robust_mask(st.comp['rgb'], ctx['target'], threshold_dev, desc,
                                 counts=robust_counts if is_fine else None, stats=row)
     if is_fine:
       ops.quantile(err, config.robustnerf_inlier_quantile, out=row[0:1])
     return mask
 
-  def split_level(n_levels, world):
-    """Level after whose backward the first gradient segment is final (None: exchange everything at the end)."""
-    early = early_segments(n_levels) if world > 1 else {}
+  def split_level(n_levels, world, B):
+    """Level after whose backward the first gradient segment is final (None: exchange everything at the end, as a
+    step of several passes always does: a gradient is final only after the last pass)."""
+    early = early_segments(n_levels) if world > 1 and n_passes(B) == 1 else {}
     return (max(early), early[max(early)]) if early else (None, None)
 
   def exchange_early(params, mname):
@@ -242,11 +291,69 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
     for w in pending:
       w.wait()
 
+  def n_passes(B):
+    """Forward/backward passes of a step over B rays per process (Config.train_chunk_size)."""
+    c = config.train_chunk_size
+    return 1 if c in (0, B) else B // c
+
+  def batch_draws(rng, B, sched):
+    """The whole batch's random draws of every level, drawn once (a step of several passes gives each pass its
+    rows, so its samples are those of the one-pass step given the same explicit draws)."""
+    if rng is None or not config.randomized:
+      return None
+    if isinstance(rng, dict):
+      return {k: [None if v is None else torch.as_tensor(v).to(dev) for v in vs] for k, vs in rng.items()}
+    lo, hi = mcfg.bg_intensity_range
+    out = {'jitter': [], 'bottleneck_noise': [], 'density_noise': [], 'bg': []}
+    for i, lv in enumerate(sched):
+      S = lv['S']
+      plan = model.plans['NerfMLP_0' if (mcfg.single_mlp or not lv['is_prop']) else 'PropMLP_0']
+      out['jitter'].append(torch.rand((B,) if mcfg.single_jitter else (B, S), device=dev, generator=rng))
+      out['bottleneck_noise'].append(
+          torch.randn(B * S, plan.cfg.bottleneck_width, device=dev, generator=rng)
+          if plan.cfg.bottleneck_noise > 0 and plan.has_bottleneck else None)
+      out['density_noise'].append(
+          torch.randn(B, S, device=dev, generator=rng) if plan.cfg.density_noise > 0 else None)
+      out['bg'].append(torch.rand(B, 3, device=dev, generator=rng) if lo != hi else None)
+    return out
+
+  def passes_fwd_bwd(rng, rays, target, train_frac, anneal_ptr):
+    """Forward + backward of a step over B rays in B / train_chunk_size passes, accumulated into the same
+    gradients and statistics.  The loss normalisers, the random draws and the robustnerf quantile are the whole
+    batch's; the level buffers have the pass's shape and every pass reuses them."""
+    params = model.params
+    B = rays.origins.shape[0]
+    C = B // n_passes(B)
+    lossmult, inv_denom = loss_norm(rays)
+    err = None
+    if robust:
+      err = G.get(('robust_err', B))
+      if err is None:
+        err = G[('robust_err', B)] = torch.empty(B, device=dev)
+    rand = batch_draws(rng, B, model.level_schedule(train_frac)[2])
+    params.grads_ext.zero_()
+    for lo in range(0, B, C):
+      rows = None if rand is None else {k: [None if v is None else v.reshape(B, -1)[lo:lo + C] for v in vs]
+                                        for k, vs in rand.items()}
+      ctx = fb_begin(rows, _ray_rows(rays, lo, lo + C), target[lo:lo + C], train_frac, anneal_ptr,
+                     whole=dict(B=B, lo=lo, hi=lo + C, lossmult=lossmult, inv_denom=inv_denom, err=err))
+      for i in range(len(ctx['states']) - 1, -1, -1):
+        fb_level(ctx, i)
+    if robust:
+      ops.quantile(err, config.robustnerf_inlier_quantile, out=stats_rows(params)[-1][0:1])
+
   def fwd_bwd(rng, rays, target, train_frac, anneal_ptr, world=1):
     """Eager step body: forward, backward last level to first, gradient exchange (world > 1)."""
+    if n_passes(rays.origins.shape[0]) > 1:
+      passes_fwd_bwd(rng, rays, target, train_frac, anneal_ptr)
+      if decay_views:
+        weight_decay()
+      if world > 1:
+        exchange_rest(model.params, [], [])
+      return
     ctx = fb_begin(rng, rays, target, train_frac, anneal_ptr)
     n = len(ctx['states'])
-    split, seg = split_level(n, world)
+    split, seg = split_level(n, world, rays.origins.shape[0])
     pending, done = [], []
     for i in range(n - 1, -1, -1):
       fb_level(ctx, i)
@@ -354,6 +461,7 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
       model.bind(params)
       G['state'] = 0
     rays = batch.rays
+    check_chunk_config(config, math.prod(tuple(rays.lossmult.shape)[:-1]))    # before any device work
     if config.cast_rays_in_train_step:
       if not isinstance(rays, utils.Pixels):
         raise ValueError('cast_rays_in_train_step: batch.rays must be a utils.Pixels')
@@ -400,7 +508,7 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
       torch.cuda.synchronize()
       before = ops.LAUNCHES
       n_lv = len(sched)
-      split, seg = split_level(n_lv, world)
+      split, seg = split_level(n_lv, world, B)
       G['split'] = None
       if world > 1 and not GRAPH_NCCL:
         # NCCL stays outside the graphs (capturing it hung on this stack, round 2): the step is two graphs around
@@ -409,11 +517,14 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
         # [clip + Adam + repack] -- so the big NerfMLP exchange overlaps the PropMLP backward
         G['fb'] = torch.cuda.CUDAGraph()
         with torch.cuda.graph(G['fb']):
-          ctx = fb_begin(rand, G['rays'], G['target'], train_frac, anneal_dev)
-          for i in range(n_lv - 1, (split if split is not None else 0) - 1, -1):
-            fb_level(ctx, i)
-          if split is None and decay_views:
-            weight_decay()
+          if n_passes(B) > 1:
+            fwd_bwd(rand, G['rays'], G['target'], train_frac, anneal_dev)     # every pass, no exchange
+          else:
+            ctx = fb_begin(rand, G['rays'], G['target'], train_frac, anneal_dev)
+            for i in range(n_lv - 1, (split if split is not None else 0) - 1, -1):
+              fb_level(ctx, i)
+            if split is None and decay_views:
+              weight_decay()
         if split is not None:
           G['split'] = seg
           G['fb2'] = torch.cuda.CUDAGraph()
