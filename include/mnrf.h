@@ -197,6 +197,8 @@ typedef struct {
   int32_t splits;     /* reduction splits (WGRAD; 1 otherwise) */
   int32_t tiles;      /* work items: row blocks x column blocks x splits */
   int32_t grid;       /* persistent CTAs */
+  int32_t pingpong;   /* FWD / DGRAD: 1 each consumer warpgroup runs whole 128 x 128 sub-tiles of the 128 x block_n
+                         tiles, alternating, so one's epilogue runs under the other's MMAs; 0 both run each tile */
 } mnrf_gemm_instance;
 int mnrf_gemm_plan(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
                    const float* rowv, const float* colv, const mnrf_bf16* mask, const uint32_t* maskbits,

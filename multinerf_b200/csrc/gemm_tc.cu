@@ -517,7 +517,301 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   }
 }
 
+// ---------------------------------------------------------------------------- ping-pong schedule (FWD / DGRAD)
+// gemm_tc_kernel runs both consumer warpgroups through the main loop and then through the epilogue together, so the
+// tensor cores idle for the whole epilogue (a third to two thirds of a tile's time at the NerfMLP shapes).  Here each
+// consumer warpgroup owns whole 128 x 128 sub-tiles instead: the CTA's tiles (the same 128 x BN tiles in the same
+// order as gemm_tc_kernel) are cut into BN / 128 column sub-tiles, numbered it = 0, 1, ... in order, and warpgroup
+// it & 1 runs sub-tile it.  An ordered hand-off (mma_turn) lets a warpgroup issue its sub-tile's wgmmas only once the
+// other has issued all of the previous sub-tile's, so one warpgroup's epilogue runs under the other's MMAs.  Each
+// output still accumulates its k-blocks in order through the same k16 steps: the outputs equal gemm_tc_kernel's bit
+// for bit.  Staged store only; no column sums, no smooth activation.
+constexpr int PP_BN = 128;             // sub-tile width
+constexpr int PP_STAGES = 5;           // operand ring: 5 x 32 KB
+constexpr int PP_SB = 2;               // staging blocks per warpgroup (a sub-tile stages 4 blocks of 64 x 64)
+// DGRAD mask blocks by TMA, sub-tile it in buffer it % PP_MASK_BUFS: four, so that the producer loads sub-tile
+// it + 2's mask and operands while sub-tile it's epilogue still reads its mask block
+constexpr int PP_MASK_BUFS = 4;
+constexpr int pp_smem_bytes(int mode) {
+  return PP_STAGES * (A_STAGE_BYTES + PP_BN * BLOCK_K * 2) + 2 * PP_SB * STAGING_BLOCK_BYTES +
+         (mode == MNRF_GEMM_DGRAD ? PP_MASK_BUFS * BLOCK_M * mask_words(PP_BN) * 4 : 0) + 256 /*barriers*/ +
+         1024 /*align*/;
+}
+
+// Accumulator fragments of the two wgmma m64n128 of a sub-tile (per consumer thread): acc[g][4i + 2h + e] is row
+// 64g + 16*warp + lane/4 + 8h, column 8i + 2*(lane%4) + e of the warpgroup's 128 x 128 sub-tile.
+template <int MODE, int BN>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                        const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_m,
+                        const GemmParams p) {
+  constexpr int STAGES = PP_STAGES;
+  constexpr int B_STAGE = PP_BN * BLOCK_K * 2;
+  constexpr int SUB = BN / PP_BN;        // sub-tiles per tile
+  constexpr int MW = mask_words(PP_BN);
+  constexpr int SB = PP_SB;
+  constexpr bool kDgrad = (MODE == MNRF_GEMM_DGRAD);
+  static_assert(MODE != MNRF_GEMM_WGRAD && (BN == 128 || BN == 256), "FWD / DGRAD tiles of 128 or 256 columns");
+  extern __shared__ uint8_t smem_dyn[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
+  uint8_t* smem_c = smem_b + STAGES * B_STAGE;                                   // [2 warpgroups][SB] blocks
+  uint32_t* mask_s = reinterpret_cast<uint32_t*>(smem_c + 2 * SB * STAGING_BLOCK_BYTES);  // [PP_MASK_BUFS][BLOCK_M][MW]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(mask_s + (kDgrad ? PP_MASK_BUFS * BLOCK_M * MW : 0));  // [STAGES]
+  uint64_t* empty_bar = full_bar + STAGES;                                       // [STAGES]
+  uint64_t* mask_full = empty_bar + STAGES;                                      // [PP_MASK_BUFS]
+  uint64_t* mask_empty = mask_full + PP_MASK_BUFS;                               // [PP_MASK_BUFS]
+  uint64_t* mma_turn = mask_empty + PP_MASK_BUFS;                               // [2]: warpgroup c may issue
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
+  const int total_tiles = p.num_m_blocks * p.num_n_blocks;
+  const int nk = p.num_k_blocks;         // k-blocks of every sub-tile
+  const bool mask_tma = kDgrad && p.mask_tma;
+
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tmap_a);
+    prefetch_tmap(&tmap_b);
+    prefetch_tmap(&tmap_c);
+    if (mask_tma) prefetch_tmap(&tmap_m);
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 4);     // the 4 warps of the warpgroup that consumes the stage
+    }
+    for (int i = 0; i < PP_MASK_BUFS; ++i) {
+      mbar_init(&mask_full[i], 1);
+      mbar_init(&mask_empty[i], 4);
+    }
+    for (int i = 0; i < 2; ++i) mbar_init(&mma_turn[i], 4);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_launch_dependents();
+  pdl_wait();
+
+  if (wg == 0) {
+    // ===================== TMA producer: the sub-tiles' k-blocks in order, into one ring =====================
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      uint32_t stage = 0, phase = 0;
+      int it = 0;
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const int n_blk = tile % p.num_n_blocks;
+        const int m_blk = tile / p.num_n_blocks;
+        for (int s = 0; s < SUB; ++s, ++it) {
+          const int ncol0 = n_blk * BN + s * PP_BN;
+          if (mask_tma) {
+            // the sub-tile's [128 rows x MW words] of mask bits (mask_mod, a multiple of 128: 128 consecutive
+            // mask rows); rows past the end are zero-filled
+            const int mb = it % PP_MASK_BUFS;
+            mbar_wait(&mask_empty[mb], ((it / PP_MASK_BUFS) & 1) ^ 1, 4);
+            mbar_expect_tx(&mask_full[mb], BLOCK_M * MW * 4);
+            const int64_t r0 = (int64_t)m_blk * BLOCK_M;
+            tma_load_2d(mask_s + mb * (BLOCK_M * MW), &tmap_m, &mask_full[mb], ncol0 / 32,
+                        (int)(p.mask_mod > 0 ? r0 % p.mask_mod : r0));
+          }
+          for (int kb = 0; kb < nk; ++kb) {
+            mbar_wait(&empty_bar[stage], phase ^ 1, 1);
+            mbar_expect_tx(&full_bar[stage], A_STAGE_BYTES + B_STAGE);
+            tma_load_2d(smem_a + stage * A_STAGE_BYTES, &tmap_a, &full_bar[stage], kb * BLOCK_K, m_blk * BLOCK_M);
+            tma_load_2d(smem_b + stage * B_STAGE, &tmap_b, &full_bar[stage], kb * BLOCK_K, ncol0);
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          }
+        }
+      }
+    }
+  } else {
+    // ===================== consumers: warpgroup c runs sub-tiles it = c, c + 2, ... =====================
+    setmaxnreg_inc<232>();
+    const int c = wg - 1;
+    const int w = warp & 3;
+    const int cq = 2 * (lane & 3);
+    const bool leader = (threadIdx.x & 127) == 0;   // issues and waits on the warpgroup's bulk stores
+    // this thread's row (h = 0) in the warpgroup's first staging block
+    const uint32_t c_row = smem_u32(smem_c) + c * (SB * STAGING_BLOCK_BYTES) + (16 * w + (lane >> 2)) * 128 + (cq << 1);
+    float acc[2][64];
+    for (int it = c; ; it += 2) {                // sub-tile it: column block it % SUB of the CTA's tile it / SUB
+      const int tile = blockIdx.x + (it / SUB) * (int)gridDim.x;
+      if (tile >= total_tiles) break;
+      const int s = it % SUB;
+      const int n_blk = tile % p.num_n_blocks;
+      const int m_blk = tile / p.num_n_blocks;
+      const int ncol0 = n_blk * BN + s * PP_BN;
+      // the ring slots of this sub-tile: the producer fills nk per sub-tile, in order
+      const uint32_t slot = (uint32_t)it * (uint32_t)nk;
+      uint32_t stage = slot % STAGES, phase = (slot / STAGES) & 1;
+      // the other warpgroup has issued every wgmma of sub-tile it - 1
+      if (it > 0) mbar_wait(&mma_turn[c], ((it - 1) >> 1) & 1, 7);
+      int prev = -1;
+      fence_acc(acc[0]);
+      fence_acc(acc[1]);
+      for (int kb = 0; kb < nk; ++kb) {
+        mbar_wait(&full_bar[stage], phase, 3);
+        const uint32_t sa = smem_u32(smem_a + stage * A_STAGE_BYTES);
+        const uint32_t sb = smem_u32(smem_b + stage * B_STAGE);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / WGMMA_K; ++k) {
+          const uint64_t bdesc = make_smem_desc(sb + k * (WGMMA_K * 2), 0, 1024);
+#pragma unroll
+          for (int g = 0; g < 2; ++g)
+            Wgmma<PP_BN, 0, 0>::mma(acc[g], make_smem_desc(sa + g * (64 * 128) + k * (WGMMA_K * 2), 0, 1024), bdesc,
+                                    (kb > 0 || k > 0) ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                        // the k-block before this one has been read: release its slot
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = (int)stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      // every wgmma of this sub-tile is issued: the other warpgroup's next sub-tile may start
+      if (blockIdx.x + ((it + 1) / SUB) * (int)gridDim.x < total_tiles) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&mma_turn[c ^ 1]);
+      }
+      wgmma_wait<0>();
+      fence_acc(acc[0]);
+      fence_acc(acc[1]);
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+
+      // ---- epilogue: rows [64g, 64g + 64) of the sub-tile from acc[0], one 64 x 64 staging block per 8 columns.
+      // A rolled loop that moves acc[1] into acc[0] for its second pass: unrolled, nvcc hoists the second half's
+      // loads into the first and the DGRAD instances spill 2.4 KB.
+      const uint32_t m_base = smem_u32(mask_s) + (it % PP_MASK_BUFS) * (BLOCK_M * MW * 4);
+      if (mask_tma) mbar_wait(&mask_full[it % PP_MASK_BUFS], (it / PP_MASK_BUFS) & 1, 5);
+#pragma unroll 1
+      for (int g = 0; g < 2; ++g) {
+        const int r_in = 64 * g + 16 * w + (lane >> 2);
+        int64_t rows[2];
+        bool row_ok[2];
+        float rv[2] = {0.f, 0.f};
+        const uint32_t* mrow[2] = {nullptr, nullptr};
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          rows[h] = (int64_t)m_blk * BLOCK_M + r_in + 8 * h;
+          row_ok[h] = rows[h] < p.m;
+          if (kDgrad && row_ok[h]) {
+            if (p.rowv) rv[h] = p.rowv[rows[h]];
+            if (p.maskbits && !mask_tma)
+              mrow[h] = p.maskbits + (p.mask_mod > 0 ? rows[h] % p.mask_mod : rows[h]) * p.ldmaskbits;
+          }
+        }
+        const uint32_t m_row = m_base + r_in * (MW * 4);
+        uint32_t bits[2] = {0u, 0u};
+        uint32_t mw[2] = {0u, 0u};              // DGRAD mask bits: the rows' words of the current 32 columns
+#pragma unroll
+        for (int i = 0; i < PP_BN / 8; ++i) {
+          const int col = ncol0 + 8 * i + cq;
+          if (kDgrad && p.maskbits && (i & 3) == 0) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              mw[h] = mask_tma ? ld_shared_u32(m_row + (8 * h * MW + (i >> 2)) * 4)
+                               : row_ok[h] ? __ldg(mrow[h] + (col >> 5)) : 0u;
+          }
+          float v[2][2];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) { v[h][0] = acc[0][4 * i + 2 * h]; v[h][1] = acc[0][4 * i + 2 * h + 1]; }
+          if (!kDgrad) {
+            if (p.bias) {
+              const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+#pragma unroll
+              for (int h = 0; h < 2; ++h) { v[h][0] += b.x; v[h][1] += b.y; }
+            }
+            if (p.act == MNRF_ACT_RELU) {
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  v[h][e] = fmaxf(v[h][e], 0.f);
+                  bits[h] |= (v[h][e] > 0.f ? 1u : 0u) << ((8 * i + cq + e) & 31);
+                }
+            }
+          } else {
+            float2 cv = make_float2(0.f, 0.f);
+            if (p.rowv) cv = __ldg(reinterpret_cast<const float2*>(p.colv + col));
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              if (p.rowv) { v[h][0] += rv[h] * cv.x; v[h][1] += rv[h] * cv.y; }
+              if (p.maskbits) {
+                if (!((mw[h] >> (col & 31)) & 1u)) v[h][0] = 0.f;
+                if (!((mw[h] >> ((col + 1) & 31)) & 1u)) v[h][1] = 0.f;
+              } else if (p.mask && row_ok[h]) {
+                const uint32_t mm = __ldg(reinterpret_cast<const unsigned int*>(p.mask + rows[h] * p.ldmask + col));
+                if (!(bf16_lo(mm) > 0.f)) v[h][0] = 0.f;
+                if (!(bf16_hi(mm) > 0.f)) v[h][1] = 0.f;
+              }
+              if (p.addend && row_ok[h]) {
+                const uint32_t aa = __ldg(reinterpret_cast<const unsigned int*>(p.addend + rows[h] * p.ldadd + col));
+                v[h][0] += bf16_lo(aa);
+                v[h][1] += bf16_hi(aa);
+              }
+            }
+          }
+          // staging block (i / 8) % SB, row 16 w + lane / 4 + 8h, 16-byte chunk (i % 8) ^ (row % 8), byte 2 * cq
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            st_shared_u32(c_row + ((i >> 3) & (SB - 1)) * STAGING_BLOCK_BYTES + h * (8 * 128) +
+                              (((i & 7) ^ ((lane >> 2) & 7)) << 4),
+                          pack_bf16(v[h][0], v[h][1]));
+          if (!kDgrad && p.act == MNRF_ACT_RELU && p.maskbits && (i & 3) == 3) {
+            // one 32-column mask word per row: the four lanes of a quad hold its 32 bits between them
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              bits[h] |= __shfl_xor_sync(0xffffffffu, bits[h], 1);
+              bits[h] |= __shfl_xor_sync(0xffffffffu, bits[h], 2);
+              if ((lane & 3) == ((i >> 2) & 3) && row_ok[h]) p.maskbits[rows[h] * p.ldmaskbits + (col >> 5)] = bits[h];
+              bits[h] = 0u;
+            }
+          }
+          if ((i & 7) == 7) {
+            fence_proxy_async();                // generic-proxy writes -> visible to the bulk store (async proxy)
+            // the store of the previous block, in the staging block that the next block overwrites, has been read
+            if (leader) tma_store_wait_read<0>();
+            named_bar_sync(2 + c, 128);
+            if (leader) {                       // TMA clips the rows past M
+              tma_store_2d(&tmap_c, smem_c + (c * SB + ((i >> 3) & (SB - 1))) * STAGING_BLOCK_BYTES,
+                           ncol0 + 8 * (i & ~7), (int)((int64_t)m_blk * BLOCK_M + 64 * g));
+              tma_store_commit();
+            }
+          }
+        }
+#pragma unroll
+        for (int e = 0; e < 64; ++e) acc[0][e] = acc[1][e];   // rows [64, 128) next
+      }
+      if (mask_tma) {                           // this warp has read its mask words: the buffer may be refilled
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&mask_empty[it % PP_MASK_BUFS]);
+      }
+    }
+    if ((threadIdx.x & 127) == 0) tma_store_wait_all();
+  }
+}
+
 // ------------------------------------------------------------------------------------ host
+template <int MODE, int BN>
+static int launch_gemm_tc_pingpong(int grid, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
+                                   const CUtensorMap& tm, const GemmParams& p, cudaStream_t stream) {
+  static bool attr_set = false;
+  constexpr int kSmem = pp_smem_bytes(MODE);
+  static_assert(kSmem <= 232448, "shared memory budget");
+  auto kern = gemm_tc_pingpong_kernel<MODE, BN>;
+  if (!attr_set) {
+    MNRF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
+    attr_set = true;
+  }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(NUM_THREADS);
+  cfg.dynamicSmemBytes = kSmem; cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  MNRF_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, tc, tm, p));
+  return 0;
+}
+
 template <int MODE, int BN, bool TS, bool SIDE, bool SMOOTH>
 static int launch_gemm_tc(int grid, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
                           const CUtensorMap& tm, const GemmParams& p, cudaStream_t stream) {
@@ -627,6 +921,9 @@ static int gemm_tc_plan(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_
   // epilogue loads them itself.
   const bool mask_tma = d->mode == MNRF_GEMM_DGRAD && maskbits && mask_words(block_n) > 0 && d->ldmaskbits % 4 == 0 &&
                         ((uintptr_t)maskbits % 16) == 0 && (d->mask_mod == 0 || d->mask_mod % BLOCK_M == 0);
+  // FWD and DGRAD run the ping-pong schedule (gemm_tc_pingpong_kernel) wherever it has an epilogue: staged store,
+  // whole 128-column sub-tiles, ReLU or no activation, no column sums.
+  const bool pingpong = d->mode != MNRF_GEMM_WGRAD && ts && d->n % PP_BN == 0 && !smooth && !colsum;
   const int tiles = num_m_blocks * num_n_blocks * num_splits;
   plan->block_n = block_n;
   plan->staged = ts;
@@ -636,6 +933,7 @@ static int gemm_tc_plan(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_
   plan->splits = num_splits;
   plan->tiles = tiles;
   plan->grid = std::min(tiles, workers);
+  plan->pingpong = pingpong;
   return 0;
 }
 
@@ -675,7 +973,7 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
   CUtensorMap ta, tb, tc;
   if (d->mode != MNRF_GEMM_WGRAD) {
     if (make_tmap(&ta, a, d->m, d->k, d->lda, BLOCK_K, BLOCK_M)) return 1;
-    if (make_tmap(&tb, b, d->n, d->k, d->ldb, BLOCK_K, block_n)) return 1;
+    if (make_tmap(&tb, b, d->n, d->k, d->ldb, BLOCK_K, plan.pingpong ? PP_BN : block_n)) return 1;
   } else {
     // A = X[R, Mo], B = dY[R, N]; reduction index on rows
     if (make_tmap(&ta, a, d->k, d->m, d->lda, 64, BLOCK_K)) return 1;
@@ -689,7 +987,7 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
   CUtensorMap tm = tb;   // not read unless p.mask_tma
   if (p.mask_tma &&
       make_tmap(&tm, maskbits, d->mask_mod > 0 ? d->mask_mod : d->m, d->n / 32, d->ldmaskbits,
-                mask_words(block_n), BLOCK_M, CU_TENSOR_MAP_DATA_TYPE_UINT32, 4,
+                mask_words(plan.pingpong ? PP_BN : block_n), BLOCK_M, CU_TENSOR_MAP_DATA_TYPE_UINT32, 4,
                 CU_TENSOR_MAP_SWIZZLE_NONE))
     return 1;
   const int grid = plan.grid;
@@ -714,7 +1012,17 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
       default: if (MODE_ != MNRF_GEMM_WGRAD) MNRF_LAUNCH_TC2(MODE_, 16); break;                       \
     }                                                                                                 \
   } while (0)
-  if (smooth) {
+  if (plan.pingpong) {
+    const bool fwd = d->mode == MNRF_GEMM_FWD;
+    int rc;
+    if (block_n == 256)
+      rc = fwd ? launch_gemm_tc_pingpong<MNRF_GEMM_FWD, 256>(grid, ta, tb, tc, tm, p, stream)
+               : launch_gemm_tc_pingpong<MNRF_GEMM_DGRAD, 256>(grid, ta, tb, tc, tm, p, stream);
+    else
+      rc = fwd ? launch_gemm_tc_pingpong<MNRF_GEMM_FWD, 128>(grid, ta, tb, tc, tm, p, stream)
+               : launch_gemm_tc_pingpong<MNRF_GEMM_DGRAD, 128>(grid, ta, tb, tc, tm, p, stream);
+    if (rc) return rc;
+  } else if (smooth) {
     if (int rc = gemm_tc_smooth_launch(d->mode, block_n, grid, ta, tb, tc, p, stream)) return rc;
   } else if (d->mode == MNRF_GEMM_FWD) MNRF_LAUNCH_TC(MNRF_GEMM_FWD);
   else if (d->mode == MNRF_GEMM_DGRAD) MNRF_LAUNCH_TC(MNRF_GEMM_DGRAD);
