@@ -34,7 +34,7 @@ extern "C" {
 typedef uint16_t mnrf_bf16;
 typedef void* mnrf_stream;   /* cudaStream_t */
 
-#define MNRF_ABI_VERSION 1
+#define MNRF_ABI_VERSION 2
 
 /* ---- library ------------------------------------------------------------------------- */
 int mnrf_abi_version(void);
@@ -51,6 +51,9 @@ int mnrf_num_sms(void);
  *   sdist_prev [B, P+1], w_prev [B, P]           previous step function
  *   u_base     [S]      host-computed linspace grid of stepfun.py:194-206
  *   jitter     raw U[0,1): NULL | [B] (single_jitter) | [B, S]
+ *   anneal_dev optional device scalar: the annealing exponent is read from anneal_dev[0] at run time
+ *              instead of d->anneal, so that a captured CUDA graph can be replayed while train_frac
+ *              advances (models.py:174-179)
  *   cw_in      optional [B, P'+1] CDF to use instead of the internally computed one
  *              (P' = 3P-2 with dilation, else P) -- lets tests pin the integer search
  *   sdist_out  [B, S+1]
@@ -67,14 +70,9 @@ typedef struct {
 } mnrf_sample_desc;
 
 int mnrf_sample_level(const mnrf_sample_desc* d, const float* sdist_prev, const float* w_prev,
-                      const float* u_base, const float* jitter, const float* cw_in,
+                      const float* u_base, const float* jitter, const float* anneal_dev, const float* cw_in,
                       float* sdist_out, int32_t* idx_out, float* cw_out, float* tdil_out,
                       float* wdil_out, mnrf_stream stream);
-/* Same, but the annealing exponent is read from device memory (`anneal_dev[0]`) at run time so
- * that a captured CUDA graph can be replayed while train_frac advances (models.py:174-179). */
-int mnrf_sample_level_dyn(const mnrf_sample_desc* d, const float* sdist_prev, const float* w_prev,
-                          const float* u_base, const float* jitter, const float* anneal_dev,
-                          float* sdist_out, mnrf_stream stream);
 
 /* ---- ray casting + integrated positional encoding ------------------------------------
  * Replaces coord.construct_ray_warps s_to_t (coord.py:63-99), render.cast_rays
@@ -84,6 +82,13 @@ int mnrf_sample_level_dyn(const mnrf_sample_desc* d, const float* sdist_prev, co
  *   feat_bf16  [B*S, ld_feat] row stride in elements; columns [2KL, feat_cols) zero-filled
  *   feat_f32   optional [B*S, 2KL] (fp32 copy for parity tests)
  *   tdist_out  optional [B, S+1]
+ *   tfeat_bf16 optional: the tangent features d(feature)/d(mean_x|y|z) as three stacked bf16 blocks
+ *              tfeat[dir*B*S + m, ld_tfeat] (input of the forward-mode density-normal chain that replaces
+ *              vmap(value_and_grad(predict_density)), models.py:473-492).  The derivative is taken with respect
+ *              to the world-space mean: with warp_contract it runs through the contraction, including the
+ *              dependence of the warped covariance J Sigma J^T on the mean (coord.track_linearize,
+ *              coord.py:39-60).  ld_tfeat >= feat_cols, a multiple of 8, tfeat 16-byte aligned; refused
+ *              together with feat_f32 or tdist_out.
  */
 enum { MNRF_RAYDIST_NONE = 0, MNRF_RAYDIST_RECIPROCAL, MNRF_RAYDIST_LOG, MNRF_RAYDIST_EXP,
        MNRF_RAYDIST_SQRT, MNRF_RAYDIST_SQUARE, MNRF_RAYDIST_PIECEWISE };
@@ -99,16 +104,7 @@ typedef struct {
 int mnrf_encode(const mnrf_encode_desc* d, const float* sdist, const float* origins,
                 const float* directions, const float* radii, const float* near,
                 const float* far, const float* basis, mnrf_bf16* feat_bf16, float* feat_f32,
-                float* tdist_out, mnrf_stream stream);
-/* Same, plus the tangent features d(feature)/d(mean_x|y|z) as three stacked bf16 blocks
- * tfeat[dir*B*S + m, ld_tfeat] (input of the forward-mode density-normal chain that replaces
- * vmap(value_and_grad(predict_density)), models.py:473-492).  The derivative is taken with respect to
- * the world-space mean: with warp_contract it runs through the contraction, including the dependence of
- * the warped covariance J Sigma J^T on the mean (coord.track_linearize, coord.py:39-60). */
-int mnrf_encode_tangent(const mnrf_encode_desc* d, const float* sdist, const float* origins,
-                        const float* directions, const float* radii, const float* near,
-                        const float* far, const float* basis, mnrf_bf16* feat_bf16,
-                        mnrf_bf16* tfeat_bf16, int32_t ld_tfeat, mnrf_stream stream);
+                float* tdist_out, mnrf_bf16* tfeat_bf16, int32_t ld_tfeat, mnrf_stream stream);
 
 /* View-direction positional encoding, coord.pos_enc (coord.py:136-147) with
  * append_identity, broadcast over the S samples of each ray (models.py:550-554) and
@@ -133,7 +129,7 @@ int mnrf_viewdir_enc(int32_t num_rays, int32_t num_samples, int32_t deg, const f
  */
 enum { MNRF_GEMM_FWD = 0, MNRF_GEMM_DGRAD = 1, MNRF_GEMM_WGRAD = 2 };
 /* Activations of the Dense layers (MLP.net_activation, models.py:457,578): SOFTPLUS is jax.nn.softplus
- * (logaddexp(z, 0)), SILU is jax.nn.silu (z * sigmoid(z)).  The two smooth ones run through mnrf_gemm_act. */
+ * (logaddexp(z, 0)), SILU is jax.nn.silu (z * sigmoid(z)). */
 enum { MNRF_ACT_NONE = 0, MNRF_ACT_RELU = 1, MNRF_ACT_SOFTPLUS = 2, MNRF_ACT_SILU = 3 };
 
 typedef struct {
@@ -156,22 +152,19 @@ typedef struct {
  * of the layer whose activation masks this dgrad; reduced from the epilogue registers (fp32,
  * before the bf16 rounding of the stored output) -- no separate pass over dY.
  * addend (optional, DGRAD only): out += addend[M, ldadd] (bf16), added after the mask -- the second
- * gradient contribution to an input consumed twice (skip connection of the view MLP). */
-int mnrf_gemm(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
-              const float* rowv, const float* colv, const mnrf_bf16* mask, uint32_t* maskbits,
-              float* colsum, const mnrf_bf16* addend, void* out, mnrf_stream stream);
-
-/* The FWD and DGRAD GEMMs of a layer with a smooth activation, d->act = MNRF_ACT_SOFTPLUS or MNRF_ACT_SILU.  The
- * backward needs a'(z) (and, for density normals, a''(z)) of the pre-activation z, which the output h = a(z) does
- * not give back for SiLU, so the forward stores z itself in place of mask bits:
+ * gradient contribution to an input consumed twice (skip connection of the view MLP).
+ * z / ldz: the pre-activation of a smooth activation (d->act = MNRF_ACT_SOFTPLUS or MNRF_ACT_SILU; refused with any
+ * other act).  The backward needs a'(z) (and, for density normals, a''(z)), which the output h = a(z) does not give
+ * back for SiLU, so the forward stores z itself in place of mask bits:
  *   mode FWD  : out[M,N] = a(z), z = A Bt^T + bias;  z[M, ldz] (optional, bf16) receives z
  *   mode DGRAD: out[M,N] = a'(z[r]) * (A Bt^T + rowv colv) + addend, with z row r = output row mod d->mask_mod (when
  *               > 0: the three tangent streams share the primal's z); colsum[N] += column sums of out
- * rowv/colv, addend and colsum are those of mnrf_gemm; `mask` and `maskbits` have no counterpart here.  N must be a
- * multiple of 64 and `out` 16-byte aligned with a row pitch that is a multiple of 8 on the tensor-core path (impl 0). */
-int mnrf_gemm_act(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
-                  const float* rowv, const float* colv, float* colsum, const mnrf_bf16* addend, mnrf_bf16* z,
-                  int64_t ldz, void* out, mnrf_stream stream);
+ * A smooth activation takes FWD or DGRAD only, z (required for DGRAD) with ldz >= N, and no `mask` / `maskbits`; N
+ * must be a multiple of 64 and `out` 16-byte aligned with a row pitch that is a multiple of 8 on the tensor-core path
+ * (impl 0). */
+int mnrf_gemm(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
+              const float* rowv, const float* colv, const mnrf_bf16* mask, uint32_t* maskbits,
+              float* colsum, const mnrf_bf16* addend, mnrf_bf16* z, int64_t ldz, void* out, mnrf_stream stream);
 
 /* Weight gradient with side sums computed from the operand tiles the main loop stages (by the three warps of
  * the producer warpgroup that issue no loads), so the bias gradient and the gradient of a Dense(1) head on the
@@ -184,15 +177,15 @@ int mnrf_gemm_act(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* 
 int mnrf_gemm_wgrad(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, float* bsum,
                     const float* side_w, float* side_aw, float* out, mnrf_stream stream);
 
-/* The kernel instance and launch shape the tensor-core path (impl 0) of mnrf_gemm / mnrf_gemm_act /
- * mnrf_gemm_wgrad chooses for these arguments, which take the places they have there (z / ldz: mnrf_gemm_act;
- * bsum / side_w / side_aw: mnrf_gemm_wgrad; null where the call has none).  Host-only: no pointer is dereferenced
+/* The kernel instance and launch shape the tensor-core path (impl 0) of mnrf_gemm / mnrf_gemm_wgrad chooses for
+ * these arguments, which take the places they have there (bsum / side_w / side_aw: mnrf_gemm_wgrad; null where the
+ * call has none).  Host-only: no pointer is dereferenced
  * and nothing is launched.  Returns nonzero, with the launch's error message, for arguments the launch refuses. */
 typedef struct {
   int32_t block_n;    /* output tile width BN: 256, 128, 64, 32 or 16 */
   int32_t staged;     /* 1: the bf16 output goes through shared memory and TMA bulk stores; 0: register stores */
   int32_t mask_tma;   /* DGRAD mask bits: 1 loaded by TMA with the operands; 0 loaded by the epilogue (or none) */
-  int32_t smooth;     /* softplus / SiLU epilogue (mnrf_gemm_act) */
+  int32_t smooth;     /* softplus / SiLU epilogue */
   int32_t side;       /* WGRAD side sums (bsum / side_aw) */
   int32_t splits;     /* reduction splits (WGRAD; 1 otherwise) */
   int32_t tiles;      /* work items: row blocks x column blocks x splits */
@@ -267,8 +260,8 @@ int mnrf_mlp_chain_max_layers(void);
 
 /* ---- small heads (N <= 4 outputs): density / rgb / predicted normals ---------------------
  * raw[M, n_out] = X[M, K](bf16) * W[n_out, K](bf16) + b, fp32 accumulate; models.py:460,585.
- * Backward: dX[M, K] (bf16, optionally relu-masked by X > 0; optional accumulate is not
- * provided -- the trunk adds the density term through mnrf_gemm's rowv/colv),
+ * Backward: dX[M, K] (bf16, multiplied by the derivative of the activation `act` that produced X; optional
+ * accumulate is not provided -- the trunk adds the density term through mnrf_gemm's rowv/colv),
  * dW[K, n_out] += (the fp32 master layout [in, out]), db[n_out] += (fp32 atomics);
  * dxsum[K] += column sums of dX (optional: bias gradient of the layer that produced X).
  * 0 < dw_split < n_out splits dW between two master matrices: outputs [0, dw_split) go to
@@ -276,22 +269,22 @@ int mnrf_mlp_chain_max_layers(void);
  * of a view-independent model run as one stacked head; their weights live apart).  dx_cols (0: K) limits dX and
  * dxsum to the first dx_cols columns (a head reading [hidden | features] needs the gradient of the hidden part only).
  * dx2 (optional, needs dx_cols < K): dx2[M, K - dx_cols] (bf16, row pitch lddx2) receives the input gradient of
- * columns [dx_cols, K), never relu-masked and not summed into dxsum -- the rgb head of a view MLP that ends on a
- * skip layer reads [hidden | view input], and the second part is its contribution to the view input's gradient.
+ * columns [dx_cols, K), never multiplied by the activation derivative and not summed into dxsum -- the rgb head of a
+ * view MLP that ends on a skip layer reads [hidden | view input], and the second part is its contribution to the view
+ * input's gradient.
+ * act: the factor applied to dx[m, k] for k < dx_cols (dxsum sums the factored dx):
+ *   MNRF_ACT_NONE                      none
+ *   MNRF_ACT_RELU                      the ReLU mask X > 0
+ *   MNRF_ACT_SOFTPLUS | MNRF_ACT_SILU  a'(z[m, k]), z [M, ldz] bf16 the pre-activation of the layer that produced X
+ *                                      (mnrf_gemm FWD); needs dx, ldz a multiple of 8 and z 16-byte aligned
+ * z is refused with any other act.
  */
 int mnrf_head_fwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx,
                   const mnrf_bf16* w, const float* b, float* raw, mnrf_stream stream);
 int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx,
                   const mnrf_bf16* w, const float* draw, mnrf_bf16* dx, int64_t lddx,
-                  int32_t relu_mask, float* dw, float* dw2, int32_t dw_split, float* db, float* dxsum,
-                  int32_t dx_cols, mnrf_bf16* dx2, int64_t lddx2, mnrf_stream stream);
-/* Same, with the derivative of a smooth activation (act = MNRF_ACT_SOFTPLUS | MNRF_ACT_SILU) in place of the ReLU
- * mask: dx[m, k] *= a'(z[m, k]) for k < dx_cols, z [M, ldz] bf16 the pre-activation of the layer that produced X
- * (mnrf_gemm_act FWD); ldz a multiple of 8, z 16-byte aligned.  dxsum sums the factored dx. */
-int mnrf_head_bwd_act(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx,
-                      const mnrf_bf16* w, const float* draw, mnrf_bf16* dx, int64_t lddx,
-                      int32_t act, const mnrf_bf16* z, int64_t ldz, float* dw, float* dw2, int32_t dw_split,
-                      float* db, float* dxsum, int32_t dx_cols, mnrf_bf16* dx2, int64_t lddx2, mnrf_stream stream);
+                  int32_t act, const mnrf_bf16* z, int64_t ldz, float* dw, float* dw2, int32_t dw_split,
+                  float* db, float* dxsum, int32_t dx_cols, mnrf_bf16* dx2, int64_t lddx2, mnrf_stream stream);
 
 /* Column sums of a bf16 matrix into fp32 (bias gradients): out[N] += sum_m x[m, :]. */
 int mnrf_colsum(int64_t m, int32_t n, const mnrf_bf16* x, int64_t ldx, float* out,
@@ -341,6 +334,12 @@ int mnrf_composite_fwd(const mnrf_composite_desc* d, const float* raw_density,
  * and rgb-activation derivatives.
  *   outputs: d_raw_density [B,S]; d_raw_rgb [B,S,3] or NULL; stats[8] += (fp32 atomics):
  *     [0] data loss (already weighted by data_mult)  [1] mse  [2] distortion  [3] interlevel
+ *   data_mask  optional [B] fp32 per-ray 0/1 weight on the data loss (data_loss_type 'robustnerf',
+ *              train_utils.py:104-108): the data-loss value and its gradient of ray r are multiplied by
+ *              data_mask[r]; the mse stat (stats[1]) stays unmasked.  NULL: unmasked.
+ *   batch_rays the ray count the distortion and interlevel means divide by (>= num_rays): num_rays for a one-pass
+ *              step; the whole batch for one pass of a train step that runs its batch in several passes, so each
+ *              pass adds its share to stats and every per-sample gradient equals the one-pass step's.
  */
 enum { MNRF_LOSS_MSE = 0, MNRF_LOSS_CHARB = 1, MNRF_LOSS_RAWNERF = 2 };
 
@@ -362,35 +361,10 @@ int mnrf_composite_bwd(const mnrf_loss_desc* d, const float* raw_density, const 
                        const float* extra_dw /* [B,S] added to dL/dweights, or NULL */,
                        const float* target_rgb,
                        const float* lossmult, const float* inv_denom /* device scalar */,
-                       const float* sdist_fine, const float* weights_fine,
+                       const float* sdist_fine, const float* weights_fine, const float* data_mask,
                        float* d_raw_density, float* d_raw_rgb, float* d_rgb_scale /* [B,3] or NULL */,
-                       float* d_raw_diffuse, float* d_raw_tint, float* stats, mnrf_stream stream);
-/* Same, with a per-ray 0/1 weight on the data loss (data_loss_type 'robustnerf', train_utils.py:104-108):
- * the data-loss value and its gradient of ray r are multiplied by data_mask[r] ([B] fp32); the mse stat
- * (stats[1]) stays unmasked.  data_mask == NULL is mnrf_composite_bwd. */
-int mnrf_composite_bwd_masked(const mnrf_loss_desc* d, const float* raw_density, const float* raw_rgb,
-                              const float* density_noise, const float* sdist, const float* directions,
-                              const float* near, const float* far, const float* bg_rgb,
-                              const float* rgb_scale, const float* raw_diffuse, const float* raw_tint,
-                              const float* extra_dw, const float* target_rgb,
-                              const float* lossmult, const float* inv_denom,
-                              const float* sdist_fine, const float* weights_fine, const float* data_mask,
-                              float* d_raw_density, float* d_raw_rgb, float* d_rgb_scale,
-                              float* d_raw_diffuse, float* d_raw_tint, float* stats, mnrf_stream stream);
-/* Same as mnrf_composite_bwd_masked (data_mask may be NULL) for one pass of a train step that runs its batch in
- * several passes: the distortion and interlevel losses are means over `batch_rays` rays (the whole batch,
- * >= num_rays) instead of the launch's num_rays, so each pass adds its share to stats and every per-sample gradient
- * equals the one-pass step's.  batch_rays == num_rays is mnrf_composite_bwd_masked. */
-int mnrf_composite_bwd_chunk(const mnrf_loss_desc* d, const float* raw_density, const float* raw_rgb,
-                             const float* density_noise, const float* sdist, const float* directions,
-                             const float* near, const float* far, const float* bg_rgb,
-                             const float* rgb_scale, const float* raw_diffuse, const float* raw_tint,
-                             const float* extra_dw, const float* target_rgb,
-                             const float* lossmult, const float* inv_denom,
-                             const float* sdist_fine, const float* weights_fine, const float* data_mask,
-                             float* d_raw_density, float* d_raw_rgb, float* d_rgb_scale,
-                             float* d_raw_diffuse, float* d_raw_tint, float* stats, int32_t batch_rays,
-                             mnrf_stream stream);
+                       float* d_raw_diffuse, float* d_raw_tint, float* stats, int32_t batch_rays,
+                       mnrf_stream stream);
 
 /* ---- RobustNeRF mask and inlier threshold (robustnerf.py:8-115) ------------------------------
  * mnrf_robust_mask: one CTA per patch; rays are patch-major [num_rays / p^2, p, p].
@@ -398,8 +372,10 @@ int mnrf_composite_bwd_chunk(const mnrf_loss_desc* d, const float* raw_density, 
  *   mask [B] fp32 0/1 (all ones when enable == 0); error_per_pixel [B] = mean over the 3 channels of
  *   (rgb - target)^2, rounded as ((r0 + r1) + r2) / 3
  *   stats (optional): stats[1..4] += per-rank means of is_inlier_loss, has_inlier_neighbors,
- *   is_inlier_patch, mask (only mask when enable == 0); needs `counts`, a uint32[5] workspace that is
- *   zero before the first launch and that every launch leaves zero.
+ *   is_inlier_patch, mask (only mask when enable == 0), as count / batch_rays; needs `counts`, a uint32[5]
+ *   workspace that is zero before the first launch and that every launch leaves zero.
+ *   batch_rays (>= num_rays): num_rays for a one-pass step; the whole batch for one pass of a step over several,
+ *   so the passes of a step add up to the batch's means.
  * Requires p*p <= 1024, num_rays a multiple of p*p, and (enable) inner_patch_size <= p, odd filter_size <= p.
  * Comparisons on neighbourhood / patch means use fl32(count / size) > fl32(1 - quantile); see csrc/robust.cu
  * for the tie rule of the box filter.
@@ -415,12 +391,8 @@ typedef struct {
 } mnrf_robust_desc;
 
 int mnrf_robust_mask(const mnrf_robust_desc* d, const float* rgb, const float* target, const float* threshold,
-                     float* mask, float* error_per_pixel, uint32_t* counts, float* stats, mnrf_stream stream);
-/* Same for one pass of a batch of batch_rays (>= num_rays) rays: stats[1..4] += count / batch_rays, so the passes
- * of a step add up to the batch's means.  batch_rays == num_rays is mnrf_robust_mask. */
-int mnrf_robust_mask_chunk(const mnrf_robust_desc* d, const float* rgb, const float* target, const float* threshold,
-                           float* mask, float* error_per_pixel, uint32_t* counts, float* stats, int32_t batch_rays,
-                           mnrf_stream stream);
+                     float* mask, float* error_per_pixel, uint32_t* counts, float* stats, int32_t batch_rays,
+                     mnrf_stream stream);
 int mnrf_quantile(int32_t n, float q, const float* x, float* out, mnrf_stream stream);
 
 /* ---- Ref-NeRF per-sample stage ---------------------------------------------------------------
@@ -546,6 +518,8 @@ int mnrf_spherical_rays(const mnrf_spherical_desc* d, float* origins, float* dir
  * train_utils.clip_gradients (train_utils.py:200-218: value clip, then global-norm clip with
  * eps in the denominator), nan_to_num (:328) and optax.adam on one flat fp32 parameter
  * group (one top-level module).  norm_sq_scratch: device float[1], zeroed by the call.
+ * dyn (optional): (lr, 1-beta1^t, 1-beta2^t) read from device memory dyn[0..2] instead of computed from d
+ * (graph replay).
  */
 typedef struct {
   int64_t n;
@@ -556,17 +530,11 @@ typedef struct {
 } mnrf_adam_desc;
 
 int mnrf_clip_adam(const mnrf_adam_desc* d, float* params, const float* grads, float* mu,
-                   float* nu, float* norm_sq_scratch, mnrf_stream stream);
-/* Same, but (lr, 1-beta1^t, 1-beta2^t) are read from device memory `dyn[0..2]` (graph replay). */
-int mnrf_clip_adam_dyn(const mnrf_adam_desc* d, float* params, const float* grads, float* mu,
-                       float* nu, float* norm_sq_scratch, const float* dyn, mnrf_stream stream);
+                   float* nu, float* norm_sq_scratch, const float* dyn, mnrf_stream stream);
 
 /* fp32 master [in_pad, out] (row-major) -> bf16 shadows: w_nk [out, in_pad] (K-major operand
- * of the forward GEMM) and w_kn [in_pad, out] (K-major operand of the dgrad GEMM). */
-int mnrf_pack_weights(int32_t in_pad, int32_t out, const float* master, mnrf_bf16* w_nk,
-                      mnrf_bf16* w_kn, mnrf_stream stream);
-
-/* The same for `count` layers in one launch (the optimizer epilogue of a train step).  `items` is a
+ * of the forward GEMM) and w_kn [in_pad, out] (K-major operand of the dgrad GEMM), for `count` layers
+ * in one launch (the optimizer epilogue of a train step).  `items` is a
  * DEVICE array of mnrf_pack_item, ordered as the layers' 32x32 tiles are numbered: item i owns tiles
  * [tile0, tile0 + ceil(out/32) * ceil(in_pad/32)), tile0 of item i+1 = the end of item i;
  * total_tiles = the end of the last item. */

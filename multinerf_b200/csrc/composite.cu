@@ -515,17 +515,15 @@ extern "C" int mnrf_composite_fwd(const mnrf_composite_desc* d, const float* raw
   return 0;
 }
 
-// mnrf_composite_bwd, mnrf_composite_bwd_masked and mnrf_composite_bwd_chunk share this body (data_mask == NULL: no
-// mask; batch_rays: the ray count the per-ray means divide by, num_rays unless the launch is one pass of a batch).
-static int composite_bwd_launch(const mnrf_loss_desc* d, const float* raw_density, const float* raw_rgb,
-                                const float* density_noise, const float* sdist, const float* directions,
-                                const float* near, const float* far, const float* bg_rgb, const float* rgb_scale,
-                                const float* raw_diffuse, const float* raw_tint, const float* extra_dw,
-                                const float* target_rgb, const float* lossmult, const float* inv_denom,
-                                const float* sdist_fine, const float* weights_fine, const float* data_mask,
-                                float* d_raw_density, float* d_raw_rgb, float* d_rgb_scale,
-                                float* d_raw_diffuse, float* d_raw_tint, float* stats, int32_t batch_rays,
-                                mnrf_stream stream) {
+extern "C" int mnrf_composite_bwd(const mnrf_loss_desc* d, const float* raw_density, const float* raw_rgb,
+                                  const float* density_noise, const float* sdist, const float* directions,
+                                  const float* near, const float* far, const float* bg_rgb, const float* rgb_scale,
+                                  const float* raw_diffuse, const float* raw_tint, const float* extra_dw,
+                                  const float* target_rgb, const float* lossmult, const float* inv_denom,
+                                  const float* sdist_fine, const float* weights_fine, const float* data_mask,
+                                  float* d_raw_density, float* d_raw_rgb, float* d_rgb_scale,
+                                  float* d_raw_diffuse, float* d_raw_tint, float* stats, int32_t batch_rays,
+                                  mnrf_stream stream) {
   using namespace mnrf;
   MNRF_CHECK(d->c.rgb_mode == 0 || (raw_rgb && raw_diffuse && d_raw_diffuse && (!raw_tint || d_raw_tint)),
              "mnrf_composite_bwd: rgb_mode 1 needs raw_diffuse / d_raw_diffuse (and d_raw_tint with raw_tint)");
@@ -538,7 +536,7 @@ static int composite_bwd_launch(const mnrf_loss_desc* d, const float* raw_densit
              "mnrf_composite_bwd: interlevel loss needs the final level's sdist/weights");
   MNRF_CHECK(d->lossmult_channels == 1 || d->lossmult_channels == 3, "lossmult_channels must be 1 or 3");
   MNRF_CHECK(d->loss_type >= 0 && d->loss_type <= 2, "unknown data_loss_type");
-  MNRF_CHECK(batch_rays >= d->c.num_rays, "mnrf_composite_bwd_chunk: batch_rays %d < num_rays %d", batch_rays,
+  MNRF_CHECK(batch_rays >= d->c.num_rays, "mnrf_composite_bwd: batch_rays %d < num_rays %d", batch_rays,
              d->c.num_rays);
   if (d->c.num_rays == 0) return 0;
   const int nw = 4;
@@ -552,57 +550,4 @@ static int composite_bwd_launch(const mnrf_loss_desc* d, const float* raw_densit
       d_raw_rgb, d_rgb_scale, d_raw_diffuse, d_raw_tint, stats, batch_rays)));
   MNRF_LAUNCH_CHECK();
   return 0;
-}
-
-extern "C" int mnrf_composite_bwd(const mnrf_loss_desc* d, const float* raw_density,
-                                  const float* raw_rgb, const float* density_noise,
-                                  const float* sdist, const float* directions, const float* near,
-                                  const float* far, const float* bg_rgb, const float* rgb_scale,
-                                  const float* raw_diffuse, const float* raw_tint, const float* extra_dw,
-                                  const float* target_rgb,
-                                  const float* lossmult, const float* inv_denom,
-                                  const float* sdist_fine, const float* weights_fine,
-                                  float* d_raw_density, float* d_raw_rgb, float* d_rgb_scale,
-                                  float* d_raw_diffuse, float* d_raw_tint, float* stats,
-                                  mnrf_stream stream) {
-  return composite_bwd_launch(d, raw_density, raw_rgb, density_noise, sdist, directions, near, far, bg_rgb,
-                              rgb_scale, raw_diffuse, raw_tint, extra_dw, target_rgb, lossmult, inv_denom,
-                              sdist_fine, weights_fine, nullptr, d_raw_density, d_raw_rgb, d_rgb_scale,
-                              d_raw_diffuse, d_raw_tint, stats, d ? d->c.num_rays : 0, stream);
-}
-
-extern "C" int mnrf_composite_bwd_masked(const mnrf_loss_desc* d, const float* raw_density,
-                                         const float* raw_rgb, const float* density_noise,
-                                         const float* sdist, const float* directions, const float* near,
-                                         const float* far, const float* bg_rgb, const float* rgb_scale,
-                                         const float* raw_diffuse, const float* raw_tint, const float* extra_dw,
-                                         const float* target_rgb,
-                                         const float* lossmult, const float* inv_denom,
-                                         const float* sdist_fine, const float* weights_fine,
-                                         const float* data_mask,
-                                         float* d_raw_density, float* d_raw_rgb, float* d_rgb_scale,
-                                         float* d_raw_diffuse, float* d_raw_tint, float* stats,
-                                         mnrf_stream stream) {
-  return composite_bwd_launch(d, raw_density, raw_rgb, density_noise, sdist, directions, near, far, bg_rgb,
-                              rgb_scale, raw_diffuse, raw_tint, extra_dw, target_rgb, lossmult, inv_denom,
-                              sdist_fine, weights_fine, data_mask, d_raw_density, d_raw_rgb, d_rgb_scale,
-                              d_raw_diffuse, d_raw_tint, stats, d ? d->c.num_rays : 0, stream);
-}
-
-extern "C" int mnrf_composite_bwd_chunk(const mnrf_loss_desc* d, const float* raw_density,
-                                        const float* raw_rgb, const float* density_noise,
-                                        const float* sdist, const float* directions, const float* near,
-                                        const float* far, const float* bg_rgb, const float* rgb_scale,
-                                        const float* raw_diffuse, const float* raw_tint, const float* extra_dw,
-                                        const float* target_rgb,
-                                        const float* lossmult, const float* inv_denom,
-                                        const float* sdist_fine, const float* weights_fine,
-                                        const float* data_mask,
-                                        float* d_raw_density, float* d_raw_rgb, float* d_rgb_scale,
-                                        float* d_raw_diffuse, float* d_raw_tint, float* stats,
-                                        int32_t batch_rays, mnrf_stream stream) {
-  return composite_bwd_launch(d, raw_density, raw_rgb, density_noise, sdist, directions, near, far, bg_rgb,
-                              rgb_scale, raw_diffuse, raw_tint, extra_dw, target_rgb, lossmult, inv_denom,
-                              sdist_fine, weights_fine, data_mask, d_raw_density, d_raw_rgb, d_rgb_scale,
-                              d_raw_diffuse, d_raw_tint, stats, batch_rays, stream);
 }

@@ -497,19 +497,20 @@ viewdir_enc_rows_kernel(int num_rays, int S, int deg, const float* __restrict__ 
 
 }  // namespace mnrf
 
-static int encode_impl(const mnrf_encode_desc* d, const float* sdist, const float* origins,
-                       const float* directions, const float* radii, const float* near,
-                       const float* far, const float* basis, mnrf_bf16* feat_bf16,
-                       float* feat_f32, float* tdist_out, mnrf_bf16* tfeat, int ld_tfeat,
-                       mnrf_stream stream) {
+extern "C" int mnrf_encode(const mnrf_encode_desc* d, const float* sdist, const float* origins,
+                           const float* directions, const float* radii, const float* near,
+                           const float* far, const float* basis, mnrf_bf16* feat_bf16,
+                           float* feat_f32, float* tdist_out, mnrf_bf16* tfeat, int32_t ld_tfeat,
+                           mnrf_stream stream) {
   using namespace mnrf;
   if (d && d->num_rays == 0) return 0;            // nothing to do (and empty tensors carry null pointers)
-  if (tfeat) {
-    MNRF_CHECK(ld_tfeat >= d->feat_cols && ld_tfeat % 8 == 0 && ((uintptr_t)tfeat % 16) == 0,
-               "mnrf_encode_tangent: tangent rows must be 16-byte aligned");
-  }
   MNRF_CHECK(d && sdist && origins && directions && radii && near && far && basis && feat_bf16,
              "mnrf_encode: null pointer");
+  if (tfeat) {
+    MNRF_CHECK(!feat_f32 && !tdist_out, "mnrf_encode: the tangent features take no feat_f32 / tdist_out");
+    MNRF_CHECK(ld_tfeat >= d->feat_cols && ld_tfeat % 8 == 0 && ((uintptr_t)tfeat % 16) == 0,
+               "mnrf_encode: tangent rows must be 16-byte aligned");
+  }
   MNRF_CHECK(d->ray_shape == MNRF_RAY_CONE || d->ray_shape == MNRF_RAY_CYLINDER,
              "ray_shape must be 'cone' or 'cylinder'");
   const int KL2 = 2 * d->basis_k * (d->max_deg - d->min_deg);
@@ -564,25 +565,6 @@ static int encode_impl(const mnrf_encode_desc* d, const float* sdist, const floa
       reinterpret_cast<__nv_bfloat16*>(tfeat), ld_tfeat);
   MNRF_LAUNCH_CHECK();
   return 0;
-}
-
-extern "C" int mnrf_encode(const mnrf_encode_desc* d, const float* sdist, const float* origins,
-                           const float* directions, const float* radii, const float* near,
-                           const float* far, const float* basis, mnrf_bf16* feat_bf16,
-                           float* feat_f32, float* tdist_out, mnrf_stream stream) {
-  return encode_impl(d, sdist, origins, directions, radii, near, far, basis, feat_bf16, feat_f32, tdist_out,
-                     nullptr, 0, stream);
-}
-
-extern "C" int mnrf_encode_tangent(const mnrf_encode_desc* d, const float* sdist, const float* origins,
-                                   const float* directions, const float* radii, const float* near,
-                                   const float* far, const float* basis, mnrf_bf16* feat_bf16,
-                                   mnrf_bf16* tfeat_bf16, int32_t ld_tfeat, mnrf_stream stream) {
-  mnrf::set_error("");
-  if (d && d->num_rays == 0) return 0;
-  if (!tfeat_bf16) { mnrf::set_error("mnrf_encode_tangent: null tangent buffer"); return 1; }
-  return encode_impl(d, sdist, origins, directions, radii, near, far, basis, feat_bf16, nullptr, nullptr,
-                     tfeat_bf16, ld_tfeat, stream);
 }
 
 extern "C" int mnrf_viewdir_enc(int32_t num_rays, int32_t num_samples, int32_t deg,

@@ -83,8 +83,7 @@ __global__ void gemm_ref_tn_kernel(mnrf_gemm_desc d, const __nv_bfloat16* __rest
 
 }  // namespace mnrf
 
-// mnrf_gemm and mnrf_gemm_act: z (smooth activations) is null for mnrf_gemm
-static int gemm_dispatch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
+extern "C" int mnrf_gemm(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
                          const float* rowv, const float* colv, const mnrf_bf16* mask, uint32_t* maskbits,
                          float* colsum, const mnrf_bf16* addend, mnrf_bf16* z, int64_t ldz, void* out,
                          mnrf_stream stream) {
@@ -92,6 +91,14 @@ static int gemm_dispatch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf
   if (d && (d->m == 0 || d->n == 0 || d->k == 0)) return 0;   // empty operand: nothing to compute or accumulate
   MNRF_CHECK(d && a && b && out, "mnrf_gemm: null pointer");
   MNRF_CHECK(d->mode >= 0 && d->mode <= 2, "mnrf_gemm: unknown mode %d", d->mode);
+  if (d->act == MNRF_ACT_SOFTPLUS || d->act == MNRF_ACT_SILU) {
+    MNRF_CHECK(d->mode == MNRF_GEMM_FWD || d->mode == MNRF_GEMM_DGRAD, "mnrf_gemm: a smooth activation is FWD or DGRAD");
+    MNRF_CHECK(d->mode == MNRF_GEMM_FWD || z, "mnrf_gemm: the DGRAD of a smooth activation needs z");
+    MNRF_CHECK(!z || ldz >= d->n, "mnrf_gemm: ldz %lld < N %d", (long long)ldz, d->n);
+    MNRF_CHECK(!mask && !maskbits, "mnrf_gemm: a smooth activation takes z, not a ReLU mask");
+  } else {
+    MNRF_CHECK(!z, "mnrf_gemm: z is the pre-activation of a smooth activation, act %d is not one", d->act);
+  }
   MNRF_CHECK((rowv == nullptr) == (colv == nullptr), "mnrf_gemm: rowv and colv come together");
   // the bf16 mask has a row per output row (mask_mod is for the 1-bit masks and z of the stacked tangent streams)
   MNRF_CHECK(!mask || d->mask_mod == 0, "mnrf_gemm: mask_mod applies to maskbits and z, not to a bf16 mask");
@@ -132,26 +139,6 @@ static int gemm_dispatch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf
   return 0;
 }
 
-extern "C" int mnrf_gemm(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
-                         const float* rowv, const float* colv, const mnrf_bf16* mask, uint32_t* maskbits,
-                         float* colsum, const mnrf_bf16* addend, void* out, mnrf_stream stream) {
-  return gemm_dispatch(d, a, b, bias, rowv, colv, mask, maskbits, colsum, addend, nullptr, 0, out, stream);
-}
-
-extern "C" int mnrf_gemm_act(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
-                             const float* rowv, const float* colv, float* colsum, const mnrf_bf16* addend,
-                             mnrf_bf16* z, int64_t ldz, void* out, mnrf_stream stream) {
-  using namespace mnrf;
-  MNRF_CHECK(d, "mnrf_gemm_act: null pointer");
-  MNRF_CHECK(d->act == MNRF_ACT_SOFTPLUS || d->act == MNRF_ACT_SILU,
-             "mnrf_gemm_act: act %d is not a smooth activation (softplus %d, silu %d)", d->act, MNRF_ACT_SOFTPLUS,
-             MNRF_ACT_SILU);
-  MNRF_CHECK(d->mode == MNRF_GEMM_FWD || d->mode == MNRF_GEMM_DGRAD, "mnrf_gemm_act: FWD or DGRAD only");
-  MNRF_CHECK(d->mode == MNRF_GEMM_FWD || z, "mnrf_gemm_act: the DGRAD needs z");
-  MNRF_CHECK(!z || ldz >= d->n, "mnrf_gemm_act: ldz %lld < N %d", (long long)ldz, d->n);
-  return gemm_dispatch(d, a, b, bias, rowv, colv, nullptr, nullptr, colsum, addend, z, ldz, out, stream);
-}
-
 extern "C" int mnrf_gemm_wgrad(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, float* bsum,
                                const float* side_w, float* side_aw, float* out, mnrf_stream stream) {
   using namespace mnrf;
@@ -163,12 +150,14 @@ extern "C" int mnrf_gemm_wgrad(const mnrf_gemm_desc* d, const mnrf_bf16* a, cons
   if (d->impl == 0) return gemm_tc_launch(d, a, b, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, out,
                                           (cudaStream_t)stream, bsum, side_w, side_aw, nullptr, 0);
   // SIMT reference: the weight gradient, then the side sums as separate passes over the same operands
-  if (int rc = mnrf_gemm(d, a, b, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, out, stream)) return rc;
+  if (int rc = mnrf_gemm(d, a, b, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, out,
+                         stream))
+    return rc;
   if (bsum)
     if (int rc = mnrf_colsum(d->k, d->n, b, d->ldb, bsum, stream)) return rc;
   if (side_aw)      // side_aw[m] += sum_r side_w[r] * A[r, m]  ==  the dW of a Dense(1) head on A with draw = side_w
-    if (int rc = mnrf_head_bwd(d->k, (int32_t)d->m, 1, a, d->lda, a, side_w, nullptr, 0, 0, side_aw, nullptr, 0,
-                               nullptr, nullptr, 0, nullptr, 0, stream))
+    if (int rc = mnrf_head_bwd(d->k, (int32_t)d->m, 1, a, d->lda, a, side_w, nullptr, 0, MNRF_ACT_NONE, nullptr, 0,
+                               side_aw, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, stream))
       return rc;
   return 0;
 }

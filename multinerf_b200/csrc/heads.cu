@@ -391,23 +391,6 @@ colsum_kernel(int64_t M, int N, const __nv_bfloat16* __restrict__ x, int64_t ldx
   for (int e = 0; e < 8; ++e) atomicAdd(&out[col + e], acc[e]);
 }
 
-__global__ void pack_weights_kernel(int in_pad, int out, const float* __restrict__ master,
-                                    __nv_bfloat16* __restrict__ w_nk, __nv_bfloat16* __restrict__ w_kn) {
-  __shared__ float tile[32][33];
-  const int k0 = blockIdx.y * 32, n0 = blockIdx.x * 32;
-  for (int r = threadIdx.y; r < 32; r += blockDim.y) {
-    int k = k0 + r, n = n0 + threadIdx.x;
-    float v = (k < in_pad && n < out) ? master[(size_t)k * out + n] : 0.f;
-    tile[r][threadIdx.x] = v;
-    if (w_kn && k < in_pad && n < out) w_kn[(size_t)k * out + n] = __float2bfloat16(v);
-  }
-  __syncthreads();
-  for (int r = threadIdx.y; r < 32; r += blockDim.y) {
-    int n = n0 + r, k = k0 + threadIdx.x;
-    if (w_nk && n < out && k < in_pad) w_nk[(size_t)n * in_pad + k] = __float2bfloat16(tile[threadIdx.x][r]);
-  }
-}
-
 // One launch for every layer: blockIdx.x is a global tile number, the owning layer is found by a
 // binary search over the items' first tiles.
 __global__ void pack_weights_batched_kernel(int count, const mnrf_pack_item* __restrict__ items) {
@@ -520,11 +503,10 @@ extern "C" int mnrf_head_fwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf1
   return 0;
 }
 
-// mnrf_head_bwd and mnrf_head_bwd_act: z (the smooth activation's pre-activation) is null for mnrf_head_bwd
-static int head_bwd_impl(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx, const mnrf_bf16* w,
-                         const float* draw, mnrf_bf16* dx, int64_t lddx, int32_t relu_mask, int32_t act,
-                         const mnrf_bf16* z_, int64_t ldz, float* dw, float* dw2, int32_t dw_split, float* db,
-                         float* dxsum, int32_t dx_cols, mnrf_bf16* dx2, int64_t lddx2, mnrf_stream stream) {
+extern "C" int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx,
+                             const mnrf_bf16* w, const float* draw, mnrf_bf16* dx, int64_t lddx, int32_t act,
+                             const mnrf_bf16* z_, int64_t ldz, float* dw, float* dw2, int32_t dw_split, float* db,
+                             float* dxsum, int32_t dx_cols, mnrf_bf16* dx2, int64_t lddx2, mnrf_stream stream) {
   using namespace mnrf;
   const __nv_bfloat16* z = reinterpret_cast<const __nv_bfloat16*>(z_);
   if (m == 0) return 0;
@@ -539,6 +521,14 @@ static int head_bwd_impl(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x
   MNRF_CHECK(!dx2 || (dx_cols < k && lddx2 % 8 == 0 && ((uintptr_t)dx2 % 16) == 0),
              "mnrf_head_bwd: dx2 needs dx_cols < K, a pitch that is a multiple of 8 and a 16-byte aligned pointer");
   MNRF_CHECK(dw_split == n_out || (dw && dw2), "mnrf_head_bwd: a split weight gradient needs dw and dw2");
+  MNRF_CHECK(act >= MNRF_ACT_NONE && act <= MNRF_ACT_SILU, "mnrf_head_bwd: unknown act %d", act);
+  const bool smooth = act == MNRF_ACT_SOFTPLUS || act == MNRF_ACT_SILU;
+  MNRF_CHECK(smooth || !z, "mnrf_head_bwd: z is the pre-activation of a smooth activation, act %d is not one", act);
+  MNRF_CHECK(!smooth || (z && dx && ldz % 8 == 0 && ((uintptr_t)z % 16) == 0),
+             "mnrf_head_bwd: a smooth activation needs dx and a 16-byte aligned z with a pitch that is a multiple of 8");
+  // the kernels take the ReLU mask as a flag of its own and `act` for the smooth derivative only
+  const int32_t relu_mask = act == MNRF_ACT_RELU;
+  if (!smooth) act = MNRF_ACT_NONE;
   if (m == 0) return 0;
   if ((k == 256 || k == 128 || k == 64) && ((uintptr_t)w % 16) == 0) {
     // rows of one / half / a quarter of a warp's 16-byte chunks (see head_bwd_sub_kernel)
@@ -590,28 +580,6 @@ static int head_bwd_impl(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x
   return 0;
 }
 
-extern "C" int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx,
-                             const mnrf_bf16* w, const float* draw, mnrf_bf16* dx, int64_t lddx,
-                             int32_t relu_mask, float* dw, float* dw2, int32_t dw_split, float* db, float* dxsum,
-                             int32_t dx_cols, mnrf_bf16* dx2, int64_t lddx2, mnrf_stream stream) {
-  return head_bwd_impl(m, k, n_out, x, ldx, w, draw, dx, lddx, relu_mask, MNRF_ACT_NONE, nullptr, 0, dw, dw2, dw_split,
-                       db, dxsum, dx_cols, dx2, lddx2, stream);
-}
-
-extern "C" int mnrf_head_bwd_act(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx,
-                                 const mnrf_bf16* w, const float* draw, mnrf_bf16* dx, int64_t lddx,
-                                 int32_t act, const mnrf_bf16* z, int64_t ldz, float* dw, float* dw2, int32_t dw_split,
-                                 float* db, float* dxsum, int32_t dx_cols, mnrf_bf16* dx2, int64_t lddx2,
-                                 mnrf_stream stream) {
-  using namespace mnrf;
-  MNRF_CHECK(act == MNRF_ACT_SOFTPLUS || act == MNRF_ACT_SILU, "mnrf_head_bwd_act: act %d is not a smooth activation",
-             act);
-  MNRF_CHECK(z && dx && ldz % 8 == 0 && ((uintptr_t)z % 16) == 0,
-             "mnrf_head_bwd_act: needs dx and a 16-byte aligned z with a pitch that is a multiple of 8");
-  return head_bwd_impl(m, k, n_out, x, ldx, w, draw, dx, lddx, 0, act, z, ldz, dw, dw2, dw_split, db, dxsum, dx_cols,
-                       dx2, lddx2, stream);
-}
-
 extern "C" int mnrf_colsum(int64_t m, int32_t n, const mnrf_bf16* x, int64_t ldx, float* out,
                            mnrf_stream stream) {
   using namespace mnrf;
@@ -632,17 +600,6 @@ extern "C" int mnrf_colsum(int64_t m, int32_t n, const mnrf_bf16* x, int64_t ldx
   return 0;
 }
 
-extern "C" int mnrf_pack_weights(int32_t in_pad, int32_t out, const float* master, mnrf_bf16* w_nk,
-                                 mnrf_bf16* w_kn, mnrf_stream stream) {
-  using namespace mnrf;
-  MNRF_CHECK(master, "mnrf_pack_weights: null pointer");
-  dim3 grid((out + 31) / 32, (in_pad + 31) / 32), block(32, 8);
-  pack_weights_kernel<<<grid, block, 0, (cudaStream_t)stream>>>(
-      in_pad, out, master, reinterpret_cast<__nv_bfloat16*>(w_nk), reinterpret_cast<__nv_bfloat16*>(w_kn));
-  MNRF_LAUNCH_CHECK();
-  return 0;
-}
-
 extern "C" int mnrf_pack_weights_batched(int32_t count, const mnrf_pack_item* items, int32_t total_tiles,
                                          mnrf_stream stream) {
   using namespace mnrf;
@@ -653,8 +610,8 @@ extern "C" int mnrf_pack_weights_batched(int32_t count, const mnrf_pack_item* it
   return 0;
 }
 
-static int clip_adam_impl(const mnrf_adam_desc* d, float* params, const float* grads, float* mu,
-                          float* nu, float* norm_sq_scratch, const float* dyn, mnrf_stream stream) {
+extern "C" int mnrf_clip_adam(const mnrf_adam_desc* d, float* params, const float* grads, float* mu,
+                              float* nu, float* norm_sq_scratch, const float* dyn, mnrf_stream stream) {
   using namespace mnrf;
   MNRF_CHECK(d && params && grads && mu && nu && norm_sq_scratch, "mnrf_clip_adam: null pointer");
   MNRF_CHECK(d->step >= 1, "mnrf_clip_adam: step is the 1-based update count");
@@ -669,15 +626,4 @@ static int clip_adam_impl(const mnrf_adam_desc* d, float* params, const float* g
   clip_adam_kernel<<<blocks, 256, 0, s>>>(*d, params, grads, mu, nu, norm_sq_scratch, dyn);
   MNRF_LAUNCH_CHECK();
   return 0;
-}
-
-extern "C" int mnrf_clip_adam(const mnrf_adam_desc* d, float* params, const float* grads, float* mu,
-                              float* nu, float* norm_sq_scratch, mnrf_stream stream) {
-  return clip_adam_impl(d, params, grads, mu, nu, norm_sq_scratch, nullptr, stream);
-}
-
-extern "C" int mnrf_clip_adam_dyn(const mnrf_adam_desc* d, float* params, const float* grads, float* mu,
-                                  float* nu, float* norm_sq_scratch, const float* dyn, mnrf_stream stream) {
-  MNRF_CHECK(dyn, "mnrf_clip_adam_dyn: null dyn");
-  return clip_adam_impl(d, params, grads, mu, nu, norm_sq_scratch, dyn, stream);
 }

@@ -185,10 +185,9 @@ quantile_kernel(int n, float q, const float* __restrict__ x, float* __restrict__
 
 }  // namespace mnrf
 
-// mnrf_robust_mask and mnrf_robust_mask_chunk share this body; the mask means divide by batch_rays.
-static int robust_mask_launch(const mnrf_robust_desc* d, const float* rgb, const float* target,
-                              const float* threshold, float* mask, float* error_per_pixel, uint32_t* counts,
-                              float* stats, int32_t batch_rays, mnrf_stream stream) {
+extern "C" int mnrf_robust_mask(const mnrf_robust_desc* d, const float* rgb, const float* target,
+                                const float* threshold, float* mask, float* error_per_pixel, uint32_t* counts,
+                                float* stats, int32_t batch_rays, mnrf_stream stream) {
   using namespace mnrf;
   MNRF_CHECK(d && rgb && target && threshold && mask && error_per_pixel, "mnrf_robust_mask: null pointer");
   MNRF_CHECK(!stats || counts, "mnrf_robust_mask: stats need the counts workspace");
@@ -203,7 +202,7 @@ static int robust_mask_launch(const mnrf_robust_desc* d, const float* rgb, const
     MNRF_CHECK(d->filter_size >= 1 && d->filter_size % 2 == 1 && d->filter_size <= p,
                "mnrf_robust_mask: filter_size %d must be odd and <= patch_size %d", d->filter_size, p);
   }
-  MNRF_CHECK(batch_rays >= d->num_rays, "mnrf_robust_mask_chunk: batch_rays %d < num_rays %d", batch_rays,
+  MNRF_CHECK(batch_rays >= d->num_rays, "mnrf_robust_mask: batch_rays %d < num_rays %d", batch_rays,
              d->num_rays);
   if (d->num_rays == 0) return 0;
   const int threads = (p * p + 31) / 32 * 32;
@@ -211,19 +210,6 @@ static int robust_mask_launch(const mnrf_robust_desc* d, const float* rgb, const
       *d, rgb, target, threshold, mask, error_per_pixel, counts, stats, batch_rays);
   MNRF_LAUNCH_CHECK();
   return 0;
-}
-
-extern "C" int mnrf_robust_mask(const mnrf_robust_desc* d, const float* rgb, const float* target,
-                                const float* threshold, float* mask, float* error_per_pixel, uint32_t* counts,
-                                float* stats, mnrf_stream stream) {
-  return robust_mask_launch(d, rgb, target, threshold, mask, error_per_pixel, counts, stats, d ? d->num_rays : 0,
-                            stream);
-}
-
-extern "C" int mnrf_robust_mask_chunk(const mnrf_robust_desc* d, const float* rgb, const float* target,
-                                      const float* threshold, float* mask, float* error_per_pixel, uint32_t* counts,
-                                      float* stats, int32_t batch_rays, mnrf_stream stream) {
-  return robust_mask_launch(d, rgb, target, threshold, mask, error_per_pixel, counts, stats, batch_rays, stream);
 }
 
 extern "C" int mnrf_quantile(int32_t n, float q, const float* x, float* out, mnrf_stream stream) {

@@ -207,11 +207,11 @@ sample_level_kernel(mnrf_sample_desc d, const float* __restrict__ sdist_prev,
 
 }  // namespace mnrf
 
-static int sample_level_impl(const mnrf_sample_desc* d, const float* sdist_prev,
-                             const float* w_prev, const float* u_base, const float* jitter,
-                             const float* cw_in, float* sdist_out, int32_t* idx_out,
-                             float* cw_out, float* tdil_out, float* wdil_out,
-                             const float* anneal_dev, mnrf_stream stream) {
+extern "C" int mnrf_sample_level(const mnrf_sample_desc* d, const float* sdist_prev,
+                                 const float* w_prev, const float* u_base, const float* jitter,
+                                 const float* anneal_dev, const float* cw_in, float* sdist_out,
+                                 int32_t* idx_out, float* cw_out, float* tdil_out, float* wdil_out,
+                                 mnrf_stream stream) {
   using namespace mnrf;
   if (d && d->num_rays == 0) return 0;
   MNRF_CHECK(d && sdist_prev && w_prev && u_base && sdist_out, "mnrf_sample_level: null pointer");
@@ -238,20 +238,4 @@ static int sample_level_impl(const mnrf_sample_desc* d, const float* sdist_prev,
       anneal_dev);
   MNRF_LAUNCH_CHECK();
   return 0;
-}
-
-extern "C" int mnrf_sample_level(const mnrf_sample_desc* d, const float* sdist_prev,
-                                 const float* w_prev, const float* u_base, const float* jitter,
-                                 const float* cw_in, float* sdist_out, int32_t* idx_out,
-                                 float* cw_out, float* tdil_out, float* wdil_out,
-                                 mnrf_stream stream) {
-  return sample_level_impl(d, sdist_prev, w_prev, u_base, jitter, cw_in, sdist_out, idx_out, cw_out,
-                           tdil_out, wdil_out, nullptr, stream);
-}
-
-extern "C" int mnrf_sample_level_dyn(const mnrf_sample_desc* d, const float* sdist_prev,
-                                     const float* w_prev, const float* u_base, const float* jitter,
-                                     const float* anneal_dev, float* sdist_out, mnrf_stream stream) {
-  return sample_level_impl(d, sdist_prev, w_prev, u_base, jitter, nullptr, sdist_out, nullptr, nullptr,
-                           nullptr, nullptr, anneal_dev, stream);
 }

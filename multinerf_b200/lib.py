@@ -131,33 +131,24 @@ _SIGNATURES = {
     'mnrf_last_error': (C.c_char_p, []),
     'mnrf_device_ok': (C.c_int, []),
     'mnrf_num_sms': (C.c_int, []),
-    'mnrf_sample_level': (C.c_int, [C.POINTER(SampleDesc)] + [_P] * 11),
-    'mnrf_sample_level_dyn': (C.c_int, [C.POINTER(SampleDesc)] + [_P] * 7),
-    'mnrf_encode': (C.c_int, [C.POINTER(EncodeDesc)] + [_P] * 11),
+    'mnrf_sample_level': (C.c_int, [C.POINTER(SampleDesc)] + [_P] * 12),
+    'mnrf_encode': (C.c_int, [C.POINTER(EncodeDesc)] + [_P] * 11 + [C.c_int32, _P]),
     'mnrf_viewdir_enc': (C.c_int, [C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_int32, C.c_int32,
                                    C.c_int32, _P]),
-    'mnrf_gemm': (C.c_int, [C.POINTER(GemmDesc)] + [_P] * 11),
-    'mnrf_gemm_act': (C.c_int, [C.POINTER(GemmDesc)] + [_P] * 8 + [C.c_int64, _P, _P]),
+    'mnrf_gemm': (C.c_int, [C.POINTER(GemmDesc)] + [_P] * 10 + [C.c_int64, _P, _P]),
     'mnrf_gemm_wgrad': (C.c_int, [C.POINTER(GemmDesc)] + [_P] * 7),
     'mnrf_gemm_plan': (C.c_int, [C.POINTER(GemmDesc)] + [_P] * 10 + [C.c_int64] + [_P] * 4 +
                        [C.POINTER(GemmInstance)]),
     'mnrf_mlp_chain': (C.c_int, [C.POINTER(ChainDesc), _P]),
     'mnrf_mlp_chain_max_layers': (C.c_int, []),
     'mnrf_head_fwd': (C.c_int, [C.c_int64, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P, _P, _P]),
-    'mnrf_head_bwd': (C.c_int, [C.c_int64, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P, _P,
-                                C.c_int64, C.c_int32, _P, _P, C.c_int32, _P, _P, C.c_int32, _P, C.c_int64, _P]),
-    'mnrf_head_bwd_act': (C.c_int, [C.c_int64, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P, _P, C.c_int64,
-                                    C.c_int32, _P, C.c_int64, _P, _P, C.c_int32, _P, _P, C.c_int32, _P, C.c_int64,
-                                    _P]),
+    'mnrf_head_bwd': (C.c_int, [C.c_int64, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P, _P, C.c_int64, C.c_int32,
+                                _P, C.c_int64, _P, _P, C.c_int32, _P, _P, C.c_int32, _P, C.c_int64, _P]),
     'mnrf_colsum': (C.c_int, [C.c_int64, C.c_int32, _P, C.c_int64, _P, _P]),
     'mnrf_composite_fwd': (C.c_int, [C.POINTER(CompositeDesc)] + [_P] * 18),
-    'mnrf_composite_bwd': (C.c_int, [C.POINTER(LossDesc)] + [_P] * 24),
-    'mnrf_composite_bwd_masked': (C.c_int, [C.POINTER(LossDesc)] + [_P] * 25),
-    'mnrf_composite_bwd_chunk': (C.c_int, [C.POINTER(LossDesc)] + [_P] * 24 + [C.c_int32, _P]),
-    'mnrf_robust_mask': (C.c_int, [C.POINTER(RobustDesc)] + [_P] * 8),
-    'mnrf_robust_mask_chunk': (C.c_int, [C.POINTER(RobustDesc)] + [_P] * 7 + [C.c_int32, _P]),
+    'mnrf_composite_bwd': (C.c_int, [C.POINTER(LossDesc)] + [_P] * 24 + [C.c_int32, _P]),
+    'mnrf_robust_mask': (C.c_int, [C.POINTER(RobustDesc)] + [_P] * 7 + [C.c_int32, _P]),
     'mnrf_quantile': (C.c_int, [C.c_int32, C.c_float, _P, _P, _P]),
-    'mnrf_encode_tangent': (C.c_int, [C.POINTER(EncodeDesc)] + [_P] * 9 + [C.c_int32, _P]),
     'mnrf_refdir_fwd': (C.c_int, [C.POINTER(RefdirDesc)] + [_P] * 10 + [C.c_float, C.c_float, C.c_int32, _P, _P]),
     'mnrf_refdir_bwd': (C.c_int, [C.POINTER(RefdirDesc)] + [_P] * 8 + [C.c_int32, C.c_float, C.c_float, C.c_int32] +
                         [_P] * 8),
@@ -169,9 +160,7 @@ _SIGNATURES = {
     'mnrf_act_tangent_bwd': (C.c_int, [C.c_int64, C.c_int32, C.c_int32] + [_P, C.c_int64] * 5 + [C.c_int32, _P]),
     'mnrf_pixels_to_rays': (C.c_int, [C.POINTER(CameraDesc)] + [_P] * 11),
     'mnrf_spherical_rays': (C.c_int, [C.POINTER(SphericalDesc)] + [_P] * 6),
-    'mnrf_clip_adam': (C.c_int, [C.POINTER(AdamDesc)] + [_P] * 6),
-    'mnrf_clip_adam_dyn': (C.c_int, [C.POINTER(AdamDesc)] + [_P] * 7),
-    'mnrf_pack_weights': (C.c_int, [C.c_int32, C.c_int32, _P, _P, _P, _P]),
+    'mnrf_clip_adam': (C.c_int, [C.POINTER(AdamDesc)] + [_P] * 7),
     'mnrf_pack_weights_batched': (C.c_int, [C.c_int32, _P, C.c_int32, _P]),
 }
 EXPORTED = tuple(_SIGNATURES)
@@ -196,7 +185,7 @@ def load(build_if_missing=False):
     fn = getattr(lib, name)          # AttributeError if the .so lacks a declared symbol
     fn.restype = res
     fn.argtypes = args
-  if lib.mnrf_abi_version() != 1:
+  if lib.mnrf_abi_version() != 2:
     raise MnrfError('ABI version mismatch')
   _lib = lib
   return lib

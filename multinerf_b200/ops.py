@@ -24,6 +24,20 @@ def _count(n=1):
   LAUNCHES += n
 
 
+def _gemm_call(flops, fn, *args):
+  """One counted GEMM launch fn(*args); with GEMM_EVENTS a list, it runs between two CUDA events appended there
+  with its `flops`."""
+  _count()
+  if GEMM_EVENTS is None:
+    L.check(fn(*args))
+    return
+  ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+  ev[0].record()
+  L.check(fn(*args))
+  ev[1].record()
+  GEMM_EVENTS.append((ev[0], ev[1], flops))
+
+
 def _f32(t):
   assert t is None or (t.dtype == torch.float32 and t.is_contiguous()), 'need contiguous fp32'
   return t
@@ -79,14 +93,8 @@ def sample_level(sdist_prev, w_prev, num_samples, *, dilation=0.0, use_dilation=
   tdil = torch.empty(B, nb + 1, device=dev) if want_debug else None
   wdil = torch.empty(B, nb, device=dev) if want_debug else None
   _count()
-  if anneal_dev is not None:
-    assert cw_in is None and not want_index and not want_debug
-    L.check(lib.mnrf_sample_level_dyn(C.byref(d), L.ptr(_f32(sdist_prev)), L.ptr(_f32(w_prev)),
-                                      L.ptr(_f32(u_base)), L.ptr(_f32(jitter)), L.ptr(anneal_dev),
-                                      L.ptr(sdist), L.stream_ptr()))
-    return sdist
   L.check(lib.mnrf_sample_level(C.byref(d), L.ptr(_f32(sdist_prev)), L.ptr(_f32(w_prev)),
-                                L.ptr(_f32(u_base)), L.ptr(_f32(jitter)), L.ptr(_f32(cw_in)),
+                                L.ptr(_f32(u_base)), L.ptr(_f32(jitter)), L.ptr(anneal_dev), L.ptr(_f32(cw_in)),
                                 L.ptr(sdist), L.ptr(idx), L.ptr(cw), L.ptr(tdil), L.ptr(wdil),
                                 L.stream_ptr()))
   if want_index or want_debug:
@@ -115,18 +123,13 @@ def encode(sdist, origins, directions, radii, near, far, basis, *, min_deg, max_
                    int(disable_integration), K, min_deg, max_deg, ld, feat_cols)
   f32 = torch.empty(B * S, F, device=sdist.device) if want_f32 else None
   tdist = torch.empty(B, S + 1, device=sdist.device) if want_tdist else None
-  _count()
   if tfeat is not None:
-    assert tfeat.dtype == torch.bfloat16 and tfeat.stride(1) == 1 and not want_f32 and not want_tdist
-    L.check(lib.mnrf_encode_tangent(C.byref(d), L.ptr(_f32(sdist)), L.ptr(_f32(origins)),
-                                    L.ptr(_f32(directions)), L.ptr(_f32(radii)), L.ptr(_f32(near)),
-                                    L.ptr(_f32(far)), L.ptr(_f32(basis)), L.ptr(feat), L.ptr(tfeat),
-                                    tfeat.stride(0), L.stream_ptr()))
-    return feat, None, None
+    assert tfeat.dtype == torch.bfloat16 and tfeat.stride(1) == 1
+  _count()
   L.check(lib.mnrf_encode(C.byref(d), L.ptr(_f32(sdist)), L.ptr(_f32(origins)),
                           L.ptr(_f32(directions)), L.ptr(_f32(radii)), L.ptr(_f32(near)),
                           L.ptr(_f32(far)), L.ptr(_f32(basis)), L.ptr(feat), L.ptr(f32),
-                          L.ptr(tdist), L.stream_ptr()))
+                          L.ptr(tdist), L.ptr(tfeat), tfeat.stride(0) if tfeat is not None else 0, L.stream_ptr()))
   return feat, f32, tdist
 
 
@@ -140,34 +143,21 @@ def viewdir_enc(viewdirs, num_samples, deg, out, col0, col_end):
 
 def gemm(mode, a, b, out, *, m, n, k, act=L.ACT_NONE, bias=None, rowv=None, colv=None, mask=None,
          maskbits=None, colsum=None, mask_mod=0, addend=None, z=None, impl=0):
-  """Dense-layer GEMM (see include/mnrf.h).  a/b/out/mask/z are 2-D views with unit inner stride.  A smooth `act`
-  (L.SMOOTH_ACTS) runs mnrf_gemm_act: FWD writes the pre-activation to z (optional), DGRAD multiplies by a'(z)."""
+  """Dense-layer GEMM (see include/mnrf.h).  a/b/out/mask/z are 2-D views with unit inner stride.  With a smooth
+  `act` (L.SMOOTH_ACTS), FWD writes the pre-activation to z (optional) and DGRAD multiplies by a'(z)."""
   lib = L.load()
   for t in (a, b, out) + tuple(t for t in (mask, z) if t is not None):
     assert t.stride(-1) == 1
   if maskbits is not None:
     assert maskbits.dtype == torch.int32 and maskbits.stride(-1) == 1
+  assert z is None or z.dtype == torch.bfloat16
   d = L.GemmDesc(mode, act, m, n, k, a.stride(0), b.stride(0), out.stride(0),
                  mask.stride(0) if mask is not None else 0,
                  maskbits.stride(0) if maskbits is not None else 0,
                  addend.stride(0) if addend is not None else 0, mask_mod, impl)
-  _count()
-  ev = None
-  if GEMM_EVENTS is not None:
-    ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
-    ev[0].record()
-  if act in L.SMOOTH_ACTS and mode != L.GEMM_WGRAD:
-    assert mask is None and maskbits is None and (z is None or z.dtype == torch.bfloat16)
-    L.check(lib.mnrf_gemm_act(C.byref(d), L.ptr(a), L.ptr(b), L.ptr(bias), L.ptr(rowv), L.ptr(colv), L.ptr(colsum),
-                              L.ptr(addend), L.ptr(z), z.stride(0) if z is not None else 0, L.ptr(out),
-                              L.stream_ptr()))
-  else:
-    assert z is None, 'z is the pre-activation of a smooth activation'
-    L.check(lib.mnrf_gemm(C.byref(d), L.ptr(a), L.ptr(b), L.ptr(bias), L.ptr(rowv), L.ptr(colv),
-                          L.ptr(mask), L.ptr(maskbits), L.ptr(colsum), L.ptr(addend), L.ptr(out), L.stream_ptr()))
-  if ev is not None:
-    ev[1].record()
-    GEMM_EVENTS.append((ev[0], ev[1], 2.0 * m * n * k))
+  _gemm_call(2.0 * m * n * k, lib.mnrf_gemm, C.byref(d), L.ptr(a), L.ptr(b), L.ptr(bias), L.ptr(rowv), L.ptr(colv),
+             L.ptr(mask), L.ptr(maskbits), L.ptr(colsum), L.ptr(addend), L.ptr(z), z.stride(0) if z is not None else 0,
+             L.ptr(out), L.stream_ptr())
   return out
 
 
@@ -181,17 +171,8 @@ def gemm_wgrad(x, dy, out, *, m, n, k, bsum=None, side_w=None, side_aw=None, imp
   assert x.stride(-1) == 1 and dy.stride(-1) == 1 and out.stride(-1) == 1
   assert (side_w is None) == (side_aw is None)
   d = L.GemmDesc(L.GEMM_WGRAD, L.ACT_NONE, m, n, k, x.stride(0), dy.stride(0), out.stride(0), 0, 0, 0, 0, impl)
-  _count()
-  ev = None
-  if GEMM_EVENTS is not None:
-    ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
-    ev[0].record()
-  L.check(lib.mnrf_gemm_wgrad(C.byref(d), L.ptr(x), L.ptr(dy), L.ptr(bsum),
-                              L.ptr(_f32(side_w)), L.ptr(side_aw), L.ptr(out),
-                              L.stream_ptr()))
-  if ev is not None:
-    ev[1].record()
-    GEMM_EVENTS.append((ev[0], ev[1], 2.0 * m * n * k))
+  _gemm_call(2.0 * m * n * k, lib.mnrf_gemm_wgrad, C.byref(d), L.ptr(x), L.ptr(dy), L.ptr(bsum),
+             L.ptr(_f32(side_w)), L.ptr(side_aw), L.ptr(out), L.stream_ptr())
   return out
 
 
@@ -254,15 +235,7 @@ def mlp_chain(desc):
   """One launch for a whole 256-wide trunk (forward) or its input-gradient chain (backward)."""
   lib = L.load()
   d, flops = desc
-  _count()
-  ev = None
-  if GEMM_EVENTS is not None:
-    ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
-    ev[0].record()
-  L.check(lib.mnrf_mlp_chain(C.byref(d), L.stream_ptr()))
-  if ev is not None:
-    ev[1].record()
-    GEMM_EVENTS.append((ev[0], ev[1], flops))
+  _gemm_call(flops, lib.mnrf_mlp_chain, C.byref(d), L.stream_ptr())
 
 
 def head_fwd(x, w_nk, bias, n_out, k, raw=None):
@@ -280,21 +253,20 @@ def head_bwd(x, w_nk, draw, n_out, k, dx=None, relu_mask=False, dw=None, db=None
              dx_cols=0, dx2=None, act=L.ACT_NONE, z=None):
   """dw2 / dw_split: outputs [dw_split, n_out) put their weight gradient in dw2; dx_cols: dx and dxsum cover the
   first dx_cols columns only; dx2 [M, k - dx_cols]: the input gradient of the columns past dx_cols, unmasked
-  (include/mnrf.h).  z (with a smooth `act`, instead of relu_mask): dx *= a'(z), z the pre-activation of x."""
+  (include/mnrf.h).  relu_mask: dx is masked by x > 0; z (with a smooth `act`, instead of relu_mask): dx *= a'(z), z
+  the pre-activation of x."""
   lib = L.load()
   M = x.shape[0]
-  _count()
   if z is not None:
     assert not relu_mask and z.dtype == torch.bfloat16 and z.stride(-1) == 1
-    L.check(lib.mnrf_head_bwd_act(M, k, n_out, L.ptr(x), x.stride(0), L.ptr(w_nk), L.ptr(_f32(draw)), L.ptr(dx),
-                                  dx.stride(0), act, L.ptr(z), z.stride(0), L.ptr(dw), L.ptr(dw2), int(dw_split),
-                                  L.ptr(db), L.ptr(dxsum), int(dx_cols), L.ptr(dx2),
-                                  dx2.stride(0) if dx2 is not None else 0, L.stream_ptr()))
-    return
+  else:
+    act = L.ACT_RELU if relu_mask else L.ACT_NONE
+  _count()
   L.check(lib.mnrf_head_bwd(M, k, n_out, L.ptr(x), x.stride(0), L.ptr(w_nk), L.ptr(_f32(draw)),
-                            L.ptr(dx), dx.stride(0) if dx is not None else 0, int(relu_mask),
-                            L.ptr(dw), L.ptr(dw2), int(dw_split), L.ptr(db), L.ptr(dxsum), int(dx_cols),
-                            L.ptr(dx2), dx2.stride(0) if dx2 is not None else 0, L.stream_ptr()))
+                            L.ptr(dx), dx.stride(0) if dx is not None else 0, act,
+                            L.ptr(z), z.stride(0) if z is not None else 0, L.ptr(dw), L.ptr(dw2), int(dw_split),
+                            L.ptr(db), L.ptr(dxsum), int(dx_cols), L.ptr(dx2), dx2.stride(0) if dx2 is not None else 0,
+                            L.stream_ptr()))
 
 
 def colsum(x, n, out):
@@ -344,8 +316,8 @@ def composite_bwd(raw_density, raw_rgb, sdist, directions, near, far, target_rgb
                   raw_diffuse=None, raw_tint=None, extra_dw=None, d_raw_diffuse=None, d_raw_tint=None,
                   data_mask=None, batch_rays=None):
   """Losses + compositing backward of one level; `data_mask` [B] (optional) weights each ray's data loss
-  (robustnerf) through mnrf_composite_bwd_masked.  `batch_rays`: these B rays are one pass of a step over that
-  many rays, which the distortion and interlevel means divide by (mnrf_composite_bwd_chunk)."""
+  (robustnerf).  `batch_rays`: these B rays are one pass of a step over that many rays, which the distortion and
+  interlevel means divide by (default B)."""
   lib = L.load()
   B, S = raw_density.shape
   dev = raw_density.device
@@ -360,22 +332,16 @@ def composite_bwd(raw_density, raw_rgb, sdist, directions, near, far, target_rgb
   # the gradients share the raw values' sample spacing (one pair of strides in the descriptor)
   d.c.ld_density, d.c.ld_rgb = _sample_ld(raw_density, 0), _sample_ld(raw_rgb, 3)
   assert _sample_ld(d_raw_density, 0) == d.c.ld_density and (raw_rgb is None or _sample_ld(d_raw_rgb, 3) == d.c.ld_rgb)
-  _count()
-  head = (C.byref(d), L.ptr(raw_density), L.ptr(raw_rgb), L.ptr(_f32(density_noise)),
-          L.ptr(_f32(sdist)), L.ptr(_f32(directions)), L.ptr(_f32(near)), L.ptr(_f32(far)), L.ptr(_f32(bg_rgb)),
-          L.ptr(_f32(rgb_scale)), L.ptr(_f32(raw_diffuse)), L.ptr(_f32(raw_tint)), L.ptr(_f32(extra_dw)),
-          L.ptr(_f32(target_rgb)), L.ptr(_f32(lossmult)), L.ptr(_f32(inv_denom)), L.ptr(_f32(sdist_fine)),
-          L.ptr(_f32(weights_fine)))
-  tail = (L.ptr(d_raw_density), L.ptr(d_raw_rgb), L.ptr(d_rgb_scale), L.ptr(d_raw_diffuse), L.ptr(d_raw_tint),
-          L.ptr(stats), L.stream_ptr())
   if data_mask is not None:
     assert data_mask.numel() == B
-  if batch_rays is not None:
-    L.check(lib.mnrf_composite_bwd_chunk(*head, L.ptr(_f32(data_mask)), *tail[:-1], int(batch_rays), tail[-1]))
-  elif data_mask is not None:
-    L.check(lib.mnrf_composite_bwd_masked(*head, L.ptr(_f32(data_mask)), *tail))
-  else:
-    L.check(lib.mnrf_composite_bwd(*head, *tail))
+  _count()
+  L.check(lib.mnrf_composite_bwd(
+      C.byref(d), L.ptr(raw_density), L.ptr(raw_rgb), L.ptr(_f32(density_noise)), L.ptr(_f32(sdist)),
+      L.ptr(_f32(directions)), L.ptr(_f32(near)), L.ptr(_f32(far)), L.ptr(_f32(bg_rgb)), L.ptr(_f32(rgb_scale)),
+      L.ptr(_f32(raw_diffuse)), L.ptr(_f32(raw_tint)), L.ptr(_f32(extra_dw)), L.ptr(_f32(target_rgb)),
+      L.ptr(_f32(lossmult)), L.ptr(_f32(inv_denom)), L.ptr(_f32(sdist_fine)), L.ptr(_f32(weights_fine)),
+      L.ptr(_f32(data_mask)), L.ptr(d_raw_density), L.ptr(d_raw_rgb), L.ptr(d_rgb_scale), L.ptr(d_raw_diffuse),
+      L.ptr(d_raw_tint), L.ptr(stats), int(B if batch_rays is None else batch_rays), L.stream_ptr()))
   return d_raw_density, d_raw_rgb
 
 
@@ -390,7 +356,7 @@ def robust_mask(rgb, target, threshold, desc, *, mask=None, error=None, counts=N
   """robustnerf.robustnerf_mask for patch-major rays: returns (mask [B], error_per_pixel [B]).
   `threshold` is a device scalar; with `stats` (a row of >= 5 floats), stats[1:5] += the per-rank means of
   is_inlier_loss, has_inlier_neighbors, is_inlier_patch and mask, using `counts` (int32[5], zero, left zero).
-  `batch_rays`: these B rays are one pass of a step over that many rays, and the means divide by it."""
+  `batch_rays`: these B rays are one pass of a step over that many rays, and the means divide by it (default B)."""
   lib = L.load()
   B = rgb.shape[0]
   assert desc.num_rays == B and rgb.shape == (B, 3) and target.shape == (B, 3) and threshold.numel() == 1
@@ -402,12 +368,9 @@ def robust_mask(rgb, target, threshold, desc, *, mask=None, error=None, counts=N
     assert counts is not None and counts.dtype == torch.int32 and counts.numel() >= 5
     assert stats.is_contiguous() and stats.numel() >= 5
   _count()
-  args = (C.byref(desc), L.ptr(_f32(rgb)), L.ptr(_f32(target)), L.ptr(_f32(threshold)), L.ptr(mask), L.ptr(error),
-          L.ptr(counts), L.ptr(stats))
-  if batch_rays is not None:
-    L.check(lib.mnrf_robust_mask_chunk(*args, int(batch_rays), L.stream_ptr()))
-  else:
-    L.check(lib.mnrf_robust_mask(*args, L.stream_ptr()))
+  L.check(lib.mnrf_robust_mask(C.byref(desc), L.ptr(_f32(rgb)), L.ptr(_f32(target)), L.ptr(_f32(threshold)),
+                               L.ptr(mask), L.ptr(error), L.ptr(counts), L.ptr(stats),
+                               int(B if batch_rays is None else batch_rays), L.stream_ptr()))
   return mask, error
 
 
@@ -428,20 +391,8 @@ def clip_adam(params, grads, mu, nu, scratch, *, step, lr, beta1, beta2, eps, gr
   d = L.AdamDesc(params.numel(), float(grad_max_val), float(grad_max_norm), float(lr), float(beta1),
                  float(beta2), float(eps), int(step), float(grad_scale))
   _count(2 if grad_max_norm > 0 else 1)
-  if dyn is not None:
-    L.check(lib.mnrf_clip_adam_dyn(C.byref(d), L.ptr(params), L.ptr(grads), L.ptr(mu), L.ptr(nu),
-                                   L.ptr(scratch), L.ptr(dyn), L.stream_ptr()))
-    return
   L.check(lib.mnrf_clip_adam(C.byref(d), L.ptr(params), L.ptr(grads), L.ptr(mu), L.ptr(nu),
-                             L.ptr(scratch), L.stream_ptr()))
-
-
-def pack_weights(master, w_nk, w_kn):
-  lib = L.load()
-  in_pad, out = master.shape
-  _count()
-  L.check(lib.mnrf_pack_weights(in_pad, out, L.ptr(master), L.ptr(w_nk), L.ptr(w_kn),
-                                L.stream_ptr()))
+                             L.ptr(scratch), L.ptr(dyn), L.stream_ptr()))
 
 
 def pack_table(layers, device):

@@ -1,4 +1,4 @@
-"""fp64 reference of the Dense-layer GEMM (mnrf_gemm / mnrf_gemm_act / mnrf_gemm_wgrad) with a per-element bound.
+"""fp64 reference of the Dense-layer GEMM (mnrf_gemm / mnrf_gemm_wgrad) with a per-element bound.
 
 `ref_fwd / ref_dgrad / ref_wgrad` take exactly the operands the kernel gets (bf16 A / B, fp32 bias, rowv, colv, bf16
 mask or packed mask bits, addend, z) and return the fp64 value of every output together with a bound on how far a

@@ -2,9 +2,11 @@
 table for every activation, the config errors that name their field, and the C entry points of the smooth
 activations."""
 import os
+import re
 
 import pytest
 
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ALL = ('relu', 'softplus', 'silu')     # what models.Model builds its plans for
 
 
@@ -49,12 +51,19 @@ def test_unsupported_activation_names_its_field(text, field):
     MLPPlan(b.nerf_mlp, activations=ALL)
 
 
-def test_smooth_activation_entry_points_are_exported():
+def test_smooth_activations_run_through_the_base_entry_points():
   from multinerf_b200 import lib
   if not os.path.exists(lib.LIB_PATH):
     from multinerf_b200 import build
     build.build()
   l = lib.load()
-  for name in ('mnrf_gemm_act', 'mnrf_head_bwd_act', 'mnrf_act_tangent_bwd'):
+  for name in ('mnrf_gemm', 'mnrf_head_bwd', 'mnrf_act_tangent_bwd'):
     assert name in lib.EXPORTED and hasattr(l, name)
+  # the smooth activations run through the base entries, which take the pre-activation z and its pitch
+  header = open(os.path.join(ROOT, 'include', 'mnrf.h')).read()
+  for name in ('mnrf_gemm', 'mnrf_head_bwd'):
+    decl = re.search(r'\b' + name + r'\(([^;]*)\);', header)
+    assert decl and 'mnrf_bf16* z' in decl.group(1) and 'int64_t ldz' in decl.group(1), name
+  for name in ('mnrf_gemm_act', 'mnrf_head_bwd_act'):
+    assert name not in lib.EXPORTED and not hasattr(l, name)
   assert (lib.ACT_NONE, lib.ACT_RELU, lib.ACT_SOFTPLUS, lib.ACT_SILU) == (0, 1, 2, 3)

@@ -1,4 +1,4 @@
-"""Compositing and loss kernels (mnrf_composite_fwd, mnrf_composite_bwd[_masked]) against an fp64 reference.
+"""Compositing and loss kernels (mnrf_composite_fwd, mnrf_composite_bwd) against an fp64 reference.
 
 The reference (tests/composite_ref.py) is the oracle evaluated on the kernels' own fp32 inputs promoted to float64
 and differentiated by torch.autograd.  Tolerance: per ray, the kernel's largest error against fp64 may be at most 4x

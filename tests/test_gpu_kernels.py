@@ -356,15 +356,18 @@ def test_heads_and_colsum(ops):
   close(out, x.float().sum(0), atol=2e-2, rtol=1e-4, msg='colsum')
 
 
-def test_pack_weights_and_adam(ops):
+def test_pack_weights_batched_and_adam(ops):
   from oracle import o_train
   rng = np.random.default_rng(9)
   master = torch.tensor(rng.normal(size=(320, 128)).astype(np.float32))
   w_nk = torch.empty(128, 320, dtype=torch.bfloat16, device='cuda')
   w_kn = torch.empty(320, 128, dtype=torch.bfloat16, device='cuda')
-  ops.pack_weights(master.cuda(), w_nk, w_kn)
+  ops.pack_weights_batched(ops.pack_table([(master.cuda(), w_nk, w_kn)], 'cuda'))      # one layer
   assert torch.equal(w_kn.cpu(), master.to(torch.bfloat16))
   assert torch.equal(w_nk.cpu(), master.T.contiguous().to(torch.bfloat16))
+  w_kn.fill_(7.0)
+  ops.pack_weights_batched(ops.pack_table([(master.cuda(), None, w_kn)], 'cuda'))      # without the w_nk copy
+  assert torch.equal(w_kn.cpu(), master.to(torch.bfloat16))
   # all layers of a module in one launch (ragged shapes, an item without the w_kn copy)
   shapes = [(320, 128), (64, 3), (100, 257), (512, 256), (33, 1)]
   masters = [torch.tensor(rng.normal(size=sh).astype(np.float32)).cuda() for sh in shapes]

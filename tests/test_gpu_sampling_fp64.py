@@ -1,4 +1,4 @@
-"""Proposal resampler (mnrf_sample_level / mnrf_sample_level_dyn) against the fp64 reference of
+"""Proposal resampler (mnrf_sample_level, with d->anneal or a device-side anneal) against the fp64 reference of
 tests/sampling_ref.py, on every warp plan, jitter mode, dilation and anneal source.  Needs an H100.
 
 Every case checks: the dilated fenceposts bit for bit; the dilated weights, CDF, interval endpoints and interval
@@ -213,6 +213,8 @@ def _bad_calls():
   from multinerf_b200 import ops as _ops
   ub = _ops.u_grid(S, False)[0].cuda()
 
+  anneal = torch.ones(1, device='cuda')
+
   def call(num_prev=P, num_samples=S, jitter_mode=0, null=None):
     out, buf = _guarded(torch.zeros(B, S + 1), SENTINEL)
     out.fill_(SENTINEL)
@@ -221,9 +223,10 @@ def _bad_calls():
     if null:
       p[null] = None
 
-    def run(lib):
-      L.check(lib.mnrf_sample_level(C.byref(d), p['t'], p['w'], p['ub'], None, None, p['out'], None, None, None,
-                                    None, L.stream_ptr()))
+    def run(lib, device_anneal):
+      L.check(lib.mnrf_sample_level(C.byref(d), p['t'], p['w'], p['ub'], None,
+                                    L.ptr(anneal) if device_anneal else None, None, p['out'], None, None, None, None,
+                                    L.stream_ptr()))
     return run, buf
   return {'num_samples 1': lambda: call(num_samples=1), 'num_samples 0': lambda: call(num_samples=0),
           'num_prev 0': lambda: call(num_prev=0), 'num_prev 1025': lambda: call(num_prev=1025),
@@ -237,23 +240,25 @@ BAD = ['num_samples 1', 'num_samples 0', 'num_prev 0', 'num_prev 1025', 'jitter_
        'jitter_mode 2 without jitter', 'null sdist_prev', 'null w_prev', 'null u_base', 'null sdist_out']
 
 
+@pytest.mark.parametrize('anneal', ['host anneal', 'device anneal'])
 @pytest.mark.parametrize('name', BAD)
-def test_rejected_arguments(ops, name):
+def test_rejected_arguments(ops, name, anneal):
   from multinerf_b200 import lib as L
   run, buf = _bad_calls()[name]()
   with pytest.raises(L.MnrfError):
-    run(L.load())
+    run(L.load(), anneal == 'device anneal')
   torch.cuda.synchronize()
   assert _pads_intact(buf, SENTINEL) and (buf == SENTINEL).all(), f'{name}: the refused call wrote its output'
 
 
-def test_zero_rays(ops):
+def test_zero_rays_with_either_anneal_source(ops):
   from multinerf_b200 import lib as L
   out, buf = _guarded(torch.zeros(4), SENTINEL)
   out.fill_(SENTINEL)
   d = L.SampleDesc(0, 4, 6, 1, 0.01, 0.0, 1.0, 1.0, 0.0, 1, 0.1)
   x = L.ptr(out)
-  L.check(L.load().mnrf_sample_level(C.byref(d), x, x, x, x, None, x, None, None, None, None, L.stream_ptr()))
-  L.check(L.load().mnrf_sample_level_dyn(C.byref(d), x, x, x, x, x, x, L.stream_ptr()))
+  for anneal_dev in (None, x):       # d->anneal, then the exponent read from the device
+    L.check(L.load().mnrf_sample_level(C.byref(d), x, x, x, x, anneal_dev, None, x, None, None, None, None,
+                                       L.stream_ptr()))
   torch.cuda.synchronize()
   assert (buf == SENTINEL).all()

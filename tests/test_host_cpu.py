@@ -12,13 +12,13 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_abi_library_loads_and_exports_header_symbols():
+def test_abi_v2_library_loads_and_exports_header_symbols():
   from multinerf_b200 import lib
   if not os.path.exists(lib.LIB_PATH):
     from multinerf_b200 import build
     build.build()
   l = lib.load()
-  assert l.mnrf_abi_version() == 1
+  assert l.mnrf_abi_version() == 2
   header = open(os.path.join(ROOT, 'include', 'mnrf.h')).read()
   declared = set(re.findall(r'\b(mnrf_[a-z0-9_]+)\s*\(', header))
   declared -= {'mnrf_bf16', 'mnrf_stream'}
@@ -36,6 +36,35 @@ def test_abi_library_loads_and_exports_header_symbols():
                    ctypes.sizeof(lib.CompositeDesc), ctypes.sizeof(lib.LossDesc), ctypes.sizeof(lib.AdamDesc),
                    ctypes.sizeof(lib.RefdirDesc), ctypes.sizeof(lib.CameraDesc), ctypes.sizeof(lib.PackItem),
                    ctypes.sizeof(lib.ChainLayer), ctypes.sizeof(lib.ChainDesc)]
+
+
+def test_binding_argtypes_match_header_prototypes():
+  """Every prototype of mnrf.h against its ctypes binding, parameter by parameter: a wrong argtype would pass a
+  float in a pointer register (or an int32 where the callee reads 64 bits) and nothing else would notice."""
+  import ctypes as C
+  from multinerf_b200 import lib
+  header = re.sub(r'/\*.*?\*/', '', open(os.path.join(ROOT, 'include', 'mnrf.h')).read(), flags=re.S)
+  # host descriptors passed by reference; every other pointer (mnrf_pack_item's table included) is a device address
+  descs = {'mnrf_sample_desc': lib.SampleDesc, 'mnrf_encode_desc': lib.EncodeDesc, 'mnrf_gemm_desc': lib.GemmDesc,
+           'mnrf_gemm_instance': lib.GemmInstance, 'mnrf_chain_desc': lib.ChainDesc,
+           'mnrf_composite_desc': lib.CompositeDesc, 'mnrf_loss_desc': lib.LossDesc, 'mnrf_robust_desc': lib.RobustDesc,
+           'mnrf_refdir_desc': lib.RefdirDesc, 'mnrf_camera_desc': lib.CameraDesc,
+           'mnrf_spherical_desc': lib.SphericalDesc, 'mnrf_adam_desc': lib.AdamDesc}
+  types = {'int': C.c_int, 'constchar*': C.c_char_p, 'int32_t': C.c_int32, 'int64_t': C.c_int64, 'float': C.c_float,
+           'double': C.c_double, 'mnrf_stream': C.c_void_p}
+  protos = re.findall(r'^(int|const char\*)\s+(mnrf_\w+)\(([^;]*)\);', header, re.M)
+  assert {name for _, name, _ in protos} == set(lib.EXPORTED)
+  for res, name, params in protos:
+    want = []
+    for p in params.split(','):
+      ctype = p.strip().rsplit(None, 1)[0].replace('const ', '').strip()
+      if p.strip() == 'void':
+        continue
+      if ctype.endswith('*'):
+        want.append(C.POINTER(descs[ctype[:-1]]) if ctype[:-1] in descs else C.c_void_p)
+      else:
+        want.append(types[ctype])
+    assert lib._SIGNATURES[name] == (types[res.replace(' ', '')], want), name
 
 
 def test_no_cpu_fallback():

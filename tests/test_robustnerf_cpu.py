@@ -101,14 +101,14 @@ def test_config_validation_errors():
                                                  enable_robustnerf_loss=False, robustnerf_inner_patch_size=8), 17)
 
 
-def test_robust_abi_symbols_exported():
+def test_robust_abi_v2_symbols_exported():
   from multinerf_b200 import lib
   if not os.path.exists(lib.LIB_PATH):
     from multinerf_b200 import build
     build.build()
   l = lib.load()
-  assert l.mnrf_abi_version() == 1
-  for name in ('mnrf_robust_mask', 'mnrf_quantile', 'mnrf_composite_bwd_masked', 'mnrf_composite_bwd'):
+  assert l.mnrf_abi_version() == 2
+  for name in ('mnrf_robust_mask', 'mnrf_quantile', 'mnrf_composite_bwd'):
     assert name in lib.EXPORTED and hasattr(l, name)
   import ctypes
   import subprocess

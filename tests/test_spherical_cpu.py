@@ -44,13 +44,13 @@ def test_fixture_cases_are_not_degenerate():
   assert rad.min() > 0 and rad.max() / rad.min() > 1.9
 
 
-def test_spherical_abi_symbol_exported():
+def test_spherical_abi_v2_symbol_exported():
   from multinerf_b200 import lib
   if not os.path.exists(lib.LIB_PATH):
     from multinerf_b200 import build
     build.build()
   l = lib.load()
-  assert l.mnrf_abi_version() == 1
+  assert l.mnrf_abi_version() == 2
   assert 'mnrf_spherical_rays' in lib.EXPORTED and hasattr(l, 'mnrf_spherical_rays')
   src = ('#include <stdio.h>\n#include "mnrf.h"\n'
          'int main(){printf("%zu\\n", sizeof(mnrf_spherical_desc)); return 0;}')

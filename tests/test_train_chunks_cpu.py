@@ -59,22 +59,20 @@ def _sizeof(types):
   return [int(x) for x in out.split()]
 
 
-def test_chunk_entry_points_declared_and_exported():
+def test_batch_rays_declared_on_the_base_entry_points():
   from multinerf_b200 import lib
   header = open(os.path.join(ROOT, 'include', 'mnrf.h')).read()
-  for name in ('mnrf_composite_bwd_chunk', 'mnrf_robust_mask_chunk'):
-    decl = re.search(name + r'\(([^;]*)\);', header)
+  for name in ('mnrf_composite_bwd', 'mnrf_robust_mask'):
+    decl = re.search(r'\b' + name + r'\(([^;]*)\);', header)
     assert decl and 'int32_t batch_rays' in decl.group(1), name
     assert name in lib.EXPORTED
-  # the chunk entries take the arguments of the entries they extend, then batch_rays, then the stream
-  sig = lib._SIGNATURES
-  assert sig['mnrf_composite_bwd_chunk'][1][:-2] == sig['mnrf_composite_bwd_masked'][1][:-1]
-  assert sig['mnrf_robust_mask_chunk'][1][:-2] == sig['mnrf_robust_mask'][1][:-1]
+  assert 'const float* data_mask' in re.search(r'\bmnrf_composite_bwd\(([^;]*)\);', header).group(1)
   if not os.path.exists(lib.LIB_PATH):
     from multinerf_b200 import build
     build.build()
   l = lib.load()
-  assert hasattr(l, 'mnrf_composite_bwd_chunk') and hasattr(l, 'mnrf_robust_mask_chunk')
+  for name in ('mnrf_composite_bwd_chunk', 'mnrf_composite_bwd_masked', 'mnrf_robust_mask_chunk'):
+    assert name not in header and name not in lib.EXPORTED and not hasattr(l, name)
 
 
 def test_existing_descriptors_unchanged():

@@ -84,10 +84,19 @@ def _bundles(configs):
     b.model.single_mlp = True
     return b
 
-  def robust(b):
+  def robust(b, patch_size=8):
     c = b.config
-    c.data_loss_type, c.patch_size, c.enable_robustnerf_loss = 'robustnerf', 8, True
+    c.data_loss_type, c.patch_size, c.enable_robustnerf_loss = 'robustnerf', patch_size, True
     c.robustnerf_inner_patch_size, c.robustnerf_smoothed_filter_size = 4, 3
+    return b
+
+  def activation(b, act, mlps=None):
+    for mlp in mlps or (b.prop_mlp, b.nerf_mlp):
+      mlp.net_activation = act
+    return b
+
+  def chunks(b, size=32):
+    b.config.train_chunk_size = size     # two passes of the B = 64 rays of run_case
     return b
 
   def skip_end(b):
@@ -132,6 +141,11 @@ def _bundles(configs):
       ('view_depth0_360', lambda: view_layout(b360(), depth=0), {}),
       ('view_depth0_glo', lambda: view_layout(glo(b256()), depth=0), {}),
       ('view_skips_end_glo', lambda: view_layout(glo(b256()), depth=9, skip=4), {}),
+      ('softplus_normals', lambda: activation(normal_losses(b256(), pred=True), 'softplus'), {}),
+      ('silu_refnerf', lambda: activation(bref(), 'silu'), {}),
+      ('chunks_360', lambda: chunks(b360()), {}),
+      # a 32-ray pass holds whole 4 x 4 patches; 8 x 8 patches do not divide it
+      ('chunks_robust', lambda: chunks(robust(b360(), patch_size=4)), {}),
   ]
 
 
