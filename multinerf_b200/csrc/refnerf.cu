@@ -470,6 +470,40 @@ act_tangent_bwd_kernel(int64_t M, int N, int act, const __nv_bfloat16* __restric
   }
 }
 
+// Host checks shared by mnrf_refdir_fwd and mnrf_refdir_bwd: the IDE tables, the normals and roughness the flags
+// switch on, the normals the losses read, and the slab columns [col0, col_end) within a row of `ld` holding
+// `min_cols` (the encoding in the forward, the encoding and the 11 head gradients in the backward).  Returns the
+// MNRF_CHECK code.
+inline int check_refdir(const char* fn, const mnrf_refdir_desc* d, const float* ide_mat, const int32_t* ide_ml,
+                        const float* grad_pred, const float* raw_grad_density, const float* raw_rough,
+                        float orient_mult, float prednorm_mult, int32_t orient_on_pred, bool losses, int64_t ld,
+                        bool bwd) {
+  MNRF_CHECK(d->num_samples > 0, "%s: num_samples must be positive", fn);
+  MNRF_CHECK(!d->use_ide || (ide_mat && ide_ml && d->deg_view >= 1 && d->deg_view <= 5),
+             "Only deg_view of at most 5 is numerically stable.");
+  int ide_n = 0;
+  for (int i = 0; d->use_ide && i < d->deg_view; ++i) ide_n += (1 << i) + 1;
+  MNRF_CHECK(!d->use_ide || d->ide_n == ide_n, "%s: ide_n %d does not match deg_view %d (%d (m, l) pairs)", fn,
+             d->ide_n, d->deg_view, ide_n);
+  MNRF_CHECK(d->use_ide || d->deg_view >= 0, "%s: deg_view must not be negative", fn);
+  MNRF_CHECK(!d->use_ide || d->use_roughness, "%s: the IDE needs a roughness (kappa_inv)", fn);
+  MNRF_CHECK(d->use_pred_normals || d->use_density_normals || !(d->use_reflections || d->use_n_dot_v),
+             "Normals must be computed for reflection directions.");
+  MNRF_CHECK(!d->use_pred_normals || grad_pred, "%s: use_pred_normals needs grad_pred", fn);
+  MNRF_CHECK(!d->use_density_normals || raw_grad_density, "%s: use_density_normals needs raw_grad_density", fn);
+  MNRF_CHECK(!d->use_roughness || raw_rough, "%s: use_roughness needs raw_rough", fn);
+  MNRF_CHECK(!losses || !(orient_mult > 0.f) || (orient_on_pred ? d->use_pred_normals : d->use_density_normals),
+             "Normals cannot be None if orientation loss is on.");
+  MNRF_CHECK(!losses || !(prednorm_mult > 0.f) || (d->use_pred_normals && d->use_density_normals),
+             "Predicted normals and gradient normals cannot be None if predicted normal loss is on.");
+  const int64_t enc = (d->use_ide ? 2 * (int64_t)ide_n : 3 + 6 * (int64_t)d->deg_view) + (d->use_n_dot_v ? 1 : 0);
+  const int64_t min_cols = bwd ? std::max<int64_t>(enc, 11) : enc;
+  MNRF_CHECK(d->col0 >= 0 && (int64_t)d->col_end - d->col0 >= min_cols && d->col_end <= ld,
+             "%s: the slab columns [%d, %d) of a row of %lld must hold %lld columns", fn, d->col0, d->col_end,
+             (long long)ld, (long long)min_cols);
+  return 0;
+}
+
 }  // namespace mnrf
 
 extern "C" int mnrf_refdir_fwd(const mnrf_refdir_desc* d, const float* ide_mat, const int32_t* ide_ml,
@@ -480,11 +514,10 @@ extern "C" int mnrf_refdir_fwd(const mnrf_refdir_desc* d, const float* ide_mat, 
   using namespace mnrf;
   if (d && d->M == 0) return 0;
   MNRF_CHECK(d && viewdirs && slab, "mnrf_refdir_fwd: null pointer");
-  MNRF_CHECK(!d->use_ide || (ide_mat && ide_ml && d->ide_n <= kIdeMax && d->deg_view >= 1 && d->deg_view <= 5),
-             "Only deg_view of at most 5 is numerically stable.");
-  MNRF_CHECK(!d->use_ide || d->use_roughness, "mnrf_refdir_fwd: the IDE needs a roughness (kappa_inv)");
-  MNRF_CHECK(d->use_pred_normals || d->use_density_normals || !(d->use_reflections || d->use_n_dot_v),
-             "Normals must be computed for reflection directions.");
+  if (check_refdir("mnrf_refdir_fwd", d, ide_mat, ide_ml, grad_pred, raw_grad_density, raw_rough, orient_mult,
+                   prednorm_mult, orient_on_pred, extra_dw != nullptr, d->ld, false))
+    return 1;
+  MNRF_CHECK(!d->use_roughness || roughness, "mnrf_refdir_fwd: use_roughness needs the roughness output");
   if (d->M == 0) return 0;
   RefDesc r{d->M, d->num_samples, d->use_pred_normals, d->use_density_normals, d->use_reflections, d->use_ide,
             d->use_n_dot_v, d->use_roughness, d->deg_view, d->roughness_bias, d->ld, d->col0, d->col_end};
@@ -507,8 +540,13 @@ extern "C" int mnrf_refdir_bwd(const mnrf_refdir_desc* d, const float* ide_mat, 
   using namespace mnrf;
   if (d && d->M == 0) return 0;
   MNRF_CHECK(d && viewdirs && weights && d_slab && stats, "mnrf_refdir_bwd: null pointer");
-  MNRF_CHECK(d->col_end - d->col0 >= 11, "mnrf_refdir_bwd: the slab must hold the 11 head gradients");
-  MNRF_CHECK(!d->use_ide || (ide_mat && ide_ml && d->ide_n <= kIdeMax), "mnrf_refdir_bwd: bad IDE tables");
+  if (check_refdir("mnrf_refdir_bwd", d, ide_mat, ide_ml, grad_pred, raw_grad_density, raw_rough, orient_mult,
+                   prednorm_mult, orient_on_pred, true, ld_dslab, true))
+    return 1;
+  MNRF_CHECK(!d->use_roughness || d_raw_rough, "mnrf_refdir_bwd: use_roughness needs d_raw_rough");
+  MNRF_CHECK(!d->use_pred_normals || d_grad_pred, "mnrf_refdir_bwd: use_pred_normals needs d_grad_pred");
+  MNRF_CHECK(!d->use_density_normals || d_raw_grad_density,
+             "mnrf_refdir_bwd: use_density_normals needs d_raw_grad_density");
   if (d->M == 0) return 0;
   RefDesc r{d->M, d->num_samples, d->use_pred_normals, d->use_density_normals, d->use_reflections, d->use_ide,
             d->use_n_dot_v, d->use_roughness, d->deg_view, d->roughness_bias, d->ld, d->col0, d->col_end};

@@ -409,91 +409,6 @@ def test_composite_diffuse_specular_mode(ops):
     close(got, ref, atol=2e-5 * float(ref.abs().max()), rtol=3e-4, msg=name)
 
 
-@pytest.mark.parametrize('mode', ['refnerf', 'viewdir_pe_normals'])
-def test_refdir_stage_vs_oracle_autograd(ops, mode):
-  """normals / roughness / reflection / IDE (or PE) / n.v slab, the two normal losses, and the
-  adjoint of all of it (csrc/refnerf.cu) against the oracle differentiated by torch autograd."""
-  from multinerf_b200 import ref_utils
-  rng = np.random.default_rng(41)
-  B, S = 37, 8
-  M = B * S
-  ide = mode == 'refnerf'
-  deg = 5 if ide else 4
-  v = rng.normal(size=(B, 3)).astype(np.float32)
-  v /= np.linalg.norm(v, axis=-1, keepdims=True)
-  vt = torch.tensor(v)
-  leaves = [torch.tensor(rng.normal(size=sh).astype(np.float32) * sc, requires_grad=True)
-            for sh, sc in [((B, S, 3), 1.0), ((B, S, 1), 1.0), ((3, B, S), 30.0)]]
-  grad_pred, raw_rough, rgd = leaves
-  w = torch.tensor(rng.uniform(0, 0.2, (B, S)).astype(np.float32))
-  dim = ref_utils.ide_dim(5) if ide else 3 + 6 * deg
-  ncols = dim + 1
-  col0, ld = 64, 64 + 128
-  g_slab = torch.tensor(rng.normal(size=(B, S, ncols)).astype(np.float32)).to(torch.bfloat16).float()
-  om, pm = 0.1 / B, 3e-4 / B
-  # oracle
-  n_pred = -o_coord.l2_normalize(grad_pred)
-  n_den = -o_coord.l2_normalize(rgd.permute(1, 2, 0))
-  rough = torch.nn.functional.softplus(raw_rough - 1.0)
-  if ide:
-    refd = o_coord.reflect(-vt[:, None, :], n_pred)
-    enc = o_coord.generate_ide_fn(5)(refd, rough)
-  else:
-    enc = o_coord.pos_enc(vt, 0, deg)[:, None, :].expand(B, S, dim)
-  ndv = (n_pred * vt[:, None, :]).sum(-1, keepdim=True)
-  slab_o = torch.cat([enc, ndv], -1)
-  l_or = om * (w * torch.clamp((n_pred * -vt[:, None, :]).sum(-1), max=0.0) ** 2).sum()
-  l_pn = pm * (w * (1.0 - (n_den * n_pred).sum(-1))).sum()
-  loss = (slab_o * g_slab).sum() + l_or + l_pn
-  grads = torch.autograd.grad(loss, leaves, allow_unused=True)
-  grads = [torch.zeros_like(x) if g_ is None else g_ for g_, x in zip(grads, leaves)]   # PE ignores roughness
-  # device
-  m, l, mat = ref_utils.ide_tables(5)
-  mat_d = torch.tensor(mat, dtype=torch.float32).cuda().contiguous()
-  ml_d = torch.tensor(np.stack([m, l]), dtype=torch.int32).cuda().contiguous()
-  desc = ops.refdir_desc(M, S, use_pred_normals=True, use_density_normals=True, use_reflections=ide, use_ide=ide,
-                         use_n_dot_v=True, use_roughness=True, deg_view=deg, ide_n=len(m), roughness_bias=-1.0,
-                         ld=ld, col0=col0, col_end=ld)
-  slab = torch.full((M, ld), 5.0, dtype=torch.bfloat16, device='cuda')
-  npd, nd_, rgh, edw = (torch.empty(M, 3, device='cuda'), torch.empty(M, 3, device='cuda'),
-                        torch.empty(M, device='cuda'), torch.empty(M, device='cuda'))
-  gp_c = grad_pred.detach().reshape(M, 3).contiguous().cuda()
-  rr_c = raw_rough.detach().reshape(M).contiguous().cuda()
-  rgd_c = rgd.detach().reshape(3, M).contiguous().cuda()
-  ops.refdir_fwd(desc, mat_d, ml_d, gp_c, rr_c, rgd_c, vt.cuda(), npd, nd_, rgh, slab, om, pm, True, edw)
-  torch.cuda.synchronize()
-  close(npd.cpu().view(B, S, 3), n_pred.detach(), msg='normals_pred')
-  close(nd_.cpu().view(B, S, 3), n_den.detach(), atol=1e-5, rtol=1e-4, msg='normals')
-  close(rgh.cpu().view(B, S, 1), rough.detach(), msg='roughness')
-  got = slab.float().cpu().view(B, S, ld)
-  close(got[..., col0:col0 + ncols], slab_o.detach().to(torch.bfloat16).float(), atol=1.6e-2, rtol=1.6e-2, msg='slab')
-  assert (got[..., :col0] == 5).all() and (got[..., col0 + ncols:] == 0).all()
-  ref_edw = om * torch.clamp((n_pred * -vt[:, None, :]).sum(-1), max=0.0) ** 2 + pm * (1.0 - (n_den * n_pred).sum(-1))
-  close(edw.cpu().view(B, S), ref_edw.detach(), atol=1e-9, rtol=1e-4, msg='extra_dw')
-  # backward
-  d_slab = torch.zeros(M, ld, dtype=torch.bfloat16, device='cuda')
-  d_slab[:, col0:col0 + ncols] = g_slab.reshape(M, ncols).to(torch.bfloat16).cuda()
-  d_gp, d_rr, d_rgd = torch.empty(M, 3, device='cuda'), torch.empty(M, device='cuda'), torch.empty(3, M, device='cuda')
-  stats = torch.zeros(8, device='cuda')
-  drd = torch.tensor(rng.normal(size=M).astype(np.float32)).cuda()
-  ddf = torch.tensor(rng.normal(size=(M, 3)).astype(np.float32)).cuda()
-  ops.refdir_bwd(desc, mat_d, ml_d, gp_c, rr_c, rgd_c, vt.cuda(), w.reshape(M).contiguous().cuda(), d_slab, om, pm,
-                 True, drd, ddf, None, d_gp, d_rr, d_rgd, stats)
-  torch.cuda.synchronize()
-  for got_, ref, name in [(d_gp.cpu().view(B, S, 3), grads[0], 'd grad_pred'),
-                          (d_rr.cpu().view(B, S, 1), grads[1], 'd raw_rough'),
-                          (d_rgd.cpu().view(3, B, S), grads[2], 'd raw_grad_density')]:
-    close(got_, ref, atol=2e-4 * float(ref.abs().max()) + 1e-9, rtol=2e-3, msg=name)
-  close(stats[4].cpu(), l_or.detach(), rtol=1e-4, atol=1e-9, msg='orientation loss')
-  close(stats[5].cpu(), l_pn.detach(), rtol=1e-4, atol=1e-9, msg='pred-normal loss')
-  hs = d_slab.float().cpu()[:, col0:col0 + 11]
-  close(hs[:, 0], drd.cpu().to(torch.bfloat16).float(), atol=0, rtol=0, msg='head slab density')
-  close(hs[:, 1:4], d_gp.cpu().to(torch.bfloat16).float(), atol=0, rtol=0, msg='head slab grad_pred')
-  close(hs[:, 4:7], ddf.cpu().to(torch.bfloat16).float(), atol=0, rtol=0, msg='head slab diffuse')
-  assert (hs[:, 7:10] == 0).all()
-  close(hs[:, 10], d_rr.cpu().to(torch.bfloat16).float(), atol=0, rtol=0, msg='head slab roughness')
-
-
 @pytest.mark.parametrize('on_pred', [True, False])
 def test_normals_stage_matches_refdir_stage(ops, on_pred):
   """The colourless stage (mnrf_normals_fwd/bwd) and the Ref-NeRF stage share their normals and normal-loss
