@@ -106,6 +106,17 @@ int mnrf_encode(const mnrf_encode_desc* d, const float* sdist, const float* orig
                 const float* far, const float* basis, mnrf_bf16* feat_bf16, float* feat_f32,
                 float* tdist_out, mnrf_bf16* tfeat_bf16, int32_t ld_tfeat, mnrf_stream stream);
 
+/* Point form of the encoder: the MLP input of the Gaussian with mean points[i] and covariance var * I, in place of
+ * a cast ray interval (density queries on a grid, multinerf_b200/mesh.py).  The same contraction (covariance through
+ * the Jacobian when warp_contract), lift onto the basis and IPE (lifted variance 0 with disable_integration) as
+ * mnrf_encode, and the same bf16 rows:
+ *   d->num_rays = point count N; d->num_samples must be 1, d->raydist_fn and d->ray_shape 0
+ *   points [N, 3]; var >= 0; basis [K, 3]
+ *   feat_bf16 [N, ld_feat], columns [2KL, feat_cols) zero-filled; feat_f32 optional [N, 2KL]
+ */
+int mnrf_encode_points(const mnrf_encode_desc* d, const float* points, float var, const float* basis,
+                       mnrf_bf16* feat_bf16, float* feat_f32, mnrf_stream stream);
+
 /* View-direction positional encoding, coord.pos_enc (coord.py:136-147) with
  * append_identity, broadcast over the S samples of each ray (models.py:550-554) and
  * written as bf16 into columns [col0, col0 + 3 + 6*deg) of a [B*S, ld] buffer; columns up
@@ -549,6 +560,23 @@ typedef struct {
 
 int mnrf_pack_weights_batched(int32_t count, const mnrf_pack_item* items, int32_t total_tiles,
                               mnrf_stream stream);
+
+/* ---- mesh extraction -----------------------------------------------------------------------
+ * Marching cubes on an fp32 grid [nz, ny, nx] (each side in [2, 1024]); a point is inside when its value is
+ * > level.  Point p = (z * ny + y) * nx + x owns the edges leaving it along +x, +y, +z (edge id 3 p + axis) and
+ * the cell whose lowest corner it is (cell id p).  No reference counterpart (the reference has no mesh export).
+ *   phase COUNT: edge_cut [3 N] uint8 = 1 where the edge crosses the level; cell_tris [N] uint8 = triangles of the
+ *                cell (0 where p starts no cell).  N = nx * ny * nz.
+ *   phase EMIT:  edge_scan [3 N] / tri_scan [N] int64: inclusive scans of edge_cut / cell_tris (V, F = their last
+ *                elements); writes vertices [V, 3] (x, y, z in grid units: the linear crossing on the edge), one
+ *                per cut edge in edge order, and faces [F, 3] int32 (V < 2^31) in cell order, wound so that normals
+ *                point from inside to outside.
+ * The mesh of a level set that stays off the grid boundary is closed and consistently wound.
+ */
+enum { MNRF_MC_COUNT = 0, MNRF_MC_EMIT = 1 };
+int mnrf_marching_cubes(int32_t phase, int32_t nx, int32_t ny, int32_t nz, const float* grid, float level,
+                        uint8_t* edge_cut, uint8_t* cell_tris, const int64_t* edge_scan, const int64_t* tri_scan,
+                        float* vertices, int32_t* faces, mnrf_stream stream);
 
 #ifdef __cplusplus
 }

@@ -18,7 +18,7 @@ SOURCES = {
     'lib.cu': [], 'sampling.cu': ['-fmad=false'], 'encode.cu': ['-fmad=false'],
     'composite.cu': ['-fmad=false'], 'heads.cu': [], 'gemm_tc.cu': [], 'gemm_tc_act.cu': [], 'chain.cu': [],
     'gemm_ref.cu': [],
-    'refnerf.cu': [], 'camera.cu': ['-fmad=false'], 'robust.cu': ['-fmad=false'],
+    'refnerf.cu': [], 'camera.cu': ['-fmad=false'], 'robust.cu': ['-fmad=false'], 'mesh.cu': ['-fmad=false'],
 }
 
 
@@ -30,7 +30,7 @@ def _nvcc():
 
 
 # sources a unit includes besides the shared headers
-INCLUDES = {'gemm_tc_act.cu': ['gemm_tc.cu']}
+INCLUDES = {'gemm_tc_act.cu': ['gemm_tc.cu'], 'mesh.cu': ['mc_tables.cuh']}
 
 
 def _stamp(path, flags):

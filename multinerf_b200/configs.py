@@ -117,6 +117,12 @@ class Config:
   num_border_pixels_to_mask: int = 0
   autoexpose_renders: bool = False
   eval_raw_affine_cc: bool = False
+  # extract_mesh.py (multinerf_b200/mesh.py): grid points along the longest side of the box (cells are cubes), the
+  # density level of the surface, and the box (x0, y0, z0, x1, y1, z1) in world coordinates; None: [-1.5, 1.5]^3,
+  # or [-1, 1]^3 under the scene contraction.  Forward-facing (NDC) scenes need an explicit box.
+  mesh_resolution: int = 512
+  mesh_level: float = 10.
+  mesh_bbox: Optional[Tuple[float, ...]] = None
 
 
 @dataclasses.dataclass

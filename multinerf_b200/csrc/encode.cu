@@ -301,6 +301,99 @@ __device__ __forceinline__ float ex2_ftz(float x) {
   return r;
 }
 
+// The Gaussian-to-feature tail of the fast path, shared by the ray and the point encoders: lifts the g <= G
+// Gaussians at gs (kGaussStride floats apart, shared memory) onto the basis and writes their feature rows m0 ..
+// m0 + g - 1 (bf16, staged in `row`, G rows of row_elems; fp32 copy when feat_f32 is given).
+__device__ __forceinline__ void gauss_feature_rows(const mnrf_encode_desc& d, int g, const float* gs,
+                                                   const float* sb, __nv_bfloat16* row, int row_elems, size_t m0,
+                                                   __nv_bfloat16* __restrict__ feat, float* __restrict__ feat_f32,
+                                                   int lane) {
+  const int K = d.basis_k, L = d.max_deg - d.min_deg, KL = K * L;
+  const float sc0 = __int_as_float((127 + d.min_deg) << 23);       // 2^min_deg
+  const float sc_top = exp2f((float)(L + 1));                      // bound on the growth of |y| over the degrees (+ pi/2)
+  const int chunks = row_elems / 8;
+  for (int j0 = 0; j0 < g * K; j0 += 32) {
+    // uniform trip count (warp-wide max below): lanes past the last item redo it and store the same values
+    const int j = min(j0 + lane, g * K - 1);
+    const int sl = j / K;
+    const int k = j - sl * K;
+    const float* gp = gs + sl * kGaussStride;
+    const float b0 = sb[k * 3 + 0], b1 = sb[k * 3 + 1], b2 = sb[k * 3 + 2];
+    const float lm = gp[0] * b0 + gp[1] * b1 + gp[2] * b2;
+    const float c0 = gp[3] * b0 + gp[4] * b1 + gp[5] * b2;
+    const float c1 = gp[6] * b0 + gp[7] * b1 + gp[8] * b2;
+    const float c2 = gp[9] * b0 + gp[10] * b1 + gp[11] * b2;
+    const float lv = d.disable_integration ? 0.f : (b0 * c0 + b1 * c1 + b2 * c2);
+    float y = lm * sc0;
+    float v = lv * (sc0 * sc0);
+    __nv_bfloat16* rp = row + sl * row_elems + k;
+    float* fp = feat_f32 ? feat_f32 + (m0 + sl) * (size_t)(2 * KL) + k : nullptr;
+    // Leading degrees for which EVERY lane's |y| and |y + pi/2| stay below 100*pi need none of safe_sin's
+    // large-argument handling (two compare-and-branch pairs with their reconvergence barriers per degree, a
+    // fifth of the loop's instructions): |y| 2^l <= 311  <=>  l <= floor(log2(311 / |y|)), read off the exponent.
+    const float ymax = warp_max(fabsf(y));
+    int n_fast = ((__float_as_int(__fdividef(311.f, ymax)) >> 23) & 0xff) - 126;
+    n_fast = min(max(n_fast, 0), L);
+    int l = 0;
+#pragma unroll 4
+    for (; l < n_fast; ++l) {
+      // exp(-v/2): (-0.5 v) is exact, so one multiply by -0.5*log2(e) rounds like __expf's own
+      const float e = ex2_ftz(v * -0.72134751081466674805f);
+      const float fs = e * sin_below_100pi(y);
+      const float fc = e * sin_below_100pi(y + 1.57079637050628662109375f);
+      rp[l * K] = __float2bfloat16(fs);
+      rp[KL + l * K] = __float2bfloat16(fc);
+      if (fp) { fp[l * K] = fs; fp[KL + l * K] = fc; }
+      y = y * 2.f;
+      v = v * 4.f;
+    }
+    // remaining degrees: the branch-free large-argument form while every argument stays below its 1.3e9 limit
+    // (warp-uniform test), the general one otherwise
+    if (ymax * sc_top < 1e9f) {
+#pragma unroll 4
+      for (; l < L; ++l) {
+        const float e = ex2_ftz(v * -0.72134751081466674805f);
+        const float fs = e * safe_sin_nobranch(y);
+        const float fc = e * safe_sin_nobranch(y + 1.57079637050628662109375f);
+        rp[l * K] = __float2bfloat16(fs);
+        rp[KL + l * K] = __float2bfloat16(fc);
+        if (fp) { fp[l * K] = fs; fp[KL + l * K] = fc; }
+        y = y * 2.f;
+        v = v * 4.f;
+      }
+    }
+    for (; l < L; ++l) {
+      const float e = ex2_ftz(v * -0.72134751081466674805f);
+      const float fs = e * safe_sin_fast(y);
+      const float fc = e * safe_sin_fast(y + 1.57079637050628662109375f);
+      rp[l * K] = __float2bfloat16(fs);
+      rp[KL + l * K] = __float2bfloat16(fc);
+      if (fp) { fp[l * K] = fs; fp[KL + l * K] = fc; }
+      y = y * 2.f;
+      v = v * 4.f;
+    }
+  }
+  __syncwarp();
+  for (int r = 0; r < g; ++r) {
+    const uint4* src = reinterpret_cast<const uint4*>(row + r * row_elems);
+    uint4* dst = reinterpret_cast<uint4*>(feat + (m0 + r) * (size_t)d.ld_feat);
+    for (int c = lane; c < chunks; c += 32) dst[c] = src[c];
+  }
+  __syncwarp();
+}
+
+// Samples per group of the fast path: fill the 32-lane passes over (sample, direction) items as fully as possible.
+static int encode_group_size(int basis_k, int max_g) {
+  int G = 1;
+  double best = 0.0;
+  for (int g = 1; g <= 16 && g <= max_g; ++g) {
+    const int items = g * basis_k;
+    const double eff = (double)items / (32.0 * ((items + 31) / 32));
+    if (eff > best + 1e-9) { best = eff; G = g; }
+  }
+  return G;
+}
+
 // A ray may be split into `nseg` segments of `seg_len` samples (a multiple of G), one warp each: with few rays per
 // launch (a 2048-ray shard of an 8-GPU step) one warp per ray leaves most of the machine idle.
 __global__ void __launch_bounds__(256, 4)
@@ -312,7 +405,7 @@ encode_fast_kernel(mnrf_encode_desc d, int G, int nseg, int seg_len, const float
                    float* __restrict__ tdist_out) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  const int S = d.num_samples, K = d.basis_k, L = d.max_deg - d.min_deg, KL = K * L;
+  const int S = d.num_samples, K = d.basis_k;
   float* sb = reinterpret_cast<float*>(smem_raw);                 // basis [K][3]
   const int row_bytes = ((d.feat_cols * 2 + 15) / 16) * 16;
   const int row_elems = row_bytes / 2;
@@ -325,9 +418,6 @@ encode_fast_kernel(mnrf_encode_desc d, int G, int nseg, int seg_len, const float
   for (int i = threadIdx.x; i < 3 * K; i += blockDim.x) sb[i] = basis[i];
   __syncthreads();
   for (int i = lane; i < G * row_elems; i += 32) row[i] = __float2bfloat16(0.f);   // zero pad columns once
-  const float sc0 = __int_as_float((127 + d.min_deg) << 23);       // 2^min_deg
-  const float sc_top = exp2f((float)(L + 1));                      // bound on the growth of |y| over the degrees (+ pi/2)
-  const int chunks = row_bytes / 16;
 
   const int64_t num_items = (int64_t)d.num_rays * nseg;
   for (int64_t item = (int64_t)blockIdx.x * nw + wib; item < num_items; item += (int64_t)gridDim.x * nw) {
@@ -360,77 +450,54 @@ encode_fast_kernel(mnrf_encode_desc d, int G, int nseg, int seg_len, const float
     }
     __syncwarp();
     // phase B: G samples at a time
-    for (int s0 = s_begin; s0 < s_end; s0 += G) {
-      const int g = min(G, s_end - s0);
-      for (int j0 = 0; j0 < g * K; j0 += 32) {
-        // uniform trip count (warp-wide max below): lanes past the last item redo it and store the same values
-        const int j = min(j0 + lane, g * K - 1);
-        const int sl = j / K;
-        const int k = j - sl * K;
-        const float* gp = gs + (s0 + sl) * kGaussStride;
-        const float b0 = sb[k * 3 + 0], b1 = sb[k * 3 + 1], b2 = sb[k * 3 + 2];
-        const float lm = gp[0] * b0 + gp[1] * b1 + gp[2] * b2;
-        const float c0 = gp[3] * b0 + gp[4] * b1 + gp[5] * b2;
-        const float c1 = gp[6] * b0 + gp[7] * b1 + gp[8] * b2;
-        const float c2 = gp[9] * b0 + gp[10] * b1 + gp[11] * b2;
-        const float lv = d.disable_integration ? 0.f : (b0 * c0 + b1 * c1 + b2 * c2);
-        float y = lm * sc0;
-        float v = lv * (sc0 * sc0);
-        __nv_bfloat16* rp = row + sl * row_elems + k;
-        float* fp = feat_f32 ? feat_f32 + ((size_t)ray * S + s0 + sl) * (size_t)(2 * KL) + k : nullptr;
-        // Leading degrees for which EVERY lane's |y| and |y + pi/2| stay below 100*pi need none of safe_sin's
-        // large-argument handling (two compare-and-branch pairs with their reconvergence barriers per degree, a
-        // fifth of the loop's instructions): |y| 2^l <= 311  <=>  l <= floor(log2(311 / |y|)), read off the exponent.
-        const float ymax = warp_max(fabsf(y));
-        int n_fast = ((__float_as_int(__fdividef(311.f, ymax)) >> 23) & 0xff) - 126;
-        n_fast = min(max(n_fast, 0), L);
-        int l = 0;
-#pragma unroll 4
-        for (; l < n_fast; ++l) {
-          // exp(-v/2): (-0.5 v) is exact, so one multiply by -0.5*log2(e) rounds like __expf's own
-          const float e = ex2_ftz(v * -0.72134751081466674805f);
-          const float fs = e * sin_below_100pi(y);
-          const float fc = e * sin_below_100pi(y + 1.57079637050628662109375f);
-          rp[l * K] = __float2bfloat16(fs);
-          rp[KL + l * K] = __float2bfloat16(fc);
-          if (fp) { fp[l * K] = fs; fp[KL + l * K] = fc; }
-          y = y * 2.f;
-          v = v * 4.f;
-        }
-        // remaining degrees: the branch-free large-argument form while every argument stays below its 1.3e9 limit
-        // (warp-uniform test), the general one otherwise
-        if (ymax * sc_top < 1e9f) {
-#pragma unroll 4
-          for (; l < L; ++l) {
-            const float e = ex2_ftz(v * -0.72134751081466674805f);
-            const float fs = e * safe_sin_nobranch(y);
-            const float fc = e * safe_sin_nobranch(y + 1.57079637050628662109375f);
-            rp[l * K] = __float2bfloat16(fs);
-            rp[KL + l * K] = __float2bfloat16(fc);
-            if (fp) { fp[l * K] = fs; fp[KL + l * K] = fc; }
-            y = y * 2.f;
-            v = v * 4.f;
-          }
-        }
-        for (; l < L; ++l) {
-          const float e = ex2_ftz(v * -0.72134751081466674805f);
-          const float fs = e * safe_sin_fast(y);
-          const float fc = e * safe_sin_fast(y + 1.57079637050628662109375f);
-          rp[l * K] = __float2bfloat16(fs);
-          rp[KL + l * K] = __float2bfloat16(fc);
-          if (fp) { fp[l * K] = fs; fp[KL + l * K] = fc; }
-          y = y * 2.f;
-          v = v * 4.f;
-        }
+    for (int s0 = s_begin; s0 < s_end; s0 += G)
+      gauss_feature_rows(d, min(G, s_end - s0), gs + s0 * kGaussStride, sb, row, row_elems, (size_t)ray * S + s0,
+                         feat, feat_f32, lane);
+  }
+}
+
+// Point form: the Gaussian of point i has mean points[i] and covariance var * I.  One warp encodes G points at a
+// time through the fast path's tail.
+__global__ void __launch_bounds__(256, 4)
+encode_points_kernel(mnrf_encode_desc d, int G, const float* __restrict__ points, float var,
+                     const float* __restrict__ basis, __nv_bfloat16* __restrict__ feat, float* __restrict__ feat_f32) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  const int K = d.basis_k;
+  float* sb = reinterpret_cast<float*>(smem_raw);                 // basis [K][3]
+  const int row_bytes = ((d.feat_cols * 2 + 15) / 16) * 16;
+  const int row_elems = row_bytes / 2;
+  float* gs = sb + 3 * K + (size_t)wib * G * kGaussStride;
+  unsigned char* rows = smem_raw + (((size_t)(3 * K + nw * G * kGaussStride) * 4 + 15) / 16) * 16;
+  __nv_bfloat16* row = reinterpret_cast<__nv_bfloat16*>(rows + (size_t)wib * G * row_bytes);
+
+  for (int i = threadIdx.x; i < 3 * K; i += blockDim.x) sb[i] = basis[i];
+  __syncthreads();
+  for (int i = lane; i < G * row_elems; i += 32) row[i] = __float2bfloat16(0.f);   // zero pad columns once
+
+  const int64_t num_groups = ((int64_t)d.num_rays + G - 1) / G;
+  for (int64_t grp = (int64_t)blockIdx.x * nw + wib; grp < num_groups; grp += (int64_t)gridDim.x * nw) {
+    const int64_t p0 = grp * G;
+    const int g = (int)min((int64_t)G, (int64_t)d.num_rays - p0);
+    __syncwarp();
+    if (lane < g) {
+      Gauss ga;
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+        ga.mean[i] = points[(p0 + lane) * 3 + i];
+#pragma unroll
+        for (int j = 0; j < 3; ++j) ga.cov[i][j] = i == j ? var : 0.f;
       }
-      __syncwarp();
-      for (int r = 0; r < g; ++r) {
-        const uint4* src = reinterpret_cast<const uint4*>(row + r * row_elems);
-        uint4* dst = reinterpret_cast<uint4*>(feat + ((size_t)ray * S + s0 + r) * (size_t)d.ld_feat);
-        for (int c = lane; c < chunks; c += 32) dst[c] = src[c];
-      }
-      __syncwarp();
+      if (d.warp_contract) contract_gauss(ga);
+      float* gp = gs + lane * kGaussStride;
+      gp[0] = ga.mean[0]; gp[1] = ga.mean[1]; gp[2] = ga.mean[2];
+#pragma unroll
+      for (int i = 0; i < 3; ++i)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) gp[3 + i * 3 + j] = ga.cov[i][j];
     }
+    __syncwarp();
+    gauss_feature_rows(d, g, gs, sb, row, row_elems, (size_t)p0, feat, feat_f32, lane);
   }
 }
 
@@ -525,14 +592,7 @@ extern "C" int mnrf_encode(const mnrf_encode_desc* d, const float* sdist, const 
   const int max_blocks = mnrf_num_sms() * 8;
   if (blocks > max_blocks) blocks = max_blocks;
   if (!tfeat) {
-    // samples per group: fill the 32-lane passes over (sample, direction) items as fully as possible
-    int G = 1;
-    double best = 0.0;
-    for (int g = 1; g <= 16 && g <= d->num_samples; ++g) {
-      const int items = g * d->basis_k;
-      const double eff = (double)items / (32.0 * ((items + 31) / 32));
-      if (eff > best + 1e-9) { best = eff; G = g; }
-    }
+    const int G = encode_group_size(d->basis_k, d->num_samples);
     size_t smem = (((size_t)(3 * d->basis_k + nw * ((d->num_samples + 1) + d->num_samples * kGaussStride)) * 4 + 15) / 16) * 16 +
                   (size_t)nw * G * row_bytes;
     MNRF_CHECK(smem <= 200 * 1024, "mnrf_encode: shared memory %zu too large", smem);
@@ -563,6 +623,38 @@ extern "C" int mnrf_encode(const mnrf_encode_desc* d, const float* sdist, const 
       *d, sdist, origins, directions, radii, near, far, basis,
       reinterpret_cast<__nv_bfloat16*>(feat_bf16), feat_f32, tdist_out,
       reinterpret_cast<__nv_bfloat16*>(tfeat), ld_tfeat);
+  MNRF_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int mnrf_encode_points(const mnrf_encode_desc* d, const float* points, float var, const float* basis,
+                                  mnrf_bf16* feat_bf16, float* feat_f32, mnrf_stream stream) {
+  using namespace mnrf;
+  MNRF_CHECK(d, "mnrf_encode_points: null descriptor");
+  MNRF_CHECK(d->num_rays >= 0, "mnrf_encode_points: negative point count %d", d->num_rays);
+  if (d->num_rays == 0) return 0;
+  MNRF_CHECK(points && basis && feat_bf16, "mnrf_encode_points: null pointer");
+  MNRF_CHECK(d->num_samples == 1 && d->raydist_fn == 0 && d->ray_shape == 0,
+             "mnrf_encode_points: num_samples must be 1 and raydist_fn, ray_shape 0 (got %d, %d, %d)",
+             d->num_samples, d->raydist_fn, d->ray_shape);
+  MNRF_CHECK(var >= 0.f, "mnrf_encode_points: var %g < 0", var);
+  MNRF_CHECK(d->basis_k > 0 && d->max_deg > d->min_deg, "mnrf_encode_points: empty encoding");
+  const int KL2 = 2 * d->basis_k * (d->max_deg - d->min_deg);
+  MNRF_CHECK(d->feat_cols >= KL2 && d->ld_feat >= d->feat_cols, "mnrf_encode_points: feat_cols %d < 2KL %d or ld %d",
+             d->feat_cols, KL2, d->ld_feat);
+  MNRF_CHECK(d->feat_cols % 8 == 0 && d->ld_feat % 8 == 0 && ((uintptr_t)feat_bf16 % 16) == 0,
+             "mnrf_encode_points: feature rows must be 16-byte aligned");
+  const int nw = 8;
+  const int G = encode_group_size(d->basis_k, 16);
+  const int row_bytes = ((d->feat_cols * 2 + 15) / 16) * 16;
+  const size_t smem = (((size_t)(3 * d->basis_k + nw * G * kGaussStride) * 4 + 15) / 16) * 16 +
+                      (size_t)nw * G * row_bytes;
+  MNRF_CHECK(smem <= 200 * 1024, "mnrf_encode_points: shared memory %zu too large", smem);
+  MNRF_CUDA(cudaFuncSetAttribute(encode_points_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int64_t groups = ((int64_t)d->num_rays + G - 1) / G;
+  const int blocks = (int)std::min<int64_t>((groups + nw - 1) / nw, (int64_t)mnrf_num_sms() * 8);
+  encode_points_kernel<<<blocks, nw * 32, smem, (cudaStream_t)stream>>>(
+      *d, G, points, var, basis, reinterpret_cast<__nv_bfloat16*>(feat_bf16), feat_f32);
   MNRF_LAUNCH_CHECK();
   return 0;
 }

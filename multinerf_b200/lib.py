@@ -162,7 +162,10 @@ _SIGNATURES = {
     'mnrf_spherical_rays': (C.c_int, [C.POINTER(SphericalDesc)] + [_P] * 6),
     'mnrf_clip_adam': (C.c_int, [C.POINTER(AdamDesc)] + [_P] * 7),
     'mnrf_pack_weights_batched': (C.c_int, [C.c_int32, _P, C.c_int32, _P]),
+    'mnrf_encode_points': (C.c_int, [C.POINTER(EncodeDesc), _P, C.c_float, _P, _P, _P, _P]),
+    'mnrf_marching_cubes': (C.c_int, [C.c_int32] * 4 + [_P, C.c_float] + [_P] * 7),
 }
+MC_COUNT, MC_EMIT = 0, 1
 EXPORTED = tuple(_SIGNATURES)
 
 _lib = None

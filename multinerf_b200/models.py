@@ -557,10 +557,11 @@ class Model:
                 rgb_mode=1 if (cfg.use_diffuse_color and not cfg.disable_rgb) else 0)
 
   # ------------------------------------------------------------------ buffers
-  def _level_state(self, key, mname, B, S):
+  def _level_state(self, key, mname, B, S, trunk_only=False):
     # one buffer set per (level, module, shape), never replaced: captured CUDA graphs (train step, render
     # chunks) hold raw pointers into these buffers, so a differently shaped call (the ragged last chunk of
-    # an image) must not free them
+    # an image) must not free them.  trunk_only: the buffers of encode -> trunk -> density head alone, for a
+    # render-only pass no graph captures (query_density); not kept, so they are freed with the caller's reference
     key = (key, mname, B, S)
     st = self._levels.get(key)
     if st is not None:
@@ -588,8 +589,12 @@ class Model:
     relu = plan.act == L.ACT_RELU
     if relu:
       st.bits = [torch.empty(M, W // 32, device=dev, dtype=torch.int32) for _ in range(cfg.net_depth)]
-    else:
+    elif not trunk_only:
       st.zs = [torch.empty(M, W, device=dev, dtype=bf) for _ in range(cfg.net_depth)]
+    if trunk_only:
+      st.keep_acts = False
+      st.raw_head = torch.empty(M, plan.head_n, device=dev)
+      return st
     if plan.density_normals:
       # forward-mode tangents d(.)/d(mean_x|y|z), three stacked streams of M rows
       st.tacts, st.tfeat, st.tfeat_copies = trunk_buffers(3 * M)
@@ -683,12 +688,18 @@ class Model:
     """Encoding, the trunk (one chained launch, or one GEMM per layer) and the density (or stacked) head."""
     plan = mlp.plan
     cfg = plan.cfg
-    W = cfg.net_width
     m = self.mcfg
     ops.encode(st.sdist, rays.origins, rays.directions, rays.radii_flat, rays.near_flat,
                rays.far_flat, mlp.basis, min_deg=cfg.min_deg_point, max_deg=cfg.max_deg_point,
                raydist_fn=m.raydist_fn, ray_shape=m.ray_shape, warp_contract=cfg.warp_fn == 'contract',
                disable_integration=m.disable_integration, feat=st.feat, feat_cols=plan.Fpad, tfeat=st.tfeat)
+    self._trunk_layers(st, mlp, impl)
+
+  def _trunk_layers(self, st, mlp, impl):
+    """The trunk (one chained launch, or one GEMM per layer) and the density (or stacked) head on the encoded
+    st.feat."""
+    plan = mlp.plan
+    W = plan.cfg.net_width
     for c in st.feat_copies:
       c.copy_(st.feat)
     x = st.feat
@@ -707,6 +718,34 @@ class Model:
       d = plan.one('density')
       ops.head_fwd(x, mlp.w_head, mlp.b(d), plan.head_n, d.in_pad, raw=st.raw_head)
     st.x_last = x
+
+  def query_density(self, points, var, impl=0):
+    """Density of the final level's MLP (NerfMLP_0) at world points [N, 3] (tensor or array): the point encoder on
+    the Gaussians (point, var * I), the trunk and the density head in their render form, then
+    density_activation(raw + density_bias), without density noise -> fp32 [N] on the device.  Runs in chunks of
+    render_chunk_size * num_nerf_samples rows, the rows of one render chunk's final level."""
+    mname = 'NerfMLP_0'
+    mlp = self.mlps[mname]
+    plan = mlp.plan
+    cfg = plan.cfg
+    points = torch.as_tensor(points, dtype=torch.float32, device=self.device).reshape(-1, 3).contiguous()
+    N = points.shape[0]
+    density = torch.empty(N, device=self.device)
+    chunk = self.config.render_chunk_size * self.mcfg.num_nerf_samples
+    states = {}
+    for i0 in range(0, N, chunk):
+      p = points[i0:i0 + chunk]
+      n = p.shape[0]
+      if n not in states:
+        states[n] = self._level_state('query', mname, n, 1, trunk_only=True)
+      st = states[n]
+      ops.encode_points(p, var, mlp.basis, min_deg=cfg.min_deg_point, max_deg=cfg.max_deg_point,
+                        warp_contract=cfg.warp_fn == 'contract', disable_integration=self.mcfg.disable_integration,
+                        feat=st.feat, feat_cols=plan.Fpad)
+      self._trunk_layers(st, mlp, impl)
+      # density_activation: softplus, the only one MLPPlan accepts
+      torch.nn.functional.softplus(st.raw_head[:, 0] + cfg.density_bias, out=density[i0:i0 + n])
+    return density
 
   def _tangent_fwd(self, st, mlp, impl):
     """raw_grad_density = d raw_density / d mean by forward mode (replaces vmap(value_and_grad),

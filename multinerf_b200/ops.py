@@ -133,6 +133,55 @@ def encode(sdist, origins, directions, radii, near, far, basis, *, min_deg, max_
   return feat, f32, tdist
 
 
+def encode_points(points, var, basis, *, min_deg, max_deg, warp_contract=False, disable_integration=False,
+                  feat=None, feat_cols=None, want_f32=False):
+  """Point form of `encode`: features of the Gaussians (points[i], var * I) -> bf16 [N, ld] (+ fp32 [N, 2KL])."""
+  lib = L.load()
+  N = points.shape[0]
+  K = basis.shape[0]
+  F = 2 * K * (max_deg - min_deg)
+  if feat_cols is None:
+    feat_cols = (F + 63) // 64 * 64
+  if feat is None:
+    feat = torch.empty(N, feat_cols, device=points.device, dtype=torch.bfloat16)
+  assert feat.dtype == torch.bfloat16 and feat.stride(1) == 1
+  d = L.EncodeDesc(N, 1, 0, 0, int(warp_contract), int(disable_integration), K, min_deg, max_deg, feat.stride(0),
+                   feat_cols)
+  f32 = torch.empty(N, F, device=points.device) if want_f32 else None
+  _count()
+  L.check(lib.mnrf_encode_points(C.byref(d), L.ptr(_f32(points)), float(var), L.ptr(_f32(basis)), L.ptr(feat),
+                                 L.ptr(f32), L.stream_ptr()))
+  return feat, f32
+
+
+def marching_cubes(grid, level):
+  """Marching cubes on an fp32 grid [nz, ny, nx] (inside: value > level) -> (vertices [V, 3] fp32 in grid units
+  (x, y, z), faces [F, 3] int32).  Reads the two totals back once, between the count and emit phases."""
+  lib = L.load()
+  grid = _f32(grid)
+  assert grid.dim() == 3, 'grid must be [nz, ny, nx]'
+  nz, ny, nx = grid.shape
+  n = grid.numel()
+  dev = grid.device
+  edge_cut = torch.empty(3 * n, device=dev, dtype=torch.uint8)
+  cell_tris = torch.empty(n, device=dev, dtype=torch.uint8)
+  args = (nx, ny, nz, L.ptr(grid), float(level), L.ptr(edge_cut), L.ptr(cell_tris))
+  _count()
+  L.check(lib.mnrf_marching_cubes(L.MC_COUNT, *args, None, None, None, None, L.stream_ptr()))
+  edge_scan = torch.cumsum(edge_cut, 0, dtype=torch.int64)
+  tri_scan = torch.cumsum(cell_tris, 0, dtype=torch.int64)
+  V, F = (int(v) for v in torch.stack([edge_scan[-1], tri_scan[-1]]).cpu())
+  if V >= 2 ** 31:
+    raise ValueError(f'marching_cubes: {V} vertices do not fit the int32 face indices')
+  vertices = torch.empty(V, 3, device=dev)
+  faces = torch.empty(F, 3, device=dev, dtype=torch.int32)
+  if V:
+    _count()
+    L.check(lib.mnrf_marching_cubes(L.MC_EMIT, *args, L.ptr(edge_scan), L.ptr(tri_scan), L.ptr(vertices),
+                                    L.ptr(faces), L.stream_ptr()))
+  return vertices, faces
+
+
 def viewdir_enc(viewdirs, num_samples, deg, out, col0, col_end):
   lib = L.load()
   B = viewdirs.shape[0]

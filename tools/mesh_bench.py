@@ -1,0 +1,123 @@
+#!/usr/bin/env python
+"""Mesh extraction timings on one GPU (multinerf_b200/mesh.py), printed as one JSON line:
+
+  query:  Model.query_density rows/s over `--rows` random points (wall time around a synchronised window), and the
+          query GEMM launches' TFLOP/s over their CUDA-event kernel time, on the NerfMLPs of 360.gin (8 x 1024,
+          per-layer GEMMs) and blender_256.gin (8 x 256, the chained trunk), random init;
+  mc:     ops.marching_cubes (count, scans, one read-back of the totals, emit) at 256^3 and 512^3 on a sphere plus
+          smooth noise;
+  extract: mesh.extract_mesh end to end at --extract_res^3 on the 360.gin model (random init, level = the grid's
+          median density over a first, untimed extraction);
+  device: the card's name and power limit, read in the same run.
+
+  python tools/mesh_bench.py [--rows 8388608] [--extract_res 512] [--out result.json]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+from multinerf_b200 import configs, lib, mesh, models, ops  # noqa: E402
+
+
+def device_info():
+  q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
+                     capture_output=True, text=True)
+  return {'torch_name': torch.cuda.get_device_name(), 'nvidia_smi': q.stdout.strip().splitlines()[:1]}
+
+
+def timed(fn, reps):
+  torch.cuda.synchronize()
+  t0 = time.perf_counter()
+  for _ in range(reps):
+    out = fn()
+  torch.cuda.synchronize()
+  return (time.perf_counter() - t0) / reps, out
+
+
+def bench_query(bundle, rows, reps):
+  model = models.Model(bundle)
+  model.init(seed=0)
+  g = torch.Generator(device='cuda')
+  g.manual_seed(0)
+  pts = torch.rand(rows, 3, device='cuda', generator=g) * 3 - 1.5
+  var = (3.0 / 511) ** 2 / 12
+  model.query_density(pts, var)                      # warm-up: every chunk shape, plans, module loads
+  wall, _ = timed(lambda: model.query_density(pts, var), reps)
+  ops.GEMM_EVENTS = []
+  model.query_density(pts, var)
+  torch.cuda.synchronize()
+  ev, ops.GEMM_EVENTS = ops.GEMM_EVENTS, None
+  kern_s = sum(a.elapsed_time(b) for a, b, _ in ev) / 1e3
+  flops = sum(f for _, _, f in ev)
+  plan = model.plans['NerfMLP_0']
+  return {'rows': rows, 'chained': model._use_chain(plan, bundle.config.render_chunk_size *
+                                                     bundle.model.num_nerf_samples),
+          'wall_s': round(wall, 4), 'rows_per_s': round(rows / wall), 'gemm_launches': len(ev),
+          'gemm_kernel_s': round(kern_s, 4), 'gemm_tflops': round(flops / kern_s / 1e12, 1),
+          'gemm_share_of_wall': round(kern_s / wall, 3), 'gemm_flop_per_row': flops / rows}
+
+
+def sphere_noise(n, seed=0):
+  g = torch.Generator(device='cuda')
+  g.manual_seed(seed)
+  ax = torch.linspace(-1, 1, n, device='cuda')
+  z, y, x = torch.meshgrid(ax, ax, ax, indexing='ij')
+  f = 0.7 - torch.sqrt(x * x + y * y + z * z)
+  k = torch.randn(8, 3, device='cuda', generator=g) * 6
+  ph = torch.rand(8, device='cuda', generator=g) * 6.283
+  for i in range(8):
+    f += 0.03 * torch.cos(k[i, 0] * x + k[i, 1] * y + k[i, 2] * z + ph[i])
+  return f.contiguous()
+
+
+def bench_mc(n, reps):
+  grid = sphere_noise(n)
+  ops.marching_cubes(grid, 0.0)
+  t, (v, f) = timed(lambda: ops.marching_cubes(grid, 0.0), reps)
+  return {'grid': n, 's': round(t, 4), 'vertices': int(v.shape[0]), 'faces': int(f.shape[0])}
+
+
+def main():
+  ap = argparse.ArgumentParser()
+  ap.add_argument('--rows', type=int, default=1 << 23)
+  ap.add_argument('--reps', type=int, default=3)
+  ap.add_argument('--extract_res', type=int, default=512)
+  ap.add_argument('--out', default=None)
+  args = ap.parse_args()
+  lib.require_device()
+  res = {'device': device_info(), 'query': {}, 'mc': [], 'extract': None}
+  for name, make in (('360', configs.bundle_360), ('blender_256', configs.bundle_blender_256)):
+    res['query'][name] = bench_query(make(), args.rows, args.reps)
+    torch.cuda.empty_cache()
+  for n in (256, 512):
+    res['mc'].append(bench_mc(n, args.reps))
+    torch.cuda.empty_cache()
+  b = configs.bundle_360()
+  model = models.Model(b)
+  model.init(seed=0)
+  bbox = mesh.default_bbox(b)
+  grid, _ = mesh.density_grid(model, bbox, args.extract_res)
+  level = float(grid.median())
+  del grid
+  torch.cuda.empty_cache()
+  t, (v, f) = timed(lambda: mesh.extract_mesh(model, bbox, args.extract_res, level), 1)
+  res['extract'] = {'config': '360.gin NerfMLP, random init', 'grid': args.extract_res, 'level': level,
+                    's': round(t, 3), 'vertices': int(v.shape[0]), 'faces': int(f.shape[0])}
+  res['device_after'] = device_info()
+  line = json.dumps(res)
+  print(line, flush=True)
+  if args.out:
+    with open(args.out, 'w') as fh:
+      fh.write(line + '\n')
+
+
+if __name__ == '__main__':
+  main()
