@@ -289,6 +289,8 @@ int mnrf_mlp_chain_max_layers(void);
  *   MNRF_ACT_SOFTPLUS | MNRF_ACT_SILU  a'(z[m, k]), z [M, ldz] bf16 the pre-activation of the layer that produced X
  *                                      (mnrf_gemm FWD); needs dx, ldz a multiple of 8 and z 16-byte aligned
  * z is refused with any other act.
+ * x (and dx) are read (written) in 16-byte chunks: both launches need them 16-byte aligned, with pitches that are
+ * multiples of 8.  The forward needs w 16-byte aligned too; the backward takes any w.
  */
 int mnrf_head_fwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx,
                   const mnrf_bf16* w, const float* b, float* raw, mnrf_stream stream);
@@ -297,7 +299,31 @@ int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64
                   int32_t act, const mnrf_bf16* z, int64_t ldz, float* dw, float* dw2, int32_t dw_split,
                   float* db, float* dxsum, int32_t dx_cols, mnrf_bf16* dx2, int64_t lddx2, mnrf_stream stream);
 
-/* Column sums of a bf16 matrix into fp32 (bias gradients): out[N] += sum_m x[m, :]. */
+/* The kernel instances and launch shapes mnrf_head_fwd and mnrf_head_bwd choose for these arguments (the ones the
+ * choice depends on; x, w, z and dx take their places in the launches).  Host-only: no pointer is dereferenced and
+ * nothing is launched.  Returns nonzero, with the backward launch's error message, for arguments mnrf_head_bwd
+ * refuses; fwd_kernel is MNRF_HEAD_NONE where mnrf_head_fwd alone refuses them (w not 16-byte aligned). */
+enum { MNRF_HEAD_NONE = 0, MNRF_HEAD_FWD_SUB = 1, MNRF_HEAD_FWD_WARP = 2, MNRF_HEAD_BWD_SUB = 3,
+       MNRF_HEAD_BWD_WARP = 4 };
+typedef struct {
+  int32_t fwd_kernel;         /* MNRF_HEAD_FWD_SUB (head_fwd_sub_kernel) or MNRF_HEAD_FWD_WARP (head_fwd_kernel) */
+  int32_t fwd_lpr;            /* sub kernel: lanes per row, K / 8 (32, 16 or 8); 0 otherwise */
+  int32_t fwd_grid;           /* blocks */
+  int32_t bwd_kernel;         /* MNRF_HEAD_BWD_SUB (head_bwd_sub_kernel) or MNRF_HEAD_BWD_WARP (head_bwd_kernel) */
+  int32_t bwd_n_out;          /* template N_OUT */
+  int32_t bwd_lpr;            /* sub kernel: lanes per row, K / 8; 0 otherwise */
+  int32_t bwd_chunks;         /* warp-per-row kernel: kMaxChunks, 16-byte chunks per lane (1, 2, 4 or 6); 0 otherwise */
+  int32_t bwd_smooth;         /* SMOOTH template flag: dx *= a'(z) */
+  int32_t bwd_grid;           /* blocks */
+  int32_t reserved;
+  int64_t fwd_rows_per_pass;  /* rows one block covers per pass of its grid-stride loop */
+  int64_t bwd_rows_per_block; /* rows of each block's range (the last block's may be shorter) */
+} mnrf_head_instance;
+int mnrf_head_plan(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, const mnrf_bf16* w, int32_t act,
+                   const mnrf_bf16* z, const mnrf_bf16* dx, mnrf_head_instance* plan);
+
+/* Column sums of a bf16 matrix into fp32 (bias gradients): out[N] += sum_m x[m, :].  x 16-byte aligned, N and ldx
+ * multiples of 8. */
 int mnrf_colsum(int64_t m, int32_t n, const mnrf_bf16* x, int64_t ldx, float* out,
                 mnrf_stream stream);
 

@@ -472,6 +472,60 @@ clip_adam_kernel(mnrf_adam_desc d, float* __restrict__ p, const float* __restric
   }
 }
 
+// The launch choices of mnrf_head_fwd / mnrf_head_bwd after their argument checks (mnrf_head_plan reports them).
+static void head_fwd_plan(int64_t m, int k, mnrf_head_instance* p) {
+  if (k == 256 || k == 128 || k == 64) {
+    // rows of one / half / a quarter of a warp's 16-byte chunks: 4 independent loads in flight per lane
+    p->fwd_kernel = MNRF_HEAD_FWD_SUB;
+    p->fwd_lpr = k / 8;
+    p->fwd_rows_per_pass = 8 * (256 / k) * 4;
+  } else {
+    p->fwd_kernel = MNRF_HEAD_FWD_WARP;
+    p->fwd_lpr = 0;
+    p->fwd_rows_per_pass = 8;
+  }
+  p->fwd_grid = (int)std::min<int64_t>((m + p->fwd_rows_per_pass - 1) / p->fwd_rows_per_pass,
+                                       (int64_t)mnrf_num_sms() * 8);
+}
+
+static void head_bwd_plan(int64_t m, int k, int n_out, const mnrf_bf16* w, bool smooth, mnrf_head_instance* p) {
+  p->bwd_n_out = n_out;
+  p->bwd_smooth = smooth;
+  if ((k == 256 || k == 128 || k == 64) && ((uintptr_t)w % 16) == 0) {
+    // rows of one / half / a quarter of a warp's 16-byte chunks (see head_bwd_sub_kernel)
+    // every block ends with n_out*K + K global atomics on the same addresses: two blocks per SM keep enough loads
+    // in flight (8 warps x 4 x 512 B each) without serialising the flush
+    p->bwd_kernel = MNRF_HEAD_BWD_SUB;
+    p->bwd_lpr = k / 8;
+    p->bwd_chunks = 0;
+    p->bwd_grid = (int)std::min<int64_t>((m + 511) / 512, (int64_t)mnrf_num_sms() * 2);
+    p->bwd_rows_per_block = ((m + p->bwd_grid - 1) / p->bwd_grid + 7) / 8 * 8;
+    return;
+  }
+  const int chunks = (k / 8 + 31) / 32;
+  p->bwd_kernel = MNRF_HEAD_BWD_WARP;
+  p->bwd_lpr = 0;
+  p->bwd_chunks = chunks <= 1 ? 1 : chunks <= 2 ? 2 : chunks <= 4 ? 4 : 6;
+  p->bwd_grid = (int)std::min<int64_t>((m + 7) / 8, (int64_t)mnrf_num_sms() * 4);
+  p->bwd_rows_per_block = (m + p->bwd_grid - 1) / p->bwd_grid;
+}
+
+// The checks of mnrf_head_bwd on the arguments mnrf_head_plan takes as well.
+static int head_bwd_check(int k, int n_out, const mnrf_bf16* x, const mnrf_bf16* w, int act, const mnrf_bf16* z,
+                          const mnrf_bf16* dx) {
+  MNRF_CHECK(x && w, "mnrf_head_bwd: null pointer");
+  MNRF_CHECK(n_out >= 1 && n_out <= kMaxHead, "mnrf_head_bwd: n_out %d not in [1,4]", n_out);
+  MNRF_CHECK(k % 8 == 0 && k <= 1536, "mnrf_head_bwd: K must be a multiple of 8 and <= 1536");
+  // both kernels read the rows of x, and write those of dx, in 16-byte chunks
+  MNRF_CHECK(((uintptr_t)x % 16) == 0 && ((uintptr_t)dx % 16) == 0, "mnrf_head_bwd: x and dx must be 16-byte aligned");
+  MNRF_CHECK(act >= MNRF_ACT_NONE && act <= MNRF_ACT_SILU, "mnrf_head_bwd: unknown act %d", act);
+  const bool smooth = act == MNRF_ACT_SOFTPLUS || act == MNRF_ACT_SILU;
+  MNRF_CHECK(smooth || !z, "mnrf_head_bwd: z is the pre-activation of a smooth activation, act %d is not one", act);
+  MNRF_CHECK(!smooth || (z && dx && ((uintptr_t)z % 16) == 0),
+             "mnrf_head_bwd: a smooth activation needs dx and a 16-byte aligned z");
+  return 0;
+}
+
 }  // namespace mnrf
 
 extern "C" int mnrf_head_fwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, int64_t ldx,
@@ -482,21 +536,18 @@ extern "C" int mnrf_head_fwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf1
   MNRF_CHECK(n_out >= 1 && n_out <= kMaxHead, "mnrf_head_fwd: n_out %d not in [1,4]", n_out);
   MNRF_CHECK(k % 8 == 0 && ldx % 8 == 0 && ((uintptr_t)x % 16) == 0 && ((uintptr_t)w % 16) == 0,
              "mnrf_head_fwd: K/ld must be multiples of 8 and pointers 16-byte aligned");
-  if (m == 0) return 0;
-  if (k == 256 || k == 128 || k == 64) {
-    // rows of one / half / a quarter of a warp's 16-byte chunks: 4 independent loads in flight per lane
-    const int rows_per_block = 8 * (256 / k) * 4;
-    const int blocks = (int)std::min<int64_t>((m + rows_per_block - 1) / rows_per_block, (int64_t)mnrf_num_sms() * 8);
+  mnrf_head_instance p = {};
+  head_fwd_plan(m, k, &p);
+  if (p.fwd_kernel == MNRF_HEAD_FWD_SUB) {
 #define MNRF_HFS(LPR_)                                                                                 \
-  head_fwd_sub_kernel<LPR_, 4><<<blocks, 256, 0, (cudaStream_t)stream>>>(                               \
+  head_fwd_sub_kernel<LPR_, 4><<<p.fwd_grid, 256, 0, (cudaStream_t)stream>>>(                           \
       m, n_out, reinterpret_cast<const __nv_bfloat16*>(x), ldx, reinterpret_cast<const __nv_bfloat16*>(w), b, raw)
-    if (k == 256) MNRF_HFS(32); else if (k == 128) MNRF_HFS(16); else MNRF_HFS(8);
+    if (p.fwd_lpr == 32) MNRF_HFS(32); else if (p.fwd_lpr == 16) MNRF_HFS(16); else MNRF_HFS(8);
     MNRF_LAUNCH_CHECK();
     return 0;
   }
   size_t smem = (size_t)n_out * k * 2;
-  int blocks = (int)std::min<int64_t>((m + 7) / 8, (int64_t)mnrf_num_sms() * 8);
-  head_fwd_kernel<<<blocks, 256, smem, (cudaStream_t)stream>>>(
+  head_fwd_kernel<<<p.fwd_grid, 256, smem, (cudaStream_t)stream>>>(
       m, k, n_out, reinterpret_cast<const __nv_bfloat16*>(x), ldx,
       reinterpret_cast<const __nv_bfloat16*>(w), b, raw);
   MNRF_LAUNCH_CHECK();
@@ -510,40 +561,33 @@ extern "C" int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf1
   using namespace mnrf;
   const __nv_bfloat16* z = reinterpret_cast<const __nv_bfloat16*>(z_);
   if (m == 0) return 0;
-  MNRF_CHECK(x && w && draw, "mnrf_head_bwd: null pointer");
+  MNRF_CHECK(draw, "mnrf_head_bwd: null pointer");
+  if (int rc = head_bwd_check(k, n_out, x, w, act, z_, dx)) return rc;
   MNRF_CHECK(!dxsum || dx, "mnrf_head_bwd: dxsum needs dx");
-  MNRF_CHECK(n_out >= 1 && n_out <= kMaxHead, "mnrf_head_bwd: n_out %d not in [1,4]", n_out);
-  MNRF_CHECK(k % 8 == 0 && k <= 1536 && ldx % 8 == 0 && (!dx || lddx % 8 == 0),
-             "mnrf_head_bwd: K must be a multiple of 8 and <= 1536");
+  MNRF_CHECK(ldx % 8 == 0 && (!dx || lddx % 8 == 0), "mnrf_head_bwd: the pitches of x and dx must be multiples of 8");
   if (dw_split <= 0 || dw_split >= n_out) dw_split = n_out;
   if (dx_cols <= 0) dx_cols = k;
   MNRF_CHECK(dx_cols <= k && dx_cols % 8 == 0, "mnrf_head_bwd: dx_cols must be a multiple of 8 and <= K");
   MNRF_CHECK(!dx2 || (dx_cols < k && lddx2 % 8 == 0 && ((uintptr_t)dx2 % 16) == 0),
              "mnrf_head_bwd: dx2 needs dx_cols < K, a pitch that is a multiple of 8 and a 16-byte aligned pointer");
   MNRF_CHECK(dw_split == n_out || (dw && dw2), "mnrf_head_bwd: a split weight gradient needs dw and dw2");
-  MNRF_CHECK(act >= MNRF_ACT_NONE && act <= MNRF_ACT_SILU, "mnrf_head_bwd: unknown act %d", act);
   const bool smooth = act == MNRF_ACT_SOFTPLUS || act == MNRF_ACT_SILU;
-  MNRF_CHECK(smooth || !z, "mnrf_head_bwd: z is the pre-activation of a smooth activation, act %d is not one", act);
-  MNRF_CHECK(!smooth || (z && dx && ldz % 8 == 0 && ((uintptr_t)z % 16) == 0),
-             "mnrf_head_bwd: a smooth activation needs dx and a 16-byte aligned z with a pitch that is a multiple of 8");
+  MNRF_CHECK(!smooth || ldz % 8 == 0, "mnrf_head_bwd: the pitch of z must be a multiple of 8");
   // the kernels take the ReLU mask as a flag of its own and `act` for the smooth derivative only
   const int32_t relu_mask = act == MNRF_ACT_RELU;
   if (!smooth) act = MNRF_ACT_NONE;
-  if (m == 0) return 0;
-  if ((k == 256 || k == 128 || k == 64) && ((uintptr_t)w % 16) == 0) {
-    // rows of one / half / a quarter of a warp's 16-byte chunks (see head_bwd_sub_kernel)
-    // every block ends with n_out*K + K global atomics on the same addresses: two blocks per SM keep enough loads
-    // in flight (8 warps x 4 x 512 B each) without serialising the flush
-    const int blocks_s = (int)std::min<int64_t>((m + 511) / 512, (int64_t)mnrf_num_sms() * 2);
-    const int64_t rpb_s = ((m + blocks_s - 1) / blocks_s + 7) / 8 * 8;
+  mnrf_head_instance p = {};
+  head_bwd_plan(m, k, n_out, w, smooth, &p);
+  const int64_t rpb = p.bwd_rows_per_block;
+  if (p.bwd_kernel == MNRF_HEAD_BWD_SUB) {
 #define MNRF_HBS2(NO, LPR_, SM_)                                                                        \
-  head_bwd_sub_kernel<NO, LPR_, 4, SM_><<<blocks_s, 256, 0, (cudaStream_t)stream>>>(                    \
+  head_bwd_sub_kernel<NO, LPR_, 4, SM_><<<p.bwd_grid, 256, 0, (cudaStream_t)stream>>>(                  \
       m, reinterpret_cast<const __nv_bfloat16*>(x), ldx, reinterpret_cast<const __nv_bfloat16*>(w), draw, \
       reinterpret_cast<__nv_bfloat16*>(dx), lddx, relu_mask, dw, dw2, dw_split, db, dxsum, dx_cols,      \
-      reinterpret_cast<__nv_bfloat16*>(dx2), lddx2, rpb_s, act, z, ldz)
-#define MNRF_HBS(NO, LPR_) do { if (z) MNRF_HBS2(NO, LPR_, true); else MNRF_HBS2(NO, LPR_, false); } while (0)
-#define MNRF_HBS_N(NO) do { if (k == 256) MNRF_HBS(NO, 32); else if (k == 128) MNRF_HBS(NO, 16); else MNRF_HBS(NO, 8); } while (0)
-    switch (n_out) {
+      reinterpret_cast<__nv_bfloat16*>(dx2), lddx2, rpb, act, z, ldz)
+#define MNRF_HBS(NO, LPR_) do { if (p.bwd_smooth) MNRF_HBS2(NO, LPR_, true); else MNRF_HBS2(NO, LPR_, false); } while (0)
+#define MNRF_HBS_N(NO) do { if (p.bwd_lpr == 32) MNRF_HBS(NO, 32); else if (p.bwd_lpr == 16) MNRF_HBS(NO, 16); else MNRF_HBS(NO, 8); } while (0)
+    switch (p.bwd_n_out) {
       case 1: MNRF_HBS_N(1); break;
       case 2: MNRF_HBS_N(2); break;
       case 3: MNRF_HBS_N(3); break;
@@ -554,23 +598,20 @@ extern "C" int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf1
   }
   size_t smem = (size_t)n_out * k * (4 + 2);
   MNRF_CHECK(smem <= 48 * 1024, "mnrf_head_bwd: n_out*K too large for the shared-memory staging");
-  int blocks = (int)std::min<int64_t>((m + 7) / 8, (int64_t)mnrf_num_sms() * 4);
-  int64_t rpb = (m + blocks - 1) / blocks;
-  const int chunks = (k / 8 + 31) / 32;
 #define MNRF_HB2(NO, CK, SM_)                                                                   \
-  head_bwd_kernel<NO, CK, SM_><<<blocks, 256, smem, (cudaStream_t)stream>>>(                    \
+  head_bwd_kernel<NO, CK, SM_><<<p.bwd_grid, 256, smem, (cudaStream_t)stream>>>(                \
       m, k, reinterpret_cast<const __nv_bfloat16*>(x), ldx, reinterpret_cast<const __nv_bfloat16*>(w), \
       draw, reinterpret_cast<__nv_bfloat16*>(dx), lddx, relu_mask, dw, dw2, dw_split, db, dxsum, dx_cols, \
       reinterpret_cast<__nv_bfloat16*>(dx2), lddx2, rpb, act, z, ldz)
-#define MNRF_HB(NO, CK) do { if (z) MNRF_HB2(NO, CK, true); else MNRF_HB2(NO, CK, false); } while (0)
+#define MNRF_HB(NO, CK) do { if (p.bwd_smooth) MNRF_HB2(NO, CK, true); else MNRF_HB2(NO, CK, false); } while (0)
 #define MNRF_HB_N(NO)                                      \
   do {                                                     \
-    if (chunks <= 1) MNRF_HB(NO, 1);                       \
-    else if (chunks <= 2) MNRF_HB(NO, 2);                  \
-    else if (chunks <= 4) MNRF_HB(NO, 4);                  \
+    if (p.bwd_chunks == 1) MNRF_HB(NO, 1);                 \
+    else if (p.bwd_chunks == 2) MNRF_HB(NO, 2);            \
+    else if (p.bwd_chunks == 4) MNRF_HB(NO, 4);            \
     else MNRF_HB(NO, 6);                                   \
   } while (0)
-  switch (n_out) {
+  switch (p.bwd_n_out) {
     case 1: MNRF_HB_N(1); break;
     case 2: MNRF_HB_N(2); break;
     case 3: MNRF_HB_N(3); break;
@@ -580,13 +621,25 @@ extern "C" int mnrf_head_bwd(int64_t m, int32_t k, int32_t n_out, const mnrf_bf1
   return 0;
 }
 
+extern "C" int mnrf_head_plan(int64_t m, int32_t k, int32_t n_out, const mnrf_bf16* x, const mnrf_bf16* w,
+                              int32_t act, const mnrf_bf16* z, const mnrf_bf16* dx, mnrf_head_instance* plan) {
+  using namespace mnrf;
+  MNRF_CHECK(plan, "mnrf_head_plan: null pointer");
+  MNRF_CHECK(m > 0, "mnrf_head_plan: m must be positive (an empty launch runs no kernel)");
+  if (int rc = head_bwd_check(k, n_out, x, w, act, z, dx)) return rc;
+  *plan = mnrf_head_instance{};
+  if (((uintptr_t)w % 16) == 0) head_fwd_plan(m, k, plan);
+  head_bwd_plan(m, k, n_out, w, act == MNRF_ACT_SOFTPLUS || act == MNRF_ACT_SILU, plan);
+  return 0;
+}
+
 extern "C" int mnrf_colsum(int64_t m, int32_t n, const mnrf_bf16* x, int64_t ldx, float* out,
                            mnrf_stream stream) {
   using namespace mnrf;
   if (m == 0) return 0;
   MNRF_CHECK(x && out, "mnrf_colsum: null pointer");
-  MNRF_CHECK(n % 8 == 0 && ldx % 8 == 0, "mnrf_colsum: N and ld must be multiples of 8");
-  if (m == 0) return 0;
+  MNRF_CHECK(n % 8 == 0 && ldx % 8 == 0 && ((uintptr_t)x % 16) == 0,
+             "mnrf_colsum: N and ld must be multiples of 8 and x 16-byte aligned");
   const int threads = 128;
   dim3 grid;
   grid.y = (n / 8 + threads - 1) / threads;

@@ -46,6 +46,13 @@ class GemmInstance(C.Structure):
               ('pingpong', C.c_int32)]
 
 
+class HeadInstance(C.Structure):
+  _fields_ = [('fwd_kernel', C.c_int32), ('fwd_lpr', C.c_int32), ('fwd_grid', C.c_int32), ('bwd_kernel', C.c_int32),
+              ('bwd_n_out', C.c_int32), ('bwd_lpr', C.c_int32), ('bwd_chunks', C.c_int32), ('bwd_smooth', C.c_int32),
+              ('bwd_grid', C.c_int32), ('reserved', C.c_int32), ('fwd_rows_per_pass', C.c_int64),
+              ('bwd_rows_per_block', C.c_int64)]
+
+
 class CompositeDesc(C.Structure):
   _fields_ = [('num_rays', C.c_int32), ('num_samples', C.c_int32), ('raydist_fn', C.c_int32),
               ('opaque_background', C.c_int32), ('density_bias', C.c_float),
@@ -144,6 +151,8 @@ _SIGNATURES = {
     'mnrf_head_fwd': (C.c_int, [C.c_int64, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P, _P, _P]),
     'mnrf_head_bwd': (C.c_int, [C.c_int64, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P, _P, C.c_int64, C.c_int32,
                                 _P, C.c_int64, _P, _P, C.c_int32, _P, _P, C.c_int32, _P, C.c_int64, _P]),
+    # the plan is written to a host HeadInstance, passed by reference (ops.head_plan)
+    'mnrf_head_plan': (C.c_int, [C.c_int64, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P, _P, _P]),
     'mnrf_colsum': (C.c_int, [C.c_int64, C.c_int32, _P, C.c_int64, _P, _P]),
     'mnrf_composite_fwd': (C.c_int, [C.POINTER(CompositeDesc)] + [_P] * 18),
     'mnrf_composite_bwd': (C.c_int, [C.POINTER(LossDesc)] + [_P] * 24 + [C.c_int32, _P]),
@@ -166,6 +175,7 @@ _SIGNATURES = {
     'mnrf_marching_cubes': (C.c_int, [C.c_int32] * 4 + [_P, C.c_float] + [_P] * 7),
 }
 MC_COUNT, MC_EMIT = 0, 1
+HEAD_NONE, HEAD_FWD_SUB, HEAD_FWD_WARP, HEAD_BWD_SUB, HEAD_BWD_WARP = 0, 1, 2, 3, 4
 EXPORTED = tuple(_SIGNATURES)
 
 _lib = None

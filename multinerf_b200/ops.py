@@ -318,6 +318,18 @@ def head_bwd(x, w_nk, draw, n_out, k, dx=None, relu_mask=False, dw=None, db=None
                             L.stream_ptr()))
 
 
+def head_plan(x, w_nk, n_out, k, *, act=L.ACT_NONE, z=None, dx=None):
+  """The kernel instances and launch shapes head_fwd and head_bwd run for these arguments (M = x.shape[0]): a dict
+  of the fields of mnrf_head_instance (include/mnrf.h).  Reads only shapes and addresses, so the tensors may live
+  on any device; raises MnrfError where head_bwd refuses the arguments."""
+  lib = L.load()
+  def p(t):
+    return None if t is None else C.c_void_p(t.data_ptr())
+  plan = L.HeadInstance()
+  L.check(lib.mnrf_head_plan(x.shape[0], k, n_out, p(x), p(w_nk), act, p(z), p(dx), C.byref(plan)))
+  return {name: int(getattr(plan, name)) for name, _ in L.HeadInstance._fields_}
+
+
 def colsum(x, n, out):
   lib = L.load()
   _count()

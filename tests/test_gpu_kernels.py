@@ -258,111 +258,6 @@ def test_gemm_wgrad_side_sums(ops, impl, R, Mo, N):
   close(o4, x.float().T @ dy.float(), atol=2e-3 * math.sqrt(R), rtol=1e-4, msg='strided x')
 
 
-def test_heads_and_colsum(ops):
-  rng = np.random.default_rng(5)
-  for M, K, n_out in [(1000, 1024, 1), (777, 128, 3), (300, 256, 4), (515, 64, 2), (4099, 256, 1), (1, 128, 3),
-                      (70001, 128, 3), (333, 192, 2)]:
-    x = _bf(rng.normal(size=(M, K)).astype(np.float32))
-    w = _bf(rng.normal(size=(n_out, K)).astype(np.float32) / math.sqrt(K))
-    b = torch.tensor(rng.normal(size=(n_out,)).astype(np.float32))
-    raw = ops.head_fwd(x.cuda(), w.cuda(), b.cuda(), n_out, K)
-    close(raw, x.float() @ w.float().T + b, atol=1e-4, rtol=1e-4, msg='head fwd')
-    draw = torch.tensor(rng.normal(size=(M, n_out)).astype(np.float32))
-    dx = torch.empty(M, K, dtype=torch.bfloat16, device='cuda')
-    dw = torch.zeros(K, n_out, device='cuda')
-    db = torch.zeros(n_out, device='cuda')
-    dxsum = torch.ones(K, device='cuda')
-    ops.head_bwd(x.cuda(), w.cuda(), draw.cuda(), n_out, K, dx=dx, relu_mask=True, dw=dw, db=db, dxsum=dxsum)
-    ref_dx = (draw @ w.float()) * (x.float() > 0)
-    close(dxsum, ref_dx.sum(0) + 1.0, atol=2e-3 * math.sqrt(M), rtol=1e-4, msg='head dxsum')
-    close(dx.float(), ref_dx.to(torch.bfloat16).float(), atol=1e-2, rtol=1e-2, msg='head dx')
-    close(dw, x.float().T @ draw, atol=2e-3 * math.sqrt(M / 1000 + 1), rtol=1e-4, msg='head dw')
-    close(db, draw.sum(0), atol=1e-3 * math.sqrt(M / 1000 + 1), rtol=1e-4, msg='head db')
-    # parameter gradients only (no dx): the form the Ref-NeRF heads and the chained PropMLP's tangent pass use
-    dw2 = torch.zeros(K, n_out, device='cuda')
-    db2 = torch.zeros(n_out, device='cuda')
-    ops.head_bwd(x.cuda(), w.cuda(), draw.cuda(), n_out, K, dx=None, dw=dw2, db=db2)
-    close(dw2, x.float().T @ draw, atol=2e-3 * math.sqrt(M / 1000 + 1), rtol=1e-4, msg='head dw (no dx)')
-    close(db2, draw.sum(0), atol=1e-3 * math.sqrt(M / 1000 + 1), rtol=1e-4, msg='head db (no dx)')
-  x = _bf(rng.normal(size=(5000, 256)).astype(np.float32))
-  out = torch.zeros(256, device='cuda')
-  ops.colsum(x.cuda(), 256, out)
-  close(out, x.float().sum(0), atol=2e-2, rtol=1e-4, msg='colsum')
-
-
-def test_pack_weights_batched_and_adam(ops):
-  from oracle import o_train
-  rng = np.random.default_rng(9)
-  master = torch.tensor(rng.normal(size=(320, 128)).astype(np.float32))
-  w_nk = torch.empty(128, 320, dtype=torch.bfloat16, device='cuda')
-  w_kn = torch.empty(320, 128, dtype=torch.bfloat16, device='cuda')
-  ops.pack_weights_batched(ops.pack_table([(master.cuda(), w_nk, w_kn)], 'cuda'))      # one layer
-  assert torch.equal(w_kn.cpu(), master.to(torch.bfloat16))
-  assert torch.equal(w_nk.cpu(), master.T.contiguous().to(torch.bfloat16))
-  w_kn.fill_(7.0)
-  ops.pack_weights_batched(ops.pack_table([(master.cuda(), None, w_kn)], 'cuda'))      # without the w_nk copy
-  assert torch.equal(w_kn.cpu(), master.to(torch.bfloat16))
-  # all layers of a module in one launch (ragged shapes, an item without the w_kn copy)
-  shapes = [(320, 128), (64, 3), (100, 257), (512, 256), (33, 1)]
-  masters = [torch.tensor(rng.normal(size=sh).astype(np.float32)).cuda() for sh in shapes]
-  nks = [torch.full((o, i), 7.0, dtype=torch.bfloat16, device='cuda') for i, o in shapes]
-  kns = [None if j == 1 else torch.full((i, o), 7.0, dtype=torch.bfloat16, device='cuda') for j, (i, o) in enumerate(shapes)]
-  table = ops.pack_table(list(zip(masters, nks, kns)), 'cuda')
-  ops.pack_weights_batched(table)
-  torch.cuda.synchronize()
-  for mst, nk, kn in zip(masters, nks, kns):
-    assert torch.equal(nk, mst.T.contiguous().to(torch.bfloat16))
-    if kn is not None:
-      assert torch.equal(kn, mst.to(torch.bfloat16))
-
-  class Cfg:
-    adam_beta1, adam_beta2, adam_eps = 0.9, 0.999, 1e-6
-  n = 100003
-  p = torch.tensor(rng.normal(size=n).astype(np.float32))
-  g = torch.tensor(rng.normal(size=n).astype(np.float32) * 1e-3)
-  g[5] = float('nan')
-  m = torch.tensor(rng.normal(size=n).astype(np.float32) * 1e-4)
-  v = torch.tensor(rng.uniform(size=n).astype(np.float32) * 1e-8)
-  gc = g.clone()
-  norm = torch.sqrt((gc ** 2).nansum())
-  # reference semantics: norm includes NaN -> mult NaN -> nan_to_num -> 0 everywhere; test the
-  # finite case for values and the NaN case for "no NaN reaches the parameters"
-  gf = torch.nan_to_num(gc)
-  mult = torch.clamp(1e-3 / (o_train.EPS + torch.sqrt((gf ** 2).sum())), max=1.0)
-  p_ref, m_ref, v_ref = o_train.adam_update(p, mult * gf, m, v, 6, 1.5e-3, Cfg)
-  pc, mc, vc = p.cuda(), m.cuda(), v.cuda()
-  scratch = torch.zeros(1, device='cuda')
-  ops.clip_adam(pc, gf.cuda(), mc, vc, scratch, step=7, lr=1.5e-3, beta1=0.9, beta2=0.999, eps=1e-6,
-                grad_max_val=0.0, grad_max_norm=1e-3)
-  close(pc, p_ref, atol=1e-7, rtol=1e-5, msg='adam p')
-  close(mc, m_ref, atol=1e-9, rtol=1e-5, msg='adam m')
-  close(vc, v_ref, atol=1e-14, rtol=1e-5, msg='adam v')
-  pc2 = p.cuda()
-  ops.clip_adam(pc2, g.cuda(), m.cuda(), v.cuda(), scratch, step=7, lr=1.5e-3, beta1=0.9, beta2=0.999,
-                eps=1e-6, grad_max_val=0.0, grad_max_norm=1e-3)
-  assert torch.isfinite(pc2).all()
-  # Reference order (train_utils.py:200-218 then :328): value clip -> norm clip -> nan_to_num.  jnp.clip and
-  # jnp.minimum propagate NaN, so one NaN makes the module's mult NaN and the WHOLE module's gradient 0:
-  # Adam then sees g = 0 everywhere (moments decay, parameters move by the momentum term only).
-  zero = torch.zeros(n)
-  for max_val in (0.0, 0.1):
-    p_z, m_z, v_z = o_train.adam_update(p, zero, m, v, 6, 1.5e-3, Cfg)
-    pc3, mc3, vc3 = p.cuda(), m.cuda(), v.cuda()
-    ops.clip_adam(pc3, g.cuda(), mc3, vc3, scratch, step=7, lr=1.5e-3, beta1=0.9, beta2=0.999, eps=1e-6,
-                  grad_max_val=max_val, grad_max_norm=1e-3)
-    close(pc3, p_z, atol=1e-7, rtol=1e-5, msg='adam p after a NaN gradient (module update zeroed)')
-    close(mc3, m_z, atol=1e-9, rtol=1e-5, msg='adam m after a NaN gradient')
-  # without norm clipping only the NaN element itself is zeroed (nan_to_num), also under a value clip
-  g2 = g.clone()
-  gf2 = torch.nan_to_num(g2).clamp(-1e-3, 1e-3)
-  p_r, m_r, _ = o_train.adam_update(p, gf2, m, v, 6, 1.5e-3, Cfg)
-  pc4, mc4 = p.cuda(), m.cuda()
-  ops.clip_adam(pc4, g2.cuda(), mc4, v.cuda(), scratch, step=7, lr=1.5e-3, beta1=0.9, beta2=0.999, eps=1e-6,
-                grad_max_val=1e-3, grad_max_norm=0.0)
-  close(mc4, m_r, atol=1e-9, rtol=1e-5, msg='adam m, value clip with a NaN element')
-  assert float(mc4[5]) == float(0.9 * m[5])          # NaN -> 0, not -grad_max_val
-
-
 def test_composite_diffuse_specular_mode(ops):
   """rgb_mode 1 (Ref-NeRF, models.py:588-602): value and gradients vs oracle autograd."""
   from oracle import o_train
