@@ -501,29 +501,11 @@ extern "C" int mnrf_mlp_chain(const mnrf_chain_desc* d, mnrf_stream stream_) {
   if (d->head_w) MNRF_CHECK(d->mode == MNRF_CHAIN_FWD && d->head_out && ((uintptr_t)d->head_w % 16) == 0,
                             "mnrf_mlp_chain: the head is a forward output (16-byte aligned weights)");
   MNRF_CHECK(head_n == 1 || (head_n == 4 && d->head_w), "mnrf_mlp_chain: head_n must be 1 or 4, got %d", head_n);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)std::min<int64_t>(p.num_units, sms)); cfg.blockDim = dim3(CH_THREADS);
-  cfg.dynamicSmemBytes = CH_SMEM; cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  if (d->mode == MNRF_CHAIN_FWD && head_n == 4) {
-    static bool set4 = false;
-    auto kern = mlp_chain_kernel<0, 4>;
-    if (!set4) { MNRF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, CH_SMEM)); set4 = true; }
-    MNRF_CUDA(cudaLaunchKernelEx(&cfg, kern, maps, p));
-  } else if (d->mode == MNRF_CHAIN_FWD) {
-    static bool set0 = false;
-    auto kern = mlp_chain_kernel<0, 1>;
-    if (!set0) { MNRF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, CH_SMEM)); set0 = true; }
-    MNRF_CUDA(cudaLaunchKernelEx(&cfg, kern, maps, p));
-  } else {
-    static bool set1 = false;
-    auto kern = mlp_chain_kernel<1, 1>;
-    if (!set1) { MNRF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, CH_SMEM)); set1 = true; }
-    MNRF_CUDA(cudaLaunchKernelEx(&cfg, kern, maps, p));
-  }
+  const int grid = (int)std::min<int64_t>(p.num_units, sms);
+  const int rc = d->mode == MNRF_CHAIN_BWD ? launch_tc<mlp_chain_kernel<1, 1>>(grid, CH_THREADS, CH_SMEM, stream, maps, p)
+                 : head_n == 4             ? launch_tc<mlp_chain_kernel<0, 4>>(grid, CH_THREADS, CH_SMEM, stream, maps, p)
+                                           : launch_tc<mlp_chain_kernel<0, 1>>(grid, CH_THREADS, CH_SMEM, stream, maps, p);
+  if (rc) return rc;
   MNRF_LAUNCH_CHECK();
   return 0;
 }

@@ -81,6 +81,19 @@ struct GemmParams {
   void* out;
 };
 
+// Work item `tile` of the persistent loop: its column block, row block and the k-blocks [kb0, kb1) of its split
+struct Tile {
+  int n_blk, m_blk, kb0, kb1;
+};
+__device__ __forceinline__ Tile decode_tile(const GemmParams& p, int tile) {
+  const int n_blk = tile % p.num_n_blocks;
+  const int rest = tile / p.num_n_blocks;
+  const int m_blk = rest % p.num_m_blocks;
+  const int split = rest / p.num_m_blocks;
+  const int kb0 = split * p.kblocks_per_split;
+  return {n_blk, m_blk, kb0, min(p.num_k_blocks, kb0 + p.kblocks_per_split)};
+}
+
 // WGRAD side sums of one operand, run by NT threads of the producer warpgroup (t = 0..NT-1) beside the consumers:
 //   B (WEIGHTED = false): out = bsum,    out[n_blk * BN + col]  += sum_r B[r, col]
 //   A (WEIGHTED = true):  out = side_aw, out[m_blk * 128 + col] += sum_r side_w[r] A[r, col]
@@ -108,12 +121,7 @@ __device__ __forceinline__ void wgrad_side_sums(const GemmParams& p, int t, uint
   const int step = every * G;                        // row stride of a thread
   uint32_t slot = 0;                                 // k-blocks consumed: stage slot % STAGES
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-    const int n_blk = tile % p.num_n_blocks;
-    const int rest = tile / p.num_n_blocks;
-    const int m_blk = rest % p.num_m_blocks;
-    const int split = rest / p.num_m_blocks;
-    const int kb0 = split * p.kblocks_per_split;
-    const int kb1 = min(p.num_k_blocks, kb0 + p.kblocks_per_split);
+    const auto [n_blk, m_blk, kb0, kb1] = decode_tile(p, tile);
     const int own = WEIGHTED ? n_blk : m_blk;        // first row of each k-block this tile sums
     float acc[8];
 #pragma unroll
@@ -169,8 +177,162 @@ __device__ __forceinline__ void wgrad_side_sums(const GemmParams& p, int t, uint
   }
 }
 
-// Accumulator fragment of wgmma m64nBN (per consumer thread): acc[4i + 2h + e] is row 16*warp + lane/4 + 8h,
-// column 8i + 2*(lane%4) + e of the warpgroup's 64 x BN tile.
+// The FWD / DGRAD epilogue of one consumer warpgroup, from the accumulator fragment of wgmma m64nNC (per thread:
+// acc[4i + 2h + e] is row 16*warp + lane/4 + 8h, column 8i + 2*(lane%4) + e of the warpgroup's 64 x NC block):
+// FWD bias, then ReLU and mask bits or a smooth a(z) | DGRAD rank-1 term, mask bits (from the TMA-loaded mask block
+// at m_tile if mask_tma, else from global memory), bf16 mask or a'(z), addend and, if do_cs, column sums into the
+// warp's shared-memory slice at cs_lane.  The block is rows [r0, r0 + 64) of the 128-row tile m_blk and columns
+// [ncol0, ncol0 + NC); warpgroup wg (0 or 1) owns named barrier 2 + wg and staging blocks [wg * SB, wg * SB + SB).
+// TS: the bf16 output goes through a ring of SB (1 or 2) staging blocks of [64 rows x 64 cols], one TMA bulk store
+// per 64 columns; else it is stored from registers.
+template <int MODE, int NC, bool TS, int SB, bool SMOOTH>
+__device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const CUtensorMap* tmap_c, const float (&acc)[NC / 2],
+                                              int m_blk, int r0, int ncol0, int wg, uint8_t* smem_c, bool mask_tma,
+                                              uint32_t m_tile, bool do_cs, uint32_t cs_lane) {
+  constexpr int MW = mask_words(NC);
+  const int lane = threadIdx.x & 31;
+  const int r_in = r0 + (16 * ((threadIdx.x >> 5) & 3) + (lane >> 2));   // this thread's row (h = 0) in the tile
+  const int cq = 2 * (lane & 3);
+  const bool leader = (threadIdx.x & 127) == 0;   // TS: issues and waits on the warpgroup's bulk stores
+  // TS: this thread's row (h = 0) in the warpgroup's first staging block
+  const uint32_t c_row = smem_u32(smem_c) + wg * (SB * STAGING_BLOCK_BYTES) + (r_in - r0) * 128 + (cq << 1);
+  const uint32_t m_row = m_tile + r_in * (MW * 4);
+  int64_t rows[2];
+  bool row_ok[2];
+  float rv[2] = {0.f, 0.f};
+  const uint32_t* mrow[2] = {nullptr, nullptr};
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    rows[h] = (int64_t)m_blk * BLOCK_M + r_in + 8 * h;
+    row_ok[h] = rows[h] < p.m;
+    if (MODE == MNRF_GEMM_DGRAD && row_ok[h]) {
+      if (p.rowv) rv[h] = p.rowv[rows[h]];
+      if (p.maskbits && !mask_tma)
+        mrow[h] = p.maskbits + (p.mask_mod > 0 ? rows[h] % p.mask_mod : rows[h]) * p.ldmaskbits;
+    }
+  }
+  uint32_t bits[2] = {0u, 0u};
+  uint32_t mw[2] = {0u, 0u};                    // DGRAD mask bits: the rows' words of the current 32 columns
+#pragma unroll
+  for (int i = 0; i < NC / 8; ++i) {
+    const int col = ncol0 + 8 * i + cq;
+    if (TS && SB == 1 && (i & 7) == 0) {
+      // the previous bulk store must have finished reading the staging block
+      if (leader) tma_store_wait_read<0>();
+      named_bar_sync(2 + wg, 128);
+    }
+    if (MODE == MNRF_GEMM_DGRAD && p.maskbits && (i & 3) == 0) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        mw[h] = mask_tma ? ld_shared_u32(m_row + (8 * h * MW + (i >> 2)) * 4)
+                         : row_ok[h] ? __ldg(mrow[h] + (col >> 5)) : 0u;
+    }
+    float v[2][2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) { v[h][0] = acc[4 * i + 2 * h]; v[h][1] = acc[4 * i + 2 * h + 1]; }
+    if (MODE == MNRF_GEMM_FWD) {
+      if (p.bias) {
+        const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) { v[h][0] += b.x; v[h][1] += b.y; }
+      }
+      if constexpr (SMOOTH) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (p.mask && row_ok[h])
+            *reinterpret_cast<uint32_t*>(const_cast<__nv_bfloat16*>(p.mask) + rows[h] * p.ldmask + col) =
+                pack_bf16(v[h][0], v[h][1]);
+          v[h][0] = act_fwd(p.act, v[h][0]);
+          v[h][1] = act_fwd(p.act, v[h][1]);
+        }
+      } else if (p.act == MNRF_ACT_RELU) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            v[h][e] = fmaxf(v[h][e], 0.f);
+            bits[h] |= (v[h][e] > 0.f ? 1u : 0u) << ((8 * i + cq + e) & 31);
+          }
+      }
+    } else {
+      float2 cv = make_float2(0.f, 0.f);
+      if (p.rowv) cv = __ldg(reinterpret_cast<const float2*>(p.colv + col));
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (p.rowv) { v[h][0] += rv[h] * cv.x; v[h][1] += rv[h] * cv.y; }
+        if constexpr (SMOOTH) {
+          if (row_ok[h]) {
+            const int64_t zr = p.mask_mod > 0 ? rows[h] % p.mask_mod : rows[h];
+            const uint32_t zz = __ldg(reinterpret_cast<const unsigned int*>(p.mask + zr * p.ldmask + col));
+            v[h][0] *= act_d1(p.act, bf16_lo(zz));
+            v[h][1] *= act_d1(p.act, bf16_hi(zz));
+          }
+        } else if (p.maskbits) {
+          if (!((mw[h] >> (col & 31)) & 1u)) v[h][0] = 0.f;
+          if (!((mw[h] >> ((col + 1) & 31)) & 1u)) v[h][1] = 0.f;
+        } else if (p.mask && row_ok[h]) {
+          const uint32_t mm = __ldg(reinterpret_cast<const unsigned int*>(p.mask + rows[h] * p.ldmask + col));
+          if (!(bf16_lo(mm) > 0.f)) v[h][0] = 0.f;
+          if (!(bf16_hi(mm) > 0.f)) v[h][1] = 0.f;
+        }
+        if (p.addend && row_ok[h]) {
+          const uint32_t aa = __ldg(reinterpret_cast<const unsigned int*>(p.addend + rows[h] * p.ldadd + col));
+          v[h][0] += bf16_lo(aa);
+          v[h][1] += bf16_hi(aa);
+        }
+      }
+      if (do_cs) {
+        // column sums over the warp's 16 rows (rows past M hold zeros: zero-filled A tile, rv = 0).  The first
+        // butterfly step swaps halves: lane bit 2 keeps column col + bit 2, so the two columns share the
+        // remaining steps and one slice word.  Each sum is added in the same pairwise order as a butterfly per
+        // column.  Lanes 0-7 own 8 distinct words of the warp's own slice: a plain load and store.
+        const bool hi = (lane >> 2) & 1;
+        const float s0 = v[0][0] + v[1][0], s1 = v[0][1] + v[1][1];
+        float t = (hi ? s1 : s0) + __shfl_xor_sync(0xffffffffu, hi ? s0 : s1, 4);
+        t += __shfl_xor_sync(0xffffffffu, t, 8);
+        t += __shfl_xor_sync(0xffffffffu, t, 16);
+        if (lane < 8) {
+          const uint32_t a = cs_lane + 8 * i * 4;
+          st_shared_u32(a, __float_as_uint(__uint_as_float(ld_shared_u32(a)) + t));
+        }
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (TS) {
+        // staging block (i / 8) % SB, row r_in - r0 + 8h, 16-byte chunk (i % 8) ^ (row % 8), byte 2 * cq
+        st_shared_u32(c_row + ((i >> 3) & (SB - 1)) * STAGING_BLOCK_BYTES + h * (8 * 128) +
+                          (((i & 7) ^ ((lane >> 2) & 7)) << 4),
+                      pack_bf16(v[h][0], v[h][1]));
+      } else if (row_ok[h]) {
+        *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + rows[h] * p.ldc + col) =
+            pack_bf16(v[h][0], v[h][1]);
+      }
+    }
+    if (MODE == MNRF_GEMM_FWD && p.act == MNRF_ACT_RELU && p.maskbits && (i & 3) == 3) {
+      // one 32-column mask word per row: the four lanes of a quad hold its 32 bits between them
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        bits[h] |= __shfl_xor_sync(0xffffffffu, bits[h], 1);
+        bits[h] |= __shfl_xor_sync(0xffffffffu, bits[h], 2);
+        if ((lane & 3) == ((i >> 2) & 3) && row_ok[h]) p.maskbits[rows[h] * p.ldmaskbits + (col >> 5)] = bits[h];
+        bits[h] = 0u;
+      }
+    }
+    if (TS && (i & 7) == 7) {
+      fence_proxy_async();                      // generic-proxy writes -> visible to the bulk store (async proxy)
+      // SB = 2: the store of the previous block, in the staging block that the next block overwrites, has been read
+      if (SB == 2 && leader) tma_store_wait_read<0>();
+      named_bar_sync(2 + wg, 128);
+      if (leader) {                             // TMA clips the rows past M
+        tma_store_2d(tmap_c, smem_c + (wg * SB + ((i >> 3) & (SB - 1))) * STAGING_BLOCK_BYTES, ncol0 + 8 * (i & ~7),
+                     (int)((int64_t)m_blk * BLOCK_M + r0));
+        tma_store_commit();
+      }
+    }
+  }
+}
+
 // SMOOTH: the epilogue of a softplus / SiLU layer (p.act): FWD stores z and applies a(z), DGRAD multiplies by a'(z)
 // where the ReLU instances handle mask bits.  Separate instances, so the ReLU ones keep their code.
 template <int MODE, int BN, bool TS, bool SIDE, bool SMOOTH = false>
@@ -240,12 +402,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       const uint32_t stage_bytes = A_STAGE_BYTES + B_STAGE;
       uint32_t stage = 0, phase = 0;
       for (int tile = blockIdx.x, it = 0; tile < total_tiles; tile += gridDim.x, ++it) {
-        const int n_blk = tile % p.num_n_blocks;
-        const int rest = tile / p.num_n_blocks;
-        const int m_blk = rest % p.num_m_blocks;
-        const int split = rest / p.num_m_blocks;
-        const int kb0 = split * p.kblocks_per_split;
-        const int kb1 = min(p.num_k_blocks, kb0 + p.kblocks_per_split);
+        const auto [n_blk, m_blk, kb0, kb1] = decode_tile(p, tile);
         if (mask_tma) {
           // the tile's [128 rows x MW words] of mask bits; with mask_mod (a multiple of 128) the tile's rows map to
           // 128 consecutive mask rows.  Rows past the end are zero-filled.
@@ -304,12 +461,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     // DGRAD: this warp's column-sum slice, at the column pair of lanes 0-7 after the butterfly below
     const uint32_t cs_lane = smem_u32(cs_s) + ((warp - 4) * BN + cq + ((lane >> 2) & 1)) * 4;
     for (int tile = blockIdx.x, it = 0; tile < total_tiles; tile += gridDim.x, ++it) {
-      const int n_blk = tile % p.num_n_blocks;
-      const int rest = tile / p.num_n_blocks;
-      const int m_blk = rest % p.num_m_blocks;
-      const int split = rest / p.num_m_blocks;
-      const int kb0 = split * p.kblocks_per_split;
-      const int kb1 = min(p.num_k_blocks, kb0 + p.kblocks_per_split);
+      const auto [n_blk, m_blk, kb0, kb1] = decode_tile(p, tile);
       int prev = -1;
       fence_acc(acc);
       for (int kb = kb0; kb < kb1; ++kb) {
@@ -351,147 +503,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         }
         continue;
       }
-      const bool leader = (threadIdx.x & 127) == 0;   // TS: issues and waits on the warpgroup's bulk stores
-      // TS: this thread's row (h = 0) in the warpgroup's first staging block
-      const uint32_t c_row = smem_u32(smem_c) + c * (SB * STAGING_BLOCK_BYTES) + (r_in - 64 * c) * 128 + (cq << 1);
-      int64_t rows[2];
-      bool row_ok[2];
-      float rv[2] = {0.f, 0.f};
-      const uint32_t* mrow[2] = {nullptr, nullptr};
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        rows[h] = (int64_t)m_blk * BLOCK_M + r_in + 8 * h;
-        row_ok[h] = rows[h] < p.m;
-        if (MODE == MNRF_GEMM_DGRAD && row_ok[h]) {
-          if (p.rowv) rv[h] = p.rowv[rows[h]];
-          if (p.maskbits && !mask_tma)
-            mrow[h] = p.maskbits + (p.mask_mod > 0 ? rows[h] % p.mask_mod : rows[h]) * p.ldmaskbits;
-        }
-      }
-      // mask_tma: this thread's row (h = 0) of the tile's mask block, once the producer's load has landed
-      const uint32_t m_row = smem_u32(mask_s) + ((it % MASK_BUFS) * BLOCK_M + r_in) * (MW * 4);
       if (mask_tma) mbar_wait(&mask_full[it % MASK_BUFS], (it / MASK_BUFS) & 1, 5);
-      uint32_t bits[2] = {0u, 0u};
-      uint32_t mw[2] = {0u, 0u};                // DGRAD mask bits: the rows' words of the current 32 columns
-#pragma unroll
-      for (int i = 0; i < BN / 8; ++i) {
-        const int col = ncol0 + 8 * i + cq;
-        if (TS && SB == 1 && (i & 7) == 0) {
-          // the previous bulk store must have finished reading the staging block
-          if (leader) tma_store_wait_read<0>();
-          named_bar_sync(2 + c, 128);
-        }
-        if (MODE == MNRF_GEMM_DGRAD && p.maskbits && (i & 3) == 0) {
-#pragma unroll
-          for (int h = 0; h < 2; ++h)
-            mw[h] = mask_tma ? ld_shared_u32(m_row + (8 * h * MW + (i >> 2)) * 4)
-                             : row_ok[h] ? __ldg(mrow[h] + (col >> 5)) : 0u;
-        }
-        float v[2][2];
-#pragma unroll
-        for (int h = 0; h < 2; ++h) { v[h][0] = acc[4 * i + 2 * h]; v[h][1] = acc[4 * i + 2 * h + 1]; }
-        if (MODE == MNRF_GEMM_FWD) {
-          if (p.bias) {
-            const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-#pragma unroll
-            for (int h = 0; h < 2; ++h) { v[h][0] += b.x; v[h][1] += b.y; }
-          }
-          if constexpr (SMOOTH) {
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              if (p.mask && row_ok[h])
-                *reinterpret_cast<uint32_t*>(const_cast<__nv_bfloat16*>(p.mask) + rows[h] * p.ldmask + col) =
-                    pack_bf16(v[h][0], v[h][1]);
-              v[h][0] = act_fwd(p.act, v[h][0]);
-              v[h][1] = act_fwd(p.act, v[h][1]);
-            }
-          } else if (p.act == MNRF_ACT_RELU) {
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                v[h][e] = fmaxf(v[h][e], 0.f);
-                bits[h] |= (v[h][e] > 0.f ? 1u : 0u) << ((8 * i + cq + e) & 31);
-              }
-          }
-        } else {
-          float2 cv = make_float2(0.f, 0.f);
-          if (p.rowv) cv = __ldg(reinterpret_cast<const float2*>(p.colv + col));
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            if (p.rowv) { v[h][0] += rv[h] * cv.x; v[h][1] += rv[h] * cv.y; }
-            if constexpr (SMOOTH) {
-              if (row_ok[h]) {
-                const int64_t zr = p.mask_mod > 0 ? rows[h] % p.mask_mod : rows[h];
-                const uint32_t zz = __ldg(reinterpret_cast<const unsigned int*>(p.mask + zr * p.ldmask + col));
-                v[h][0] *= act_d1(p.act, bf16_lo(zz));
-                v[h][1] *= act_d1(p.act, bf16_hi(zz));
-              }
-            } else if (p.maskbits) {
-              if (!((mw[h] >> (col & 31)) & 1u)) v[h][0] = 0.f;
-              if (!((mw[h] >> ((col + 1) & 31)) & 1u)) v[h][1] = 0.f;
-            } else if (p.mask && row_ok[h]) {
-              const uint32_t mm = __ldg(reinterpret_cast<const unsigned int*>(p.mask + rows[h] * p.ldmask + col));
-              if (!(bf16_lo(mm) > 0.f)) v[h][0] = 0.f;
-              if (!(bf16_hi(mm) > 0.f)) v[h][1] = 0.f;
-            }
-            if (p.addend && row_ok[h]) {
-              const uint32_t aa = __ldg(reinterpret_cast<const unsigned int*>(p.addend + rows[h] * p.ldadd + col));
-              v[h][0] += bf16_lo(aa);
-              v[h][1] += bf16_hi(aa);
-            }
-          }
-          if (do_cs) {
-            // column sums over the warp's 16 rows (rows past M hold zeros: zero-filled A tile, rv = 0).  The first
-            // butterfly step swaps halves: lane bit 2 keeps column col + bit 2, so the two columns share the
-            // remaining steps and one slice word.  Each sum is added in the same pairwise order as a butterfly per
-            // column.  Lanes 0-7 own 8 distinct words of the warp's own slice: a plain load and store.
-            const bool hi = (lane >> 2) & 1;
-            const float s0 = v[0][0] + v[1][0], s1 = v[0][1] + v[1][1];
-            float t = (hi ? s1 : s0) + __shfl_xor_sync(0xffffffffu, hi ? s0 : s1, 4);
-            t += __shfl_xor_sync(0xffffffffu, t, 8);
-            t += __shfl_xor_sync(0xffffffffu, t, 16);
-            if (lane < 8) {
-              const uint32_t a = cs_lane + 8 * i * 4;
-              st_shared_u32(a, __float_as_uint(__uint_as_float(ld_shared_u32(a)) + t));
-            }
-          }
-        }
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (TS) {
-            // staging block (i / 8) % SB (SB is 1 or 2), row r_in - 64c + 8h, 16-byte chunk (i % 8) ^ (row % 8),
-            // byte 2 * cq
-            st_shared_u32(c_row + ((i >> 3) & (SB - 1)) * STAGING_BLOCK_BYTES + h * (8 * 128) +
-                              (((i & 7) ^ ((lane >> 2) & 7)) << 4),
-                          pack_bf16(v[h][0], v[h][1]));
-          } else if (row_ok[h]) {
-            *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + rows[h] * p.ldc + col) =
-                pack_bf16(v[h][0], v[h][1]);
-          }
-        }
-        if (MODE == MNRF_GEMM_FWD && p.act == MNRF_ACT_RELU && p.maskbits && (i & 3) == 3) {
-          // one 32-column mask word per row: the four lanes of a quad hold its 32 bits between them
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            bits[h] |= __shfl_xor_sync(0xffffffffu, bits[h], 1);
-            bits[h] |= __shfl_xor_sync(0xffffffffu, bits[h], 2);
-            if ((lane & 3) == ((i >> 2) & 3) && row_ok[h]) p.maskbits[rows[h] * p.ldmaskbits + (col >> 5)] = bits[h];
-            bits[h] = 0u;
-          }
-        }
-        if (TS && (i & 7) == 7) {
-          fence_proxy_async();                  // generic-proxy writes -> visible to the bulk store (async proxy)
-          // SB = 2: the store of the previous block, in the staging block that the next block overwrites, has been read
-          if (SB == 2 && leader) tma_store_wait_read<0>();
-          named_bar_sync(2 + c, 128);
-          if (leader) {                         // TMA clips the rows past M
-            tma_store_2d(&tmap_c, smem_c + (c * SB + ((i >> 3) & (SB - 1))) * STAGING_BLOCK_BYTES, ncol0 + 8 * (i & ~7),
-                         (int)((int64_t)m_blk * BLOCK_M + 64 * c));
-            tma_store_commit();
-          }
-        }
-      }
+      gemm_epilogue<MODE, BN, TS, SB, SMOOTH>(p, &tmap_c, acc, m_blk, 64 * c, ncol0, c, smem_c, mask_tma,
+                                              smem_u32(mask_s) + (it % MASK_BUFS) * (BLOCK_M * MW * 4), do_cs, cs_lane);
       if (mask_tma) {                           // this warp has read its mask words: the buffer may be refilled
         __syncwarp();
         if (lane == 0) mbar_arrive(&mask_empty[it % MASK_BUFS]);
@@ -564,7 +578,6 @@ gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
   uint64_t* mask_empty = mask_full + PP_MASK_BUFS;                               // [PP_MASK_BUFS]
   uint64_t* mma_turn = mask_empty + PP_MASK_BUFS;                               // [2]: warpgroup c may issue
 
-  const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int wg = threadIdx.x >> 7;
   const int total_tiles = p.num_m_blocks * p.num_n_blocks;
@@ -626,11 +639,6 @@ gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
     // ===================== consumers: warpgroup c runs sub-tiles it = c, c + 2, ... =====================
     setmaxnreg_inc<232>();
     const int c = wg - 1;
-    const int w = warp & 3;
-    const int cq = 2 * (lane & 3);
-    const bool leader = (threadIdx.x & 127) == 0;   // issues and waits on the warpgroup's bulk stores
-    // this thread's row (h = 0) in the warpgroup's first staging block
-    const uint32_t c_row = smem_u32(smem_c) + c * (SB * STAGING_BLOCK_BYTES) + (16 * w + (lane >> 2)) * 128 + (cq << 1);
     float acc[2][64];
     for (int it = c; ; it += 2) {                // sub-tile it: column block it % SUB of the CTA's tile it / SUB
       const int tile = blockIdx.x + (it / SUB) * (int)gridDim.x;
@@ -683,100 +691,8 @@ gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
       if (mask_tma) mbar_wait(&mask_full[it % PP_MASK_BUFS], (it / PP_MASK_BUFS) & 1, 5);
 #pragma unroll 1
       for (int g = 0; g < 2; ++g) {
-        const int r_in = 64 * g + 16 * w + (lane >> 2);
-        int64_t rows[2];
-        bool row_ok[2];
-        float rv[2] = {0.f, 0.f};
-        const uint32_t* mrow[2] = {nullptr, nullptr};
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          rows[h] = (int64_t)m_blk * BLOCK_M + r_in + 8 * h;
-          row_ok[h] = rows[h] < p.m;
-          if (kDgrad && row_ok[h]) {
-            if (p.rowv) rv[h] = p.rowv[rows[h]];
-            if (p.maskbits && !mask_tma)
-              mrow[h] = p.maskbits + (p.mask_mod > 0 ? rows[h] % p.mask_mod : rows[h]) * p.ldmaskbits;
-          }
-        }
-        const uint32_t m_row = m_base + r_in * (MW * 4);
-        uint32_t bits[2] = {0u, 0u};
-        uint32_t mw[2] = {0u, 0u};              // DGRAD mask bits: the rows' words of the current 32 columns
-#pragma unroll
-        for (int i = 0; i < PP_BN / 8; ++i) {
-          const int col = ncol0 + 8 * i + cq;
-          if (kDgrad && p.maskbits && (i & 3) == 0) {
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-              mw[h] = mask_tma ? ld_shared_u32(m_row + (8 * h * MW + (i >> 2)) * 4)
-                               : row_ok[h] ? __ldg(mrow[h] + (col >> 5)) : 0u;
-          }
-          float v[2][2];
-#pragma unroll
-          for (int h = 0; h < 2; ++h) { v[h][0] = acc[0][4 * i + 2 * h]; v[h][1] = acc[0][4 * i + 2 * h + 1]; }
-          if (!kDgrad) {
-            if (p.bias) {
-              const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-#pragma unroll
-              for (int h = 0; h < 2; ++h) { v[h][0] += b.x; v[h][1] += b.y; }
-            }
-            if (p.act == MNRF_ACT_RELU) {
-#pragma unroll
-              for (int h = 0; h < 2; ++h)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                  v[h][e] = fmaxf(v[h][e], 0.f);
-                  bits[h] |= (v[h][e] > 0.f ? 1u : 0u) << ((8 * i + cq + e) & 31);
-                }
-            }
-          } else {
-            float2 cv = make_float2(0.f, 0.f);
-            if (p.rowv) cv = __ldg(reinterpret_cast<const float2*>(p.colv + col));
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              if (p.rowv) { v[h][0] += rv[h] * cv.x; v[h][1] += rv[h] * cv.y; }
-              if (p.maskbits) {
-                if (!((mw[h] >> (col & 31)) & 1u)) v[h][0] = 0.f;
-                if (!((mw[h] >> ((col + 1) & 31)) & 1u)) v[h][1] = 0.f;
-              } else if (p.mask && row_ok[h]) {
-                const uint32_t mm = __ldg(reinterpret_cast<const unsigned int*>(p.mask + rows[h] * p.ldmask + col));
-                if (!(bf16_lo(mm) > 0.f)) v[h][0] = 0.f;
-                if (!(bf16_hi(mm) > 0.f)) v[h][1] = 0.f;
-              }
-              if (p.addend && row_ok[h]) {
-                const uint32_t aa = __ldg(reinterpret_cast<const unsigned int*>(p.addend + rows[h] * p.ldadd + col));
-                v[h][0] += bf16_lo(aa);
-                v[h][1] += bf16_hi(aa);
-              }
-            }
-          }
-          // staging block (i / 8) % SB, row 16 w + lane / 4 + 8h, 16-byte chunk (i % 8) ^ (row % 8), byte 2 * cq
-#pragma unroll
-          for (int h = 0; h < 2; ++h)
-            st_shared_u32(c_row + ((i >> 3) & (SB - 1)) * STAGING_BLOCK_BYTES + h * (8 * 128) +
-                              (((i & 7) ^ ((lane >> 2) & 7)) << 4),
-                          pack_bf16(v[h][0], v[h][1]));
-          if (!kDgrad && p.act == MNRF_ACT_RELU && p.maskbits && (i & 3) == 3) {
-            // one 32-column mask word per row: the four lanes of a quad hold its 32 bits between them
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              bits[h] |= __shfl_xor_sync(0xffffffffu, bits[h], 1);
-              bits[h] |= __shfl_xor_sync(0xffffffffu, bits[h], 2);
-              if ((lane & 3) == ((i >> 2) & 3) && row_ok[h]) p.maskbits[rows[h] * p.ldmaskbits + (col >> 5)] = bits[h];
-              bits[h] = 0u;
-            }
-          }
-          if ((i & 7) == 7) {
-            fence_proxy_async();                // generic-proxy writes -> visible to the bulk store (async proxy)
-            // the store of the previous block, in the staging block that the next block overwrites, has been read
-            if (leader) tma_store_wait_read<0>();
-            named_bar_sync(2 + c, 128);
-            if (leader) {                       // TMA clips the rows past M
-              tma_store_2d(&tmap_c, smem_c + (c * SB + ((i >> 3) & (SB - 1))) * STAGING_BLOCK_BYTES,
-                           ncol0 + 8 * (i & ~7), (int)((int64_t)m_blk * BLOCK_M + 64 * g));
-              tma_store_commit();
-            }
-          }
-        }
+        gemm_epilogue<MODE, PP_BN, true, SB, false>(p, &tmap_c, acc[0], m_blk, 64 * g, ncol0, c, smem_c, mask_tma, m_base,
+                                                    false, 0);
 #pragma unroll
         for (int e = 0; e < 64; ++e) acc[0][e] = acc[1][e];   // rows [64, 128) next
       }
@@ -793,45 +709,17 @@ gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
 template <int MODE, int BN>
 static int launch_gemm_tc_pingpong(int grid, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
                                    const CUtensorMap& tm, const GemmParams& p, cudaStream_t stream) {
-  static bool attr_set = false;
   constexpr int kSmem = pp_smem_bytes(MODE);
   static_assert(kSmem <= 232448, "shared memory budget");
-  auto kern = gemm_tc_pingpong_kernel<MODE, BN>;
-  if (!attr_set) {
-    MNRF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
-    attr_set = true;
-  }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = kSmem; cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  MNRF_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, tc, tm, p));
-  return 0;
+  return launch_tc<gemm_tc_pingpong_kernel<MODE, BN>>(grid, NUM_THREADS, kSmem, stream, ta, tb, tc, tm, p);
 }
 
-template <int MODE, int BN, bool TS, bool SIDE, bool SMOOTH>
+template <int MODE, int BN, bool TS, bool SIDE, bool SMOOTH = false>
 static int launch_gemm_tc(int grid, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
                           const CUtensorMap& tm, const GemmParams& p, cudaStream_t stream) {
-  static bool attr_set = false;
   constexpr int kSmem = smem_bytes(MODE, BN, TS, SIDE);
   static_assert(kSmem <= 232448, "shared memory budget");
-  auto kern = gemm_tc_kernel<MODE, BN, TS, SIDE, SMOOTH>;
-  if (!attr_set) {
-    MNRF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
-    attr_set = true;
-  }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = kSmem; cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  MNRF_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, tc, tm, p));
-  return 0;
+  return launch_tc<gemm_tc_kernel<MODE, BN, TS, SIDE, SMOOTH>>(grid, NUM_THREADS, kSmem, stream, ta, tb, tc, tm, p);
 }
 
 // The SMOOTH instances are compiled in a translation unit of their own (gemm_tc_act.cu): instantiated beside the
@@ -848,11 +736,13 @@ static int pick_block_n(int n) {
 }
 
 // The host-side choices of gemm_tc_launch, after every argument check: tile width, store path, where DGRAD's mask
-// bits come from, instance family, reduction splits and grid.  Dereferences nothing (mnrf_gemm_plan).
+// bits come from, instance family, reduction splits and grid, and the tile counts of the launch parameters `p`.
+// Dereferences nothing (mnrf_gemm_plan).
 static int gemm_tc_plan(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
                         const float* colv, const mnrf_bf16* mask, const uint32_t* maskbits, const float* colsum,
                         const mnrf_bf16* addend, const void* out, const float* bsum, const float* side_w,
-                        const float* side_aw, const mnrf_bf16* z, int64_t ldz, mnrf_gemm_instance* plan) {
+                        const float* side_aw, const mnrf_bf16* z, int64_t ldz, mnrf_gemm_instance* plan,
+                        GemmParams* p) {
   // K-major modes: the reduction index is the contiguous one and layers are padded to 64.  WGRAD reduces
   // over the sample rows, any count: the last 64-row block is zero-filled by TMA past the tensor's end.
   MNRF_CHECK(d->mode == MNRF_GEMM_WGRAD || d->k % BLOCK_K == 0,
@@ -934,7 +824,70 @@ static int gemm_tc_plan(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_
   plan->tiles = tiles;
   plan->grid = std::min(tiles, workers);
   plan->pingpong = pingpong;
+  p->num_m_blocks = num_m_blocks;
+  p->num_n_blocks = num_n_blocks;
+  p->num_k_blocks = num_k_blocks;
+  p->num_splits = num_splits;
+  p->kblocks_per_split = kblocks_per_split;
   return 0;
+}
+
+// FWD / DGRAD through the register store, at every tile width
+template <int MODE>
+static int launch_register_store(int block_n, int grid, const CUtensorMap& ta, const CUtensorMap& tb,
+                                 const CUtensorMap& tc, const CUtensorMap& tm, const GemmParams& p,
+                                 cudaStream_t stream) {
+  switch (block_n) {
+    case 256: return launch_gemm_tc<MODE, 256, false, false>(grid, ta, tb, tc, tm, p, stream);
+    case 128: return launch_gemm_tc<MODE, 128, false, false>(grid, ta, tb, tc, tm, p, stream);
+    case 64: return launch_gemm_tc<MODE, 64, false, false>(grid, ta, tb, tc, tm, p, stream);
+    case 32: return launch_gemm_tc<MODE, 32, false, false>(grid, ta, tb, tc, tm, p, stream);
+    case 16: return launch_gemm_tc<MODE, 16, false, false>(grid, ta, tb, tc, tm, p, stream);
+  }
+  set_error("mnrf_gemm(tc): no register-store instance at BN=%d", block_n);
+  return 1;
+}
+
+// Launches the instance of a plan.  Only the combinations gemm_tc_plan produces have one: FWD and DGRAD with the
+// staged store at BN >= 128 run the ping-pong kernel unless the activation is smooth or DGRAD has column sums, and
+// WGRAD needs BN >= 64.
+static int launch_gemm_tc_plan(int mode, const mnrf_gemm_instance& plan, const CUtensorMap& ta, const CUtensorMap& tb,
+                               const CUtensorMap& tc, const CUtensorMap& tm, const GemmParams& p,
+                               cudaStream_t stream) {
+  const int bn = plan.block_n, grid = plan.grid;
+  const bool fwd = mode == MNRF_GEMM_FWD;
+  if (plan.pingpong) {
+    if (bn == 256)
+      return fwd ? launch_gemm_tc_pingpong<MNRF_GEMM_FWD, 256>(grid, ta, tb, tc, tm, p, stream)
+                 : launch_gemm_tc_pingpong<MNRF_GEMM_DGRAD, 256>(grid, ta, tb, tc, tm, p, stream);
+    if (bn == 128)
+      return fwd ? launch_gemm_tc_pingpong<MNRF_GEMM_FWD, 128>(grid, ta, tb, tc, tm, p, stream)
+                 : launch_gemm_tc_pingpong<MNRF_GEMM_DGRAD, 128>(grid, ta, tb, tc, tm, p, stream);
+  } else if (plan.smooth) {
+    return gemm_tc_smooth_launch(mode, bn, grid, ta, tb, tc, p, stream);
+  } else if (mode == MNRF_GEMM_WGRAD) {
+    if (bn == 256)
+      return plan.side ? launch_gemm_tc<MNRF_GEMM_WGRAD, 256, false, true>(grid, ta, tb, tc, tm, p, stream)
+                       : launch_gemm_tc<MNRF_GEMM_WGRAD, 256, false, false>(grid, ta, tb, tc, tm, p, stream);
+    if (bn == 128)
+      return plan.side ? launch_gemm_tc<MNRF_GEMM_WGRAD, 128, false, true>(grid, ta, tb, tc, tm, p, stream)
+                       : launch_gemm_tc<MNRF_GEMM_WGRAD, 128, false, false>(grid, ta, tb, tc, tm, p, stream);
+    if (bn == 64)
+      return plan.side ? launch_gemm_tc<MNRF_GEMM_WGRAD, 64, false, true>(grid, ta, tb, tc, tm, p, stream)
+                       : launch_gemm_tc<MNRF_GEMM_WGRAD, 64, false, false>(grid, ta, tb, tc, tm, p, stream);
+  } else if (!plan.staged) {
+    return fwd ? launch_register_store<MNRF_GEMM_FWD>(bn, grid, ta, tb, tc, tm, p, stream)
+               : launch_register_store<MNRF_GEMM_DGRAD>(bn, grid, ta, tb, tc, tm, p, stream);
+  } else if (bn == 64) {
+    return fwd ? launch_gemm_tc<MNRF_GEMM_FWD, 64, true, false>(grid, ta, tb, tc, tm, p, stream)
+               : launch_gemm_tc<MNRF_GEMM_DGRAD, 64, true, false>(grid, ta, tb, tc, tm, p, stream);
+  } else if (!fwd) {   // DGRAD with column sums
+    if (bn == 256) return launch_gemm_tc<MNRF_GEMM_DGRAD, 256, true, false>(grid, ta, tb, tc, tm, p, stream);
+    if (bn == 128) return launch_gemm_tc<MNRF_GEMM_DGRAD, 128, true, false>(grid, ta, tb, tc, tm, p, stream);
+  }
+  set_error("mnrf_gemm(tc): no kernel instance for mode %d, BN=%d, staged %d, side sums %d", mode, bn, plan.staged,
+            plan.side);
+  return 1;
 }
 
 int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
@@ -942,18 +895,13 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
                    float* colsum, const mnrf_bf16* addend, void* out, cudaStream_t stream, float* bsum,
                    const float* side_w, float* side_aw, mnrf_bf16* z, int64_t ldz) {
   mnrf_gemm_instance plan;
+  GemmParams p{};
   if (int rc = gemm_tc_plan(d, a, b, bias, colv, mask, maskbits, colsum, addend, out, bsum, side_w, side_aw, z, ldz,
-                            &plan))
+                            &plan, &p))
     return rc;
   const int block_n = plan.block_n;
-  const bool ts = plan.staged, side = plan.side, smooth = plan.smooth;
-  GemmParams p{};
+  const bool ts = plan.staged;
   p.mode = d->mode; p.act = d->act; p.m = d->m; p.n = d->n; p.k = d->k;
-  p.num_m_blocks = (int)((d->m + BLOCK_M - 1) / BLOCK_M);
-  p.num_n_blocks = d->n / block_n;
-  p.num_k_blocks = (d->k + BLOCK_K - 1) / BLOCK_K;
-  p.num_splits = plan.splits;
-  p.kblocks_per_split = (p.num_k_blocks + p.num_splits - 1) / p.num_splits;
   p.ldc = d->ldc; p.ldmask = d->ldmask;
   p.bias = bias; p.rowv = rowv; p.colv = colv;
   p.mask = reinterpret_cast<const __nv_bfloat16*>(mask);
@@ -965,7 +913,7 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
   p.ldadd = d->ldadd;
   p.colsum = colsum;
   p.bsum = bsum; p.side_w = side_w; p.side_aw = side_aw;
-  if (smooth) {
+  if (plan.smooth) {
     p.mask = reinterpret_cast<const __nv_bfloat16*>(z);
     p.ldmask = ldz;
   }
@@ -990,43 +938,8 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
                 mask_words(plan.pingpong ? PP_BN : block_n), BLOCK_M, CU_TENSOR_MAP_DATA_TYPE_UINT32, 4,
                 CU_TENSOR_MAP_SWIZZLE_NONE))
     return 1;
-  const int grid = plan.grid;
-  if (grid == 0) return 0;
-#define MNRF_LAUNCH_TC3(MODE_, BN_, TS_, SIDE_)                                                       \
-  do {                                                                                                \
-    if (int rc = launch_gemm_tc<MODE_, BN_, TS_, SIDE_, false>(grid, ta, tb, tc, tm, p, stream)) return rc; \
-  } while (0)
-#define MNRF_LAUNCH_TC2(MODE_, BN_)                                                                   \
-  do {                                                                                                \
-    if (side) MNRF_LAUNCH_TC3(MODE_, BN_, false, MODE_ == MNRF_GEMM_WGRAD && BN_ >= 64);              \
-    else if (ts) MNRF_LAUNCH_TC3(MODE_, BN_, MODE_ != MNRF_GEMM_WGRAD && BN_ >= 64, false);           \
-    else MNRF_LAUNCH_TC3(MODE_, BN_, false, false);                                                   \
-  } while (0)
-#define MNRF_LAUNCH_TC(MODE_)                                                                         \
-  do {                                                                                                \
-    switch (block_n) {                                                                                \
-      case 256: MNRF_LAUNCH_TC2(MODE_, 256); break;                                                   \
-      case 128: MNRF_LAUNCH_TC2(MODE_, 128); break;                                                   \
-      case 64: MNRF_LAUNCH_TC2(MODE_, 64); break;                                                     \
-      case 32: if (MODE_ != MNRF_GEMM_WGRAD) MNRF_LAUNCH_TC2(MODE_, 32); break;                       \
-      default: if (MODE_ != MNRF_GEMM_WGRAD) MNRF_LAUNCH_TC2(MODE_, 16); break;                       \
-    }                                                                                                 \
-  } while (0)
-  if (plan.pingpong) {
-    const bool fwd = d->mode == MNRF_GEMM_FWD;
-    int rc;
-    if (block_n == 256)
-      rc = fwd ? launch_gemm_tc_pingpong<MNRF_GEMM_FWD, 256>(grid, ta, tb, tc, tm, p, stream)
-               : launch_gemm_tc_pingpong<MNRF_GEMM_DGRAD, 256>(grid, ta, tb, tc, tm, p, stream);
-    else
-      rc = fwd ? launch_gemm_tc_pingpong<MNRF_GEMM_FWD, 128>(grid, ta, tb, tc, tm, p, stream)
-               : launch_gemm_tc_pingpong<MNRF_GEMM_DGRAD, 128>(grid, ta, tb, tc, tm, p, stream);
-    if (rc) return rc;
-  } else if (smooth) {
-    if (int rc = gemm_tc_smooth_launch(d->mode, block_n, grid, ta, tb, tc, p, stream)) return rc;
-  } else if (d->mode == MNRF_GEMM_FWD) MNRF_LAUNCH_TC(MNRF_GEMM_FWD);
-  else if (d->mode == MNRF_GEMM_DGRAD) MNRF_LAUNCH_TC(MNRF_GEMM_DGRAD);
-  else MNRF_LAUNCH_TC(MNRF_GEMM_WGRAD);
+  if (plan.grid == 0) return 0;
+  if (int rc = launch_gemm_tc_plan(d->mode, plan, ta, tb, tc, tm, p, stream)) return rc;
   MNRF_LAUNCH_CHECK();
   return 0;
 }
@@ -1043,7 +956,8 @@ extern "C" int mnrf_gemm_plan(const mnrf_gemm_desc* d, const mnrf_bf16* a, const
   MNRF_CHECK(d && plan, "mnrf_gemm_plan: null pointer");
   MNRF_CHECK((rowv == nullptr) == (colv == nullptr), "mnrf_gemm: rowv and colv come together");
   MNRF_CHECK(!mask || d->mask_mod == 0, "mnrf_gemm: mask_mod applies to maskbits and z, not to a bf16 mask");
+  mnrf::GemmParams p;
   return mnrf::gemm_tc_plan(d, a, b, bias, colv, mask, maskbits, colsum, addend, out, bsum, side_w, side_aw, z, ldz,
-                            plan);
+                            plan, &p);
 }
 #endif

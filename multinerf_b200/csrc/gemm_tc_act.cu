@@ -9,16 +9,20 @@ namespace mnrf {
 int gemm_tc_smooth_launch(int mode, int block_n, int grid, const CUtensorMap& ta, const CUtensorMap& tb,
                           const CUtensorMap& tc, const GemmParams& p, cudaStream_t stream) {
   // the staged bulk store (TS) only: gemm_tc_launch checked that the output allows it
-#define MNRF_LAUNCH_SMOOTH(MODE_, BN_) launch_gemm_tc<MODE_, BN_, true, false, true>(grid, ta, tb, tc, tb, p, stream)
-  if (mode == MNRF_GEMM_FWD) {
-    return block_n == 256   ? MNRF_LAUNCH_SMOOTH(MNRF_GEMM_FWD, 256)
-           : block_n == 128 ? MNRF_LAUNCH_SMOOTH(MNRF_GEMM_FWD, 128)
-                            : MNRF_LAUNCH_SMOOTH(MNRF_GEMM_FWD, 64);
+  const bool fwd = mode == MNRF_GEMM_FWD;
+  switch (block_n) {
+    case 256:
+      return fwd ? launch_gemm_tc<MNRF_GEMM_FWD, 256, true, false, true>(grid, ta, tb, tc, tb, p, stream)
+                 : launch_gemm_tc<MNRF_GEMM_DGRAD, 256, true, false, true>(grid, ta, tb, tc, tb, p, stream);
+    case 128:
+      return fwd ? launch_gemm_tc<MNRF_GEMM_FWD, 128, true, false, true>(grid, ta, tb, tc, tb, p, stream)
+                 : launch_gemm_tc<MNRF_GEMM_DGRAD, 128, true, false, true>(grid, ta, tb, tc, tb, p, stream);
+    case 64:
+      return fwd ? launch_gemm_tc<MNRF_GEMM_FWD, 64, true, false, true>(grid, ta, tb, tc, tb, p, stream)
+                 : launch_gemm_tc<MNRF_GEMM_DGRAD, 64, true, false, true>(grid, ta, tb, tc, tb, p, stream);
   }
-  return block_n == 256   ? MNRF_LAUNCH_SMOOTH(MNRF_GEMM_DGRAD, 256)
-         : block_n == 128 ? MNRF_LAUNCH_SMOOTH(MNRF_GEMM_DGRAD, 128)
-                          : MNRF_LAUNCH_SMOOTH(MNRF_GEMM_DGRAD, 64);
-#undef MNRF_LAUNCH_SMOOTH
+  set_error("mnrf_gemm(tc): no smooth-activation instance at BN=%d", block_n);
+  return 1;
 }
 
 }  // namespace mnrf

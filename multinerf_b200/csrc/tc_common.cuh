@@ -150,6 +150,26 @@ inline bool pdl_enabled() {
   return on;
 }
 
+// Launches Kernel<<<grid, block, smem, stream>>>(args...), as a programmatic dependent when pdl_enabled().  The
+// dynamic shared-memory limit is raised once per kernel: the flag is a template static, so there is one per Kernel.
+template <auto Kernel, class... Args>
+inline int launch_tc(int grid, int block, int smem, cudaStream_t stream, const Args&... args) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    MNRF_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    attr_set = true;
+  }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(block);
+  cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  MNRF_CUDA(cudaLaunchKernelEx(&cfg, Kernel, args...));
+  return 0;
+}
+
 inline EncodeTiledFn get_encode_fn() {
   static EncodeTiledFn fn = nullptr;
   if (fn) return fn;
