@@ -4,7 +4,8 @@
   python extract_mesh.py --gin_configs=configs/360.gin --gin_bindings="Config.checkpoint_dir = '...'" \
       --gin_bindings="Config.mesh_level = 10." --gin_bindings="Config.mesh_resolution = 512"
 Writes <checkpoint_dir>/mesh/mesh_step_<step>.ply (multinerf_b200/mesh.py; Config.mesh_bbox sets the box, and
-forward-facing scenes must set it).  One process on one GPU.
+forward-facing scenes must set it; Config.mesh_vertex_colors = True adds vertex normals and colours).  One process on
+one GPU.
 """
 import os
 import sys
@@ -29,13 +30,14 @@ def main(argv=None):
   state = checkpoints.restore_checkpoint(config.checkpoint_dir, state, model=model)
   step = int(state.step)
   t0 = time.time()
-  vertices, faces = mesh.extract_mesh(model, bbox, config.mesh_resolution, config.mesh_level)
+  vertices, faces, *extra = mesh.extract_mesh(model, bbox, config.mesh_resolution, config.mesh_level,
+                                              colors=config.mesh_vertex_colors)
   torch.cuda.synchronize()
   elapsed = time.time() - t0
   out_dir = os.path.join(config.checkpoint_dir, 'mesh')
   os.makedirs(out_dir, exist_ok=True)
   path = os.path.join(out_dir, f'mesh_step_{step}.ply')
-  mesh.write_ply(path, vertices, faces)
+  mesh.write_ply(path, vertices, faces, *extra)
   print(f'{vertices.shape[0]} vertices, {faces.shape[0]} faces in {elapsed:.2f} s '
         f'(grid {config.mesh_resolution} along the longest side of {bbox}, level {config.mesh_level}) -> {path}',
         flush=True)

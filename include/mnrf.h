@@ -117,6 +117,13 @@ int mnrf_encode(const mnrf_encode_desc* d, const float* sdist, const float* orig
 int mnrf_encode_points(const mnrf_encode_desc* d, const float* points, float var, const float* basis,
                        mnrf_bf16* feat_bf16, float* feat_f32, mnrf_stream stream);
 
+/* mnrf_encode_points plus the tangent rows d feature / d point (the input of the density-normal chain, as
+ * mnrf_encode's tfeat_bf16): the same feature rows, and tfeat_bf16[dir * N + i, ld_tfeat] = d feat_i / d point_i[dir],
+ * through the contraction and the dependence of its covariance on the mean when warp_contract.  var finite and
+ * >= 0; ld_tfeat >= feat_cols, a multiple of 8, tfeat_bf16 16-byte aligned. */
+int mnrf_encode_points_tangent(const mnrf_encode_desc* d, const float* points, float var, const float* basis,
+                               mnrf_bf16* feat_bf16, mnrf_bf16* tfeat_bf16, int32_t ld_tfeat, mnrf_stream stream);
+
 /* View-direction positional encoding, coord.pos_enc (coord.py:136-147) with
  * append_identity, broadcast over the S samples of each ray (models.py:550-554) and
  * written as bf16 into columns [col0, col0 + 3 + 6*deg) of a [B*S, ld] buffer; columns up
@@ -364,6 +371,14 @@ int mnrf_composite_fwd(const mnrf_composite_desc* d, const float* raw_density,
                        float* density_out, float* rgb_samples, float* acc, float* dist,
                        mnrf_stream stream);
 
+/* The activated, padded colour of M independent samples, as mnrf_composite_fwd's rgb_samples without compositing
+ * and without a per-sample scale (colours of points, e.g. mesh vertices).  Reads d's rgb_act, rgb_premult, rgb_bias,
+ * rgb_padding and rgb_mode only.
+ *   raw_rgb [M, ld_rgb] (ld_rgb >= 3: 4 reads the rgb columns of a stacked [density | rgb] head in place, passed at
+ *   its column 1); raw_diffuse [M, 3] with rgb_mode 1; raw_tint [M, 3] or NULL; rgb_out [M, 3] */
+int mnrf_point_rgb(const mnrf_composite_desc* d, int64_t M, const float* raw_rgb, int32_t ld_rgb,
+                   const float* raw_diffuse, const float* raw_tint, float* rgb_out, mnrf_stream stream);
+
 /* Losses + compositing backward for one level (train_utils.py:72-159 + the adjoint of
  * render.py:130-213).  Fuses: data loss (mse | charb | rawnerf) on this level's pixel,
  * distortion loss (final level), interlevel loss (proposal levels, against the final
@@ -603,6 +618,16 @@ enum { MNRF_MC_COUNT = 0, MNRF_MC_EMIT = 1 };
 int mnrf_marching_cubes(int32_t phase, int32_t nx, int32_t ny, int32_t nz, const float* grid, float level,
                         uint8_t* edge_cut, uint8_t* cell_tris, const int64_t* edge_scan, const int64_t* tri_scan,
                         float* vertices, int32_t* faces, mnrf_stream stream);
+
+/* Vertex normals of a marching-cubes mesh: after phase EMIT, with the same grid, level, edge_cut and edge_scan,
+ * writes normals [V, 3], one unit vector per cut edge at the edge's rank -- the order of EMIT's vertices, so
+ * normals[i] belongs to vertices[i].  The gradient of the grid at each end of the edge is taken by central
+ * differences (one-sided on the grid boundary), the two are interpolated with the vertex's t, and the normal is
+ * -g / |g|: from dense to empty space, the side the faces' winding faces.  Where g is zero or not finite the normal
+ * is the edge's direction from its inside end to its outside end.  Cells are cubes, so the normals hold in world
+ * space too. */
+int mnrf_mc_normals(int32_t nx, int32_t ny, int32_t nz, const float* grid, float level, const uint8_t* edge_cut,
+                    const int64_t* edge_scan, float* normals, mnrf_stream stream);
 
 #ifdef __cplusplus
 }

@@ -123,6 +123,8 @@ class Config:
   mesh_resolution: int = 512
   mesh_level: float = 10.
   mesh_bbox: Optional[Tuple[float, ...]] = None
+  # also write vertex normals and colours (each vertex's radiance seen head-on from outside, GLO zeroed)
+  mesh_vertex_colors: bool = False
 
 
 @dataclasses.dataclass

@@ -478,6 +478,25 @@ composite_bwd_kernel(mnrf_loss_desc L, const float* __restrict__ raw_density,
   }
 }
 
+// The activated, padded colour of each of M independent samples: ray_forward's colour without compositing and
+// without the per-ray scale (one thread per sample; raw_rgb rows ld_rgb floats apart)
+__global__ void __launch_bounds__(256)
+point_rgb_kernel(mnrf_composite_desc d, int64_t M, const float* __restrict__ raw_rgb, int ld_rgb,
+                 const float* __restrict__ raw_diffuse, const float* __restrict__ raw_tint, float* __restrict__ rgb_out) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < M; i += (int64_t)gridDim.x * blockDim.x) {
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+      const float z = d.rgb_premult * raw_rgb[i * ld_rgb + ch] + d.rgb_bias;
+      float zd = 0.f, zt = 0.f;
+      if (d.rgb_mode == 1) {
+        zd = raw_diffuse[i * 3 + ch];
+        if (raw_tint) zt = raw_tint[i * 3 + ch];
+      }
+      rgb_out[i * 3 + ch] = colour_fwd(d, z, zd, zt, raw_tint != nullptr);
+    }
+  }
+}
+
 }  // namespace mnrf
 
 #define MNRF_DISPATCH_CH(S, CALL)                         \
@@ -511,6 +530,25 @@ extern "C" int mnrf_composite_fwd(const mnrf_composite_desc* d, const float* raw
   MNRF_DISPATCH_CH(d->num_samples, (composite_fwd_kernel<CH><<<blocks, nw * 32, smem, (cudaStream_t)stream>>>(
       *d, raw_density, raw_rgb, density_noise, sdist, directions, near, far, bg_rgb, rgb_scale, raw_diffuse,
       raw_tint, weights, rgb_out, density_out, rgb_samples, acc, dist)));
+  MNRF_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int mnrf_point_rgb(const mnrf_composite_desc* d, int64_t M, const float* raw_rgb, int32_t ld_rgb,
+                              const float* raw_diffuse, const float* raw_tint, float* rgb_out, mnrf_stream stream) {
+  using namespace mnrf;
+  MNRF_CHECK(d, "mnrf_point_rgb: null descriptor");
+  MNRF_CHECK(M >= 0, "mnrf_point_rgb: negative sample count %lld", (long long)M);
+  if (M == 0) return 0;
+  MNRF_CHECK(raw_rgb && rgb_out, "mnrf_point_rgb: null pointer");
+  MNRF_CHECK(ld_rgb >= 3, "mnrf_point_rgb: ld_rgb %d < 3", ld_rgb);
+  MNRF_CHECK(d->rgb_act == MNRF_RGB_SIGMOID || d->rgb_act == MNRF_RGB_SAFE_EXP, "mnrf_point_rgb: unknown rgb_act %d",
+             d->rgb_act);
+  MNRF_CHECK(d->rgb_mode == 0 || d->rgb_mode == 1, "mnrf_point_rgb: unknown rgb_mode %d", d->rgb_mode);
+  MNRF_CHECK(d->rgb_mode == 0 || raw_diffuse, "mnrf_point_rgb: rgb_mode 1 needs raw_diffuse");
+  const int64_t maxb = (int64_t)mnrf_num_sms() * 16;
+  const int blocks = (int)((M + 255) / 256 < maxb ? (M + 255) / 256 : maxb);
+  point_rgb_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(*d, M, raw_rgb, ld_rgb, raw_diffuse, raw_tint, rgb_out);
   MNRF_LAUNCH_CHECK();
   return 0;
 }

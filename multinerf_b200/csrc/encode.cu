@@ -10,6 +10,7 @@
 // Output: bf16 feature rows written straight into the MLP's input buffer (row stride
 // ld_feat), staged through shared memory so that each lane stores 16 B.
 #include <algorithm>
+#include <cmath>
 
 #include "common.cuh"
 
@@ -117,6 +118,149 @@ __device__ __forceinline__ void contract_terms(const Gauss& g, ContractTerms& t)
 constexpr int kGaussStride = 13;   // 12 floats (mean 3 + cov 9), padded against bank conflicts
 constexpr int kContractStride = 25;   // + xh 3, pre-warp cov 6, (s, q, s_r, q_r) 4: odd against bank conflicts
 
+// Phase A of the general encoder for one Gaussian: stores it at gp (stride floats: kGaussStride, or kContractStride
+// with the terms of the tangent rows through the contraction ahead of the warp), contracted when d.warp_contract.
+template <bool Contract>
+__device__ __forceinline__ void store_gauss(const mnrf_encode_desc& d, Gauss& g, float* gp) {
+  if (Contract) {
+    ContractTerms t;
+    contract_terms(g, t);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) gp[12 + i] = t.xh[i];
+#pragma unroll
+    for (int i = 0; i < 6; ++i) gp[15 + i] = t.cov[i];
+    gp[21] = t.s; gp[22] = t.q; gp[23] = t.s_r; gp[24] = t.q_r;
+  }
+  if (d.warp_contract) contract_gauss(g);
+  gp[0] = g.mean[0]; gp[1] = g.mean[1]; gp[2] = g.mean[2];
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) gp[3 + i * 3 + j] = g.cov[i][j];
+}
+
+// The general encoder's per-warp shared memory: lift scratch and staged rows
+struct TangentScratch {
+  float *lm, *lv, *dlm, *dlv;      // lifted mean / variance [K]; Contract: their derivatives [dir][K]
+  __nv_bfloat16 *row, *trow;       // feature row, then (tfeat) three tangent rows, trow_elems apart
+  int trow_elems, row_bytes;
+};
+
+// Phase B of the general encoder for one Gaussian (stored at gp by store_gauss): lift onto the basis, then write
+// feature row m (bf16, fp32 copy when feat_f32 is given) and, with tfeat, the tangent rows dir * M_total + m,
+// d feature / d mean_dir.  Shared by the ray and the point encoder.
+template <bool Contract>
+__device__ __forceinline__ void gauss_tangent_rows(const mnrf_encode_desc& d, const float* gp, const float* sb,
+                                                   const TangentScratch& ws, size_t m, size_t M_total,
+                                                   __nv_bfloat16* __restrict__ feat, float* __restrict__ feat_f32,
+                                                   __nv_bfloat16* __restrict__ tfeat, int ld_tfeat, int lane) {
+  const int K = d.basis_k, L = d.max_deg - d.min_deg, KL = K * L;
+  float* lm = ws.lm;
+  float* lv = ws.lv;
+  float* dlm = ws.dlm;
+  float* dlv = ws.dlv;
+  __nv_bfloat16* row = ws.row;
+  __nv_bfloat16* trow = ws.trow;
+  const int trow_elems = ws.trow_elems, row_bytes = ws.row_bytes;
+  // (l, k) of feature f = l*K + k advance by 32 features per iteration without integer division
+  const int q32 = 32 / K, r32 = 32 - q32 * K;
+  const int l_first = lane / K, k_first = lane - l_first * K;
+  for (int k = lane; k < K; k += 32) {
+    float b0 = sb[k * 3 + 0], b1 = sb[k * 3 + 1], b2 = sb[k * 3 + 2];
+    lm[k] = gp[0] * b0 + gp[1] * b1 + gp[2] * b2;
+    float c0 = gp[3] * b0 + gp[4] * b1 + gp[5] * b2;
+    float c1 = gp[6] * b0 + gp[7] * b1 + gp[8] * b2;
+    float c2 = gp[9] * b0 + gp[10] * b1 + gp[11] * b2;
+    lv[k] = d.disable_integration ? 0.f : (b0 * c0 + b1 * c1 + b2 * c2);
+    if (Contract) {
+      const float b[3] = {b0, b1, b2};
+      const float* xh = gp + 12;
+      const float* cv = gp + 15;                 // xx xy xz yy yz zz
+      const float sj = gp[21], qj = gp[22], s_r = gp[23], q_r = gp[24];
+      const float beta = xh[0] * b0 + xh[1] * b1 + xh[2] * b2;
+      float bt[3], u[3], v[3], vt[3];
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+        bt[i] = b[i] - beta * xh[i];
+        u[i] = sj * bt[i] + (qj * beta) * xh[i];
+      }
+      v[0] = cv[0] * u[0] + cv[1] * u[1] + cv[2] * u[2];
+      v[1] = cv[1] * u[0] + cv[3] * u[1] + cv[4] * u[2];
+      v[2] = cv[2] * u[0] + cv[4] * u[1] + cv[5] * u[2];
+      const float gamma = xh[0] * v[0] + xh[1] * v[1] + xh[2] * v[2];
+#pragma unroll
+      for (int i = 0; i < 3; ++i) vt[i] = v[i] - gamma * xh[i];
+      const float btv = bt[0] * v[0] + bt[1] * v[1] + bt[2] * v[2];
+      const float radial = s_r * btv + q_r * (beta * gamma);
+#pragma unroll
+      for (int a = 0; a < 3; ++a) {
+        dlm[a * K + k] = u[a];
+        dlv[a * K + k] = d.disable_integration ? 0.f
+                                               : 2.f * (xh[a] * radial + s_r * (beta * vt[a] + gamma * bt[a]));
+      }
+    }
+  }
+  __syncwarp();
+  int l = l_first, k = k_first;
+  for (int f = lane; f < KL; f += 32) {
+    const float sc = __int_as_float((127 + d.min_deg + l) << 23);       // 2^(min_deg + l)
+    float y = lm[k] * sc;
+    float v = lv[k] * (sc * sc);
+    float e = __expf(-0.5f * v);
+    float fs, fc;
+    if (tfeat) {
+      // d/d mean_dir of e * safe_sin(lm * sc) = e * cos(reduced arg) * sc * basis[k][dir]
+      float s0, c0, s1, c1;
+      safe_sincos_fast(y, s0, c0);
+      safe_sincos_fast(y + 1.57079637050628662109375f, s1, c1);
+      fs = e * s0;
+      fc = e * s1;
+      if (Contract) {
+        // d feature = e cos(y) sc d lift_mean - 1/2 sc^2 feature d lift_var
+        const float esc = e * sc, hsc2 = 0.5f * (sc * sc);
+#pragma unroll
+        for (int dir = 0; dir < 3; ++dir) {
+          const float dm = dlm[dir * K + k] * esc, dvar = dlv[dir * K + k] * hsc2;
+          trow[dir * trow_elems + f] = __float2bfloat16(c0 * dm - fs * dvar);
+          trow[dir * trow_elems + KL + f] = __float2bfloat16(c1 * dm - fc * dvar);
+        }
+      } else {
+#pragma unroll
+        for (int dir = 0; dir < 3; ++dir) {
+          const float bk = sb[k * 3 + dir] * sc * e;
+          trow[dir * trow_elems + f] = __float2bfloat16(c0 * bk);
+          trow[dir * trow_elems + KL + f] = __float2bfloat16(c1 * bk);
+        }
+      }
+    } else {
+      fs = e * safe_sin_fast(y);
+      fc = e * safe_sin_fast(y + 1.57079637050628662109375f);
+    }
+    row[f] = __float2bfloat16(fs);
+    row[KL + f] = __float2bfloat16(fc);
+    if (feat_f32) {
+      feat_f32[m * (2 * KL) + f] = fs;
+      feat_f32[m * (2 * KL) + KL + f] = fc;
+    }
+    k += r32;
+    l += q32;
+    if (k >= K) { k -= K; l += 1; }
+  }
+  __syncwarp();
+  const uint4* src = reinterpret_cast<const uint4*>(row);
+  uint4* dst = reinterpret_cast<uint4*>(feat + m * (size_t)d.ld_feat);
+  for (int c = lane; c < row_bytes / 16; c += 32) dst[c] = src[c];
+  if (tfeat) {
+#pragma unroll
+    for (int dir = 0; dir < 3; ++dir) {
+      const uint4* ts = reinterpret_cast<const uint4*>(trow + dir * trow_elems);
+      uint4* td = reinterpret_cast<uint4*>(tfeat + ((size_t)dir * M_total + m) * (size_t)ld_tfeat);
+      for (int c = lane; c < row_bytes / 16; c += 32) td[c] = ts[c];
+    }
+  }
+  __syncwarp();
+}
+
 template <bool Contract>
 __global__ void __launch_bounds__(256)
 encode_kernel(mnrf_encode_desc d, const float* __restrict__ sdist,
@@ -127,7 +271,7 @@ encode_kernel(mnrf_encode_desc d, const float* __restrict__ sdist,
               float* __restrict__ tdist_out, __nv_bfloat16* __restrict__ tfeat, int ld_tfeat) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  const int S = d.num_samples, K = d.basis_k, L = d.max_deg - d.min_deg, KL = K * L;
+  const int S = d.num_samples, K = d.basis_k;
   float* sb = reinterpret_cast<float*>(smem_raw);                 // basis [K][3]
   const int row_bytes = ((d.feat_cols * 2 + 15) / 16) * 16;
   constexpr int stride = Contract ? kContractStride : kGaussStride;
@@ -135,23 +279,23 @@ encode_kernel(mnrf_encode_desc d, const float* __restrict__ sdist,
   float* wbase = sb + 3 * K + (size_t)wib * per_warp_f;
   float* tds = wbase;
   float* gs = tds + (S + 1);
-  float* lm = gs + S * stride;
-  float* lv = lm + K;
-  float* dlm = lv + K;         // Contract only: [dir][K]
-  float* dlv = dlm + 3 * K;
+  TangentScratch ws;
+  ws.lm = gs + S * stride;
+  ws.lv = ws.lm + K;
+  ws.dlm = ws.lv + K;
+  ws.dlv = ws.dlm + 3 * K;
   unsigned char* rows = smem_raw + (((size_t)(3 * K + nw * per_warp_f) * 4 + 15) / 16) * 16;
   const int rows_per_warp = tfeat ? 4 : 1;        // feature row + three tangent rows
-  __nv_bfloat16* row = reinterpret_cast<__nv_bfloat16*>(rows + (size_t)wib * rows_per_warp * row_bytes);
-  __nv_bfloat16* trow = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<unsigned char*>(row) + row_bytes);
-  const int trow_elems = row_bytes / 2;
+  ws.row = reinterpret_cast<__nv_bfloat16*>(rows + (size_t)wib * rows_per_warp * row_bytes);
+  ws.trow = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<unsigned char*>(ws.row) + row_bytes);
+  ws.trow_elems = row_bytes / 2;
+  ws.row_bytes = row_bytes;
   const size_t M_total = (size_t)d.num_rays * d.num_samples;
 
   for (int i = threadIdx.x; i < 3 * K; i += blockDim.x) sb[i] = basis[i];
   __syncthreads();
-  for (int i = lane; i < d.feat_cols * rows_per_warp; i += 32) row[i + (i / d.feat_cols) * (trow_elems - d.feat_cols)] = __float2bfloat16(0.f);
-  // (l, k) of feature f = l*K + k advance by 32 features per iteration without integer division
-  const int q32 = 32 / K, r32 = 32 - q32 * K;
-  const int l_first = lane / K, k_first = lane - l_first * K;
+  for (int i = lane; i < d.feat_cols * rows_per_warp; i += 32)
+    ws.row[i + (i / d.feat_cols) * (ws.trow_elems - d.feat_cols)] = __float2bfloat16(0.f);
 
   for (int ray = blockIdx.x * nw + wib; ray < d.num_rays; ray += gridDim.x * nw) {
     const float o[3] = {origins[ray * 3 + 0], origins[ray * 3 + 1], origins[ray * 3 + 2]};
@@ -169,123 +313,67 @@ encode_kernel(mnrf_encode_desc d, const float* __restrict__ sdist,
     for (int s = lane; s < S; s += 32) {
       Gauss g;
       cast_one(d.ray_shape, tds[s], tds[s + 1], o, dv, radius, g);
-      float* gp = gs + s * stride;
-      if (Contract) {
-        ContractTerms t;
-        contract_terms(g, t);
-#pragma unroll
-        for (int i = 0; i < 3; ++i) gp[12 + i] = t.xh[i];
-#pragma unroll
-        for (int i = 0; i < 6; ++i) gp[15 + i] = t.cov[i];
-        gp[21] = t.s; gp[22] = t.q; gp[23] = t.s_r; gp[24] = t.q_r;
-      }
-      if (d.warp_contract) contract_gauss(g);
-      gp[0] = g.mean[0]; gp[1] = g.mean[1]; gp[2] = g.mean[2];
-#pragma unroll
-      for (int i = 0; i < 3; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j) gp[3 + i * 3 + j] = g.cov[i][j];
+      store_gauss<Contract>(d, g, gs + s * stride);
     }
     __syncwarp();
     // phase B: per sample, lift onto the basis and emit the 2*K*L features
-    for (int s = 0; s < S; ++s) {
-      const float* gp = gs + s * stride;
-      for (int k = lane; k < K; k += 32) {
-        float b0 = sb[k * 3 + 0], b1 = sb[k * 3 + 1], b2 = sb[k * 3 + 2];
-        lm[k] = gp[0] * b0 + gp[1] * b1 + gp[2] * b2;
-        float c0 = gp[3] * b0 + gp[4] * b1 + gp[5] * b2;
-        float c1 = gp[6] * b0 + gp[7] * b1 + gp[8] * b2;
-        float c2 = gp[9] * b0 + gp[10] * b1 + gp[11] * b2;
-        lv[k] = d.disable_integration ? 0.f : (b0 * c0 + b1 * c1 + b2 * c2);
-        if (Contract) {
-          const float b[3] = {b0, b1, b2};
-          const float* xh = gp + 12;
-          const float* cv = gp + 15;                 // xx xy xz yy yz zz
-          const float sj = gp[21], qj = gp[22], s_r = gp[23], q_r = gp[24];
-          const float beta = xh[0] * b0 + xh[1] * b1 + xh[2] * b2;
-          float bt[3], u[3], v[3], vt[3];
+    for (int s = 0; s < S; ++s)
+      gauss_tangent_rows<Contract>(d, gs + s * stride, sb, ws, (size_t)ray * S + s, M_total, feat, feat_f32, tfeat,
+                                   ld_tfeat, lane);
+  }
+}
+
+// Point form with tangent rows: the Gaussian of point i has mean points[i] and covariance var * I.  One warp takes
+// 32 points at a time, one lane per point in phase A, then the general encoder's phase B point by point.
+template <bool Contract>
+__global__ void __launch_bounds__(256)
+encode_points_tangent_kernel(mnrf_encode_desc d, const float* __restrict__ points, float var,
+                             const float* __restrict__ basis, __nv_bfloat16* __restrict__ feat,
+                             __nv_bfloat16* __restrict__ tfeat, int ld_tfeat) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  const int K = d.basis_k;
+  float* sb = reinterpret_cast<float*>(smem_raw);                 // basis [K][3]
+  const int row_bytes = ((d.feat_cols * 2 + 15) / 16) * 16;
+  constexpr int stride = Contract ? kContractStride : kGaussStride;
+  const int per_warp_f = 32 * stride + (Contract ? 8 : 2) * K;
+  float* gs = sb + 3 * K + (size_t)wib * per_warp_f;
+  TangentScratch ws;
+  ws.lm = gs + 32 * stride;
+  ws.lv = ws.lm + K;
+  ws.dlm = ws.lv + K;
+  ws.dlv = ws.dlm + 3 * K;
+  unsigned char* rows = smem_raw + (((size_t)(3 * K + nw * per_warp_f) * 4 + 15) / 16) * 16;
+  ws.row = reinterpret_cast<__nv_bfloat16*>(rows + (size_t)wib * 4 * row_bytes);
+  ws.trow = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<unsigned char*>(ws.row) + row_bytes);
+  ws.trow_elems = row_bytes / 2;
+  ws.row_bytes = row_bytes;
+  const size_t N = (size_t)d.num_rays;
+
+  for (int i = threadIdx.x; i < 3 * K; i += blockDim.x) sb[i] = basis[i];
+  __syncthreads();
+  for (int i = lane; i < d.feat_cols * 4; i += 32)
+    ws.row[i + (i / d.feat_cols) * (ws.trow_elems - d.feat_cols)] = __float2bfloat16(0.f);
+
+  const int64_t num_groups = ((int64_t)N + 31) / 32;
+  for (int64_t grp = (int64_t)blockIdx.x * nw + wib; grp < num_groups; grp += (int64_t)gridDim.x * nw) {
+    const int64_t p0 = grp * 32;
+    const int g = (int)min((int64_t)32, (int64_t)N - p0);
+    __syncwarp();
+    if (lane < g) {
+      Gauss ga;
 #pragma unroll
-          for (int i = 0; i < 3; ++i) {
-            bt[i] = b[i] - beta * xh[i];
-            u[i] = sj * bt[i] + (qj * beta) * xh[i];
-          }
-          v[0] = cv[0] * u[0] + cv[1] * u[1] + cv[2] * u[2];
-          v[1] = cv[1] * u[0] + cv[3] * u[1] + cv[4] * u[2];
-          v[2] = cv[2] * u[0] + cv[4] * u[1] + cv[5] * u[2];
-          const float gamma = xh[0] * v[0] + xh[1] * v[1] + xh[2] * v[2];
+      for (int i = 0; i < 3; ++i) {
+        ga.mean[i] = points[(p0 + lane) * 3 + i];
 #pragma unroll
-          for (int i = 0; i < 3; ++i) vt[i] = v[i] - gamma * xh[i];
-          const float btv = bt[0] * v[0] + bt[1] * v[1] + bt[2] * v[2];
-          const float radial = s_r * btv + q_r * (beta * gamma);
-#pragma unroll
-          for (int a = 0; a < 3; ++a) {
-            dlm[a * K + k] = u[a];
-            dlv[a * K + k] = d.disable_integration ? 0.f
-                                                   : 2.f * (xh[a] * radial + s_r * (beta * vt[a] + gamma * bt[a]));
-          }
-        }
+        for (int j = 0; j < 3; ++j) ga.cov[i][j] = i == j ? var : 0.f;
       }
-      __syncwarp();
-      const size_t m = (size_t)ray * S + s;
-      int l = l_first, k = k_first;
-      for (int f = lane; f < KL; f += 32) {
-        const float sc = __int_as_float((127 + d.min_deg + l) << 23);       // 2^(min_deg + l)
-        float y = lm[k] * sc;
-        float v = lv[k] * (sc * sc);
-        float e = __expf(-0.5f * v);
-        float fs, fc;
-        if (tfeat) {
-          // d/d mean_dir of e * safe_sin(lm * sc) = e * cos(reduced arg) * sc * basis[k][dir]
-          float s0, c0, s1, c1;
-          safe_sincos_fast(y, s0, c0);
-          safe_sincos_fast(y + 1.57079637050628662109375f, s1, c1);
-          fs = e * s0;
-          fc = e * s1;
-          if (Contract) {
-            // d feature = e cos(y) sc d lift_mean - 1/2 sc^2 feature d lift_var
-            const float esc = e * sc, hsc2 = 0.5f * (sc * sc);
-#pragma unroll
-            for (int dir = 0; dir < 3; ++dir) {
-              const float dm = dlm[dir * K + k] * esc, dvar = dlv[dir * K + k] * hsc2;
-              trow[dir * trow_elems + f] = __float2bfloat16(c0 * dm - fs * dvar);
-              trow[dir * trow_elems + KL + f] = __float2bfloat16(c1 * dm - fc * dvar);
-            }
-          } else {
-#pragma unroll
-            for (int dir = 0; dir < 3; ++dir) {
-              const float bk = sb[k * 3 + dir] * sc * e;
-              trow[dir * trow_elems + f] = __float2bfloat16(c0 * bk);
-              trow[dir * trow_elems + KL + f] = __float2bfloat16(c1 * bk);
-            }
-          }
-        } else {
-          fs = e * safe_sin_fast(y);
-          fc = e * safe_sin_fast(y + 1.57079637050628662109375f);
-        }
-        row[f] = __float2bfloat16(fs);
-        row[KL + f] = __float2bfloat16(fc);
-        if (feat_f32) {
-          feat_f32[m * (2 * KL) + f] = fs;
-          feat_f32[m * (2 * KL) + KL + f] = fc;
-        }
-        k += r32;
-        l += q32;
-        if (k >= K) { k -= K; l += 1; }
-      }
-      __syncwarp();
-      const uint4* src = reinterpret_cast<const uint4*>(row);
-      uint4* dst = reinterpret_cast<uint4*>(feat + m * (size_t)d.ld_feat);
-      for (int c = lane; c < row_bytes / 16; c += 32) dst[c] = src[c];
-      if (tfeat) {
-#pragma unroll
-        for (int dir = 0; dir < 3; ++dir) {
-          const uint4* ts = reinterpret_cast<const uint4*>(trow + dir * trow_elems);
-          uint4* td = reinterpret_cast<uint4*>(tfeat + ((size_t)dir * M_total + m) * (size_t)ld_tfeat);
-          for (int c = lane; c < row_bytes / 16; c += 32) td[c] = ts[c];
-        }
-      }
-      __syncwarp();
+      store_gauss<Contract>(d, ga, gs + lane * stride);
     }
+    __syncwarp();
+    for (int s = 0; s < g; ++s)
+      gauss_tangent_rows<Contract>(d, gs + s * stride, sb, ws, (size_t)p0 + s, N, feat, nullptr, tfeat, ld_tfeat,
+                                   lane);
   }
 }
 
@@ -655,6 +743,44 @@ extern "C" int mnrf_encode_points(const mnrf_encode_desc* d, const float* points
   const int blocks = (int)std::min<int64_t>((groups + nw - 1) / nw, (int64_t)mnrf_num_sms() * 8);
   encode_points_kernel<<<blocks, nw * 32, smem, (cudaStream_t)stream>>>(
       *d, G, points, var, basis, reinterpret_cast<__nv_bfloat16*>(feat_bf16), feat_f32);
+  MNRF_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int mnrf_encode_points_tangent(const mnrf_encode_desc* d, const float* points, float var,
+                                          const float* basis, mnrf_bf16* feat_bf16, mnrf_bf16* tfeat_bf16,
+                                          int32_t ld_tfeat, mnrf_stream stream) {
+  using namespace mnrf;
+  MNRF_CHECK(d, "mnrf_encode_points_tangent: null descriptor");
+  MNRF_CHECK(d->num_rays >= 0, "mnrf_encode_points_tangent: negative point count %d", d->num_rays);
+  if (d->num_rays == 0) return 0;
+  MNRF_CHECK(points && basis && feat_bf16 && tfeat_bf16, "mnrf_encode_points_tangent: null pointer");
+  MNRF_CHECK(d->num_samples == 1 && d->raydist_fn == 0 && d->ray_shape == 0,
+             "mnrf_encode_points_tangent: num_samples must be 1 and raydist_fn, ray_shape 0 (got %d, %d, %d)",
+             d->num_samples, d->raydist_fn, d->ray_shape);
+  MNRF_CHECK(var >= 0.f && std::isfinite(var), "mnrf_encode_points_tangent: var %g is not finite and >= 0", var);
+  MNRF_CHECK(d->basis_k > 0 && d->max_deg > d->min_deg, "mnrf_encode_points_tangent: empty encoding");
+  const int KL2 = 2 * d->basis_k * (d->max_deg - d->min_deg);
+  MNRF_CHECK(d->feat_cols >= KL2 && d->ld_feat >= d->feat_cols,
+             "mnrf_encode_points_tangent: feat_cols %d < 2KL %d or ld %d", d->feat_cols, KL2, d->ld_feat);
+  MNRF_CHECK(d->feat_cols % 8 == 0 && d->ld_feat % 8 == 0 && ((uintptr_t)feat_bf16 % 16) == 0,
+             "mnrf_encode_points_tangent: feature rows must be 16-byte aligned");
+  MNRF_CHECK(ld_tfeat >= d->feat_cols && ld_tfeat % 8 == 0 && ((uintptr_t)tfeat_bf16 % 16) == 0,
+             "mnrf_encode_points_tangent: tangent rows must be 16-byte aligned");
+  const int nw = 8;
+  const bool contract = d->warp_contract != 0;
+  const int stride = contract ? kContractStride : kGaussStride;
+  const int row_bytes = ((d->feat_cols * 2 + 15) / 16) * 16;
+  const size_t smem = (((size_t)(3 * d->basis_k + nw * (32 * stride + (contract ? 8 : 2) * d->basis_k)) * 4 + 15) /
+                       16) * 16 + (size_t)nw * 4 * row_bytes;
+  MNRF_CHECK(smem <= 200 * 1024, "mnrf_encode_points_tangent: shared memory %zu too large", smem);
+  auto kernel = contract ? encode_points_tangent_kernel<true> : encode_points_tangent_kernel<false>;
+  MNRF_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int64_t groups = ((int64_t)d->num_rays + 31) / 32;
+  const int blocks = (int)std::min<int64_t>((groups + nw - 1) / nw, (int64_t)mnrf_num_sms() * 8);
+  kernel<<<blocks, nw * 32, smem, (cudaStream_t)stream>>>(*d, points, var, basis,
+                                                          reinterpret_cast<__nv_bfloat16*>(feat_bf16),
+                                                          reinterpret_cast<__nv_bfloat16*>(tfeat_bf16), ld_tfeat);
   MNRF_LAUNCH_CHECK();
   return 0;
 }

@@ -9,6 +9,8 @@
 // The case table (mc_tables.cuh, tools/gen_mc_tables.py) pairs the cut edges of each face from the face's corners
 // alone, so the two cells that share a face agree on it: the mesh is closed and consistently wound wherever the
 // level set stays off the grid boundary.
+// A third pass (mc_normals_kernel), run after emit with the same scan, writes one unit normal per vertex, also at the
+// edge's rank.
 #include <algorithm>
 
 #include "common.cuh"
@@ -95,6 +97,62 @@ mc_emit_kernel(McGrid g, const float* __restrict__ f, const uint8_t* __restrict_
   }
 }
 
+// Gradient of the grid at point p = (x, y, z): central differences, one-sided on the grid boundary
+__device__ __forceinline__ void mc_grad(const McGrid& g, const float* __restrict__ f, int64_t p, int x, int y, int z,
+                                        float grad[3]) {
+  const int c[3] = {x, y, z};
+  const int dim[3] = {g.nx, g.ny, g.nz};
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const int64_t s = mc_stride(g, a);
+    if (c[a] == 0) grad[a] = __ldg(f + p + s) - __ldg(f + p);
+    else if (c[a] == dim[a] - 1) grad[a] = __ldg(f + p) - __ldg(f + p - s);
+    else grad[a] = 0.5f * (__ldg(f + p + s) - __ldg(f + p - s));
+  }
+}
+
+// One unit normal per cut edge, at the edge's rank (the index of its vertex): -grad / |grad| with the gradients of
+// the edge's two ends interpolated at the vertex's t.  The gradient is scaled by its largest component before it is
+// squared, so no finite gradient overflows; a zero or non-finite one gives the edge's direction from its inside end
+// to its outside end.
+__global__ void __launch_bounds__(256)
+mc_normals_kernel(McGrid g, const float* __restrict__ f, const uint8_t* __restrict__ edge_cut,
+                  const int64_t* __restrict__ edge_scan, float* __restrict__ normals) {
+  for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < g.n; p += (int64_t)gridDim.x * blockDim.x) {
+    int x, y, z;
+    mc_coords(g, p, x, y, z);
+    const float f0 = __ldg(f + p);
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      if (!edge_cut[3 * p + a]) continue;
+      const int64_t q = p + mc_stride(g, a);
+      const float f1 = __ldg(f + q);
+      const float t = (g.level - f0) / (f1 - f0);     // as mc_emit_kernel
+      float g0[3], g1[3], n[3];
+      mc_grad(g, f, p, x, y, z, g0);
+      mc_grad(g, f, q, x + (a == 0), y + (a == 1), z + (a == 2), g1);
+#pragma unroll
+      for (int i = 0; i < 3; ++i) n[i] = g0[i] + t * (g1[i] - g0[i]);
+      const float m = fmaxf(fabsf(n[0]), fmaxf(fabsf(n[1]), fabsf(n[2])));
+      if (m > 0.f && isfinite(m)) {
+#pragma unroll
+        for (int i = 0; i < 3; ++i) n[i] = n[i] / m;
+        const float len = sqrtf(n[0] * n[0] + n[1] * n[1] + n[2] * n[2]);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) n[i] = -n[i] / len;
+      } else {
+        const float dir = f0 > g.level ? 1.f : -1.f;   // inside end first: +axis when the lower end is inside
+#pragma unroll
+        for (int i = 0; i < 3; ++i) n[i] = i == a ? dir : 0.f;
+      }
+      float* o = normals + 3 * (edge_scan[3 * p + a] - 1);
+      o[0] = n[0];
+      o[1] = n[1];
+      o[2] = n[2];
+    }
+  }
+}
+
 }  // namespace mnrf
 
 extern "C" int mnrf_marching_cubes(int32_t phase, int32_t nx, int32_t ny, int32_t nz, const float* grid, float level,
@@ -116,6 +174,19 @@ extern "C" int mnrf_marching_cubes(int32_t phase, int32_t nx, int32_t ny, int32_
     mc_emit_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(g, grid, edge_cut, cell_tris, edge_scan, tri_scan,
                                                              vertices, faces);
   }
+  MNRF_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int mnrf_mc_normals(int32_t nx, int32_t ny, int32_t nz, const float* grid, float level,
+                               const uint8_t* edge_cut, const int64_t* edge_scan, float* normals, mnrf_stream stream) {
+  using namespace mnrf;
+  MNRF_CHECK(nx >= 2 && ny >= 2 && nz >= 2 && nx <= kMcMaxDim && ny <= kMcMaxDim && nz <= kMcMaxDim,
+             "mnrf_mc_normals: grid %d x %d x %d (nz x ny x nx), each side must be in [2, %d]", nz, ny, nx, kMcMaxDim);
+  MNRF_CHECK(grid && edge_cut && edge_scan && normals, "mnrf_mc_normals: null pointer");
+  const McGrid g{nx, ny, nz, (int64_t)nx * ny * nz, level};
+  const int blocks = (int)std::min<int64_t>((g.n + 255) / 256, (int64_t)mnrf_num_sms() * 16);
+  mc_normals_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(g, grid, edge_cut, edge_scan, normals);
   MNRF_LAUNCH_CHECK();
   return 0;
 }

@@ -4,7 +4,9 @@
 cells spanning `bbox`, z-slab by z-slab, and extracts the level set `density = level` with
 `ops.marching_cubes` (csrc/mesh.cu).  Each grid point is queried as the Gaussian (point, h^2/12 I), the moments of
 a uniform cell of side h, so the grid samples the anti-aliased field at the footprint of one cell, as the rays'
-IPE does at the footprint of a ray interval.  `write_ply` stores the result as binary little-endian PLY.
+IPE does at the footprint of a ray interval.  With `colors=True` each vertex also gets a unit normal from the
+density grid's gradient and a colour from `Model.query_radiance`, seen along the inward normal.  `write_ply` stores
+the result as binary little-endian PLY.
 """
 import math
 
@@ -64,27 +66,59 @@ def density_grid(model, bbox, resolution, slab_planes=None):
   return grid, h
 
 
-def extract_mesh(model, bbox, resolution, level, slab_planes=None):
+def extract_mesh(model, bbox, resolution, level, slab_planes=None, colors=False):
   """(vertices [V, 3] fp32, faces [F, 3] int32) on the device: the surface density = `level` of `model`'s final
   level inside `bbox` (x0, y0, z0, x1, y1, z1), on a grid of `resolution` points along the longest side.
-  Vertices are in world coordinates; face normals point from dense to empty space."""
+  Vertices are in world coordinates; face normals point from dense to empty space.  With `colors`, returns
+  (vertices, faces, normals [V, 3] fp32, rgb [V, 3] uint8): unit vertex normals from the density grid's gradient,
+  and each vertex's colour from `vertex_colors`."""
   grid, h = density_grid(model, bbox, resolution, slab_planes)
-  vertices, faces = ops.marching_cubes(grid, level)
-  lo = torch.tensor([float(v) for v in bbox[:3]], device=vertices.device)
-  return vertices * h + lo, faces
+  out = ops.marching_cubes(grid, level, normals=colors)
+  del grid
+  lo = torch.tensor([float(v) for v in bbox[:3]], device=out[0].device)
+  vertices = out[0] * h + lo
+  if not colors:
+    return vertices, out[1]
+  # cubic cells: the grid's normals are the world's
+  return vertices, out[1], out[2], vertex_colors(model, vertices, out[2], h * h / 12)
 
 
-def write_ply(path, vertices, faces):
-  """Binary little-endian PLY: `float x, y, z` per vertex, `list uchar int vertex_indices` per face."""
-  v = np.ascontiguousarray(torch.as_tensor(vertices).detach().cpu().numpy(), dtype='<f4').reshape(-1, 3)
-  f = np.ascontiguousarray(torch.as_tensor(faces).detach().cpu().numpy(), dtype='<i4').reshape(-1, 3)
+def vertex_colors(model, vertices, normals, var):
+  """rgb [V, 3] uint8 of each vertex: `model.query_radiance` at the Gaussian (vertex, var * I) seen along -normal,
+  the surface viewed head-on from outside, as round(clip(rgb, 0, 1) * 255).  A RawNeRF model's colours are its
+  linear raw values, clipped as they are.  var: the footprint the density was sampled at (h^2 / 12 for grid cells
+  of side h)."""
+  _, rgb = model.query_radiance(vertices, var, -normals)
+  return (rgb.clamp(0, 1) * 255).round().to(torch.uint8)
+
+
+def write_ply(path, vertices, faces, normals=None, colors=None):
+  """Binary little-endian PLY: `float x, y, z` per vertex, then `float nx, ny, nz` when `normals` and
+  `uchar red, green, blue` when `colors` (uint8) are given, and `list uchar int vertex_indices` per face."""
+  def host(t, dtype):
+    return np.ascontiguousarray(torch.as_tensor(t).detach().cpu().numpy(), dtype=dtype).reshape(-1, 3)
+  v = host(vertices, '<f4')
+  f = host(faces, '<i4')
+  props = [('x', '<f4'), ('y', '<f4'), ('z', '<f4')]
+  cols = [v]
+  if normals is not None:
+    props += [('nx', '<f4'), ('ny', '<f4'), ('nz', '<f4')]
+    cols.append(host(normals, '<f4'))
+  if colors is not None:
+    props += [('red', 'u1'), ('green', 'u1'), ('blue', 'u1')]
+    cols.append(host(colors, 'u1'))
+  ply_type = {'<f4': 'float', 'u1': 'uchar'}
   header = ('ply\nformat binary_little_endian 1.0\n'
-            f'element vertex {len(v)}\nproperty float x\nproperty float y\nproperty float z\n'
+            f'element vertex {len(v)}\n' + ''.join(f'property {ply_type[t]} {n}\n' for n, t in props) +
             f'element face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n')
+  vrec = np.empty(len(v), dtype=props)
+  for c, block in enumerate(cols):
+    for j in range(3):
+      vrec[props[3 * c + j][0]] = block[:, j]
   rec = np.empty(len(f), dtype=[('n', 'u1'), ('idx', '<i4', (3,))])
   rec['n'] = 3
   rec['idx'] = f
   with open(path, 'wb') as fh:
     fh.write(header.encode('ascii'))
-    fh.write(v.tobytes())
+    fh.write(vrec.tobytes())
     fh.write(rec.tobytes())

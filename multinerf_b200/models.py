@@ -557,13 +557,14 @@ class Model:
                 rgb_mode=1 if (cfg.use_diffuse_color and not cfg.disable_rgb) else 0)
 
   # ------------------------------------------------------------------ buffers
-  def _level_state(self, key, mname, B, S, trunk_only=False):
+  def _level_state(self, key, mname, B, S, trunk_only=False, keep=True):
     # one buffer set per (level, module, shape), never replaced: captured CUDA graphs (train step, render
     # chunks) hold raw pointers into these buffers, so a differently shaped call (the ragged last chunk of
     # an image) must not free them.  trunk_only: the buffers of encode -> trunk -> density head alone, for a
-    # render-only pass no graph captures (query_density); not kept, so they are freed with the caller's reference
+    # render-only pass no graph captures (query_density).  keep=False, and trunk_only: not kept, so they are freed
+    # with the caller's reference (point queries, which no graph captures)
     key = (key, mname, B, S)
-    st = self._levels.get(key)
+    st = self._levels.get(key) if keep else None
     if st is not None:
       return st
     plan = self.plans[mname]
@@ -634,7 +635,8 @@ class Model:
       if plan.ref_stage and cfg.enable_pred_roughness:
         st.roughness = torch.empty(M, device=dev)
       st.extra_dw = torch.empty(B, S, device=dev)
-    self._levels[key] = st
+    if keep:
+      self._levels[key] = st
     return st
 
   @staticmethod
@@ -653,7 +655,7 @@ class Model:
       return dict(relu_mask=True) if head else dict(maskbits=(st.vbits if view else st.bits)[i])
     return dict(act=plan.act, z=(st.vzs if view else st.zs)[i])
 
-  def _refdir_args(self, st, mlp, rays):
+  def _refdir_args(self, st, mlp, viewdirs):
     """The leading arguments of ops.refdir_fwd / refdir_bwd: descriptor, IDE tables and the stage's inputs."""
     plan = mlp.plan
     cfg = plan.cfg
@@ -663,7 +665,7 @@ class Model:
         use_reflections=cfg.use_reflections, use_ide=cfg.use_directional_enc, use_n_dot_v=cfg.use_n_dot_v,
         use_roughness=cfg.enable_pred_roughness, deg_view=cfg.deg_view, ide_n=ide_n,
         roughness_bias=cfg.roughness_bias, ld=st.vin.stride(0), col0=plan.enc_col0, col_end=plan.vin_pad)
-    return desc, mat, ml, st.heads.get('grad_pred'), st.heads.get('roughness'), st.rgd, rays.viewdirs
+    return desc, mat, ml, st.heads.get('grad_pred'), st.heads.get('roughness'), st.rgd, viewdirs
 
   # ------------------------------------------------------------------ forward
   def _mlp_forward(self, st: LevelState, mlp: MLPDevice, rays, impl=0, loss_mults=None):
@@ -671,7 +673,19 @@ class Model:
     of rays, + orientation target flag: when given, the normals stage (Ref-NeRF or colourless) also emits
     d(loss)/d(weights)."""
     plan = mlp.plan
-    self._trunk_fwd(st, mlp, rays, impl)
+    cfg = plan.cfg
+    m = self.mcfg
+    ops.encode(st.sdist, rays.origins, rays.directions, rays.radii_flat, rays.near_flat,
+               rays.far_flat, mlp.basis, min_deg=cfg.min_deg_point, max_deg=cfg.max_deg_point,
+               raydist_fn=m.raydist_fn, ray_shape=m.ray_shape, warp_contract=cfg.warp_fn == 'contract',
+               disable_integration=m.disable_integration, feat=st.feat, feat_cols=plan.Fpad, tfeat=st.tfeat)
+    self._mlp_stages(st, mlp, rays.viewdirs, impl, loss_mults)
+
+  def _mlp_stages(self, st, mlp, viewdirs, impl=0, loss_mults=None):
+    """The MLP on the encoded st.feat (and st.tfeat), after the ray or the point encoder: trunk, tangents, narrow
+    heads, normals or Ref-NeRF stage, view branch.  viewdirs: one unit direction per ray of the level ([B, 3])."""
+    plan = mlp.plan
+    self._trunk_layers(st, mlp, impl)
     if plan.density_normals:
       self._tangent_fwd(st, mlp, impl)
     for sp in plan.narrow:
@@ -679,21 +693,10 @@ class Model:
     # (orientation, predicted-normal, target flag, d(loss)/d(weights) output) of the normals stage
     normals_args = _loss_args(loss_mults) + (st.extra_dw if loss_mults is not None else None,)
     if plan.normals_stage:
-      ops.normals_fwd(st.M, st.S, st.heads.get('grad_pred'), st.rgd, rays.viewdirs, st.normals_pred,
+      ops.normals_fwd(st.M, st.S, st.heads.get('grad_pred'), st.rgd, viewdirs, st.normals_pred,
                       st.normals, *normals_args)
     if plan.top == 'view':
-      self._view_fwd(st, mlp, rays, impl, normals_args)
-
-  def _trunk_fwd(self, st, mlp, rays, impl):
-    """Encoding, the trunk (one chained launch, or one GEMM per layer) and the density (or stacked) head."""
-    plan = mlp.plan
-    cfg = plan.cfg
-    m = self.mcfg
-    ops.encode(st.sdist, rays.origins, rays.directions, rays.radii_flat, rays.near_flat,
-               rays.far_flat, mlp.basis, min_deg=cfg.min_deg_point, max_deg=cfg.max_deg_point,
-               raydist_fn=m.raydist_fn, ray_shape=m.ray_shape, warp_contract=cfg.warp_fn == 'contract',
-               disable_integration=m.disable_integration, feat=st.feat, feat_cols=plan.Fpad, tfeat=st.tfeat)
-    self._trunk_layers(st, mlp, impl)
+      self._view_fwd(st, mlp, viewdirs, impl, normals_args)
 
   def _trunk_layers(self, st, mlp, impl):
     """The trunk (one chained launch, or one GEMM per layer) and the density (or stacked) head on the encoded
@@ -747,6 +750,50 @@ class Model:
       torch.nn.functional.softplus(st.raw_head[:, 0] + cfg.density_bias, out=density[i0:i0 + n])
     return density
 
+  def query_radiance(self, points, var, viewdirs, impl=0):
+    """Density and colour of the final level's MLP (NerfMLP_0) at world points [N, 3] seen along unit view
+    directions viewdirs [N, 3] (ignored, and may be None, for a view-independent model) -> (density [N], rgb [N, 3])
+    fp32 on the device.  Each point is one sample: the point encoder on the Gaussian (point, var * I), then the
+    level's MLP as a render runs it (Model._mlp_stages: density normals and the Ref-NeRF stage included), with
+    the GLO vector zeroed, no density or bottleneck noise, and no exposure scale; rgb is the activated, padded
+    sample colour (ops.point_rgb), zero for an MLP without colour.  Density as query_density.  Runs in chunks of
+    render_chunk_size * num_nerf_samples rows."""
+    mname = 'NerfMLP_0'
+    mlp = self.mlps[mname]
+    plan = mlp.plan
+    cfg = plan.cfg
+    dev = self.device
+    points = torch.as_tensor(points, dtype=torch.float32, device=dev).reshape(-1, 3).contiguous()
+    N = points.shape[0]
+    if plan.top == 'view':
+      if viewdirs is None:
+        raise ValueError('query_radiance: this model\'s colour depends on the view direction: give viewdirs')
+      viewdirs = torch.as_tensor(viewdirs, dtype=torch.float32, device=dev).reshape(-1, 3).contiguous()
+      if viewdirs.shape[0] != N:
+        raise ValueError(f'query_radiance: {viewdirs.shape[0]} view directions for {N} points')
+    density = torch.empty(N, device=dev)
+    rgb = torch.zeros(N, 3, device=dev)
+    comp_cfg = self._comp_cfg(cfg)
+    chunk = self.config.render_chunk_size * self.mcfg.num_nerf_samples
+    states = {}
+    for i0 in range(0, N, chunk):
+      p = points[i0:i0 + chunk]
+      n = p.shape[0]
+      if n not in states:
+        states[n] = self._level_state('radiance', mname, n, 1, keep=False)
+        # the tangent GEMMs read the trunk's ReLU masks or pre-activations (as forward_levels sets keep_acts)
+        states[n].keep_acts = plan.density_normals
+      st = states[n]
+      ops.encode_points(p, var, mlp.basis, min_deg=cfg.min_deg_point, max_deg=cfg.max_deg_point,
+                        warp_contract=cfg.warp_fn == 'contract', disable_integration=self.mcfg.disable_integration,
+                        feat=st.feat, feat_cols=plan.Fpad, tfeat=st.tfeat)
+      self._mlp_stages(st, mlp, viewdirs[i0:i0 + n] if plan.top == 'view' else None, impl)
+      torch.nn.functional.softplus(st.raw_head[:, 0] + cfg.density_bias, out=density[i0:i0 + n])
+      if st.raw_rgb is not None:
+        ops.point_rgb(st.raw_rgb.reshape(n, 3), cfg=comp_cfg, raw_diffuse=st.heads.get('diffuse'),
+                      raw_tint=st.heads.get('tint'), out=rgb[i0:i0 + n])
+    return density, rgb
+
   def _tangent_fwd(self, st, mlp, impl):
     """raw_grad_density = d raw_density / d mean by forward mode (replaces vmap(value_and_grad),
     models.py:473-492): tangents see the same weights, no bias, and the primal's activation derivative (ReLU masks,
@@ -764,7 +811,7 @@ class Model:
     d = plan.one('density')
     ops.head_fwd(t, mlp.w_nk[d.name], None, 1, d.in_pad, raw=st.rgd.view(3 * st.M, 1))
 
-  def _view_fwd(self, st, mlp, rays, impl, normals_args):
+  def _view_fwd(self, st, mlp, viewdirs, impl, normals_args):
     """Bottleneck, Ref-NeRF stage or direction encoding, GLO, view MLP and rgb head."""
     plan = mlp.plan
     cfg = plan.cfg
@@ -777,10 +824,10 @@ class Model:
         # models.py:529-533 (regulariser, unused by the shipped configs): plain elementwise add
         st.vin[:, :bt.out_dim].add_((cfg.bottleneck_noise * st.bneck_noise).to(torch.bfloat16))
     if plan.ref_stage:
-      ops.refdir_fwd(*self._refdir_args(st, mlp, rays), st.normals_pred, st.normals, st.roughness, st.vin,
+      ops.refdir_fwd(*self._refdir_args(st, mlp, viewdirs), st.normals_pred, st.normals, st.roughness, st.vin,
                      *normals_args)
     else:
-      ops.viewdir_enc(rays.viewdirs, S, cfg.deg_view, st.vin, plan.enc_col0, plan.vin_pad)
+      ops.viewdir_enc(viewdirs, S, cfg.deg_view, st.vin, plan.enc_col0, plan.vin_pad)
     if plan.glo_features > 0:
       # GLO vector of the ray's camera, broadcast over the samples (models.py:565-569).  Written after the Ref-NeRF
       # stage: its slab zero-fill would also clear the GLO columns.
@@ -1138,7 +1185,7 @@ class Model:
       self.params.seg('Embed_0', self.params.grads).view(self.mcfg.num_glo_embeddings, -1).index_add_(
           0, rays.cam_idx[:, 0].long(), d_glo)
     if plan.ref_stage:
-      ops.refdir_bwd(*self._refdir_args(st, mlp, rays), st.comp['weights'], sc.d_vin, *lm, st.d_raw_density,
+      ops.refdir_bwd(*self._refdir_args(st, mlp, rays.viewdirs), st.comp['weights'], sc.d_vin, *lm, st.d_raw_density,
                      st.d_heads.get('diffuse'), st.d_heads.get('tint'), st.d_heads.get('grad_pred'),
                      st.d_heads['roughness'].view(st.M) if 'roughness' in st.d_heads else None, st.d_rgd, stats)
       self._narrow_heads_bwd(st, mlp)

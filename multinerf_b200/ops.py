@@ -134,8 +134,9 @@ def encode(sdist, origins, directions, radii, near, far, basis, *, min_deg, max_
 
 
 def encode_points(points, var, basis, *, min_deg, max_deg, warp_contract=False, disable_integration=False,
-                  feat=None, feat_cols=None, want_f32=False):
-  """Point form of `encode`: features of the Gaussians (points[i], var * I) -> bf16 [N, ld] (+ fp32 [N, 2KL])."""
+                  feat=None, feat_cols=None, want_f32=False, tfeat=None):
+  """Point form of `encode`: features of the Gaussians (points[i], var * I) -> bf16 [N, ld] (+ fp32 [N, 2KL]).
+  With `tfeat` [3N, ld_t] bf16, also the tangent rows d feature / d point (no fp32 copy then)."""
   lib = L.load()
   N = points.shape[0]
   K = basis.shape[0]
@@ -147,16 +148,23 @@ def encode_points(points, var, basis, *, min_deg, max_deg, warp_contract=False, 
   assert feat.dtype == torch.bfloat16 and feat.stride(1) == 1
   d = L.EncodeDesc(N, 1, 0, 0, int(warp_contract), int(disable_integration), K, min_deg, max_deg, feat.stride(0),
                    feat_cols)
-  f32 = torch.empty(N, F, device=points.device) if want_f32 else None
   _count()
+  if tfeat is not None:
+    assert not want_f32 and tfeat.dtype == torch.bfloat16 and tfeat.stride(1) == 1
+    L.check(lib.mnrf_encode_points_tangent(C.byref(d), L.ptr(_f32(points)), float(var), L.ptr(_f32(basis)),
+                                           L.ptr(feat), L.ptr(tfeat), tfeat.stride(0), L.stream_ptr()))
+    return feat, None
+  f32 = torch.empty(N, F, device=points.device) if want_f32 else None
   L.check(lib.mnrf_encode_points(C.byref(d), L.ptr(_f32(points)), float(var), L.ptr(_f32(basis)), L.ptr(feat),
                                  L.ptr(f32), L.stream_ptr()))
   return feat, f32
 
 
-def marching_cubes(grid, level):
+def marching_cubes(grid, level, normals=False):
   """Marching cubes on an fp32 grid [nz, ny, nx] (inside: value > level) -> (vertices [V, 3] fp32 in grid units
-  (x, y, z), faces [F, 3] int32).  Reads the two totals back once, between the count and emit phases."""
+  (x, y, z), faces [F, 3] int32), and with `normals` the unit vertex normals [V, 3] (from dense to empty space, the
+  grid's gradient interpolated along each vertex's edge).  Reads the two totals back once, between the count and
+  emit phases."""
   lib = L.load()
   grid = _f32(grid)
   assert grid.dim() == 3, 'grid must be [nz, ny, nx]'
@@ -179,7 +187,14 @@ def marching_cubes(grid, level):
     _count()
     L.check(lib.mnrf_marching_cubes(L.MC_EMIT, *args, L.ptr(edge_scan), L.ptr(tri_scan), L.ptr(vertices),
                                     L.ptr(faces), L.stream_ptr()))
-  return vertices, faces
+  if not normals:
+    return vertices, faces
+  vnormals = torch.empty(V, 3, device=dev)
+  if V:
+    _count()
+    L.check(lib.mnrf_mc_normals(nx, ny, nz, L.ptr(grid), float(level), L.ptr(edge_cut), L.ptr(edge_scan),
+                                L.ptr(vnormals), L.stream_ptr()))
+  return vertices, faces, vnormals
 
 
 def viewdir_enc(viewdirs, num_samples, deg, out, col0, col_end):
@@ -368,6 +383,22 @@ def composite_fwd(raw_density, raw_rgb, sdist, directions, near, far, *, cfg, de
                                  L.ptr(_f32(raw_tint)), L.ptr(weights), L.ptr(rgb),
                                  L.ptr(dens), L.ptr(rgbs), L.ptr(acc), L.ptr(dist), L.stream_ptr()))
   return dict(weights=weights, rgb=rgb, density=dens, rgb_samples=rgbs, acc=acc, dist=dist)
+
+
+def point_rgb(raw_rgb, *, cfg, raw_diffuse=None, raw_tint=None, out=None):
+  """The activated, padded colour of each row of raw_rgb [M, 3] (row stride from the tensor: a stacked head's
+  [M, 4] output is read in place through its column view), without compositing -> fp32 [M, 3].  cfg: kwargs of
+  _cdesc."""
+  lib = L.load()
+  M = raw_rgb.shape[0]
+  assert raw_rgb.dtype == torch.float32 and raw_rgb.dim() == 2 and raw_rgb.shape[1] == 3 and raw_rgb.stride(1) == 1
+  d = _cdesc(M, 1, **cfg)
+  if out is None:
+    out = torch.empty(M, 3, device=raw_rgb.device)
+  _count()
+  L.check(lib.mnrf_point_rgb(C.byref(d), M, L.ptr(raw_rgb), raw_rgb.stride(0), L.ptr(_f32(raw_diffuse)),
+                             L.ptr(_f32(raw_tint)), L.ptr(_f32(out)), L.stream_ptr()))
+  return out
 
 
 def composite_bwd(raw_density, raw_rgb, sdist, directions, near, far, target_rgb, lossmult,

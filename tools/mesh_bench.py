@@ -8,6 +8,9 @@
           smooth noise;
   extract: mesh.extract_mesh end to end at --extract_res^3 on the 360.gin model (random init, level = the grid's
           median density over a first, untimed extraction);
+  color:  Model.query_radiance rows/s and its GEMM TFLOP/s as for `query`, on the same NerfMLPs and points, with
+          unit view directions; mnrf_mc_normals alone (CUDA events over --reps launches) at 256^3 and 512^3 on the
+          `mc` grids; mesh.extract_mesh at --extract_res^3 without and with colours, alternated --reps times;
   device: the card's name and power limit, read in the same run.
 
   python tools/mesh_bench.py [--rows 8388608] [--extract_res 512] [--out result.json]
@@ -42,17 +45,23 @@ def timed(fn, reps):
   return (time.perf_counter() - t0) / reps, out
 
 
-def bench_query(bundle, rows, reps):
+def bench_query(bundle, rows, reps, radiance=False):
+  """query_density, or with `radiance` query_radiance (view directions uniform on the sphere)."""
   model = models.Model(bundle)
   model.init(seed=0)
   g = torch.Generator(device='cuda')
   g.manual_seed(0)
   pts = torch.rand(rows, 3, device='cuda', generator=g) * 3 - 1.5
   var = (3.0 / 511) ** 2 / 12
-  model.query_density(pts, var)                      # warm-up: every chunk shape, plans, module loads
-  wall, _ = timed(lambda: model.query_density(pts, var), reps)
+  if radiance:
+    vd = torch.nn.functional.normalize(torch.randn(rows, 3, device='cuda', generator=g), dim=-1)
+    query = lambda: model.query_radiance(pts, var, vd)
+  else:
+    query = lambda: model.query_density(pts, var)
+  query()                                            # warm-up: every chunk shape, plans, module loads
+  wall, _ = timed(query, reps)
   ops.GEMM_EVENTS = []
-  model.query_density(pts, var)
+  query()
   torch.cuda.synchronize()
   ev, ops.GEMM_EVENTS = ops.GEMM_EVENTS, None
   kern_s = sum(a.elapsed_time(b) for a, b, _ in ev) / 1e3
@@ -85,6 +94,32 @@ def bench_mc(n, reps):
   return {'grid': n, 's': round(t, 4), 'vertices': int(v.shape[0]), 'faces': int(f.shape[0])}
 
 
+def bench_mc_normals(n, reps):
+  """mnrf_mc_normals alone on the `bench_mc` grid: the count phase and the edge scan once, then CUDA events around
+  `reps` normal launches."""
+  L = lib.load()
+  grid = sphere_noise(n)
+  edge_cut = torch.empty(3 * grid.numel(), device='cuda', dtype=torch.uint8)
+  cell_tris = torch.empty(grid.numel(), device='cuda', dtype=torch.uint8)
+  lib.check(L.mnrf_marching_cubes(lib.MC_COUNT, n, n, n, lib.ptr(grid), 0.0, lib.ptr(edge_cut), lib.ptr(cell_tris),
+                                  None, None, None, None, lib.stream_ptr()))
+  edge_scan = torch.cumsum(edge_cut, 0, dtype=torch.int64)
+  V = int(edge_scan[-1])
+  normals = torch.empty(V, 3, device='cuda')
+
+  def launch():
+    lib.check(L.mnrf_mc_normals(n, n, n, lib.ptr(grid), 0.0, lib.ptr(edge_cut), lib.ptr(edge_scan), lib.ptr(normals),
+                                lib.stream_ptr()))
+  launch()
+  ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+  ev[0].record()
+  for _ in range(reps):
+    launch()
+  ev[1].record()
+  torch.cuda.synchronize()
+  return {'grid': n, 'vertices': V, 'ms': round(ev[0].elapsed_time(ev[1]) / reps, 3)}
+
+
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--rows', type=int, default=1 << 23)
@@ -111,6 +146,25 @@ def main():
   t, (v, f) = timed(lambda: mesh.extract_mesh(model, bbox, args.extract_res, level), 1)
   res['extract'] = {'config': '360.gin NerfMLP, random init', 'grid': args.extract_res, 'level': level,
                     's': round(t, 3), 'vertices': int(v.shape[0]), 'faces': int(f.shape[0])}
+  del v, f
+  torch.cuda.empty_cache()
+  color = {'query': {}, 'mc_normals': [], 'extract': {'plain_s': [], 'colors_s': []}}
+  for name, make in (('360', configs.bundle_360), ('blender_256', configs.bundle_blender_256)):
+    color['query'][name] = bench_query(make(), args.rows, args.reps, radiance=True)
+    torch.cuda.empty_cache()
+  for n in (256, 512):
+    color['mc_normals'].append(bench_mc_normals(n, 20))
+    torch.cuda.empty_cache()
+  mesh.extract_mesh(model, bbox, args.extract_res, level, colors=True)      # warm-up of the colour query's shapes
+  torch.cuda.empty_cache()
+  for _ in range(args.reps):
+    for key, colors in (('plain_s', False), ('colors_s', True)):
+      t, out = timed(lambda: mesh.extract_mesh(model, bbox, args.extract_res, level, colors=colors), 1)
+      color['extract'][key].append(round(t, 3))
+      color['extract']['vertices'] = int(out[0].shape[0])
+      del out
+      torch.cuda.empty_cache()
+  res['color'] = color
   res['device_after'] = device_info()
   line = json.dumps(res)
   print(line, flush=True)
