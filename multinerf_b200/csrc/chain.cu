@@ -321,8 +321,9 @@ mlp_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainParams p) {
             for (int h = 0; h < 2; ++h) {
               v[h][0] += b.x;
               v[h][1] += b.y;
-              // ReLU is folded into the bf16 conversion; the mask is the sign of the fp32 pre-activation
-              // (v > 0  <=>  stored activation > 0: bf16 keeps fp32's exponent range)
+              // ReLU is folded into the bf16 conversion (a NaN stays NaN, with mask bit 0); the mask is the sign of
+              // the fp32 pre-activation: stored > 0 implies the bit, and a set bit over a stored 0 only where the
+              // pre-activation is in (0, 2^-134], which rounds to a bf16 zero
               bits[h] |= ((v[h][0] > 0.f ? 1u : 0u) | (v[h][1] > 0.f ? 2u : 0u)) << (col & 31);
               o[h] = pack_bf16_relu(v[h][0], v[h][1]);
             }
@@ -446,6 +447,9 @@ extern "C" int mnrf_mlp_chain(const mnrf_chain_desc* d, mnrf_stream stream_) {
   using namespace mnrf;
   cudaStream_t stream = (cudaStream_t)stream_;
   MNRF_CHECK(d, "mnrf_mlp_chain: null descriptor");
+  // the TMA row coordinates of a unit are int32
+  MNRF_CHECK(d->m >= 0 && (d->m + CH_ROWS - 1) / CH_ROWS * CH_ROWS <= INT32_MAX,
+             "mnrf_mlp_chain: m must be in [0, %d], got %lld", INT32_MAX / CH_ROWS * CH_ROWS, (long long)d->m);
   if (d->m == 0) return 0;
   MNRF_CHECK(d->mode == MNRF_CHAIN_FWD || d->mode == MNRF_CHAIN_BWD, "mnrf_mlp_chain: bad mode %d", d->mode);
   MNRF_CHECK(d->num_layers >= 1 && d->num_layers <= CH_MAX_LAYERS, "mnrf_mlp_chain: 1..%d layers, got %d",
@@ -464,6 +468,8 @@ extern "C" int mnrf_mlp_chain(const mnrf_chain_desc* d, mnrf_stream stream_) {
     ChainLayer& L = p.layer[j];
     MNRF_CHECK(s.n_res == 0 || s.n_res == CH_W / 64, "mnrf_mlp_chain: layer %d: n_res must be 0 or %d", j, CH_W / 64);
     MNRF_CHECK(s.n_stream >= 0 && (s.n_stream > 0 || s.n_res > 0), "mnrf_mlp_chain: layer %d has no operand", j);
+    MNRF_CHECK(s.stream_col0 >= 0 && s.stream_kb0 >= 0 && s.res_kb0 >= 0,
+               "mnrf_mlp_chain: layer %d: negative column or k-block offset", j);
     MNRF_CHECK(j > 0 || s.n_res == 0, "mnrf_mlp_chain: the first layer has no resident operand");
     MNRF_CHECK(s.w && ((uintptr_t)s.w % 16) == 0 && s.ldw % 8 == 0, "mnrf_mlp_chain: layer %d: weights must be 16-byte aligned", j);
     const int kblocks = std::max(s.n_stream > 0 ? s.stream_kb0 + s.n_stream : 0, s.n_res > 0 ? s.res_kb0 + s.n_res : 0);
@@ -493,6 +499,8 @@ extern "C" int mnrf_mlp_chain(const mnrf_chain_desc* d, mnrf_stream stream_) {
   if (any_stream) {
     MNRF_CHECK(d->stream && ((uintptr_t)d->stream % 16) == 0 && d->ldstream % 8 == 0 && d->stream_cols % 64 == 0,
                "mnrf_mlp_chain: streamed operand must be 16-byte aligned with a multiple of 64 columns");
+    MNRF_CHECK(d->ldstream >= d->stream_cols, "mnrf_mlp_chain: stream pitch %lld < %d columns",
+               (long long)d->ldstream, d->stream_cols);
     // each consumer warpgroup waits on its own 64 rows
     if (make_tmap(&maps.stream, d->stream, d->m, d->stream_cols, d->ldstream, 64, CH_ROWS / 2)) return 1;
   }

@@ -36,6 +36,13 @@ constexpr float kEps = 1.1920929e-07f;        // jnp.finfo(float32).eps
 constexpr float kEpsSq = 1.4210855e-14f;      // eps**2 (stepfun.py:89,121)
 constexpr unsigned kFull = 0xffffffffu;
 
+// ReLU that keeps a NaN, as torch.relu and jnp.maximum do (fmaxf returns the other operand): one max.NaN.f32
+__device__ __forceinline__ float relu_nan(float x) {
+  float r;
+  asm("max.NaN.f32 %0, %1, 0f00000000;" : "=f"(r) : "f"(x));
+  return r;
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);

@@ -38,7 +38,7 @@ __global__ void gemm_ref_nt_kernel(mnrf_gemm_desc d, const __nv_bfloat16* __rest
   if (d.mode == MNRF_GEMM_FWD) {
     if (bias) acc += bias[n];
     if (d.act == MNRF_ACT_RELU) {
-      acc = fmaxf(acc, 0.f);
+      acc = relu_nan(acc);
       if (maskbits && acc > 0.f) atomicOr(&maskbits[m * d.ldmaskbits + (n >> 5)], 1u << (n & 31));
     } else if (d.act == MNRF_ACT_SOFTPLUS || d.act == MNRF_ACT_SILU) {
       if (z) z[m * ldz + n] = __float2bfloat16(acc);

@@ -250,7 +250,7 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const CUtenso
         for (int h = 0; h < 2; ++h)
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            v[h][e] = fmaxf(v[h][e], 0.f);
+            v[h][e] = relu_nan(v[h][e]);
             bits[h] |= (v[h][e] > 0.f ? 1u : 0u) << ((8 * i + cq + e) & 31);
           }
       }

@@ -139,12 +139,11 @@ def ref_dgrad(a, b, *, rowv=None, colv=None, mask=None, maskbits=None, mask_mod=
     v = t * f
     e = f.abs() * e + t.abs() * _fast_d1_err(act_code, zz)
     e = _round_add(v, e)
-  elif maskbits is not None:
-    f = unpack_bits(maskbits, n)[rows].double()
-    v, e = t * f, e * f
-  elif mask is not None:
-    f = (mask.double()[rows] > 0).double()
-    v, e = t * f, e * f
+  elif maskbits is not None or mask is not None:
+    # a select, not a product: a masked-out element is 0 even where the sum is NaN or infinite (jax.nn.relu's JVP,
+    # torch's threshold_backward)
+    keep = unpack_bits(maskbits, n)[rows] if maskbits is not None else mask.double()[rows] > 0
+    v, e = torch.where(keep, t, 0.0), torch.where(keep, e, 0.0)
   else:
     v = t
   if addend is not None:
@@ -206,13 +205,19 @@ def check(got, value, bound, what):
   return worst
 
 
-def check_bits(words, stored, value, bound, what):
-  """FWD ReLU mask bits: exactly (stored output > 0); against fp64 they may differ only where |value| <= bound."""
+def check_bits(words, stored, z, bound, what):
+  """FWD ReLU mask bits, the sign of the fp32 pre-activation, against the stored output and the fp64 pre-activation z
+  (known to within bound before its bf16 rounding).  stored > 0 implies the bit; a set bit over a stored 0 only where
+  the fp32 pre-activation may lie in (0, 2^-134], which rounds to a bf16 zero; against fp64 the bits may differ only
+  where |z| <= bound.  A NaN pre-activation has bit 0."""
   n = stored.shape[1]
-  bits = unpack_bits(words, n)
-  assert torch.equal(bits, stored.float() > 0), f'{what}: mask bits differ from (stored output > 0)'
-  disagree = bits != (value > 0)
-  assert not (disagree & (value.abs() > bound)).any(), f'{what}: mask bits wrong where fp64 is clearly signed'
+  bits = unpack_bits(words, n).to(stored.device)
+  pos = stored.float() > 0
+  assert not (pos & ~bits).any(), f'{what}: a positive stored output without its mask bit'
+  tiny = (z - bound <= 2.0 ** -134) & (z + bound > 0)
+  assert not (bits & ~pos & ~tiny).any(), f'{what}: a mask bit over a stored 0 whose pre-activation is not tiny'
+  disagree = bits != (z > 0)
+  assert not (disagree & ~(z.abs() <= bound)).any(), f'{what}: mask bits wrong where fp64 is clearly signed'
 
 
 # ---------------------------------------------------------------------------------------------- buffers

@@ -127,7 +127,7 @@ def test_fwd_emulation_inside_bound(order, code, m, n, k):
   G.check(zq, r['z'], r['z_bound'], f'fwd z {order}')
   G.check(pre, r['out'], r['pre_bound'], f'fwd fp32 {order}')
   if code == G.RELU and n % 32 == 0:
-    G.check_bits(G.pack_bits(out.float() > 0), out, r['out'], r['out_bound'], 'bits')
+    G.check_bits(G.pack_bits(out.float() > 0), out, r['z'], r['pre_bound'], 'bits')
   # without a bias, the zero-by-cancellation outputs get a bound of the accumulation error alone, far below the
   # bf16 resolution of the products summed
   r0 = G.ref_fwd(a, b)
@@ -244,11 +244,11 @@ def test_flags_flipped_mask_bit():
   r = G.ref_fwd(a, b, bias=bias, act_code=G.RELU)
   out, _, _ = _emulate_fwd(a, b, bias, G.RELU, 'sequential', gen)
   words = G.pack_bits(out.float() > 0)
-  G.check_bits(words, out, r['out'], r['out_bound'], 'unmutated')
+  G.check_bits(words, out, r['z'], r['pre_bound'], 'unmutated')
   bad = words.clone()
   bad[150, 3] ^= 1 << 7
   with pytest.raises(AssertionError):
-    G.check_bits(bad, out, r['out'], r['out_bound'], 'mutated')
+    G.check_bits(bad, out, r['z'], r['pre_bound'], 'mutated')
   # DGRAD reading the flipped bit: the output at that element is masked wrongly
   maskb = torch.rand(M, N, generator=gen) > 0.5
   dy = _bf16(torch.randn(M, K, generator=gen))

@@ -291,7 +291,7 @@ def verify(c, v, bufs, init):
     if 'z' in v:
       worst['z'] = G.check(v['z'], r['z'], r['z_bound'], 'z')
     if 'maskbits' in v:
-      G.check_bits(v['maskbits'], v['out'], r['out'], r['out_bound'], 'mask bits')
+      G.check_bits(v['maskbits'], v['out'], r['z'], r['pre_bound'], 'mask bits')
     return worst
   r = G.ref_dgrad(v['a'], v['b'], rowv=v.get('rowv'), colv=v.get('colv'), mask=v.get('mask'),
                   maskbits=v.get('maskbits'), mask_mod=c['M'] // c['rep'] if c['rep'] else 0,
@@ -518,3 +518,47 @@ def test_rejected_wgrad(ops, n):
     ops.gemm(L.GEMM_WGRAD, x, dy, out, m=256, n=n, k=128)
   torch.cuda.synchronize()
   assert torch.equal(_bits(before), _bits(buf))
+
+
+# ---------------------------------------------------------------------------------------------- non-finite input
+@pytest.mark.gpu
+@pytest.mark.parametrize('impl', [0, 1])
+@pytest.mark.parametrize('n', [256, 128, 64])
+def test_non_finite_rows(ops, n, impl):
+  """NaN and +-inf in designated rows of A.  FWD ReLU: a NaN pre-activation stays NaN (torch.relu, jnp.maximum) with
+  mask bit 0, +-inf follows fp64.  DGRAD with mask bits: a masked-out element is 0 whatever the sum (a select).
+  Every other row equals the clean launch bit for bit."""
+  from multinerf_b200 import lib as L
+  rows = {5: float('nan'), 130: float('inf'), 131: -float('inf'), 999: float('nan')}
+  for mode, c in (('fwd', case('fwd', 1000, n, 192, act='relu', bits=True, impl=impl)),
+                  ('dgrad', case('dgrad', 1000, n, 192, mask='bits', impl=impl))):
+    v0, _, _ = run(ops, c, seed=n)
+    v, bufs = layout(c, 'cuda')
+    _fill(c, v, seed=n)
+    for r, x in rows.items():
+      v['a'][r, 7 + r % 100] = x
+    ops.gemm(L.GEMM_FWD if mode == 'fwd' else L.GEMM_DGRAD, v['a'], v['b'], v['out'], impl=impl,
+             **_call_kwargs(c, v))
+    torch.cuda.synchronize()
+    for name in ('out', 'maskbits') if mode == 'fwd' else ('out',):
+      assert G.padding_intact(v[name], bufs[name]), name
+    idx = sorted(rows)
+    others = torch.ones(c['M'], dtype=torch.bool, device='cuda')
+    others[idx] = False
+    assert torch.equal(_bits(v['out'][others]), _bits(v0['out'][others])), f'{mode}: another row changed'
+    a = v['a'][idx]
+    if mode == 'fwd':
+      r = G.ref_fwd(a, v['b'], bias=v['bias'], act_code=G.RELU)
+    else:
+      r = G.ref_dgrad(a, v['b'], maskbits=v['maskbits'][idx])
+    got = v['out'][idx].double()
+    want = r['out'].to(torch.bfloat16).double()
+    for what, f in (('NaN', torch.isnan), ('+inf', torch.isposinf), ('-inf', torch.isneginf)):
+      assert torch.equal(f(got), f(want)), f'{mode} {what}: {int((f(got) != f(want)).sum())} elements differ'
+    if mode == 'fwd':
+      assert bool(torch.isnan(got).any()), 'no NaN reached the output'
+      bits = G.unpack_bits(v['maskbits'][idx], n)
+      assert torch.equal(bits, r['z'] > 0), 'mask bits of the non-finite rows'
+    else:
+      keep = G.unpack_bits(v['maskbits'][idx], n)
+      assert bool((got[~keep] == 0).all()), 'a masked-out element is not 0'
