@@ -11,6 +11,7 @@ The reference runs one process with `jax.pmap`; here it is one process per GPU
 NCCL: all-reduce(mean) of the flat gradient (pmean, train_utils.py:319-321) and
 all-gather of the rendered pixels (train_utils.py:380-388).
 """
+import dataclasses
 import math
 
 import torch
@@ -90,21 +91,16 @@ def check_chunk_config(config, rays_per_rank):
                      'robustnerf patch would straddle two passes')
 
 
-def _ray_rows(rays, lo, hi):
-  """Rows [lo, hi) of flat device rays (every field and the flat near/far/radii): views, no copies."""
-  import dataclasses
-  r = type(rays)(**{f.name: (None if getattr(rays, f.name) is None else getattr(rays, f.name)[lo:hi])
-                    for f in dataclasses.fields(rays)})
-  for extra in ('radii_flat', 'near_flat', 'far_flat'):
-    setattr(r, extra, getattr(rays, extra)[lo:hi])
-  return r
-
-
-def _anneal(mcfg, train_frac):
-  if mcfg.anneal_slope > 0:
-    sl = mcfg.anneal_slope
-    return (sl * train_frac) / ((sl - 1) * train_frac + 1)
-  return 1.0
+def _map_rays(fn, rays, *rest):
+  """Flat device rays whose every set field, and radii_flat, near_flat and far_flat, is `fn` of that field of `rays`
+  and of the same field of each of `rest`."""
+  names = [f.name for f in dataclasses.fields(rays)]
+  out = type(rays)(**dict.fromkeys(names))
+  for name in names + ['radii_flat', 'near_flat', 'far_flat']:
+    v = getattr(rays, name)
+    if v is not None:
+      setattr(out, name, fn(v, *(getattr(r, name) for r in rest)))
+  return out
 
 
 def create_train_step(model: models.Model, config: configs.Config, impl=0, use_graph=False, dataset=None):
@@ -114,14 +110,14 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
   on the device from `cameras` first (train_utils.py:266-268; camera type from `dataset.camtype`
   as train_utils.py:234-237).
 
-  use_graph=True captures the step into two CUDA graphs (forward+backward | clip+Adam+repack,
-  with the NCCL all-reduce between them) after one eager warm-up step; per-step scalars
-  (annealing exponent, learning rate, Adam bias corrections) and the jitter draws live in device
+  use_graph=True captures the step into one CUDA graph after one eager warm-up step; with more than one
+  process, two (forward+backward | clip+Adam+repack, with the NCCL all-reduce between them).  Per-step
+  scalars (annealing exponent, learning rate, Adam bias corrections) and the jitter draws live in device
   buffers that are refreshed before each replay, so train_frac and the step count may advance.
 
   With `config.train_chunk_size` C (0 < C < rays per process), the forward and backward passes run on C rays at a
   time into the same gradients and statistics, and the exchange, clipping and Adam step follow the last pass
-  (passes_fwd_bwd); under use_graph every pass is in one graph.
+  (fwd_bwd); under use_graph every pass is in one graph.
   """
   mcfg = model.mcfg
   camtype = getattr(dataset, 'camtype', camera_utils.ProjectionType.PERSPECTIVE)
@@ -168,26 +164,6 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
   robust_counts = torch.zeros(5, dtype=torch.int32, device=dev) if robust else None   # left zero by every launch
   G = {'state': 0, 'fb': None, 'opt': None, 'rays': None, 'target': None, 'jitter': None,
        'noise': None, 'launches': 0}
-  import os
-  # capturing the NCCL all-reduce inside the step graph has been seen to hang with torch 2.11 / NCCL 2.28: opt-in
-  # only
-  GRAPH_NCCL = os.environ.get('MNRF_GRAPH_NCCL', '0') == '1'
-  EARLY_EXCHANGE = os.environ.get('MNRF_EARLY_EXCHANGE', '0') == '1'
-
-  # Backward runs the levels last to first, so a module's gradient is final once the lowest level that
-  # uses it is done: for 360.gin the NerfMLP segment (34.7 of 36 MB) is final after level 2 and its
-  # all-reduce overlaps the two PropMLP backward levels.
-  def early_segments(n_levels):
-    # Opt-in (MNRF_EARLY_EXCHANGE=1): overlapping the NerfMLP all-reduce with the PropMLP backward.  The backward
-    # kernels are persistent, one CTA per SM with most of its shared memory, so they cannot share SMs with NCCL's
-    # channel CTAs and an overlapped kernel waits for the collective on the SMs it needs.
-    if decay_views or not EARLY_EXCHANGE:
-      return {}                      # weight decay touches every gradient after the last level
-    first_use = {}
-    for i in range(n_levels):
-      mname = 'NerfMLP_0' if (mcfg.single_mlp or i == n_levels - 1) else 'PropMLP_0'
-      first_use.setdefault(mname, i)
-    return {i: mname for mname, i in first_use.items() if i > 0}
 
   def loss_norm(rays):
     """The data loss's per-ray weights and 1 / their sum (train_utils.py:72-136), over all of `rays`."""
@@ -197,21 +173,14 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
     lm_ch = lossmult.shape[-1]
     return lossmult, (1.0 / (lossmult.sum() * (3 if lm_ch == 1 else 1))).reshape(1)
 
-  def fb_begin(rng, rays, target, train_frac, anneal_ptr, whole=None):
-    """Zero the gradients, run the forward pass of every level; returns the context of the backward pass.
-    `whole`: the rays are rows [lo, hi) of a step over whole['B'] rays, whose loss weights and normaliser it carries;
-    the gradients are not zeroed (the step did that before its first pass)."""
+  def fb_begin(rng, rays, target, train_frac, anneal_ptr, whole):
+    """Run the forward pass of every level; returns the context of the backward pass.  The rays are rows [lo, hi)
+    of a step over whole['B'] rays, whose loss weights and normaliser `whole` carries."""
     params = model.params
-    if whole is None:
-      lossmult, inv_denom = loss_norm(rays)
-      params.grads_ext.zero_()
-    else:
-      lossmult, inv_denom = whole['lossmult'][whole['lo']:whole['hi']], whole['inv_denom']
-    states = model.forward_levels(rng if config.randomized else None, rays, train_frac,
-                                  compute_extras=False, want_samples=False, impl=impl,
-                                  anneal_dev=anneal_ptr, loss_config=config, zero_glo=False,
-                                  batch_rays=None if whole is None else whole['B'])
-    return dict(params=params, states=states, rays=rays, target=target, lossmult=lossmult, inv_denom=inv_denom,
+    states = model.forward_levels(rng, rays, train_frac, compute_extras=False, want_samples=False, impl=impl,
+                                  anneal_dev=anneal_ptr, loss_config=config, zero_glo=False, batch_rays=whole['B'])
+    return dict(params=params, states=states, rays=rays, target=target,
+                lossmult=whole['lossmult'][whole['lo']:whole['hi']], inv_denom=whole['inv_denom'],
                 stats=stats_view(params), whole=whole)
 
   def fb_level(ctx, i):
@@ -235,7 +204,7 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
         raw_diffuse=st.heads.get('diffuse'), raw_tint=st.heads.get('tint'),
         extra_dw=st.extra_dw if st.loss_mults is not None else None,
         d_raw_diffuse=st.d_heads.get('diffuse'), d_raw_tint=st.d_heads.get('tint'),
-        batch_rays=None if ctx['whole'] is None else ctx['whole']['B'])
+        batch_rays=ctx['whole']['B'])
     if st.rgb_scale is not None and mcfg.learned_exposure_scaling:
       # d offsets[idx] += [idx > 0] * exposure_values * d_scale   (adjoint of models.py:262-267)
       eidx = rays.exposure_idx[:, 0].long()
@@ -246,7 +215,9 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
 
   def robust_level(ctx, st, is_fine):
     """robustnerf_mask of this level's pixels (train_utils.py:104-108) against the threshold in `threshold_dev`;
-    the final level also writes the stats row: its mask means and the quantile that is the next threshold."""
+    the final level also adds its mask means to the stats row and writes its per-pixel errors to their rows of the
+    batch's buffer, whose quantile, the next threshold, the step takes after its last pass (fwd_bwd).  The mask
+    means divide by the batch's ray count."""
     B = ctx['target'].shape[0]
     p = config.patch_size
     if not config.enable_robustnerf_loss and B % (p * p) != 0:
@@ -258,38 +229,10 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
                            enable=config.enable_robustnerf_loss)
     row = stats_rows(ctx['params'])[-1] if is_fine else None
     whole = ctx['whole']
-    if whole is not None:
-      # one pass of a longer step: the final level's errors go to their rows of the batch's buffer, whose quantile
-      # the step takes after its last pass (passes_fwd_bwd); the mask means divide by the batch's ray count
-      mask, _ = ops.robust_mask(st.comp['rgb'], ctx['target'], threshold_dev, desc,
-                                error=whole['err'][whole['lo']:whole['hi']] if is_fine else None,
-                                counts=robust_counts if is_fine else None, stats=row, batch_rays=whole['B'])
-      return mask
-    mask, err = ops.robust_mask(st.comp['rgb'], ctx['target'], threshold_dev, desc,
-                                counts=robust_counts if is_fine else None, stats=row)
-    if is_fine:
-      ops.quantile(err, config.robustnerf_inlier_quantile, out=row[0:1])
+    mask, _ = ops.robust_mask(st.comp['rgb'], ctx['target'], threshold_dev, desc,
+                              error=whole['err'][whole['lo']:whole['hi']] if is_fine else None,
+                              counts=robust_counts if is_fine else None, stats=row, batch_rays=whole['B'])
     return mask
-
-  def split_level(n_levels, world, B):
-    """Level after whose backward the first gradient segment is final (None: exchange everything at the end, as a
-    step of several passes always does: a gradient is final only after the last pass)."""
-    early = early_segments(n_levels) if world > 1 and n_passes(B) == 1 else {}
-    return (max(early), early[max(early)]) if early else (None, None)
-
-  def exchange_early(params, mname):
-    o, cnt = params.offsets[mname]
-    return dist.all_reduce(params.grads_ext[o:o + cnt], op=dist.ReduceOp.SUM, async_op=True), (o, o + cnt)
-
-  def exchange_rest(params, done, pending):
-    """Everything not yet exchanged (contiguous ranges of the flat buffer, statistics tail included)."""
-    pos = 0
-    for lo, hi in sorted(done) + [(params.grads_ext.numel(), params.grads_ext.numel())]:
-      if lo > pos:
-        dist.all_reduce(params.grads_ext[pos:lo], op=dist.ReduceOp.SUM)
-      pos = hi
-    for w in pending:
-      w.wait()
 
   def n_passes(B):
     """Forward/backward passes of a step over B rays per process (Config.train_chunk_size)."""
@@ -317,10 +260,11 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
       out['bg'].append(torch.rand(B, 3, device=dev, generator=rng) if lo != hi else None)
     return out
 
-  def passes_fwd_bwd(rng, rays, target, train_frac, anneal_ptr):
-    """Forward + backward of a step over B rays in B / train_chunk_size passes, accumulated into the same
-    gradients and statistics.  The loss normalisers, the random draws and the robustnerf quantile are the whole
-    batch's; the level buffers have the pass's shape and every pass reuses them."""
+  def fwd_bwd(rng, rays, target, train_frac, anneal_ptr):
+    """Forward + backward of a step over B rays in n_passes(B) passes, each running every level forward and then
+    backward, last level to first, into the same gradients and statistics; weight decay follows the last pass.  The
+    loss normalisers, the random draws and the robustnerf quantile are the whole batch's; the level buffers have the
+    pass's shape and every pass reuses them."""
     params = model.params
     B = rays.origins.shape[0]
     C = B // n_passes(B)
@@ -335,36 +279,14 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
     for lo in range(0, B, C):
       rows = None if rand is None else {k: [None if v is None else v.reshape(B, -1)[lo:lo + C] for v in vs]
                                         for k, vs in rand.items()}
-      ctx = fb_begin(rows, _ray_rows(rays, lo, lo + C), target[lo:lo + C], train_frac, anneal_ptr,
+      ctx = fb_begin(rows, _map_rays(lambda v: v[lo:lo + C], rays), target[lo:lo + C], train_frac, anneal_ptr,
                      whole=dict(B=B, lo=lo, hi=lo + C, lossmult=lossmult, inv_denom=inv_denom, err=err))
       for i in range(len(ctx['states']) - 1, -1, -1):
         fb_level(ctx, i)
     if robust:
       ops.quantile(err, config.robustnerf_inlier_quantile, out=stats_rows(params)[-1][0:1])
-
-  def fwd_bwd(rng, rays, target, train_frac, anneal_ptr, world=1):
-    """Eager step body: forward, backward last level to first, gradient exchange (world > 1)."""
-    if n_passes(rays.origins.shape[0]) > 1:
-      passes_fwd_bwd(rng, rays, target, train_frac, anneal_ptr)
-      if decay_views:
-        weight_decay()
-      if world > 1:
-        exchange_rest(model.params, [], [])
-      return
-    ctx = fb_begin(rng, rays, target, train_frac, anneal_ptr)
-    n = len(ctx['states'])
-    split, seg = split_level(n, world, rays.origins.shape[0])
-    pending, done = [], []
-    for i in range(n - 1, -1, -1):
-      fb_level(ctx, i)
-      if i == split:
-        w, rng_ = exchange_early(ctx['params'], seg)
-        pending.append(w)
-        done.append(rng_)
     if decay_views:
       weight_decay()
-    if world > 1:
-      exchange_rest(ctx['params'], done, pending)
 
   def weight_decay():
     # loss += mult * sum(w^2)  ->  grad += 2 mult w ; the loss value goes to stats row 0, slot 6
@@ -484,7 +406,8 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
       # eager step (also the warm-up that allocates every buffer before a capture)
       if robust:
         stage_threshold(loss_threshold, in_dyn=False)
-      fwd_bwd(draw_randomness(rng, B, sched) if use_graph else rng, rays, target, train_frac, None, world)
+      fwd_bwd(draw_randomness(rng, B, sched) if use_graph else rng, rays, target, train_frac, None)
+      allreduce_flat_(params, world)
       optim(grad_scale, params.step, lr, None)
       G['state'] = 1 if use_graph else 0
       G['B'] = B
@@ -493,81 +416,43 @@ def create_train_step(model: models.Model, config: configs.Config, impl=0, use_g
       raise ValueError(f'graph mode needs a fixed batch size ({G["B"]} rays per rank), got {B}')
     rand = draw_randomness(rng, B, sched)
     host_thr = float(loss_threshold) if robust and not torch.is_tensor(loss_threshold) else 1.0
-    set_dyn(params.step, lr, _anneal(mcfg, train_frac), host_thr)
+    set_dyn(params.step, lr, sched[-1]['anneal'], host_thr)
     if robust:
       stage_threshold(loss_threshold, in_dyn=True)
     if G['state'] == 1:
       # capture: inputs live in static buffers from now on
-      import dataclasses
-      G['rays'] = rays
-      G['rays'] = type(rays)(**{f.name: (None if getattr(rays, f.name) is None else getattr(rays, f.name).clone())
-                                for f in dataclasses.fields(rays)})
-      for extra in ('radii_flat', 'near_flat', 'far_flat'):
-        setattr(G['rays'], extra, getattr(rays, extra).clone())
+      G['rays'] = _map_rays(torch.clone, rays)
       G['target'] = target.clone()
       torch.cuda.synchronize()
       before = ops.LAUNCHES
-      n_lv = len(sched)
-      split, seg = split_level(n_lv, world, B)
-      G['split'] = None
-      if world > 1 and not GRAPH_NCCL:
-        # NCCL stays outside the graphs (capturing it hung on this stack, round 2): the step is two graphs around
-        # the exchange, or THREE when a gradient segment is final early -- [forward + backward down to the split
-        # level] | async all-reduce of that segment | [remaining backward levels] | all-reduce of the rest |
-        # [clip + Adam + repack] -- so the big NerfMLP exchange overlaps the PropMLP backward
-        G['fb'] = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(G['fb']):
-          if n_passes(B) > 1:
-            fwd_bwd(rand, G['rays'], G['target'], train_frac, anneal_dev)     # every pass, no exchange
-          else:
-            ctx = fb_begin(rand, G['rays'], G['target'], train_frac, anneal_dev)
-            for i in range(n_lv - 1, (split if split is not None else 0) - 1, -1):
-              fb_level(ctx, i)
-            if split is None and decay_views:
-              weight_decay()
-        if split is not None:
-          G['split'] = seg
-          G['fb2'] = torch.cuda.CUDAGraph()
-          with torch.cuda.graph(G['fb2'], pool=G['fb'].pool()):
-            for i in range(split - 1, -1, -1):
-              fb_level(ctx, i)
+      # one graph for the whole step; with more than one process, NCCL stays outside the graphs (capturing the
+      # all-reduce has been seen to hang): forward + backward | all-reduce | clip + Adam + repack
+      G['fb'] = torch.cuda.CUDAGraph()
+      with torch.cuda.graph(G['fb']):
+        fwd_bwd(rand, G['rays'], G['target'], train_frac, anneal_dev)
+        if world == 1:
+          optim(grad_scale, params.step, lr, dyn)
+      if world > 1:
         G['opt'] = torch.cuda.CUDAGraph()
         with torch.cuda.graph(G['opt']):
           optim(grad_scale, params.step, lr, dyn)
-      else:
-        # ONE graph for the whole step: forward, backward, (world > 1: the gradient all-reduces, captured on
-        # NCCL's stream as parallel branches), clip + Adam + weight repack
-        G['fb'] = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(G['fb']):
-          fwd_bwd(rand, G['rays'], G['target'], train_frac, anneal_dev, world)
-          optim(grad_scale, params.step, lr, dyn)
-        G['opt'] = None
       G['launches'] = ops.LAUNCHES - before
       G['state'] = 2
     else:
-      import dataclasses
-      # one fused multi-tensor copy of the step's inputs into the graph's static buffers
-      dsts, srcs = [G['target']], [target]
-      for name in [f.name for f in dataclasses.fields(rays)] + ['radii_flat', 'near_flat', 'far_flat']:
-        v = getattr(rays, name)
-        if v is not None:
-          dsts.append(getattr(G['rays'], name))
-          srcs.append(v)
+      # one fused multi-tensor copy per dtype pair of the step's inputs into the graph's static buffers
       by_dtype = {}
-      for d_, s_ in zip(dsts, srcs):
-        by_dtype.setdefault((d_.dtype, s_.dtype), ([], []))
-        by_dtype[(d_.dtype, s_.dtype)][0].append(d_)
-        by_dtype[(d_.dtype, s_.dtype)][1].append(s_)
-      for (dd, ss) in by_dtype.values():
-        torch._foreach_copy_(dd, ss, non_blocking=True)
+
+      def stage(src, dst):
+        dsts, srcs = by_dtype.setdefault((dst.dtype, src.dtype), ([], []))
+        dsts.append(dst)
+        srcs.append(src)
+      stage(target, G['target'])
+      _map_rays(stage, rays, G['rays'])
+      for dsts, srcs in by_dtype.values():
+        torch._foreach_copy_(dsts, srcs, non_blocking=True)
     G['fb'].replay()
     if G['opt'] is not None:
-      if G['split'] is not None:
-        w, rng_ = exchange_early(params, G['split'])
-        G['fb2'].replay()
-        exchange_rest(params, [rng_], [w])
-      else:
-        allreduce_flat_(params, world)
+      allreduce_flat_(params, world)
       G['opt'].replay()
     ops.LAUNCHES += G['launches']
     return state, LazyStats(stats_rows(params).clone(), n, grad_scale, robust_cfg), rng
@@ -651,17 +536,6 @@ def allreduce_flat_(params, world):
   return 1.0 / world
 
 
-def allreduce_mean_(grads, stats, world):
-  """pmean of gradients and stats (train_utils.py:319-321): SUM all-reduce here, the 1/world
-  factor is applied to the gradient inside clip_adam (grad_scale) and to the stats in place."""
-  if world <= 1:
-    return 1.0
-  dist.all_reduce(grads, op=dist.ReduceOp.SUM)
-  dist.all_reduce(stats, op=dist.ReduceOp.SUM)
-  stats.div_(world)
-  return 1.0 / world
-
-
 def create_render_fn(model: models.Model, use_graph=False):
   """render_eval_pfn(variables, train_frac, _, rays): deterministic render of this rank's rays,
   with the per-rank pixel buffers all-gathered (train_utils.py:377-396).
@@ -669,7 +543,6 @@ def create_render_fn(model: models.Model, use_graph=False):
   use_graph=True replays one captured CUDA graph per (chunk size, train_frac): a full image is ~100 chunks
   of the same shape, and at 8 GPUs a 16384-ray chunk leaves 2048 rays per rank, where the ~45 launches of
   a forward pass cost more host time than device time.  Ragged chunks (the last one) run eagerly."""
-  import dataclasses
   G = {}
 
   def render_eval_fn(variables, train_frac, _, rays):
@@ -690,13 +563,8 @@ def create_render_fn(model: models.Model, use_graph=False):
       G[key] = {'graph': None}
       renderings, ray_history = model.call_prepped(None, r, lead, train_frac, True)
       return gather_renderings(renderings, world), ray_history
-    fields = [f.name for f in dataclasses.fields(r) if getattr(r, f.name) is not None] + \
-        ['radii_flat', 'near_flat', 'far_flat']
     if ent['graph'] is None:
-      ent['rays'] = type(r)(**{f.name: (None if getattr(r, f.name) is None else getattr(r, f.name).clone())
-                               for f in dataclasses.fields(r)})
-      for extra in ('radii_flat', 'near_flat', 'far_flat'):
-        setattr(ent['rays'], extra, getattr(r, extra).clone())
+      ent['rays'] = _map_rays(torch.clone, r)
       torch.cuda.synchronize()
       before = ops.LAUNCHES
       ent['graph'] = torch.cuda.CUDAGraph()
@@ -704,8 +572,7 @@ def create_render_fn(model: models.Model, use_graph=False):
         ent['out'] = model.call_prepped(None, ent['rays'], lead, train_frac, True)
       ent['launches'] = ops.LAUNCHES - before
     else:
-      for name in fields:
-        getattr(ent['rays'], name).copy_(getattr(r, name), non_blocking=True)
+      _map_rays(lambda src, dst: dst.copy_(src, non_blocking=True), r, ent['rays'])
     ent['graph'].replay()
     ops.LAUNCHES += ent['launches']
     renderings, ray_history = ent['out']

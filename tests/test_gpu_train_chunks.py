@@ -308,6 +308,51 @@ def test_train_loop_with_gin_bound_chunks(mods, tmp_path):
   assert checkpoints.latest_checkpoint(ck).endswith('checkpoint_8')
 
 
+def test_generator_step_equals_explicit_draws(mods):
+  """9. An eager one-pass step driven by a seeded torch.Generator draws, per level and in this order, the jitter, the
+  bottleneck noise, the density noise and the background colours: the same step given those draws explicitly, taken
+  from a copy of the generator, computes the same per-sample values bit for bit and consumes no other draw."""
+  models, train_utils = mods
+  from multinerf_b200 import utils
+  B = 256
+  b = mini360()
+  b.prop_mlp.density_noise = b.nerf_mlp.density_noise = 1.0
+  b.nerf_mlp.bottleneck_noise = 1.0
+  b.model.bg_intensity_range = (0.0, 1.0)
+  b.config.batch_size = B
+  m = b.model
+  rays, rng = synth_rays(17, B, 0.2, 1e6)
+  target = rng.uniform(0, 1, (B, 3)).astype(F32)
+  gen = torch.Generator(device='cuda').manual_seed(23)
+  copy = torch.Generator(device='cuda')
+  copy.set_state(gen.get_state())
+  rand = {'jitter': [], 'bottleneck_noise': [], 'density_noise': [], 'bg': []}
+  for i in range(m.num_levels):
+    fine = i == m.num_levels - 1
+    S = m.num_nerf_samples if fine else m.num_prop_samples
+    rand['jitter'].append(torch.rand((B,) if m.single_jitter else (B, S), device='cuda', generator=copy))
+    rand['bottleneck_noise'].append(
+        torch.randn(B * S, b.nerf_mlp.bottleneck_width, device='cuda', generator=copy) if fine else None)
+    rand['density_noise'].append(torch.randn(B, S, device='cuda', generator=copy))
+    rand['bg'].append(torch.rand(B, 3, device='cuda', generator=copy))
+  runs = []
+  for draws in (gen, rand):
+    model, variables = models.construct_model(9, rays, b)
+    step_fn = train_utils.create_train_step(model, b.config)
+    step_fn(draws, train_utils.TrainState(variables), utils.Batch(rays=rays, rgb=target), None, 0.5)
+    torch.cuda.synchronize()
+    runs.append(model)
+  assert torch.equal(gen.get_state(), copy.get_state())
+  gs, es = _levels(runs[0], B), _levels(runs[1], B)
+  assert len(gs) == len(es) == m.num_levels
+  for i, (g, e) in enumerate(zip(gs, es)):
+    assert g.bneck_noise is not None if i == m.num_levels - 1 else g.bneck_noise is None, i
+    assert g.noise is not None and g.bg_rgb is not None, i
+    for key in ('sdist', 'raw_density', 'd_raw_density'):
+      assert torch.equal(getattr(g, key), getattr(e, key)), (i, key)
+    assert torch.equal(g.comp['weights'], e.comp['weights']), (i, 'weights')
+
+
 def test_validation_before_device_work(mods):
   models, train_utils = mods
   from multinerf_b200 import utils
