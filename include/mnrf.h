@@ -210,6 +210,9 @@ typedef struct {
   int32_t grid;       /* persistent CTAs */
   int32_t pingpong;   /* FWD / DGRAD: 1 each consumer warpgroup runs whole 128 x 128 sub-tiles of the 128 x block_n
                          tiles, alternating, so one's epilogue runs under the other's MMAs; 0 both run each tile */
+  int32_t epilogue;   /* ping-pong DGRAD epilogue operand set, compiled into its instance: 1 mask bits by TMA only,
+                         2 mask bits by TMA and the rank-1 term rowv (x) colv; 0 any operands, tested at run time
+                         (also every other instance) */
 } mnrf_gemm_instance;
 int mnrf_gemm_plan(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
                    const float* rowv, const float* colv, const mnrf_bf16* mask, const uint32_t* maskbits,

@@ -177,19 +177,56 @@ __device__ __forceinline__ void wgrad_side_sums(const GemmParams& p, int t, uint
   }
 }
 
+// MNRF_GEMM_CLOCKS: a build for measurement only.  The first thread of each consumer warpgroup of CTA 0 of
+// gemm_tc_pingpong_kernel splits its clock64() time into the classes below and adds them to g_gemm_clk[warpgroup]
+// at the end of the launch (mnrf_gemm_clocks reads them).  Without it GemmClk is empty and tick() compiles to nothing.
+enum { GK_TURN, GK_FULL, GK_MMA, GK_EPI_LOOP, GK_EPI_SYNC, GK_MASK, GK_N };
+#ifdef MNRF_GEMM_CLOCKS
+__device__ unsigned long long g_gemm_clk[2][GK_N];
+struct GemmClk {
+  long long t[GK_N] = {};
+  long long last = 0;
+  __device__ __forceinline__ void start() { last = clock64(); }
+  __device__ __forceinline__ void tick(int k) {
+    const long long now = clock64();
+    t[k] += now - last;
+    last = now;
+  }
+};
+#else
+struct GemmClk {
+  __device__ __forceinline__ void start() {}
+  __device__ __forceinline__ void tick(int) {}
+};
+#endif
+
+// DGRAD epilogue operand sets (mnrf_gemm_instance.epilogue).  The ping-pong kernel has an instance per set, so the
+// model's DGRADs run an epilogue that tests no optional operand; the generic set tests each at run time.
+enum { EPI_GENERIC = 0, EPI_BITS_TMA = 1, EPI_BITS_TMA_RANK1 = 2 };
+
 // The FWD / DGRAD epilogue of one consumer warpgroup, from the accumulator fragment of wgmma m64nNC (per thread:
 // acc[4i + 2h + e] is row 16*warp + lane/4 + 8h, column 8i + 2*(lane%4) + e of the warpgroup's 64 x NC block):
 // FWD bias, then ReLU and mask bits or a smooth a(z) | DGRAD rank-1 term, mask bits (from the TMA-loaded mask block
 // at m_tile if mask_tma, else from global memory), bf16 mask or a'(z), addend and, if do_cs, column sums into the
-// warp's shared-memory slice at cs_lane.  The block is rows [r0, r0 + 64) of the 128-row tile m_blk and columns
+// warp's shared-memory slice at cs_lane.  DGRAD operand set OPS other than EPI_GENERIC fixes which of these are
+// present at compile time.  The block is rows [r0, r0 + 64) of the 128-row tile m_blk and columns
 // [ncol0, ncol0 + NC); warpgroup wg (0 or 1) owns named barrier 2 + wg and staging blocks [wg * SB, wg * SB + SB).
-// TS: the bf16 output goes through a ring of SB (1 or 2) staging blocks of [64 rows x 64 cols], one TMA bulk store
-// per 64 columns; else it is stored from registers.
-template <int MODE, int NC, bool TS, int SB, bool SMOOTH>
+// TS: the bf16 output goes through a ring of SB (1 to 3) staging blocks of [64 rows x 64 cols], one TMA bulk store
+// per 64 columns; else it is stored from registers.  SB = 3 carries the ring position `sblk` across calls (a
+// call stages two or four blocks); with SB = 1 or 2 block j of a call uses staging block j % SB.
+template <int MODE, int NC, bool TS, int SB, bool SMOOTH, int OPS = EPI_GENERIC>
 __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const CUtensorMap* tmap_c, const float (&acc)[NC / 2],
                                               int m_blk, int r0, int ncol0, int wg, uint8_t* smem_c, bool mask_tma,
-                                              uint32_t m_tile, bool do_cs, uint32_t cs_lane) {
+                                              uint32_t m_tile, bool do_cs, uint32_t cs_lane, int& sblk, GemmClk& clk) {
   constexpr int MW = mask_words(NC);
+  static_assert(OPS == EPI_GENERIC || (MODE == MNRF_GEMM_DGRAD && TS && !SMOOTH && MW > 0),
+                "fixed operand sets are DGRAD epilogues of the staged store with TMA-loaded mask bits");
+  constexpr bool kFixed = OPS != EPI_GENERIC;
+  const bool has_rowv = kFixed ? OPS == EPI_BITS_TMA_RANK1 : p.rowv != nullptr;
+  const bool has_bits = kFixed || p.maskbits != nullptr;
+  const bool bits_tma = kFixed || mask_tma;
+  const bool has_mask = !kFixed && p.mask != nullptr;
+  const bool has_addend = !kFixed && p.addend != nullptr;
   const int lane = threadIdx.x & 31;
   const int r_in = r0 + (16 * ((threadIdx.x >> 5) & 3) + (lane >> 2));   // this thread's row (h = 0) in the tile
   const int cq = 2 * (lane & 3);
@@ -206,8 +243,8 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const CUtenso
     rows[h] = (int64_t)m_blk * BLOCK_M + r_in + 8 * h;
     row_ok[h] = rows[h] < p.m;
     if (MODE == MNRF_GEMM_DGRAD && row_ok[h]) {
-      if (p.rowv) rv[h] = p.rowv[rows[h]];
-      if (p.maskbits && !mask_tma)
+      if (has_rowv) rv[h] = p.rowv[rows[h]];
+      if (has_bits && !bits_tma)
         mrow[h] = p.maskbits + (p.mask_mod > 0 ? rows[h] % p.mask_mod : rows[h]) * p.ldmaskbits;
     }
   }
@@ -216,15 +253,18 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const CUtenso
 #pragma unroll
   for (int i = 0; i < NC / 8; ++i) {
     const int col = ncol0 + 8 * i + cq;
+    const int sb = SB == 3 ? sblk : (i >> 3) & (SB - 1);   // TS: the block's staging block
     if (TS && SB == 1 && (i & 7) == 0) {
       // the previous bulk store must have finished reading the staging block
+      clk.tick(GK_EPI_LOOP);
       if (leader) tma_store_wait_read<0>();
       named_bar_sync(2 + wg, 128);
+      clk.tick(GK_EPI_SYNC);
     }
-    if (MODE == MNRF_GEMM_DGRAD && p.maskbits && (i & 3) == 0) {
+    if (MODE == MNRF_GEMM_DGRAD && has_bits && (i & 3) == 0) {
 #pragma unroll
       for (int h = 0; h < 2; ++h)
-        mw[h] = mask_tma ? ld_shared_u32(m_row + (8 * h * MW + (i >> 2)) * 4)
+        mw[h] = bits_tma ? ld_shared_u32(m_row + (8 * h * MW + (i >> 2)) * 4)
                          : row_ok[h] ? __ldg(mrow[h] + (col >> 5)) : 0u;
     }
     float v[2][2];
@@ -256,10 +296,10 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const CUtenso
       }
     } else {
       float2 cv = make_float2(0.f, 0.f);
-      if (p.rowv) cv = __ldg(reinterpret_cast<const float2*>(p.colv + col));
+      if (has_rowv) cv = __ldg(reinterpret_cast<const float2*>(p.colv + col));
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        if (p.rowv) { v[h][0] += rv[h] * cv.x; v[h][1] += rv[h] * cv.y; }
+        if (has_rowv) { v[h][0] += rv[h] * cv.x; v[h][1] += rv[h] * cv.y; }
         if constexpr (SMOOTH) {
           if (row_ok[h]) {
             const int64_t zr = p.mask_mod > 0 ? rows[h] % p.mask_mod : rows[h];
@@ -267,15 +307,15 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const CUtenso
             v[h][0] *= act_d1(p.act, bf16_lo(zz));
             v[h][1] *= act_d1(p.act, bf16_hi(zz));
           }
-        } else if (p.maskbits) {
+        } else if (has_bits) {
           if (!((mw[h] >> (col & 31)) & 1u)) v[h][0] = 0.f;
           if (!((mw[h] >> ((col + 1) & 31)) & 1u)) v[h][1] = 0.f;
-        } else if (p.mask && row_ok[h]) {
+        } else if (has_mask && row_ok[h]) {
           const uint32_t mm = __ldg(reinterpret_cast<const unsigned int*>(p.mask + rows[h] * p.ldmask + col));
           if (!(bf16_lo(mm) > 0.f)) v[h][0] = 0.f;
           if (!(bf16_hi(mm) > 0.f)) v[h][1] = 0.f;
         }
-        if (p.addend && row_ok[h]) {
+        if (has_addend && row_ok[h]) {
           const uint32_t aa = __ldg(reinterpret_cast<const unsigned int*>(p.addend + rows[h] * p.ldadd + col));
           v[h][0] += bf16_lo(aa);
           v[h][1] += bf16_hi(aa);
@@ -300,9 +340,8 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const CUtenso
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       if (TS) {
-        // staging block (i / 8) % SB, row r_in - r0 + 8h, 16-byte chunk (i % 8) ^ (row % 8), byte 2 * cq
-        st_shared_u32(c_row + ((i >> 3) & (SB - 1)) * STAGING_BLOCK_BYTES + h * (8 * 128) +
-                          (((i & 7) ^ ((lane >> 2) & 7)) << 4),
+        // staging block sb, row r_in - r0 + 8h, 16-byte chunk (i % 8) ^ (row % 8), byte 2 * cq
+        st_shared_u32(c_row + sb * STAGING_BLOCK_BYTES + h * (8 * 128) + (((i & 7) ^ ((lane >> 2) & 7)) << 4),
                       pack_bf16(v[h][0], v[h][1]));
       } else if (row_ok[h]) {
         *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + rows[h] * p.ldc + col) =
@@ -321,14 +360,17 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const CUtenso
     }
     if (TS && (i & 7) == 7) {
       fence_proxy_async();                      // generic-proxy writes -> visible to the bulk store (async proxy)
-      // SB = 2: the store of the previous block, in the staging block that the next block overwrites, has been read
-      if (SB == 2 && leader) tma_store_wait_read<0>();
+      clk.tick(GK_EPI_LOOP);
+      // SB >= 2: the store of block j - SB + 1, in the staging block that block j + 1 overwrites, has been read
+      if (SB >= 2 && leader) tma_store_wait_read<SB - 2>();
       named_bar_sync(2 + wg, 128);
       if (leader) {                             // TMA clips the rows past M
-        tma_store_2d(tmap_c, smem_c + (wg * SB + ((i >> 3) & (SB - 1))) * STAGING_BLOCK_BYTES, ncol0 + 8 * (i & ~7),
+        tma_store_2d(tmap_c, smem_c + (wg * SB + sb) * STAGING_BLOCK_BYTES, ncol0 + 8 * (i & ~7),
                      (int)((int64_t)m_blk * BLOCK_M + r0));
         tma_store_commit();
       }
+      if (SB == 3) sblk = sblk == 2 ? 0 : sblk + 1;
+      clk.tick(GK_EPI_SYNC);
     }
   }
 }
@@ -504,8 +546,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         continue;
       }
       if (mask_tma) mbar_wait(&mask_full[it % MASK_BUFS], (it / MASK_BUFS) & 1, 5);
+      int sblk = 0;                             // not read: SB < 3
+      GemmClk clk;                              // the split covers the ping-pong kernel only
+      clk.start();
       gemm_epilogue<MODE, BN, TS, SB, SMOOTH>(p, &tmap_c, acc, m_blk, 64 * c, ncol0, c, smem_c, mask_tma,
-                                              smem_u32(mask_s) + (it % MASK_BUFS) * (BLOCK_M * MW * 4), do_cs, cs_lane);
+                                              smem_u32(mask_s) + (it % MASK_BUFS) * (BLOCK_M * MW * 4), do_cs, cs_lane,
+                                              sblk, clk);
       if (mask_tma) {                           // this warp has read its mask words: the buffer may be refilled
         __syncwarp();
         if (lane == 0) mbar_arrive(&mask_empty[it % MASK_BUFS]);
@@ -542,19 +588,23 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
 // for bit.  Staged store only; no column sums, no smooth activation.
 constexpr int PP_BN = 128;             // sub-tile width
 constexpr int PP_STAGES = 5;           // operand ring: 5 x 32 KB
-constexpr int PP_SB = 2;               // staging blocks per warpgroup (a sub-tile stages 4 blocks of 64 x 64)
+// staging blocks per warpgroup (a sub-tile stages 4 blocks of 64 x 64).  DGRAD: three, so that before the bulk
+// store of block j the leader waits only for block j - 2's to have been read, not for block j - 1's, issued just
+// before.  FWD keeps two: with three, its 1024-wide layers measured slower (DESIGN.md section 3).
+constexpr int pp_staging_blocks(int mode) { return mode == MNRF_GEMM_DGRAD ? 3 : 2; }
 // DGRAD mask blocks by TMA, sub-tile it in buffer it % PP_MASK_BUFS: four, so that the producer loads sub-tile
 // it + 2's mask and operands while sub-tile it's epilogue still reads its mask block
 constexpr int PP_MASK_BUFS = 4;
 constexpr int pp_smem_bytes(int mode) {
-  return PP_STAGES * (A_STAGE_BYTES + PP_BN * BLOCK_K * 2) + 2 * PP_SB * STAGING_BLOCK_BYTES +
+  return PP_STAGES * (A_STAGE_BYTES + PP_BN * BLOCK_K * 2) + 2 * pp_staging_blocks(mode) * STAGING_BLOCK_BYTES +
          (mode == MNRF_GEMM_DGRAD ? PP_MASK_BUFS * BLOCK_M * mask_words(PP_BN) * 4 : 0) + 256 /*barriers*/ +
          1024 /*align*/;
 }
 
 // Accumulator fragments of the two wgmma m64n128 of a sub-tile (per consumer thread): acc[g][4i + 2h + e] is row
-// 64g + 16*warp + lane/4 + 8h, column 8i + 2*(lane%4) + e of the warpgroup's 128 x 128 sub-tile.
-template <int MODE, int BN>
+// 64g + 16*warp + lane/4 + 8h, column 8i + 2*(lane%4) + e of the warpgroup's 128 x 128 sub-tile.  OPS: the DGRAD
+// epilogue operand set (EPI_GENERIC for FWD).
+template <int MODE, int BN, int OPS>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                         const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_m,
@@ -563,7 +613,7 @@ gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
   constexpr int B_STAGE = PP_BN * BLOCK_K * 2;
   constexpr int SUB = BN / PP_BN;        // sub-tiles per tile
   constexpr int MW = mask_words(PP_BN);
-  constexpr int SB = PP_SB;
+  constexpr int SB = pp_staging_blocks(MODE);
   constexpr bool kDgrad = (MODE == MNRF_GEMM_DGRAD);
   static_assert(MODE != MNRF_GEMM_WGRAD && (BN == 128 || BN == 256), "FWD / DGRAD tiles of 128 or 256 columns");
   extern __shared__ uint8_t smem_dyn[];
@@ -582,7 +632,7 @@ gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
   const int wg = threadIdx.x >> 7;
   const int total_tiles = p.num_m_blocks * p.num_n_blocks;
   const int nk = p.num_k_blocks;         // k-blocks of every sub-tile
-  const bool mask_tma = kDgrad && p.mask_tma;
+  const bool mask_tma = kDgrad && (OPS != EPI_GENERIC || p.mask_tma);
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_a);
@@ -640,6 +690,9 @@ gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
     setmaxnreg_inc<232>();
     const int c = wg - 1;
     float acc[2][64];
+    int sblk = 0;                                // SB = 3: the warpgroup's next staging block
+    GemmClk clk;
+    clk.start();
     for (int it = c; ; it += 2) {                // sub-tile it: column block it % SUB of the CTA's tile it / SUB
       const int tile = blockIdx.x + (it / SUB) * (int)gridDim.x;
       if (tile >= total_tiles) break;
@@ -650,13 +703,16 @@ gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
       // the ring slots of this sub-tile: the producer fills nk per sub-tile, in order
       const uint32_t slot = (uint32_t)it * (uint32_t)nk;
       uint32_t stage = slot % STAGES, phase = (slot / STAGES) & 1;
+      clk.tick(GK_EPI_LOOP);
       // the other warpgroup has issued every wgmma of sub-tile it - 1
       if (it > 0) mbar_wait(&mma_turn[c], ((it - 1) >> 1) & 1, 7);
+      clk.tick(GK_TURN);
       int prev = -1;
       fence_acc(acc[0]);
       fence_acc(acc[1]);
       for (int kb = 0; kb < nk; ++kb) {
         mbar_wait(&full_bar[stage], phase, 3);
+        clk.tick(GK_FULL);
         const uint32_t sa = smem_u32(smem_a + stage * A_STAGE_BYTES);
         const uint32_t sb = smem_u32(smem_b + stage * B_STAGE);
         wgmma_fence();
@@ -673,6 +729,7 @@ gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
         if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
         prev = (int)stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        clk.tick(GK_MMA);
       }
       // every wgmma of this sub-tile is issued: the other warpgroup's next sub-tile may start
       if (blockIdx.x + ((it + 1) / SUB) * (int)gridDim.x < total_tiles) {
@@ -683,16 +740,18 @@ gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
       fence_acc(acc[0]);
       fence_acc(acc[1]);
       if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      clk.tick(GK_MMA);
 
       // ---- epilogue: rows [64g, 64g + 64) of the sub-tile from acc[0], one 64 x 64 staging block per 8 columns.
       // A rolled loop that moves acc[1] into acc[0] for its second pass: unrolled, nvcc hoists the second half's
       // loads into the first and the DGRAD instances spill 2.4 KB.
       const uint32_t m_base = smem_u32(mask_s) + (it % PP_MASK_BUFS) * (BLOCK_M * MW * 4);
       if (mask_tma) mbar_wait(&mask_full[it % PP_MASK_BUFS], (it / PP_MASK_BUFS) & 1, 5);
+      clk.tick(GK_MASK);
 #pragma unroll 1
       for (int g = 0; g < 2; ++g) {
-        gemm_epilogue<MODE, PP_BN, true, SB, false>(p, &tmap_c, acc[0], m_blk, 64 * g, ncol0, c, smem_c, mask_tma, m_base,
-                                                    false, 0);
+        gemm_epilogue<MODE, PP_BN, true, SB, false, OPS>(p, &tmap_c, acc[0], m_blk, 64 * g, ncol0, c, smem_c, mask_tma,
+                                                         m_base, false, 0, sblk, clk);
 #pragma unroll
         for (int e = 0; e < 64; ++e) acc[0][e] = acc[1][e];   // rows [64, 128) next
       }
@@ -702,16 +761,34 @@ gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
       }
     }
     if ((threadIdx.x & 127) == 0) tma_store_wait_all();
+#ifdef MNRF_GEMM_CLOCKS
+    clk.tick(GK_EPI_SYNC);
+    if (blockIdx.x == 0 && (threadIdx.x & 127) == 0)
+      for (int k = 0; k < GK_N; ++k) atomicAdd(&g_gemm_clk[c][k], (unsigned long long)clk.t[k]);
+#endif
   }
 }
 
 // ------------------------------------------------------------------------------------ host
-template <int MODE, int BN>
+template <int MODE, int BN, int OPS = EPI_GENERIC>
 static int launch_gemm_tc_pingpong(int grid, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
                                    const CUtensorMap& tm, const GemmParams& p, cudaStream_t stream) {
   constexpr int kSmem = pp_smem_bytes(MODE);
   static_assert(kSmem <= 232448, "shared memory budget");
-  return launch_tc<gemm_tc_pingpong_kernel<MODE, BN>>(grid, NUM_THREADS, kSmem, stream, ta, tb, tc, tm, p);
+  return launch_tc<gemm_tc_pingpong_kernel<MODE, BN, OPS>>(grid, NUM_THREADS, kSmem, stream, ta, tb, tc, tm, p);
+}
+
+// DGRAD ping-pong at tile width BN, in the instance of its epilogue operand set
+template <int BN>
+static int launch_dgrad_pingpong(int ops, int grid, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
+                                 const CUtensorMap& tm, const GemmParams& p, cudaStream_t stream) {
+  switch (ops) {
+    case EPI_BITS_TMA:
+      return launch_gemm_tc_pingpong<MNRF_GEMM_DGRAD, BN, EPI_BITS_TMA>(grid, ta, tb, tc, tm, p, stream);
+    case EPI_BITS_TMA_RANK1:
+      return launch_gemm_tc_pingpong<MNRF_GEMM_DGRAD, BN, EPI_BITS_TMA_RANK1>(grid, ta, tb, tc, tm, p, stream);
+  }
+  return launch_gemm_tc_pingpong<MNRF_GEMM_DGRAD, BN>(grid, ta, tb, tc, tm, p, stream);
 }
 
 template <int MODE, int BN, bool TS, bool SIDE, bool SMOOTH = false>
@@ -814,6 +891,11 @@ static int gemm_tc_plan(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_
   // FWD and DGRAD run the ping-pong schedule (gemm_tc_pingpong_kernel) wherever it has an epilogue: staged store,
   // whole 128-column sub-tiles, ReLU or no activation, no column sums.
   const bool pingpong = d->mode != MNRF_GEMM_WGRAD && ts && d->n % PP_BN == 0 && !smooth && !colsum;
+  // The ping-pong DGRAD epilogue's operand set: mask bits by TMA, with or without the rank-1 term (rowv and colv
+  // come together), and nothing else has an instance of its own; any other combination runs the generic one.
+  int epilogue = EPI_GENERIC;
+  if (pingpong && d->mode == MNRF_GEMM_DGRAD && mask_tma && !mask && !addend)
+    epilogue = colv ? EPI_BITS_TMA_RANK1 : EPI_BITS_TMA;
   const int tiles = num_m_blocks * num_n_blocks * num_splits;
   plan->block_n = block_n;
   plan->staged = ts;
@@ -824,6 +906,7 @@ static int gemm_tc_plan(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_
   plan->tiles = tiles;
   plan->grid = std::min(tiles, workers);
   plan->pingpong = pingpong;
+  plan->epilogue = epilogue;
   p->num_m_blocks = num_m_blocks;
   p->num_n_blocks = num_n_blocks;
   p->num_k_blocks = num_k_blocks;
@@ -859,10 +942,10 @@ static int launch_gemm_tc_plan(int mode, const mnrf_gemm_instance& plan, const C
   if (plan.pingpong) {
     if (bn == 256)
       return fwd ? launch_gemm_tc_pingpong<MNRF_GEMM_FWD, 256>(grid, ta, tb, tc, tm, p, stream)
-                 : launch_gemm_tc_pingpong<MNRF_GEMM_DGRAD, 256>(grid, ta, tb, tc, tm, p, stream);
+                 : launch_dgrad_pingpong<256>(plan.epilogue, grid, ta, tb, tc, tm, p, stream);
     if (bn == 128)
       return fwd ? launch_gemm_tc_pingpong<MNRF_GEMM_FWD, 128>(grid, ta, tb, tc, tm, p, stream)
-                 : launch_gemm_tc_pingpong<MNRF_GEMM_DGRAD, 128>(grid, ta, tb, tc, tm, p, stream);
+                 : launch_dgrad_pingpong<128>(plan.epilogue, grid, ta, tb, tc, tm, p, stream);
   } else if (plan.smooth) {
     return gemm_tc_smooth_launch(mode, bn, grid, ta, tb, tc, p, stream);
   } else if (mode == MNRF_GEMM_WGRAD) {
@@ -960,4 +1043,15 @@ extern "C" int mnrf_gemm_plan(const mnrf_gemm_desc* d, const mnrf_bf16* a, const
   return mnrf::gemm_tc_plan(d, a, b, bias, colv, mask, maskbits, colsum, addend, out, bsum, side_w, side_aw, z, ldz,
                             plan, &p);
 }
+
+#ifdef MNRF_GEMM_CLOCKS
+// measurement build only: read (and clear) the ping-pong kernel's clock64() classes, [warpgroup][class], summed since
+// the last call
+extern "C" int mnrf_gemm_clocks(unsigned long long* out) {
+  unsigned long long zero[2 * mnrf::GK_N] = {};
+  if (cudaDeviceSynchronize() != cudaSuccess) return 1;
+  if (cudaMemcpyFromSymbol(out, mnrf::g_gemm_clk, sizeof(zero)) != cudaSuccess) return 1;
+  return cudaMemcpyToSymbol(mnrf::g_gemm_clk, zero, sizeof(zero)) != cudaSuccess;
+}
+#endif
 #endif

@@ -43,7 +43,7 @@ class GemmDesc(C.Structure):
 class GemmInstance(C.Structure):
   _fields_ = [('block_n', C.c_int32), ('staged', C.c_int32), ('mask_tma', C.c_int32), ('smooth', C.c_int32),
               ('side', C.c_int32), ('splits', C.c_int32), ('tiles', C.c_int32), ('grid', C.c_int32),
-              ('pingpong', C.c_int32)]
+              ('pingpong', C.c_int32), ('epilogue', C.c_int32)]
 
 
 class HeadInstance(C.Structure):
