@@ -1,12 +1,15 @@
 #!/usr/bin/env python
-"""Mesh extraction entry point: the surface of the newest checkpoint's final-level density as a PLY file.
+"""Mesh extraction entry point: the surface of the newest checkpoint's scene as a PLY file.
 
-  python extract_mesh.py --gin_configs=configs/360.gin --gin_bindings="Config.checkpoint_dir = '...'" \
+  python extract_mesh.py --gin_configs=configs/360.gin --gin_bindings="Config.checkpoint_dir = '...'" \\
       --gin_bindings="Config.mesh_level = 10." --gin_bindings="Config.mesh_resolution = 512"
 Writes <checkpoint_dir>/mesh/mesh_step_<step>.ply (multinerf_b200/mesh.py; Config.mesh_bbox sets the box, and
-forward-facing scenes must set it; Config.mesh_vertex_colors = True adds vertex normals and colours).  One process on
-one GPU.
+forward-facing scenes must set it; Config.mesh_vertex_colors = True adds vertex normals and colours).
+Config.mesh_method = 'density' (default) meshes the final level's density at Config.mesh_level; 'tsdf' renders every
+training view, fuses the rendered depth into a truncated signed-distance grid (Config.mesh_tsdf_truncation cells) and
+meshes its zero crossing.  One process on one GPU.
 """
+import dataclasses
 import os
 import sys
 import time
@@ -15,7 +18,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 import torch  # noqa: E402
 
-from multinerf_b200 import checkpoints, configs, mesh, train_utils  # noqa: E402
+from multinerf_b200 import checkpoints, configs, datasets, mesh, train_utils  # noqa: E402
 from train import parse  # noqa: E402
 
 
@@ -23,15 +26,26 @@ def main(argv=None):
   args = parse(argv)
   bundle = configs.load_config(args.gin_configs, args.gin_bindings, search_paths=[ROOT, os.getcwd()])
   config = bundle.config
+  method = mesh.validate_config(bundle)
   bbox = mesh.default_bbox(bundle)
   if checkpoints.latest_checkpoint(config.checkpoint_dir) is None:
     raise FileNotFoundError(f'no checkpoint in {config.checkpoint_dir!r}')
   model, state, _, _, _ = train_utils.setup_model(bundle, 20200823)
   state = checkpoints.restore_checkpoint(config.checkpoint_dir, state, model=model)
   step = int(state.step)
+  if method == 'tsdf':
+    # every training camera, all pixels, no render path
+    dataset = datasets.load_dataset('train', config.data_dir, dataclasses.replace(config, render_path=False),
+                                    device=model.device)
   t0 = time.time()
-  vertices, faces, *extra = mesh.extract_mesh(model, bbox, config.mesh_resolution, config.mesh_level,
-                                              colors=config.mesh_vertex_colors)
+  if method == 'tsdf':
+    vertices, faces, *extra = mesh.extract_mesh_tsdf(model, dataset, bbox, config.mesh_resolution,
+                                                     config.mesh_tsdf_truncation, colors=config.mesh_vertex_colors)
+    what = f'{dataset.size} views fused, truncation {config.mesh_tsdf_truncation} cells'
+  else:
+    vertices, faces, *extra = mesh.extract_mesh(model, bbox, config.mesh_resolution, config.mesh_level,
+                                                colors=config.mesh_vertex_colors)
+    what = f'level {config.mesh_level}'
   torch.cuda.synchronize()
   elapsed = time.time() - t0
   out_dir = os.path.join(config.checkpoint_dir, 'mesh')
@@ -39,8 +53,7 @@ def main(argv=None):
   path = os.path.join(out_dir, f'mesh_step_{step}.ply')
   mesh.write_ply(path, vertices, faces, *extra)
   print(f'{vertices.shape[0]} vertices, {faces.shape[0]} faces in {elapsed:.2f} s '
-        f'(grid {config.mesh_resolution} along the longest side of {bbox}, level {config.mesh_level}) -> {path}',
-        flush=True)
+        f'(grid {config.mesh_resolution} along the longest side of {bbox}, {what}) -> {path}', flush=True)
   return path
 
 

@@ -616,6 +616,9 @@ int mnrf_pack_weights_batched(int32_t count, const mnrf_pack_item* items, int32_
  *                per cut edge in edge order, and faces [F, 3] int32 (V < 2^31) in cell order, wound so that normals
  *                point from inside to outside.
  * The mesh of a level set that stays off the grid boundary is closed and consistently wound.
+ * A NaN grid point is unobserved: a cell with a NaN corner has no triangles, an edge with a NaN end is not cut, and
+ * an edge is cut only if at least one cell it borders has eight non-NaN corners, so every vertex is used by a face.
+ * On grids without NaN the output does not depend on this rule.
  */
 enum { MNRF_MC_COUNT = 0, MNRF_MC_EMIT = 1 };
 int mnrf_marching_cubes(int32_t phase, int32_t nx, int32_t ny, int32_t nz, const float* grid, float level,
@@ -626,11 +629,32 @@ int mnrf_marching_cubes(int32_t phase, int32_t nx, int32_t ny, int32_t nz, const
  * writes normals [V, 3], one unit vector per cut edge at the edge's rank -- the order of EMIT's vertices, so
  * normals[i] belongs to vertices[i].  The gradient of the grid at each end of the edge is taken by central
  * differences (one-sided on the grid boundary), the two are interpolated with the vertex's t, and the normal is
- * -g / |g|: from dense to empty space, the side the faces' winding faces.  Where g is zero or not finite the normal
+ * -g / |g|: from dense to empty space, the side the faces' winding faces.  The difference is one-sided next to a
+ * NaN neighbour too; where both neighbours along an axis are NaN or missing, or g is zero or not finite, the normal
  * is the edge's direction from its inside end to its outside end.  Cells are cubes, so the normals hold in world
  * space too. */
 int mnrf_mc_normals(int32_t nx, int32_t ny, int32_t nz, const float* grid, float level, const uint8_t* edge_cut,
                     const int64_t* edge_scan, float* normals, mnrf_stream stream);
+
+/* Truncated signed-distance fusion of rendered depth maps into the grid points lo + h (x, y, z) of an [nz, ny, nx]
+ * grid (each side in [2, 1024]; the points are rounded to fp32 from fp64, as mesh.density_grid places them).
+ * cam: the camera model -- camtype, has_distortion, k1..k4, p1, p2 are read; num_cameras is the number of
+ * camera-to-pixel matrices (1, shared, or num_views); has_ndc must be 0; the other fields are not read.
+ * worldtocams [num_views, 3, 4]: world -> camera (OpenGL axes, the inverse of camtoworld); camtopixs
+ * [num_cameras, 3, 3]: the inverse of pixtocam; depth, acc [num_views, height, width] fp32: each view's median
+ * distance and opacity, distances in the units of the rays' directions; rgb [num_views, height, width, 3] or NULL.
+ * State, updated in place: tsdf, weight [nz * ny * nx]; with rgb, color_sum [N, 3] and color_weight [N].
+ * Per point and view, in view order: the view is skipped when the point has no pixel (behind a perspective camera,
+ * theta = pi of a fisheye), its pixel (floor(u), floor(v)) is off the image or the depth is not finite.
+ * d = depth - t (t: the point's parameter along its pixel's ray) where acc >= 0.5, +inf otherwise (the median
+ * distance sits at `far`); skipped when d < -tau; else tsdf = (weight tsdf + min(d, tau) / tau) / (weight + 1),
+ * weight += 1, and where |d| <= tau, color_sum += rgb, color_weight += 1.  One thread per point, no atomics: the
+ * state depends on the views and their order, not on how they are split into calls. */
+int mnrf_tsdf_integrate(const mnrf_camera_desc* cam, int32_t nx, int32_t ny, int32_t nz, double x0, double y0,
+                        double z0, double h, int32_t num_views, int32_t height, int32_t width,
+                        const float* worldtocams, const float* camtopixs, const float* depth, const float* acc,
+                        const float* rgb, float tau, float* tsdf, float* weight, float* color_sum,
+                        float* color_weight, mnrf_stream stream);
 
 #ifdef __cplusplus
 }

@@ -30,7 +30,7 @@ def _nvcc():
 
 
 # sources a unit includes besides the shared headers
-INCLUDES = {'gemm_tc_act.cu': ['gemm_tc.cu'], 'mesh.cu': ['mc_tables.cuh']}
+INCLUDES = {'gemm_tc_act.cu': ['gemm_tc.cu'], 'mesh.cu': ['mc_tables.cuh', 'camera.cuh'], 'camera.cu': ['camera.cuh']}
 
 
 def _stamp(path, flags):

@@ -125,6 +125,11 @@ class Config:
   mesh_bbox: Optional[Tuple[float, ...]] = None
   # also write vertex normals and colours (each vertex's radiance seen head-on from outside, GLO zeroed)
   mesh_vertex_colors: bool = False
+  # 'density': marching cubes on the density grid at mesh_level; 'tsdf': render the training views, fuse their
+  # median distances into a truncated signed-distance grid and mesh its zero crossing (no level to choose; vertex
+  # colours are the rendered colours).  mesh_tsdf_truncation: the band, in cells (>= 1).
+  mesh_method: str = 'density'
+  mesh_tsdf_truncation: float = 3.
 
 
 @dataclasses.dataclass

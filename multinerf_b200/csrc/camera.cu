@@ -9,71 +9,17 @@
 // `xnp=jnp` path of train_utils.py:266-268 (Config.cast_rays_in_train_step).
 // HBM-bound: reads 12 B (pixel + camera index; the camera matrices stay in L1/L2), writes 48 B
 // per ray.  Compiled without FMA contraction so the fp32 rounding follows the reference's
-// unfused elementwise graph.
-#include "common.cuh"
+// unfused elementwise graph.  The camera model itself (camera_dir) is in camera.cuh, shared with the TSDF fusion
+// of mesh.cu.
+#include "camera.cuh"
 
 namespace mnrf {
-
-template <typename T> struct Vec3 { T x, y, z; };
-using V3 = Vec3<float>;
 
 // mip-NeRF cone radius from the distances to the dx / dy neighbours: the std of a unit box is 1/sqrt(12)
 constexpr double kSqrt12 = 3.4641016151377544;
 template <typename T>
 __device__ __forceinline__ T cone_radius(T dx_norm, T dy_norm) {
   return (T(0.5) * (dx_norm + dy_norm)) * T(2) / T(kSqrt12);
-}
-
-template <typename T>
-__device__ __forceinline__ Vec3<T> mat3_vec(const T* __restrict__ m, int ld, Vec3<T> v) {
-  Vec3<T> r;
-  r.x = m[0] * v.x + m[1] * v.y + m[2] * v.z;
-  r.y = m[ld] * v.x + m[ld + 1] * v.y + m[ld + 2] * v.z;
-  r.z = m[2 * ld] * v.x + m[2 * ld + 1] * v.y + m[2 * ld + 2] * v.z;
-  return r;
-}
-
-__device__ __forceinline__ void undistort(const mnrf_camera_desc& d, float xd, float yd, float& xo, float& yo) {
-  float x = xd, y = yd;
-  const float k1 = d.k1, k2 = d.k2, k3 = d.k3, k4 = d.k4, p1 = d.p1, p2 = d.p2;
-  for (int it = 0; it < d.undistort_iters; ++it) {
-    const float r = x * x + y * y;
-    const float dd = 1.0f + r * (k1 + r * (k2 + r * (k3 + r * k4)));
-    const float fx = dd * x + 2.f * p1 * x * y + p2 * (r + 2.f * x * x) - xd;
-    const float fy = dd * y + 2.f * p2 * x * y + p1 * (r + 2.f * y * y) - yd;
-    const float d_r = k1 + r * (2.0f * k2 + r * (3.0f * k3 + r * 4.0f * k4));
-    const float d_x = 2.0f * x * d_r;
-    const float d_y = 2.0f * y * d_r;
-    const float fx_x = dd + d_x * x + 2.0f * p1 * y + 6.0f * p2 * x;
-    const float fx_y = d_y * x + 2.0f * p1 * x + 2.0f * p2 * y;
-    const float fy_x = d_x * y + 2.0f * p2 * y + 2.0f * p1 * x;
-    const float fy_y = dd + d_y * y + 2.0f * p2 * x + 6.0f * p1 * y;
-    const float den = fy_x * fx_y - fx_x * fy_y;
-    const float xn = fx * fy_y - fy * fx_y;
-    const float yn = fy * fx_x - fx * fy_x;
-    const bool ok = fabsf(den) > d.undistort_eps;
-    x = x + (ok ? xn / den : 0.f);
-    y = y + (ok ? yn / den : 0.f);
-  }
-  xo = x; yo = y;
-}
-
-// camera-space direction of pixel centre (px, py): inverse intrinsics, undistortion, fisheye,
-// OpenCV -> OpenGL flip
-__device__ __forceinline__ V3 camera_dir(const mnrf_camera_desc& d, const float* __restrict__ p2c, float px, float py) {
-  V3 v = mat3_vec(p2c, 3, V3{px + 0.5f, py + 0.5f, 1.0f});
-  if (d.has_distortion) {
-    float x, y;
-    undistort(d, v.x, v.y, x, y);
-    v = V3{x, y, 1.0f};
-  }
-  if (d.camtype == MNRF_CAM_FISHEYE) {
-    float theta = sqrtf(v.x * v.x + v.y * v.y);
-    theta = fminf(3.14159274101257324f, theta);
-    const float s = sinf(theta) / theta;
-    v = V3{v.x * s, v.y * s, cosf(theta)};
-  }
-  return V3{v.x, -v.y, -v.z};
 }
 
 // convert_to_ndc: returns the NDC origin; `dir` is overwritten with the NDC direction

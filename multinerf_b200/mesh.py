@@ -7,6 +7,13 @@ a uniform cell of side h, so the grid samples the anti-aliased field at the foot
 IPE does at the footprint of a ray interval.  With `colors=True` each vertex also gets a unit normal from the
 density grid's gradient and a colour from `Model.query_radiance`, seen along the inward normal.  `write_ply` stores
 the result as binary little-endian PLY.
+
+`extract_mesh_tsdf(model, dataset, bbox, resolution, truncation)` (Config.mesh_method = 'tsdf') meshes what the
+renders show instead: it renders every camera of `dataset`, fuses each pixel's median distance into a truncated
+signed-distance grid on the same points (`fuse_tsdf`, `ops.tsdf_integrate`, csrc/mesh.cu), and extracts the zero
+crossing where the grid was observed.  No density level is chosen; space a camera saw through is carved away; space
+no camera saw gives no faces (marching cubes skips cells with an unobserved, NaN, corner); and a vertex's colour is
+the mean of the colours rendered for it across the views whose surface lies within the truncation band.
 """
 import math
 
@@ -90,6 +97,129 @@ def vertex_colors(model, vertices, normals, var):
   of side h)."""
   _, rgb = model.query_radiance(vertices, var, -normals)
   return (rgb.clamp(0, 1) * 255).round().to(torch.uint8)
+
+
+MESH_METHODS = ('density', 'tsdf')
+
+
+def validate_config(bundle):
+  """The mesh method of `bundle`'s Config, checked: 'density' or 'tsdf'; the TSDF method needs perspective or fisheye
+  views (not NDC) and a truncation of at least one cell, so no cut edge of the fused grid has an unobserved end."""
+  config = bundle.config
+  if config.mesh_method not in MESH_METHODS:
+    raise ValueError(f'Config.mesh_method = {config.mesh_method!r}: want one of {MESH_METHODS}')
+  if config.mesh_method == 'tsdf':
+    if config.forward_facing:
+      raise ValueError("Config.mesh_method = 'tsdf' does not support forward-facing (NDC) scenes")
+    if not config.mesh_tsdf_truncation >= 1:
+      raise ValueError(f'Config.mesh_tsdf_truncation = {config.mesh_tsdf_truncation!r}: want at least 1 cell')
+  return config.mesh_method
+
+
+def camera_matrices(cameras, device):
+  """(worldtocams [N, 3, 4], camtopixs [N or 1, 3, 3]) fp32 on `device` from a dataset's (pixtocams, camtoworlds,
+  ...): the inverses, computed in fp64 and rounded once."""
+  pixtocams, camtoworlds = (np.asarray(c.detach().cpu() if isinstance(c, torch.Tensor) else c, np.float64)
+                            for c in cameras[:2])
+  c2w = camtoworlds.reshape(-1, *camtoworlds.shape[-2:])[:, :3, :4]
+  rot_t = np.transpose(c2w[:, :, :3], (0, 2, 1))
+  w2c = np.concatenate([rot_t, -rot_t @ c2w[:, :, 3:]], -1)
+  c2p = np.linalg.inv(pixtocams.reshape(-1, 3, 3))
+  to = lambda a: torch.tensor(a, dtype=torch.float32, device=device).contiguous()
+  return to(w2c), to(c2p)
+
+
+def fuse_tsdf(views, cameras, camtype, bbox, resolution, truncation, colors=False, batch=8, device='cuda'):
+  """Fuse rendered views into a TSDF on the grid of `bbox` at `resolution` (grid_shape; the points density_grid
+  uses).  views: iterable of (cam_idx, depth [H, W], acc [H, W], rgb [H, W, 3] or None) device tensors -- each
+  view's median distance (in the units of its rays' directions), opacity and colour; cameras: (pixtocams,
+  camtoworlds, distortion_params, pixtocam_ndc) as a dataset holds them; camtype: camera_utils.ProjectionType or its
+  value; truncation: the band in cells.  Views are fused `batch` at a time, in order; the result does not depend on
+  `batch`.  Returns ((tsdf, weight, color_sum, color_weight), h): [nz, ny, nx] fp32 grids ([nz, ny, nx, 3] for
+  color_sum; the colour pair is None without `colors`) and the cell size."""
+  from . import camera_utils
+  if cameras[3] is not None:
+    raise ValueError('TSDF fusion does not support NDC cameras')
+  camtype = camera_utils.ProjectionType(camtype.value if hasattr(camtype, 'value') else camtype)
+  (nx, ny, nz), h = grid_shape(bbox, resolution)
+  w2c, c2p = camera_matrices(cameras, device)
+  tau = float(truncation) * h
+  z = lambda *sh: torch.zeros(nz, ny, nx, *sh, device=device)
+  tsdf, weight = z(), z()
+  color_sum, color_weight = (z(3), z()) if colors else (None, None)
+
+  def flush(items):
+    idx = torch.tensor([v[0] for v in items], device=device)
+    H, W = items[0][1].shape[:2]
+    depth = torch.stack([v[1].reshape(H, W) for v in items]).float()
+    acc = torch.stack([v[2].reshape(H, W) for v in items]).float()
+    rgb = torch.stack([v[3].reshape(H, W, 3) for v in items]).float() if colors else None
+    ops.tsdf_integrate((nx, ny, nz), bbox[:3], h, 0 if camtype == camera_utils.ProjectionType.PERSPECTIVE else 1,
+                       cameras[2], w2c[idx].contiguous(), c2p if c2p.shape[0] == 1 else c2p[idx].contiguous(),
+                       depth, acc, rgb, tau, tsdf, weight, color_sum, color_weight)
+
+  items = []
+  for view in views:
+    items.append(tuple(view))
+    if len(items) == batch:
+      flush(items)
+      items = []
+  if items:
+    flush(items)
+  return (tsdf, weight, color_sum, color_weight), h
+
+
+def tsdf_mesh(state, bbox, h, colors=False):
+  """Marching cubes on the fused TSDF `state` (fuse_tsdf): the zero crossing of -tsdf (inside > 0, so faces and
+  normals point out of the surface), with every point no view observed (weight 0) NaN, so it gives no faces.
+  Returns (vertices, faces) in world coordinates, and with `colors` also (normals [V, 3], rgb [V, 3] uint8): each
+  vertex's colour is color_sum / color_weight interpolated linearly along its grid edge, rounded as vertex_colors
+  rounds."""
+  tsdf, weight, color_sum, color_weight = state
+  grid = torch.where(weight > 0, -tsdf, torch.full_like(tsdf, float('nan')))
+  out = ops.marching_cubes(grid, 0.0, normals=colors)
+  del grid
+  lo = torch.tensor([float(v) for v in bbox[:3]], device=out[0].device)
+  vertices = out[0] * h + lo
+  if not colors:
+    return vertices, out[1]
+  # a vertex lies on a grid edge: its two other coordinates are integers, so the trilinear weights reduce to the
+  # linear interpolation between the edge's two ends
+  nz, ny, nx = tsdf.shape
+  dims = torch.tensor([nx, ny, nz], device=out[0].device)
+  base = torch.minimum(out[0].floor().long(), dims - 2).clamp_min(0)
+  frac = out[0] - base
+  cs = torch.zeros(len(vertices), 3, device=vertices.device)
+  cw = torch.zeros(len(vertices), device=vertices.device)
+  for corner in range(8):
+    off = torch.tensor([corner & 1, corner >> 1 & 1, corner >> 2 & 1], device=vertices.device)
+    wgt = torch.where(off.bool(), frac, 1 - frac).prod(-1)
+    q = base + off
+    p = (q[:, 2] * ny + q[:, 1]) * nx + q[:, 0]
+    cs += wgt[:, None] * color_sum.view(-1, 3)[p]
+    cw += wgt * color_weight.view(-1)[p]
+  rgb = torch.where(cw[:, None] > 0, cs / cw.clamp_min(1e-30)[:, None], torch.zeros_like(cs))
+  return vertices, out[1], out[2], (rgb.clamp(0, 1) * 255).round().to(torch.uint8)
+
+
+def render_views(model, dataset):
+  """Yields (cam_idx, distance_median, acc, rgb) of every camera of `dataset`, rendered by `model` with the
+  graph-replayed render chunks of train_utils.create_render_fn, GLO zeroed, at train_frac 1 (as eval_lib.render)."""
+  from . import models, train_utils
+  render_fn = train_utils.create_render_fn(model, use_graph=True)
+  for idx in range(dataset.size):
+    rays = dataset.generate_ray_batch(idx).rays
+    r = models.render_image(lambda rng_, c: render_fn(model.params, 1., None, c), rays, None, model.config,
+                            verbose=False)
+    yield idx, r['distance_median'], r['acc'], r['rgb']
+
+
+def extract_mesh_tsdf(model, dataset, bbox, resolution, truncation=3.0, colors=False, batch=8):
+  """Config.mesh_method = 'tsdf': render every camera of `dataset` (render_views), fuse the renders (fuse_tsdf, a
+  band of `truncation` cells) and mesh the result (tsdf_mesh).  Returns what extract_mesh returns."""
+  state, h = fuse_tsdf(render_views(model, dataset), dataset.cameras, dataset.camtype, bbox, resolution, truncation,
+                       colors=colors, batch=batch, device=model.device)
+  return tsdf_mesh(state, bbox, h, colors=colors)
 
 
 def write_ply(path, vertices, faces, normals=None, colors=None):

@@ -197,6 +197,26 @@ def marching_cubes(grid, level, normals=False):
   return vertices, faces, vnormals
 
 
+def tsdf_integrate(shape, lo, h, camtype, distortion_params, worldtocams, camtopixs, depth, acc, rgb, tau, tsdf,
+                   weight, color_sum=None, color_weight=None):
+  """Fuse K views into the TSDF state in place (mnrf_tsdf_integrate, csrc/mesh.cu).  shape (nx, ny, nz) and lo, h:
+  the grid points lo + h (x, y, z); camtype 0 perspective / 1 fisheye; distortion_params: dict of k1..k4, p1, p2
+  or None; worldtocams [K, 3, 4], camtopixs [K or 1, 3, 3], depth, acc [K, H, W], rgb [K, H, W, 3] or None, fp32 on
+  the device; tsdf, weight [nz, ny, nx] and, with rgb, color_sum [nz, ny, nx, 3], color_weight [nz, ny, nx]."""
+  lib = L.load()
+  nx, ny, nz = shape
+  K, H, W = depth.shape
+  dp = dict(distortion_params or {})
+  d = L.CameraDesc(0, camtopixs.shape[0], int(camtype), int(distortion_params is not None),
+                   *(float(dp.get(k, 0.0)) for k in ('k1', 'k2', 'k3', 'k4', 'p1', 'p2')), 0.0, 0, 0, 1.0, 1.0, 1.0)
+  _count()
+  L.check(lib.mnrf_tsdf_integrate(C.byref(d), nx, ny, nz, *(float(v) for v in lo), float(h), K, H, W,
+                                  L.ptr(_f32(worldtocams)), L.ptr(_f32(camtopixs)), L.ptr(_f32(depth)),
+                                  L.ptr(_f32(acc)), L.ptr(_f32(rgb)), float(tau), L.ptr(_f32(tsdf)),
+                                  L.ptr(_f32(weight)), L.ptr(_f32(color_sum)), L.ptr(_f32(color_weight)),
+                                  L.stream_ptr()))
+
+
 def viewdir_enc(viewdirs, num_samples, deg, out, col0, col_end):
   lib = L.load()
   B = viewdirs.shape[0]
