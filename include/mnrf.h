@@ -532,6 +532,7 @@ int mnrf_act_tangent_bwd(int64_t M, int32_t n, int32_t act, const mnrf_bf16* z, 
  * optional NDC projection (convert_to_ndc :32-97), mip-NeRF cone radii from the dx/dy neighbours.
  * pixtocams [num_cameras, 3, 3] and camtoworlds [num_cameras, 3, 4] are row-major fp32;
  * cam_idx may be NULL when num_cameras == 1.  Outputs are [num_rays, 3|3|3|1|2] fp32.
+ * Fisheye: sin(theta) / theta is 1 on the optical axis (theta = 0), where the reference's 0 / 0 gives NaN rays.
  */
 #define MNRF_CAM_PERSPECTIVE 0
 #define MNRF_CAM_FISHEYE 1

@@ -45,7 +45,8 @@ __device__ __forceinline__ void undistort(const mnrf_camera_desc& d, float xd, f
 }
 
 // camera-space direction of pixel centre (px, py): inverse intrinsics, undistortion, fisheye,
-// OpenCV -> OpenGL flip
+// OpenCV -> OpenGL flip.  The fisheye's sin(theta) / theta is taken as its limit 1 on the optical axis (theta = 0,
+// the centre pixel of an odd-sized image with cx = W / 2), where the reference divides 0 by 0.
 __device__ __forceinline__ V3 camera_dir(const mnrf_camera_desc& d, const float* __restrict__ p2c, float px, float py) {
   V3 v = mat3_vec(p2c, 3, V3{px + 0.5f, py + 0.5f, 1.0f});
   if (d.has_distortion) {
@@ -56,7 +57,7 @@ __device__ __forceinline__ V3 camera_dir(const mnrf_camera_desc& d, const float*
   if (d.camtype == MNRF_CAM_FISHEYE) {
     float theta = sqrtf(v.x * v.x + v.y * v.y);
     theta = fminf(3.14159274101257324f, theta);
-    const float s = sinf(theta) / theta;
+    const float s = theta > 0.f ? sinf(theta) / theta : 1.0f;
     v = V3{v.x * s, v.y * s, cosf(theta)};
   }
   return V3{v.x, -v.y, -v.z};

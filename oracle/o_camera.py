@@ -90,7 +90,8 @@ def pixels_to_rays(pix_x_int, pix_y_int, pixtocams, camtoworlds, distortion_para
   if camtype == FISHEYE:
     theta = torch.sqrt((cam_dirs[..., :2] ** 2).sum(dim=-1))
     theta = torch.clamp(theta, max=math.pi)
-    s = torch.sin(theta) / theta
+    # the reference divides 0 by 0 on the optical axis (NaN rays); take sin(theta) / theta at its limit 1 there
+    s = torch.where(theta > 0, torch.sin(theta) / theta, torch.ones_like(theta))
     cam_dirs = torch.stack([cam_dirs[..., 0] * s, cam_dirs[..., 1] * s, torch.cos(theta)], dim=-1)
   cam_dirs = cam_dirs * torch.tensor([1.0, -1.0, -1.0], dtype=dtype)     # OpenCV -> OpenGL
   imageplane = cam_dirs[0, ..., :2]

@@ -21,13 +21,16 @@ operation adds its rounding to the errors it inherits.  With u = 2**-24:
                  the result.
   a * b          |a| e_b + |b| e_a + e_a e_b + u |result|.  Products by a power of two (the halvings of cast_one,
                  2^l and 4^l of the degrees, reached in the kernel by exact doubling) add nothing.
-  a / b, sqrt    (e_a + |a / b| e_b) / (|b| - e_b) + u |result|;  sqrt(a) - sqrt(a - e_a) + u |result|: both are
-                 correctly rounded (the library is built without fast-math).
+  a / b, sqrt    (e_a + |a / b| e_b) / (|b| - e_b) + u |result|;  the larger of sqrt(a) - sqrt(max(a - e_a, 0))
+                 and sqrt(a + e_a) - sqrt(a), + u |result|: both are correctly rounded (the library is built without
+                 fast-math).
   constants      4/15 and 5/12 are fp32 constants in the kernel and exact in the reference: relative error u.
   logf, expf     documented at 1 and 2 ulp: 2u and 4u of the result, after the inherited error through the
                  function's own slope.  1/x under `reciprocal` is a division: as s -> 1 the inverse's conditioning
                  enters through e_b / (|b| - e_b).
-  max(c, x)      1-Lipschitz: the error is inherited unchanged.
+  sinf, cosf     documented at 2 ulp without fast math: 4u of the result, after the inherited error through the
+                 slope (used by camera_ref.py).
+  max(c, x)      1-Lipschitz: the error is inherited unchanged; so is min(c, x).
   branches       |x|^2 <= 1 of the contraction and the two halves of `piecewise` are taken on the fp64 value.  Both
                  functions are C^1 across the branch, so a sample within rounding of it moves by O(e^2).
 The second evaluation's values agree with the oracle's to fp64 rounding; their difference is added to the bound, and
@@ -128,9 +131,10 @@ class _V:
   def __rtruediv__(self, o):
     return _V.of(o) / self
 
-  def sqrt(self):
+  def sqrt(self):              # sqrt is concave: the step down bounds the step up unless a - e_a < 0
     v = torch.sqrt(self.val)
-    return self._rounded(v, v - torch.sqrt((self.val - self.err).clamp(min=0)))
+    return self._rounded(v, torch.maximum(v - torch.sqrt((self.val - self.err).clamp(min=0)),
+                                          torch.sqrt(self.val + self.err) - v))
 
   def log(self):
     v = torch.log(self.val)
@@ -143,11 +147,24 @@ class _V:
     e = v * torch.expm1(self.err)
     return _V(v, e + 4 * U * (v + e))
 
-  def scale(self, p):          # by a power of two: exact
-    return _V(self.val * p, self.err * p)
+  def sin(self):               # sinf: 2 ulp (4u of the result); the slope over [v - e, v + e] is <= |cos v| + e
+    v = torch.sin(self.val)
+    e = (torch.cos(self.val).abs() + self.err).clamp(max=1) * self.err
+    return _V(v, e + 4 * U * (v.abs() + e))
+
+  def cos(self):               # cosf: 2 ulp, as sinf
+    v = torch.cos(self.val)
+    e = (torch.sin(self.val).abs() + self.err).clamp(max=1) * self.err
+    return _V(v, e + 4 * U * (v.abs() + e))
+
+  def scale(self, p):          # by a power of two (or its negative): exact
+    return _V(self.val * p, self.err * abs(p))
 
   def maxc(self, c):
     return _V(self.val.clamp(min=c), self.err)
+
+  def minc(self, c):
+    return _V(self.val.clamp(max=c), self.err)
 
   def u(self):                 # a trailing axis to broadcast over
     return _V(self.val[..., None], self.err[..., None])

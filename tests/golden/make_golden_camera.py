@@ -41,6 +41,73 @@ def random_pose(rng):
   return np.concatenate([q, t], axis=1)
 
 
+def forward_pose(rng):
+  w = rng.normal(size=3) * 0.08
+  K = np.array([[0, -w[2], w[1]], [w[2], 0, -w[0]], [-w[1], w[0], 0]])
+  q, _ = np.linalg.qr(np.eye(3) + K + 0.5 * K @ K)
+  q = q * np.sign(np.diag(q))[None, :]
+  return np.concatenate([q, rng.uniform(-0.3, 0.3, (3, 1))], axis=1)
+
+
+def extra_cases(rng, out):
+  """The edges of the camera model, each stored under its own prefix with its inputs: `corners` (the border and
+  corners of the image under strong barrel distortion), `aniso` (fx != fy and off-centre principal points),
+  `widefish` (every pixel of a fisheye whose corners pass theta = pi; even-sized, so no pixel sits on the axis),
+  `ndcwide` (NDC on a non-square image) and `fishcentre` (every pixel of a 5 x 5 fisheye: its centre maps to
+  (0, 0), where sin(theta) / theta is 0 / 0 and the reference returns NaN)."""
+  P, FISH = camera_utils.ProjectionType.PERSPECTIVE, camera_utils.ProjectionType.FISHEYE
+  W, H = 160, 120
+  xs, ys = np.arange(W), np.arange(H)
+  bx = np.concatenate([xs, xs, np.zeros(H, int), np.full(H, W - 1)]).astype(np.int32)
+  by = np.concatenate([np.zeros(W, int), np.full(W, H - 1), ys, ys]).astype(np.int32)
+  grid = lambda w, h: [a.reshape(-1).astype(np.int32) for a in np.meshgrid(np.arange(w), np.arange(h), indexing='xy')]
+  cases = {}
+  cases['corners'] = dict(
+      p2c=np.stack([camera_utils.get_pixtocam(f, W, H) for f in (140.0, 170.0, 200.0)]),
+      poses=np.stack([random_pose(rng) for _ in range(3)]), pix=(bx, by),
+      dist=dict(k1=-0.25, k2=0.03, k3=0.0, k4=0.0, p1=0.0, p2=0.0), camtype=P)
+  aniso = []
+  for _ in range(3):
+    fx = rng.uniform(60, 140)
+    fy = fx * np.exp(rng.uniform(np.log(0.5), np.log(2.0)))
+    aniso.append(np.linalg.inv(camera_utils.intrinsic_matrix(fx, fy, W * rng.uniform(0.4, 0.6),
+                                                             H * rng.uniform(0.4, 0.6))))
+  cases['aniso'] = dict(p2c=np.stack(aniso), poses=np.stack([random_pose(rng) for _ in range(3)]),
+                        pix=(rng.integers(0, W, 300).astype(np.int32), rng.integers(0, H, 300).astype(np.int32)),
+                        camtype=P)
+  cases['widefish'] = dict(p2c=camera_utils.get_pixtocam(8.0, 60, 44)[None], poses=random_pose(rng)[None],
+                           pix=grid(60, 44), camtype=FISH)
+  cases['ndcwide'] = dict(p2c=np.stack([camera_utils.get_pixtocam(f, W, 80) for f in (100.0, 110.0, 90.0)]),
+                          poses=np.stack([forward_pose(rng) for _ in range(3)]),
+                          pix=(rng.integers(0, W, 300).astype(np.int32), rng.integers(0, 80, 300).astype(np.int32)),
+                          ndc=camera_utils.get_pixtocam(100.0, W, 80), camtype=P)
+  cases['fishcentre'] = dict(p2c=camera_utils.get_pixtocam(7.0, 5, 5)[None], poses=random_pose(rng)[None],
+                             pix=grid(5, 5), camtype=FISH)
+  out['fishcentre_size'] = np.array([5, 5], np.int32)
+  for name, c in cases.items():
+    px, py = c['pix']
+    B = px.shape[0]
+    n = c['p2c'].shape[0]
+    cam_idx = (rng.integers(0, n, (B, 1)) if n > 1 else np.zeros((B, 1))).astype(np.int32)
+    out.update({f'{name}_pix_x': px, f'{name}_pix_y': py, f'{name}_cam_idx': cam_idx,
+                f'{name}_pixtocams': c['p2c'], f'{name}_camtoworlds': c['poses']})
+    if c.get('dist'):
+      out[f'{name}_dist_keys'] = np.array(list(c['dist'].keys()))
+      out[f'{name}_dist_vals'] = np.array(list(c['dist'].values()))
+    if c.get('ndc') is not None:
+      out[f'{name}_pixtocam_ndc'] = c['ndc']
+    meta = lambda v: np.full((B, 1), v, F)
+    for tag, xnp, dt in [('f64', np, np.float64), ('f32', jnp, np.float32)]:
+      cams = (c['p2c'].astype(dt), c['poses'].astype(dt), c.get('dist'),
+              None if c.get('ndc') is None else c['ndc'].astype(dt))
+      pixels = utils.Pixels(pix_x_int=px, pix_y_int=py, lossmult=meta(1), near=meta(0.2), far=meta(1e6),
+                            cam_idx=cam_idx)
+      with np.errstate(all='ignore'):
+        rays = camera_utils.cast_ray_batch(cams, pixels, c['camtype'], xnp=xnp)
+      for f in ['origins', 'directions', 'viewdirs', 'radii', 'imageplane']:
+        out[f'{name}_{tag}_{f}'] = np.asarray(getattr(rays, f))
+
+
 def main():
   rng = np.random.default_rng(11)
   out = {}
@@ -91,6 +158,7 @@ def main():
   d = np.array([0., 0., -1.]) + rng.uniform(-.5, .5, (100, 3))
   on, dn = camera_utils.convert_to_ndc(o, d, pixtocam_ndc, 1.0)
   out.update(ndc_in_o=o, ndc_in_d=d, ndc_out_o=on, ndc_out_d=dn)
+  extra_cases(rng, out)
   path = os.path.join(HERE, 'camera.npz')
   np.savez_compressed(path, **out)
   print('camera.npz', len(out), 'arrays')
