@@ -508,7 +508,7 @@ int mnrf_normals_bwd(int64_t M, int32_t num_samples, const float* grad_pred, con
                      float* d_grad_pred, float* d_raw_grad_density, mnrf_bf16* head_grads, int64_t ld_head_grads,
                      float* stats, mnrf_stream stream);
 /* out[r, n] bf16 = maskbit(r mod mask_mod, n) ? rowv[r] * colv[n] : 0 -- the first dY of the
- * density-normal (tangent) backward chain. */
+ * density-normal (tangent) backward chain.  N a multiple of 32, ld a multiple of 8, out 16-byte aligned. */
 int mnrf_outer_mask(int64_t rows, int32_t n, int64_t mask_mod, const float* rowv, const float* colv,
                     const uint32_t* maskbits, int64_t ldmaskbits, mnrf_bf16* out, int64_t ldo,
                     mnrf_stream stream);

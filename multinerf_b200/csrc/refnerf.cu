@@ -567,7 +567,7 @@ extern "C" int mnrf_outer_mask(int64_t rows, int32_t n, int64_t mask_mod, const 
   if (rows == 0) return 0;
   MNRF_CHECK(rowv && colv && out, "mnrf_outer_mask: null pointer");
   MNRF_CHECK(n % 32 == 0 && ldo % 8 == 0, "mnrf_outer_mask: N %% 32 == 0 and ld %% 8 == 0 required");
-  if (rows == 0) return 0;
+  MNRF_CHECK((reinterpret_cast<uintptr_t>(out) & 15) == 0, "mnrf_outer_mask: out must be 16-byte aligned");
   int64_t total = rows * (n / 8);
   int blocks = (int)std::min<int64_t>((total + 255) / 256, (int64_t)mnrf_num_sms() * 16);
   outer_mask_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(rows, n, mask_mod, rowv, colv, maskbits, ldmaskbits,

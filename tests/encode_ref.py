@@ -288,11 +288,134 @@ def bf16_bound(value, bound):
   return bound + 2.0 ** -8 * (value.abs() + bound) + 2.0 ** -134
 
 
+def _contract_terms(x):
+  """contract_terms on the pre-warp mean: xh, s, q, s_r, q_r (the identity's 0, 1, 1, 0, 0 inside the ball) and
+  `unsure`, the samples whose |x|^2 lies within its rounding of 1, where the kernel may take either branch."""
+  m = (x[0] * x[0] + x[1] * x[1] + x[2] * x[2]).maxc(EPS)
+  inside = m.val <= 1
+  unsure = (m.val - 1).abs() <= m.err
+  mo = _V.where(inside, 2.0, m)          # the branch not taken: keep its arithmetic finite
+  r = mo.sqrt()
+  ir = 1.0 / r
+  q_r = -2.0 / (mo * r)
+  pick = lambda v, ident: _V.where(inside, ident, v)
+  return ([pick(x[i] * ir, 0.0) for i in range(3)], pick(2.0 / r - 1.0 / mo, 1.0), pick(1.0 / mo, 1.0),
+          pick((r - 1.0) * q_r, 0.0), pick(q_r, 0.0), unsure)
+
+
+def _lift_tangent(x, cov, basis, disable_integration):
+  """d lift_mean / d x_a and d lift_var / d x_a [3] of [.., K] _V, in gauss_tangent_rows' order, and `unsure`."""
+  xh, s, q, s_r, q_r, unsure = _contract_terms(x)
+  xh = [t.u() for t in xh]
+  s, q, s_r, q_r = s.u(), q.u(), s_r.u(), q_r.u()
+  b = [_V(basis[:, i]) for i in range(3)]
+  cv = [cov[0][0].u(), cov[0][1].u(), cov[0][2].u(), cov[1][1].u(), cov[1][2].u(), cov[2][2].u()]
+  beta = xh[0] * b[0] + xh[1] * b[1] + xh[2] * b[2]
+  bt = [b[i] - beta * xh[i] for i in range(3)]
+  u = [s * bt[i] + (q * beta) * xh[i] for i in range(3)]
+  v = [cv[0] * u[0] + cv[1] * u[1] + cv[2] * u[2], cv[1] * u[0] + cv[3] * u[1] + cv[4] * u[2],
+       cv[2] * u[0] + cv[4] * u[1] + cv[5] * u[2]]
+  gamma = xh[0] * v[0] + xh[1] * v[1] + xh[2] * v[2]
+  vt = [v[i] - gamma * xh[i] for i in range(3)]
+  btv = bt[0] * v[0] + bt[1] * v[1] + bt[2] * v[2]
+  radial = s_r * btv + q_r * (beta * gamma)
+  if disable_integration:
+    dlv = [_V(torch.zeros_like(beta.val)) for _ in range(3)]
+  else:
+    dlv = [(xh[a] * radial + s_r * (beta * vt[a] + gamma * bt[a])).scale(2.0) for a in range(3)]
+  return u, dlv, unsure
+
+
+def _reduced(y):
+  return torch.where(y.abs() < T32, y, torch.remainder(y, T32))
+
+
+def _tangent_features(lm, lv, lm_err, lv_err, dl, basis, min_deg, max_deg):
+  """[3, .., 2KL] d feature / d x_dir in integrated_pos_enc's layout with its fp32 bound.  dl: (dlm, dlv) of
+  _lift_tangent with the contraction, None without it (d lift_mean / d x_dir = basis[k][dir])."""
+  sc_all = 2.0 ** torch.arange(min_deg, max_deg, dtype=torch.float64)
+  out = [[[], []] for _ in range(3)]
+  for sc in sc_all.tolist():
+    y, dy = lm * sc, lm_err * sc
+    v, dv = lv * sc * sc, lv_err * sc * sc
+    e = torch.exp(-0.5 * v)
+    re = torch.expm1((0.5 * dv).clamp(max=40.0)) + (3 + 0.6 * (v.abs() + dv)) * 2 * U
+    E = _V(e, e * re + 2.0 ** -126)        # __expf flushes results below 2^-126 to 0
+    for half in range(2):
+      if half:                   # the kernel reduces y + pi/2 on its own, as the feature rows do
+        y = y + 0.5 * math.pi
+        dy = dy + U * (y.abs() + dy) + abs(HALF_PI32 - 0.5 * math.pi)
+      jumps = (_k_eff(y + dy) - _k_eff(y - dy)).abs()
+      ds = (dy + jumps * JUMP + C_SIN).clamp(max=2.0)
+      arg = _reduced(y)
+      f = E * _V(torch.sin(arg), ds)
+      cs = _V(torch.cos(arg), ds)
+      for a in range(3):
+        if dl is None:
+          t = cs * (_V(basis[:, a] * sc) * E)
+        else:
+          dlm, dlv = dl
+          t = cs * (dlm[a] * E.scale(sc)) - f * dlv[a].scale(0.5 * sc * sc)
+        out[a][half].append(t)
+  shape = lm.shape[:-1] + (-1,)
+  val = torch.stack([torch.cat([torch.stack([t.val for t in out[a][h]], -2).reshape(shape) for h in range(2)], -1)
+                     for a in range(3)])
+  err = torch.stack([torch.cat([torch.stack([t.err for t in out[a][h]], -2).reshape(shape) for h in range(2)], -1)
+                     for a in range(3)])
+  return val, SLACK * err + TINY
+
+
+def tangent_reference(x, cov, lm, lv, lm_err, lv_err, feat_vacuous, basis, *, min_deg, max_deg, warp_contract,
+                      disable_integration):
+  """Tangent rows of gauss_tangent_rows on the pre-warp Gaussian (x [3], cov [3][3] of _V): (value, bound,
+  bound_bf16, vacuous), each [3, .., 2KL], and `unsure` [..], the samples within rounding of |x| = 1.  Vacuous: the feature's own bound says nothing, or (contraction) the
+  sample lies within rounding of |x| = 1, where the q_r term of d lift_var jumps from -2 / r^3 to 0."""
+  b = basis.double()
+  dl = None
+  unsure = torch.zeros(lm.shape[:-1], dtype=torch.bool)
+  if warp_contract:
+    dlm, dlv, unsure = _lift_tangent(x, cov, b, disable_integration)
+    dl = (dlm, dlv)
+  val, bound = _tangent_features(lm, lv, lm_err, lv_err, dl, b, min_deg, max_deg)
+  vac = feat_vacuous[None] | unsure[None, ..., None] | ~torch.isfinite(bound)
+  return val, bound, bf16_bound(val, bound), vac, unsure
+
+
+def points_reference(points, var, basis, *, min_deg, max_deg, warp_contract=False, disable_integration=False):
+  """mnrf_encode_points_tangent: features and tangent rows of the Gaussians (points[i], var I), var and points fp32.
+  Returns feat / bound / bound_bf16 / vacuous [N, 2KL], tangent / tangent_bound / tangent_bound_bf16 /
+  tangent_vacuous [3, N, 2KL] and chain_gap (the running evaluation against the oracle's lift)."""
+  p = torch.as_tensor(points).detach().cpu().double()
+  bd = torch.as_tensor(basis).detach().cpu().double()
+  v32 = 0.0 if disable_integration else float(np.float32(var))
+  x = [_V(p[:, i]) for i in range(3)]
+  cov = [[_V(torch.full_like(p[:, 0], float(np.float32(var)) if i == j else 0.0)) for j in range(3)] for i in range(3)]
+  mean, covw = _contract(x, cov) if warp_contract else (x, cov)
+  lmv, lvv = _lift(mean, covw, bd, disable_integration)
+  covs = (torch.eye(3, dtype=torch.float64) * v32).expand(p.shape[0], 3, 3)
+  om, oc = o_coord.track_linearize_contract(p, covs) if warp_contract else (p, covs)
+  lm, lv = o_coord.lift_and_diagonalize(om, oc, bd.T.contiguous())
+  out = types.SimpleNamespace(lm=lm, lv=lv)
+  out.chain_gap = max(float(((lmv.val - lm).abs() / (lmv.err + 1e-300)).max()),
+                      float(((lvv.val - lv).abs() / (lvv.err + 1e-300)).max()))
+  lm_err, lv_err = lmv.err + (lmv.val - lm).abs(), lvv.err + (lvv.val - lv).abs()
+  out.feat, out.bound = _features(lm, lv, lm_err, lv_err, min_deg, max_deg)
+  out.bound_bf16 = bf16_bound(out.feat, out.bound)
+  out.vacuous = ~(out.bound <= VACUOUS)
+  out.tangent, out.tangent_bound, out.tangent_bound_bf16, out.tangent_vacuous, out.unsure = tangent_reference(
+      x, cov, lm, lv, lm_err, lv_err, out.vacuous, bd, min_deg=min_deg, max_deg=max_deg, warp_contract=warp_contract,
+      disable_integration=disable_integration)
+  return out
+
+
 def reference(sdist, origins, directions, radii, near, far, basis, *, min_deg, max_deg, raydist_fn=None,
-              ray_shape='cone', warp_contract=False, disable_integration=False, tdist=None, dtype=torch.float64):
+              ray_shape='cone', warp_contract=False, disable_integration=False, tdist=None, dtype=torch.float64,
+              tangent=False):
   """fp64 reference of mnrf_encode with per-element bounds.  `tdist`: the kernel's own fp32 tdist to stage the
   Gaussians on (default: the reference's, rounded to fp32).  Returns tdist / tdist_bound [B, S+1], feat / bound /
-  bound_bf16 / vacuous [B, S, 2KL], and the lifted lm, lv [B, S, K] the features were formed from."""
+  bound_bf16 / vacuous [B, S, 2KL], and the lifted lm, lv [B, S, K] the features were formed from; with `tangent`
+  also the tangent rows tangent / tangent_bound / tangent_bound_bf16 / tangent_vacuous [3, B, S, 2KL], `unsure`
+  [B, S] (samples within rounding of |x| = 1) and `xnorm` [B, S], the fp64 |x| of the pre-warp means."""
   if ray_shape not in ('cone', 'cylinder'):
     raise ValueError("ray_shape must be 'cone' or 'cylinder'")
   c = lambda t: t.detach().cpu().to(dtype)
@@ -315,9 +438,8 @@ def reference(sdist, origins, directions, radii, near, far, basis, *, min_deg, m
   out.tdist_bound = SLACK * (tv.err + (tv.val - out.tdist).abs()) + TINY
   t = _V(staged.double())
   ov, dv = [_V(o[:, i:i + 1]) for i in range(3)], [_V(d[:, i:i + 1]) for i in range(3)]
-  mean, cov = _cast(ray_shape, _V(t.val[:, :-1]), _V(t.val[:, 1:]), ov, dv, _V(rad))
-  if warp_contract:
-    mean, cov = _contract(mean, cov)
+  x, xcov = _cast(ray_shape, _V(t.val[:, :-1]), _V(t.val[:, 1:]), ov, dv, _V(rad))
+  mean, cov = _contract(x, xcov) if warp_contract else (x, xcov)
   lmv, lvv = _lift(mean, cov, b, disable_integration)
   # how far the running evaluation's values are from the oracle's: fp64 rounding (asserted in the CPU tests)
   out.chain_gap = max(float(((lmv.val - lm).abs() / (lmv.err + 1e-300)).max()),
@@ -326,6 +448,11 @@ def reference(sdist, origins, directions, radii, near, far, basis, *, min_deg, m
   out.feat, out.bound = _features(lm, lv, out.lm_err, out.lv_err, min_deg, max_deg)
   out.bound_bf16 = bf16_bound(out.feat, out.bound)
   out.vacuous = ~(out.bound <= VACUOUS)
+  if tangent:
+    out.xnorm = torch.sqrt(x[0].val ** 2 + x[1].val ** 2 + x[2].val ** 2)
+    out.tangent, out.tangent_bound, out.tangent_bound_bf16, out.tangent_vacuous, out.unsure = tangent_reference(
+        x, xcov, lm, lv, out.lm_err, out.lv_err, out.vacuous, b, min_deg=min_deg, max_deg=max_deg,
+        warp_contract=warp_contract, disable_integration=disable_integration)
   return out
 
 

@@ -71,7 +71,9 @@ def _fast_act_err(code, z, y):
 
 
 def _fast_d1_err(code, z):
-  """Error of the epilogue's a'(z): the sigmoid's (as above), through d a' / d s = 1 + z (1 - 2s) for SiLU."""
+  """Error of the epilogue's a'(z): the sigmoid's (as above), through d a' / d s = 1 + z (1 - 2s) for SiLU.
+  A closed form that grows with |z|: it says little where |z| is large.  tests/tangent_ref.py (act_derivs) bounds
+  the same a'(z), and a''(z), by a running error that stays tight for any z; the GEMM tests keep this one."""
   s = torch.sigmoid(z)
   return 2 * s * (1 + 2 * z.abs()) * (6 + 1.2 * z.abs()) * 2.0 ** -23
 

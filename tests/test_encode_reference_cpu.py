@@ -201,11 +201,188 @@ def emulate(pos, kw, num_sms=SMS, dirn=1, mut=None):
   return torch.tensor(tdist), torch.tensor(feat[:, :S]), count
 
 
-def check(name, dirn=1, mut=None):
+def _sincos(x, dirn):
+  """safe_sincos_fast: the floor reduction by fl32(100 pi), Cody-Waite by 2 pi, MUFU.SIN / MUFU.COS moved by 2^-21.41."""
+  r = _reduce(x, 3, None)
+  q = rint_small(r * F(0.15915494309189535))
+  r = fma(q, F(1.7484555e-7), fma(-q, F(6.2831854820251465), r))
+  r64 = np.float64(r)
+  return (np.sin(r64) + dirn * 2.0 ** -21.41).astype(F), (np.cos(r64) + dirn * 2.0 ** -21.41).astype(F)
+
+
+def emulate_tangent_rows(x, cov, basis, kw, dirn=1, mut=None):
+  """gauss_tangent_rows' tangent rows of the pre-warp fp32 Gaussians x [3] / cov [3][3] (arrays [..]): contract_terms,
+  store_gauss, the lift and d lift, __expf moved by its documented error, safe_sincos_fast, the bf16 store.
+  Returns [3, .., 2KL] float32 (bf16 values)."""
+  K, L = basis.shape[0], kw['max_deg'] - kw['min_deg']
+  contract, no_int = kw['warp_contract'], kw['disable_integration']
+  with np.errstate(all='ignore'):
+    mean, covw = _contract(x, cov, None) if contract else (x, cov)
+    b = [basis[:, i] for i in range(3)]
+    lm = mean[0][..., None] * b[0] + mean[1][..., None] * b[1] + mean[2][..., None] * b[2]
+    cc = [covw[i][0][..., None] * b[0] + covw[i][1][..., None] * b[1] + covw[i][2][..., None] * b[2] for i in range(3)]
+    lv = np.zeros_like(lm) if no_int else b[0] * cc[0] + b[1] * cc[1] + b[2] * cc[2]
+    if contract:
+      m = np.maximum(F(ER.EPS), x[0] * x[0] + x[1] * x[1] + x[2] * x[2])
+      inside = m <= 1
+      mo = np.where(inside, F(2), m)
+      r = np.sqrt(mo)
+      ir = F(1) / r
+      xh = [np.where(inside, F(0), x[i] * ir)[..., None] for i in range(3)]
+      sj = np.where(inside, F(1), F(2) / r - F(1) / mo)[..., None]
+      qj = np.where(inside, F(1), F(1) / mo)[..., None]
+      q_r = F(-2) / (mo * r)
+      s_r = np.where(inside, F(0), ((r + F(1)) if mut == 's_r_r_plus_1' else (r - F(1))) * q_r)[..., None]
+      q_r = np.where(inside, F(0), q_r)[..., None]
+      cv = [cov[0][0], cov[0][1], cov[0][2], cov[1][1], cov[1][2], cov[2][2]]
+      cv = [c[..., None] for c in cv]
+      beta = xh[0] * b[0] + xh[1] * b[1] + xh[2] * b[2]
+      bt = [b[i] - beta * xh[i] for i in range(3)]
+      u = [(qj if mut == 'u_q_for_s' else sj) * bt[i] + (qj * beta) * xh[i] for i in range(3)]
+      v = [cv[0] * u[0] + cv[1] * u[1] + cv[2] * u[2], cv[1] * u[0] + cv[3] * u[1] + cv[4] * u[2],
+           cv[2] * u[0] + cv[4] * u[1] + cv[5] * u[2]]
+      gamma = xh[0] * v[0] + xh[1] * v[1] + xh[2] * v[2]
+      vt = [v[i] - gamma * xh[i] for i in range(3)]
+      btv = bt[0] * v[0] + bt[1] * v[1] + bt[2] * v[2]
+      radial = s_r * btv + (-q_r if mut == 'q_r_sign' else q_r) * (beta * gamma)
+      two = F(1) if mut == 'dlv_no2' else F(2)
+      dlv = [np.zeros_like(lm) if (no_int or mut == 'no_dlv') else
+             two * (xh[a] * radial + s_r * (beta * vt[a] + gamma * bt[a])) for a in range(3)]
+    out = np.zeros((3,) + lm.shape[:-1] + (2 * K * L,), F)
+    for l in range(L):
+      sc = F(2.0 ** (kw['min_deg'] + l))
+      y, vv = lm * sc, lv * (sc * sc)
+      ex = np.float64(F(-0.5) * vv)
+      e = (np.exp(ex) * (1 + dirn * (1.5 + 1.173 * np.abs(ex)) * 2.0 ** -23)).astype(F)
+      e = np.where(e < F(2.0 ** -126), F(0), e)
+      s0, c0 = _sincos(y, dirn)
+      s1, c1 = _sincos(y + PI2, dirn)
+      fs, fc = e * s0, e * s1
+      for a in range(3):
+        if contract:
+          esc = sc if mut == 'esc_no_e' else e * sc
+          hsc2 = F(0.5) * (sc if mut == 'hsc2_sc' else sc * sc)
+          dm, dvar = u[a] * esc, dlv[a] * hsc2
+          ts, tc = c0 * dm - fs * dvar, c1 * dm - fc * dvar
+        else:
+          bk = (basis.reshape(-1)[a * K:(a + 1) * K] if mut == 'basis_dir_k' else basis[:, a]) * sc * e
+          ts, tc = c0 * bk, c1 * bk
+        out[a, ..., l * K:(l + 1) * K] = ts
+        out[a, ..., K * L + l * K:K * L + (l + 1) * K] = tc
+  return torch.tensor(out).to(torch.bfloat16).float()
+
+
+def _pre_warp(pos, kw):
+  """tdist and the pre-warp Gaussians [B, S] of the general (tangent) encoder, in fp32."""
+  sdist, o, d, radii, near, far, basis = [t.numpy() for t in pos]
+  fn = kw['raydist_fn']
+  with np.errstate(all='ignore'):
+    s_near, s_far = _fwd(fn, near)[:, None], _fwd(fn, far)[:, None]
+    tdist = _inv(fn, sdist * s_far + (F(1) - sdist) * s_near).astype(F)
+    x, cov = _cast(kw['ray_shape'], tdist[:, :-1], tdist[:, 1:], [o[:, i:i + 1] for i in range(3)],
+                   [d[:, i:i + 1] for i in range(3)], radii[:, None], None)
+  return tdist, x, cov
+
+
+def check_tangent(name, dirn=1, mut=None):
+  """(reference, emulated tangent rows [3, B, S, 2KL], mask of broken bounds) of a case."""
+  pos, kw = make_inputs(name, SMS, rays=RAYS)
+  tdist, x, cov = _pre_warp(pos, kw)
+  got = emulate_tangent_rows(x, cov, pos[6].numpy(), kw, dirn, mut)
+  if mut == 'row_dir_seg':              # stream dir at row dir * S + m of the [3 B S] rows instead of dir * B S + m
+    B, S = got.shape[1], got.shape[2]
+    rows = torch.zeros_like(got).view(3 * B * S, -1)
+    for a in range(3):
+      rows[a * S:a * S + B * S] = got[a].reshape(B * S, -1)
+    got = rows.view(got.shape)
+  ref = ER.reference(*pos, **kw, tdist=torch.tensor(tdist), tangent=True)
+  broken = ((got.double() - ref.tangent).abs() > ref.tangent_bound_bf16) & ~ref.tangent_vacuous
+  return ref, got, broken
+
+
+TANGENT_CASES = [n for n in CASES if case(n)['tangent']]
+
+
+@pytest.mark.parametrize('name', TANGENT_CASES)
+def test_tangent_emulation_within_bounds(name):
+  c = case(name)
+  K, L = c['K'], c['max_deg'] - c['min_deg']
+  deg = ER.degree_of(K, L)
+  for dirn in (1, -1):
+    ref, got, broken = check_tangent(name, dirn)
+    ratio = torch.where(ref.tangent_vacuous, torch.zeros_like(ref.tangent),
+                        (got.double() - ref.tangent).abs() / ref.tangent_bound_bf16)
+    assert not broken.any(), (name, dirn, float(ratio.max()), np.unravel_index(int(ratio.argmax()), ratio.shape))
+  checked = 1 - float(ref.tangent_vacuous.double().mean())
+  print(f'\n{name} tangent: worst err/bound per stream ' +
+        ' '.join(f'{float(ratio[a].max()):.2f}' for a in range(3)) + ' | per degree ' +
+        ' '.join(f'{float(ratio[..., deg == l].max()):.2f}' for l in range(L)) +
+        f' | checked {checked:.3f} (floor {c.get("tfloor", c["floor"])})')
+  assert checked >= min(1.0, c.get('tfloor', c['floor']) + 0.02), (name, checked)
+
+
+@pytest.mark.parametrize('warp_contract,disable_integration,var', [
+    (False, False, 1e-4), (True, False, 1e-4), (True, True, 1e-4), (True, False, 0.0), (False, False, 0.0),
+    (True, False, 3e-2)])
+def test_points_tangent_emulation_within_bounds(warp_contract, disable_integration, var):
+  """The point form (mnrf_encode_points_tangent: mean = point, cov = var I) on the point set of
+  test_gpu_mesh_color.test_encode_points_tangent_features_vs_fp64."""
+  from multinerf_b200 import geopoly
+  basis = np.ascontiguousarray(geopoly.generate_basis('octahedron', 2), dtype=F)
+  rng = np.random.default_rng(3)
+  pts = np.concatenate([rng.uniform(-0.57, 0.57, (400, 3)), rng.uniform(-3, 3, (400, 3)),
+                        rng.normal(size=(201, 3)) * 50]).astype(F)
+  kw = dict(min_deg=0, max_deg=12, warp_contract=warp_contract, disable_integration=disable_integration)
+  ref = ER.points_reference(pts, var, basis, **kw)
+  assert ref.chain_gap < 1e-3
+  x = [pts[:, i] for i in range(3)]
+  cov = [[np.full(len(pts), F(var) if i == j else F(0), F) for j in range(3)] for i in range(3)]
+  for dirn in (1, -1):
+    got = emulate_tangent_rows(x, cov, basis, kw, dirn)
+    ratio = torch.where(ref.tangent_vacuous, torch.zeros_like(ref.tangent),
+                        (got.double() - ref.tangent).abs() / ref.tangent_bound_bf16)
+    assert float(ratio.max()) <= 1, (dirn, float(ratio.max()), np.unravel_index(int(ratio.argmax()), ratio.shape))
+  assert float(ref.tangent_vacuous.double().mean()) < 0.4
+  print(f'\npoints contract {warp_contract} no_int {disable_integration} var {var}: worst err/bound '
+        f'{float(ratio.max()):.2f} | checked {1 - float(ref.tangent_vacuous.double().mean()):.3f}')
+
+
+def _autograd_tangent(pos, kw, tdist):
+  """d integrated_pos_enc / d mean of the oracle chain, by forward-mode autograd in fp64: [3, B, S, 2KL]."""
+  from torch.func import jvp
+  sd, o, d, rad, near, far, basis = [t.double() for t in pos]
+  means, covs = o_render.cast_rays(tdist.double(), o, d, rad[:, None], kw['ray_shape'], diag=False)
+
+  def enc(m):
+    mm, cc = o_coord.track_linearize_contract(m, covs) if kw['warp_contract'] else (m, covs)
+    lm, lv = o_coord.lift_and_diagonalize(mm, cc, basis.T.contiguous())
+    return o_coord.integrated_pos_enc(lm, torch.zeros_like(lv) if kw['disable_integration'] else lv,
+                                      kw['min_deg'], kw['max_deg'])
+  return torch.stack([jvp(enc, (means,), (torch.eye(3, dtype=torch.float64)[a].expand_as(means),))[1]
+                      for a in range(3)])
+
+
+@pytest.mark.parametrize('name', TANGENT_CASES)
+def test_tangent_value_is_the_oracle_derivative(name, monkeypatch):
+  """The reference's fp64 tangent rows are autograd's derivative of the oracle chain (safe_sin reducing by the fp32
+  constant, as the reference does), to fp64 rounding, away from |x| = 1."""
+  from oracle import o_math
+  monkeypatch.setattr(o_math, '_T_SAFE', ER.T32)
+  pos, kw = make_inputs(name, SMS, rays=8)
+  tdist, _, _ = _pre_warp(pos, kw)
+  ref = ER.reference(*pos, **kw, tdist=torch.tensor(tdist), tangent=True)
+  ag = _autograd_tangent(pos, kw, torch.tensor(tdist))
+  scale = ag.abs().amax(-1, keepdim=True).clamp_min(1e-300)
+  far = ~ref.tangent_vacuous.all(-1, keepdim=True).expand_as(ag)       # samples off the |x| = 1 shell
+  rel = float(((ref.tangent - ag).abs() / scale)[far].max())
+  assert rel < 1e-12, (name, rel)
+
+
+def check(name, dirn=1, mut=None, tangent=False):
   """Reference of a case on the emulation's tdist; (reference, got, [B, S, 2KL] mask of broken bounds)."""
   pos, kw = make_inputs(name, SMS, rays=RAYS)
   tdist, got, count = emulate(pos, kw, dirn=dirn, mut=mut)
-  ref = ER.reference(*pos, **kw, tdist=tdist)
+  ref = ER.reference(*pos, **kw, tdist=tdist, tangent=tangent)
   broken = ((got.double() - ref.feat).abs() > ref.bound) & ~ref.vacuous
   return ref, tdist, got, broken, count
 
@@ -216,7 +393,7 @@ def test_emulation_within_bounds(name):
   K, L = c['K'], c['max_deg'] - c['min_deg']
   deg = ER.degree_of(K, L)
   for dirn in (1, -1):
-    ref, tdist, got, broken, count = check(name, dirn)
+    ref, tdist, got, broken, count = check(name, dirn, tangent=c['tangent'])
     rt = (tdist.double() - ref.tdist).abs() / ref.tdist_bound
     assert float(rt.max()) <= 1, (name, 'tdist', float(rt.max()))
     ratio = torch.where(ref.vacuous, torch.zeros_like(ref.bound), (got.double() - ref.feat).abs() / ref.bound)
@@ -236,7 +413,7 @@ def test_emulation_within_bounds(name):
   for t in (1, 2, 3):
     assert abs(tr.count(t) - count[t]) <= slack, (name, t, tr.count(t), count[t])
   if c['rays'] is not None and not {'nseg>1', 'nseg1', 'short-last'} & set(c['reach']):
-    reach(name, p, tr, c['S'])
+    reach(name, p, tr, c['S'], ref)
   else:
     reach(name, ER.plan(c['rays'] or 32 * SMS + 37, c['S'], K, SMS), tr, c['S'])
 
@@ -248,6 +425,28 @@ MUTATIONS = {
     'reduce_small': ('blender', 'K9'), 'swap_rows': ('S1', 'K9'), 'row_plus1': ('S5-K9', 'K9'),
     'seg_late': ('S33-K21', 'S50-K9'),
 }
+
+
+# tangent-row mutation: the cases tried, in order
+TANGENT_MUTATIONS = {
+    'no_dlv': ('360', 'far-contracted'), 'dlv_no2': ('360', 'far-contracted'), 'q_r_sign': ('far-contracted', '360'),
+    's_r_r_plus_1': ('far-contracted', '360'), 'u_q_for_s': ('far-contracted', '360'),
+    'hsc2_sc': ('360', 'piecewise'), 'esc_no_e': ('360', 'piecewise'), 'basis_dir_k': ('K9', 'K32'),
+    'row_dir_seg': ('S5-K9', 'K9'),
+}
+
+
+@pytest.mark.parametrize('mut', list(TANGENT_MUTATIONS))
+def test_tangent_mutation_is_caught(mut):
+  for name in TANGENT_MUTATIONS[mut]:
+    ref, got, broken = check_tangent(name, mut=mut)
+    if broken.any():
+      r = torch.where(broken, (got.double() - ref.tangent).abs() / ref.tangent_bound_bf16, torch.zeros_like(got.double()))
+      i = tuple(int(v) for v in np.unravel_index(int(r.argmax()), r.shape))
+      print(f'\n{mut}: caught by {name} on {int(broken.sum())} elements, worst at [stream, ray, sample, column] {i}: '
+            f'{float(r[i]):.1f} bounds')
+      return
+  raise AssertionError(f'{mut}: no case notices')
 
 
 @pytest.mark.parametrize('mut', list(MUTATIONS))

@@ -137,46 +137,6 @@ def test_head_bwd_factor(mods, name, K, n_out):
   close(db, draw.sum(0), atol=1e-3, rtol=1e-5, msg='db')
 
 
-def test_tangent_seed_then_factor(mods):
-  """The unmasked tangent seed d_rgd (x) w_density, then a'(z) by the second-order kernel: a'(z_last) * seed."""
-  _, _, ops, lib = mods
-  M, N = 500, 256
-  g = torch.Generator().manual_seed(11)
-  rowv, colv = torch.randn(3 * M, generator=g).cuda(), torch.randn(N, generator=g).cuda()
-  z = _bf(torch.randn(M, N, generator=g) * 2).cuda()
-  u = _bf(torch.randn(3 * M, N, generator=g)).cuda()
-  seed = torch.empty(3 * M, N, device='cuda', dtype=torch.bfloat16)
-  ops.outer_mask(rowv, colv, None, seed, rows=3 * M, n=N, mask_mod=M)
-  gbuf = torch.empty(M, N, device='cuda', dtype=torch.bfloat16)
-  ops.act_tangent_bwd(lib.ACT_SILU, z, seed, u, seed, gbuf)
-  close(seed.float(), _d1('silu', z.float()).repeat(3, 1) * (rowv[:, None] * colv[None, :]), atol=2e-2, rtol=1e-2,
-        msg="a'(z) * seed")
-
-
-@pytest.mark.parametrize('name', ACTS)
-@pytest.mark.parametrize('accumulate', [False, True])
-def test_second_order_kernel_vs_double_backward(mods, name, accumulate):
-  """du = dL/du and g = the a''(z) part of dL/dz for L = sum_s <T_s, a'(z) u_s>, by fp64 torch.autograd taken twice."""
-  _, _, ops, lib = mods
-  M, N = 700, 128
-  g = torch.Generator().manual_seed(5)
-  z = _bf(torch.randn(M, N, generator=g) * 3).cuda()
-  T = _bf(torch.randn(3 * M, N, generator=g)).cuda()
-  u = _bf(torch.randn(3 * M, N, generator=g)).cuda()
-  g0 = _bf(torch.randn(M, N, generator=g)).cuda()
-  zd = z.double().cpu().requires_grad_(True)
-  ud = u.double().cpu().requires_grad_(True)
-  (d1,) = torch.autograd.grad(_act(name)(zd).sum(), zd, create_graph=True)
-  t = d1.repeat(3, 1) * ud
-  dz, du_ref = torch.autograd.grad((T.double().cpu() * t).sum(), (zd, ud))
-  gbuf = g0.clone() if accumulate else torch.empty_like(g0)
-  du = T.clone()
-  ops.act_tangent_bwd(_code(lib, name), z, du, u, du, gbuf, accumulate=accumulate)     # in place, as the model runs it
-  torch.cuda.synchronize()
-  close(du.double().cpu(), du_ref, atol=1e-2, rtol=1e-2, msg='du')
-  close(gbuf.double().cpu(), dz + (g0.double().cpu() if accumulate else 0), atol=3e-2, rtol=1e-2, msg='g')
-
-
 # ------------------------------------------------------------------ model
 
 def with_act(bundle, nerf, prop=None):

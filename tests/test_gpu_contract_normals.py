@@ -1,6 +1,7 @@
 """Density normals through the scene contraction (`warp_fn = contract` with `disable_density_normals = False`):
-the tangent rows of csrc/encode.cu with warp_contract, and the normals, normal losses and Ref-NeRF stage of
-360-style models built on them, against the CPU oracle.  Needs an H100.
+the normals, normal losses and Ref-NeRF stage of 360-style models built on the tangent rows of csrc/encode.cu with
+warp_contract, against the CPU oracle.  Needs an H100.  The tangent rows themselves are checked element by element in
+test_gpu_encode_fp64.py.
 
 Reference: internal/models.py:441-492 (vmap(value_and_grad(predict_density)) with respect to the world-space
 mean, through coord.track_linearize(contract, ...), coord.py:39-60).
@@ -23,84 +24,6 @@ def mods():
   from multinerf_b200 import lib, models, train_utils
   lib.require_device()
   return models, train_utils
-
-
-# ------------------------------------------------------------------ kernel
-
-def _tangent_reference(means, covs, basis_t, maxdeg, mean_term_only=False):
-  """d(IPE feature)/d(world mean) by torch autograd in fp64, [3, B, S, F]."""
-  m = means.detach().clone().requires_grad_(True)
-  if mean_term_only:
-    jac = o_coord.contract_jacobian(m).detach()
-    z, c = o_coord.contract(m), jac @ covs @ jac.transpose(-1, -2)
-  else:
-    z, c = o_coord.track_linearize_contract(m, covs)
-  lm, lv = o_coord.lift_and_diagonalize(z, c, basis_t)
-  enc = o_coord.integrated_pos_enc(lm, lv, 0, maxdeg)
-  jac = torch.stack([torch.autograd.grad(enc[..., f].sum(), m, retain_graph=True)[0]
-                     for f in range(enc.shape[-1])], -1)
-  return jac.permute(2, 0, 1, 3), enc.detach()
-
-
-@pytest.mark.parametrize('rshape,no_integration,far', [('cone', False, False), ('cylinder', False, False),
-                                                       ('cone', True, False), ('cone', False, True)])
-def test_encode_tangent_through_contraction(mods, rshape, no_integration, far):
-  from multinerf_b200 import geopoly, ops
-  rng = np.random.default_rng(71)
-  B, S = 48, 16
-  # maxdeg 8 and cones 0.01-0.03 wide: the degrees where exp(-sc^2 var / 2) turns over, and with them the
-  # covariance term, carry weight against the bound's 2e-4 * max|d feature| floor
-  maxdeg = 8
-  o = torch.tensor(rng.uniform(-1, 1, (B, 3)).astype(np.float32))
-  d = rng.normal(size=(B, 3))
-  d = torch.tensor((d / np.linalg.norm(d, axis=-1, keepdims=True) * rng.uniform(0.8, 1.2, (B, 1))).astype(np.float32))
-  radii = torch.tensor(rng.uniform(0.01, 0.03, (B, 1)).astype(np.float32))
-  if far:
-    # an unbounded capture's ray: reciprocal distances out to 1e6, 1 - s log-uniform so that the samples reach
-    # |x| ~ 1e5, where the contraction's Jacobian is ~1e-10 and the variance term's parts span many decades
-    raydist, near, farv_ = 'reciprocal', 0.2, 1e6
-    sdist = torch.tensor(np.sort(1 - 10 ** rng.uniform(-6.5, 0, (B, S + 1)), -1).astype(np.float32))
-  else:
-    raydist, near, farv_ = None, 0.05, 4.0
-    sdist = torch.tensor(np.sort(rng.uniform(0, 1, (B, S + 1)).astype(np.float32), -1))
-  nearv, farv = torch.full((B, 1), near), torch.full((B, 1), farv_)
-  basis = torch.tensor(geopoly.generate_basis('octahedron', 1), dtype=torch.float32)
-  _, s_to_t = o_coord.construct_ray_warps(raydist, nearv, farv)
-  means, covs = o_render.cast_rays(s_to_t(sdist).double(), o.double(), d.double(), radii.double(), rshape,
-                                   diag=False)
-  mag = means.norm(dim=-1)
-  assert float((mag < 1).float().mean()) > 0.02 and float((mag > 1).float().mean()) > 0.5
-  if far:
-    assert float((mag > 1e4).float().mean()) > 0.1
-  if no_integration:
-    covs = torch.zeros_like(covs)
-  ref, enc = _tangent_reference(means, covs, basis.double().T.contiguous(), maxdeg)
-  F = ref.shape[-1]
-  M = B * S
-  feat = torch.empty(M, 128, dtype=torch.bfloat16, device='cuda')
-  tfeat = torch.empty(3 * M, 128, dtype=torch.bfloat16, device='cuda')
-  ops.encode(sdist.cuda(), o.cuda(), d.cuda(), radii[:, 0].contiguous().cuda(), nearv[:, 0].contiguous().cuda(),
-             farv[:, 0].contiguous().cuda(), basis.cuda(), min_deg=0, max_deg=maxdeg, raydist_fn=raydist,
-             ray_shape=rshape, warp_contract=True, disable_integration=no_integration, feat=feat, feat_cols=128, tfeat=tfeat)
-  got = tfeat.float().cpu().view(3, B, S, 128)[..., :F].double()
-
-  def bad_fraction(r):     # the bound of test_encode_tangent_features
-    scale = float(r.abs().max())
-    return float(((got - r).abs() > 1e-2 * r.abs() + 2e-4 * scale).float().mean())
-
-  def bad_fraction_far(r):  # the same bound with each sample's own scale, on the samples beyond |x| = 100
-    scale = r.abs().amax(dim=(0, 3), keepdim=True)
-    return float(((got - r).abs() > 1e-2 * r.abs() + 2e-4 * scale)[:, mag > 100].float().mean())
-  assert bad_fraction(ref) < 2e-3, bad_fraction(ref)
-  if far:
-    assert bad_fraction_far(ref) < 2e-3, bad_fraction_far(ref)
-  close(feat.float().cpu().view(B, S, 128)[..., :F], enc.float().to(torch.bfloat16).float(), atol=8e-3, rtol=0,
-        msg='features')
-  if not no_integration:
-    ref_mean, _ = _tangent_reference(means, covs, basis.double().T.contiguous(), maxdeg, mean_term_only=True)
-    assert bad_fraction(ref_mean) > 2e-2, bad_fraction(ref_mean)
-    if far:
-      assert bad_fraction_far(ref_mean) > 2e-2, bad_fraction_far(ref_mean)
 
 
 # ------------------------------------------------------------------ model

@@ -8,9 +8,14 @@ the fast kernel's rows within twice the bound; zero pad columns; `feat`, `tfeat`
 between sentinel pads, which must survive; the same bits of `feat` with and without the optional outputs.  Elements
 whose bound says nothing (encode_ref.VACUOUS) are counted, printed per degree, and held to the case's floor on the
 checked share.  Each case asserts through encode_ref.plan / tiers that it reaches the launch plan and the sine tiers it
-was written for, and prints the plan, the passes per tier and the worst err / bound per degree.  The tangent rows
-themselves (d feature / d mean) stay with test_gpu_kernels.test_encode_tangent_features and
-test_gpu_contract_normals.test_encode_tangent_through_contraction.
+was written for, and prints the plan, the passes per tier and the worst err / bound per degree.
+
+The tangent kernel's tangent rows (d feature / d mean, three streams at rows dir * M + m of tfeat) are checked the same
+way against encode_ref.tangent_reference on every `tangent` case, per stream and degree, with their own floor
+(`tfloor`, default `floor`): elements are vacuous where the feature is, and on samples within rounding of |x| = 1,
+where the contraction's d lift_var jumps.  'unit-shell' puts samples within 2e-6 of that sphere; 'cos-straddle' puts
+y below fl32(100 pi) and y + pi/2 above it, so the two halves reduce differently; it shows the bounds sound there
+but cannot tell the two reductions apart, whose difference lies far below a bf16 half-ulp.
 """
 import ctypes as C
 
@@ -59,6 +64,17 @@ CASES = {
                        reach=('mixed', 'zero', 'padded', 'tier1', 'tier2', 'tier3'), floor=0.95),
     'far-contracted': dict(contract=True, raydist='reciprocal', near=0.2, far=1e6, S=16, rays=48, radii=(0.01, 0.03),
                            sdist='far'),
+    # the contraction with cylinders, and without integration (d lift_var = 0), for the tangent rows
+    'cylinder-contracted': dict(contract=True, shape='cylinder', near=0.05, far=4.0, radii=(0.01, 0.03), S=16, rays=48),
+    'no-integration-contracted': dict(contract=True, no_int=True, near=0.05, far=4.0, radii=(0.01, 0.03), S=16,
+                                      rays=48),
+    # tangent rows: samples within 1e-6 of |x| = 1, where d lift_var jumps (a share of them within rounding of it)
+    'unit-shell': dict(contract=True, near=0.0, far=2.0, origins='zero', sdist='shell', S=16, rays=48, tfloor=0.75,
+                       reach=('shell',)),
+    # degrees whose y + pi/2 crosses fl32(100 pi) while y stays below it: the two halves reduce differently.  This
+    # shows the bounds sound there; it cannot tell the reductions apart (reducing y for the cosine half instead moves
+    # the argument by 5.9e-6, some 1e-3 of a tangent element at degree 8, far below its bf16 half-ulp)
+    'cos-straddle': dict(K=3, max_deg=12, origins='straddle', reach=('straddle',)),
 }
 
 
@@ -95,8 +111,17 @@ def make_inputs(name, num_sms, rays=None):
     o = o * 1e-3
     o[::8] = 1e4 * basis[0].numpy()
     o[1], d[1] = 0, 0
+  elif c['origins'] == 'zero':
+    o = o * 0
+  elif c['origins'] == 'straddle':
+    # lm_0 2^8 = fl32(100 pi) - 0.8 +- 0.6 along basis[0]; directions 1e-4 long keep the samples there
+    o = basis[0].numpy() * (ER.T32 - 0.8) / 256 * rng.uniform(1 - 2e-3, 1 + 2e-3, (B, 1))
+    d = d * 1e-4
   radii = rng.uniform(*c['radii'], B)
-  if c['sdist'] == 'far':
+  if c['sdist'] == 'shell':
+    # t = 2 s: the frustum means lie at |x| = 1 +- 2e-6 (o = 0)
+    sdist = np.sort(0.5 / np.linalg.norm(d, axis=-1, keepdims=True) * (1 + rng.uniform(-2e-6, 2e-6, (B, S + 1))), -1)
+  elif c['sdist'] == 'far':
     sdist = np.sort(1 - 10 ** rng.uniform(-6.5, 0, (B, S + 1)), -1)
   else:
     sdist = np.sort(rng.uniform(0, 1, (B, S + 1)), -1)
@@ -108,10 +133,29 @@ def make_inputs(name, num_sms, rays=None):
   return pos, kw
 
 
-def reach(name, p, tr, S):
+def straddles(ref, min_deg, max_deg):
+  """[.., L, K] lifted means whose y = lm 2^l lies below fl32(100 pi) while y + pi/2 does not."""
+  y = ref.lm[..., None, :].abs() * 2.0 ** torch.arange(min_deg, max_deg, dtype=torch.float64)[:, None]
+  return (y < ER.T32) & (y + 0.5 * np.pi >= ER.T32)
+
+
+def shell(ref):
+  """[3] bool: samples within rounding of |x| = 1 (vacuous tangent rows), and samples with a checked bound within
+  1e-6 of it inside and outside."""
+  if not hasattr(ref, 'unsure'):
+    return torch.zeros(3, dtype=torch.bool)
+  d = ref.xnorm - 1
+  return torch.stack([ref.unsure.any(), (~ref.unsure & (d < 0) & (d >= -1e-6)).any(),
+                      (~ref.unsure & (d > 0) & (d <= 1e-6)).any()])
+
+
+def reach(name, p, tr, S, ref=None):
   """The case got the launch plan and the sine tiers it was written for."""
-  for what in case(name)['reach']:
-    ok = {'nseg1': p.nseg == 1, 'nseg>1': p.nseg > 1, 'short-last': p.nseg > 1 and p.nseg * p.seg_len != S, 'S%G': S % p.G != 0,
+  c = case(name)
+  for what in c['reach']:
+    ok = {'straddle': ref is not None and bool(straddles(ref, c['min_deg'], c['max_deg']).any()),
+          'shell': ref is not None and bool(shell(ref).all()),
+          'nseg1': p.nseg == 1, 'nseg>1': p.nseg > 1, 'short-last': p.nseg > 1 and p.nseg * p.seg_len != S, 'S%G': S % p.G != 0,
           'padded': bool(tr.padded.any()), 'mixed': bool((tr.mixed & ~tr.unsure).any()),
           'zero': bool(tr.zero.any()), 'tier1': tr.count(1) > 0, 'tier2': tr.count(2) > 0,
           'tier3': int(((tr.rest == 3) & ~tr.unsure).sum()) > 0}.get(what)
@@ -170,12 +214,12 @@ def test_encode_case(ops, name):
 
   feat, f32, tdist = ops.encode(*dev, **kw, want_f32=True, want_tdist=True)
   assert feat.shape == (M, cols)
-  ref = ER.reference(*pos, **kw, tdist=tdist)
+  ref = ER.reference(*pos, **kw, tdist=tdist, tangent=c['tangent'])
   p = ER.plan(B, S, K, sms)
   tr = ER.tiers(ref, p, c['min_deg'], c['max_deg'])
   print(f'\n{name}: rays {B} S {S} K {K} L {Ld} | plan G {p.G} nseg {p.nseg} seg_len {p.seg_len} | passes per tier '
         f'1: {tr.count(1)} 2: {tr.count(2)} 3: {tr.count(3)} (unsure {int(tr.unsure.sum())})')
-  reach(name, p, tr, S)
+  reach(name, p, tr, S, ref)
 
   rt = (tdist.cpu().double() - ref.tdist).abs() / ref.tdist_bound
   assert float(rt.max()) <= 1, (name, 'tdist', float(rt.max()), int(rt.argmax()))
@@ -224,6 +268,15 @@ def test_encode_case(ops, name):
     assert float(cross.max()) <= 1, (name, 'tangent kernel against fast kernel', float(cross.max()))
     print(f'{name} tangent kernel against fast kernel: worst difference / (2 bound) {float(cross.max()):.2f}, '
           f'{float((gott[..., :F] == gotbf[..., :F]).double().mean()):.4f} of the elements bit-equal')
+    # the tangent rows d feature / d mean_dir: stream dir at rows dir * M + m
+    tchecked = 1 - float(ref.tangent_vacuous.double().mean())
+    tfloor = c.get('tfloor', c['floor'])
+    assert tchecked >= tfloor, f'{name}: only {tchecked:.3f} of the tangent elements have a bound that says anything'
+    gtan = tview.float().cpu().view(3, B, S, cols)[..., :F]
+    for a in range(3):
+      print(report(name, f'tangent stream {a}', gtan[a], ref.tangent[a], ref.tangent_bound_bf16[a],
+                   ref.tangent_vacuous[a], K, Ld))
+    print(f'{name} tangent rows: checked share {tchecked:.3f} (floor {tfloor})')
 
 
 def test_encode_refusals(ops):

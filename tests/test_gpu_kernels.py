@@ -374,34 +374,3 @@ def test_outer_mask_and_gemm_mask_mod_addend(ops):
              addend=add.cuda(), impl=impl)
     ref2 = (a.float() @ w.float().T) * maskb.repeat(3, 1) + add.float()
     close(o2.float(), ref2.to(torch.bfloat16).float(), atol=3e-2, rtol=1.6e-2, msg=f'mask_mod+addend impl={impl}')
-
-
-def test_encode_tangent_features(ops):
-  """d(IPE feature)/d(mean) against torch autograd of the oracle (no contraction)."""
-  from multinerf_b200 import geopoly
-  rng = np.random.default_rng(61)
-  B, S, maxdeg = 40, 16, 16
-  o, d, radii = kernel_rays(rng, B)
-  o = o * 3
-  sdist = torch.tensor(np.sort(rng.uniform(0, 1, (B, S + 1)).astype(np.float32), -1))
-  nearv, farv = torch.full((B, 1), 2.0), torch.full((B, 1), 6.0)
-  basis = torch.tensor(geopoly.generate_basis('octahedron', 1), dtype=torch.float32)
-  _, s_to_t = o_coord.construct_ray_warps(None, nearv, farv)
-  means, covs = o_render.cast_rays(s_to_t(sdist), o, d, radii, 'cone', diag=False)
-  means = means.detach().requires_grad_(True)
-  lm, lv = o_coord.lift_and_diagonalize(means, covs, basis.T.contiguous())
-  enc = o_coord.integrated_pos_enc(lm, lv, 0, maxdeg)          # [B,S,F]
-  F = enc.shape[-1]
-  jac = torch.stack([torch.autograd.grad(enc[..., f].sum(), means, retain_graph=True)[0] for f in range(F)], -1)
-  M = B * S
-  feat = torch.empty(M, 128, dtype=torch.bfloat16, device='cuda')
-  tfeat = torch.empty(3 * M, 128, dtype=torch.bfloat16, device='cuda')
-  ops.encode(sdist.cuda(), o.cuda(), d.cuda(), radii[:, 0].contiguous().cuda(), nearv[:, 0].contiguous().cuda(),
-             farv[:, 0].contiguous().cuda(), basis.cuda(), min_deg=0, max_deg=maxdeg, feat=feat, feat_cols=128,
-             tfeat=tfeat)
-  got = tfeat.float().cpu().view(3, B, S, 128)[..., :F]          # [dir, B, S, F]
-  ref = jac.permute(2, 0, 1, 3)                                  # [3, B, S, F]
-  scale = float(ref.abs().max())
-  assert float(((got - ref).abs() > 1e-2 * ref.abs() + 2e-4 * scale).float().mean()) < 2e-3
-  close(feat.float().cpu().view(B, S, 128)[..., :F], enc.detach().to(torch.bfloat16).float(), atol=8e-3, rtol=0,
-        msg='features unchanged')
