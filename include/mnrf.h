@@ -202,7 +202,8 @@ int mnrf_gemm_wgrad(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16
 typedef struct {
   int32_t block_n;    /* output tile width BN: 256, 128, 64, 32 or 16 */
   int32_t staged;     /* 1: the bf16 output goes through shared memory and TMA bulk stores; 0: register stores */
-  int32_t mask_tma;   /* DGRAD mask bits: 1 loaded by TMA with the operands; 0 loaded by the epilogue (or none) */
+  int32_t mask_tma;   /* mask bits by TMA: DGRAD 1 loaded with the operands, 0 loaded by the epilogue (or none);
+                         FWD 1 stored from shared memory by the epilogue set 3, 0 stored from registers (or none) */
   int32_t smooth;     /* softplus / SiLU epilogue */
   int32_t side;       /* WGRAD side sums (bsum / side_aw) */
   int32_t splits;     /* reduction splits (WGRAD; 1 otherwise) */
@@ -210,9 +211,10 @@ typedef struct {
   int32_t grid;       /* persistent CTAs */
   int32_t pingpong;   /* FWD / DGRAD: 1 each consumer warpgroup runs whole 128 x 128 sub-tiles of the 128 x block_n
                          tiles, alternating, so one's epilogue runs under the other's MMAs; 0 both run each tile */
-  int32_t epilogue;   /* ping-pong DGRAD epilogue operand set, compiled into its instance: 1 mask bits by TMA only,
-                         2 mask bits by TMA and the rank-1 term rowv (x) colv; 0 any operands, tested at run time
-                         (also every other instance) */
+  int32_t epilogue;   /* ping-pong epilogue operand set, compiled into its instance.  DGRAD: 1 mask bits by TMA
+                         only, 2 mask bits by TMA and the rank-1 term rowv (x) colv.  FWD: 3 bias + ReLU + mask bits
+                         stored by TMA, 4 bias + ReLU without mask bits, 5 bias alone.  0 any operands, tested at run
+                         time (also every other instance) */
 } mnrf_gemm_instance;
 int mnrf_gemm_plan(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16* b, const float* bias,
                    const float* rowv, const float* colv, const mnrf_bf16* mask, const uint32_t* maskbits,

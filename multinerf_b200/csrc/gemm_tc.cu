@@ -200,16 +200,26 @@ struct GemmClk {
 };
 #endif
 
-// DGRAD epilogue operand sets (mnrf_gemm_instance.epilogue).  The ping-pong kernel has an instance per set, so the
-// model's DGRADs run an epilogue that tests no optional operand; the generic set tests each at run time.
-enum { EPI_GENERIC = 0, EPI_BITS_TMA = 1, EPI_BITS_TMA_RANK1 = 2 };
+// Epilogue operand sets of the ping-pong kernel (mnrf_gemm_instance.epilogue), one instance each, so the model's
+// FWDs and DGRADs run an epilogue that tests no optional operand; the generic set tests each at run time.
+//   DGRAD: mask bits by TMA (the trunk), and with the rank-1 term (the bottleneck);
+//   FWD:   bias + ReLU + mask bits stored by TMA (trunk and view layers in training), bias + ReLU (the same layers
+//          in a render), bias alone (the bottleneck).
+enum {
+  EPI_GENERIC = 0, EPI_BITS_TMA = 1, EPI_BITS_TMA_RANK1 = 2,
+  EPI_FWD_BIAS_RELU_BITS = 3, EPI_FWD_BIAS_RELU = 4, EPI_FWD_BIAS = 5
+};
+constexpr bool epi_fwd(int ops) { return ops >= EPI_FWD_BIAS_RELU_BITS; }
 
 // The FWD / DGRAD epilogue of one consumer warpgroup, from the accumulator fragment of wgmma m64nNC (per thread:
 // acc[4i + 2h + e] is row 16*warp + lane/4 + 8h, column 8i + 2*(lane%4) + e of the warpgroup's 64 x NC block):
 // FWD bias, then ReLU and mask bits or a smooth a(z) | DGRAD rank-1 term, mask bits (from the TMA-loaded mask block
 // at m_tile if mask_tma, else from global memory), bf16 mask or a'(z), addend and, if do_cs, column sums into the
-// warp's shared-memory slice at cs_lane.  DGRAD operand set OPS other than EPI_GENERIC fixes which of these are
-// present at compile time.  The block is rows [r0, r0 + 64) of the 128-row tile m_blk and columns
+// warp's shared-memory slice at cs_lane.  An operand set OPS other than EPI_GENERIC fixes which of these are
+// present at compile time; the FWD sets read the bias of columns [ncol0, ncol0 + NC) from shared memory at bias_s,
+// and EPI_FWD_BIAS_RELU_BITS builds the mask words of the tile's 128 rows in the [128 rows x MW words] block at
+// m_tile, which the call for rows [64, 128) writes out with one bulk store by tmap_m along with its last output
+// block.  The block is rows [r0, r0 + 64) of the 128-row tile m_blk and columns
 // [ncol0, ncol0 + NC); warpgroup wg (0 or 1) owns named barrier 2 + wg and staging blocks [wg * SB, wg * SB + SB).
 // TS: the bf16 output goes through a ring of SB (1 to 3) staging blocks of [64 rows x 64 cols], one TMA bulk store
 // per 64 columns; else it is stored from registers.  SB = 3 carries the ring position `sblk` across calls (a
@@ -217,16 +227,20 @@ enum { EPI_GENERIC = 0, EPI_BITS_TMA = 1, EPI_BITS_TMA_RANK1 = 2 };
 template <int MODE, int NC, bool TS, int SB, bool SMOOTH, int OPS = EPI_GENERIC>
 __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const CUtensorMap* tmap_c, const float (&acc)[NC / 2],
                                               int m_blk, int r0, int ncol0, int wg, uint8_t* smem_c, bool mask_tma,
-                                              uint32_t m_tile, bool do_cs, uint32_t cs_lane, int& sblk, GemmClk& clk) {
+                                              uint32_t m_tile, bool do_cs, uint32_t cs_lane, int& sblk, GemmClk& clk,
+                                              const CUtensorMap* tmap_m = nullptr, uint32_t bias_s = 0) {
   constexpr int MW = mask_words(NC);
-  static_assert(OPS == EPI_GENERIC || (MODE == MNRF_GEMM_DGRAD && TS && !SMOOTH && MW > 0),
-                "fixed operand sets are DGRAD epilogues of the staged store with TMA-loaded mask bits");
+  static_assert(OPS == EPI_GENERIC || ((MODE == MNRF_GEMM_FWD) == epi_fwd(OPS) && TS && !SMOOTH && MW > 0),
+                "fixed operand sets are FWD / DGRAD epilogues of the staged store with mask words by TMA");
   constexpr bool kFixed = OPS != EPI_GENERIC;
+  constexpr bool kFwdFixed = kFixed && epi_fwd(OPS);
   const bool has_rowv = kFixed ? OPS == EPI_BITS_TMA_RANK1 : p.rowv != nullptr;
-  const bool has_bits = kFixed || p.maskbits != nullptr;
+  const bool has_bits = kFixed ? OPS == EPI_FWD_BIAS_RELU_BITS || !kFwdFixed : p.maskbits != nullptr;
   const bool bits_tma = kFixed || mask_tma;
   const bool has_mask = !kFixed && p.mask != nullptr;
   const bool has_addend = !kFixed && p.addend != nullptr;
+  const bool has_bias = kFixed || p.bias != nullptr;
+  const bool relu = kFixed ? OPS != EPI_FWD_BIAS : p.act == MNRF_ACT_RELU;
   const int lane = threadIdx.x & 31;
   const int r_in = r0 + (16 * ((threadIdx.x >> 5) & 3) + (lane >> 2));   // this thread's row (h = 0) in the tile
   const int cq = 2 * (lane & 3);
@@ -271,8 +285,9 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const CUtenso
 #pragma unroll
     for (int h = 0; h < 2; ++h) { v[h][0] = acc[4 * i + 2 * h]; v[h][1] = acc[4 * i + 2 * h + 1]; }
     if (MODE == MNRF_GEMM_FWD) {
-      if (p.bias) {
-        const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+      if (has_bias) {
+        const float2 b = kFwdFixed ? ld_shared_f2(bias_s + (8 * i + cq) * 4)
+                                   : __ldg(reinterpret_cast<const float2*>(p.bias + col));
 #pragma unroll
         for (int h = 0; h < 2; ++h) { v[h][0] += b.x; v[h][1] += b.y; }
       }
@@ -285,13 +300,14 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const CUtenso
           v[h][0] = act_fwd(p.act, v[h][0]);
           v[h][1] = act_fwd(p.act, v[h][1]);
         }
-      } else if (p.act == MNRF_ACT_RELU) {
+      } else if (relu) {
+        // bit 8 * (i % 4) + e of this thread's share of the word: shifted by cq once the word is complete
 #pragma unroll
         for (int h = 0; h < 2; ++h)
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             v[h][e] = relu_nan(v[h][e]);
-            bits[h] |= (v[h][e] > 0.f ? 1u : 0u) << ((8 * i + cq + e) & 31);
+            bits[h] |= (v[h][e] > 0.f ? 1u : 0u) << (8 * (i & 3) + e);
           }
       }
     } else {
@@ -348,13 +364,18 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const CUtenso
             pack_bf16(v[h][0], v[h][1]);
       }
     }
-    if (MODE == MNRF_GEMM_FWD && p.act == MNRF_ACT_RELU && p.maskbits && (i & 3) == 3) {
-      // one 32-column mask word per row: the four lanes of a quad hold its 32 bits between them
+    if (MODE == MNRF_GEMM_FWD && relu && has_bits && (i & 3) == 3) {
+      // one 32-column mask word per row: the four lanes of a quad hold its 32 bits between them.  The fixed set
+      // builds the tile's words in shared memory (rows past M included: the bulk store clips them).
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
+        bits[h] <<= cq;
         bits[h] |= __shfl_xor_sync(0xffffffffu, bits[h], 1);
         bits[h] |= __shfl_xor_sync(0xffffffffu, bits[h], 2);
-        if ((lane & 3) == ((i >> 2) & 3) && row_ok[h]) p.maskbits[rows[h] * p.ldmaskbits + (col >> 5)] = bits[h];
+        if ((lane & 3) == ((i >> 2) & 3)) {
+          if (kFwdFixed) st_shared_u32(m_row + (8 * h * MW + (i >> 2)) * 4, bits[h]);
+          else if (row_ok[h]) p.maskbits[rows[h] * p.ldmaskbits + (col >> 5)] = bits[h];
+        }
         bits[h] = 0u;
       }
     }
@@ -367,6 +388,9 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const CUtenso
       if (leader) {                             // TMA clips the rows past M
         tma_store_2d(tmap_c, smem_c + (wg * SB + sb) * STAGING_BLOCK_BYTES, ncol0 + 8 * (i & ~7),
                      (int)((int64_t)m_blk * BLOCK_M + r0));
+        // the tile's mask words are complete once the second half's last block is staged
+        if (OPS == EPI_FWD_BIAS_RELU_BITS && i == NC / 8 - 1 && r0 == BLOCK_M - 64)
+          tma_store_2d(tmap_m, m_tile, ncol0 / 32, m_blk * BLOCK_M);
         tma_store_commit();
       }
       if (SB == 3) sblk = sblk == 2 ? 0 : sblk + 1;
@@ -592,18 +616,23 @@ constexpr int PP_STAGES = 5;           // operand ring: 5 x 32 KB
 // store of block j the leader waits only for block j - 2's to have been read, not for block j - 1's, issued just
 // before.  FWD keeps two: with three, its 1024-wide layers measured slower (DESIGN.md section 3).
 constexpr int pp_staging_blocks(int mode) { return mode == MNRF_GEMM_DGRAD ? 3 : 2; }
-// DGRAD mask blocks by TMA, sub-tile it in buffer it % PP_MASK_BUFS: four, so that the producer loads sub-tile
-// it + 2's mask and operands while sub-tile it's epilogue still reads its mask block
+// Mask blocks of [128 rows x 4 words], sub-tile it in buffer it % PP_MASK_BUFS (warpgroup it & 1 owns buffers
+// it & 1 and (it & 1) + 2).  DGRAD, loaded by TMA: four, so that the producer loads sub-tile it + 2's mask and
+// operands while sub-tile it's epilogue still reads its mask block.  FWD with mask bits, built by the epilogue and
+// stored by TMA: two per warpgroup, so that sub-tile it + 2 builds its words while sub-tile it's bulk store may
+// still read them; the leader's wait for block 0 of sub-tile it + 2's output covers that store before it + 4.
+// The FWD sets then keep each warpgroup's sub-tile bias, [PP_BN] fp32.
 constexpr int PP_MASK_BUFS = 4;
-constexpr int pp_smem_bytes(int mode) {
+constexpr int pp_smem_bytes(int mode, int ops) {
   return PP_STAGES * (A_STAGE_BYTES + PP_BN * BLOCK_K * 2) + 2 * pp_staging_blocks(mode) * STAGING_BLOCK_BYTES +
-         (mode == MNRF_GEMM_DGRAD ? PP_MASK_BUFS * BLOCK_M * mask_words(PP_BN) * 4 : 0) + 256 /*barriers*/ +
-         1024 /*align*/;
+         (mode == MNRF_GEMM_DGRAD || ops == EPI_FWD_BIAS_RELU_BITS ? PP_MASK_BUFS * BLOCK_M * mask_words(PP_BN) * 4
+                                                                   : 0) +
+         (epi_fwd(ops) ? 2 * PP_BN * 4 : 0) + 256 /*barriers*/ + 1024 /*align*/;
 }
 
 // Accumulator fragments of the two wgmma m64n128 of a sub-tile (per consumer thread): acc[g][4i + 2h + e] is row
-// 64g + 16*warp + lane/4 + 8h, column 8i + 2*(lane%4) + e of the warpgroup's 128 x 128 sub-tile.  OPS: the DGRAD
-// epilogue operand set (EPI_GENERIC for FWD).
+// 64g + 16*warp + lane/4 + 8h, column 8i + 2*(lane%4) + e of the warpgroup's 128 x 128 sub-tile.  OPS: the
+// epilogue operand set.
 template <int MODE, int BN, int OPS>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
@@ -615,6 +644,8 @@ gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
   constexpr int MW = mask_words(PP_BN);
   constexpr int SB = pp_staging_blocks(MODE);
   constexpr bool kDgrad = (MODE == MNRF_GEMM_DGRAD);
+  constexpr bool kFwdFixed = epi_fwd(OPS);                         // bias from shared memory
+  constexpr bool kFwdBits = OPS == EPI_FWD_BIAS_RELU_BITS;         // mask words stored by TMA
   static_assert(MODE != MNRF_GEMM_WGRAD && (BN == 128 || BN == 256), "FWD / DGRAD tiles of 128 or 256 columns");
   extern __shared__ uint8_t smem_dyn[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
@@ -622,7 +653,8 @@ gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
   uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
   uint8_t* smem_c = smem_b + STAGES * B_STAGE;                                   // [2 warpgroups][SB] blocks
   uint32_t* mask_s = reinterpret_cast<uint32_t*>(smem_c + 2 * SB * STAGING_BLOCK_BYTES);  // [PP_MASK_BUFS][BLOCK_M][MW]
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(mask_s + (kDgrad ? PP_MASK_BUFS * BLOCK_M * MW : 0));  // [STAGES]
+  float* bias_s = reinterpret_cast<float*>(mask_s + (kDgrad || kFwdBits ? PP_MASK_BUFS * BLOCK_M * MW : 0));  // [2][PP_BN]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(bias_s + (kFwdFixed ? 2 * PP_BN : 0));  // [STAGES]
   uint64_t* empty_bar = full_bar + STAGES;                                       // [STAGES]
   uint64_t* mask_full = empty_bar + STAGES;                                      // [PP_MASK_BUFS]
   uint64_t* mask_empty = mask_full + PP_MASK_BUFS;                               // [PP_MASK_BUFS]
@@ -638,7 +670,7 @@ gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_b);
     prefetch_tmap(&tmap_c);
-    if (mask_tma) prefetch_tmap(&tmap_m);
+    if (mask_tma || kFwdBits) prefetch_tmap(&tmap_m);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 4);     // the 4 warps of the warpgroup that consumes the stage
@@ -700,6 +732,8 @@ gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
       const int n_blk = tile % p.num_n_blocks;
       const int m_blk = tile / p.num_n_blocks;
       const int ncol0 = n_blk * BN + s * PP_BN;
+      // FWD sets: one bias value of the sub-tile per thread, loaded under the main loop
+      const float bias_v = kFwdFixed ? __ldg(p.bias + ncol0 + (threadIdx.x & 127)) : 0.f;
       // the ring slots of this sub-tile: the producer fills nk per sub-tile, in order
       const uint32_t slot = (uint32_t)it * (uint32_t)nk;
       uint32_t stage = slot % STAGES, phase = (slot / STAGES) & 1;
@@ -747,11 +781,18 @@ gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
       // loads into the first and the DGRAD instances spill 2.4 KB.
       const uint32_t m_base = smem_u32(mask_s) + (it % PP_MASK_BUFS) * (BLOCK_M * MW * 4);
       if (mask_tma) mbar_wait(&mask_full[it % PP_MASK_BUFS], (it / PP_MASK_BUFS) & 1, 5);
+      // FWD sets: the bias into the warpgroup's slice.  Every read of the previous sub-tile's bias came before the
+      // warpgroup's last named barrier of that epilogue; the barrier here orders the writes before this one's reads.
+      const uint32_t bias_wg = smem_u32(bias_s) + c * (PP_BN * 4);
+      if (kFwdFixed) {
+        st_shared_u32(bias_wg + (threadIdx.x & 127) * 4, __float_as_uint(bias_v));
+        named_bar_sync(2 + c, 128);
+      }
       clk.tick(GK_MASK);
 #pragma unroll 1
       for (int g = 0; g < 2; ++g) {
         gemm_epilogue<MODE, PP_BN, true, SB, false, OPS>(p, &tmap_c, acc[0], m_blk, 64 * g, ncol0, c, smem_c, mask_tma,
-                                                         m_base, false, 0, sblk, clk);
+                                                         m_base, false, 0, sblk, clk, &tmap_m, bias_wg);
 #pragma unroll
         for (int e = 0; e < 64; ++e) acc[0][e] = acc[1][e];   // rows [64, 128) next
       }
@@ -773,7 +814,7 @@ gemm_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
 template <int MODE, int BN, int OPS = EPI_GENERIC>
 static int launch_gemm_tc_pingpong(int grid, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
                                    const CUtensorMap& tm, const GemmParams& p, cudaStream_t stream) {
-  constexpr int kSmem = pp_smem_bytes(MODE);
+  constexpr int kSmem = pp_smem_bytes(MODE, OPS);
   static_assert(kSmem <= 232448, "shared memory budget");
   return launch_tc<gemm_tc_pingpong_kernel<MODE, BN, OPS>>(grid, NUM_THREADS, kSmem, stream, ta, tb, tc, tm, p);
 }
@@ -789,6 +830,21 @@ static int launch_dgrad_pingpong(int ops, int grid, const CUtensorMap& ta, const
       return launch_gemm_tc_pingpong<MNRF_GEMM_DGRAD, BN, EPI_BITS_TMA_RANK1>(grid, ta, tb, tc, tm, p, stream);
   }
   return launch_gemm_tc_pingpong<MNRF_GEMM_DGRAD, BN>(grid, ta, tb, tc, tm, p, stream);
+}
+
+// FWD ping-pong at tile width BN, in the instance of its epilogue operand set
+template <int BN>
+static int launch_fwd_pingpong(int ops, int grid, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
+                               const CUtensorMap& tm, const GemmParams& p, cudaStream_t stream) {
+  switch (ops) {
+    case EPI_FWD_BIAS_RELU_BITS:
+      return launch_gemm_tc_pingpong<MNRF_GEMM_FWD, BN, EPI_FWD_BIAS_RELU_BITS>(grid, ta, tb, tc, tm, p, stream);
+    case EPI_FWD_BIAS_RELU:
+      return launch_gemm_tc_pingpong<MNRF_GEMM_FWD, BN, EPI_FWD_BIAS_RELU>(grid, ta, tb, tc, tm, p, stream);
+    case EPI_FWD_BIAS:
+      return launch_gemm_tc_pingpong<MNRF_GEMM_FWD, BN, EPI_FWD_BIAS>(grid, ta, tb, tc, tm, p, stream);
+  }
+  return launch_gemm_tc_pingpong<MNRF_GEMM_FWD, BN>(grid, ta, tb, tc, tm, p, stream);
 }
 
 template <int MODE, int BN, bool TS, bool SIDE, bool SMOOTH = false>
@@ -883,19 +939,29 @@ static int gemm_tc_plan(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_
   // the smooth epilogues exist for the staged store only: every hidden layer is a multiple of 64 wide
   MNRF_CHECK(!smooth || ts, "mnrf_gemm(tc): a smooth activation needs N %% 64 == 0 and a 16-byte aligned output "
              "with a row pitch that is a multiple of 8");
-  // DGRAD mask bits go through TMA when the tile is at least 128 columns wide and the mask rows of a 128-row tile
-  // are 128 consecutive rows of a TMA-addressable array (16-byte aligned base and row pitch); otherwise the
-  // epilogue loads them itself.
-  const bool mask_tma = d->mode == MNRF_GEMM_DGRAD && maskbits && mask_words(block_n) > 0 && d->ldmaskbits % 4 == 0 &&
-                        ((uintptr_t)maskbits % 16) == 0 && (d->mask_mod == 0 || d->mask_mod % BLOCK_M == 0);
+  // Mask words can move by TMA when the tile is at least 128 columns wide and the words are a TMA-addressable array
+  // (16-byte aligned base and row pitch).  DGRAD loads them so when the mask rows of a 128-row tile are 128
+  // consecutive rows; otherwise the epilogue loads them itself.
+  const bool bits_tma_ok = maskbits && mask_words(block_n) > 0 && d->ldmaskbits % 4 == 0 &&
+                           ((uintptr_t)maskbits % 16) == 0;
+  bool mask_tma = d->mode == MNRF_GEMM_DGRAD && bits_tma_ok && (d->mask_mod == 0 || d->mask_mod % BLOCK_M == 0);
   // FWD and DGRAD run the ping-pong schedule (gemm_tc_pingpong_kernel) wherever it has an epilogue: staged store,
   // whole 128-column sub-tiles, ReLU or no activation, no column sums.
   const bool pingpong = d->mode != MNRF_GEMM_WGRAD && ts && d->n % PP_BN == 0 && !smooth && !colsum;
-  // The ping-pong DGRAD epilogue's operand set: mask bits by TMA, with or without the rank-1 term (rowv and colv
-  // come together), and nothing else has an instance of its own; any other combination runs the generic one.
+  // The ping-pong epilogue's operand set.  DGRAD: mask bits by TMA, with or without the rank-1 term (rowv and colv
+  // come together).  FWD with a bias: ReLU with mask bits the epilogue stores by TMA, ReLU without mask bits, or no
+  // activation and no mask bits; FWD mask bits are stored by TMA only in that set.  Any other combination runs the
+  // generic one.
   int epilogue = EPI_GENERIC;
   if (pingpong && d->mode == MNRF_GEMM_DGRAD && mask_tma && !mask && !addend)
     epilogue = colv ? EPI_BITS_TMA_RANK1 : EPI_BITS_TMA;
+  if (pingpong && d->mode == MNRF_GEMM_FWD && bias) {
+    if (d->act == MNRF_ACT_RELU)
+      epilogue = !maskbits ? EPI_FWD_BIAS_RELU : bits_tma_ok ? EPI_FWD_BIAS_RELU_BITS : EPI_GENERIC;
+    else if (d->act == MNRF_ACT_NONE && !maskbits)
+      epilogue = EPI_FWD_BIAS;
+    mask_tma = epilogue == EPI_FWD_BIAS_RELU_BITS;
+  }
   const int tiles = num_m_blocks * num_n_blocks * num_splits;
   plan->block_n = block_n;
   plan->staged = ts;
@@ -941,10 +1007,10 @@ static int launch_gemm_tc_plan(int mode, const mnrf_gemm_instance& plan, const C
   const bool fwd = mode == MNRF_GEMM_FWD;
   if (plan.pingpong) {
     if (bn == 256)
-      return fwd ? launch_gemm_tc_pingpong<MNRF_GEMM_FWD, 256>(grid, ta, tb, tc, tm, p, stream)
+      return fwd ? launch_fwd_pingpong<256>(plan.epilogue, grid, ta, tb, tc, tm, p, stream)
                  : launch_dgrad_pingpong<256>(plan.epilogue, grid, ta, tb, tc, tm, p, stream);
     if (bn == 128)
-      return fwd ? launch_gemm_tc_pingpong<MNRF_GEMM_FWD, 128>(grid, ta, tb, tc, tm, p, stream)
+      return fwd ? launch_fwd_pingpong<128>(plan.epilogue, grid, ta, tb, tc, tm, p, stream)
                  : launch_dgrad_pingpong<128>(plan.epilogue, grid, ta, tb, tc, tm, p, stream);
   } else if (plan.smooth) {
     return gemm_tc_smooth_launch(mode, bn, grid, ta, tb, tc, p, stream);
@@ -1015,9 +1081,11 @@ int gemm_tc_launch(const mnrf_gemm_desc* d, const mnrf_bf16* a, const mnrf_bf16*
   } else {
     tc = tb;   // not read
   }
+  // DGRAD loads [128 rows x words] blocks of the mask words by it, FWD stores them (FWD ignores mask_mod)
   CUtensorMap tm = tb;   // not read unless p.mask_tma
   if (p.mask_tma &&
-      make_tmap(&tm, maskbits, d->mask_mod > 0 ? d->mask_mod : d->m, d->n / 32, d->ldmaskbits,
+      make_tmap(&tm, maskbits, d->mode == MNRF_GEMM_DGRAD && d->mask_mod > 0 ? d->mask_mod : d->m, d->n / 32,
+                d->ldmaskbits,
                 mask_words(plan.pingpong ? PP_BN : block_n), BLOCK_M, CU_TENSOR_MAP_DATA_TYPE_UINT32, 4,
                 CU_TENSOR_MAP_SWIZZLE_NONE))
     return 1;

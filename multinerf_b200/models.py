@@ -641,10 +641,10 @@ class Model:
 
   @staticmethod
   def _act_out(plan, st, i, view=False):
-    """What the FWD GEMM of hidden layer i (trunk, or view MLP) keeps for the backward: ReLU mask bits, or the
-    pre-activation z of a smooth activation (not kept by a render-only pass)."""
+    """What the FWD GEMM of hidden layer i (trunk, or view MLP) keeps for the backward and the tangent GEMMs: ReLU
+    mask bits, or the pre-activation z of a smooth activation (neither kept by a render-only pass)."""
     if plan.act == L.ACT_RELU:
-      return dict(act=L.ACT_RELU, maskbits=(st.vbits if view else st.bits)[i])
+      return dict(act=L.ACT_RELU, maskbits=(st.vbits if view else st.bits)[i] if st.keep_acts else None)
     return dict(act=plan.act, z=(st.vzs if view else st.zs)[i] if st.keep_acts else None)
 
   @staticmethod

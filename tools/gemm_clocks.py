@@ -1,16 +1,20 @@
 """Where the time of the ping-pong Dense-layer GEMM (gemm_tc_pingpong_kernel) goes, on the NerfMLP shapes of 360.gin.
 
-  python tools/gemm_clocks.py [--rows 524288] [--iters 20] [--lib PATH [--lib PATH ...] [--rounds R]]
+  python tools/gemm_clocks.py [--rows 524288] [--width 1024] [--iters 20] [--hash]
+                              [--lib PATH [--lib PATH ...] [--rounds R]]
 
 Times FWD (bias + ReLU + mask bits) of the 1024-wide trunk at K = 512, 1024 and 1536, its DGRAD with mask bits at
-K = 1024, and the bottleneck DGRAD (N = 1024, K = 256, mask bits + rank-1 term), then prints the card's name, power
-limit and SM clock.  A library built with -DMNRF_GEMM_CLOCKS (csrc/gemm_tc.cu) also gets, per consumer warpgroup,
+K = 1024, the bottleneck FWD (N = 256, K = 1024, bias only) and DGRAD (N = 1024, K = 256, mask bits + rank-1 term),
+then prints the card's name, power limit and SM clock, and for each launch the epilogue operand set it ran
+(mnrf_gemm_instance.epilogue).  `--width` sets the trunk width.  `--hash` also prints the SHA-256 of each FWD's
+output and mask words, to compare two builds on the same data.  A library built with -DMNRF_GEMM_CLOCKS (csrc/gemm_tc.cu) also gets, per consumer warpgroup,
 the clock64() split of the first thread of CTA 0 as shares of that thread's time.  `--build DIR` builds such a
 library into DIR first (from this tree's sources) and runs with it.  With `--lib`, each named build is run in a
 process of its own (the library is chosen at import), the builds alternating R times.
 """
 import argparse
 import ctypes
+import hashlib
 import os
 import subprocess
 import sys
@@ -76,6 +80,8 @@ def clocks(lib):
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--rows', type=int, default=524288)
+  ap.add_argument('--width', type=int, default=1024)
+  ap.add_argument('--hash', action='store_true')
   ap.add_argument('--iters', type=int, default=20)
   ap.add_argument('--lib', action='append', default=[])
   ap.add_argument('--rounds', type=int, default=2)
@@ -85,7 +91,8 @@ def main():
     a.lib = [build_clocks(a.build)]
     a.rounds = 1
   if a.lib:
-    args = [sys.executable, os.path.abspath(__file__), '--rows', str(a.rows), '--iters', str(a.iters)]
+    args = [sys.executable, os.path.abspath(__file__), '--rows', str(a.rows), '--width', str(a.width), '--iters',
+            str(a.iters)] + (['--hash'] if a.hash else [])
     for r in range(a.rounds):
       for path in a.lib:
         print(f'## round {r}: {path}', flush=True)
@@ -95,7 +102,7 @@ def main():
   lib = ctypes.CDLL(L.LIB_PATH)
   dev, bf = 'cuda', torch.bfloat16
   g = torch.Generator(device=dev).manual_seed(0)
-  M, W = a.rows, 1024
+  M, W = a.rows, a.width
   rnd = lambda *s, scale=1.0: (torch.randn(*s, device=dev, generator=g) * scale)
   bits = torch.randint(-2**31, 2**31 - 1, (M, W // 32), device=dev, dtype=torch.int32, generator=g)
   out = torch.empty(M, W, device=dev, dtype=bf)
@@ -106,27 +113,42 @@ def main():
     x = rnd(M, k, scale=0.5).to(bf)
     w = rnd(W, k, scale=0.05).to(bf)
     runs.append((f'fwd K={k} bias+relu+bits', 2.0 * M * W * k,
-                 lambda x=x, w=w, k=k: ops.gemm(L.GEMM_FWD, x, w, out, m=M, n=W, k=k, act=L.ACT_RELU, bias=bias,
-                                                maskbits=obits)))
+                 (L.GEMM_FWD, x, w, out, dict(m=M, n=W, k=k, act=L.ACT_RELU, bias=bias, maskbits=obits))))
   dy = rnd(M, W, scale=0.1).to(bf)
   w_kn = rnd(W, W, scale=0.05).to(bf)
   runs.append(('dgrad K=1024 bits', 2.0 * M * W * W,
-               lambda: ops.gemm(L.GEMM_DGRAD, dy, w_kn, out, m=M, n=W, k=W, maskbits=bits)))
+               (L.GEMM_DGRAD, dy, w_kn, out, dict(m=M, n=W, k=W, maskbits=bits))))
+  # the bottleneck: FWD from the trunk output to 256 columns, bias only, and its DGRAD back
+  xb = rnd(M, W, scale=0.5).to(bf)
+  wbf = rnd(256, W, scale=0.05).to(bf)
+  bout = torch.empty(M, 256, device=dev, dtype=bf)
+  bbias = rnd(256, scale=0.1)
+  runs.append((f'fwd K={W} bias (bottleneck)', 2.0 * M * 256 * W,
+               (L.GEMM_FWD, xb, wbf, bout, dict(m=M, n=256, k=W, bias=bbias))))
   dbott = rnd(M, 256, scale=0.1).to(bf)
   wb = rnd(W, 256, scale=0.05).to(bf)
   rowv, colv = rnd(M), rnd(W)
   runs.append(('dgrad K=256 bits+rank-1 (bottleneck)', 2.0 * M * W * 256,
-               lambda: ops.gemm(L.GEMM_DGRAD, dbott, wb, out, m=M, n=W, k=256, maskbits=bits, rowv=rowv, colv=colv)))
+               (L.GEMM_DGRAD, dbott, wb, out, dict(m=M, n=W, k=256, maskbits=bits, rowv=rowv, colv=colv))))
+  has_plan = hasattr(lib, 'mnrf_gemm_plan')
   res = []
-  for name, fl, fn in runs:
+  for name, fl, (mode, x, w, o, kw) in runs:
+    fn = lambda: ops.gemm(mode, x, w, o, **kw)
     fn()
     torch.cuda.synchronize()
+    digest = ''
+    if a.hash and mode == L.GEMM_FWD:
+      h = hashlib.sha256(o.view(torch.int16).cpu().numpy().tobytes())
+      if 'maskbits' in kw:
+        h.update(kw['maskbits'].cpu().numpy().tobytes())
+      digest = h.hexdigest()[:16]
+    epi = ops.gemm_plan(mode, x, w, o, **kw)['epilogue'] if has_plan else '-'
     clocks(lib)                                    # clear: the split below is of the timed launches
     ms = timeit(fn, a.iters)
-    res.append((name, ms, fl, clocks(lib)))
-  print(f'# M = {M}; {card()}; {L.LIB_PATH}')
-  for name, ms, fl, split in res:
-    print(f'{name:40s} {ms * 1e3:8.1f} us  {fl / ms / 1e9:7.1f} TFLOP/s', flush=True)
+    res.append((name, ms, fl, clocks(lib), epi, digest))
+  print(f'# M = {M}, N = {W}; {card()}; {L.LIB_PATH}')
+  for name, ms, fl, split, epi, digest in res:
+    print(f'{name:40s} {ms * 1e3:8.1f} us  {fl / ms / 1e9:7.1f} TFLOP/s  set {epi}  {digest}', flush=True)
     for wgi, shares in enumerate(split or []):
       print(f'    warpgroup {wgi}: ' + ', '.join(f'{n} {100 * s:.1f} %' for n, s in zip(CLASSES, shares)))
 
