@@ -7,7 +7,8 @@ Writes <checkpoint_dir>/mesh/mesh_step_<step>.ply (multinerf_b200/mesh.py; Confi
 forward-facing scenes must set it; Config.mesh_vertex_colors = True adds vertex normals and colours).
 Config.mesh_method = 'density' (default) meshes the final level's density at Config.mesh_level; 'tsdf' renders every
 training view, fuses the rendered depth into a truncated signed-distance grid (Config.mesh_tsdf_truncation cells) and
-meshes its zero crossing.  One process on one GPU.
+meshes its zero crossing.  Config.mesh_min_views drops what fewer training views see, and
+Config.mesh_keep_components keeps only the largest connected components (mesh.clean_mesh).  One process on one GPU.
 """
 import dataclasses
 import os
@@ -33,21 +34,29 @@ def main(argv=None):
   model, state, _, _, _ = train_utils.setup_model(bundle, 20200823)
   state = checkpoints.restore_checkpoint(config.checkpoint_dir, state, model=model)
   step = int(state.step)
-  if method == 'tsdf':
+  dataset = None
+  if method == 'tsdf' or config.mesh_min_views > 0:
     # every training camera, all pixels, no render path
     dataset = datasets.load_dataset('train', config.data_dir, dataclasses.replace(config, render_path=False),
                                     device=model.device)
+  clean = dict(keep_components=config.mesh_keep_components, min_views=config.mesh_min_views, stats={})
   t0 = time.time()
   if method == 'tsdf':
     vertices, faces, *extra = mesh.extract_mesh_tsdf(model, dataset, bbox, config.mesh_resolution,
-                                                     config.mesh_tsdf_truncation, colors=config.mesh_vertex_colors)
+                                                     config.mesh_tsdf_truncation, colors=config.mesh_vertex_colors,
+                                                     **clean)
     what = f'{dataset.size} views fused, truncation {config.mesh_tsdf_truncation} cells'
   else:
     vertices, faces, *extra = mesh.extract_mesh(model, bbox, config.mesh_resolution, config.mesh_level,
-                                                colors=config.mesh_vertex_colors)
+                                                colors=config.mesh_vertex_colors, dataset=dataset, **clean)
     what = f'level {config.mesh_level}'
   torch.cuda.synchronize()
   elapsed = time.time() - t0
+  if config.mesh_keep_components or config.mesh_min_views:
+    s = clean['stats']
+    print(f"cleaning removed {s['vertices_removed']} vertices, {s['faces_removed']} faces and "
+          f"{s['components_removed']} components (mesh_min_views {config.mesh_min_views}, "
+          f"mesh_keep_components {config.mesh_keep_components})", flush=True)
   out_dir = os.path.join(config.checkpoint_dir, 'mesh')
   os.makedirs(out_dir, exist_ok=True)
   path = os.path.join(out_dir, f'mesh_step_{step}.ply')

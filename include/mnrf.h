@@ -659,6 +659,31 @@ int mnrf_tsdf_integrate(const mnrf_camera_desc* cam, int32_t nx, int32_t ny, int
                         const float* rgb, float tau, float* tsdf, float* weight, float* color_sum,
                         float* color_weight, mnrf_stream stream);
 
+/* Connected components of a triangle mesh (mesh cleaning, mesh.clean_mesh): the graph whose nodes are the
+ * num_vertices vertices and whose edges are the edges of the num_faces faces [num_faces, 3] int32.  Every index must
+ * lie in [0, num_vertices); the kernel does not check (ops.mesh_components does, on the device, before the call).
+ * Writes labels [num_vertices] int32: each vertex's label is the smallest vertex index of its component, so a vertex
+ * no face uses is its own label.  Union-find in three grid-stride passes with no host synchronisation: labels[v] = v;
+ * hook (per face, join v0 with v1 and v0 with v2: find both roots, atomicCAS the larger root's parent from itself to
+ * the smaller, retry on failure, path halving on the way); compress (labels[v] = v's root, walked without halving
+ * stores, so every store of this pass is a root).  Parents only move to smaller indices, so the
+ * labels are bit-deterministic whatever the thread schedule.  Degenerate and duplicate faces are fine.
+ * No reference counterpart. */
+int mnrf_mesh_components(int32_t num_vertices, int64_t num_faces, const int32_t* faces, int32_t* labels,
+                         mnrf_stream stream);
+
+/* For each of n points [n, 3] fp32 (world coordinates), the number of views whose image it lands on:
+ * counts [n] int32.  Views and the camera as mnrf_tsdf_integrate reads them (cam: camtype perspective or fisheye,
+ * has_distortion, k1..k4, p1, p2; num_cameras = 1 or num_views camera-to-pixel matrices; has_ndc must be 0;
+ * worldtocams [num_views, 3, 4], camtopixs [num_cameras, 3, 3]).  A point lands on a view when it has a pixel there
+ * (not behind a perspective camera, not at theta = pi of a fisheye) and that pixel (floor(u), floor(v)) lies in
+ * [0, width) x [0, height): the rule mnrf_tsdf_integrate applies before it reads a pixel, from the same device
+ * function.  Frustum only: occlusion is not considered.  One thread per point; deterministic.
+ * No reference counterpart. */
+int mnrf_points_view_count(const mnrf_camera_desc* cam, int64_t n, const float* points, int32_t num_views,
+                           int32_t height, int32_t width, const float* worldtocams, const float* camtopixs,
+                           int32_t* counts, mnrf_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -130,6 +130,11 @@ class Config:
   # colours are the rendered colours).  mesh_tsdf_truncation: the band, in cells (>= 1).
   mesh_method: str = 'density'
   mesh_tsdf_truncation: float = 3.
+  # cleaning, right after marching cubes (mesh.clean_mesh); 0 turns each off.  mesh_min_views: drop vertices that
+  # land on the images of fewer training views (frustum culling, no occlusion; not NDC) and the faces using them.
+  # mesh_keep_components: then keep only this many connected components, the largest by face count.
+  mesh_min_views: int = 0
+  mesh_keep_components: int = 0
 
 
 @dataclasses.dataclass

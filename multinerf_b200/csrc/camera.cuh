@@ -1,5 +1,6 @@
 // The camera model on the device, both ways: pixel -> camera-space direction (camera_dir, the ray caster of
-// camera.cu) and world point -> continuous pixel and ray parameter (project_point, the TSDF fusion of mesh.cu).
+// camera.cu) and world point -> continuous pixel and ray parameter (project_point, and project_to_pixel for the
+// TSDF fusion and the view counts of mesh.cu).
 // One copy, included by both units; each is compiled with -fmad=false, so the fp32 rounding is the same in both.
 #pragma once
 
@@ -102,6 +103,20 @@ __device__ __forceinline__ bool project_point(const mnrf_camera_desc& d, const f
   const V3 h = mat3_vec(c2p, 3, V3{x, y, 1.0f});
   u = h.x / h.z;
   v = h.y / h.z;
+  return true;
+}
+
+// Whether world point p lands on a width x height image: project_point succeeds and its pixel (px, py) =
+// (floor(u), floor(v)) lies in [0, width) x [0, height).  The one rule both the TSDF fusion and the view counts of
+// mesh.cu use; t is project_point's ray parameter.
+__device__ __forceinline__ bool project_to_pixel(const mnrf_camera_desc& d, const float* __restrict__ w2c,
+                                                 const float* __restrict__ c2p, V3 p, int width, int height,
+                                                 int& px, int& py, float& t) {
+  float u, v;
+  if (!project_point(d, w2c, c2p, p, u, v, t)) return false;
+  if (!(u >= 0.f && u < (float)width && v >= 0.f && v < (float)height)) return false;
+  px = (int)floorf(u);     // u < width and v < height: in range
+  py = (int)floorf(v);
   return true;
 }
 

@@ -17,7 +17,12 @@
 //
 // Also the TSDF fusion of rendered depth maps (tsdf_integrate_kernel): one thread per grid point, its running
 // truncated signed distance, weight and colour sums held in registers across every view of a launch.
+//
+// And the two passes of mesh cleaning: connected components by union-find (uf_*_kernel) and the number of views
+// each vertex lands in (points_view_count_kernel).
 #include <algorithm>
+
+#include <cuda/atomic>
 
 #include "camera.cuh"
 #include "mc_tables.cuh"
@@ -239,7 +244,6 @@ template <bool kColor>
 __global__ void __launch_bounds__(256)
 tsdf_integrate_kernel(const TsdfArgs a) {
   const float tau = a.tau;
-  const float fw = (float)a.width, fh = (float)a.height;
   for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < a.n; p += (int64_t)gridDim.x * blockDim.x) {
     const int64_t row = p / a.nx;
     const int x = (int)(p - row * a.nx);
@@ -253,10 +257,11 @@ tsdf_integrate_kernel(const TsdfArgs a) {
       cw = a.color_weight[p];
     }
     for (int k = 0; k < a.num_views; ++k) {
-      float u, v, t;
-      if (!project_point(a.cam, a.w2c + 12 * (int64_t)k, a.c2p + a.c2p_stride * k, pt, u, v, t)) continue;
-      if (!(u >= 0.f && u < fw && v >= 0.f && v < fh)) continue;
-      const int64_t px = (int)floorf(u), py = (int)floorf(v);     // u < W and v < H: in range
+      int px, py;
+      float t;
+      if (!project_to_pixel(a.cam, a.w2c + 12 * (int64_t)k, a.c2p + a.c2p_stride * k, pt, a.width, a.height, px, py,
+                            t))
+        continue;
       const int64_t i = ((int64_t)k * a.height + py) * a.width + px;
       const float dep = __ldg(a.depth + i);
       if (!isfinite(dep)) continue;
@@ -277,6 +282,88 @@ tsdf_integrate_kernel(const TsdfArgs a) {
       a.color_sum[3 * p] = c0; a.color_sum[3 * p + 1] = c1; a.color_sum[3 * p + 2] = c2;
       a.color_weight[p] = cw;
     }
+  }
+}
+
+// ------------------------------------------------------------------------------------------ mesh cleaning
+// Connected components of a triangle mesh by union-find on `parent` (the labels array): initialise parent[v] = v;
+// hook every face's edges; compress.  A root is only ever hooked under a smaller root, and path halving only moves a
+// parent to one of its ancestors, so parent[v] <= v always and each root is its component's minimum vertex: after
+// compression every label is that minimum, whatever the thread schedule.  Loads of parent go through relaxed
+// device-scope atomics so that no thread keeps a stale copy across the loop of find; the halving stores of the hook
+// pass are relaxed stores.  A non-root never becomes a root again, so a halving store never overwrites a hook.
+using ParentRef = cuda::atomic_ref<int, cuda::thread_scope_device>;
+
+__device__ __forceinline__ int uf_find(int* parent, int x) {
+  while (true) {
+    const int p = ParentRef(parent[x]).load(cuda::memory_order_relaxed);
+    if (p == x) return x;
+    const int gp = ParentRef(parent[p]).load(cuda::memory_order_relaxed);
+    if (gp == p) return p;
+    ParentRef(parent[x]).store(gp, cuda::memory_order_relaxed);      // path halving: gp is an ancestor of x
+    x = gp;
+  }
+}
+
+__device__ __forceinline__ void uf_union(int* parent, int a, int b) {
+  while (true) {
+    a = uf_find(parent, a);
+    b = uf_find(parent, b);
+    if (a == b) return;
+    if (a < b) { const int s = a; a = b; b = s; }
+    if (atomicCAS(parent + a, a, b) == a) return;     // a was still a root: hooked under b; else retry from find
+  }
+}
+
+__global__ void __launch_bounds__(256) uf_init_kernel(int32_t n, int* __restrict__ parent) {
+  for (int64_t v = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; v < n; v += (int64_t)gridDim.x * blockDim.x)
+    parent[v] = (int)v;
+}
+
+// one thread per face: its edges (v0, v1) and (v0, v2) join all three corners
+__global__ void __launch_bounds__(256) uf_hook_kernel(int64_t num_faces, const int32_t* __restrict__ faces,
+                                                      int* parent) {
+  for (int64_t f = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; f < num_faces;
+       f += (int64_t)gridDim.x * blockDim.x) {
+    const int v0 = __ldg(faces + 3 * f), v1 = __ldg(faces + 3 * f + 1), v2 = __ldg(faces + 3 * f + 2);
+    uf_union(parent, v0, v1);
+    uf_union(parent, v0, v2);
+  }
+}
+
+// Each label becomes its root.  The walk makes no halving stores: one could land on a vertex whose thread has
+// already stored its root and put back a non-root ancestor.  The only stores of this pass are roots.
+__global__ void __launch_bounds__(256) uf_compress_kernel(int32_t n, int* parent) {
+  for (int64_t v = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; v < n; v += (int64_t)gridDim.x * blockDim.x) {
+    int x = (int)v;
+    for (int p; (p = ParentRef(parent[x]).load(cuda::memory_order_relaxed)) != x;) x = p;
+    ParentRef(parent[v]).store(x, cuda::memory_order_relaxed);
+  }
+}
+
+struct ViewCountArgs {
+  mnrf_camera_desc cam;
+  int64_t n;
+  const float* points;   // [n, 3]
+  int num_views, height, width;
+  const float* w2c;      // [K, 3, 4]
+  const float* c2p;      // [K or 1, 3, 3]
+  int64_t c2p_stride;    // 9 or 0
+  int32_t* counts;
+};
+
+// One thread per point: the number of views whose image it lands on (project_to_pixel, the rule of the fusion).
+__global__ void __launch_bounds__(256) points_view_count_kernel(const ViewCountArgs a) {
+  for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < a.n; p += (int64_t)gridDim.x * blockDim.x) {
+    const V3 pt{__ldg(a.points + 3 * p), __ldg(a.points + 3 * p + 1), __ldg(a.points + 3 * p + 2)};
+    int c = 0;
+    for (int k = 0; k < a.num_views; ++k) {
+      int px, py;
+      float t;
+      c += project_to_pixel(a.cam, a.w2c + 12 * (int64_t)k, a.c2p + a.c2p_stride * k, pt, a.width, a.height, px, py,
+                            t);
+    }
+    a.counts[p] = c;
   }
 }
 
@@ -351,6 +438,54 @@ extern "C" int mnrf_tsdf_integrate(const mnrf_camera_desc* cam, int32_t nx, int3
     tsdf_integrate_kernel<true><<<blocks, 256, 0, (cudaStream_t)stream>>>(a);
   else
     tsdf_integrate_kernel<false><<<blocks, 256, 0, (cudaStream_t)stream>>>(a);
+  MNRF_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int mnrf_mesh_components(int32_t num_vertices, int64_t num_faces, const int32_t* faces, int32_t* labels,
+                                    mnrf_stream stream) {
+  using namespace mnrf;
+  set_error("");
+  MNRF_CHECK(num_vertices >= 0 && num_faces >= 0, "mnrf_mesh_components: %d vertices, %lld faces", num_vertices,
+             (long long)num_faces);
+  MNRF_CHECK(num_faces == 0 || num_vertices > 0, "mnrf_mesh_components: %lld faces on no vertices",
+             (long long)num_faces);
+  if (num_vertices == 0) return 0;
+  MNRF_CHECK(labels && (faces || num_faces == 0), "mnrf_mesh_components: null pointer");
+  const int cap = mnrf_num_sms() * 16;
+  const int vblocks = (int)std::min<int64_t>((num_vertices + 255) / 256, cap);
+  uf_init_kernel<<<vblocks, 256, 0, (cudaStream_t)stream>>>(num_vertices, labels);
+  if (num_faces > 0) {
+    const int fblocks = (int)std::min<int64_t>((num_faces + 255) / 256, cap);
+    uf_hook_kernel<<<fblocks, 256, 0, (cudaStream_t)stream>>>(num_faces, faces, labels);
+  }
+  uf_compress_kernel<<<vblocks, 256, 0, (cudaStream_t)stream>>>(num_vertices, labels);
+  MNRF_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int mnrf_points_view_count(const mnrf_camera_desc* cam, int64_t n, const float* points, int32_t num_views,
+                                      int32_t height, int32_t width, const float* worldtocams,
+                                      const float* camtopixs, int32_t* counts, mnrf_stream stream) {
+  using namespace mnrf;
+  set_error("");
+  MNRF_CHECK(cam, "mnrf_points_view_count: null camera descriptor");
+  MNRF_CHECK(n >= 0 && num_views >= 0 && height >= 1 && width >= 1,
+             "mnrf_points_view_count: %lld points, %d views of %d x %d pixels", (long long)n, num_views, height,
+             width);
+  MNRF_CHECK(cam->camtype == MNRF_CAM_PERSPECTIVE || cam->camtype == MNRF_CAM_FISHEYE,
+             "mnrf_points_view_count: camtype must be perspective or fisheye");
+  MNRF_CHECK(!cam->has_ndc, "mnrf_points_view_count: NDC cameras are not supported");
+  MNRF_CHECK(cam->num_cameras == 1 || cam->num_cameras == num_views,
+             "mnrf_points_view_count: num_cameras = %d camera-to-pixel matrices for %d views", cam->num_cameras,
+             num_views);
+  if (n == 0) return 0;
+  MNRF_CHECK(points && counts, "mnrf_points_view_count: null point or count pointer");
+  MNRF_CHECK(num_views == 0 || (worldtocams && camtopixs), "mnrf_points_view_count: null view pointer");
+  const ViewCountArgs a{*cam, n, points, num_views, height, width, worldtocams, camtopixs,
+                        cam->num_cameras == 1 ? 0 : 9, counts};
+  const int blocks = (int)std::min<int64_t>((n + 255) / 256, (int64_t)mnrf_num_sms() * 16);
+  points_view_count_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(a);
   MNRF_LAUNCH_CHECK();
   return 0;
 }

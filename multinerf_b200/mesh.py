@@ -73,21 +73,24 @@ def density_grid(model, bbox, resolution, slab_planes=None):
   return grid, h
 
 
-def extract_mesh(model, bbox, resolution, level, slab_planes=None, colors=False):
+def extract_mesh(model, bbox, resolution, level, slab_planes=None, colors=False, keep_components=0, min_views=0,
+                 dataset=None, stats=None):
   """(vertices [V, 3] fp32, faces [F, 3] int32) on the device: the surface density = `level` of `model`'s final
   level inside `bbox` (x0, y0, z0, x1, y1, z1), on a grid of `resolution` points along the longest side.
   Vertices are in world coordinates; face normals point from dense to empty space.  With `colors`, returns
   (vertices, faces, normals [V, 3] fp32, rgb [V, 3] uint8): unit vertex normals from the density grid's gradient,
-  and each vertex's colour from `vertex_colors`."""
+  and each vertex's colour from `vertex_colors`.  `keep_components`, `min_views` (with the training cameras of
+  `dataset`) and `stats`: clean_mesh, applied before the colours are queried."""
   grid, h = density_grid(model, bbox, resolution, slab_planes)
   out = ops.marching_cubes(grid, level, normals=colors)
   del grid
   lo = torch.tensor([float(v) for v in bbox[:3]], device=out[0].device)
-  vertices = out[0] * h + lo
+  vertices, faces, *normals = clean_mesh(out[0] * h + lo, *out[1:], **_clean_args(keep_components, min_views,
+                                                                                   dataset, stats))
   if not colors:
-    return vertices, out[1]
+    return vertices, faces
   # cubic cells: the grid's normals are the world's
-  return vertices, out[1], out[2], vertex_colors(model, vertices, out[2], h * h / 12)
+  return vertices, faces, normals[0], vertex_colors(model, vertices, normals[0], h * h / 12)
 
 
 def vertex_colors(model, vertices, normals, var):
@@ -104,10 +107,17 @@ MESH_METHODS = ('density', 'tsdf')
 
 def validate_config(bundle):
   """The mesh method of `bundle`'s Config, checked: 'density' or 'tsdf'; the TSDF method needs perspective or fisheye
-  views (not NDC) and a truncation of at least one cell, so no cut edge of the fused grid has an unobserved end."""
+  views (not NDC) and a truncation of at least one cell, so no cut edge of the fused grid has an unobserved end.
+  The cleaning options must not be negative, and mesh_min_views projects into the views, so it needs them not NDC
+  either."""
   config = bundle.config
   if config.mesh_method not in MESH_METHODS:
     raise ValueError(f'Config.mesh_method = {config.mesh_method!r}: want one of {MESH_METHODS}')
+  for name in ('mesh_keep_components', 'mesh_min_views'):
+    if getattr(config, name) < 0:
+      raise ValueError(f'Config.{name} = {getattr(config, name)!r}: want 0 (off) or more')
+  if config.mesh_min_views > 0 and config.forward_facing:
+    raise ValueError('Config.mesh_min_views does not support forward-facing (NDC) scenes')
   if config.mesh_method == 'tsdf':
     if config.forward_facing:
       raise ValueError("Config.mesh_method = 'tsdf' does not support forward-facing (NDC) scenes")
@@ -169,26 +179,29 @@ def fuse_tsdf(views, cameras, camtype, bbox, resolution, truncation, colors=Fals
   return (tsdf, weight, color_sum, color_weight), h
 
 
-def tsdf_mesh(state, bbox, h, colors=False):
+def tsdf_mesh(state, bbox, h, colors=False, clean_args=None):
   """Marching cubes on the fused TSDF `state` (fuse_tsdf): the zero crossing of -tsdf (inside > 0, so faces and
   normals point out of the surface), with every point no view observed (weight 0) NaN, so it gives no faces.
   Returns (vertices, faces) in world coordinates, and with `colors` also (normals [V, 3], rgb [V, 3] uint8): each
   vertex's colour is color_sum / color_weight interpolated linearly along its grid edge, rounded as vertex_colors
-  rounds."""
+  rounds.  clean_args: keyword arguments of clean_mesh, applied before the colours are interpolated."""
   tsdf, weight, color_sum, color_weight = state
   grid = torch.where(weight > 0, -tsdf, torch.full_like(tsdf, float('nan')))
   out = ops.marching_cubes(grid, 0.0, normals=colors)
   del grid
   lo = torch.tensor([float(v) for v in bbox[:3]], device=out[0].device)
-  vertices = out[0] * h + lo
+  # the grid-unit vertices ride along as a per-vertex array: the colours are interpolated from them
+  vertices, faces, *per = clean_mesh(out[0] * h + lo, out[1], *((out[2], out[0]) if colors else ()),
+                                     **(clean_args or {}))
   if not colors:
-    return vertices, out[1]
+    return vertices, faces
+  normals, gv = per
   # a vertex lies on a grid edge: its two other coordinates are integers, so the trilinear weights reduce to the
   # linear interpolation between the edge's two ends
   nz, ny, nx = tsdf.shape
-  dims = torch.tensor([nx, ny, nz], device=out[0].device)
-  base = torch.minimum(out[0].floor().long(), dims - 2).clamp_min(0)
-  frac = out[0] - base
+  dims = torch.tensor([nx, ny, nz], device=gv.device)
+  base = torch.minimum(gv.floor().long(), dims - 2).clamp_min(0)
+  frac = gv - base
   cs = torch.zeros(len(vertices), 3, device=vertices.device)
   cw = torch.zeros(len(vertices), device=vertices.device)
   for corner in range(8):
@@ -199,7 +212,7 @@ def tsdf_mesh(state, bbox, h, colors=False):
     cs += wgt[:, None] * color_sum.view(-1, 3)[p]
     cw += wgt * color_weight.view(-1)[p]
   rgb = torch.where(cw[:, None] > 0, cs / cw.clamp_min(1e-30)[:, None], torch.zeros_like(cs))
-  return vertices, out[1], out[2], (rgb.clamp(0, 1) * 255).round().to(torch.uint8)
+  return vertices, faces, normals, (rgb.clamp(0, 1) * 255).round().to(torch.uint8)
 
 
 def render_views(model, dataset):
@@ -214,12 +227,82 @@ def render_views(model, dataset):
     yield idx, r['distance_median'], r['acc'], r['rgb']
 
 
-def extract_mesh_tsdf(model, dataset, bbox, resolution, truncation=3.0, colors=False, batch=8):
+def extract_mesh_tsdf(model, dataset, bbox, resolution, truncation=3.0, colors=False, batch=8, keep_components=0,
+                      min_views=0, stats=None):
   """Config.mesh_method = 'tsdf': render every camera of `dataset` (render_views), fuse the renders (fuse_tsdf, a
-  band of `truncation` cells) and mesh the result (tsdf_mesh).  Returns what extract_mesh returns."""
+  band of `truncation` cells) and mesh the result (tsdf_mesh).  Returns what extract_mesh returns.
+  `keep_components`, `min_views` (against the cameras of `dataset`) and `stats`: clean_mesh, applied before the
+  colours are interpolated."""
   state, h = fuse_tsdf(render_views(model, dataset), dataset.cameras, dataset.camtype, bbox, resolution, truncation,
                        colors=colors, batch=batch, device=model.device)
-  return tsdf_mesh(state, bbox, h, colors=colors)
+  return tsdf_mesh(state, bbox, h, colors=colors,
+                   clean_args=_clean_args(keep_components, min_views, dataset, stats))
+
+
+def clean_mesh(vertices, faces, *per_vertex, keep_components=0, min_views=0, cameras=None, camtype=None,
+               image_size=None, stats=None):
+  """Drops what a user would cut from a raw marching-cubes mesh first, on the device.  Returns (vertices, faces,
+  *per_vertex) in the shape it was given.
+
+  min_views > 0: a vertex counts a view when it lands on that view's image (ops.points_view_count: the pixel rule of
+  the TSDF fusion; frustum only, no occlusion); vertices with fewer than `min_views` views and every face using one
+  are dropped.  cameras: (pixtocams, camtoworlds, distortion_params, pixtocam_ndc) as a dataset holds them;
+  camtype: camera_utils.ProjectionType or its value; image_size: (height, width).
+  keep_components > 0: of the connected components of the remaining faces (ops.mesh_components), ranked by face
+  count, largest first, ties to the smaller minimum vertex index, only the first `keep_components` are kept.
+  A vertex is kept if and only if a kept face uses it; vertices and faces keep their relative order, face indices
+  are renumbered, and each per-vertex array [V, ...] (normals, colours) follows its vertices.  With both options
+  at 0 the inputs come back untouched and nothing is launched.  stats: a dict, given the counts of vertices,
+  faces and components removed (components: those the ranking dropped)."""
+  if keep_components < 0 or min_views < 0:
+    raise ValueError(f'clean_mesh: keep_components = {keep_components}, min_views = {min_views}: want >= 0')
+  if stats is not None:
+    stats.update(vertices_removed=0, faces_removed=0, components_removed=0)
+  if not keep_components and not min_views:
+    return (vertices, faces, *per_vertex)
+  V = vertices.shape[0]
+  keep_face = torch.ones(faces.shape[0], device=faces.device, dtype=torch.bool)
+  if min_views:
+    if cameras is None or camtype is None or image_size is None:
+      raise ValueError('clean_mesh: min_views needs the cameras, camtype and image_size')
+    from . import camera_utils
+    if cameras[3] is not None:
+      raise ValueError('clean_mesh: min_views does not support NDC cameras')
+    camtype = camera_utils.ProjectionType(camtype.value if hasattr(camtype, 'value') else camtype)
+    w2c, c2p = camera_matrices(cameras, vertices.device)
+    counts = ops.points_view_count(vertices, 0 if camtype == camera_utils.ProjectionType.PERSPECTIVE else 1,
+                                   cameras[2], w2c, c2p, *image_size)
+    keep_face = (counts >= min_views)[faces.long()].all(-1)
+  if keep_components:
+    culled = faces[keep_face]
+    labels = ops.mesh_components(culled, V)
+    comp = labels[culled[:, 0].long()].long()                  # a face's component: its first corner's label
+    size = torch.bincount(comp, minlength=V)
+    ids = torch.nonzero(size).view(-1)                         # components with faces, by minimum vertex index
+    order = torch.sort(size[ids], descending=True, stable=True).indices
+    keep_label = torch.zeros(V, device=faces.device, dtype=torch.bool)
+    keep_label[ids[order[:keep_components]]] = True
+    keep_face[keep_face.clone()] = keep_label[comp]
+    if stats is not None:
+      stats['components_removed'] = max(0, len(ids) - keep_components)
+  kept = faces[keep_face]
+  used = torch.zeros(V, device=faces.device, dtype=torch.bool)
+  used[kept.view(-1).long()] = True
+  new_index = (torch.cumsum(used, 0, dtype=torch.int32) - 1)
+  out = (vertices[used], new_index[kept.long()], *(t[used] for t in per_vertex))
+  if stats is not None:
+    stats.update(vertices_removed=V - out[0].shape[0], faces_removed=faces.shape[0] - kept.shape[0])
+  return out
+
+
+def _clean_args(keep_components, min_views, dataset, stats):
+  """clean_mesh's keyword arguments, the cameras taken from `dataset` when `min_views` needs them."""
+  args = dict(keep_components=keep_components, min_views=min_views, stats=stats)
+  if min_views:
+    if dataset is None:
+      raise ValueError('min_views needs the training cameras: pass the dataset')
+    args.update(cameras=dataset.cameras, camtype=dataset.camtype, image_size=(dataset.height, dataset.width))
+  return args
 
 
 def write_ply(path, vertices, faces, normals=None, colors=None):

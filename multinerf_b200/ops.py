@@ -197,6 +197,50 @@ def marching_cubes(grid, level, normals=False):
   return vertices, faces, vnormals
 
 
+def _projection_desc(camtype, distortion_params, num_cameras):
+  """The camera descriptor the forward projection reads (mnrf_tsdf_integrate, mnrf_points_view_count)."""
+  dp = dict(distortion_params or {})
+  return L.CameraDesc(0, num_cameras, int(camtype), int(distortion_params is not None),
+                      *(float(dp.get(k, 0.0)) for k in ('k1', 'k2', 'k3', 'k4', 'p1', 'p2')), 0.0, 0, 0, 1.0, 1.0,
+                      1.0)
+
+
+def mesh_components(faces, num_vertices):
+  """Connected components of the mesh with `num_vertices` vertices and faces [F, 3] int32 on the device
+  (mnrf_mesh_components, csrc/mesh.cu) -> labels [V] int32: each vertex's label is the smallest vertex index of its
+  component.  Checks on the device that every face index lies in [0, V) and reads that one flag back; an index out
+  of range raises ValueError and never reaches the kernel."""
+  lib = L.load()
+  assert faces.dtype == torch.int32 and faces.is_contiguous() and faces.dim() == 2 and faces.shape[1] == 3
+  V, F = int(num_vertices), faces.shape[0]
+  if not 0 <= V < 2 ** 31:
+    raise ValueError(f'mesh_components: {V} vertices')
+  if F and bool(((faces < 0) | (faces >= V)).any()):
+    raise ValueError(f'mesh_components: a face index lies outside [0, {V})')
+  labels = torch.empty(V, device=faces.device, dtype=torch.int32)
+  if V:
+    _count(3 if F else 2)
+    L.check(lib.mnrf_mesh_components(V, F, L.ptr(faces), L.ptr(labels), L.stream_ptr()))
+  return labels
+
+
+def points_view_count(points, camtype, distortion_params, worldtocams, camtopixs, height, width):
+  """For each point [N, 3] fp32 on the device, the number of views whose height x width image it lands on
+  (mnrf_points_view_count, csrc/mesh.cu: the pixel rule of tsdf_integrate) -> counts [N] int32.  camtype 0
+  perspective / 1 fisheye; distortion_params: dict of k1..k4, p1, p2 or None; worldtocams [K, 3, 4], camtopixs
+  [K or 1, 3, 3] fp32 on the device."""
+  lib = L.load()
+  N, K = points.shape[0], worldtocams.shape[0]
+  d = _projection_desc(camtype, distortion_params, camtopixs.shape[0])
+  counts = torch.empty(N, device=points.device, dtype=torch.int32)
+  if N:
+    _count()
+    L.check(lib.mnrf_points_view_count(C.byref(d), N, L.ptr(_f32(points)), K, int(height), int(width),
+                                       L.ptr(_f32(worldtocams)), L.ptr(_f32(camtopixs)), L.ptr(counts),
+                                       L.stream_ptr()))
+  return counts
+
+
 def tsdf_integrate(shape, lo, h, camtype, distortion_params, worldtocams, camtopixs, depth, acc, rgb, tau, tsdf,
                    weight, color_sum=None, color_weight=None):
   """Fuse K views into the TSDF state in place (mnrf_tsdf_integrate, csrc/mesh.cu).  shape (nx, ny, nz) and lo, h:
@@ -206,9 +250,7 @@ def tsdf_integrate(shape, lo, h, camtype, distortion_params, worldtocams, camtop
   lib = L.load()
   nx, ny, nz = shape
   K, H, W = depth.shape
-  dp = dict(distortion_params or {})
-  d = L.CameraDesc(0, camtopixs.shape[0], int(camtype), int(distortion_params is not None),
-                   *(float(dp.get(k, 0.0)) for k in ('k1', 'k2', 'k3', 'k4', 'p1', 'p2')), 0.0, 0, 0, 1.0, 1.0, 1.0)
+  d = _projection_desc(camtype, distortion_params, camtopixs.shape[0])
   _count()
   L.check(lib.mnrf_tsdf_integrate(C.byref(d), nx, ny, nz, *(float(v) for v in lo), float(h), K, H, W,
                                   L.ptr(_f32(worldtocams)), L.ptr(_f32(camtopixs)), L.ptr(_f32(depth)),

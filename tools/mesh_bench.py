@@ -11,9 +11,12 @@
   color:  Model.query_radiance rows/s and its GEMM TFLOP/s as for `query`, on the same NerfMLPs and points, with
           unit view directions; mnrf_mc_normals alone (CUDA events over --reps launches) at 256^3 and 512^3 on the
           `mc` grids; mesh.extract_mesh at --extract_res^3 without and with colours, alternated --reps times;
+  components: ops.mesh_components and mesh.clean_mesh(keep_components=1) (CUDA events over --reps calls) on the
+          512^3 `mc` mesh and on the 512^3 random-init 360.gin extraction, with the bytes the union-find moves by
+          count; mesh.extract_mesh at --extract_res^3 with mesh_keep_components 0 and 1, alternated --reps times;
   device: the card's name and power limit, read in the same run.
 
-  python tools/mesh_bench.py [--rows 8388608] [--extract_res 512] [--out result.json]
+  python tools/mesh_bench.py [--rows 8388608] [--extract_res 512] [--sections all|components] [--out result.json]
 """
 import argparse
 import json
@@ -120,15 +123,82 @@ def bench_mc_normals(n, reps):
   return {'grid': n, 'vertices': V, 'ms': round(ev[0].elapsed_time(ev[1]) / reps, 3)}
 
 
+def events(fn, reps):
+  """Mean ms of fn() over `reps` calls between two CUDA events, after one warm-up call."""
+  fn()
+  ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+  ev[0].record()
+  for _ in range(reps):
+    fn()
+  ev[1].record()
+  torch.cuda.synchronize()
+  return ev[0].elapsed_time(ev[1]) / reps
+
+
+def bench_components(name, v, f, reps):
+  """ops.mesh_components and clean_mesh(keep_components=1) on one mesh.  Bytes by count: the faces read once
+  (12 B a face), the four first parent loads of a face's two unions (16 B), and the labels written by the
+  initialisation and read and written by compression (12 B a vertex)."""
+  V, F = int(v.shape[0]), int(f.shape[0])
+  labels = ops.mesh_components(f, V)
+  ncomp = int((labels == torch.arange(V, device='cuda', dtype=torch.int32)).sum())
+  del labels
+  ms = events(lambda: ops.mesh_components(f, V), reps)
+  clean_ms = events(lambda: mesh.clean_mesh(v, f, keep_components=1), reps)
+  kv, kf = mesh.clean_mesh(v, f, keep_components=1)
+  nbytes = 28 * F + 12 * V
+  return {'mesh': name, 'vertices': V, 'faces': F, 'components_incl_lone_vertices': ncomp,
+          'kept_vertices': int(kv.shape[0]), 'kept_faces': int(kf.shape[0]), 'mesh_components_ms': round(ms, 3),
+          'bytes_by_count': nbytes, 'tb_per_s_by_count': round(nbytes / (ms * 1e-3) / 1e12, 3),
+          'clean_mesh_keep1_ms': round(clean_ms, 3)}
+
+
+def bench_components_section(model, bbox, level, args):
+  out = {'meshes': [], 'extract': {'keep0_s': [], 'keep1_s': []}}
+  v, f = ops.marching_cubes(sphere_noise(512), 0.0)
+  torch.cuda.empty_cache()
+  out['meshes'].append(bench_components('mc 512^3 sphere + noise', v, f, args.reps))
+  del v, f
+  torch.cuda.empty_cache()
+  v, f = mesh.extract_mesh(model, bbox, args.extract_res, level)
+  out['meshes'].append(bench_components(f'360.gin random init, {args.extract_res}^3', v, f, args.reps))
+  del v, f
+  torch.cuda.empty_cache()
+  mesh.extract_mesh(model, bbox, args.extract_res, level, keep_components=1)      # warm-up
+  torch.cuda.empty_cache()
+  for _ in range(args.reps):
+    for key, keep in (('keep0_s', 0), ('keep1_s', 1)):
+      t, o = timed(lambda: mesh.extract_mesh(model, bbox, args.extract_res, level, keep_components=keep), 1)
+      out['extract'][key].append(round(t, 3))
+      out['extract'][f'{key[:5]}_vertices'] = int(o[0].shape[0])
+      del o
+      torch.cuda.empty_cache()
+  return out
+
+
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--rows', type=int, default=1 << 23)
   ap.add_argument('--reps', type=int, default=3)
   ap.add_argument('--extract_res', type=int, default=512)
+  ap.add_argument('--sections', default='all', choices=('all', 'components'))
   ap.add_argument('--out', default=None)
   args = ap.parse_args()
   lib.require_device()
   res = {'device': device_info(), 'query': {}, 'mc': [], 'extract': None}
+  if args.sections == 'components':
+    b = configs.bundle_360()
+    model = models.Model(b)
+    model.init(seed=0)
+    bbox = mesh.default_bbox(b)
+    grid, _ = mesh.density_grid(model, bbox, args.extract_res)
+    level = float(grid.median())
+    del grid
+    torch.cuda.empty_cache()
+    res = {'device': res['device'], 'level': level,
+           'components': bench_components_section(model, bbox, level, args), 'device_after': device_info()}
+    emit(res, args.out)
+    return
   for name, make in (('360', configs.bundle_360), ('blender_256', configs.bundle_blender_256)):
     res['query'][name] = bench_query(make(), args.rows, args.reps)
     torch.cuda.empty_cache()
@@ -165,11 +235,17 @@ def main():
       del out
       torch.cuda.empty_cache()
   res['color'] = color
+  torch.cuda.empty_cache()
+  res['components'] = bench_components_section(model, bbox, level, args)
   res['device_after'] = device_info()
+  emit(res, args.out)
+
+
+def emit(res, path):
   line = json.dumps(res)
   print(line, flush=True)
-  if args.out:
-    with open(args.out, 'w') as fh:
+  if path:
+    with open(path, 'w') as fh:
       fh.write(line + '\n')
 
 
