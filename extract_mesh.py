@@ -8,7 +8,9 @@ forward-facing scenes must set it; Config.mesh_vertex_colors = True adds vertex 
 Config.mesh_method = 'density' (default) meshes the final level's density at Config.mesh_level; 'tsdf' renders every
 training view, fuses the rendered depth into a truncated signed-distance grid (Config.mesh_tsdf_truncation cells) and
 meshes its zero crossing.  Config.mesh_min_views drops what fewer training views see, and
-Config.mesh_keep_components keeps only the largest connected components (mesh.clean_mesh).  One process on one GPU.
+Config.mesh_keep_components keeps only the largest connected components (mesh.clean_mesh).
+Config.mesh_target_faces then simplifies the mesh to about that many faces by quadric edge collapse
+(mesh.simplify_mesh).  One process on one GPU.
 """
 import dataclasses
 import os
@@ -39,7 +41,8 @@ def main(argv=None):
     # every training camera, all pixels, no render path
     dataset = datasets.load_dataset('train', config.data_dir, dataclasses.replace(config, render_path=False),
                                     device=model.device)
-  clean = dict(keep_components=config.mesh_keep_components, min_views=config.mesh_min_views, stats={})
+  clean = dict(keep_components=config.mesh_keep_components, min_views=config.mesh_min_views,
+               target_faces=config.mesh_target_faces, stats={})
   t0 = time.time()
   if method == 'tsdf':
     vertices, faces, *extra = mesh.extract_mesh_tsdf(model, dataset, bbox, config.mesh_resolution,
@@ -57,6 +60,12 @@ def main(argv=None):
     print(f"cleaning removed {s['vertices_removed']} vertices, {s['faces_removed']} faces and "
           f"{s['components_removed']} components (mesh_min_views {config.mesh_min_views}, "
           f"mesh_keep_components {config.mesh_keep_components})", flush=True)
+  if config.mesh_target_faces:
+    s = clean['stats']
+    print(f"simplified {s['faces_before']} -> {s['faces_after']} faces in {s['rounds']} rounds "
+          f"(mesh_target_faces {config.mesh_target_faces})" +
+          ('' if s['target_reached'] else ': stalled before the target, no edge left that may be collapsed'),
+          flush=True)
   out_dir = os.path.join(config.checkpoint_dir, 'mesh')
   os.makedirs(out_dir, exist_ok=True)
   path = os.path.join(out_dir, f'mesh_step_{step}.ply')

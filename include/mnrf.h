@@ -684,6 +684,69 @@ int mnrf_points_view_count(const mnrf_camera_desc* cam, int64_t n, const float* 
                            int32_t height, int32_t width, const float* worldtocams, const float* camtopixs,
                            int32_t* counts, mnrf_stream stream);
 
+/* ---- mesh simplification by quadric edge collapse (mesh.simplify_mesh) -----------------------------------------
+ * Parallel greedy quadric edge collapse (Garland and Heckbert 1997) in rounds.  No reference counterpart.  The
+ * mesh: num_vertices vertices [V, 3] fp32 and num_faces faces [F, 3] int32; every face index lies in [0, V) and no
+ * face repeats an index (mesh.simplify_mesh checks both on the device before the first call); V < 2^31.
+ * The topology of the current faces, rebuilt by the caller before each round (mesh.mesh_topology):
+ *   edges [E, 2] int32: the unique undirected edges (a, b), a < b, sorted by (a, b); E < 2^32, so an edge index
+ *     fits the low 32 bits of a key;
+ *   edge_off [E + 1] int64, edge_face [edge_off[E]] int32: the faces of edge e, ascending, at
+ *     edge_face[edge_off[e] .. edge_off[e + 1]) (its face count is the difference);
+ *   vf_off [V + 1] int64, vf_face [3 F] int32: the faces at vertex v, ascending, at vf_face[vf_off[v] .. vf_off[v + 1]).
+ * A quadric is 10 fp64 values (aa, ab, ac, ad, bb, bc, bd, cc, cd, dd) of w (a, b, c, d)^T (a, b, c, d) for the
+ * plane a x + b y + c z + d = 0 of unit normal (a, b, c) and weight w.  All geometry is fp64 in registers; the kernels
+ * are compiled without FMA contraction, so their results are bit-reproducible from the stated operations
+ * (tests/mesh_simplify_ref.py restates them).  The only atomics are atomicOr of flag bits and atomicMin of keys, so
+ * every output is bit-deterministic. */
+
+/* quadrics [V, 10] fp64: per vertex, the sum in this order of the plane quadric of each face at it (in face order),
+ * weighted by the face's area (0 for a zero-area face), then of each boundary edge at it (in edge order): the plane
+ * containing the edge and perpendicular to its face, weighted by 1000 |e|^2 (kBoundaryWeight).  The boundary edges
+ * (the edges in exactly one face) of the current faces: boundary_edges [nb, 2] int32 in edge order, boundary_face
+ * [nb] int32 their faces, vb_off [V + 1] int64 and vb_edge [2 nb] int32 the boundary edges at each vertex,
+ * ascending. */
+int mnrf_mesh_quadrics(int32_t num_vertices, int64_t num_faces, const float* vertices, const int32_t* faces,
+                       const int64_t* vf_off, const int32_t* vf_face, int64_t num_boundary,
+                       const int32_t* boundary_edges, const int32_t* boundary_face, const int64_t* vb_off,
+                       const int32_t* vb_edge, double* quadrics, mnrf_stream stream);
+
+/* Per edge e = (a, b): positions [E, 3] fp32, where a collapse of e puts the survivor, and keys [E] uint64.
+ * Q = Q_a + Q_b; the position solves A v = -(q_ad, q_bd, q_cd) (A the upper 3x3 of Q) by cofactors unless
+ * |det A| <= 1e-10 max|A_ij|^3 (kDetRel) or the solution lies farther than |b - a| from the midpoint; then it is the
+ * cheapest of a, b and the midpoint (rounded to fp32), ties to the earlier.  The solution is rounded to fp32 before
+ * its cost v^T Q v is taken; the cost is clamped to >= 0.  key = (fp32 bits of the cost, rounded to nearest) << 32 | e
+ * when the edge may be collapsed, UINT64_MAX when not.  It may be collapsed when: it has 1 or 2 faces; neither end
+ * touches an edge of more than 2 faces; it is not an edge of 2 faces whose ends are both on the boundary; at most 24
+ * faces (kMaxValence) are at each end; every common neighbour of a and b is an apex of one of its faces, and no two
+ * faces (a, x, y) and (b, x, y) exist; the collapse leaves a face of star(a) u star(b); and each face with exactly
+ * one of a, b, that corner moved to the position, keeps a nonzero normal n' with n'.n > 0 where its normal n is
+ * nonzero.  flags [V] int32 is scratch (bit 0: on the boundary, bit 1: on an edge of more than 2 faces). */
+int mnrf_mesh_edge_cost(int32_t num_vertices, int64_t num_faces, int64_t num_edges, const float* vertices,
+                        const int32_t* faces, const double* quadrics, const int32_t* edges, const int64_t* edge_off,
+                        const int32_t* edge_face, const int64_t* vf_off, const int32_t* vf_face, int32_t* flags,
+                        uint64_t* keys, float* positions, mnrf_stream stream);
+
+/* selected [E] uint8 = 1 for the edges a round collapses: with vmin[v] the least key of the edges at v, fmin[f] the
+ * least vmin of f's corners and rmin[v] the least fmin of the faces at v, edge (a, b) is selected when its key is
+ * not UINT64_MAX and rmin[a] == rmin[b] == key.  No face touches two selected edges, and the least key is always
+ * selected.  vmin, rmin [V] uint64 are scratch (they end holding those minima). */
+int mnrf_mesh_collapse_select(int32_t num_vertices, int64_t num_faces, int64_t num_edges, const int32_t* faces,
+                              const int32_t* edges, const uint64_t* keys, uint64_t* vmin, uint64_t* rmin,
+                              uint8_t* selected, mnrf_stream stream);
+
+/* Collapses each edge e = (a, b) with collapse[e] != 0, in place; the collapsed edges must be selected ones (a
+ * subset of mnrf_mesh_collapse_select's, on the same topology and positions).  a survives: vertices[a] =
+ * positions[e], quadrics[a] = Q_a + Q_b; with normals [V, 3] (may be NULL), normals[a] = the normalised
+ * (1 - t) n_a + t n_b, t = clamp((p - a).(b - a) / |b - a|^2, 0, 1) (0 when a = b), unchanged when the blend is
+ * zero.  The faces of e get face_alive[f] = 0 (every other face 1); in the other faces at b, b becomes a, so
+ * the winding is kept.  b keeps its (now unused) entries. */
+int mnrf_mesh_collapse_apply(int32_t num_vertices, int64_t num_faces, int64_t num_edges, const uint8_t* collapse,
+                             const int32_t* edges, const int64_t* edge_off, const int32_t* edge_face,
+                             const int64_t* vf_off, const int32_t* vf_face, const float* positions, float* vertices,
+                             double* quadrics, float* normals, int32_t* faces, uint8_t* face_alive,
+                             mnrf_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

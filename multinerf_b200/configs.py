@@ -135,6 +135,9 @@ class Config:
   # mesh_keep_components: then keep only this many connected components, the largest by face count.
   mesh_min_views: int = 0
   mesh_keep_components: int = 0
+  # simplification, right after cleaning (mesh.simplify_mesh): quadric edge collapse down to about this many faces;
+  # 0 turns it off.
+  mesh_target_faces: int = 0
 
 
 @dataclasses.dataclass

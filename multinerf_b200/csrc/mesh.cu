@@ -19,7 +19,7 @@
 // truncated signed distance, weight and colour sums held in registers across every view of a launch.
 //
 // And the two passes of mesh cleaning: connected components by union-find (uf_*_kernel) and the number of views
-// each vertex lands in (points_view_count_kernel).
+// each vertex lands in (points_view_count_kernel); and mesh simplification by quadric edge collapse (qem_*_kernel).
 #include <algorithm>
 
 #include <cuda/atomic>
@@ -367,6 +367,306 @@ __global__ void __launch_bounds__(256) points_view_count_kernel(const ViewCountA
   }
 }
 
+// ------------------------------------------------------------------------------------- mesh simplification
+// Parallel greedy quadric edge collapse (Garland and Heckbert 1997) in rounds; mesh.simplify_mesh drives it and
+// tests/mesh_simplify_ref.py restates every kernel below in numpy.  All geometry is fp64 in registers (positions are
+// stored fp32, quadrics fp64) and the unit is compiled with -fmad=false, so each expression rounds exactly as its
+// numpy restatement, operation by operation: keep both in the same order.  The only atomics are atomicOr of
+// constant flag bits and atomicMin of 64-bit keys, whose results do not depend on their order.
+// A quadric is 10 fp64 values: (aa, ab, ac, ad, bb, bc, bd, cc, cd, dd) of w (a, b, c, d)^T (a, b, c, d).
+constexpr double kBoundaryWeight = 1000.0;    // boundary-edge planes, times |e|^2
+constexpr double kDetRel = 1e-10;             // |det A| <= kDetRel max|A_ij|^3: A is near-singular
+constexpr int kMaxValence = 24;               // faces at a vertex; edges at a vertex with more are never collapsed
+constexpr int kFlagBoundary = 1, kFlagNonManifold = 2;
+
+struct D3 {
+  double x, y, z;
+};
+
+__device__ __forceinline__ D3 ld_pos(const float* __restrict__ v, int i) {
+  return D3{(double)v[3 * (int64_t)i], (double)v[3 * (int64_t)i + 1], (double)v[3 * (int64_t)i + 2]};
+}
+__device__ __forceinline__ D3 sub(D3 a, D3 b) { return D3{a.x - b.x, a.y - b.y, a.z - b.z}; }
+__device__ __forceinline__ double dot(D3 a, D3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
+__device__ __forceinline__ D3 cross(D3 a, D3 b) {
+  return D3{a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x};
+}
+
+// q += w (a, b, c, d)^T (a, b, c, d), each product as w * (a * b)
+__device__ __forceinline__ void add_plane(double q[10], double a, double b, double c, double d, double w) {
+  q[0] = q[0] + w * (a * a); q[1] = q[1] + w * (a * b); q[2] = q[2] + w * (a * c); q[3] = q[3] + w * (a * d);
+  q[4] = q[4] + w * (b * b); q[5] = q[5] + w * (b * c); q[6] = q[6] + w * (b * d);
+  q[7] = q[7] + w * (c * c); q[8] = q[8] + w * (c * d); q[9] = q[9] + w * (d * d);
+}
+
+// The unit normal of the plane through p0, p1, p2 (from (p1 - p0) x (p2 - p0)) and twice the triangle's area;
+// false when the area is 0.
+__device__ __forceinline__ bool face_plane(D3 p0, D3 p1, D3 p2, D3& u, double& len) {
+  const D3 n = cross(sub(p1, p0), sub(p2, p0));
+  len = sqrt(dot(n, n));
+  if (!(len > 0.0)) return false;
+  u = D3{n.x / len, n.y / len, n.z / len};
+  return true;
+}
+
+// v^T Q v of the homogeneous point (v, 1)
+__device__ __forceinline__ double quadric_eval(const double q[10], D3 v) {
+  return v.x * (q[0] * v.x + 2.0 * (q[1] * v.y + q[2] * v.z + q[3])) + v.y * (q[4] * v.y + 2.0 * (q[5] * v.z + q[6])) +
+         v.z * (q[7] * v.z + 2.0 * q[8]) + q[9];
+}
+
+__device__ __forceinline__ D3 round_f32(D3 v) {
+  return D3{(double)__double2float_rn(v.x), (double)__double2float_rn(v.y), (double)__double2float_rn(v.z)};
+}
+
+__device__ __forceinline__ bool has_corner(const int32_t* __restrict__ faces, int f, int v) {
+  const int64_t o = 3 * (int64_t)f;
+  return faces[o] == v || faces[o + 1] == v || faces[o + 2] == v;
+}
+
+struct QemArgs {
+  int32_t nv;
+  int64_t nf, ne, nb;
+  float* vertices;          // [nv, 3]
+  int32_t* faces;           // [nf, 3]
+  double* quadrics;         // [nv, 10]
+  float* normals;           // [nv, 3] or null
+  const int32_t* edges;     // [ne, 2]: (a, b), a < b, sorted
+  const int64_t* edge_off;  // [ne + 1]: faces of edge e at edge_face[edge_off[e], edge_off[e + 1])
+  const int32_t* edge_face;
+  const int64_t* vf_off;    // [nv + 1]: faces at v at vf_face[vf_off[v], vf_off[v + 1]), ascending
+  const int32_t* vf_face;
+  const int32_t* bnd_edges; // [nb, 2]: the boundary edges, in edge order
+  const int32_t* bnd_face;  // [nb]: the one face of each
+  const int64_t* vb_off;    // [nv + 1]: boundary edges at v at vb_edge[vb_off[v], vb_off[v + 1]), ascending
+  const int32_t* vb_edge;
+  int32_t* flags;           // [nv]
+  uint64_t* keys;           // [ne]
+  float* positions;         // [ne, 3]
+  uint64_t* vmin;           // [nv]
+  uint64_t* rmin;           // [nv]
+  uint8_t* selected;        // [ne]
+  const uint8_t* collapse;  // [ne]
+  uint8_t* face_alive;      // [nf]
+};
+
+#define QEM_LOOP(i, n) for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < (n); \
+                            i += (int64_t)gridDim.x * blockDim.x)
+
+// Per vertex: the area-weighted planes of its faces in face order, then the boundary-edge planes of its boundary
+// edges in edge order.  A boundary edge's plane contains the edge and is perpendicular to its face.
+__global__ void __launch_bounds__(256) qem_quadrics_kernel(const QemArgs a) {
+  QEM_LOOP(v, a.nv) {
+    double q[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    for (int64_t k = a.vf_off[v]; k < a.vf_off[v + 1]; ++k) {
+      const int64_t f = a.vf_face[k];
+      const D3 p0 = ld_pos(a.vertices, a.faces[3 * f]);
+      D3 u;
+      double len;
+      if (!face_plane(p0, ld_pos(a.vertices, a.faces[3 * f + 1]), ld_pos(a.vertices, a.faces[3 * f + 2]), u, len))
+        continue;
+      add_plane(q, u.x, u.y, u.z, -dot(u, p0), 0.5 * len);
+    }
+    for (int64_t k = a.vb_off[v]; k < a.vb_off[v + 1]; ++k) {
+      const int64_t e = a.vb_edge[k], f = a.bnd_face[e];
+      D3 u;
+      double len;
+      if (!face_plane(ld_pos(a.vertices, a.faces[3 * f]), ld_pos(a.vertices, a.faces[3 * f + 1]),
+                      ld_pos(a.vertices, a.faces[3 * f + 2]), u, len))
+        continue;
+      const D3 x = ld_pos(a.vertices, a.bnd_edges[2 * e]);
+      const D3 ev = sub(ld_pos(a.vertices, a.bnd_edges[2 * e + 1]), x);
+      const D3 m = cross(ev, u);
+      const double ml = sqrt(dot(m, m));
+      if (!(ml > 0.0)) continue;
+      const D3 mu{m.x / ml, m.y / ml, m.z / ml};
+      add_plane(q, mu.x, mu.y, mu.z, -dot(mu, x), kBoundaryWeight * dot(ev, ev));
+    }
+    for (int i = 0; i < 10; ++i) a.quadrics[10 * v + i] = q[i];
+  }
+}
+
+__global__ void __launch_bounds__(256) qem_flags_kernel(const QemArgs a) {
+  QEM_LOOP(e, a.ne) {
+    const int64_t c = a.edge_off[e + 1] - a.edge_off[e];
+    const int bit = c == 1 ? kFlagBoundary : c > 2 ? kFlagNonManifold : 0;
+    if (bit) {
+      atomicOr(a.flags + a.edges[2 * e], bit);
+      atomicOr(a.flags + a.edges[2 * e + 1], bit);
+    }
+  }
+}
+
+// Whether moving corner `from` of face f to p keeps the face's orientation: the new normal is not zero, and where
+// the old one is not zero, their dot product is positive.
+__device__ __forceinline__ bool keeps_orientation(const QemArgs& a, int64_t f, int from, D3 p) {
+  const int v0 = a.faces[3 * f], v1 = a.faces[3 * f + 1], v2 = a.faces[3 * f + 2];
+  const D3 c0 = ld_pos(a.vertices, v0), c1 = ld_pos(a.vertices, v1), c2 = ld_pos(a.vertices, v2);
+  const D3 d0 = v0 == from ? p : c0, d1 = v1 == from ? p : c1, d2 = v2 == from ? p : c2;
+  const D3 n = cross(sub(c1, c0), sub(c2, c0));
+  const D3 m = cross(sub(d1, d0), sub(d2, d0));
+  if (m.x == 0.0 && m.y == 0.0 && m.z == 0.0) return false;
+  if (n.x == 0.0 && n.y == 0.0 && n.z == 0.0) return true;
+  return dot(m, n) > 0.0;
+}
+
+// Whether a face at v has x as a corner: x is a neighbour of v
+__device__ __forceinline__ bool star_has(const QemArgs& a, int v, int x) {
+  for (int64_t k = a.vf_off[v]; k < a.vf_off[v + 1]; ++k)
+    if (has_corner(a.faces, a.vf_face[k], x)) return true;
+  return false;
+}
+
+// Per edge (a, b): the position and cost of its collapse and, when it may be collapsed, its key.  (256, 1): at the
+// default bound ptxas caps the kernel at 80 registers and spills.
+__global__ void __launch_bounds__(256, 1) qem_cost_kernel(const QemArgs a) {
+  QEM_LOOP(e, a.ne) {
+    const int va = a.edges[2 * e], vb = a.edges[2 * e + 1];
+    double q[10];
+    for (int i = 0; i < 10; ++i) q[i] = a.quadrics[10 * (int64_t)va + i] + a.quadrics[10 * (int64_t)vb + i];
+    const D3 pa = ld_pos(a.vertices, va), pb = ld_pos(a.vertices, vb);
+    // the minimiser of v^T Q v: A v = -(q3, q6, q8) by cofactors
+    const double c00 = q[4] * q[7] - q[5] * q[5], c01 = q[5] * q[2] - q[1] * q[7], c02 = q[1] * q[5] - q[4] * q[2];
+    const double c11 = q[0] * q[7] - q[2] * q[2], c12 = q[1] * q[2] - q[0] * q[5], c22 = q[0] * q[4] - q[1] * q[1];
+    const double det = q[0] * c00 + q[1] * c01 + q[2] * c02;
+    const double s = fmax(fmax(fmax(fabs(q[0]), fabs(q[1])), fmax(fabs(q[2]), fabs(q[4]))), fmax(fabs(q[5]), fabs(q[7])));
+    const D3 mid{(pa.x + pb.x) * 0.5, (pa.y + pb.y) * 0.5, (pa.z + pb.z) * 0.5};
+    const D3 ev = sub(pb, pa);
+    bool solved = fabs(det) > kDetRel * (s * s * s);
+    D3 p;
+    double cost;
+    if (solved) {
+      const D3 x{-(c00 * q[3] + c01 * q[6] + c02 * q[8]) / det, -(c01 * q[3] + c11 * q[6] + c12 * q[8]) / det,
+                 -(c02 * q[3] + c12 * q[6] + c22 * q[8]) / det};
+      const D3 dm = sub(x, mid);
+      solved = dot(dm, dm) <= dot(ev, ev);
+      if (solved) {
+        p = round_f32(x);
+        cost = quadric_eval(q, p);
+      }
+    }
+    if (!solved) {   // the cheapest of a, b and the midpoint, ties to the earlier
+      p = pa;
+      cost = quadric_eval(q, pa);
+      const double cb = quadric_eval(q, pb);
+      if (cb < cost) { p = pb; cost = cb; }
+      const D3 pm = round_f32(mid);
+      const double cm = quadric_eval(q, pm);
+      if (cm < cost) { p = pm; cost = cm; }
+    }
+    cost = cost > 0.0 ? cost : 0.0;
+    a.positions[3 * e] = (float)p.x;
+    a.positions[3 * e + 1] = (float)p.y;
+    a.positions[3 * e + 2] = (float)p.z;
+
+    uint64_t key = ~0ull;
+    const int64_t s0 = a.edge_off[e], nfe = a.edge_off[e + 1] - s0;
+    const int fl = a.flags[va] | a.flags[vb];
+    const int64_t da = a.vf_off[va + 1] - a.vf_off[va], db = a.vf_off[vb + 1] - a.vf_off[vb];
+    bool ok = (nfe == 1 || nfe == 2) && !(fl & kFlagNonManifold) &&
+              !(nfe == 2 && (a.flags[va] & kFlagBoundary) && (a.flags[vb] & kFlagBoundary)) && da <= kMaxValence &&
+              db <= kMaxValence && da + db - nfe > nfe;
+    // the apexes of the edge's faces
+    int apex0 = -1, apex1 = -1;
+    for (int j = 0; ok && j < nfe; ++j) {
+      const int64_t f = a.edge_face[s0 + j];
+      for (int i = 0; i < 3; ++i) {
+        const int v = a.faces[3 * f + i];
+        if (v != va && v != vb) (j == 0 ? apex0 : apex1) = v;
+      }
+    }
+    // link condition: every common neighbour of a and b is an apex, and no faces (a, x, y) and (b, x, y) both exist
+    for (int64_t k = a.vf_off[va]; ok && k < a.vf_off[va + 1]; ++k) {
+      const int64_t f = a.vf_face[k];
+      int x = -1, y = -1;
+      bool with_b = false;
+      for (int i = 0; i < 3; ++i) {
+        const int v = a.faces[3 * f + i];
+        if (v == vb) with_b = true;
+        else if (v != va) (x < 0 ? x : y) = v;
+      }
+      if (x >= 0 && x != apex0 && x != apex1 && star_has(a, vb, x)) ok = false;
+      if (y >= 0 && y != apex0 && y != apex1 && star_has(a, vb, y)) ok = false;
+      if (!ok || with_b || y < 0) continue;
+      for (int64_t l = a.vf_off[vb]; ok && l < a.vf_off[vb + 1]; ++l) {
+        const int g = a.vf_face[l];
+        if (has_corner(a.faces, g, x) && has_corner(a.faces, g, y)) ok = false;
+      }
+      if (ok) ok = keeps_orientation(a, f, va, p);
+    }
+    for (int64_t k = a.vf_off[vb]; ok && k < a.vf_off[vb + 1]; ++k) {
+      const int64_t f = a.vf_face[k];
+      if (!has_corner(a.faces, (int)f, va)) ok = keeps_orientation(a, f, vb, p);
+    }
+    if (ok) key = (uint64_t)__float_as_uint(__double2float_rn(cost)) << 32 | (uint64_t)e;
+    a.keys[e] = key;
+  }
+}
+
+__global__ void __launch_bounds__(256) qem_vmin_kernel(const QemArgs a) {
+  QEM_LOOP(e, a.ne) {
+    const uint64_t k = a.keys[e];
+    if (k == ~0ull) continue;
+    atomicMin((unsigned long long*)a.vmin + a.edges[2 * e], (unsigned long long)k);
+    atomicMin((unsigned long long*)a.vmin + a.edges[2 * e + 1], (unsigned long long)k);
+  }
+}
+
+// fmin[f] = min of vmin over f's corners, folded straight into rmin of each corner
+__global__ void __launch_bounds__(256) qem_rmin_kernel(const QemArgs a) {
+  QEM_LOOP(f, a.nf) {
+    const int v0 = a.faces[3 * f], v1 = a.faces[3 * f + 1], v2 = a.faces[3 * f + 2];
+    const uint64_t m = min(a.vmin[v0], min(a.vmin[v1], a.vmin[v2]));
+    if (m == ~0ull) continue;
+    atomicMin((unsigned long long*)a.rmin + v0, (unsigned long long)m);
+    atomicMin((unsigned long long*)a.rmin + v1, (unsigned long long)m);
+    atomicMin((unsigned long long*)a.rmin + v2, (unsigned long long)m);
+  }
+}
+
+__global__ void __launch_bounds__(256) qem_select_kernel(const QemArgs a) {
+  QEM_LOOP(e, a.ne) {
+    const uint64_t k = a.keys[e];
+    a.selected[e] = k != ~0ull && a.rmin[a.edges[2 * e]] == k && a.rmin[a.edges[2 * e + 1]] == k;
+  }
+}
+
+// Per collapsed edge (a, b), a < b: a moves to the edge's position and takes Q_a + Q_b and the blended normal; the
+// edge's faces die; b becomes a in its other faces.  Collapsed edges have disjoint stars, so nothing races.
+__global__ void __launch_bounds__(256) qem_apply_kernel(const QemArgs a) {
+  QEM_LOOP(e, a.ne) {
+    if (!a.collapse[e]) continue;
+    const int va = a.edges[2 * e], vb = a.edges[2 * e + 1];
+    const D3 p{(double)a.positions[3 * e], (double)a.positions[3 * e + 1], (double)a.positions[3 * e + 2]};
+    if (a.normals) {
+      const D3 pa = ld_pos(a.vertices, va), ev = sub(ld_pos(a.vertices, vb), pa);
+      const double el2 = dot(ev, ev);
+      double t = el2 > 0.0 ? dot(sub(p, pa), ev) / el2 : 0.0;
+      t = fmin(fmax(t, 0.0), 1.0);
+      const D3 na = ld_pos(a.normals, va), nb = ld_pos(a.normals, vb);
+      const D3 n{(1.0 - t) * na.x + t * nb.x, (1.0 - t) * na.y + t * nb.y, (1.0 - t) * na.z + t * nb.z};
+      const double len = sqrt(dot(n, n));
+      if (len > 0.0) {
+        a.normals[3 * (int64_t)va] = (float)(n.x / len);
+        a.normals[3 * (int64_t)va + 1] = (float)(n.y / len);
+        a.normals[3 * (int64_t)va + 2] = (float)(n.z / len);
+      }
+    }
+    a.vertices[3 * (int64_t)va] = (float)p.x;
+    a.vertices[3 * (int64_t)va + 1] = (float)p.y;
+    a.vertices[3 * (int64_t)va + 2] = (float)p.z;
+    for (int i = 0; i < 10; ++i)
+      a.quadrics[10 * (int64_t)va + i] = a.quadrics[10 * (int64_t)va + i] + a.quadrics[10 * (int64_t)vb + i];
+    for (int64_t k = a.edge_off[e]; k < a.edge_off[e + 1]; ++k) a.face_alive[a.edge_face[k]] = 0;
+    for (int64_t k = a.vf_off[vb]; k < a.vf_off[vb + 1]; ++k) {
+      const int64_t f = a.vf_face[k];
+      if (has_corner(a.faces, (int)f, va)) continue;
+      for (int i = 0; i < 3; ++i)
+        if (a.faces[3 * f + i] == vb) a.faces[3 * f + i] = va;
+    }
+  }
+}
+
 }  // namespace mnrf
 
 extern "C" int mnrf_marching_cubes(int32_t phase, int32_t nx, int32_t ny, int32_t nz, const float* grid, float level,
@@ -486,6 +786,113 @@ extern "C" int mnrf_points_view_count(const mnrf_camera_desc* cam, int64_t n, co
                         cam->num_cameras == 1 ? 0 : 9, counts};
   const int blocks = (int)std::min<int64_t>((n + 255) / 256, (int64_t)mnrf_num_sms() * 16);
   points_view_count_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(a);
+  MNRF_LAUNCH_CHECK();
+  return 0;
+}
+
+namespace {
+int qem_blocks(int64_t n) { return (int)std::min<int64_t>((n + 255) / 256, (int64_t)mnrf_num_sms() * 16); }
+}  // namespace
+
+extern "C" int mnrf_mesh_quadrics(int32_t num_vertices, int64_t num_faces, const float* vertices,
+                                  const int32_t* faces, const int64_t* vf_off, const int32_t* vf_face,
+                                  int64_t num_boundary, const int32_t* boundary_edges, const int32_t* boundary_face,
+                                  const int64_t* vb_off, const int32_t* vb_edge, double* quadrics,
+                                  mnrf_stream stream) {
+  using namespace mnrf;
+  set_error("");
+  MNRF_CHECK(num_vertices >= 0 && num_faces >= 0 && num_boundary >= 0,
+             "mnrf_mesh_quadrics: %d vertices, %lld faces, %lld boundary edges", num_vertices, (long long)num_faces,
+             (long long)num_boundary);
+  if (num_vertices == 0) return 0;
+  MNRF_CHECK(vertices && vf_off && vb_off && quadrics && (faces && vf_face || num_faces == 0) &&
+             (boundary_edges && boundary_face && vb_edge || num_boundary == 0),
+             "mnrf_mesh_quadrics: null pointer");
+  QemArgs a{};
+  a.nv = num_vertices; a.nf = num_faces; a.nb = num_boundary;
+  a.vertices = const_cast<float*>(vertices); a.faces = const_cast<int32_t*>(faces); a.quadrics = quadrics;
+  a.vf_off = vf_off; a.vf_face = vf_face; a.bnd_edges = boundary_edges; a.bnd_face = boundary_face;
+  a.vb_off = vb_off; a.vb_edge = vb_edge;
+  qem_quadrics_kernel<<<qem_blocks(num_vertices), 256, 0, (cudaStream_t)stream>>>(a);
+  MNRF_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int mnrf_mesh_edge_cost(int32_t num_vertices, int64_t num_faces, int64_t num_edges, const float* vertices,
+                                   const int32_t* faces, const double* quadrics, const int32_t* edges,
+                                   const int64_t* edge_off, const int32_t* edge_face, const int64_t* vf_off,
+                                   const int32_t* vf_face, int32_t* flags, uint64_t* keys, float* positions,
+                                   mnrf_stream stream) {
+  using namespace mnrf;
+  set_error("");
+  MNRF_CHECK(num_vertices >= 0 && num_faces >= 0 && num_edges >= 0 && num_edges <= (int64_t)UINT32_MAX,
+             "mnrf_mesh_edge_cost: %d vertices, %lld faces, %lld edges (at most 2^32 - 1)", num_vertices,
+             (long long)num_faces, (long long)num_edges);
+  if (num_edges == 0) return 0;
+  MNRF_CHECK(num_vertices > 0 && num_faces > 0, "mnrf_mesh_edge_cost: edges without vertices or faces");
+  MNRF_CHECK(vertices && faces && quadrics && edges && edge_off && edge_face && vf_off && vf_face && flags && keys &&
+             positions, "mnrf_mesh_edge_cost: null pointer");
+  QemArgs a{};
+  a.nv = num_vertices; a.nf = num_faces; a.ne = num_edges;
+  a.vertices = const_cast<float*>(vertices); a.faces = const_cast<int32_t*>(faces);
+  a.quadrics = const_cast<double*>(quadrics); a.edges = edges; a.edge_off = edge_off; a.edge_face = edge_face;
+  a.vf_off = vf_off; a.vf_face = vf_face; a.flags = flags; a.keys = keys; a.positions = positions;
+  MNRF_CUDA(cudaMemsetAsync(flags, 0, sizeof(int32_t) * (size_t)num_vertices, (cudaStream_t)stream));
+  qem_flags_kernel<<<qem_blocks(num_edges), 256, 0, (cudaStream_t)stream>>>(a);
+  qem_cost_kernel<<<qem_blocks(num_edges), 256, 0, (cudaStream_t)stream>>>(a);
+  MNRF_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int mnrf_mesh_collapse_select(int32_t num_vertices, int64_t num_faces, int64_t num_edges,
+                                         const int32_t* faces, const int32_t* edges, const uint64_t* keys,
+                                         uint64_t* vmin, uint64_t* rmin, uint8_t* selected, mnrf_stream stream) {
+  using namespace mnrf;
+  set_error("");
+  MNRF_CHECK(num_vertices >= 0 && num_faces >= 0 && num_edges >= 0 && num_edges <= (int64_t)UINT32_MAX,
+             "mnrf_mesh_collapse_select: %d vertices, %lld faces, %lld edges (at most 2^32 - 1)", num_vertices,
+             (long long)num_faces, (long long)num_edges);
+  if (num_edges == 0) return 0;
+  MNRF_CHECK(num_vertices > 0 && num_faces > 0, "mnrf_mesh_collapse_select: edges without vertices or faces");
+  MNRF_CHECK(faces && edges && keys && vmin && rmin && selected, "mnrf_mesh_collapse_select: null pointer");
+  QemArgs a{};
+  a.nv = num_vertices; a.nf = num_faces; a.ne = num_edges;
+  a.faces = const_cast<int32_t*>(faces); a.edges = edges; a.keys = const_cast<uint64_t*>(keys);
+  a.vmin = vmin; a.rmin = rmin; a.selected = selected;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MNRF_CUDA(cudaMemsetAsync(vmin, 0xff, sizeof(uint64_t) * (size_t)num_vertices, s));
+  MNRF_CUDA(cudaMemsetAsync(rmin, 0xff, sizeof(uint64_t) * (size_t)num_vertices, s));
+  qem_vmin_kernel<<<qem_blocks(num_edges), 256, 0, s>>>(a);
+  qem_rmin_kernel<<<qem_blocks(num_faces), 256, 0, s>>>(a);
+  qem_select_kernel<<<qem_blocks(num_edges), 256, 0, s>>>(a);
+  MNRF_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int mnrf_mesh_collapse_apply(int32_t num_vertices, int64_t num_faces, int64_t num_edges,
+                                        const uint8_t* collapse, const int32_t* edges, const int64_t* edge_off,
+                                        const int32_t* edge_face, const int64_t* vf_off, const int32_t* vf_face,
+                                        const float* positions, float* vertices, double* quadrics, float* normals,
+                                        int32_t* faces, uint8_t* face_alive, mnrf_stream stream) {
+  using namespace mnrf;
+  set_error("");
+  MNRF_CHECK(num_vertices >= 0 && num_faces >= 0 && num_edges >= 0 && num_edges <= (int64_t)UINT32_MAX,
+             "mnrf_mesh_collapse_apply: %d vertices, %lld faces, %lld edges (at most 2^32 - 1)", num_vertices,
+             (long long)num_faces, (long long)num_edges);
+  if (num_faces == 0) return 0;
+  MNRF_CHECK(num_vertices > 0, "mnrf_mesh_collapse_apply: faces without vertices");
+  MNRF_CHECK(faces && face_alive && (num_edges == 0 || collapse && edges && edge_off && edge_face && vf_off &&
+                                     vf_face && positions && vertices && quadrics),
+             "mnrf_mesh_collapse_apply: null pointer");
+  const cudaStream_t s = (cudaStream_t)stream;
+  MNRF_CUDA(cudaMemsetAsync(face_alive, 1, (size_t)num_faces, s));
+  if (num_edges == 0) return 0;
+  QemArgs a{};
+  a.nv = num_vertices; a.nf = num_faces; a.ne = num_edges;
+  a.collapse = collapse; a.edges = edges; a.edge_off = edge_off; a.edge_face = edge_face; a.vf_off = vf_off;
+  a.vf_face = vf_face; a.positions = const_cast<float*>(positions); a.vertices = vertices; a.quadrics = quadrics;
+  a.normals = normals; a.faces = faces; a.face_alive = face_alive;
+  qem_apply_kernel<<<qem_blocks(num_edges), 256, 0, s>>>(a);
   MNRF_LAUNCH_CHECK();
   return 0;
 }

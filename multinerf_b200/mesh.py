@@ -14,8 +14,12 @@ signed-distance grid on the same points (`fuse_tsdf`, `ops.tsdf_integrate`, csrc
 crossing where the grid was observed.  No density level is chosen; space a camera saw through is carved away; space
 no camera saw gives no faces (marching cubes skips cells with an unobserved, NaN, corner); and a vertex's colour is
 the mean of the colours rendered for it across the views whose surface lies within the truncation band.
+
+Either method can clean the mesh (`clean_mesh`) and then simplify it to a face budget by quadric edge collapse
+(`simplify_mesh`) before any colour is computed.
 """
 import math
+from typing import NamedTuple
 
 import numpy as np
 import torch
@@ -74,19 +78,21 @@ def density_grid(model, bbox, resolution, slab_planes=None):
 
 
 def extract_mesh(model, bbox, resolution, level, slab_planes=None, colors=False, keep_components=0, min_views=0,
-                 dataset=None, stats=None):
+                 dataset=None, stats=None, target_faces=0):
   """(vertices [V, 3] fp32, faces [F, 3] int32) on the device: the surface density = `level` of `model`'s final
   level inside `bbox` (x0, y0, z0, x1, y1, z1), on a grid of `resolution` points along the longest side.
   Vertices are in world coordinates; face normals point from dense to empty space.  With `colors`, returns
   (vertices, faces, normals [V, 3] fp32, rgb [V, 3] uint8): unit vertex normals from the density grid's gradient,
   and each vertex's colour from `vertex_colors`.  `keep_components`, `min_views` (with the training cameras of
-  `dataset`) and `stats`: clean_mesh, applied before the colours are queried."""
+  `dataset`) and `stats`: clean_mesh, applied before the colours are queried.  target_faces: then simplify_mesh
+  (its counts go to `stats` too), the normals carried along."""
   grid, h = density_grid(model, bbox, resolution, slab_planes)
   out = ops.marching_cubes(grid, level, normals=colors)
   del grid
   lo = torch.tensor([float(v) for v in bbox[:3]], device=out[0].device)
   vertices, faces, *normals = clean_mesh(out[0] * h + lo, *out[1:], **_clean_args(keep_components, min_views,
                                                                                    dataset, stats))
+  vertices, faces, *normals = simplify_mesh(vertices, faces, *normals, target_faces=target_faces, stats=stats)
   if not colors:
     return vertices, faces
   # cubic cells: the grid's normals are the world's
@@ -108,12 +114,12 @@ MESH_METHODS = ('density', 'tsdf')
 def validate_config(bundle):
   """The mesh method of `bundle`'s Config, checked: 'density' or 'tsdf'; the TSDF method needs perspective or fisheye
   views (not NDC) and a truncation of at least one cell, so no cut edge of the fused grid has an unobserved end.
-  The cleaning options must not be negative, and mesh_min_views projects into the views, so it needs them not NDC
-  either."""
+  The cleaning and simplification options must not be negative, and mesh_min_views projects into the views, so it
+  needs them not NDC either."""
   config = bundle.config
   if config.mesh_method not in MESH_METHODS:
     raise ValueError(f'Config.mesh_method = {config.mesh_method!r}: want one of {MESH_METHODS}')
-  for name in ('mesh_keep_components', 'mesh_min_views'):
+  for name in ('mesh_keep_components', 'mesh_min_views', 'mesh_target_faces'):
     if getattr(config, name) < 0:
       raise ValueError(f'Config.{name} = {getattr(config, name)!r}: want 0 (off) or more')
   if config.mesh_min_views > 0 and config.forward_facing:
@@ -179,27 +185,38 @@ def fuse_tsdf(views, cameras, camtype, bbox, resolution, truncation, colors=Fals
   return (tsdf, weight, color_sum, color_weight), h
 
 
-def tsdf_mesh(state, bbox, h, colors=False, clean_args=None):
+def tsdf_mesh(state, bbox, h, colors=False, clean_args=None, target_faces=0, stats=None):
   """Marching cubes on the fused TSDF `state` (fuse_tsdf): the zero crossing of -tsdf (inside > 0, so faces and
   normals point out of the surface), with every point no view observed (weight 0) NaN, so it gives no faces.
   Returns (vertices, faces) in world coordinates, and with `colors` also (normals [V, 3], rgb [V, 3] uint8): each
   vertex's colour is color_sum / color_weight interpolated linearly along its grid edge, rounded as vertex_colors
-  rounds.  clean_args: keyword arguments of clean_mesh, applied before the colours are interpolated."""
+  rounds.  clean_args: keyword arguments of clean_mesh, applied before the colours are interpolated.
+  target_faces: then simplify_mesh (counts to `stats`); a simplified vertex no longer lies on a grid edge, so its
+  colour is interpolated trilinearly at (vertex - lo) / h, clamped to the grid."""
   tsdf, weight, color_sum, color_weight = state
   grid = torch.where(weight > 0, -tsdf, torch.full_like(tsdf, float('nan')))
   out = ops.marching_cubes(grid, 0.0, normals=colors)
   del grid
   lo = torch.tensor([float(v) for v in bbox[:3]], device=out[0].device)
-  # the grid-unit vertices ride along as a per-vertex array: the colours are interpolated from them
-  vertices, faces, *per = clean_mesh(out[0] * h + lo, out[1], *((out[2], out[0]) if colors else ()),
+  simplify = target_faces > 0
+  # without simplification the grid-unit vertices ride along as a per-vertex array: the colours are interpolated
+  # from them
+  ride = (out[0],) if colors and not simplify else ()
+  vertices, faces, *per = clean_mesh(out[0] * h + lo, out[1], *((out[2],) if colors else ()), *ride,
                                      **(clean_args or {}))
+  if simplify:
+    vertices, faces, *per = simplify_mesh(vertices, faces, *per, target_faces=target_faces, stats=stats)
+  elif stats is not None:
+    simplify_mesh(vertices, faces, target_faces=0, stats=stats)
   if not colors:
     return vertices, faces
-  normals, gv = per
-  # a vertex lies on a grid edge: its two other coordinates are integers, so the trilinear weights reduce to the
-  # linear interpolation between the edge's two ends
+  normals, gv = (per[0], ((vertices - lo) / h).clamp_min(0)) if simplify else per
+  # unsimplified, a vertex lies on a grid edge: its two other coordinates are integers, so the trilinear weights
+  # reduce to the linear interpolation between the edge's two ends
   nz, ny, nx = tsdf.shape
   dims = torch.tensor([nx, ny, nz], device=gv.device)
+  if simplify:
+    gv = torch.minimum(gv, dims - 1)
   base = torch.minimum(gv.floor().long(), dims - 2).clamp_min(0)
   frac = gv - base
   cs = torch.zeros(len(vertices), 3, device=vertices.device)
@@ -228,15 +245,15 @@ def render_views(model, dataset):
 
 
 def extract_mesh_tsdf(model, dataset, bbox, resolution, truncation=3.0, colors=False, batch=8, keep_components=0,
-                      min_views=0, stats=None):
+                      min_views=0, stats=None, target_faces=0):
   """Config.mesh_method = 'tsdf': render every camera of `dataset` (render_views), fuse the renders (fuse_tsdf, a
   band of `truncation` cells) and mesh the result (tsdf_mesh).  Returns what extract_mesh returns.
   `keep_components`, `min_views` (against the cameras of `dataset`) and `stats`: clean_mesh, applied before the
-  colours are interpolated."""
+  colours are interpolated; `target_faces`: then simplify_mesh."""
   state, h = fuse_tsdf(render_views(model, dataset), dataset.cameras, dataset.camtype, bbox, resolution, truncation,
                        colors=colors, batch=batch, device=model.device)
-  return tsdf_mesh(state, bbox, h, colors=colors,
-                   clean_args=_clean_args(keep_components, min_views, dataset, stats))
+  return tsdf_mesh(state, bbox, h, colors=colors, clean_args=_clean_args(keep_components, min_views, dataset, stats),
+                   target_faces=target_faces, stats=stats)
 
 
 def clean_mesh(vertices, faces, *per_vertex, keep_components=0, min_views=0, cameras=None, camtype=None,
@@ -286,13 +303,137 @@ def clean_mesh(vertices, faces, *per_vertex, keep_components=0, min_views=0, cam
     if stats is not None:
       stats['components_removed'] = max(0, len(ids) - keep_components)
   kept = faces[keep_face]
-  used = torch.zeros(V, device=faces.device, dtype=torch.bool)
-  used[kept.view(-1).long()] = True
-  new_index = (torch.cumsum(used, 0, dtype=torch.int32) - 1)
-  out = (vertices[used], new_index[kept.long()], *(t[used] for t in per_vertex))
+  out = _drop_unused(vertices, kept, *per_vertex)
   if stats is not None:
     stats.update(vertices_removed=V - out[0].shape[0], faces_removed=faces.shape[0] - kept.shape[0])
   return out
+
+
+def _drop_unused(vertices, faces, *per_vertex):
+  """(vertices, faces, *per_vertex) without the vertices no face uses: the rest keep their order, face indices are
+  renumbered and each per-vertex array follows its vertices."""
+  used = torch.zeros(vertices.shape[0], device=faces.device, dtype=torch.bool)
+  used[faces.view(-1).long()] = True
+  new_index = (torch.cumsum(used, 0, dtype=torch.int32) - 1)
+  return (vertices[used], new_index[faces.long()], *(t[used] for t in per_vertex))
+
+
+class Topology(NamedTuple):
+  """The adjacency of a triangle mesh that one round of simplify_mesh reads (csrc/mesh.cu, include/mnrf.h)."""
+  edges: torch.Tensor       # [E, 2] int32: unique undirected edges (a, b), a < b, sorted by (a, b)
+  edge_off: torch.Tensor    # [E + 1] int64: faces of edge e at edge_face[edge_off[e]:edge_off[e + 1]]
+  edge_face: torch.Tensor   # [3 F] int32, ascending within an edge
+  vf_off: torch.Tensor      # [V + 1] int64: faces at vertex v at vf_face[vf_off[v]:vf_off[v + 1]]
+  vf_face: torch.Tensor     # [3 F] int32, ascending within a vertex
+
+
+def mesh_topology(faces, num_vertices):
+  """Topology of faces [F, 3] int32 on `num_vertices` vertices: stable torch sorts of the corners' edge keys
+  min * V + max and of their vertices, so faces come out in face order within an edge and within a vertex."""
+  # temporaries are freed as soon as they are used: at 155 M faces each int64 corner array takes 3.7 GB
+  corner = faces.view(-1)
+  other = faces[:, [1, 2, 0]].reshape(-1)                 # corner k's edge runs to corner k + 1
+  key = torch.minimum(corner, other).long() * num_vertices + torch.maximum(corner, other)
+  del other
+  skey, perm = torch.sort(key, stable=True)
+  del key
+  edge_face = (perm // 3).int()
+  del perm
+  uniq, counts = torch.unique_consecutive(skey, return_counts=True)
+  del skey
+  zero = torch.zeros(1, device=faces.device, dtype=torch.int64)
+  edges = torch.stack([uniq // num_vertices, uniq % num_vertices], 1).int()
+  del uniq
+  edge_off = torch.cat([zero, torch.cumsum(counts, 0)])
+  del counts
+  vf_face = (torch.sort(corner, stable=True).indices // 3).int()
+  vf_off = torch.cat([zero, torch.cumsum(torch.bincount(corner, minlength=num_vertices), 0)])
+  return Topology(edges, edge_off, edge_face, vf_off, vf_face)
+
+
+def boundary_edges(topo, num_vertices):
+  """(edges [B, 2] int32, face [B] int32, vb_off [V + 1] int64, vb_edge [2 B] int32): the edges of `topo` in exactly
+  one face, in edge order, with their faces, and the boundary edges at each vertex in ascending order."""
+  counts = topo.edge_off[1:] - topo.edge_off[:-1]
+  idx = torch.nonzero(counts == 1).view(-1)
+  edges = topo.edges[idx].contiguous()
+  face = topo.edge_face[topo.edge_off[idx]].contiguous()
+  B = idx.shape[0]
+  ends = edges.t().reshape(-1).long()
+  own = torch.arange(B, device=idx.device).repeat(2)
+  order = torch.sort(ends * max(B, 1) + own).indices
+  zero = torch.zeros(1, device=idx.device, dtype=torch.int64)
+  vb_off = torch.cat([zero, torch.cumsum(torch.bincount(ends, minlength=num_vertices), 0)])
+  return edges, face, vb_off, own[order].int()
+
+
+def simplify_mesh(vertices, faces, normals=None, *, target_faces, stats=None):
+  """Simplifies a mesh on the device to about `target_faces` faces by parallel greedy quadric edge collapse
+  (Garland and Heckbert 1997; csrc/mesh.cu).  vertices [V, 3] fp32, faces [F, 3] int32, normals [V, 3] fp32 or None
+  (carried along and blended).  Returns (vertices, faces) or, with normals, (vertices, faces, normals); vertices
+  and faces that survive keep their relative order, faces are renumbered and unused vertices dropped.
+
+  Quadrics are built once (mnrf_mesh_quadrics).  Each round rebuilds the topology (mesh_topology), prices every
+  edge and checks that it may be collapsed (mnrf_mesh_edge_cost), selects the edges whose key is the least within
+  two faces of both ends (mnrf_mesh_collapse_select), keeps the longest prefix in key order that removes no more than
+  F - target_faces faces, collapses them (mnrf_mesh_collapse_apply) and compacts the faces.  It stops at
+  target_faces or fewer, or after a round with no collapse (a stall: no edge may be collapsed, or the next one would
+  overshoot by a face).  The result is bit-deterministic.
+
+  target_faces 0 (off), or a mesh with at most target_faces faces: the inputs come back untouched and nothing is
+  launched.  stats: a dict, given faces_before, faces_after, rounds (rounds that collapsed) and target_reached
+  (faces_after <= target_faces + 1; True when off)."""
+  if target_faces < 0:
+    raise ValueError(f'simplify_mesh: target_faces = {target_faces}: want 0 (off) or more')
+  out = (vertices, faces) + (() if normals is None else (normals,))
+  F = faces.shape[0]
+  if stats is not None:
+    stats.update(faces_before=F, faces_after=F, rounds=0, target_reached=True)
+  if not target_faces or F <= target_faces:
+    return out
+  V = vertices.shape[0]
+  if not 0 < V < 2 ** 31 or F >= 2 ** 31:
+    raise ValueError(f'simplify_mesh: {V} vertices, {F} faces')
+  assert faces.dtype == torch.int32 and faces.dim() == 2 and faces.shape[1] == 3
+  f = faces.contiguous().clone()
+  fl = f.long()
+  bad = ((fl < 0) | (fl >= V)).any() | (fl[:, 0] == fl[:, 1]).any() | (fl[:, 1] == fl[:, 2]).any() | \
+      (fl[:, 2] == fl[:, 0]).any()
+  if bool(bad):
+    raise ValueError(f'simplify_mesh: a face index lies outside [0, {V}) or a face repeats a vertex')
+  del fl
+  v = vertices.contiguous().clone()
+  n = None if normals is None else normals.contiguous().clone()
+  topo = mesh_topology(f, V)
+  if topo.edges.shape[0] >= 2 ** 32:
+    raise ValueError(f'simplify_mesh: {topo.edges.shape[0]} edges do not fit 32-bit edge indices')
+  q = ops.mesh_quadrics(v, f, topo.vf_off, topo.vf_face, *boundary_edges(topo, V))
+  rounds = 0
+  while True:
+    keys, pos = ops.mesh_edge_cost(v, f, q, *topo)
+    sel = torch.nonzero(ops.mesh_collapse_select(f, topo.edges, keys, V)).view(-1)
+    if sel.shape[0] == 0:
+      break
+    sel = sel[torch.sort(keys[sel]).indices]                         # key order (keys are unique)
+    removed = torch.cumsum(topo.edge_off[sel + 1] - topo.edge_off[sel], 0)
+    keep = removed <= F - target_faces                               # a prefix: removed grows
+    applied, gone = (int(x) for x in torch.stack([keep.sum(), torch.where(keep, removed, 0).max()]).cpu())
+    if applied == 0:
+      break
+    collapse = torch.zeros(topo.edges.shape[0], device=f.device, dtype=torch.uint8)
+    collapse[sel] = keep.to(torch.uint8)
+    alive = ops.mesh_collapse_apply(collapse, topo.edges, topo.edge_off, topo.edge_face, topo.vf_off, topo.vf_face,
+                                    pos, v, q, n, f)
+    f = f[alive.bool()]
+    F -= gone
+    rounds += 1
+    if F <= target_faces:
+      break
+    del keys, pos, sel, removed, keep, collapse, alive, topo
+    topo = mesh_topology(f, V)
+  if stats is not None:
+    stats.update(faces_after=F, rounds=rounds, target_reached=F <= target_faces + 1)
+  return _drop_unused(v, f, *(() if n is None else (n,)))
 
 
 def _clean_args(keep_components, min_views, dataset, stats):

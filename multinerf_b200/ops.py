@@ -224,6 +224,80 @@ def mesh_components(faces, num_vertices):
   return labels
 
 
+def _i32(t):
+  assert t.dtype == torch.int32 and t.is_contiguous(), 'need contiguous int32'
+  return t
+
+
+def _i64(t):
+  assert t.dtype == torch.int64 and t.is_contiguous(), 'need contiguous int64'
+  return t
+
+
+def mesh_quadrics(vertices, faces, vf_off, vf_face, boundary_edges, boundary_face, vb_off, vb_edge):
+  """Per-vertex error quadrics [V, 10] fp64 of a mesh (mnrf_mesh_quadrics, csrc/mesh.cu): area-weighted face planes,
+  then boundary-edge planes.  The topology tensors as mesh.mesh_topology and mesh.boundary_edges build them."""
+  lib = L.load()
+  V, F, B = vertices.shape[0], faces.shape[0], boundary_edges.shape[0]
+  q = torch.empty(V, 10, device=vertices.device, dtype=torch.float64)
+  if V:
+    _count()
+    L.check(lib.mnrf_mesh_quadrics(V, F, L.ptr(_f32(vertices)), L.ptr(_i32(faces)), L.ptr(_i64(vf_off)),
+                                   L.ptr(_i32(vf_face)), B, L.ptr(_i32(boundary_edges)), L.ptr(_i32(boundary_face)),
+                                   L.ptr(_i64(vb_off)), L.ptr(_i32(vb_edge)), L.ptr(q), L.stream_ptr()))
+  return q
+
+
+def mesh_edge_cost(vertices, faces, quadrics, edges, edge_off, edge_face, vf_off, vf_face):
+  """Per edge, the collapse position [E, 3] fp32 and key [E] (uint64 bits in an int64 tensor; -1 where the edge may
+  not be collapsed) (mnrf_mesh_edge_cost, csrc/mesh.cu) -> (keys, positions)."""
+  lib = L.load()
+  V, F, E = vertices.shape[0], faces.shape[0], edges.shape[0]
+  dev = vertices.device
+  keys = torch.empty(E, device=dev, dtype=torch.int64)
+  pos = torch.empty(E, 3, device=dev)
+  if E:
+    flags = torch.empty(V, device=dev, dtype=torch.int32)
+    _count(2)
+    L.check(lib.mnrf_mesh_edge_cost(V, F, E, L.ptr(_f32(vertices)), L.ptr(_i32(faces)), L.ptr(quadrics),
+                                    L.ptr(_i32(edges)), L.ptr(_i64(edge_off)), L.ptr(_i32(edge_face)),
+                                    L.ptr(_i64(vf_off)), L.ptr(_i32(vf_face)), L.ptr(flags), L.ptr(keys), L.ptr(pos),
+                                    L.stream_ptr()))
+  return keys, pos
+
+
+def mesh_collapse_select(faces, edges, keys, num_vertices):
+  """The edges a round collapses, selected [E] uint8 (mnrf_mesh_collapse_select, csrc/mesh.cu): an edge whose key is
+  the least within two faces of each of its ends."""
+  lib = L.load()
+  E = edges.shape[0]
+  dev = edges.device
+  sel = torch.empty(E, device=dev, dtype=torch.uint8)
+  if E:
+    vmin = torch.empty(num_vertices, device=dev, dtype=torch.int64)
+    rmin = torch.empty_like(vmin)
+    _count(3)
+    L.check(lib.mnrf_mesh_collapse_select(num_vertices, faces.shape[0], E, L.ptr(_i32(faces)), L.ptr(_i32(edges)),
+                                          L.ptr(_i64(keys)), L.ptr(vmin), L.ptr(rmin), L.ptr(sel), L.stream_ptr()))
+  return sel
+
+
+def mesh_collapse_apply(collapse, edges, edge_off, edge_face, vf_off, vf_face, positions, vertices, quadrics,
+                        normals, faces):
+  """Collapses the edges with collapse [E] uint8 set, updating vertices, quadrics, normals (or None) and faces in
+  place (mnrf_mesh_collapse_apply, csrc/mesh.cu) -> face_alive [F] uint8."""
+  lib = L.load()
+  V, F, E = vertices.shape[0], faces.shape[0], edges.shape[0]
+  alive = torch.empty(F, device=faces.device, dtype=torch.uint8)
+  if F:
+    _count()
+    L.check(lib.mnrf_mesh_collapse_apply(V, F, E, L.ptr(collapse), L.ptr(_i32(edges)), L.ptr(_i64(edge_off)),
+                                         L.ptr(_i32(edge_face)), L.ptr(_i64(vf_off)), L.ptr(_i32(vf_face)),
+                                         L.ptr(_f32(positions)), L.ptr(_f32(vertices)), L.ptr(quadrics),
+                                         L.ptr(_f32(normals)), L.ptr(_i32(faces)), L.ptr(alive), L.stream_ptr()))
+  return alive
+
+
 def points_view_count(points, camtype, distortion_params, worldtocams, camtopixs, height, width):
   """For each point [N, 3] fp32 on the device, the number of views whose height x width image it lands on
   (mnrf_points_view_count, csrc/mesh.cu: the pixel rule of tsdf_integrate) -> counts [N] int32.  camtype 0

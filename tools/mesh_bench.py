@@ -14,9 +14,16 @@
   components: ops.mesh_components and mesh.clean_mesh(keep_components=1) (CUDA events over --reps calls) on the
           512^3 `mc` mesh and on the 512^3 random-init 360.gin extraction, with the bytes the union-find moves by
           count; mesh.extract_mesh at --extract_res^3 with mesh_keep_components 0 and 1, alternated --reps times;
+  simplify: mesh.simplify_mesh (CUDA events around whole calls, after one warm-up call) on the 512^3 `mc` mesh to
+          10 % and 1 % of its faces and on the 512^3 random-init 360.gin extraction after keep_components = 1 to
+          --simplify_faces faces: rounds, peak device memory, the PLY size by count before and after, and from one
+          more call with CUDA events around each step, the time in the torch topology rebuilds against the kernels;
+          mesh.extract_mesh at --extract_res^3 without and with target_faces = --simplify_faces, alternated --reps
+          times (not part of `all`);
   device: the card's name and power limit, read in the same run.
 
-  python tools/mesh_bench.py [--rows 8388608] [--extract_res 512] [--sections all|components] [--out result.json]
+  python tools/mesh_bench.py [--rows 8388608] [--extract_res 512] [--sections all|components|simplify]
+                             [--out result.json]
 """
 import argparse
 import json
@@ -176,17 +183,104 @@ def bench_components_section(model, bbox, level, args):
   return out
 
 
+def ply_bytes(v, f):
+  """PLY size by count without normals or colours: 12 B a vertex, 13 B a face (plus a header of under 300 B)."""
+  return 12 * int(v.shape[0]) + 13 * int(f.shape[0])
+
+
+def simplify_breakdown(v, f, target):
+  """One simplify_mesh call with CUDA events around each topology rebuild (mesh_topology, boundary_edges) and each
+  kernel call -> ms per step name, summed over rounds."""
+  names = {'topology': (mesh, 'mesh_topology'), 'boundary': (mesh, 'boundary_edges'),
+           'quadrics': (ops, 'mesh_quadrics'), 'edge_cost': (ops, 'mesh_edge_cost'),
+           'select': (ops, 'mesh_collapse_select'), 'apply': (ops, 'mesh_collapse_apply')}
+  spans = {k: [] for k in names}
+  saved = {k: getattr(m, a) for k, (m, a) in names.items()}
+
+  def wrap(key, fn):
+    def run(*args, **kw):
+      ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+      ev[0].record()
+      out = fn(*args, **kw)
+      ev[1].record()
+      spans[key].append(ev)
+      return out
+    return run
+  for k, (m, a) in names.items():
+    setattr(m, a, wrap(k, saved[k]))
+  try:
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    mesh.simplify_mesh(v, f, target_faces=target)
+    torch.cuda.synchronize()
+    wall = time.perf_counter() - t0
+  finally:
+    for k, (m, a) in names.items():
+      setattr(m, a, saved[k])
+  ms = {k: round(sum(e[0].elapsed_time(e[1]) for e in evs), 2) for k, evs in spans.items()}
+  ms['wall_ms_instrumented'] = round(wall * 1e3, 1)
+  ms['other_ms'] = round(wall * 1e3 - sum(v for k, v in ms.items() if k != 'wall_ms_instrumented'), 1)
+  return ms
+
+
+def bench_simplify(name, v, f, target, reps):
+  torch.cuda.synchronize()
+  torch.cuda.reset_peak_memory_stats()
+  base = torch.cuda.memory_allocated()
+  stats = {}
+  sv, sf = mesh.simplify_mesh(v, f, target_faces=target, stats=stats)     # warm-up, and the counts
+  torch.cuda.synchronize()
+  peak = torch.cuda.max_memory_allocated()
+  out = {'mesh': name, 'vertices': int(v.shape[0]), 'faces': int(f.shape[0]), 'target_faces': target, **stats,
+         'vertices_after': int(sv.shape[0]), 'ply_bytes_before': ply_bytes(v, f), 'ply_bytes_after': ply_bytes(sv, sf),
+         'peak_alloc_gb': round(peak / 1e9, 2), 'peak_over_input_gb': round((peak - base) / 1e9, 2)}
+  del sv, sf
+  torch.cuda.empty_cache()
+  out['ms'] = round(events(lambda: mesh.simplify_mesh(v, f, target_faces=target), reps), 1)
+  torch.cuda.empty_cache()
+  out['breakdown_ms'] = simplify_breakdown(v, f, target)
+  torch.cuda.empty_cache()
+  return out
+
+
+def bench_simplify_section(model, bbox, level, args):
+  out = {'meshes': [], 'extract': {'plain_s': [], 'simplified_s': []}}
+  v, f = ops.marching_cubes(sphere_noise(512), 0.0)
+  torch.cuda.empty_cache()
+  for frac in (0.1, 0.01):
+    out['meshes'].append(bench_simplify('mc 512^3 sphere + noise', v, f, int(f.shape[0] * frac), args.reps))
+  del v, f
+  torch.cuda.empty_cache()
+  v, f = mesh.extract_mesh(model, bbox, args.extract_res, level, keep_components=1)
+  torch.cuda.empty_cache()
+  out['meshes'].append(bench_simplify(f'360.gin random init, {args.extract_res}^3, keep_components 1', v, f,
+                                      args.simplify_faces, 1))
+  del v, f
+  torch.cuda.empty_cache()
+  mesh.extract_mesh(model, bbox, args.extract_res, level, target_faces=args.simplify_faces)      # warm-up
+  torch.cuda.empty_cache()
+  for _ in range(args.reps):
+    for key, target in (('plain_s', 0), ('simplified_s', args.simplify_faces)):
+      t, o = timed(lambda: mesh.extract_mesh(model, bbox, args.extract_res, level, target_faces=target), 1)
+      out['extract'][key].append(round(t, 3))
+      out['extract'][f'{key[:-2]}_faces'] = int(o[1].shape[0])
+      del o
+      torch.cuda.empty_cache()
+  return out
+
+
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--rows', type=int, default=1 << 23)
   ap.add_argument('--reps', type=int, default=3)
   ap.add_argument('--extract_res', type=int, default=512)
-  ap.add_argument('--sections', default='all', choices=('all', 'components'))
+  ap.add_argument('--sections', default='all', choices=('all', 'components', 'simplify'))
+  ap.add_argument('--simplify_faces', type=int, default=1_000_000)
   ap.add_argument('--out', default=None)
   args = ap.parse_args()
   lib.require_device()
   res = {'device': device_info(), 'query': {}, 'mc': [], 'extract': None}
-  if args.sections == 'components':
+  if args.sections in ('components', 'simplify'):
     b = configs.bundle_360()
     model = models.Model(b)
     model.init(seed=0)
@@ -195,8 +289,9 @@ def main():
     level = float(grid.median())
     del grid
     torch.cuda.empty_cache()
-    res = {'device': res['device'], 'level': level,
-           'components': bench_components_section(model, bbox, level, args), 'device_after': device_info()}
+    section = bench_components_section if args.sections == 'components' else bench_simplify_section
+    res = {'device': res['device'], 'level': level, args.sections: section(model, bbox, level, args),
+           'device_after': device_info()}
     emit(res, args.out)
     return
   for name, make in (('360', configs.bundle_360), ('blender_256', configs.bundle_blender_256)):
