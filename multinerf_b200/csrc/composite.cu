@@ -497,6 +497,19 @@ point_rgb_kernel(mnrf_composite_desc d, int64_t M, const float* __restrict__ raw
   }
 }
 
+// The descriptor fields both entry points branch on: anything else would silently take some other branch (an unknown
+// rgb_mode composites as mode 0) or read rows that overlap (ld_rgb 1 or 2).  ld 0 means the contiguous default.
+static int check_desc(const char* fn, const mnrf_composite_desc& d) {
+  MNRF_CHECK(d.num_rays >= 0, "%s: negative num_rays %d", fn, d.num_rays);
+  MNRF_CHECK(d.raydist_fn >= MNRF_RAYDIST_NONE && d.raydist_fn <= MNRF_RAYDIST_PIECEWISE, "%s: unknown raydist_fn %d",
+             fn, d.raydist_fn);
+  MNRF_CHECK(d.rgb_act == MNRF_RGB_SIGMOID || d.rgb_act == MNRF_RGB_SAFE_EXP, "%s: unknown rgb_act %d", fn, d.rgb_act);
+  MNRF_CHECK(d.rgb_mode == 0 || d.rgb_mode == 1, "%s: unknown rgb_mode %d", fn, d.rgb_mode);
+  MNRF_CHECK(d.ld_density >= 0, "%s: negative ld_density %d", fn, d.ld_density);
+  MNRF_CHECK(d.ld_rgb == 0 || d.ld_rgb >= 3, "%s: ld_rgb %d overlaps the rgb rows (0 or >= 3)", fn, d.ld_rgb);
+  return 0;
+}
+
 }  // namespace mnrf
 
 #define MNRF_DISPATCH_CH(S, CALL)                         \
@@ -515,13 +528,14 @@ extern "C" int mnrf_composite_fwd(const mnrf_composite_desc* d, const float* raw
                                   float* weights, float* rgb_out, float* density_out,
                                   float* rgb_samples, float* acc, float* dist, mnrf_stream stream) {
   using namespace mnrf;
-  if (d && d->num_rays == 0) return 0;
-  MNRF_CHECK(d && raw_density && sdist && directions && near && far && weights && rgb_out,
+  MNRF_CHECK(d, "mnrf_composite_fwd: null descriptor");
+  if (check_desc("mnrf_composite_fwd", *d)) return 1;
+  if (d->num_rays == 0) return 0;
+  MNRF_CHECK(raw_density && sdist && directions && near && far && weights && rgb_out,
              "mnrf_composite_fwd: null pointer");
-  MNRF_CHECK(d->num_samples >= 1 && d->num_samples <= 256, "mnrf_composite_fwd: num_samples %d > 256",
+  MNRF_CHECK(d->num_samples >= 1 && d->num_samples <= 256, "mnrf_composite_fwd: num_samples %d not in [1, 256]",
              d->num_samples);
   MNRF_CHECK(d->rgb_mode == 0 || (raw_rgb && raw_diffuse), "mnrf_composite_fwd: rgb_mode 1 needs raw_diffuse");
-  if (d->num_rays == 0) return 0;
   const int nw = 4;
   size_t smem = (size_t)nw * (2 * d->num_samples + 4) * sizeof(float);
   int blocks = ceil_div(d->num_rays, nw);
@@ -563,20 +577,23 @@ extern "C" int mnrf_composite_bwd(const mnrf_loss_desc* d, const float* raw_dens
                                   float* d_raw_diffuse, float* d_raw_tint, float* stats, int32_t batch_rays,
                                   mnrf_stream stream) {
   using namespace mnrf;
-  MNRF_CHECK(d->c.rgb_mode == 0 || (raw_rgb && raw_diffuse && d_raw_diffuse && (!raw_tint || d_raw_tint)),
-             "mnrf_composite_bwd: rgb_mode 1 needs raw_diffuse / d_raw_diffuse (and d_raw_tint with raw_tint)");
-  if (d && d->c.num_rays == 0) return 0;
-  MNRF_CHECK(d && raw_density && sdist && directions && near && far && target_rgb && lossmult &&
+  MNRF_CHECK(d, "mnrf_composite_bwd: null descriptor");
+  if (check_desc("mnrf_composite_bwd", d->c)) return 1;
+  if (d->c.num_rays == 0) return 0;
+  MNRF_CHECK(raw_density && sdist && directions && near && far && target_rgb && lossmult &&
              inv_denom && d_raw_density && stats, "mnrf_composite_bwd: null pointer");
-  MNRF_CHECK(d->c.num_samples >= 1 && d->c.num_samples <= 256, "mnrf_composite_bwd: num_samples %d > 256",
+  MNRF_CHECK(d->c.rgb_mode == 0 || (raw_rgb && d_raw_rgb && raw_diffuse && d_raw_diffuse && (!raw_tint || d_raw_tint)),
+             "mnrf_composite_bwd: rgb_mode 1 needs raw_rgb / d_raw_rgb and raw_diffuse / d_raw_diffuse (and d_raw_tint "
+             "with raw_tint)");
+  MNRF_CHECK(d->c.num_samples >= 1 && d->c.num_samples <= 256, "mnrf_composite_bwd: num_samples %d not in [1, 256]",
              d->c.num_samples);
-  MNRF_CHECK(d->interlevel_mult == 0.f || (sdist_fine && weights_fine),
-             "mnrf_composite_bwd: interlevel loss needs the final level's sdist/weights");
+  MNRF_CHECK(d->interlevel_mult == 0.f || (sdist_fine && weights_fine && d->num_samples_fine >= 1),
+             "mnrf_composite_bwd: interlevel loss needs the final level's sdist/weights (num_samples_fine %d)",
+             d->num_samples_fine);
   MNRF_CHECK(d->lossmult_channels == 1 || d->lossmult_channels == 3, "lossmult_channels must be 1 or 3");
   MNRF_CHECK(d->loss_type >= 0 && d->loss_type <= 2, "unknown data_loss_type");
   MNRF_CHECK(batch_rays >= d->c.num_rays, "mnrf_composite_bwd: batch_rays %d < num_rays %d", batch_rays,
              d->c.num_rays);
-  if (d->c.num_rays == 0) return 0;
   const int nw = 4;
   size_t smem = (size_t)nw * (4 * d->c.num_samples + 6) * sizeof(float);
   int blocks = ceil_div(d->c.num_rays, nw);
