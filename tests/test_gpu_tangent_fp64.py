@@ -21,6 +21,7 @@ import torch
 
 import gemm_ref as GR
 import tangent_ref as TR
+from launch_recorder import Recorder
 
 pytestmark = pytest.mark.gpu
 
@@ -239,40 +240,6 @@ def test_refusals_leave_outputs_untouched(ops):
 
 # ------------------------------------------------------------------ the model's launches
 
-class _Recorder:
-  """Wraps ops.gemm, ops.outer_mask and ops.act_tangent_bwd: snapshots of every tangent launch's inputs (before it,
-  since du is T) and outputs (right after it), the trunk's forward z / mask bits as its FWD GEMMs stored them, and
-  the output of every W-wide DGRAD."""
-
-  def __init__(self, ops_, W):
-    from multinerf_b200 import lib as L
-    self.L, self.W = L, W
-    self.events = []                     # ('fwd', ptr, snapshot) | ('dgrad', out ptr) | ('om', ..) | ('act', ..)
-    self._gemm, self._om, self._act = ops_.gemm, ops_.outer_mask, ops_.act_tangent_bwd
-
-  def gemm(self, mode, a, b, out, **kw):
-    r = self._gemm(mode, a, b, out, **kw)
-    L = self.L
-    keep = kw.get('z') if kw.get('z') is not None else kw.get('maskbits')
-    if mode == L.GEMM_FWD and kw['n'] == self.W and keep is not None:       # a trunk layer's forward
-      self.events.append(('fwd', keep.data_ptr(), keep.clone()))
-    elif mode == L.GEMM_DGRAD and kw['m'] == out.shape[0] and kw['n'] == self.W:
-      self.events.append(('dgrad', out.data_ptr()))
-    return r
-
-  def outer_mask(self, rowv, colv, maskbits, out, *, rows, n, mask_mod=0):
-    snap = (rowv.clone(), colv.clone(), None if maskbits is None else maskbits.clone())
-    self._om(rowv, colv, maskbits, out, rows=rows, n=n, mask_mod=mask_mod)
-    self.events.append(('om', dict(inputs=snap, bits_ptr=None if maskbits is None else maskbits.data_ptr(), rows=rows,
-                                   n=n, mask_mod=mask_mod, out=out[:rows, :n].clone())))
-
-  def act_tangent_bwd(self, act, z, t_adj, u, du, g, *, accumulate=False):
-    snap = (z.clone(), t_adj.clone(), u.clone(), g.clone() if accumulate else None)
-    self._act(act, z, t_adj, u, du, g, accumulate=accumulate)
-    self.events.append(('act', dict(act=act, inputs=snap, z_ptr=z.data_ptr(), g_ptr=g.data_ptr(), acc=accumulate,
-                                    inplace=du.data_ptr() == t_adj.data_ptr(), du=du.clone(), g=g.clone())))
-
-
 @pytest.mark.parametrize('name', ['softplus', 'silu', 'relu'])
 def test_refnerf_train_step_tangent_launches(ops, monkeypatch, name):
   """One eager train step of mini_refnerf.  Every outer_mask and act_tangent_bwd launch is checked against the fp64
@@ -281,7 +248,7 @@ def test_refnerf_train_step_tangent_launches(ops, monkeypatch, name):
   in place, the first (layer net_depth - 1) accumulating into the buffer the head's DGRAD just wrote and the others
   not, layer i reading the z its forward GEMM stored, bit for bit; none under ReLU."""
   from model_parity import level_jitter, mini_refnerf, synth_rays
-  from multinerf_b200 import models, train_utils, utils
+  from multinerf_b200 import lib as L, models, train_utils, utils
   bundle = mini_refnerf()
   bundle.nerf_mlp.net_activation = bundle.prop_mlp.net_activation = name
   bundle.config.grad_max_norm = bundle.config.grad_max_val = 0.0
@@ -291,48 +258,55 @@ def test_refnerf_train_step_tangent_launches(ops, monkeypatch, name):
   target = rng.uniform(0, 1, (B, 3)).astype(np.float32)
   model, variables = models.construct_model(82, rays, bundle)
   rand = level_jitter(rng, bundle, B)
-  rec = _Recorder(ops, W)
-  for fn in ('gemm', 'outer_mask', 'act_tangent_bwd'):
-    monkeypatch.setattr(ops, fn, getattr(rec, fn))
+  rec = Recorder(ops, ('gemm', 'outer_mask', 'act_tangent_bwd'), monkeypatch)
   step_fn = train_utils.create_train_step(model, bundle.config)
   step_fn(rand, train_utils.TrainState(variables), utils.Batch(rays=rays, rgb=target), None, 0.5)
   torch.cuda.synchronize()
   monkeypatch.undo()
 
-  ev = rec.events
+  ev = rec.calls
+
+  def kept(c):          # what a trunk layer's FWD GEMM stores for the backward: z or the mask bits
+    return next((k for k in ('z', 'maskbits') if c.args.get(k) is not None), None)
+  fwd_calls = [c for c in ev if c.fn == 'gemm' and c.args['mode'] == L.GEMM_FWD and c.args['n'] == W and kept(c)]
   # the trunk's forward layers in order, level after level: layer = index mod net_depth
-  fwd = {e[1]: (k % depth, e[2]) for k, e in enumerate(e for e in ev if e[0] == 'fwd')}
-  oms = [i for i, e in enumerate(ev) if e[0] == 'om']
+  fwd = {c.args[kept(c)].data_ptr(): (k % depth, c.after[kept(c)]) for k, c in enumerate(fwd_calls)}
+  oms = [i for i, c in enumerate(ev) if c.fn == 'outer_mask']
   assert len(oms) == bundle.model.num_levels, f'{len(oms)} outer_mask launches for {bundle.model.num_levels} levels'
   assert len(fwd) == depth * bundle.model.num_levels, 'trunk forward layers that keep z / mask bits'
   worst = {'du': 0.0, 'g': 0.0}
   for j, i0 in enumerate(oms):
-    om = ev[i0][1]
-    rowv, colv, bits = om['inputs']
-    M = om['rows'] // 3
-    assert om['n'] == W and om['mask_mod'] == M and rowv.numel() == 3 * M
-    want = TR.outer_mask_ref(rowv, colv, bits, rows=om['rows'], n=W, mask_mod=M)
-    assert torch.equal(om['out'].view(torch.int16), want.view(torch.int16)), f'level {j}: outer_mask'
+    c = ev[i0]
+    rowv, colv, bits = c.before['rowv'], c.before['colv'], c.before.get('maskbits')
+    rows, n, mod = c.args['rows'], c.args['n'], c.args.get('mask_mod', 0)
+    M = rows // 3
+    assert n == W and mod == M and rowv.numel() == 3 * M
+    want = TR.outer_mask_ref(rowv, colv, bits, rows=rows, n=W, mask_mod=M)
+    assert torch.equal(c.after['out'][:rows, :n].view(torch.int16), want.view(torch.int16)), f'level {j}: outer_mask'
     # the buffer the head's DGRAD wrote last before this level's tangent backward
-    head = [e[1] for e in ev[:i0] if e[0] == 'dgrad'][-1]
-    acts = [e[1] for e in ev[i0 + 1:oms[j + 1] if j + 1 < len(oms) else len(ev)] if e[0] == 'act']
+    head = [e.args['out'].data_ptr() for e in ev[:i0] if e.fn == 'gemm' and e.args['mode'] == L.GEMM_DGRAD and
+            e.args['m'] == e.args['out'].shape[0] and e.args['n'] == W][-1]
+    acts = [e for e in ev[i0 + 1:oms[j + 1] if j + 1 < len(oms) else len(ev)] if e.fn == 'act_tangent_bwd']
     if name == 'relu':
-      assert bits is not None and fwd[om['bits_ptr']][0] == depth - 1, 'outer_mask without the last layer\'s bits'
-      assert torch.equal(bits, fwd[om['bits_ptr']][1]), 'mask bits changed since the forward'
+      assert bits is not None and fwd[c.args['maskbits'].data_ptr()][0] == depth - 1, \
+          'outer_mask without the last layer\'s bits'
+      assert torch.equal(bits, fwd[c.args['maskbits'].data_ptr()][1]), 'mask bits changed since the forward'
       assert not acts, 'second-order launches under ReLU'
       continue
     assert bits is None, 'a smooth activation seeds the tangent chain unmasked'
     assert len(acts) == depth, f'level {j}: {len(acts)} second-order launches for {depth} trunk layers'
-    assert [a['acc'] for a in acts] == [True] + [False] * (depth - 1)
-    assert acts[0]['g_ptr'] == head, 'the accumulating launch does not add into the head DGRAD\'s output'
+    assert [a.args.get('accumulate', False) for a in acts] == [True] + [False] * (depth - 1)
+    assert acts[0].args['g'].data_ptr() == head, 'the accumulating launch does not add into the head DGRAD\'s output'
     for k, a in enumerate(acts):
-      layer, zf = fwd[a['z_ptr']]
+      layer, zf = fwd[a.args['z'].data_ptr()]
       assert layer == depth - 1 - k, f'level {j}: launch {k} reads the z of layer {layer}'
-      z, t, u, prev = a['inputs']
+      z, t, u = a.before['z'], a.before['t_adj'], a.before['u']
+      prev = a.before['g'] if a.args.get('accumulate', False) else None
       assert torch.equal(z.view(torch.int16), zf.view(torch.int16)), 'z changed since the forward'
-      assert a['inplace'] and a['act'] == ACTS[name]
-      du, dub, g, gb = TR.act_tangent_ref(a['act'], z, t, u, prev)
-      worst['du'] = max(worst['du'], GR.check(a['du'], du, dub, f'level {j} layer {layer} du'))
-      worst['g'] = max(worst['g'], GR.check(a['g'], g, gb, f'level {j} layer {layer} g'))
-  print(f'\n{name}: {len(oms)} levels, {sum(e[0] == "act" for e in ev)} second-order launches | worst err/bound '
+      assert a.args['du'].data_ptr() == a.args['t_adj'].data_ptr() and a.args['act'] == ACTS[name]
+      du, dub, g, gb = TR.act_tangent_ref(a.args['act'], z, t, u, prev)
+      worst['du'] = max(worst['du'], GR.check(a.after['du'], du, dub, f'level {j} layer {layer} du'))
+      worst['g'] = max(worst['g'], GR.check(a.after['g'], g, gb, f'level {j} layer {layer} g'))
+  n_act = sum(e.fn == 'act_tangent_bwd' for e in ev)
+  print(f'\n{name}: {len(oms)} levels, {n_act} second-order launches | worst err/bound '
         f'du {worst["du"]:.3f} g {worst["g"]:.3f}')
