@@ -10,7 +10,9 @@ training view, fuses the rendered depth into a truncated signed-distance grid (C
 meshes its zero crossing.  Config.mesh_min_views drops what fewer training views see, and
 Config.mesh_keep_components keeps only the largest connected components (mesh.clean_mesh).
 Config.mesh_target_faces then simplifies the mesh to about that many faces by quadric edge collapse
-(mesh.simplify_mesh).  One process on one GPU.
+(mesh.simplify_mesh).  Config.mesh_texture_size = S then bakes the surface colour into an S x S texture atlas
+(mesh.bake_texture) and writes mesh_step_<step>.{obj,mtl,png} beside the PLY, which is written first and unchanged.
+One process on one GPU.
 """
 import dataclasses
 import os
@@ -21,7 +23,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 import torch  # noqa: E402
 
-from multinerf_b200 import checkpoints, configs, datasets, mesh, train_utils  # noqa: E402
+from multinerf_b200 import checkpoints, configs, datasets, mesh, ops, train_utils  # noqa: E402
 from train import parse  # noqa: E402
 
 
@@ -43,35 +45,54 @@ def main(argv=None):
                                     device=model.device)
   clean = dict(keep_components=config.mesh_keep_components, min_views=config.mesh_min_views,
                target_faces=config.mesh_target_faces, stats={})
+  out_dir = os.path.join(config.checkpoint_dir, 'mesh')
+  path = os.path.join(out_dir, f'mesh_step_{step}.ply')
+  size = config.mesh_texture_size
   t0 = time.time()
+  timing = {}
+
+  def save_ply(vertices, faces, normals=None, rgb=None):
+    """The PLY as without a texture: normals and colours only with mesh_vertex_colors."""
+    torch.cuda.synchronize()
+    elapsed = time.time() - t0
+    if config.mesh_keep_components or config.mesh_min_views:
+      s = clean['stats']
+      print(f"cleaning removed {s['vertices_removed']} vertices, {s['faces_removed']} faces and "
+            f"{s['components_removed']} components (mesh_min_views {config.mesh_min_views}, "
+            f"mesh_keep_components {config.mesh_keep_components})", flush=True)
+    if config.mesh_target_faces:
+      s = clean['stats']
+      print(f"simplified {s['faces_before']} -> {s['faces_after']} faces in {s['rounds']} rounds "
+            f"(mesh_target_faces {config.mesh_target_faces})" +
+            ('' if s['target_reached'] else ': stalled before the target, no edge left that may be collapsed'),
+            flush=True)
+    os.makedirs(out_dir, exist_ok=True)
+    mesh.write_ply(path, vertices, faces, *((normals, rgb) if config.mesh_vertex_colors else ()))
+    print(f'{vertices.shape[0]} vertices, {faces.shape[0]} faces in {elapsed:.2f} s '
+          f'(grid {config.mesh_resolution} along the longest side of {bbox}, {what}) -> {path}', flush=True)
+    timing['t'] = time.time()
+
+  texture = dict(texture_size=size, before_texture=save_ply) if size else {}
   if method == 'tsdf':
+    what = f'{dataset.size} views fused, truncation {config.mesh_tsdf_truncation} cells'
     vertices, faces, *extra = mesh.extract_mesh_tsdf(model, dataset, bbox, config.mesh_resolution,
                                                      config.mesh_tsdf_truncation, colors=config.mesh_vertex_colors,
-                                                     **clean)
-    what = f'{dataset.size} views fused, truncation {config.mesh_tsdf_truncation} cells'
+                                                     **clean, **texture)
   else:
-    vertices, faces, *extra = mesh.extract_mesh(model, bbox, config.mesh_resolution, config.mesh_level,
-                                                colors=config.mesh_vertex_colors, dataset=dataset, **clean)
     what = f'level {config.mesh_level}'
+    vertices, faces, *extra = mesh.extract_mesh(model, bbox, config.mesh_resolution, config.mesh_level,
+                                                colors=config.mesh_vertex_colors, dataset=dataset, **clean,
+                                                **texture)
+  if not size:
+    save_ply(vertices, faces, *extra)
+    return path
+  normals, _, uv, tex = extra
   torch.cuda.synchronize()
-  elapsed = time.time() - t0
-  if config.mesh_keep_components or config.mesh_min_views:
-    s = clean['stats']
-    print(f"cleaning removed {s['vertices_removed']} vertices, {s['faces_removed']} faces and "
-          f"{s['components_removed']} components (mesh_min_views {config.mesh_min_views}, "
-          f"mesh_keep_components {config.mesh_keep_components})", flush=True)
-  if config.mesh_target_faces:
-    s = clean['stats']
-    print(f"simplified {s['faces_before']} -> {s['faces_after']} faces in {s['rounds']} rounds "
-          f"(mesh_target_faces {config.mesh_target_faces})" +
-          ('' if s['target_reached'] else ': stalled before the target, no edge left that may be collapsed'),
-          flush=True)
-  out_dir = os.path.join(config.checkpoint_dir, 'mesh')
-  os.makedirs(out_dir, exist_ok=True)
-  path = os.path.join(out_dir, f'mesh_step_{step}.ply')
-  mesh.write_ply(path, vertices, faces, *extra)
-  print(f'{vertices.shape[0]} vertices, {faces.shape[0]} faces in {elapsed:.2f} s '
-        f'(grid {config.mesh_resolution} along the longest side of {bbox}, {what}) -> {path}', flush=True)
+  baked = time.time() - timing['t']
+  _, c = ops.texture_atlas(faces.shape[0], size)
+  obj = mesh.write_obj(os.path.splitext(path)[0] + '.obj', vertices, faces, normals, uv, tex)[0]
+  print(f'texture {size} x {size}, {c} x {c} texels per cell, {(faces.shape[0] + 1) // 2 * c * c} texels baked in '
+        f'{baked:.2f} s -> {obj}', flush=True)
   return path
 
 

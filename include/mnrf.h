@@ -747,6 +747,28 @@ int mnrf_mesh_collapse_apply(int32_t num_vertices, int64_t num_faces, int64_t nu
                              double* quadrics, float* normals, int32_t* faces, uint8_t* face_alive,
                              mnrf_stream stream);
 
+/* ---- texture atlas of a mesh (mesh.bake_texture) ----------------------------------------------------------------
+ * Per-face charts packed two faces per square cell of an S x S atlas (S = size, in [4, 16384]): n = ceil(sqrt(ceil(F
+ * / 2))) cells per row, c = floor(S / n) texels per cell side, c >= 4 required (so at most 2 floor(S / 4)^2 faces);
+ * cell k (row-major) holds faces 2k (A) and 2k + 1 (B) and starts at texel ((k % n) c, (k / n) c).  In the cell's
+ * texel units, texel (i, j) centred at (i + 0.5, j + 0.5), a face's corners 0, 1, 2 are o, o + (d, 0), o + (0, d):
+ * A has o = (0.5, 0.5), d = c - 3; B has o = (c - 0.5, c - 0.5), d = 2 - c.  Texel (i, j) belongs to A when
+ * i + j + 2 <= c, else to B (to A when the cell has no B).  A bilinear sample inside a face's triangle reads only
+ * texels its face owns, so no face bleeds into another at mip level 0.
+ * Inputs: num_vertices vertices [V, 3] fp32, num_faces faces [F, 3] int32 (every index in [0, V); the kernel does not
+ * check, ops.mesh_texture_raster does, on the device, before the call), vertex normals [V, 3] fp32.
+ * Outputs: uv [F, 3, 2] fp32, each corner (u, v) in atlas texel units (u along a row, v down the rows; half-integers,
+ * exact); and, for each texel t of the used cells, ceil(F / 2) c^2 of them, cell-major and row-major within a cell:
+ * texel_index [T] int32 = row * S + column in the atlas, points [T, 3] = w0 p0 + w1 p1 + w2 p2 and texel_normals
+ * [T, 3], where (w1, w2) are the owner's barycentrics (the texel centre's offset from o over d) clamped to the
+ * triangle (w >= 0, then onto the hypotenuse w1 = clamp((w1 - w2 + 1) / 2, 0, 1), w2 = 1 - w1 when w1 + w2 > 1) and
+ * w0 = 1 - w1 - w2: the nearest point of the triangle.  The normal is the unit w0 n0 + w1 n1 + w2 n2; where that is
+ * zero, the face's unit (p1 - p0) x (p2 - p0); where that is zero too, (0, 0, 1).  A corner's texel has its vertex as
+ * its point exactly.  fp32, no FMA contraction; deterministic.  No reference counterpart. */
+int mnrf_mesh_texture_raster(int32_t num_vertices, int64_t num_faces, const float* vertices, const int32_t* faces,
+                             const float* normals, int32_t size, float* uv, int32_t* texel_index, float* points,
+                             float* texel_normals, mnrf_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

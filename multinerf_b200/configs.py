@@ -138,6 +138,9 @@ class Config:
   # simplification, right after cleaning (mesh.simplify_mesh): quadric edge collapse down to about this many faces;
   # 0 turns it off.
   mesh_target_faces: int = 0
+  # texture, after simplification (mesh.bake_texture): the side in texels, in [4, 16384], of a texture atlas the
+  # surface colour is baked into, written beside the PLY as mesh_step_<step>.{obj,mtl,png}; 0 turns it off.
+  mesh_texture_size: int = 0
 
 
 @dataclasses.dataclass

@@ -19,8 +19,10 @@
 // truncated signed distance, weight and colour sums held in registers across every view of a launch.
 //
 // And the two passes of mesh cleaning: connected components by union-find (uf_*_kernel) and the number of views
-// each vertex lands in (points_view_count_kernel); and mesh simplification by quadric edge collapse (qem_*_kernel).
+// each vertex lands in (points_view_count_kernel); mesh simplification by quadric edge collapse (qem_*_kernel); and
+// the texture atlas of a mesh: its per-face charts and one surface sample per texel (tex_*_kernel).
 #include <algorithm>
+#include <cmath>
 
 #include <cuda/atomic>
 
@@ -667,6 +669,103 @@ __global__ void __launch_bounds__(256) qem_apply_kernel(const QemArgs a) {
   }
 }
 
+// ------------------------------------------------------------------------------------------- texture atlas
+// Per-face charts, two faces per square cell of c x c texels, cells row-major in rows of n (mesh.bake_texture; the
+// layout is restated in tests/mesh_texture_ref.py).  Cell k holds faces 2k (A) and 2k + 1 (B).  In the cell's texel
+// units (texel (i, j) centred at (i + 0.5, j + 0.5)) each face is a right isosceles triangle with its corners on
+// texel centres: corner 0 at o, corner 1 at o + (d, 0), corner 2 at o + (0, d), with o = (0.5, 0.5), d = c - 3 for A
+// and o = (c - 0.5, c - 0.5), d = -(c - 2) for B.  Texel (i, j) belongs to A when i + j + 2 <= c, else to B (to A
+// when the cell has no B).  A bilinear sample inside A (u + v <= c - 2) reads texels with i + j < u + v + 1 <= c - 1,
+// all A's; one inside B (u + v >= c + 1) reads texels with i + j > u + v - 3 >= c - 2, all B's.  So no sample of a
+// face at mip level 0 reads another face's texel.
+struct TexAtlas {
+  int64_t nf;
+  int n, c, size;
+};
+
+// The chart of face f: its cell's first texel (x0, y0) in the atlas, and o, d in the cell's texel units
+__device__ __forceinline__ void tex_chart(const TexAtlas& a, int64_t f, int& x0, int& y0, float& o, float& d) {
+  const int64_t k = f >> 1;
+  x0 = (int)(k % a.n) * a.c;
+  y0 = (int)(k / a.n) * a.c;
+  o = f & 1 ? (float)a.c - 0.5f : 0.5f;
+  d = f & 1 ? (float)(2 - a.c) : (float)(a.c - 3);
+}
+
+// The face that owns texel (i, j) of cell k
+__device__ __forceinline__ int64_t tex_owner(const TexAtlas& a, int64_t k, int i, int j) {
+  return 2 * k + (i + j + 2 > a.c && 2 * k + 1 < a.nf);
+}
+
+__device__ __forceinline__ V3 tex_ld3(const float* __restrict__ p, int i) {
+  return V3{__ldg(p + 3 * (int64_t)i), __ldg(p + 3 * (int64_t)i + 1), __ldg(p + 3 * (int64_t)i + 2)};
+}
+
+// v / max|v_i| / |v / max|v_i||, so no finite v overflows or underflows; false when v is zero or not finite
+__device__ __forceinline__ bool tex_unit(V3& v) {
+  const float m = fmaxf(fabsf(v.x), fmaxf(fabsf(v.y), fabsf(v.z)));
+  if (!(m > 0.f) || !isfinite(m)) return false;
+  v = V3{v.x / m, v.y / m, v.z / m};
+  const float len = sqrtf(v.x * v.x + v.y * v.y + v.z * v.z);
+  v = V3{v.x / len, v.y / len, v.z / len};
+  return true;
+}
+
+__global__ void __launch_bounds__(256) tex_uv_kernel(const TexAtlas a, float* __restrict__ uv) {
+  for (int64_t f = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; f < a.nf; f += (int64_t)gridDim.x * blockDim.x) {
+    int x0, y0;
+    float o, d;
+    tex_chart(a, f, x0, y0, o, d);
+    float* q = uv + 6 * f;
+    q[0] = (float)x0 + o;     q[1] = (float)y0 + o;
+    q[2] = (float)x0 + o + d; q[3] = (float)y0 + o;
+    q[4] = (float)x0 + o;     q[5] = (float)y0 + o + d;
+  }
+}
+
+// One thread per texel t of the used cells, cell-major, row-major within a cell: its owner's barycentrics at the
+// texel centre, clamped to the triangle (the nearest point of the chart), then the surface point and the unit
+// interpolated vertex normal (the face's normal when that is zero, (0, 0, 1) when the face has no area).
+__global__ void __launch_bounds__(256)
+tex_raster_kernel(const TexAtlas a, int64_t num_texels, const float* __restrict__ vertices,
+                  const int32_t* __restrict__ faces, const float* __restrict__ vnormals,
+                  int32_t* __restrict__ texel_index, float* __restrict__ points, float* __restrict__ normals) {
+  const int cc = a.c * a.c;
+  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < num_texels;
+       t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t k = t / cc;
+    const int r = (int)(t - k * cc), j = r / a.c, i = r - j * a.c;
+    const int64_t f = tex_owner(a, k, i, j);
+    int x0, y0;
+    float o, d;
+    tex_chart(a, f, x0, y0, o, d);
+    float fa = fmaxf(((float)i + 0.5f - o) / d, 0.f), fb = fmaxf(((float)j + 0.5f - o) / d, 0.f);
+    if (fa + fb > 1.f) {
+      fa = fminf(fmaxf((fa - fb + 1.f) * 0.5f, 0.f), 1.f);
+      fb = 1.f - fa;
+    }
+    const float w0 = 1.f - fa - fb;
+    const int v0 = __ldg(faces + 3 * f), v1 = __ldg(faces + 3 * f + 1), v2 = __ldg(faces + 3 * f + 2);
+    const V3 p0 = tex_ld3(vertices, v0), p1 = tex_ld3(vertices, v1), p2 = tex_ld3(vertices, v2);
+    const V3 n0 = tex_ld3(vnormals, v0), n1 = tex_ld3(vnormals, v1), n2 = tex_ld3(vnormals, v2);
+    V3 n{w0 * n0.x + fa * n1.x + fb * n2.x, w0 * n0.y + fa * n1.y + fb * n2.y, w0 * n0.z + fa * n1.z + fb * n2.z};
+    if (!tex_unit(n)) {
+      const V3 e1{p1.x - p0.x, p1.y - p0.y, p1.z - p0.z}, e2{p2.x - p0.x, p2.y - p0.y, p2.z - p0.z};
+      n = V3{e1.y * e2.z - e1.z * e2.y, e1.z * e2.x - e1.x * e2.z, e1.x * e2.y - e1.y * e2.x};
+      if (!tex_unit(n)) n = V3{0.f, 0.f, 1.f};
+    }
+    texel_index[t] = (y0 + j) * a.size + x0 + i;
+    float* pt = points + 3 * t;
+    pt[0] = w0 * p0.x + fa * p1.x + fb * p2.x;
+    pt[1] = w0 * p0.y + fa * p1.y + fb * p2.y;
+    pt[2] = w0 * p0.z + fa * p1.z + fb * p2.z;
+    float* nt = normals + 3 * t;
+    nt[0] = n.x;
+    nt[1] = n.y;
+    nt[2] = n.z;
+  }
+}
+
 }  // namespace mnrf
 
 extern "C" int mnrf_marching_cubes(int32_t phase, int32_t nx, int32_t ny, int32_t nz, const float* grid, float level,
@@ -893,6 +992,37 @@ extern "C" int mnrf_mesh_collapse_apply(int32_t num_vertices, int64_t num_faces,
   a.vf_face = vf_face; a.positions = const_cast<float*>(positions); a.vertices = vertices; a.quadrics = quadrics;
   a.normals = normals; a.faces = faces; a.face_alive = face_alive;
   qem_apply_kernel<<<qem_blocks(num_edges), 256, 0, s>>>(a);
+  MNRF_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int mnrf_mesh_texture_raster(int32_t num_vertices, int64_t num_faces, const float* vertices,
+                                        const int32_t* faces, const float* normals, int32_t size, float* uv,
+                                        int32_t* texel_index, float* points, float* texel_normals,
+                                        mnrf_stream stream) {
+  using namespace mnrf;
+  set_error("");
+  MNRF_CHECK(num_vertices >= 0 && num_faces >= 0, "mnrf_mesh_texture_raster: %d vertices, %lld faces", num_vertices,
+             (long long)num_faces);
+  MNRF_CHECK(size >= 4 && size <= 16384, "mnrf_mesh_texture_raster: texture size %d, want [4, 16384]", size);
+  if (num_faces == 0) return 0;
+  const int64_t cells = (num_faces + 1) / 2;
+  int64_t n = (int64_t)std::sqrt((double)cells);
+  while (n * n < cells) ++n;
+  while (n > 1 && (n - 1) * (n - 1) >= cells) --n;
+  const int64_t c = size / n;
+  MNRF_CHECK(c >= 4, "mnrf_mesh_texture_raster: %lld faces do not fit a %d x %d atlas (%lld texels per cell, want >= "
+             "4; it holds at most %lld faces)", (long long)num_faces, size, size, (long long)c,
+             2 * (long long)(size / 4) * (size / 4));
+  MNRF_CHECK(num_vertices > 0 && vertices && faces && normals && uv && texel_index && points && texel_normals,
+             "mnrf_mesh_texture_raster: null pointer or no vertices");
+  const TexAtlas a{num_faces, (int)n, (int)c, size};
+  const int64_t num_texels = cells * c * c;
+  const int cap = mnrf_num_sms() * 16;
+  const cudaStream_t s = (cudaStream_t)stream;
+  tex_uv_kernel<<<(int)std::min<int64_t>((num_faces + 255) / 256, cap), 256, 0, s>>>(a, uv);
+  tex_raster_kernel<<<(int)std::min<int64_t>((num_texels + 255) / 256, cap), 256, 0, s>>>(
+      a, num_texels, vertices, faces, normals, texel_index, points, texel_normals);
   MNRF_LAUNCH_CHECK();
   return 0;
 }

@@ -16,9 +16,11 @@ no camera saw gives no faces (marching cubes skips cells with an unobserved, NaN
 the mean of the colours rendered for it across the views whose surface lies within the truncation band.
 
 Either method can clean the mesh (`clean_mesh`) and then simplify it to a face budget by quadric edge collapse
-(`simplify_mesh`) before any colour is computed.
+(`simplify_mesh`) before any colour is computed, and then bake the colour into a texture atlas (`bake_texture`,
+`texture_size`) that `write_obj` stores as a textured OBJ with its MTL and PNG.
 """
 import math
+import os
 from typing import NamedTuple
 
 import numpy as np
@@ -78,25 +80,58 @@ def density_grid(model, bbox, resolution, slab_planes=None):
 
 
 def extract_mesh(model, bbox, resolution, level, slab_planes=None, colors=False, keep_components=0, min_views=0,
-                 dataset=None, stats=None, target_faces=0):
+                 dataset=None, stats=None, target_faces=0, texture_size=0, before_texture=None):
   """(vertices [V, 3] fp32, faces [F, 3] int32) on the device: the surface density = `level` of `model`'s final
   level inside `bbox` (x0, y0, z0, x1, y1, z1), on a grid of `resolution` points along the longest side.
   Vertices are in world coordinates; face normals point from dense to empty space.  With `colors`, returns
   (vertices, faces, normals [V, 3] fp32, rgb [V, 3] uint8): unit vertex normals from the density grid's gradient,
   and each vertex's colour from `vertex_colors`.  `keep_components`, `min_views` (with the training cameras of
   `dataset`) and `stats`: clean_mesh, applied before the colours are queried.  target_faces: then simplify_mesh
-  (its counts go to `stats` too), the normals carried along."""
+  (its counts go to `stats` too), the normals carried along.  texture_size > 0: the normals are computed with or
+  without `colors`, and the colour is baked into a texture_size x texture_size atlas (bake_texture, each texel's
+  colour by `vertex_colors` at its surface point and normal); returns (vertices, faces, normals, rgb or None, uv,
+  texture).  before_texture: called with (vertices, faces, normals, rgb or None) before the texture is baked, so a
+  caller can save the mesh first (bake_texture raises ValueError when the atlas cannot hold the faces)."""
   grid, h = density_grid(model, bbox, resolution, slab_planes)
-  out = ops.marching_cubes(grid, level, normals=colors)
+  out = ops.marching_cubes(grid, level, normals=colors or texture_size > 0)
   del grid
   lo = torch.tensor([float(v) for v in bbox[:3]], device=out[0].device)
   vertices, faces, *normals = clean_mesh(out[0] * h + lo, *out[1:], **_clean_args(keep_components, min_views,
                                                                                    dataset, stats))
   vertices, faces, *normals = simplify_mesh(vertices, faces, *normals, target_faces=target_faces, stats=stats)
-  if not colors:
-    return vertices, faces
-  # cubic cells: the grid's normals are the world's
-  return vertices, faces, normals[0], vertex_colors(model, vertices, normals[0], h * h / 12)
+  var = h * h / 12
+  if not texture_size:
+    if not colors:
+      return vertices, faces
+    # cubic cells: the grid's normals are the world's
+    return vertices, faces, normals[0], vertex_colors(model, vertices, normals[0], var)
+  rgb = vertex_colors(model, vertices, normals[0], var) if colors else None
+  return _with_texture(vertices, faces, normals[0], rgb, texture_size, before_texture,
+                       lambda p, n: vertex_colors(model, p, n, var))
+
+
+def _with_texture(vertices, faces, normals, rgb, texture_size, before_texture, color_fn):
+  """(vertices, faces, normals, rgb, uv, texture): the mesh, and bake_texture's atlas of it by `color_fn`, after
+  before_texture(vertices, faces, normals, rgb) when given."""
+  if before_texture is not None:
+    before_texture(vertices, faces, normals, rgb)
+  return (vertices, faces, normals, rgb) + bake_texture(vertices, faces, normals, texture_size, color_fn)
+
+
+def bake_texture(vertices, faces, normals, size, color_fn):
+  """The colour of a mesh baked into a size x size texture atlas on the device -> (uv [F, 3, 2] fp32, each face
+  corner's position in texel units, u along a row and v down the rows; texture [size, size, 3] uint8, row 0 on top).
+  vertices [V, 3], faces [F, 3] int32, normals [V, 3]: the mesh and its unit vertex normals.  Each face gets its own
+  right-triangle chart, two per square cell of c x c texels, c >= 4 (ops.mesh_texture_raster, csrc/mesh.cu); every
+  texel of a used cell is given the colour of its face at the texel centre's nearest point of the chart:
+  color_fn(points [T, 3], normals [T, 3]) -> uint8 [T, 3] at those surface points and unit interpolated normals.
+  Texels of unused cells stay 0.  Raises ValueError when the atlas cannot hold the faces."""
+  uv, index, points, tnormals = ops.mesh_texture_raster(vertices, faces.int().contiguous(), normals.contiguous(),
+                                                        size)
+  texture = torch.zeros(size * size, 3, device=vertices.device, dtype=torch.uint8)
+  if index.shape[0]:
+    texture[index.long()] = color_fn(points, tnormals)
+  return uv, texture.view(size, size, 3)
 
 
 def vertex_colors(model, vertices, normals, var):
@@ -115,13 +150,16 @@ def validate_config(bundle):
   """The mesh method of `bundle`'s Config, checked: 'density' or 'tsdf'; the TSDF method needs perspective or fisheye
   views (not NDC) and a truncation of at least one cell, so no cut edge of the fused grid has an unobserved end.
   The cleaning and simplification options must not be negative, and mesh_min_views projects into the views, so it
-  needs them not NDC either."""
+  needs them not NDC either.  mesh_texture_size is 0 (off) or in [4, 16384]."""
   config = bundle.config
   if config.mesh_method not in MESH_METHODS:
     raise ValueError(f'Config.mesh_method = {config.mesh_method!r}: want one of {MESH_METHODS}')
   for name in ('mesh_keep_components', 'mesh_min_views', 'mesh_target_faces'):
     if getattr(config, name) < 0:
       raise ValueError(f'Config.{name} = {getattr(config, name)!r}: want 0 (off) or more')
+  lo, hi = ops.TEXTURE_SIZES
+  if config.mesh_texture_size != 0 and not lo <= config.mesh_texture_size <= hi:
+    raise ValueError(f'Config.mesh_texture_size = {config.mesh_texture_size!r}: want 0 (off) or [{lo}, {hi}]')
   if config.mesh_min_views > 0 and config.forward_facing:
     raise ValueError('Config.mesh_min_views does not support forward-facing (NDC) scenes')
   if config.mesh_method == 'tsdf':
@@ -185,51 +223,70 @@ def fuse_tsdf(views, cameras, camtype, bbox, resolution, truncation, colors=Fals
   return (tsdf, weight, color_sum, color_weight), h
 
 
-def tsdf_mesh(state, bbox, h, colors=False, clean_args=None, target_faces=0, stats=None):
+def tsdf_mesh(state, bbox, h, colors=False, clean_args=None, target_faces=0, stats=None, texture_size=0,
+              before_texture=None):
   """Marching cubes on the fused TSDF `state` (fuse_tsdf): the zero crossing of -tsdf (inside > 0, so faces and
   normals point out of the surface), with every point no view observed (weight 0) NaN, so it gives no faces.
   Returns (vertices, faces) in world coordinates, and with `colors` also (normals [V, 3], rgb [V, 3] uint8): each
   vertex's colour is color_sum / color_weight interpolated linearly along its grid edge, rounded as vertex_colors
   rounds.  clean_args: keyword arguments of clean_mesh, applied before the colours are interpolated.
   target_faces: then simplify_mesh (counts to `stats`); a simplified vertex no longer lies on a grid edge, so its
-  colour is interpolated trilinearly at (vertex - lo) / h, clamped to the grid."""
+  colour is interpolated trilinearly at (vertex - lo) / h, clamped to the grid (tsdf_colors).  texture_size > 0
+  (the state must hold the colour grid): the normals are computed with or without `colors` and the colour is baked
+  into a texture atlas, each texel's by tsdf_colors at its surface point; returns and calls `before_texture` as
+  extract_mesh does."""
   tsdf, weight, color_sum, color_weight = state
+  if texture_size and color_sum is None:
+    raise ValueError('tsdf_mesh: texture_size needs the fused colour grid (fuse_tsdf with colors=True)')
   grid = torch.where(weight > 0, -tsdf, torch.full_like(tsdf, float('nan')))
-  out = ops.marching_cubes(grid, 0.0, normals=colors)
+  out = ops.marching_cubes(grid, 0.0, normals=colors or texture_size > 0)
   del grid
   lo = torch.tensor([float(v) for v in bbox[:3]], device=out[0].device)
   simplify = target_faces > 0
   # without simplification the grid-unit vertices ride along as a per-vertex array: the colours are interpolated
   # from them
   ride = (out[0],) if colors and not simplify else ()
-  vertices, faces, *per = clean_mesh(out[0] * h + lo, out[1], *((out[2],) if colors else ()), *ride,
-                                     **(clean_args or {}))
+  vertices, faces, *per = clean_mesh(out[0] * h + lo, out[1], *out[2:], *ride, **(clean_args or {}))
   if simplify:
     vertices, faces, *per = simplify_mesh(vertices, faces, *per, target_faces=target_faces, stats=stats)
   elif stats is not None:
     simplify_mesh(vertices, faces, target_faces=0, stats=stats)
-  if not colors:
+  if not colors and not texture_size:
     return vertices, faces
-  normals, gv = (per[0], ((vertices - lo) / h).clamp_min(0)) if simplify else per
-  # unsimplified, a vertex lies on a grid edge: its two other coordinates are integers, so the trilinear weights
-  # reduce to the linear interpolation between the edge's two ends
-  nz, ny, nx = tsdf.shape
+  rgb = None
+  if colors:
+    # unsimplified, a vertex lies on a grid edge: its two other coordinates are integers, so the trilinear weights
+    # reduce to the linear interpolation between the edge's two ends
+    rgb = (tsdf_colors(color_sum, color_weight, (vertices - lo) / h) if simplify else
+           tsdf_colors(color_sum, color_weight, per[1], clamp=False))
+  if not texture_size:
+    return vertices, faces, per[0], rgb
+  return _with_texture(vertices, faces, per[0], rgb, texture_size, before_texture,
+                       lambda p, n: tsdf_colors(color_sum, color_weight, (p - lo) / h))
+
+
+def tsdf_colors(color_sum, color_weight, gv, clamp=True):
+  """rgb [N, 3] uint8 at points gv [N, 3] in grid units (x, y, z) of the fused colour grids color_sum [nz, ny, nx, 3]
+  and color_weight [nz, ny, nx] (fuse_tsdf): both interpolated trilinearly, their quotient (0 where no colour was
+  fused nearby) rounded as vertex_colors rounds.  clamp: first clamp gv to the grid, [0, n - 1] along each axis;
+  without it gv must lie there already."""
+  nz, ny, nx = color_weight.shape
   dims = torch.tensor([nx, ny, nz], device=gv.device)
-  if simplify:
-    gv = torch.minimum(gv, dims - 1)
+  if clamp:
+    gv = torch.minimum(gv.clamp_min(0), dims - 1)
   base = torch.minimum(gv.floor().long(), dims - 2).clamp_min(0)
   frac = gv - base
-  cs = torch.zeros(len(vertices), 3, device=vertices.device)
-  cw = torch.zeros(len(vertices), device=vertices.device)
+  cs = torch.zeros(len(gv), 3, device=gv.device)
+  cw = torch.zeros(len(gv), device=gv.device)
   for corner in range(8):
-    off = torch.tensor([corner & 1, corner >> 1 & 1, corner >> 2 & 1], device=vertices.device)
+    off = torch.tensor([corner & 1, corner >> 1 & 1, corner >> 2 & 1], device=gv.device)
     wgt = torch.where(off.bool(), frac, 1 - frac).prod(-1)
     q = base + off
     p = (q[:, 2] * ny + q[:, 1]) * nx + q[:, 0]
     cs += wgt[:, None] * color_sum.view(-1, 3)[p]
     cw += wgt * color_weight.view(-1)[p]
   rgb = torch.where(cw[:, None] > 0, cs / cw.clamp_min(1e-30)[:, None], torch.zeros_like(cs))
-  return vertices, faces, normals, (rgb.clamp(0, 1) * 255).round().to(torch.uint8)
+  return (rgb.clamp(0, 1) * 255).round().to(torch.uint8)
 
 
 def render_views(model, dataset):
@@ -245,15 +302,16 @@ def render_views(model, dataset):
 
 
 def extract_mesh_tsdf(model, dataset, bbox, resolution, truncation=3.0, colors=False, batch=8, keep_components=0,
-                      min_views=0, stats=None, target_faces=0):
+                      min_views=0, stats=None, target_faces=0, texture_size=0, before_texture=None):
   """Config.mesh_method = 'tsdf': render every camera of `dataset` (render_views), fuse the renders (fuse_tsdf, a
   band of `truncation` cells) and mesh the result (tsdf_mesh).  Returns what extract_mesh returns.
   `keep_components`, `min_views` (against the cameras of `dataset`) and `stats`: clean_mesh, applied before the
-  colours are interpolated; `target_faces`: then simplify_mesh."""
+  colours are interpolated; `target_faces`: then simplify_mesh; `texture_size`, `before_texture`: then the texture
+  (tsdf_mesh), the fusion keeping its colour grid for it."""
   state, h = fuse_tsdf(render_views(model, dataset), dataset.cameras, dataset.camtype, bbox, resolution, truncation,
-                       colors=colors, batch=batch, device=model.device)
+                       colors=colors or texture_size > 0, batch=batch, device=model.device)
   return tsdf_mesh(state, bbox, h, colors=colors, clean_args=_clean_args(keep_components, min_views, dataset, stats),
-                   target_faces=target_faces, stats=stats)
+                   target_faces=target_faces, stats=stats, texture_size=texture_size, before_texture=before_texture)
 
 
 def clean_mesh(vertices, faces, *per_vertex, keep_components=0, min_views=0, cameras=None, camtype=None,
@@ -476,3 +534,36 @@ def write_ply(path, vertices, faces, normals=None, colors=None):
     fh.write(header.encode('ascii'))
     fh.write(vrec.tobytes())
     fh.write(rec.tobytes())
+
+
+def write_obj(path, vertices, faces, normals, uv, texture):
+  """A textured mesh as three files beside each other: <stem>.obj (positions `v`, one texture coordinate `vt` per face
+  corner, normals `vn`, faces `f v/vt/vn`), <stem>.mtl (one material whose diffuse map is the PNG) and <stem>.png
+  (texture, uint8 [S, S, 3], written as it is).  uv [F, 3, 2]: bake_texture's corner positions in texel units; a
+  corner's `vt` is (u / S, 1 - v / S), OBJ's origin being the image's bottom-left corner.  Floats are printed with
+  %.9g, so every fp32 value reads back exactly.  Returns the paths (obj, mtl, png)."""
+  from PIL import Image
+  stem = os.path.splitext(path)[0]
+  name = os.path.basename(stem)
+  host = lambda t, dtype: np.ascontiguousarray(torch.as_tensor(t).detach().cpu().numpy(), dtype=dtype)
+  v, n = host(vertices, np.float32).reshape(-1, 3), host(normals, np.float32).reshape(-1, 3)
+  f = host(faces, np.int64).reshape(-1, 3)
+  tex = host(texture, np.uint8)
+  size = tex.shape[0]
+  assert tex.shape == (size, size, 3), 'texture must be [S, S, 3]'
+  uvh = host(uv, np.float32).reshape(-1, 2)
+  vt = np.stack([uvh[:, 0] / np.float32(size), np.float32(1) - uvh[:, 1] / np.float32(size)], -1)
+  # f a/ta/na: 1-based; face k's corners are vt 3k + 1 .. 3k + 3
+  corners = np.stack([f + 1, np.arange(1, 3 * len(f) + 1).reshape(-1, 3), f + 1], -1)
+  obj, mtl, png = stem + '.obj', stem + '.mtl', stem + '.png'
+  with open(obj, 'w') as fh:
+    fh.write(f'mtllib {name}.mtl\n')
+    fh.write(('v %.9g %.9g %.9g\n' * len(v)) % tuple(v.ravel().tolist()))
+    fh.write(('vt %.9g %.9g\n' * len(vt)) % tuple(vt.ravel().tolist()))
+    fh.write(('vn %.9g %.9g %.9g\n' * len(n)) % tuple(n.ravel().tolist()))
+    fh.write('usemtl texture\n')
+    fh.write(('f %d/%d/%d %d/%d/%d %d/%d/%d\n' * len(f)) % tuple(corners.ravel().tolist()))
+  with open(mtl, 'w') as fh:
+    fh.write(f'newmtl texture\nKa 1 1 1\nKd 1 1 1\nKs 0 0 0\nillum 1\nmap_Kd {name}.png\n')
+  Image.fromarray(tex).save(png, 'PNG')
+  return obj, mtl, png

@@ -298,6 +298,55 @@ def mesh_collapse_apply(collapse, edges, edge_off, edge_face, vf_off, vf_face, p
   return alive
 
 
+TEXTURE_SIZES = (4, 16384)
+
+
+def texture_atlas(num_faces, size):
+  """(n, c): cells per row and texels per cell side of the size x size atlas of `num_faces` per-face charts, two per
+  cell (mnrf_mesh_texture_raster, include/mnrf.h).  Raises ValueError when `size` lies outside [4, 16384] or a cell
+  would be narrower than 4 texels."""
+  if not TEXTURE_SIZES[0] <= size <= TEXTURE_SIZES[1]:
+    raise ValueError(f'texture size {size}: want [{TEXTURE_SIZES[0]}, {TEXTURE_SIZES[1]}]')
+  cells = (num_faces + 1) // 2
+  n = math.isqrt(cells - 1) + 1 if cells else 0
+  c = size // n if n else size
+  if c < 4:
+    raise ValueError(f'{num_faces} faces do not fit a {size} x {size} texture atlas, which holds at most '
+                     f'{2 * (size // 4) ** 2} faces (cells of at least 4 x 4 texels): raise the texture size or '
+                     f'simplify the mesh first (Config.mesh_target_faces)')
+  return n, c
+
+
+def mesh_texture_raster(vertices, faces, normals, size):
+  """The texture atlas of a mesh (mnrf_mesh_texture_raster, csrc/mesh.cu): vertices [V, 3], faces [F, 3] int32 and
+  vertex normals [V, 3] on the device, a size x size atlas -> (uv [F, 3, 2] fp32 corner positions in texel units,
+  texel_index [T] int32 row-major in the atlas, points [T, 3], normals [T, 3]) for the T = ceil(F / 2) c^2 texels of
+  the used cells (texture_atlas).  Checks on the device that every face index lies in [0, V) and reads that one flag
+  back; an index out of range raises ValueError and never reaches the kernel."""
+  lib = L.load()
+  assert faces.dtype == torch.int32 and faces.is_contiguous() and faces.dim() == 2 and faces.shape[1] == 3
+  V, F = vertices.shape[0], faces.shape[0]
+  n, c = texture_atlas(F, size)
+  if not 0 <= V < 2 ** 31:
+    raise ValueError(f'mesh_texture_raster: {V} vertices')
+  if normals.shape != vertices.shape or vertices.dim() != 2 or vertices.shape[1] != 3:
+    raise ValueError(f'mesh_texture_raster: vertices {tuple(vertices.shape)} and normals {tuple(normals.shape)}: '
+                     'want [V, 3] both')
+  if F and bool(((faces < 0) | (faces >= V)).any()):
+    raise ValueError(f'mesh_texture_raster: a face index lies outside [0, {V})')
+  dev = faces.device
+  T = (F + 1) // 2 * c * c
+  uv = torch.empty(F, 3, 2, device=dev)
+  index = torch.empty(T, device=dev, dtype=torch.int32)
+  points = torch.empty(T, 3, device=dev)
+  tnormals = torch.empty(T, 3, device=dev)
+  if F:
+    _count(2)
+    L.check(lib.mnrf_mesh_texture_raster(V, F, L.ptr(_f32(vertices)), L.ptr(faces), L.ptr(_f32(normals)), int(size),
+                                         L.ptr(uv), L.ptr(index), L.ptr(points), L.ptr(tnormals), L.stream_ptr()))
+  return uv, index, points, tnormals
+
+
 def points_view_count(points, camtype, distortion_params, worldtocams, camtopixs, height, width):
   """For each point [N, 3] fp32 on the device, the number of views whose height x width image it lands on
   (mnrf_points_view_count, csrc/mesh.cu: the pixel rule of tsdf_integrate) -> counts [N] int32.  camtype 0

@@ -20,9 +20,15 @@
           more call with CUDA events around each step, the time in the torch topology rebuilds against the kernels;
           mesh.extract_mesh at --extract_res^3 without and with target_faces = --simplify_faces, alternated --reps
           times (not part of `all`);
+  texture: the 512^3 `mc` mesh simplified to --texture_faces faces; mnrf_mesh_texture_raster alone (CUDA events over
+          --texture_launches launches) on it at S = 4096 and 8192; the colour query over all of the 4096 atlas's texels
+          (mesh.vertex_colors, a synchronised window) on the 360.gin and blender_256.gin NerfMLPs; mesh.write_obj and
+          the PNG alone; and mesh.extract_mesh at --extract_res^3 on the random-init 360.gin model with target_faces
+          = --simplify_faces, without and with texture_size = --texture_extract_size (large enough for the mesh the
+          simplification stalls at), alternated --reps times (not part of `all`);
   device: the card's name and power limit, read in the same run.
 
-  python tools/mesh_bench.py [--rows 8388608] [--extract_res 512] [--sections all|components|simplify]
+  python tools/mesh_bench.py [--rows 8388608] [--extract_res 512] [--sections all|components|simplify|texture]
                              [--out result.json]
 """
 import argparse
@@ -269,18 +275,84 @@ def bench_simplify_section(model, bbox, level, args):
   return out
 
 
+def bench_texture_section(model, bbox, level, args):
+  import tempfile
+  from PIL import Image
+  out = {'raster': [], 'color_query': {}, 'write': {}, 'extract': {'plain_s': [], 'textured_s': []}}
+  v, f, n = ops.marching_cubes(sphere_noise(512), 0.0, normals=True)
+  v, f, n = mesh.simplify_mesh(v, f, n, target_faces=args.texture_faces)
+  torch.cuda.empty_cache()
+  L = lib.load()
+  F = int(f.shape[0])
+  for size in (4096, 8192):
+    _, c = ops.texture_atlas(F, size)
+    T = (F + 1) // 2 * c * c
+    bufs = [torch.empty(F, 3, 2, device='cuda'), torch.empty(T, dtype=torch.int32, device='cuda'),
+            torch.empty(T, 3, device='cuda'), torch.empty(T, 3, device='cuda')]
+    launch = lambda: lib.check(L.mnrf_mesh_texture_raster(v.shape[0], F, lib.ptr(v), lib.ptr(f), lib.ptr(n), size,
+                                                          *(lib.ptr(b) for b in bufs), lib.stream_ptr()))
+    ms = events(launch, args.texture_launches)
+    # bytes by count: per texel 4 B index + 24 B point and normal written; per face 24 B of uv
+    nbytes = 28 * T + 24 * F
+    out['raster'].append({'faces': F, 'size': size, 'cell': c, 'texels': T, 'ms': round(ms, 3),
+                          'write_tb_per_s_by_count': round(nbytes / (ms * 1e-3) / 1e12, 3)})
+    del bufs
+    torch.cuda.empty_cache()
+  _, _, points, tnormals = ops.mesh_texture_raster(v, f, n, 4096)
+  for name, make in (('360', configs.bundle_360), ('blender_256', configs.bundle_blender_256)):
+    m = models.Model(make())
+    m.init(seed=0)
+    mesh.vertex_colors(m, points[:1 << 20], tnormals[:1 << 20], 1e-6)      # warm-up of the chunk shapes
+    t, _ = timed(lambda: mesh.vertex_colors(m, points, tnormals, 1e-6), 1)
+    out['color_query'][name] = {'texels': int(points.shape[0]), 's': round(t, 3),
+                                'rows_per_s': round(points.shape[0] / t / 1e6, 1)}
+    del m
+    torch.cuda.empty_cache()
+  del points, tnormals
+  uv, tex = mesh.bake_texture(v, f, n, 4096, lambda p, nn: ((p.abs() * 40) % 256).to(torch.uint8))
+  with tempfile.TemporaryDirectory() as tmp:
+    t0 = time.perf_counter()
+    mesh.write_obj(os.path.join(tmp, 'm.obj'), v, f, n, uv, tex)
+    t_obj = time.perf_counter() - t0
+    host = tex.cpu().numpy()
+    t0 = time.perf_counter()
+    Image.fromarray(host).save(os.path.join(tmp, 'p.png'), 'PNG')
+    t_png = time.perf_counter() - t0
+    out['write'] = {'faces': F, 'size': 4096, 'write_obj_s': round(t_obj, 3), 'png_alone_s': round(t_png, 3),
+                    'obj_bytes': os.path.getsize(os.path.join(tmp, 'm.obj')),
+                    'png_bytes': os.path.getsize(os.path.join(tmp, 'm.png'))}
+  del v, f, n, uv, tex
+  torch.cuda.empty_cache()
+  size = args.texture_extract_size
+  kw = dict(target_faces=args.simplify_faces)
+  mesh.extract_mesh(model, bbox, args.extract_res, level, texture_size=size, **kw)      # warm-up
+  torch.cuda.empty_cache()
+  for _ in range(args.reps):
+    for key, tsize in (('plain_s', 0), ('textured_s', size)):
+      t, o = timed(lambda: mesh.extract_mesh(model, bbox, args.extract_res, level, texture_size=tsize, **kw), 1)
+      out['extract'][key].append(round(t, 3))
+      out['extract']['faces'] = int(o[1].shape[0])
+      del o
+      torch.cuda.empty_cache()
+  out['extract'].update(texture_size=size, cell=ops.texture_atlas(out['extract']['faces'], size)[1])
+  return out
+
+
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--rows', type=int, default=1 << 23)
   ap.add_argument('--reps', type=int, default=3)
   ap.add_argument('--extract_res', type=int, default=512)
-  ap.add_argument('--sections', default='all', choices=('all', 'components', 'simplify'))
+  ap.add_argument('--sections', default='all', choices=('all', 'components', 'simplify', 'texture'))
   ap.add_argument('--simplify_faces', type=int, default=1_000_000)
+  ap.add_argument('--texture_faces', type=int, default=1_000_000)
+  ap.add_argument('--texture_launches', type=int, default=20)
+  ap.add_argument('--texture_extract_size', type=int, default=16384)
   ap.add_argument('--out', default=None)
   args = ap.parse_args()
   lib.require_device()
   res = {'device': device_info(), 'query': {}, 'mc': [], 'extract': None}
-  if args.sections in ('components', 'simplify'):
+  if args.sections in ('components', 'simplify', 'texture'):
     b = configs.bundle_360()
     model = models.Model(b)
     model.init(seed=0)
@@ -289,7 +361,8 @@ def main():
     level = float(grid.median())
     del grid
     torch.cuda.empty_cache()
-    section = bench_components_section if args.sections == 'components' else bench_simplify_section
+    section = {'components': bench_components_section, 'simplify': bench_simplify_section,
+               'texture': bench_texture_section}[args.sections]
     res = {'device': res['device'], 'level': level, args.sections: section(model, bbox, level, args),
            'device_after': device_info()}
     emit(res, args.out)
