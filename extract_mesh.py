@@ -12,6 +12,10 @@ Config.mesh_keep_components keeps only the largest connected components (mesh.cl
 Config.mesh_target_faces then simplifies the mesh to about that many faces by quadric edge collapse
 (mesh.simplify_mesh).  Config.mesh_texture_size = S then bakes the surface colour into an S x S texture atlas
 (mesh.bake_texture) and writes mesh_step_<step>.{obj,mtl,png} beside the PLY, which is written first and unchanged.
+Config.mesh_eval = True then scores the mesh against the test split (mesh.evaluate_mesh): it renders the NeRF on the
+test views for reference, traces every test pixel's ray into the mesh, shaded with the most detailed colour the run
+produced (the texture, else the vertex colours, else none), and writes mesh/eval_step_<step>/{color,normals}_NNN.png,
+distance_NNN.tiff and metric_<name>.txt (per-image values, space-separated).
 One process on one GPU.
 """
 import dataclasses
@@ -21,9 +25,10 @@ import time
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
+import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
-from multinerf_b200 import checkpoints, configs, datasets, mesh, ops, train_utils  # noqa: E402
+from multinerf_b200 import checkpoints, configs, datasets, mesh, ops, train_utils, utils  # noqa: E402
 from train import parse  # noqa: E402
 
 
@@ -85,15 +90,60 @@ def main(argv=None):
                                                 **texture)
   if not size:
     save_ply(vertices, faces, *extra)
+    if config.mesh_eval:
+      normals, rgb = extra if extra else (None, None)
+      evaluate(model, config, step, out_dir, vertices, faces, normals=normals, rgb=rgb)
     return path
-  normals, _, uv, tex = extra
+  normals, rgb, uv, tex = extra
   torch.cuda.synchronize()
   baked = time.time() - timing['t']
   _, c = ops.texture_atlas(faces.shape[0], size)
   obj = mesh.write_obj(os.path.splitext(path)[0] + '.obj', vertices, faces, normals, uv, tex)[0]
   print(f'texture {size} x {size}, {c} x {c} texels per cell, {(faces.shape[0] + 1) // 2 * c * c} texels baked in '
         f'{baked:.2f} s -> {obj}', flush=True)
+  if config.mesh_eval:
+    evaluate(model, config, step, out_dir, vertices, faces, normals=normals, uv=uv, texture=tex)
   return path
+
+
+def evaluate(model, config, step, out_dir, vertices, faces, **colour):
+  """Config.mesh_eval: the mesh against the test split, the NeRF's renders of it as the reference; writes the renders
+  and metric files to <out_dir>/eval_step_<step> and prints each metric's mean and where the time went."""
+  dataset = datasets.load_dataset('test', config.data_dir, dataclasses.replace(config, render_path=False),
+                                  device=model.device)
+  eval_dir = os.path.join(out_dir, f'eval_step_{step}')
+  os.makedirs(eval_dir, exist_ok=True)
+  nerf_time = [0.0]
+
+  def reference():
+    views = mesh.render_views(model, dataset)
+    while True:
+      t0 = time.time()
+      view = next(views, None)
+      torch.cuda.synchronize()
+      nerf_time[0] += time.time() - t0
+      if view is None:
+        return
+      yield view
+
+  def save(idx, render):
+    if render['rgb'] is not None:
+      utils.save_img_u8(render['rgb'], os.path.join(eval_dir, f'color_{idx:03d}.png'))
+    utils.save_img_u8(render['normals'] / 2. + 0.5, os.path.join(eval_dir, f'normals_{idx:03d}.png'))
+    utils.save_img_f32(render['distance'], os.path.join(eval_dir, f'distance_{idx:03d}.tiff'))
+
+  lo, hi = model.mcfg.bg_intensity_range
+  timing = {}
+  metrics = mesh.evaluate_mesh(vertices, faces, dataset, config, reference=reference(), bg=(lo + hi) / 2,
+                               save_fn=save, timing=timing, **colour)
+  for name in (metrics[0] if metrics else {}):
+    with open(os.path.join(eval_dir, f'metric_{name}.txt'), 'w') as f:
+      f.write(' '.join(str(m[name]) for m in metrics))
+    print(f'mesh eval {name:14s} = {np.mean([m[name] for m in metrics]):.4f}', flush=True)
+  print(f'mesh eval: {len(metrics)} test views, NeRF rendering {nerf_time[0]:.2f} s, BVH build '
+        f'{timing.get("build", 0.0):.3f} s, tracing and shading {timing.get("trace", 0.0):.3f} s -> {eval_dir}',
+        flush=True)
+  return metrics
 
 
 if __name__ == '__main__':

@@ -769,6 +769,51 @@ int mnrf_mesh_texture_raster(int32_t num_vertices, int64_t num_faces, const floa
                              const float* normals, int32_t size, float* uv, int32_t* texel_index, float* points,
                              float* texel_normals, mnrf_stream stream);
 
+/* ---- closest-hit ray casting into a mesh (mesh.evaluate_mesh; csrc/mesh_trace.cu) ---------------------------------
+ * A linear BVH over the faces (Karras 2012) and one thread per ray tracing it.  No reference counterpart.
+ * The mesh: num_vertices vertices [V, 3] fp32, all finite, and num_faces faces [F, 3] int32 with every index in [0, V)
+ * and 1 <= F < 2^30 (the kernels do not check; ops.mesh_bvh checks both on the device before the first call, and
+ * handles F = 0 and F = 1 on the host: a one-face tree is its leaf, with no nodes).
+ *   phase BOXES: face_boxes [F, 6] fp32 = (min xyz, max xyz) of each face's corners, and centroids [F, 3] fp32 =
+ *                ((v0 + v1) + v2) / 3 per axis, each operation rounded to nearest.
+ *   phase KEYS:  with centroid_bounds [6] fp32 = (min xyz, max xyz) of the centroids (on the device): keys [F] int64
+ *                = morton << 32 | face, morton the 30-bit interleave (x highest) of each axis' cell
+ *                floor(clamp((c - lo) / (hi - lo), 0, 1) * 1024) clamped to 1023 (0 where hi == lo).
+ *   phase TREE:  with sorted_keys [F] int64 ascending, F >= 2: nodes [F - 1, 16] (fp32 with int32 children), parent
+ *                [2 F - 1] int32, leaf_face [F] int32; counters [F - 1] int32 is scratch, zeroed by the call.  Node
+ *                c < F - 1 is internal (0 is the root, whose parent is -1); node c >= F - 1 is leaf c - (F - 1), in
+ *                key order, holding face leaf_face[c - (F - 1)] = sorted_keys[c - (F - 1)] & 0xffffffff.  Internal
+ *                node i: floats [0, 6) and [6, 12) the boxes (min xyz, max xyz) of its left and right child, [12, 14)
+ *                the children (int32), [14, 16) zero.  Children by Karras's split of the sorted keys; a leaf's box
+ *                is its face's box, an internal node's the min / max of its children's.  The keys have 62
+ *                significant bits and the common prefix grows at every level, so the depth is at most 63.
+ * No rounding in the tree phase: the result is bit-reproducible (tests/mesh_trace_ref.py restates it).  Phases
+ * BOXES and TREE read the inputs only on the device; none synchronises the host. */
+enum { MNRF_BVH_BOXES = 0, MNRF_BVH_KEYS = 1, MNRF_BVH_TREE = 2 };
+int mnrf_mesh_bvh(int32_t phase, int32_t num_vertices, int64_t num_faces, const float* vertices, const int32_t* faces,
+                  float* face_boxes, float* centroids, const float* centroid_bounds, int64_t* keys,
+                  const int64_t* sorted_keys, float* nodes, int32_t* parent, int32_t* leaf_face, int32_t* counters,
+                  mnrf_stream stream);
+
+/* Closest hit of each of num_rays rays: origins, directions [N, 3], near, far [N] fp32 (as Rays holds them).  Only
+ * hits with near <= t <= far count, t the parameter along `directions` (not normalised).  The tree of mnrf_mesh_bvh
+ * (nodes: NULL allowed when F = 1) on the same vertices and faces.  Outputs: hit_face [N] int32 (-1 for a miss),
+ * hit_t [N] fp32 (+inf for a miss), hit_bary [N, 2] fp32, the barycentrics of corners faces[f, 1] and faces[f, 2]
+ * (0 for a miss).  Among the faces tested the closest hit is the least (t, face), and the traversal is a fixed
+ * function of the tree, so two runs on the same mesh are bit-identical.  A box is skipped when its fp32 entry
+ * distance exceeds the best t, with no downward widening: where two faces' t tie exactly, a tree over the same faces
+ * in another order can settle on the other one.  Ray/box: slab test, far bound widened by 1 + 2 gamma(3) rounded up
+ * to a float (Ize 2013).  Ray/triangle: watertight
+ * (Woop, Benthin and Wald 2013), a shear onto the dominant axis of the direction, fp32 edge functions recomputed in
+ * fp64 when one is exactly 0, so a ray through a shared edge or vertex hits at least one of the faces there.  A ray
+ * with a non-finite origin or direction component, a zero direction, a NaN near or far, or near > far misses.
+ * Depth-first with a 64-entry stack per thread; should a push find it full, the ray ends as a miss and error_flag
+ * (int32, device) is or-ed with 1: the caller reads it back.  fp32, no FMA contraction; no atomics but the flag. */
+int mnrf_mesh_trace(int64_t num_rays, const float* origins, const float* directions, const float* near,
+                    const float* far, int64_t num_faces, const float* nodes, const int32_t* leaf_face,
+                    const float* vertices, const int32_t* faces, int32_t* hit_face, float* hit_t, float* hit_bary,
+                    int32_t* error_flag, mnrf_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -19,6 +19,7 @@ SOURCES = {
     'composite.cu': ['-fmad=false'], 'heads.cu': [], 'gemm_tc.cu': [], 'gemm_tc_act.cu': [], 'chain.cu': [],
     'gemm_ref.cu': [],
     'refnerf.cu': [], 'camera.cu': ['-fmad=false'], 'robust.cu': ['-fmad=false'], 'mesh.cu': ['-fmad=false'],
+    'mesh_trace.cu': ['-fmad=false'],
 }
 
 

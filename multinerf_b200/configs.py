@@ -141,6 +141,11 @@ class Config:
   # texture, after simplification (mesh.bake_texture): the side in texels, in [4, 16384], of a texture atlas the
   # surface colour is baked into, written beside the PLY as mesh_step_<step>.{obj,mtl,png}; 0 turns it off.
   mesh_texture_size: int = 0
+  # score the extracted mesh against the test views (mesh.evaluate_mesh): trace every test pixel's ray into it, write
+  # its colour, normal and distance renders and per-image metrics (psnr / ssim against the test images, and
+  # coverage, spurious hits and depth error against the NeRF's own renders) to <checkpoint_dir>/mesh/eval_step_<step>.
+  # Not for forward-facing (NDC) scenes.
+  mesh_eval: bool = False
 
 
 @dataclasses.dataclass

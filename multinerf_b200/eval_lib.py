@@ -39,6 +39,19 @@ def compute_weighted_mae(weights, normals, normals_gt):
   return float((weights * np.arccos(cos)).sum() / weights.sum() * 180.0 / np.pi)
 
 
+def image_metrics(config, postprocess_fn, metric_harness, rgb_gt, *rgbs):
+  """One metric dict (psnr, ssim) per image of `rgbs` against `rgb_gt`, all [H, W, 3]: each through
+  `postprocess_fn` (RawNeRF's, or the identity), the predictions rounded to 8 bits with Config.eval_quantize_metrics
+  (what the saved PNGs hold) and every image cropped by Config.eval_crop_borders."""
+  rgbs, rgb_gt = [postprocess_fn(x) for x in rgbs], postprocess_fn(rgb_gt)
+  if config.eval_quantize_metrics:
+    rgbs = [np.round(x * 255) / 255 for x in rgbs]
+  if config.eval_crop_borders > 0:
+    c = config.eval_crop_borders
+    rgbs, rgb_gt = [x[c:-c, c:-c] for x in rgbs], rgb_gt[c:-c, c:-c]
+  return [metric_harness(x, rgb_gt) for x in rgbs]
+
+
 def evaluate(bundle, dataset, log=print, use_graph=True, summaries=None):
   """eval.py:44-257 for one checkpoint (`eval_only_once` semantics).  Returns (metrics, metrics_cc, step)."""
   config = bundle.config
@@ -80,14 +93,8 @@ def evaluate(bundle, dataset, log=print, use_graph=True, summaries=None):
       t1 = time.time()
       rendering['rgb_cc'] = cc_fun(rendering['rgb'], gt_rgb)
       log(f'Color corrected in {(time.time() - t1):0.3f}s')
-      rgb, rgb_cc, rgb_gt = postprocess_fn(rendering['rgb']), postprocess_fn(rendering['rgb_cc']), postprocess_fn(gt_rgb)
-      if config.eval_quantize_metrics:
-        rgb, rgb_cc = np.round(rgb * 255) / 255, np.round(rgb_cc * 255) / 255      # what the saved PNGs hold
-      if config.eval_crop_borders > 0:
-        c = config.eval_crop_borders
-        rgb, rgb_cc, rgb_gt = rgb[c:-c, c:-c], rgb_cc[c:-c, c:-c], rgb_gt[c:-c, c:-c]
-      metric = metric_harness(rgb, rgb_gt)
-      metric_cc = metric_harness(rgb_cc, rgb_gt)
+      metric, metric_cc = image_metrics(config, postprocess_fn, metric_harness, gt_rgb, rendering['rgb'],
+                                        rendering['rgb_cc'])
       if config.compute_disp_metrics and batch.disps is not None:
         for tag in ['mean', 'median']:
           key = f'distance_{tag}'

@@ -186,8 +186,11 @@ _SIGNATURES = {
     'mnrf_mesh_collapse_select': (C.c_int, [C.c_int32, C.c_int64, C.c_int64] + [_P] * 7),
     'mnrf_mesh_collapse_apply': (C.c_int, [C.c_int32, C.c_int64, C.c_int64] + [_P] * 13),
     'mnrf_mesh_texture_raster': (C.c_int, [C.c_int32, C.c_int64, _P, _P, _P, C.c_int32] + [_P] * 5),
+    'mnrf_mesh_bvh': (C.c_int, [C.c_int32, C.c_int32, C.c_int64] + [_P] * 12),
+    'mnrf_mesh_trace': (C.c_int, [C.c_int64] + [_P] * 4 + [C.c_int64] + [_P] * 9),
 }
 MC_COUNT, MC_EMIT = 0, 1
+BVH_BOXES, BVH_KEYS, BVH_TREE = 0, 1, 2
 HEAD_NONE, HEAD_FWD_SUB, HEAD_FWD_WARP, HEAD_BWD_SUB, HEAD_BWD_WARP = 0, 1, 2, 3, 4
 EXPORTED = tuple(_SIGNATURES)
 

@@ -18,6 +18,10 @@ the mean of the colours rendered for it across the views whose surface lies with
 Either method can clean the mesh (`clean_mesh`) and then simplify it to a face budget by quadric edge collapse
 (`simplify_mesh`) before any colour is computed, and then bake the colour into a texture atlas (`bake_texture`,
 `texture_size`) that `write_obj` stores as a textured OBJ with its MTL and PNG.
+
+`evaluate_mesh` (Config.mesh_eval) scores the result against the test views: it traces every test pixel's ray into
+the mesh on the GPU (`ops.mesh_bvh`, `ops.mesh_trace`, csrc/mesh_trace.cu), shades the hits (`render_mesh`) and
+compares them with the test images and with the NeRF's own depth and opacity on the same rays (`mesh_metrics`).
 """
 import math
 import os
@@ -150,7 +154,8 @@ def validate_config(bundle):
   """The mesh method of `bundle`'s Config, checked: 'density' or 'tsdf'; the TSDF method needs perspective or fisheye
   views (not NDC) and a truncation of at least one cell, so no cut edge of the fused grid has an unobserved end.
   The cleaning and simplification options must not be negative, and mesh_min_views projects into the views, so it
-  needs them not NDC either.  mesh_texture_size is 0 (off) or in [4, 16384]."""
+  needs them not NDC either.  mesh_texture_size is 0 (off) or in [4, 16384].  mesh_eval traces world-space
+  meshes along the test rays, so it needs them not NDC either."""
   config = bundle.config
   if config.mesh_method not in MESH_METHODS:
     raise ValueError(f'Config.mesh_method = {config.mesh_method!r}: want one of {MESH_METHODS}')
@@ -162,6 +167,9 @@ def validate_config(bundle):
     raise ValueError(f'Config.mesh_texture_size = {config.mesh_texture_size!r}: want 0 (off) or [{lo}, {hi}]')
   if config.mesh_min_views > 0 and config.forward_facing:
     raise ValueError('Config.mesh_min_views does not support forward-facing (NDC) scenes')
+  if config.mesh_eval and config.forward_facing:
+    raise ValueError('Config.mesh_eval does not support forward-facing (NDC) scenes: the mesh is in world space and '
+                     'NDC rays are not')
   if config.mesh_method == 'tsdf':
     if config.forward_facing:
       raise ValueError("Config.mesh_method = 'tsdf' does not support forward-facing (NDC) scenes")
@@ -492,6 +500,129 @@ def simplify_mesh(vertices, faces, normals=None, *, target_faces, stats=None):
   if stats is not None:
     stats.update(faces_after=F, rounds=rounds, target_reached=F <= target_faces + 1)
   return _drop_unused(v, f, *(() if n is None else (n,)))
+
+
+def render_mesh(vertices, faces, bvh, rays, *, normals=None, rgb=None, uv=None, texture=None, bg):
+  """The mesh seen along `rays` (a utils.Rays on the device, any leading shape): each ray's closest hit in
+  near <= t <= far (ops.mesh_trace on `bvh`, ops.mesh_bvh of vertices [V, 3] and faces [F, 3] int32).  Returns a dict
+  of tensors with the rays' leading shape: hit (bool), distance (t along the rays' directions, inf on a miss),
+  normals [..., 3] (the normalised barycentric blend of the vertex `normals` [V, 3]; where there are none or the blend
+  is zero, the face normal by its winding; 0 on a miss) and rgb [..., 3] fp32 or None.  rgb: with `texture` (uint8
+  [S, S, 3]) and `uv` ([F, 3, 2] texel units, bake_texture's), the atlas sampled bilinearly at the blend of the face's
+  corner UVs (texel centres at +0.5); else with `rgb` (uint8 [V, 3] vertex colours) their blend over 255; else None.
+  A miss gets the background `bg`.  A mesh without faces is all misses, and nothing is traced or gathered."""
+  shape = rays.origins.shape[:-1]
+  dev = rays.origins.device
+  coloured = texture is not None or rgb is not None
+  if faces.shape[0] == 0:
+    n = math.prod(shape)
+    out = dict(hit=torch.zeros(n, device=dev, dtype=torch.bool), distance=torch.full((n,), math.inf, device=dev),
+               normals=torch.zeros(n, 3, device=dev),
+               rgb=torch.full((n, 3), float(bg), device=dev) if coloured else None)
+    return {k: None if v is None else v.reshape(*shape, *v.shape[1:]) for k, v in out.items()}
+  flat = lambda x: torch.as_tensor(x, device=dev, dtype=torch.float32).reshape(-1, x.shape[-1]).contiguous()
+  face, t, bary = ops.mesh_trace(bvh, flat(rays.origins), flat(rays.directions), flat(rays.near), flat(rays.far))
+  hit = face >= 0
+  fi = face.clamp_min(0).long()                  # a miss reads face 0, which exists; its values are masked below
+  corners = faces.long()[fi]
+  w = torch.cat([1 - bary.sum(-1, keepdim=True), bary], -1)                        # [N, 3]
+  blend = lambda per_vertex: (w[..., None] * per_vertex[corners].float()).sum(1)
+  p = vertices[corners]
+  fn = torch.cross(p[:, 1] - p[:, 0], p[:, 2] - p[:, 0], dim=-1)
+  n = blend(normals) if normals is not None else torch.zeros_like(fn)
+  n = torch.where((n.norm(dim=-1, keepdim=True) > 0), n, fn)
+  n = torch.where(hit[:, None], n / n.norm(dim=-1, keepdim=True).clamp_min(1e-30), torch.zeros_like(n))
+  color = None
+  if texture is not None:
+    S = texture.shape[0]
+    st = (w[..., None] * uv[fi]).sum(1) - 0.5                                       # texel index space
+    x0 = st.floor()
+    frac = st - x0
+    x0 = x0.long()
+    tex = texture.reshape(-1, 3).float() / 255
+    color = torch.zeros(len(fi), 3, device=face.device)
+    for dy in (0, 1):
+      for dx in (0, 1):
+        cx = (x0[:, 0] + dx).clamp(0, S - 1)
+        cy = (x0[:, 1] + dy).clamp(0, S - 1)
+        wt = (frac[:, 0] if dx else 1 - frac[:, 0]) * (frac[:, 1] if dy else 1 - frac[:, 1])
+        color += wt[:, None] * tex[cy * S + cx]
+  elif rgb is not None:
+    color = blend(rgb) / 255
+  if color is not None:
+    color = torch.where(hit[:, None], color, torch.full_like(color, float(bg)))
+  out = dict(hit=hit, distance=t, normals=n, rgb=color)
+  return {k: None if v is None else v.reshape(*shape, *v.shape[1:]) for k, v in out.items()}
+
+
+def mesh_metrics(render, rgb_gt, config, postprocess_fn=lambda z: z, reference=None):
+  """Per-image metrics of a mesh render (render_mesh, [H, W] leading shape) against the test image rgb_gt [H, W, 3]:
+  psnr and ssim when the render has colour (eval_lib.image_metrics: RawNeRF postprocessing, 8-bit quantisation and
+  border crop as eval_lib.evaluate applies them).  reference (distance_median, acc, rgb) of the NeRF on the same rays
+  adds nerf_psnr and nerf_ssim, coverage (the fraction of pixels with acc >= 0.5 the mesh hits), spurious (the
+  fraction of mesh hits where acc < 0.5) and depth_abs_rel (the mean |t - distance_median| / distance_median over
+  pixels with both); a fraction with no pixel to count over is NaN."""
+  from . import eval_lib, image
+  host = lambda x: x.detach().cpu().numpy() if isinstance(x, torch.Tensor) else np.asarray(x)
+  harness = image.MetricHarness()
+  gt = np.asarray(rgb_gt, np.float64)
+  metric = {}
+  if render['rgb'] is not None:
+    metric.update(eval_lib.image_metrics(config, postprocess_fn, harness, gt, host(render['rgb']).astype(np.float64))[0])
+  if reference is not None:
+    dm, acc, nerf_rgb = (host(x).astype(np.float64) for x in reference)
+    dm, acc = dm.reshape(gt.shape[:2]), acc.reshape(gt.shape[:2])
+    m = eval_lib.image_metrics(config, postprocess_fn, harness, gt, nerf_rgb.reshape(gt.shape))[0]
+    metric.update(nerf_psnr=m['psnr'], nerf_ssim=m['ssim'])
+    hit = host(render['hit']).reshape(gt.shape[:2])
+    seen = acc >= 0.5
+    frac = lambda num, den: float(num) / float(den) if den else float('nan')
+    metric['coverage'] = frac((hit & seen).sum(), seen.sum())
+    metric['spurious'] = frac((hit & ~seen).sum(), hit.sum())
+    both = hit & seen
+    t = host(render['distance']).astype(np.float64).reshape(gt.shape[:2])
+    metric['depth_abs_rel'] = float((np.abs(t - dm) / dm)[both].mean()) if both.any() else float('nan')
+  return metric
+
+
+def evaluate_mesh(vertices, faces, dataset, config, *, normals=None, rgb=None, uv=None, texture=None,
+                  reference=None, bg=1.0, save_fn=None, timing=None):
+  """Scores a mesh against the test views of `dataset` (the test split, not NDC): builds the BVH once, renders every
+  view up to Config.eval_dataset_limit with render_mesh (normals, rgb, uv, texture and bg as it takes them) and
+  returns the per-image metrics of mesh_metrics, a list of dicts.  reference: an iterable of (idx, distance_median,
+  acc, rgb) of the NeRF on the same views, as render_views yields it.  save_fn(idx, render): called per view.
+  timing: a dict, given 'build' and 'trace' seconds (device-synchronised; tracing includes the shading)."""
+  import time
+  if dataset.cameras[3] is not None:
+    raise ValueError('evaluate_mesh does not support forward-facing (NDC) scenes: the mesh is in world space')
+  metadata = getattr(dataset, 'metadata', None)
+  postprocess_fn = metadata['postprocess_fn'] if (config.rawnerf_mode and metadata) else (lambda z: z)
+  num_eval = min(dataset.size, config.eval_dataset_limit)
+  torch.cuda.synchronize()
+  t0 = time.time()
+  bvh = ops.mesh_bvh(vertices, faces)
+  torch.cuda.synchronize()
+  times = dict(build=time.time() - t0, trace=0.0)
+  ref_iter = iter(reference) if reference is not None else None
+  metrics = []
+  for idx in range(num_eval):
+    ref = None
+    if ref_iter is not None:
+      ridx, dm, acc, nerf_rgb = next(ref_iter)
+      if ridx != idx:
+        raise ValueError(f'evaluate_mesh: reference view {ridx} where view {idx} was expected')
+      ref = (dm, acc, nerf_rgb)
+    t1 = time.time()
+    rays = dataset.generate_ray_batch(idx).rays
+    render = render_mesh(vertices, faces, bvh, rays, normals=normals, rgb=rgb, uv=uv, texture=texture, bg=bg)
+    torch.cuda.synchronize()
+    times['trace'] += time.time() - t1
+    metrics.append(mesh_metrics(render, dataset.images[idx], config, postprocess_fn, ref))
+    if save_fn is not None:
+      save_fn(idx, render)
+  if timing is not None:
+    timing.update(times)
+  return metrics
 
 
 def _clean_args(keep_components, min_views, dataset, stats):

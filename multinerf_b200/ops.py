@@ -6,6 +6,7 @@ volumetric_rendering, ...) but operate on flat [B, ...] CUDA tensors.
 """
 import ctypes as C
 import math
+from typing import NamedTuple
 
 import torch
 
@@ -345,6 +346,87 @@ def mesh_texture_raster(vertices, faces, normals, size):
     L.check(lib.mnrf_mesh_texture_raster(V, F, L.ptr(_f32(vertices)), L.ptr(faces), L.ptr(_f32(normals)), int(size),
                                          L.ptr(uv), L.ptr(index), L.ptr(points), L.ptr(tnormals), L.stream_ptr()))
   return uv, index, points, tnormals
+
+
+class MeshBVH(NamedTuple):
+  """A linear BVH over the faces of a mesh (mnrf_mesh_bvh, include/mnrf.h), with the mesh it was built on."""
+  vertices: torch.Tensor    # [V, 3] fp32
+  faces: torch.Tensor       # [F, 3] int32
+  nodes: torch.Tensor       # [max(F - 1, 0), 16] fp32: both children's boxes, then the children as int32 bits
+  parent: torch.Tensor      # [max(2 F - 1, 0)] int32, -1 at the root
+  leaf_face: torch.Tensor   # [F] int32: the face of each leaf, in key order
+  keys: torch.Tensor        # [F] int64, ascending: morton << 32 | face
+
+
+def mesh_bvh(vertices, faces):
+  """The linear BVH of a mesh on the device (mnrf_mesh_bvh, csrc/mesh_trace.cu) -> MeshBVH.  vertices [V, 3] fp32,
+  faces [F, 3] int32.  Checks on the device that every face index lies in [0, V) and every vertex is finite, and
+  reads that one flag back: either failure raises ValueError and never reaches a kernel; so does F >= 2^30.  No other
+  host synchronisation: the centroid bounds go to the key kernel by device pointer.  F = 0 gives an empty tree and
+  F = 1 a tree that is its leaf, with no launch."""
+  lib = L.load()
+  if vertices.dim() != 2 or vertices.shape[1] != 3 or faces.dim() != 2 or faces.shape[1] != 3:
+    raise ValueError(f'mesh_bvh: vertices {tuple(vertices.shape)}, faces {tuple(faces.shape)}: want [V, 3] and [F, 3]')
+  vertices, faces = _f32(vertices.contiguous()), _i32(faces.contiguous())
+  V, F = vertices.shape[0], faces.shape[0]
+  if not 0 <= V < 2 ** 31 or F >= 2 ** 30:
+    raise ValueError(f'mesh_bvh: {V} vertices, {F} faces: want V < 2^31 and F < 2^30')
+  dev = vertices.device
+  bad = ~torch.isfinite(vertices).all()
+  if F:
+    bad |= ((faces < 0) | (faces >= V)).any()
+  if bool(bad):
+    raise ValueError(f'mesh_bvh: a vertex is not finite or a face index lies outside [0, {V})')
+  i32 = lambda n: torch.empty(n, device=dev, dtype=torch.int32)
+  if F <= 1:
+    keys = torch.zeros(F, device=dev, dtype=torch.int64)
+    return MeshBVH(vertices, faces, torch.empty(0, 16, device=dev), torch.full((F,), -1, device=dev,
+                                                                               dtype=torch.int32),
+                   torch.zeros(F, device=dev, dtype=torch.int32), keys)
+  boxes = torch.empty(F, 6, device=dev)
+  centroids = torch.empty(F, 3, device=dev)
+  keys = torch.empty(F, device=dev, dtype=torch.int64)
+  args = [V, F, L.ptr(vertices), L.ptr(faces), L.ptr(boxes), L.ptr(centroids)]
+  _count(4)                                    # boxes, keys, then topology and box fit
+  L.check(lib.mnrf_mesh_bvh(L.BVH_BOXES, *args, None, None, None, None, None, None, None, L.stream_ptr()))
+  bounds = torch.cat([centroids.amin(0), centroids.amax(0)]).contiguous()
+  L.check(lib.mnrf_mesh_bvh(L.BVH_KEYS, *args, L.ptr(bounds), L.ptr(keys), None, None, None, None, None,
+                            L.stream_ptr()))
+  keys = torch.sort(keys).values
+  nodes = torch.empty(F - 1, 16, device=dev)
+  parent, leaf_face, counters = i32(2 * F - 1), i32(F), i32(F - 1)
+  L.check(lib.mnrf_mesh_bvh(L.BVH_TREE, *args, None, None, L.ptr(keys), L.ptr(nodes), L.ptr(parent),
+                            L.ptr(leaf_face), L.ptr(counters), L.stream_ptr()))
+  return MeshBVH(vertices, faces, nodes, parent, leaf_face, keys)
+
+
+def mesh_trace(bvh, origins, directions, near, far):
+  """The closest hit of each ray in the mesh of `bvh` (mnrf_mesh_trace, csrc/mesh_trace.cu): origins, directions
+  [N, 3], near, far [N] or [N, 1] fp32 on the device; only hits with near <= t <= far count.  Returns (face [N] int32,
+  -1 for a miss; t [N] fp32, inf for a miss; bary [N, 2] fp32, the barycentrics of corners faces[f, 1] and
+  faces[f, 2]).  Reads the traversal's error flag back once and raises RuntimeError if it is set."""
+  lib = L.load()
+  origins, directions = _f32(origins.contiguous()), _f32(directions.contiguous())
+  N = origins.shape[0]
+  near, far = (_f32(x.reshape(-1).contiguous()) for x in (near, far))
+  if origins.shape != (N, 3) or directions.shape != (N, 3) or near.shape[0] != N or far.shape[0] != N:
+    raise ValueError(f'mesh_trace: origins {tuple(origins.shape)}, directions {tuple(directions.shape)}, near '
+                     f'{tuple(near.shape)}, far {tuple(far.shape)}: want [N, 3], [N, 3], [N], [N]')
+  dev = origins.device
+  face = torch.full((N,), -1, device=dev, dtype=torch.int32)
+  t = torch.full((N,), float('inf'), device=dev)
+  bary = torch.zeros(N, 2, device=dev)
+  F = bvh.faces.shape[0]
+  if N == 0 or F == 0:
+    return face, t, bary
+  flag = torch.zeros(1, device=dev, dtype=torch.int32)
+  _count()
+  L.check(lib.mnrf_mesh_trace(N, L.ptr(origins), L.ptr(directions), L.ptr(near), L.ptr(far), F,
+                              L.ptr(bvh.nodes) if F > 1 else None, L.ptr(bvh.leaf_face), L.ptr(bvh.vertices),
+                              L.ptr(bvh.faces), L.ptr(face), L.ptr(t), L.ptr(bary), L.ptr(flag), L.stream_ptr()))
+  if int(flag.item()):
+    raise RuntimeError('mesh_trace: a ray overflowed the traversal stack (a BVH deeper than 63 levels)')
+  return face, t, bary
 
 
 def points_view_count(points, camtype, distortion_params, worldtocams, camtopixs, height, width):

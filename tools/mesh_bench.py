@@ -26,9 +26,15 @@
           the PNG alone; and mesh.extract_mesh at --extract_res^3 on the random-init 360.gin model with target_faces
           = --simplify_faces, without and with texture_size = --texture_extract_size (large enough for the mesh the
           simplification stalls at), alternated --reps times (not part of `all`);
+  trace:  ops.mesh_bvh (CUDA events around whole calls after one warm-up, and the peak device memory above the mesh)
+          and ops.mesh_trace rays/s (CUDA events over --trace_views 1560 x 1040 perspective views orbiting the
+          origin) on the 512^3 `mc` mesh simplified to --simplify_faces faces and on the 512^3 random-init 360.gin
+          extraction after mesh_target_faces = --simplify_faces (where the simplification stalls); and
+          mesh.evaluate_mesh on one such view of the 360.gin mesh with the NeRF's render_views as its reference,
+          split into NeRF rendering, BVH build and tracing with shading (not part of `all`);
   device: the card's name and power limit, read in the same run.
 
-  python tools/mesh_bench.py [--rows 8388608] [--extract_res 512] [--sections all|components|simplify|texture]
+  python tools/mesh_bench.py [--rows 8388608] [--extract_res 512] [--sections all|components|simplify|texture|trace]
                              [--out result.json]
 """
 import argparse
@@ -338,12 +344,99 @@ def bench_texture_section(model, bbox, level, args):
   return out
 
 
+def orbit_views(n, W=1560, H=1040, radius=2.5):
+  """(pixtocam [3, 3], camtoworlds [n, 3, 4]) of n perspective views on a circle around the origin, looking at it."""
+  from multinerf_b200 import camera_utils
+  p2c = camera_utils.get_pixtocam(0.5 * W / np.tan(0.5 * 0.9), W, H)
+  poses = []
+  for i in range(n):
+    a = 2 * np.pi * i / n
+    eye = np.array([radius * np.cos(a), radius * np.sin(a), 0.3 * radius])
+    z = eye / np.linalg.norm(eye)
+    x = np.cross([0, 0, 1.0], z)
+    x /= np.linalg.norm(x)
+    poses.append(np.concatenate([np.stack([x, np.cross(z, x), z], 1), eye[:, None]], 1))
+  return p2c, np.stack(poses)
+
+
+class _OrbitDataset:
+  """The little of a test split that mesh.evaluate_mesh and mesh.render_views read, for orbit_views."""
+
+  def __init__(self, n, W=1560, H=1040, near=0.2, far=1e6):
+    from multinerf_b200 import camera_utils, utils
+    self.p2c, self.poses = orbit_views(n, W, H)
+    self.size, self.W, self.H, self.near, self.far = n, W, H, near, far
+    self.cameras = (self.p2c, self.poses, None, None)
+    self.images = np.zeros((n, H, W, 3), np.float32)
+    self._cu, self._utils = camera_utils, utils
+
+  def generate_ray_batch(self, idx):
+    xs, ys = self._cu.pixel_coordinates(self.W, self.H)
+    meta = lambda v: np.full((self.H, self.W, 1), v, np.float32)
+    pixels = self._utils.Pixels(pix_x_int=xs, pix_y_int=ys, lossmult=meta(1.0), near=meta(self.near),
+                                far=meta(self.far), cam_idx=np.zeros((self.H, self.W, 1), np.int32))
+    return self._utils.Batch(rays=self._cu.cast_ray_batch((self.p2c, self.poses[idx], None, None), pixels))
+
+
+def bench_trace_mesh(name, v, f, views, reps):
+  torch.cuda.empty_cache()
+  ops.mesh_bvh(v, f)                                           # warm-up
+  torch.cuda.synchronize()
+  base = torch.cuda.memory_allocated()
+  torch.cuda.reset_peak_memory_stats()
+  ms = events(lambda: ops.mesh_bvh(v, f), reps)
+  bvh = ops.mesh_bvh(v, f)
+  torch.cuda.synchronize()
+  peak = torch.cuda.max_memory_allocated() - base
+  ds = _OrbitDataset(views)
+  rays = [ds.generate_ray_batch(i).rays for i in range(views)]
+  dev = lambda x: torch.as_tensor(x, device='cuda', dtype=torch.float32).reshape(-1, x.shape[-1]).contiguous()
+  flat = [(dev(r.origins), dev(r.directions), dev(r.near), dev(r.far)) for r in rays]
+  ops.mesh_trace(bvh, *flat[0])
+  n_rays = sum(x[0].shape[0] for x in flat)
+  hits = sum(int((ops.mesh_trace(bvh, *x)[0] >= 0).sum()) for x in flat)
+  it = iter(range(1 << 30))
+  trace_ms = events(lambda: ops.mesh_trace(bvh, *flat[next(it) % views]), reps * views)
+  return {'mesh': name, 'faces': int(f.shape[0]), 'build_ms': round(ms, 2), 'build_peak_mb': round(peak / 2 ** 20, 1),
+          'views': f'{views} x 1560 x 1040', 'hit_fraction': round(hits / n_rays, 3),
+          'trace_ms_per_view': round(trace_ms, 2), 'mrays_per_s': round(n_rays / views / (trace_ms * 1e-3) / 1e6, 1)}
+
+
+def bench_trace_section(model, bbox, level, args):
+  out = {'meshes': []}
+  v, f = ops.marching_cubes(sphere_noise(512), 0.0)
+  v, f = mesh.simplify_mesh(v * (2 / 511) - 1, f, target_faces=args.simplify_faces)     # grid units -> [-1, 1]^3
+  out['meshes'].append(bench_trace_mesh('mc 512^3 sphere + noise, simplified', v, f, args.trace_views, args.reps))
+  del v, f
+  torch.cuda.empty_cache()
+  v, f = mesh.extract_mesh(model, bbox, args.extract_res, level, target_faces=args.simplify_faces)
+  out['meshes'].append(bench_trace_mesh(f'360.gin random init, {args.extract_res}^3, target_faces '
+                                        f'{args.simplify_faces}', v, f, args.trace_views, args.reps))
+  ds = _OrbitDataset(1)
+  timing = {}
+  nerf = [0.0]
+
+  def reference():
+    for view in mesh.render_views(model, ds):
+      torch.cuda.synchronize()
+      yield view
+  t0 = time.perf_counter()
+  gen = reference()
+  first = next(gen)
+  nerf[0] = time.perf_counter() - t0
+  mesh.evaluate_mesh(v, f, ds, model.config, reference=[first], bg=1.0, timing=timing)
+  out['evaluate'] = {'views': '1 x 1560 x 1040', 'faces': int(f.shape[0]), 'nerf_render_s': round(nerf[0], 3),
+                     'build_s': round(timing['build'], 3), 'trace_and_shade_s': round(timing['trace'], 3)}
+  return out
+
+
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--rows', type=int, default=1 << 23)
   ap.add_argument('--reps', type=int, default=3)
   ap.add_argument('--extract_res', type=int, default=512)
-  ap.add_argument('--sections', default='all', choices=('all', 'components', 'simplify', 'texture'))
+  ap.add_argument('--sections', default='all', choices=('all', 'components', 'simplify', 'texture', 'trace'))
+  ap.add_argument('--trace_views', type=int, default=4)
   ap.add_argument('--simplify_faces', type=int, default=1_000_000)
   ap.add_argument('--texture_faces', type=int, default=1_000_000)
   ap.add_argument('--texture_launches', type=int, default=20)
@@ -352,7 +445,7 @@ def main():
   args = ap.parse_args()
   lib.require_device()
   res = {'device': device_info(), 'query': {}, 'mc': [], 'extract': None}
-  if args.sections in ('components', 'simplify', 'texture'):
+  if args.sections in ('components', 'simplify', 'texture', 'trace'):
     b = configs.bundle_360()
     model = models.Model(b)
     model.init(seed=0)
@@ -362,7 +455,7 @@ def main():
     del grid
     torch.cuda.empty_cache()
     section = {'components': bench_components_section, 'simplify': bench_simplify_section,
-               'texture': bench_texture_section}[args.sections]
+               'texture': bench_texture_section, 'trace': bench_trace_section}[args.sections]
     res = {'device': res['device'], 'level': level, args.sections: section(model, bbox, level, args),
            'device_after': device_info()}
     emit(res, args.out)
