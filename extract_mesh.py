@@ -16,6 +16,9 @@ Config.mesh_eval = True then scores the mesh against the test split (mesh.evalua
 test views for reference, traces every test pixel's ray into the mesh, shaded with the most detailed colour the run
 produced (the texture, else the vertex colours, else none), and writes mesh/eval_step_<step>/{color,normals}_NNN.png,
 distance_NNN.tiff and metric_<name>.txt (per-image values, space-separated).
+Config.mesh_space = 'contracted' puts the grid of either method in the contracted space of an unbounded scene
+(360.gin), so the background is meshed too: Config.mesh_bbox is then in contracted coordinates (default [-2, 2]^3),
+Config.mesh_level a density per unit of contracted length, and the outputs are still in world coordinates.
 One process on one GPU.
 """
 import dataclasses
@@ -74,7 +77,8 @@ def main(argv=None):
     os.makedirs(out_dir, exist_ok=True)
     mesh.write_ply(path, vertices, faces, *((normals, rgb) if config.mesh_vertex_colors else ()))
     print(f'{vertices.shape[0]} vertices, {faces.shape[0]} faces in {elapsed:.2f} s '
-          f'(grid {config.mesh_resolution} along the longest side of {bbox}, {what}) -> {path}', flush=True)
+          f'(grid {config.mesh_resolution} along the longest side of {bbox} in {config.mesh_space} space, {what}) -> '
+          f'{path}', flush=True)
     timing['t'] = time.time()
 
   texture = dict(texture_size=size, before_texture=save_ply) if size else {}
@@ -82,12 +86,12 @@ def main(argv=None):
     what = f'{dataset.size} views fused, truncation {config.mesh_tsdf_truncation} cells'
     vertices, faces, *extra = mesh.extract_mesh_tsdf(model, dataset, bbox, config.mesh_resolution,
                                                      config.mesh_tsdf_truncation, colors=config.mesh_vertex_colors,
-                                                     **clean, **texture)
+                                                     space=config.mesh_space, **clean, **texture)
   else:
     what = f'level {config.mesh_level}'
     vertices, faces, *extra = mesh.extract_mesh(model, bbox, config.mesh_resolution, config.mesh_level,
-                                                colors=config.mesh_vertex_colors, dataset=dataset, **clean,
-                                                **texture)
+                                                colors=config.mesh_vertex_colors, dataset=dataset,
+                                                space=config.mesh_space, **clean, **texture)
   if not size:
     save_ply(vertices, faces, *extra)
     if config.mesh_eval:

@@ -120,7 +120,12 @@ int mnrf_encode_points(const mnrf_encode_desc* d, const float* points, float var
 /* mnrf_encode_points plus the tangent rows d feature / d point (the input of the density-normal chain, as
  * mnrf_encode's tfeat_bf16): the same feature rows, and tfeat_bf16[dir * N + i, ld_tfeat] = d feat_i / d point_i[dir],
  * through the contraction and the dependence of its covariance on the mean when warp_contract.  var finite and
- * >= 0; ld_tfeat >= feat_cols, a multiple of 8, tfeat_bf16 16-byte aligned. */
+ * >= 0; ld_tfeat >= feat_cols, a multiple of 8, tfeat_bf16 16-byte aligned.
+ * warp_contract = 2 (here and in mnrf_encode_points; mnrf_encode takes 0 or 1): the points are already contracted
+ * (|p| < 2; meshes extracted in contracted space, multinerf_b200/mesh.py).  The Gaussians (p, var * I) are encoded as
+ * they are, so the feature rows are those of warp_contract = 0; the tangent rows are the derivatives with respect to
+ * the world point x = inv_contract(p) with the footprint held fixed in contracted space: mode 0's rows times
+ * J(x) = d contract / dx (symmetric), tfeat[dir] = sum_b d feat / d p_b J[b][dir]. */
 int mnrf_encode_points_tangent(const mnrf_encode_desc* d, const float* points, float var, const float* basis,
                                mnrf_bf16* feat_bf16, mnrf_bf16* tfeat_bf16, int32_t ld_tfeat, mnrf_stream stream);
 
@@ -658,6 +663,25 @@ int mnrf_tsdf_integrate(const mnrf_camera_desc* cam, int32_t nx, int32_t ny, int
                         const float* worldtocams, const float* camtopixs, const float* depth, const float* acc,
                         const float* rgb, float tau, float* tsdf, float* weight, float* color_sum,
                         float* color_weight, mnrf_stream stream);
+
+/* mnrf_tsdf_integrate on a grid in the contracted space of an unbounded scene (coord.contract; Config.mesh_space =
+ * 'contracted'), with the same arguments, state and rules except: lo, h and tau are in contracted units; a grid point p
+ * with |p| >= 2 (no world preimage) is left untouched, so its weight stays 0; the other points are projected at
+ * x = inv_contract(p), and where acc >= 0.5, d = sign(depth - t) |contract(s) - p| with s = o + (x - o) depth / t the
+ * pixel's surface point on the ray through x (o: the camera centre of the view's worldtocam). */
+int mnrf_tsdf_integrate_contracted(const mnrf_camera_desc* cam, int32_t nx, int32_t ny, int32_t nz, double x0,
+                                   double y0, double z0, double h, int32_t num_views, int32_t height, int32_t width,
+                                   const float* worldtocams, const float* camtopixs, const float* depth,
+                                   const float* acc, const float* rgb, float tau, float* tsdf, float* weight,
+                                   float* color_sum, float* color_weight, mnrf_stream stream);
+
+/* A mesh extracted in contracted space, back to world space: world_points[i] = inv_contract(points[i]) (z inside the
+ * unit ball, z / (r (2 - r)) with r = |z| outside; |z| < 2 for a finite result), points [n, 3] fp32.  normals [n, 3] or
+ * NULL (then world_normals NULL too): level-set normals in contracted space; world_normals[i] is the unit vector
+ * along J(x) normals[i], J = d contract / dx at x = world_points[i] (symmetric: a gradient's pullback), or, where
+ * that is zero or not finite, along normals[i], else (0, 0, 1). */
+int mnrf_mesh_uncontract(int64_t n, const float* points, const float* normals, float* world_points,
+                         float* world_normals, mnrf_stream stream);
 
 /* Connected components of a triangle mesh (mesh cleaning, mesh.clean_mesh): the graph whose nodes are the
  * num_vertices vertices and whose edges are the edges of the num_faces faces [num_faces, 3] int32.  Every index must

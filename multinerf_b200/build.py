@@ -31,7 +31,8 @@ def _nvcc():
 
 
 # sources a unit includes besides the shared headers
-INCLUDES = {'gemm_tc_act.cu': ['gemm_tc.cu'], 'mesh.cu': ['mc_tables.cuh', 'camera.cuh'], 'camera.cu': ['camera.cuh']}
+INCLUDES = {'gemm_tc_act.cu': ['gemm_tc.cu'], 'mesh.cu': ['mc_tables.cuh', 'camera.cuh', 'contract.cuh'],
+            'camera.cu': ['camera.cuh'], 'encode.cu': ['contract.cuh']}
 
 
 def _stamp(path, flags):

@@ -146,6 +146,13 @@ class Config:
   # coverage, spurious hits and depth error against the NeRF's own renders) to <checkpoint_dir>/mesh/eval_step_<step>.
   # Not for forward-facing (NDC) scenes.
   mesh_eval: bool = False
+  # the space of the extraction grid: 'world', or 'contracted' for unbounded scenes under the scene contraction
+  # (coord.contract; not NDC): the grid then lies in contracted coordinates, so the background is meshed too.  There,
+  # mesh_bbox is read in contracted coordinates (None: [-2, 2]^3, all of contracted space; a grid of
+  # mesh_resolution points over it has half the foreground resolution of the world default), mesh_level is a
+  # density per unit of contracted length (the same inside the unit ball), and the TSDF band is in contracted cells.
+  # Meshes are written in world coordinates either way.
+  mesh_space: str = 'world'
 
 
 @dataclasses.dataclass

@@ -13,6 +13,7 @@
 #include <cmath>
 
 #include "common.cuh"
+#include "contract.cuh"
 
 namespace mnrf {
 
@@ -323,9 +324,30 @@ encode_kernel(mnrf_encode_desc d, const float* __restrict__ sdist,
   }
 }
 
+// Phase A of the point encoder for a Gaussian whose mean is already a contracted point p (warp_contract 2): the
+// Gaussian is stored as it is, and the terms of the tangent rows are those of the contraction at x = inv_contract(p)
+// with s_r = q_r = 0, so phase B writes d feature / d p times J(x) = d feature / d x with the footprint held fixed in
+// contracted space: the lifted variance does not move.
+__device__ __forceinline__ void store_contracted_gauss(const Gauss& g, float* gp) {
+  float x[3], s, q, xh[3];
+  inv_contract_point(g.mean, x);
+  contract_jacobian(x, s, q, xh);
+#pragma unroll
+  for (int i = 0; i < 3; ++i) gp[12 + i] = xh[i];
+  gp[15] = g.cov[0][0]; gp[16] = g.cov[0][1]; gp[17] = g.cov[0][2];
+  gp[18] = g.cov[1][1]; gp[19] = g.cov[1][2]; gp[20] = g.cov[2][2];
+  gp[21] = s; gp[22] = q; gp[23] = 0.f; gp[24] = 0.f;
+  gp[0] = g.mean[0]; gp[1] = g.mean[1]; gp[2] = g.mean[2];
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) gp[3 + i * 3 + j] = g.cov[i][j];
+}
+
 // Point form with tangent rows: the Gaussian of point i has mean points[i] and covariance var * I.  One warp takes
 // 32 points at a time, one lane per point in phase A, then the general encoder's phase B point by point.
-template <bool Contract>
+// Contracted (with Contract): the points are already contracted (store_contracted_gauss).
+template <bool Contract, bool Contracted = false>
 __global__ void __launch_bounds__(256)
 encode_points_tangent_kernel(mnrf_encode_desc d, const float* __restrict__ points, float var,
                              const float* __restrict__ basis, __nv_bfloat16* __restrict__ feat,
@@ -368,7 +390,10 @@ encode_points_tangent_kernel(mnrf_encode_desc d, const float* __restrict__ point
 #pragma unroll
         for (int j = 0; j < 3; ++j) ga.cov[i][j] = i == j ? var : 0.f;
       }
-      store_gauss<Contract>(d, ga, gs + lane * stride);
+      if (Contracted)
+        store_contracted_gauss(ga, gs + lane * stride);
+      else
+        store_gauss<Contract>(d, ga, gs + lane * stride);
     }
     __syncwarp();
     for (int s = 0; s < g; ++s)
@@ -668,6 +693,8 @@ extern "C" int mnrf_encode(const mnrf_encode_desc* d, const float* sdist, const 
   }
   MNRF_CHECK(d->ray_shape == MNRF_RAY_CONE || d->ray_shape == MNRF_RAY_CYLINDER,
              "ray_shape must be 'cone' or 'cylinder'");
+  MNRF_CHECK(d->warp_contract == 0 || d->warp_contract == 1, "mnrf_encode: warp_contract %d: want 0 or 1",
+             d->warp_contract);
   const int KL2 = 2 * d->basis_k * (d->max_deg - d->min_deg);
   MNRF_CHECK(d->feat_cols >= KL2 && d->ld_feat >= d->feat_cols, "mnrf_encode: feat_cols %d < 2KL %d or ld %d",
              d->feat_cols, KL2, d->ld_feat);
@@ -726,6 +753,10 @@ extern "C" int mnrf_encode_points(const mnrf_encode_desc* d, const float* points
              "mnrf_encode_points: num_samples must be 1 and raydist_fn, ray_shape 0 (got %d, %d, %d)",
              d->num_samples, d->raydist_fn, d->ray_shape);
   MNRF_CHECK(var >= 0.f, "mnrf_encode_points: var %g < 0", var);
+  MNRF_CHECK(d->warp_contract >= 0 && d->warp_contract <= 2, "mnrf_encode_points: warp_contract %d: want 0, 1 or 2",
+             d->warp_contract);
+  mnrf_encode_desc dd = *d;
+  if (dd.warp_contract == 2) dd.warp_contract = 0;      // already contracted: the feature rows of mode 0
   MNRF_CHECK(d->basis_k > 0 && d->max_deg > d->min_deg, "mnrf_encode_points: empty encoding");
   const int KL2 = 2 * d->basis_k * (d->max_deg - d->min_deg);
   MNRF_CHECK(d->feat_cols >= KL2 && d->ld_feat >= d->feat_cols, "mnrf_encode_points: feat_cols %d < 2KL %d or ld %d",
@@ -742,7 +773,7 @@ extern "C" int mnrf_encode_points(const mnrf_encode_desc* d, const float* points
   const int64_t groups = ((int64_t)d->num_rays + G - 1) / G;
   const int blocks = (int)std::min<int64_t>((groups + nw - 1) / nw, (int64_t)mnrf_num_sms() * 8);
   encode_points_kernel<<<blocks, nw * 32, smem, (cudaStream_t)stream>>>(
-      *d, G, points, var, basis, reinterpret_cast<__nv_bfloat16*>(feat_bf16), feat_f32);
+      dd, G, points, var, basis, reinterpret_cast<__nv_bfloat16*>(feat_bf16), feat_f32);
   MNRF_LAUNCH_CHECK();
   return 0;
 }
@@ -767,6 +798,8 @@ extern "C" int mnrf_encode_points_tangent(const mnrf_encode_desc* d, const float
              "mnrf_encode_points_tangent: feature rows must be 16-byte aligned");
   MNRF_CHECK(ld_tfeat >= d->feat_cols && ld_tfeat % 8 == 0 && ((uintptr_t)tfeat_bf16 % 16) == 0,
              "mnrf_encode_points_tangent: tangent rows must be 16-byte aligned");
+  MNRF_CHECK(d->warp_contract >= 0 && d->warp_contract <= 2,
+             "mnrf_encode_points_tangent: warp_contract %d: want 0, 1 or 2", d->warp_contract);
   const int nw = 8;
   const bool contract = d->warp_contract != 0;
   const int stride = contract ? kContractStride : kGaussStride;
@@ -774,7 +807,9 @@ extern "C" int mnrf_encode_points_tangent(const mnrf_encode_desc* d, const float
   const size_t smem = (((size_t)(3 * d->basis_k + nw * (32 * stride + (contract ? 8 : 2) * d->basis_k)) * 4 + 15) /
                        16) * 16 + (size_t)nw * 4 * row_bytes;
   MNRF_CHECK(smem <= 200 * 1024, "mnrf_encode_points_tangent: shared memory %zu too large", smem);
-  auto kernel = contract ? encode_points_tangent_kernel<true> : encode_points_tangent_kernel<false>;
+  auto kernel = d->warp_contract == 2 ? encode_points_tangent_kernel<true, true>
+              : contract              ? encode_points_tangent_kernel<true>
+                                      : encode_points_tangent_kernel<false>;
   MNRF_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int64_t groups = ((int64_t)d->num_rays + 31) / 32;
   const int blocks = (int)std::min<int64_t>((groups + nw - 1) / nw, (int64_t)mnrf_num_sms() * 8);

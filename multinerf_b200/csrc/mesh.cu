@@ -17,6 +17,9 @@
 //
 // Also the TSDF fusion of rendered depth maps (tsdf_integrate_kernel): one thread per grid point, its running
 // truncated signed distance, weight and colour sums held in registers across every view of a launch.
+// With kContract, the grid lies in the contracted space of an unbounded scene (coord.contract): each point is
+// projected at its world preimage, and its signed distance is measured in contracted space.  uncontract_kernel maps
+// the vertices and normals of a mesh extracted there back to world space.
 //
 // And the two passes of mesh cleaning: connected components by union-find (uf_*_kernel) and the number of views
 // each vertex lands in (points_view_count_kernel); mesh simplification by quadric edge collapse (qem_*_kernel); and
@@ -27,6 +30,7 @@
 #include <cuda/atomic>
 
 #include "camera.cuh"
+#include "contract.cuh"
 #include "mc_tables.cuh"
 
 namespace mnrf {
@@ -242,7 +246,12 @@ struct TsdfArgs {
 // pixel's colour into the colour sums.  No atomics: the state of a point depends on the views and their order only,
 // not on how they are split into launches.  Per point and view: 8 B of depth and acc (+ 12 B of rgb) gathered from
 // L2; per point: 8 B (+ 16 B) of state read and written once.
-template <bool kColor>
+//
+// kContract: the grid points p lie in contracted space.  A point with |p| >= 2 has no world preimage and is left
+// untouched (weight 0: unobserved).  Otherwise x = inv_contract(p) is projected; the pixel's surface point on the ray
+// through x is s = o + (x - o) depth / t (o: the camera centre of w2c), and d = sign(depth - t) |contract(s) - p|,
+// the distance in contracted space, with tau in contracted units.
+template <bool kColor, bool kContract = false>
 __global__ void __launch_bounds__(256)
 tsdf_integrate_kernel(const TsdfArgs a) {
   const float tau = a.tau;
@@ -252,6 +261,15 @@ tsdf_integrate_kernel(const TsdfArgs a) {
     const int z = (int)(row / a.ny);
     const int y = (int)(row - (int64_t)z * a.ny);
     const V3 pt{(float)(a.x0 + (double)x * a.h), (float)(a.y0 + (double)y * a.h), (float)(a.z0 + (double)z * a.h)};
+    V3 pw = pt;
+    if (kContract) {
+      if (!(pt.x * pt.x + pt.y * pt.y + pt.z * pt.z < 4.f)) continue;
+      const float zc[3] = {pt.x, pt.y, pt.z};
+      float xw[3];
+      inv_contract_point(zc, xw);
+      if (!(isfinite(xw[0]) && isfinite(xw[1]) && isfinite(xw[2]))) continue;     // |p| rounds to 2
+      pw = V3{xw[0], xw[1], xw[2]};
+    }
     float s = a.tsdf[p], w = a.weight[p];
     float c0 = 0.f, c1 = 0.f, c2 = 0.f, cw = 0.f;
     if (kColor) {
@@ -261,13 +279,32 @@ tsdf_integrate_kernel(const TsdfArgs a) {
     for (int k = 0; k < a.num_views; ++k) {
       int px, py;
       float t;
-      if (!project_to_pixel(a.cam, a.w2c + 12 * (int64_t)k, a.c2p + a.c2p_stride * k, pt, a.width, a.height, px, py,
+      if (!project_to_pixel(a.cam, a.w2c + 12 * (int64_t)k, a.c2p + a.c2p_stride * k, pw, a.width, a.height, px, py,
                             t))
         continue;
       const int64_t i = ((int64_t)k * a.height + py) * a.width + px;
       const float dep = __ldg(a.depth + i);
       if (!isfinite(dep)) continue;
-      const float d = __ldg(a.acc + i) >= 0.5f ? dep - t : INFINITY;
+      float d;
+      if (!kContract) {
+        d = __ldg(a.acc + i) >= 0.5f ? dep - t : INFINITY;
+      } else if (__ldg(a.acc + i) >= 0.5f) {
+        const float* m = a.w2c + 12 * (int64_t)k;
+        const float f = dep / t;
+        const float xw[3] = {pw.x, pw.y, pw.z};
+        float sp[3], sc[3];
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+          const float o = -(m[j] * m[3] + m[4 + j] * m[7] + m[8 + j] * m[11]);     // o = -R^T t
+          sp[j] = o + (xw[j] - o) * f;
+        }
+        contract_point(sp, sc);
+        const float e0 = sc[0] - pt.x, e1 = sc[1] - pt.y, e2 = sc[2] - pt.z;
+        const float dist = sqrtf(e0 * e0 + e1 * e1 + e2 * e2);
+        d = dep >= t ? dist : -dist;
+      } else {
+        d = INFINITY;
+      }
       if (d < -tau) continue;
       s = (w * s + fminf(d, tau) / tau) / (w + 1.f);
       w = w + 1.f;
@@ -284,6 +321,44 @@ tsdf_integrate_kernel(const TsdfArgs a) {
       a.color_sum[3 * p] = c0; a.color_sum[3 * p + 1] = c1; a.color_sum[3 * p + 2] = c2;
       a.color_weight[p] = cw;
     }
+  }
+}
+
+// Contracted mesh -> world: x = inv_contract(p) per point and, with normals, the unit world normal J(x) n of each
+// contracted level-set normal n (a gradient's pullback through y = contract(x), J symmetric).  J n is scaled by its
+// largest component before it is squared, as mc_normals_kernel scales; a zero or non-finite J n (n zero, or |p| so
+// close to 2 that x overflows) falls back to n itself, then to (0, 0, 1).
+__device__ __forceinline__ bool unit_normal(float v[3]) {
+  const float m = fmaxf(fabsf(v[0]), fmaxf(fabsf(v[1]), fabsf(v[2])));
+  if (!(m > 0.f && isfinite(m))) return false;
+#pragma unroll
+  for (int i = 0; i < 3; ++i) v[i] = v[i] / m;
+  const float len = sqrtf(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+#pragma unroll
+  for (int i = 0; i < 3; ++i) v[i] = v[i] / len;
+  return true;
+}
+
+__global__ void __launch_bounds__(256)
+uncontract_kernel(int64_t n, const float* __restrict__ points, const float* __restrict__ normals,
+                  float* __restrict__ world_points, float* __restrict__ world_normals) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const float z[3] = {points[3 * i], points[3 * i + 1], points[3 * i + 2]};
+    float x[3];
+    inv_contract_point(z, x);
+#pragma unroll
+    for (int j = 0; j < 3; ++j) world_points[3 * i + j] = x[j];
+    if (!normals) continue;
+    float s, q, xh[3], nw[3];
+    contract_jacobian(x, s, q, xh);
+    const float nc[3] = {normals[3 * i], normals[3 * i + 1], normals[3 * i + 2]};
+    contract_jacobian_apply(s, q, xh, nc, nw);
+    if (!unit_normal(nw)) {
+      nw[0] = nc[0]; nw[1] = nc[1]; nw[2] = nc[2];
+      if (!unit_normal(nw)) { nw[0] = 0.f; nw[1] = 0.f; nw[2] = 1.f; }
+    }
+#pragma unroll
+    for (int j = 0; j < 3; ++j) world_normals[3 * i + j] = nw[j];
   }
 }
 
@@ -804,39 +879,77 @@ extern "C" int mnrf_mc_normals(int32_t nx, int32_t ny, int32_t nz, const float* 
   return 0;
 }
 
-extern "C" int mnrf_tsdf_integrate(const mnrf_camera_desc* cam, int32_t nx, int32_t ny, int32_t nz, double x0,
-                                   double y0, double z0, double h, int32_t num_views, int32_t height, int32_t width,
-                                   const float* worldtocams, const float* camtopixs, const float* depth,
-                                   const float* acc, const float* rgb, float tau, float* tsdf, float* weight,
-                                   float* color_sum, float* color_weight, mnrf_stream stream) {
-  using namespace mnrf;
+namespace mnrf {
+namespace {
+// Both TSDF entry points: checks (messages under `name`) and the launch of the kContract instance.
+template <bool kContract>
+int tsdf_integrate(const char* name, const mnrf_camera_desc* cam, int32_t nx, int32_t ny, int32_t nz, double x0,
+                   double y0, double z0, double h, int32_t num_views, int32_t height, int32_t width,
+                   const float* worldtocams, const float* camtopixs, const float* depth, const float* acc,
+                   const float* rgb, float tau, float* tsdf, float* weight, float* color_sum, float* color_weight,
+                   mnrf_stream stream) {
   set_error("");
-  MNRF_CHECK(cam, "mnrf_tsdf_integrate: null camera descriptor");
+  MNRF_CHECK(cam, "%s: null camera descriptor", name);
   MNRF_CHECK(nx >= 2 && ny >= 2 && nz >= 2 && nx <= kMcMaxDim && ny <= kMcMaxDim && nz <= kMcMaxDim,
-             "mnrf_tsdf_integrate: grid %d x %d x %d (nz x ny x nx), each side must be in [2, %d]", nz, ny, nx,
-             kMcMaxDim);
-  MNRF_CHECK(num_views >= 0 && height >= 1 && width >= 1, "mnrf_tsdf_integrate: %d views of %d x %d pixels",
+             "%s: grid %d x %d x %d (nz x ny x nx), each side must be in [2, %d]", name, nz, ny, nx, kMcMaxDim);
+  MNRF_CHECK(num_views >= 0 && height >= 1 && width >= 1, "%s: %d views of %d x %d pixels", name,
              num_views, height, width);
   MNRF_CHECK(cam->camtype == MNRF_CAM_PERSPECTIVE || cam->camtype == MNRF_CAM_FISHEYE,
-             "mnrf_tsdf_integrate: camtype must be perspective or fisheye");
-  MNRF_CHECK(!cam->has_ndc, "mnrf_tsdf_integrate: NDC cameras are not supported");
+             "%s: camtype must be perspective or fisheye", name);
+  MNRF_CHECK(!cam->has_ndc, "%s: NDC cameras are not supported", name);
   MNRF_CHECK(cam->num_cameras == 1 || cam->num_cameras == num_views,
-             "mnrf_tsdf_integrate: num_cameras = %d camera-to-pixel matrices for %d views", cam->num_cameras,
-             num_views);
-  MNRF_CHECK(tau > 0.f && isfinite(tau) && h > 0.0 && isfinite(h), "mnrf_tsdf_integrate: tau %g, h %g", tau, h);
-  MNRF_CHECK(tsdf && weight, "mnrf_tsdf_integrate: null state pointer");
+             "%s: num_cameras = %d camera-to-pixel matrices for %d views", name, cam->num_cameras, num_views);
+  MNRF_CHECK(tau > 0.f && isfinite(tau) && h > 0.0 && isfinite(h), "%s: tau %g, h %g", name, tau, h);
+  MNRF_CHECK(tsdf && weight, "%s: null state pointer", name);
   MNRF_CHECK(!rgb == !color_sum && !color_sum == !color_weight,
-             "mnrf_tsdf_integrate: rgb, color_sum and color_weight go together");
+             "%s: rgb, color_sum and color_weight go together", name);
   if (num_views == 0) return 0;
-  MNRF_CHECK(worldtocams && camtopixs && depth && acc, "mnrf_tsdf_integrate: null view pointer");
+  MNRF_CHECK(worldtocams && camtopixs && depth && acc, "%s: null view pointer", name);
   TsdfArgs a{*cam, nx, ny, nz, (int64_t)nx * ny * nz, x0, y0, z0, h, num_views, height, width, tau,
              worldtocams, camtopixs, cam->num_cameras == 1 ? 0 : 9, depth, acc, rgb, tsdf, weight, color_sum,
              color_weight};
   const int blocks = (int)std::min<int64_t>((a.n + 255) / 256, (int64_t)mnrf_num_sms() * 16);
   if (rgb)
-    tsdf_integrate_kernel<true><<<blocks, 256, 0, (cudaStream_t)stream>>>(a);
+    tsdf_integrate_kernel<true, kContract><<<blocks, 256, 0, (cudaStream_t)stream>>>(a);
   else
-    tsdf_integrate_kernel<false><<<blocks, 256, 0, (cudaStream_t)stream>>>(a);
+    tsdf_integrate_kernel<false, kContract><<<blocks, 256, 0, (cudaStream_t)stream>>>(a);
+  MNRF_LAUNCH_CHECK();
+  return 0;
+}
+}  // namespace
+}  // namespace mnrf
+
+extern "C" int mnrf_tsdf_integrate(const mnrf_camera_desc* cam, int32_t nx, int32_t ny, int32_t nz, double x0,
+                                   double y0, double z0, double h, int32_t num_views, int32_t height, int32_t width,
+                                   const float* worldtocams, const float* camtopixs, const float* depth,
+                                   const float* acc, const float* rgb, float tau, float* tsdf, float* weight,
+                                   float* color_sum, float* color_weight, mnrf_stream stream) {
+  return mnrf::tsdf_integrate<false>("mnrf_tsdf_integrate", cam, nx, ny, nz, x0, y0, z0, h, num_views, height,
+                                    width, worldtocams, camtopixs, depth, acc, rgb, tau, tsdf, weight,
+                                    color_sum, color_weight, stream);
+}
+
+extern "C" int mnrf_tsdf_integrate_contracted(const mnrf_camera_desc* cam, int32_t nx, int32_t ny, int32_t nz,
+                                              double x0, double y0, double z0, double h, int32_t num_views,
+                                              int32_t height, int32_t width, const float* worldtocams,
+                                              const float* camtopixs, const float* depth, const float* acc,
+                                              const float* rgb, float tau, float* tsdf, float* weight,
+                                              float* color_sum, float* color_weight, mnrf_stream stream) {
+  return mnrf::tsdf_integrate<true>("mnrf_tsdf_integrate_contracted", cam, nx, ny, nz, x0, y0, z0, h, num_views,
+                                    height, width, worldtocams, camtopixs, depth, acc, rgb, tau, tsdf, weight,
+                                    color_sum, color_weight, stream);
+}
+
+extern "C" int mnrf_mesh_uncontract(int64_t n, const float* points, const float* normals, float* world_points,
+                                    float* world_normals, mnrf_stream stream) {
+  using namespace mnrf;
+  set_error("");
+  MNRF_CHECK(n >= 0, "mnrf_mesh_uncontract: %lld points", (long long)n);
+  MNRF_CHECK(!normals == !world_normals, "mnrf_mesh_uncontract: normals and world_normals go together");
+  if (n == 0) return 0;
+  MNRF_CHECK(points && world_points, "mnrf_mesh_uncontract: null pointer");
+  const int blocks = (int)std::min<int64_t>((n + 255) / 256, (int64_t)mnrf_num_sms() * 16);
+  uncontract_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(n, points, normals, world_points, world_normals);
   MNRF_LAUNCH_CHECK();
   return 0;
 }

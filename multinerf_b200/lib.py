@@ -178,6 +178,9 @@ _SIGNATURES = {
     'mnrf_mc_normals': (C.c_int, [C.c_int32] * 3 + [_P, C.c_float] + [_P] * 4),
     'mnrf_tsdf_integrate': (C.c_int, [C.POINTER(CameraDesc)] + [C.c_int32] * 3 + [C.c_double] * 4 + [C.c_int32] * 3 +
                             [_P] * 5 + [C.c_float] + [_P] * 5),
+    'mnrf_tsdf_integrate_contracted': (C.c_int, [C.POINTER(CameraDesc)] + [C.c_int32] * 3 + [C.c_double] * 4 +
+                                       [C.c_int32] * 3 + [_P] * 5 + [C.c_float] + [_P] * 5),
+    'mnrf_mesh_uncontract': (C.c_int, [C.c_int64] + [_P] * 5),
     'mnrf_mesh_components': (C.c_int, [C.c_int32, C.c_int64, _P, _P, _P]),
     'mnrf_points_view_count': (C.c_int, [C.POINTER(CameraDesc), C.c_int64, _P, C.c_int32, C.c_int32, C.c_int32,
                                          _P, _P, _P, _P]),

@@ -19,6 +19,15 @@ Either method can clean the mesh (`clean_mesh`) and then simplify it to a face b
 (`simplify_mesh`) before any colour is computed, and then bake the colour into a texture atlas (`bake_texture`,
 `texture_size`) that `write_obj` stores as a textured OBJ with its MTL and PNG.
 
+Both methods can also work in the contracted space of an unbounded scene (`space='contracted'`,
+Config.mesh_space): the grid then spans the model's contracted coordinates (coord.contract; the open ball of radius
+2 holds the whole world), so the background becomes faces at the resolution the model itself has there.  Grid points
+with |p| >= 2 have no world preimage: they are NaN and never queried.  The density grid holds the density per unit
+of contracted length (Model.query_density(contracted=True)), the TSDF measures distances in contracted space
+(ops.tsdf_integrate(contracted=True)), cleaning projects world positions, simplification runs on the contracted
+mesh, and the result is mapped to world space (ops.mesh_uncontract: vertices, and normals through the contraction's
+Jacobian) before colours are queried.  Outputs are always in world coordinates.
+
 `evaluate_mesh` (Config.mesh_eval) scores the result against the test views: it traces every test pixel's ray into
 the mesh on the GPU (`ops.mesh_bvh`, `ops.mesh_trace`, csrc/mesh_trace.cu), shades the hits (`render_mesh`) and
 compares them with the test images and with the NeRF's own depth and opacity on the same rays (`mesh_metrics`).
@@ -33,11 +42,17 @@ import torch
 from . import ops
 
 
+MESH_SPACES = ('world', 'contracted')
+
+
 def default_bbox(bundle):
   """Config.mesh_bbox, or the default box of the scene family: [-1, 1]^3 under the scene contraction (the cube
   around the unit ball, inside which the contraction is the identity), [-1.5, 1.5]^3 for a bounded scene.
-  Forward-facing scenes live in NDC space, where no default box means anything: they need Config.mesh_bbox."""
+  Forward-facing scenes live in NDC space, where no default box means anything: they need Config.mesh_bbox.
+  With Config.mesh_space = 'contracted' the box is in contracted coordinates, and the default [-2, 2]^3 holds all of
+  contracted space."""
   config = bundle.config
+  _check_space(bundle)
   if config.mesh_bbox is not None:
     bbox = tuple(float(v) for v in config.mesh_bbox)
     if len(bbox) != 6:
@@ -45,8 +60,29 @@ def default_bbox(bundle):
     return bbox
   if config.forward_facing:
     raise ValueError('forward-facing (NDC) scenes have no default mesh box: set Config.mesh_bbox')
-  r = 1.0 if bundle.nerf_mlp.warp_fn == 'contract' else 1.5
+  r = 2.0 if config.mesh_space == 'contracted' else 1.0 if bundle.nerf_mlp.warp_fn == 'contract' else 1.5
   return (-r, -r, -r, r, r, r)
+
+
+def _check_space(bundle):
+  """Config.mesh_space, checked: 'world' or 'contracted'; 'contracted' needs the final MLP under the scene
+  contraction and a scene that is not forward-facing (NDC)."""
+  config = bundle.config
+  if config.mesh_space not in MESH_SPACES:
+    raise ValueError(f'Config.mesh_space = {config.mesh_space!r}: want one of {MESH_SPACES}')
+  if config.mesh_space == 'contracted':
+    if bundle.nerf_mlp.warp_fn != 'contract':
+      raise ValueError("Config.mesh_space = 'contracted' needs the scene contraction (NerfMLP.warp_fn = "
+                       "@coord.contract)")
+    if config.forward_facing:
+      raise ValueError("Config.mesh_space = 'contracted' does not support forward-facing (NDC) scenes")
+  return config.mesh_space
+
+
+def _contracted(space):
+  if space not in MESH_SPACES:
+    raise ValueError(f'mesh space {space!r}: want one of {MESH_SPACES}')
+  return space == 'contracted'
 
 
 def grid_shape(bbox, resolution):
@@ -63,9 +99,12 @@ def grid_shape(bbox, resolution):
   return tuple(n), h
 
 
-def density_grid(model, bbox, resolution, slab_planes=None):
+def density_grid(model, bbox, resolution, slab_planes=None, space='world'):
   """The density of `model`'s final level at the grid points of `bbox` -> (grid [nz, ny, nx] fp32 on the device,
-  h).  Evaluated `slab_planes` z-planes at a time (default: about one query chunk of rows per slab)."""
+  h).  Evaluated `slab_planes` z-planes at a time (default: about one query chunk of rows per slab).
+  space 'contracted': the grid lies in contracted coordinates and holds Model.query_density(contracted=True), the
+  density per unit of contracted length; points with |p| >= 2 are NaN and are not queried."""
+  contracted = _contracted(space)
   (nx, ny, nz), h = grid_shape(bbox, resolution)
   dev = model.device
   lo = [float(v) for v in bbox[:3]]
@@ -79,12 +118,19 @@ def density_grid(model, bbox, resolution, slab_planes=None):
   for z0 in range(0, nz, slab_planes):
     z = zs[z0:z0 + slab_planes]
     pts = torch.stack(torch.broadcast_tensors(xs[None, None, :], ys[None, :, None], z[:, None, None]), -1)
-    grid[z0:z0 + z.shape[0]] = model.query_density(pts.reshape(-1, 3), var).view(z.shape[0], ny, nx)
+    if not contracted:
+      grid[z0:z0 + z.shape[0]] = model.query_density(pts.reshape(-1, 3), var).view(z.shape[0], ny, nx)
+      continue
+    pts = pts.reshape(-1, 3)
+    inside = pts.double().square().sum(-1) < 4
+    slab = torch.full((pts.shape[0],), float('nan'), device=dev)
+    slab[inside] = model.query_density(pts[inside], var, contracted=True)
+    grid[z0:z0 + z.shape[0]] = slab.view(z.shape[0], ny, nx)
   return grid, h
 
 
 def extract_mesh(model, bbox, resolution, level, slab_planes=None, colors=False, keep_components=0, min_views=0,
-                 dataset=None, stats=None, target_faces=0, texture_size=0, before_texture=None):
+                 dataset=None, stats=None, target_faces=0, texture_size=0, before_texture=None, space='world'):
   """(vertices [V, 3] fp32, faces [F, 3] int32) on the device: the surface density = `level` of `model`'s final
   level inside `bbox` (x0, y0, z0, x1, y1, z1), on a grid of `resolution` points along the longest side.
   Vertices are in world coordinates; face normals point from dense to empty space.  With `colors`, returns
@@ -95,31 +141,74 @@ def extract_mesh(model, bbox, resolution, level, slab_planes=None, colors=False,
   without `colors`, and the colour is baked into a texture_size x texture_size atlas (bake_texture, each texel's
   colour by `vertex_colors` at its surface point and normal); returns (vertices, faces, normals, rgb or None, uv,
   texture).  before_texture: called with (vertices, faces, normals, rgb or None) before the texture is baked, so a
-  caller can save the mesh first (bake_texture raises ValueError when the atlas cannot hold the faces)."""
-  grid, h = density_grid(model, bbox, resolution, slab_planes)
+  caller can save the mesh first (bake_texture raises ValueError when the atlas cannot hold the faces).
+  space 'contracted': `bbox` is in contracted coordinates and `level` is a density per unit of contracted length
+  (density_grid); the mesh is cleaned (min_views on its world positions) and simplified in contracted space, then
+  mapped to world space (ops.mesh_uncontract), where every output lies.  Colours are queried at the contracted
+  points, the world normals giving the view directions; the atlas is laid out on the contracted mesh."""
+  contracted = _contracted(space)
+  grid, h = density_grid(model, bbox, resolution, slab_planes, space=space)
   out = ops.marching_cubes(grid, level, normals=colors or texture_size > 0)
   del grid
   lo = torch.tensor([float(v) for v in bbox[:3]], device=out[0].device)
-  vertices, faces, *normals = clean_mesh(out[0] * h + lo, *out[1:], **_clean_args(keep_components, min_views,
-                                                                                   dataset, stats))
+  vertices, faces, *normals = _clean_in_space(out[0] * h + lo, *out[1:], contracted=contracted,
+                                              **_clean_args(keep_components, min_views, dataset, stats))
   vertices, faces, *normals = simplify_mesh(vertices, faces, *normals, target_faces=target_faces, stats=stats)
+  if contracted and target_faces:
+    vertices = clamp_to_ball(vertices)
   var = h * h / 12
+  query = lambda p, n: vertex_colors(model, p, n, var, contracted=contracted)
+  # cubic cells: the grid's normals are the world's (in contracted space, after _to_world)
+  world, *wnormals = _to_world(vertices, *normals) if contracted else (vertices, *normals)
   if not texture_size:
     if not colors:
-      return vertices, faces
-    # cubic cells: the grid's normals are the world's
-    return vertices, faces, normals[0], vertex_colors(model, vertices, normals[0], var)
-  rgb = vertex_colors(model, vertices, normals[0], var) if colors else None
-  return _with_texture(vertices, faces, normals[0], rgb, texture_size, before_texture,
-                       lambda p, n: vertex_colors(model, p, n, var))
+      return world, faces
+    return world, faces, wnormals[0], query(vertices, wnormals[0])
+  rgb = query(vertices, wnormals[0]) if colors else None
+  if contracted:
+    return _with_texture(world, faces, wnormals[0], rgb, texture_size, before_texture,
+                         lambda p, n: query(p, ops.mesh_uncontract(p, n)[1]), chart=(vertices, normals[0]))
+  return _with_texture(vertices, faces, normals[0], rgb, texture_size, before_texture, query)
 
 
-def _with_texture(vertices, faces, normals, rgb, texture_size, before_texture, color_fn):
+CONTRACTED_MAX_RADIUS = 2 - 2 ** -12
+
+
+def clamp_to_ball(vertices):
+  """Contracted vertices [V, 3] with every radius above CONTRACTED_MAX_RADIUS (2 - 2^-12, a world radius of about
+  2048) scaled back to it; the others unchanged.  A quadric collapse position may lie off the surface it
+  simplifies, and on a convex surface near |p| = 2 that can be outside the ball, where no world point exists.
+  Marching cubes never puts a vertex there, since its vertices lie on grid edges between points with |p| < 2."""
+  r = vertices.double().norm(dim=-1, keepdim=True)
+  far = r > CONTRACTED_MAX_RADIUS
+  return torch.where(far, (vertices.double() * (CONTRACTED_MAX_RADIUS / r.clamp_min(1))).float(), vertices)
+
+
+def _to_world(vertices, normals=None):
+  """A contracted mesh's vertices (and normals) in world space, as a tuple: ops.mesh_uncontract."""
+  if normals is None:
+    return (ops.mesh_uncontract(vertices),)
+  return ops.mesh_uncontract(vertices, normals)
+
+
+def _clean_in_space(vertices, faces, *per_vertex, contracted=False, **clean_args):
+  """clean_mesh of a mesh in grid coordinates.  min_views projects world positions into the views, so a contracted
+  mesh is cleaned on its world vertices with its contracted ones riding along; components are topological."""
+  if not contracted or not clean_args.get('min_views'):
+    return clean_mesh(vertices, faces, *per_vertex, **clean_args)
+  _, faces, vertices, *per_vertex = clean_mesh(ops.mesh_uncontract(vertices), faces, vertices, *per_vertex,
+                                               **clean_args)
+  return (vertices, faces, *per_vertex)
+
+
+def _with_texture(vertices, faces, normals, rgb, texture_size, before_texture, color_fn, chart=None):
   """(vertices, faces, normals, rgb, uv, texture): the mesh, and bake_texture's atlas of it by `color_fn`, after
-  before_texture(vertices, faces, normals, rgb) when given."""
+  before_texture(vertices, faces, normals, rgb) when given.  chart: (vertices, normals) of the same faces to lay the
+  atlas out on and to give color_fn its texel points and normals (the contracted mesh), instead of the mesh's own."""
   if before_texture is not None:
     before_texture(vertices, faces, normals, rgb)
-  return (vertices, faces, normals, rgb) + bake_texture(vertices, faces, normals, texture_size, color_fn)
+  cv, cn = chart if chart is not None else (vertices, normals)
+  return (vertices, faces, normals, rgb) + bake_texture(cv, faces, cn, texture_size, color_fn)
 
 
 def bake_texture(vertices, faces, normals, size, color_fn):
@@ -138,12 +227,13 @@ def bake_texture(vertices, faces, normals, size, color_fn):
   return uv, texture.view(size, size, 3)
 
 
-def vertex_colors(model, vertices, normals, var):
+def vertex_colors(model, vertices, normals, var, contracted=False):
   """rgb [V, 3] uint8 of each vertex: `model.query_radiance` at the Gaussian (vertex, var * I) seen along -normal,
   the surface viewed head-on from outside, as round(clip(rgb, 0, 1) * 255).  A RawNeRF model's colours are its
   linear raw values, clipped as they are.  var: the footprint the density was sampled at (h^2 / 12 for grid cells
-  of side h)."""
-  _, rgb = model.query_radiance(vertices, var, -normals)
+  of side h).  contracted: vertices and var in contracted space, normals in world space
+  (Model.query_radiance(contracted=True))."""
+  _, rgb = model.query_radiance(vertices, var, -normals, **({'contracted': True} if contracted else {}))
   return (rgb.clamp(0, 1) * 255).round().to(torch.uint8)
 
 
@@ -155,8 +245,10 @@ def validate_config(bundle):
   views (not NDC) and a truncation of at least one cell, so no cut edge of the fused grid has an unobserved end.
   The cleaning and simplification options must not be negative, and mesh_min_views projects into the views, so it
   needs them not NDC either.  mesh_texture_size is 0 (off) or in [4, 16384].  mesh_eval traces world-space
-  meshes along the test rays, so it needs them not NDC either."""
+  meshes along the test rays, so it needs them not NDC either.  mesh_space is 'world' or 'contracted', the latter
+  only under the scene contraction and not for NDC scenes."""
   config = bundle.config
+  _check_space(bundle)
   if config.mesh_method not in MESH_METHODS:
     raise ValueError(f'Config.mesh_method = {config.mesh_method!r}: want one of {MESH_METHODS}')
   for name in ('mesh_keep_components', 'mesh_min_views', 'mesh_target_faces'):
@@ -191,15 +283,19 @@ def camera_matrices(cameras, device):
   return to(w2c), to(c2p)
 
 
-def fuse_tsdf(views, cameras, camtype, bbox, resolution, truncation, colors=False, batch=8, device='cuda'):
+def fuse_tsdf(views, cameras, camtype, bbox, resolution, truncation, colors=False, batch=8, device='cuda',
+              space='world'):
   """Fuse rendered views into a TSDF on the grid of `bbox` at `resolution` (grid_shape; the points density_grid
   uses).  views: iterable of (cam_idx, depth [H, W], acc [H, W], rgb [H, W, 3] or None) device tensors -- each
   view's median distance (in the units of its rays' directions), opacity and colour; cameras: (pixtocams,
   camtoworlds, distortion_params, pixtocam_ndc) as a dataset holds them; camtype: camera_utils.ProjectionType or its
   value; truncation: the band in cells.  Views are fused `batch` at a time, in order; the result does not depend on
   `batch`.  Returns ((tsdf, weight, color_sum, color_weight), h): [nz, ny, nx] fp32 grids ([nz, ny, nx, 3] for
-  color_sum; the colour pair is None without `colors`) and the cell size."""
+  color_sum; the colour pair is None without `colors`) and the cell size.  space 'contracted': the grid, and so
+  the cell size and the band, are in contracted coordinates (ops.tsdf_integrate(contracted=True)); points with
+  |p| >= 2 stay unobserved."""
   from . import camera_utils
+  contracted = _contracted(space)
   if cameras[3] is not None:
     raise ValueError('TSDF fusion does not support NDC cameras')
   camtype = camera_utils.ProjectionType(camtype.value if hasattr(camtype, 'value') else camtype)
@@ -218,7 +314,7 @@ def fuse_tsdf(views, cameras, camtype, bbox, resolution, truncation, colors=Fals
     rgb = torch.stack([v[3].reshape(H, W, 3) for v in items]).float() if colors else None
     ops.tsdf_integrate((nx, ny, nz), bbox[:3], h, 0 if camtype == camera_utils.ProjectionType.PERSPECTIVE else 1,
                        cameras[2], w2c[idx].contiguous(), c2p if c2p.shape[0] == 1 else c2p[idx].contiguous(),
-                       depth, acc, rgb, tau, tsdf, weight, color_sum, color_weight)
+                       depth, acc, rgb, tau, tsdf, weight, color_sum, color_weight, contracted=contracted)
 
   items = []
   for view in views:
@@ -232,7 +328,7 @@ def fuse_tsdf(views, cameras, camtype, bbox, resolution, truncation, colors=Fals
 
 
 def tsdf_mesh(state, bbox, h, colors=False, clean_args=None, target_faces=0, stats=None, texture_size=0,
-              before_texture=None):
+              before_texture=None, space='world'):
   """Marching cubes on the fused TSDF `state` (fuse_tsdf): the zero crossing of -tsdf (inside > 0, so faces and
   normals point out of the surface), with every point no view observed (weight 0) NaN, so it gives no faces.
   Returns (vertices, faces) in world coordinates, and with `colors` also (normals [V, 3], rgb [V, 3] uint8): each
@@ -242,7 +338,10 @@ def tsdf_mesh(state, bbox, h, colors=False, clean_args=None, target_faces=0, sta
   colour is interpolated trilinearly at (vertex - lo) / h, clamped to the grid (tsdf_colors).  texture_size > 0
   (the state must hold the colour grid): the normals are computed with or without `colors` and the colour is baked
   into a texture atlas, each texel's by tsdf_colors at its surface point; returns and calls `before_texture` as
-  extract_mesh does."""
+  extract_mesh does.  space 'contracted': the state was fused in contracted space (fuse_tsdf); the mesh is cleaned
+  and simplified there, its colours interpolated there, and it is returned in world space as extract_mesh returns
+  it."""
+  contracted = _contracted(space)
   tsdf, weight, color_sum, color_weight = state
   if texture_size and color_sum is None:
     raise ValueError('tsdf_mesh: texture_size needs the fused colour grid (fuse_tsdf with colors=True)')
@@ -254,23 +353,32 @@ def tsdf_mesh(state, bbox, h, colors=False, clean_args=None, target_faces=0, sta
   # without simplification the grid-unit vertices ride along as a per-vertex array: the colours are interpolated
   # from them
   ride = (out[0],) if colors and not simplify else ()
-  vertices, faces, *per = clean_mesh(out[0] * h + lo, out[1], *out[2:], *ride, **(clean_args or {}))
+  vertices, faces, *per = _clean_in_space(out[0] * h + lo, out[1], *out[2:], *ride, contracted=contracted,
+                                          **(clean_args or {}))
   if simplify:
     vertices, faces, *per = simplify_mesh(vertices, faces, *per, target_faces=target_faces, stats=stats)
+    if contracted:
+      vertices = clamp_to_ball(vertices)
   elif stats is not None:
     simplify_mesh(vertices, faces, target_faces=0, stats=stats)
   if not colors and not texture_size:
-    return vertices, faces
+    return (_to_world(vertices)[0] if contracted else vertices), faces
   rgb = None
   if colors:
     # unsimplified, a vertex lies on a grid edge: its two other coordinates are integers, so the trilinear weights
     # reduce to the linear interpolation between the edge's two ends
     rgb = (tsdf_colors(color_sum, color_weight, (vertices - lo) / h) if simplify else
            tsdf_colors(color_sum, color_weight, per[1], clamp=False))
+  color_fn = lambda p, n: tsdf_colors(color_sum, color_weight, (p - lo) / h)
+  if contracted:
+    world, wnormals = _to_world(vertices, per[0])
+    if not texture_size:
+      return world, faces, wnormals, rgb
+    return _with_texture(world, faces, wnormals, rgb, texture_size, before_texture, color_fn,
+                         chart=(vertices, per[0]))
   if not texture_size:
     return vertices, faces, per[0], rgb
-  return _with_texture(vertices, faces, per[0], rgb, texture_size, before_texture,
-                       lambda p, n: tsdf_colors(color_sum, color_weight, (p - lo) / h))
+  return _with_texture(vertices, faces, per[0], rgb, texture_size, before_texture, color_fn)
 
 
 def tsdf_colors(color_sum, color_weight, gv, clamp=True):
@@ -310,16 +418,17 @@ def render_views(model, dataset):
 
 
 def extract_mesh_tsdf(model, dataset, bbox, resolution, truncation=3.0, colors=False, batch=8, keep_components=0,
-                      min_views=0, stats=None, target_faces=0, texture_size=0, before_texture=None):
+                      min_views=0, stats=None, target_faces=0, texture_size=0, before_texture=None, space='world'):
   """Config.mesh_method = 'tsdf': render every camera of `dataset` (render_views), fuse the renders (fuse_tsdf, a
   band of `truncation` cells) and mesh the result (tsdf_mesh).  Returns what extract_mesh returns.
   `keep_components`, `min_views` (against the cameras of `dataset`) and `stats`: clean_mesh, applied before the
   colours are interpolated; `target_faces`: then simplify_mesh; `texture_size`, `before_texture`: then the texture
-  (tsdf_mesh), the fusion keeping its colour grid for it."""
+  (tsdf_mesh), the fusion keeping its colour grid for it.  space: the grid's space (fuse_tsdf, tsdf_mesh)."""
   state, h = fuse_tsdf(render_views(model, dataset), dataset.cameras, dataset.camtype, bbox, resolution, truncation,
-                       colors=colors or texture_size > 0, batch=batch, device=model.device)
+                       colors=colors or texture_size > 0, batch=batch, device=model.device, space=space)
   return tsdf_mesh(state, bbox, h, colors=colors, clean_args=_clean_args(keep_components, min_views, dataset, stats),
-                   target_faces=target_faces, stats=stats, texture_size=texture_size, before_texture=before_texture)
+                   target_faces=target_faces, stats=stats, texture_size=texture_size, before_texture=before_texture,
+                   space=space)
 
 
 def clean_mesh(vertices, faces, *per_vertex, keep_components=0, min_views=0, cameras=None, camtype=None,

@@ -353,6 +353,14 @@ class BwdScratch:
         self.g = torch.empty(M, cfg.net_width, device=dev, dtype=bf)
 
 
+def _contracted_length_scale(points):
+  """|dx/dr_c| at contracted points p [N, 3] (|p| < 2): world length per unit of contracted length along a radial
+  ray, 1 inside the unit ball and |x|^2 = (2 - |p|)^-2 outside -> fp32 [N].  |p| is clamped below 2 as
+  inv_contract clamps it (csrc/contract.cuh), so a point whose fp32 norm rounds to 2 gets a finite scale."""
+  m = points.square().sum(-1)
+  return torch.where(m > 1, (2 - m.sqrt().clamp_max(2 - 2 ** -23)).square().reciprocal(), torch.ones_like(m))
+
+
 def _loss_args(loss_mults):
   """(orient_mult, prednorm_mult, orient_on_pred) of the normals kernels: both losses off without loss_mults."""
   return loss_mults if loss_mults is not None else (0.0, 0.0, True)
@@ -722,15 +730,29 @@ class Model:
       ops.head_fwd(x, mlp.w_head, mlp.b(d), plan.head_n, d.in_pad, raw=st.raw_head)
     st.x_last = x
 
-  def query_density(self, points, var, impl=0):
+  def _contracted_mode(self, cfg, contracted):
+    """warp_contract of the point encoder: the level's own flag, or 2 (points already contracted) with `contracted`,
+    which needs an MLP under the scene contraction."""
+    if not contracted:
+      return cfg.warp_fn == 'contract'
+    if cfg.warp_fn != 'contract':
+      raise ValueError('contracted points need an MLP under the scene contraction (warp_fn = contract)')
+    return 2
+
+  def query_density(self, points, var, impl=0, contracted=False):
     """Density of the final level's MLP (NerfMLP_0) at world points [N, 3] (tensor or array): the point encoder on
     the Gaussians (point, var * I), the trunk and the density head in their render form, then
     density_activation(raw + density_bias), without density noise -> fp32 [N] on the device.  Runs in chunks of
-    render_chunk_size * num_nerf_samples rows, the rows of one render chunk's final level."""
+    render_chunk_size * num_nerf_samples rows, the rows of one render chunk's final level.
+    contracted: the points p (|p| < 2) and the footprint var * I are in the scene contraction's space, encoded as
+    they are, and the result is the density per unit of contracted length along radial rays, sigma_c = sigma(x)
+    |dx/dr_c|: sigma inside the unit ball, sigma / (2 - |p|)^2 outside, so that one level means one opacity per
+    contracted cell everywhere."""
     mname = 'NerfMLP_0'
     mlp = self.mlps[mname]
     plan = mlp.plan
     cfg = plan.cfg
+    warp = self._contracted_mode(cfg, contracted)
     points = torch.as_tensor(points, dtype=torch.float32, device=self.device).reshape(-1, 3).contiguous()
     N = points.shape[0]
     density = torch.empty(N, device=self.device)
@@ -743,25 +765,30 @@ class Model:
         states[n] = self._level_state('query', mname, n, 1, trunk_only=True)
       st = states[n]
       ops.encode_points(p, var, mlp.basis, min_deg=cfg.min_deg_point, max_deg=cfg.max_deg_point,
-                        warp_contract=cfg.warp_fn == 'contract', disable_integration=self.mcfg.disable_integration,
+                        warp_contract=warp, disable_integration=self.mcfg.disable_integration,
                         feat=st.feat, feat_cols=plan.Fpad)
       self._trunk_layers(st, mlp, impl)
       # density_activation: softplus, the only one MLPPlan accepts
       torch.nn.functional.softplus(st.raw_head[:, 0] + cfg.density_bias, out=density[i0:i0 + n])
+    if contracted:
+      density *= _contracted_length_scale(points)
     return density
 
-  def query_radiance(self, points, var, viewdirs, impl=0):
+  def query_radiance(self, points, var, viewdirs, impl=0, contracted=False):
     """Density and colour of the final level's MLP (NerfMLP_0) at world points [N, 3] seen along unit view
     directions viewdirs [N, 3] (ignored, and may be None, for a view-independent model) -> (density [N], rgb [N, 3])
     fp32 on the device.  Each point is one sample: the point encoder on the Gaussian (point, var * I), then the
     level's MLP as a render runs it (Model._mlp_stages: density normals and the Ref-NeRF stage included), with
     the GLO vector zeroed, no density or bottleneck noise, and no exposure scale; rgb is the activated, padded
     sample colour (ops.point_rgb), zero for an MLP without colour.  Density as query_density.  Runs in chunks of
-    render_chunk_size * num_nerf_samples rows."""
+    render_chunk_size * num_nerf_samples rows.  contracted: points and footprint in contracted space, as
+    query_density takes them; viewdirs stay world directions, and density normals are taken with respect to the
+    world point (the encoder's warp_contract 2)."""
     mname = 'NerfMLP_0'
     mlp = self.mlps[mname]
     plan = mlp.plan
     cfg = plan.cfg
+    warp = self._contracted_mode(cfg, contracted)
     dev = self.device
     points = torch.as_tensor(points, dtype=torch.float32, device=dev).reshape(-1, 3).contiguous()
     N = points.shape[0]
@@ -785,13 +812,15 @@ class Model:
         states[n].keep_acts = plan.density_normals
       st = states[n]
       ops.encode_points(p, var, mlp.basis, min_deg=cfg.min_deg_point, max_deg=cfg.max_deg_point,
-                        warp_contract=cfg.warp_fn == 'contract', disable_integration=self.mcfg.disable_integration,
+                        warp_contract=warp, disable_integration=self.mcfg.disable_integration,
                         feat=st.feat, feat_cols=plan.Fpad, tfeat=st.tfeat)
       self._mlp_stages(st, mlp, viewdirs[i0:i0 + n] if plan.top == 'view' else None, impl)
       torch.nn.functional.softplus(st.raw_head[:, 0] + cfg.density_bias, out=density[i0:i0 + n])
       if st.raw_rgb is not None:
         ops.point_rgb(st.raw_rgb.reshape(n, 3), cfg=comp_cfg, raw_diffuse=st.heads.get('diffuse'),
                       raw_tint=st.heads.get('tint'), out=rgb[i0:i0 + n])
+    if contracted:
+      density *= _contracted_length_scale(points)
     return density, rgb
 
   def _tangent_fwd(self, st, mlp, impl):

@@ -137,7 +137,9 @@ def encode(sdist, origins, directions, radii, near, far, basis, *, min_deg, max_
 def encode_points(points, var, basis, *, min_deg, max_deg, warp_contract=False, disable_integration=False,
                   feat=None, feat_cols=None, want_f32=False, tfeat=None):
   """Point form of `encode`: features of the Gaussians (points[i], var * I) -> bf16 [N, ld] (+ fp32 [N, 2KL]).
-  With `tfeat` [3N, ld_t] bf16, also the tangent rows d feature / d point (no fp32 copy then)."""
+  With `tfeat` [3N, ld_t] bf16, also the tangent rows d feature / d point (no fp32 copy then).  warp_contract: False
+  / True, or 2 for points already contracted: encoded as they are, tangent rows with respect to the world point
+  inv_contract(point) (include/mnrf.h)."""
   lib = L.load()
   N = points.shape[0]
   K = basis.shape[0]
@@ -429,6 +431,31 @@ def mesh_trace(bvh, origins, directions, near, far):
   return face, t, bary
 
 
+def mesh_uncontract(points, normals=None):
+  """Contracted points [N, 3] (and their level-set normals [N, 3]) fp32 on the device -> world points [N, 3] (and unit
+  world normals [N, 3]) by mnrf_mesh_uncontract (csrc/mesh.cu): inv_contract of each point, J n of each normal.
+  Checks on the device that every point is finite and lies inside the open ball of radius 2, the contracted
+  space's extent, and reads that one flag back: a point outside raises ValueError and never reaches the kernel."""
+  lib = L.load()
+  points = _f32(points.contiguous())
+  if points.dim() != 2 or points.shape[1] != 3 or (normals is not None and normals.shape != points.shape):
+    raise ValueError(f'mesh_uncontract: points {tuple(points.shape)}, normals '
+                     f'{None if normals is None else tuple(normals.shape)}: want [N, 3] both')
+  N = points.shape[0]
+  world = torch.empty_like(points)
+  wnormals = None if normals is None else torch.empty_like(points)
+  if N == 0:
+    return world if normals is None else (world, wnormals)
+  if bool(~(points.double().square().sum(-1) < 4).all()):
+    raise ValueError('mesh_uncontract: a point is not finite or lies outside the open ball of radius 2')
+  if normals is not None:
+    normals = _f32(normals.contiguous())
+  _count()
+  L.check(lib.mnrf_mesh_uncontract(N, L.ptr(points), L.ptr(normals), L.ptr(world), L.ptr(wnormals),
+                                   L.stream_ptr()))
+  return world if normals is None else (world, wnormals)
+
+
 def points_view_count(points, camtype, distortion_params, worldtocams, camtopixs, height, width):
   """For each point [N, 3] fp32 on the device, the number of views whose height x width image it lands on
   (mnrf_points_view_count, csrc/mesh.cu: the pixel rule of tsdf_integrate) -> counts [N] int32.  camtype 0
@@ -447,17 +474,19 @@ def points_view_count(points, camtype, distortion_params, worldtocams, camtopixs
 
 
 def tsdf_integrate(shape, lo, h, camtype, distortion_params, worldtocams, camtopixs, depth, acc, rgb, tau, tsdf,
-                   weight, color_sum=None, color_weight=None):
+                   weight, color_sum=None, color_weight=None, contracted=False):
   """Fuse K views into the TSDF state in place (mnrf_tsdf_integrate, csrc/mesh.cu).  shape (nx, ny, nz) and lo, h:
   the grid points lo + h (x, y, z); camtype 0 perspective / 1 fisheye; distortion_params: dict of k1..k4, p1, p2
   or None; worldtocams [K, 3, 4], camtopixs [K or 1, 3, 3], depth, acc [K, H, W], rgb [K, H, W, 3] or None, fp32 on
-  the device; tsdf, weight [nz, ny, nx] and, with rgb, color_sum [nz, ny, nx, 3], color_weight [nz, ny, nx]."""
+  the device; tsdf, weight [nz, ny, nx] and, with rgb, color_sum [nz, ny, nx, 3], color_weight [nz, ny, nx].
+  contracted: the grid, lo, h and tau are in the scene contraction's space (mnrf_tsdf_integrate_contracted)."""
   lib = L.load()
   nx, ny, nz = shape
   K, H, W = depth.shape
   d = _projection_desc(camtype, distortion_params, camtopixs.shape[0])
   _count()
-  L.check(lib.mnrf_tsdf_integrate(C.byref(d), nx, ny, nz, *(float(v) for v in lo), float(h), K, H, W,
+  fn = lib.mnrf_tsdf_integrate_contracted if contracted else lib.mnrf_tsdf_integrate
+  L.check(fn(C.byref(d), nx, ny, nz, *(float(v) for v in lo), float(h), K, H, W,
                                   L.ptr(_f32(worldtocams)), L.ptr(_f32(camtopixs)), L.ptr(_f32(depth)),
                                   L.ptr(_f32(acc)), L.ptr(_f32(rgb)), float(tau), L.ptr(_f32(tsdf)),
                                   L.ptr(_f32(weight)), L.ptr(_f32(color_sum)), L.ptr(_f32(color_weight)),

@@ -32,9 +32,17 @@
           extraction after mesh_target_faces = --simplify_faces (where the simplification stalls); and
           mesh.evaluate_mesh on one such view of the 360.gin mesh with the NeRF's render_views as its reference,
           split into NeRF rendering, BVH build and tracing with shading (not part of `all`);
+  contracted: Config.mesh_space = 'contracted' against 'world' on the random-init 360.gin NerfMLP: mesh.density_grid
+          at --extract_res^3 over [-2, 2]^3 (contracted) and over the world default box, with the points queried and
+          skipped, rows/s of the queried points and points/s with the skipped ones counted; mesh.extract_mesh end to
+          end in both spaces at the same level, alternated --reps times, with the peak device memory of each; and
+          ops.tsdf_integrate against ops.tsdf_integrate(contracted=True) in G point-views/s (CUDA events around one
+          launch of 32 views of 1008 x 756, random depth and opacity, cameras inside the unit ball) into 512^3 and
+          1024^3 grids (not part of `all`);
   device: the card's name and power limit, read in the same run.
 
-  python tools/mesh_bench.py [--rows 8388608] [--extract_res 512] [--sections all|components|simplify|texture|trace]
+  python tools/mesh_bench.py [--rows 8388608] [--extract_res 512]
+                             [--sections all|components|simplify|texture|trace|contracted]
                              [--out result.json]
 """
 import argparse
@@ -430,12 +438,68 @@ def bench_trace_section(model, bbox, level, args):
   return out
 
 
+def bench_contracted_section(model, bbox, level, args):
+  cbox = (-2.0, -2.0, -2.0, 2.0, 2.0, 2.0)
+  out = {'grid': args.extract_res, 'world_bbox': list(bbox), 'contracted_bbox': list(cbox), 'level': level}
+  n = args.extract_res ** 3
+  for space, box in (('world', bbox), ('contracted', cbox)):
+    mesh.density_grid(model, box, args.extract_res, space=space)           # warm-up of every slab shape
+    torch.cuda.empty_cache()
+    t, (grid, _) = timed(lambda: mesh.density_grid(model, box, args.extract_res, space=space), 1)
+    queried = int(torch.isfinite(grid).sum()) if space == 'contracted' else n
+    out[f'{space}_grid'] = {'s': round(t, 3), 'points': n, 'queried': queried, 'skipped': n - queried,
+                            'queried_rows_per_s': round(queried / t), 'points_per_s': round(n / t)}
+    del grid
+    torch.cuda.empty_cache()
+  runs = {'world': [], 'contracted': []}
+  for _ in range(args.reps):
+    for space, box in (('world', bbox), ('contracted', cbox)):
+      torch.cuda.reset_peak_memory_stats()
+      base = torch.cuda.memory_allocated()
+      t, (v, f) = timed(lambda: mesh.extract_mesh(model, box, args.extract_res, level, space=space), 1)
+      runs[space].append({'s': round(t, 3), 'vertices': int(v.shape[0]), 'faces': int(f.shape[0]),
+                          'peak_gb': round((torch.cuda.max_memory_allocated() - base) / 2 ** 30, 2)})
+      del v, f
+      torch.cuda.empty_cache()
+  out['extract'] = runs
+  # TSDF fusion: one launch of K views into the grid, world against contracted
+  rng = np.random.default_rng(0)
+  K, W, H = 32, 1008, 756
+  w2c = []
+  for _ in range(K):
+    q, _ = np.linalg.qr(rng.normal(size=(3, 3)))
+    eye = rng.normal(size=3)
+    eye *= 0.8 * rng.uniform() / np.linalg.norm(eye)
+    w2c.append(np.concatenate([q.T, -q.T @ eye[:, None]], 1))
+  dev = 'cuda'
+  w2c = torch.tensor(np.stack(w2c), dtype=torch.float32, device=dev).contiguous()
+  f_ = 0.6 * W
+  c2p = torch.tensor([[[f_, 0, W / 2], [0, f_, H / 2], [0, 0, 1]]], dtype=torch.float32, device=dev)
+  depth = torch.tensor(rng.uniform(0.5, 50, (K, H, W)), dtype=torch.float32, device=dev)
+  acc = torch.tensor(rng.uniform(0, 1, (K, H, W)), dtype=torch.float32, device=dev)
+  tsdf_rows = []
+  for res in (512, 1024):
+    for space, box in (('world', bbox), ('contracted', cbox)):
+      (nx, ny, nz), h = mesh.grid_shape(box, res)
+      state = [torch.zeros(nz, ny, nx, device=dev) for _ in range(2)]
+      launch = lambda: ops.tsdf_integrate((nx, ny, nz), box[:3], h, 0, None, w2c, c2p, depth, acc, None, 3 * h,
+                                          *state, contracted=space == 'contracted')
+      ms = events(launch, args.reps)
+      tsdf_rows.append({'grid': res, 'space': space, 'views': K, 'image': [W, H], 'ms': round(ms, 3),
+                        'g_point_views_per_s': round(nx * ny * nz * K / ms / 1e6, 2)})
+      del state
+      torch.cuda.empty_cache()
+  out['tsdf'] = tsdf_rows
+  return out
+
+
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--rows', type=int, default=1 << 23)
   ap.add_argument('--reps', type=int, default=3)
   ap.add_argument('--extract_res', type=int, default=512)
-  ap.add_argument('--sections', default='all', choices=('all', 'components', 'simplify', 'texture', 'trace'))
+  ap.add_argument('--sections', default='all', choices=('all', 'components', 'simplify', 'texture', 'trace',
+                                                             'contracted'))
   ap.add_argument('--trace_views', type=int, default=4)
   ap.add_argument('--simplify_faces', type=int, default=1_000_000)
   ap.add_argument('--texture_faces', type=int, default=1_000_000)
@@ -445,7 +509,7 @@ def main():
   args = ap.parse_args()
   lib.require_device()
   res = {'device': device_info(), 'query': {}, 'mc': [], 'extract': None}
-  if args.sections in ('components', 'simplify', 'texture', 'trace'):
+  if args.sections in ('components', 'simplify', 'texture', 'trace', 'contracted'):
     b = configs.bundle_360()
     model = models.Model(b)
     model.init(seed=0)
@@ -455,7 +519,8 @@ def main():
     del grid
     torch.cuda.empty_cache()
     section = {'components': bench_components_section, 'simplify': bench_simplify_section,
-               'texture': bench_texture_section, 'trace': bench_trace_section}[args.sections]
+               'texture': bench_texture_section, 'trace': bench_trace_section,
+               'contracted': bench_contracted_section}[args.sections]
     res = {'device': res['device'], 'level': level, args.sections: section(model, bbox, level, args),
            'device_after': device_info()}
     emit(res, args.out)
