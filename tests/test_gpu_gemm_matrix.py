@@ -10,6 +10,8 @@ tile and by at least one with several tiles per persistent CTA; test_every_insta
   - no NaN: every input sits in NaN-filled padding, so a read outside an operand shows.
 test_same_bits runs instances that must agree bit for bit on the same data.  test_rejected_arguments checks that each
 argument check of the launch raises and writes nothing.  Needs an H100 (test_every_instance_has_cases does not).
+fp64_launches makes the launches of test_gemm_case and test_same_bits through the same `launch`, on CPU buffers, for
+the launch-coverage audit (test_launch_coverage_cpu.py), which asks that every launch class the models reach has one.
 """
 import math
 
@@ -31,7 +33,9 @@ def ops():
 def case(mode, M, N, K, **kw):
   """One launch.  mode 'fwd' | 'dgrad' | 'wgrad' (WGRAD: M = Mo, K = R).  Options:
     act      'none' | 'relu' | 'softplus' | 'silu'     bias   FWD bias (default on)
-    bits     FWD ReLU writes mask bits                 z      FWD smooth writes z (row pitch > N)
+    bits     FWD ReLU writes mask bits: True (pitch % 4 != 0: stored from registers) | 'tma' (16-byte aligned
+             words, pitch % 4 == 0: stored by TMA from shared memory)
+    z        FWD smooth writes z (row pitch > N)
     store    'staged' (16-byte aligned output, pitch % 8 == 0) | 'reg2' (output 2 elements off) | 'reg4' (pitch
              = 4 mod 8): the register store whatever BN
     mask     DGRAD 'none' | 'bf16' | 'bits' (16-byte aligned words, pitch % 4 == 0) | 'bits_odd' (pitch % 4 != 0)
@@ -117,6 +121,23 @@ for r in (1, 15, 37, 64, 65):
   CASES.append(case('wgrad', 200, 128, r, side='both'))
 for impl in (0, 1):
   CASES.append(case('wgrad', 320, 256, 1000, side='both', impl=impl))
+# ---- the operand sets the models launch (test_launch_coverage_cpu.py): the ping-pong epilogues compiled per operand
+# set (FWD bias alone; bias + ReLU + mask bits stored by TMA; DGRAD mask bits by TMA, with and without rowv / colv)
+# and the generic epilogue without column sums, each at every tile width the models use
+for n in (256, 128, 64):
+  CASES.append(case('fwd', BIG, n, 192))
+  CASES.append(case('fwd', WAVE + 1, 3 * n, 64, act='relu', bits='tma'))
+  CASES.append(case('dgrad', BIG, n, 192))
+  CASES.append(case('dgrad', WAVE + 1, n, 192, mask='bits'))
+  CASES.append(case('dgrad', BIG, 3 * n, 64, mask='bits', rowv=True))
+  CASES.append(case('dgrad', BIG, n, 128, addend=True))
+  CASES.append(case('dgrad', 3 * 384, n, 128, mask='bits', rep=3))
+CASES.append(case('dgrad', 3 * 200, 128, 128, mask='bits', rep=3))     # mask_mod % 128 != 0: bits by the epilogue
+for act in ('softplus', 'silu'):
+  CASES.append(case('dgrad', BIG, 256, 192, act=act))
+  CASES.append(case('dgrad', WAVE + 1, 256, 128, act=act, addend=True))
+  CASES.append(case('dgrad', 3 * 384, 256, 128, act=act, rep=3))
+CASES.append(case('dgrad', BIG, 128, 192, act='silu', colsum=True))
 
 
 # ---------------------------------------------------------------------------------------------- buffers and data
@@ -154,7 +175,9 @@ def layout(c, device, fill=True):
   if c['mode'] == 'fwd':
     if c['bias']:
       put('bias', (N,), torch.float32, nan, extra_cols=4, col0=2)
-    if c['bits']:
+    if c['bits'] == 'tma':
+      put('maskbits', (M, _words(N)), torch.int32, sen, extra_cols=(-_words(N) % 4) + 8, col0=4)
+    elif c['bits']:
       put('maskbits', (M, _words(N)), torch.int32, sen, extra_cols=3, col0=1)
     if c['z']:
       put('z', (M, N), bf, sen, extra_cols=10, col0=2)
@@ -253,11 +276,9 @@ def _fill(c, v, seed):
   return init
 
 
-def run(ops_mod, c, seed=0):
-  """Launch the case on its data; returns (views, buffers, initial values)."""
+def launch(ops_mod, c, v):
+  """The case's one launch on the views of layout(c, ...)."""
   from multinerf_b200 import lib as L
-  v, bufs = layout(c, 'cuda')
-  init = _fill(c, v, seed)
   kw = _call_kwargs(c, v)
   if c['mode'] == 'wgrad':
     if c['side'] == 'none':
@@ -268,6 +289,13 @@ def run(ops_mod, c, seed=0):
   else:
     mode = L.GEMM_FWD if c['mode'] == 'fwd' else L.GEMM_DGRAD
     ops_mod.gemm(mode, v['a'], v['b'], v['out'], impl=c['impl'], **kw)
+
+
+def run(ops_mod, c, seed=0):
+  """Launch the case on its data; returns (views, buffers, initial values)."""
+  v, bufs = layout(c, 'cuda')
+  init = _fill(c, v, seed)
+  launch(ops_mod, c, v)
   torch.cuda.synchronize()
   return v, bufs, init
 
@@ -366,6 +394,16 @@ def test_mask_mod_matches_repeated_masks(ops, m, n, rep):
   ops.gemm(L.GEMM_DGRAD, v2['a'], v2['b'], v2['out'], **_call_kwargs(c2, v2))
   torch.cuda.synchronize()
   assert torch.equal(_bits(v2['out']), _bits(v['out']))
+
+
+def fp64_launches(ops_mod):
+  """Every launch test_gemm_case and test_same_bits check against fp64, made through `launch` on uninitialised CPU
+  buffers of the same layout: under a recording library (tests/abi_record.py) these are the calls the GPU tests
+  make, which the launch-coverage audit classifies (test_launch_coverage_cpu.py)."""
+  cases = list(CASES) + [dict(base, **var) for base, variants, _ in SAME_BITS for var in [{}] + variants]
+  for c in cases:
+    v, _ = layout(c, 'cpu', fill=False)
+    launch(ops_mod, c, v)
 
 
 # ---------------------------------------------------------------------------------------------- coverage

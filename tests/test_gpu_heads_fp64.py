@@ -9,7 +9,9 @@ the library (mnrf_head_plan) which instance each case runs.  Each case checks:
   - every padding element around every output buffer unchanged, bitwise;
   - no NaN: every input sits in NaN-filled padding, so a read outside an operand shows.
 Column sums, weight packing, clip+Adam and the chained trunk's fused head get the same checks.  Needs an H100
-(test_every_instance_has_cases does not).
+(test_every_instance_has_cases does not).  fp64_launches makes the head launches of test_head_case and
+test_heads_and_colsum_fp64 through the same `launch`, on CPU buffers, for the launch-coverage audit
+(test_launch_coverage_cpu.py), which asks that every head launch class the models reach has one.
 """
 import math
 
@@ -40,9 +42,10 @@ def case(mode, M, K, n_out, **kw):
     act       bwd 'none' | 'relu' | 'softplus' | 'silu'
     out       bwd outputs: 'dx' | 'dx_sum' (dx and dxsum) | 'params' (dx=None) | 'alias' (dx=None, w = x's first row)
     dx_cols   bwd: columns of dx (0: K); the rest go to dx2      split   bwd dw_split (0: none)
-    w_off     bwd: w this many elements past a 16-byte boundary"""
+    w_off     bwd: w this many elements past a 16-byte boundary
+    db        bwd: db given (default on)                 dx2     bwd with dx_cols: dx2 given (default on)"""
   c = dict(mode=mode, M=M, K=K, n_out=n_out, bias=True, strided=False, act='none', out='dx_sum', dx_cols=0, split=0,
-           w_off=0)
+           w_off=0, db=True, dx2=True)
   assert set(kw) <= set(c), set(kw) - set(c)
   c.update(kw)
   return c
@@ -86,6 +89,24 @@ for K, w_off in BWD_WIDTHS:
   CASES.append(case('bwd', 1001, K, 3, act='relu', dx_cols=K - 16, out='dx', split=2, w_off=w_off))
   CASES.append(case('bwd', 2053, K, 1, out='alias', w_off=w_off))
 CASES.append(case('bwd', 2 ** 20 + 3, 256, 1, out='alias'))          # the dW-only pass of a Dense(1) head on x
+# ---- the output sets the models launch (test_launch_coverage_cpu.py) on contiguous operands: dW alone (no db), the
+# parameter gradients alone, dx without dxsum, dx_cols without dx2, and the stacked view-independent heads
+for K in (64, 128, 256, 1024):
+  CASES.append(case('bwd', 2053 if K != 64 else 24577, K, 1, out='params', db=False))
+for K in (64, 256):
+  CASES.append(case('bwd', 8195, K, 3, out='params'))
+  CASES.append(case('bwd', 4099 if K == 256 else 2049, K, 1, act='relu', out='dx'))
+for K in (128, 256, 1024):
+  CASES.append(case('bwd', 2049, K, 4, act='relu', out='dx', split=1))
+for K in (128, 256):
+  CASES.append(case('bwd', 2049, K, 4, out='params', split=1))
+CASES.append(case('bwd', 1001, 64, 3, act='relu'))
+CASES.append(case('bwd', 8195, 192, 1, act='relu', out='dx', dx_cols=64, dx2=False))
+CASES.append(case('bwd', 2049, 320, 3, out='dx', dx_cols=256, dx2=False, strided=True))
+CASES.append(case('bwd', 2049, 320, 3, out='dx'))
+CASES.append(case('bwd', 2049, 448, 3, act='relu', dx_cols=128))
+CASES.append(case('bwd', 2049, 128, 3, act='softplus'))
+CASES.append(case('bwd', 8195, 128, 3, act='silu'))
 
 
 def _embed_flat(shape, dtype, dev, col0, fill):
@@ -126,10 +147,11 @@ def layout(c, device, fill=True):
   put('dw', _embed_flat((K, split), torch.float32, device, 2, sen))
   if split < n:
     put('dw2', _embed_flat((K, n - split), torch.float32, device, 2, sen))
-  put('db', _embed_flat((n,), torch.float32, device, 2, sen))
+  if c['db']:
+    put('db', _embed_flat((n,), torch.float32, device, 2, sen))
   if c['out'] in ('dx', 'dx_sum'):
     put('dx', G.embed((M, cols), bf, device, fill=sen, **pad))
-    if cols < K:
+    if cols < K and c['dx2']:
       put('dx2', G.embed((M, K - cols), bf, device, fill=sen, **pad))
     if c['out'] == 'dx_sum':
       put('dxsum', _embed_flat((cols,), torch.float32, device, 2, sen))
@@ -190,16 +212,21 @@ def _fill(c, v, seed):
   return init
 
 
-def run(ops_mod, c, seed=0):
-  v, bufs = layout(c, 'cuda')
-  init = _fill(c, v, seed)
+def launch(ops_mod, c, v):
+  """The case's one launch on the views of layout(c, ...)."""
   if c['mode'] == 'fwd':
     ops_mod.head_fwd(v['x'], v['w'], v.get('b'), c['n_out'], c['K'], raw=v['raw'])
   else:
     act = ACTS[c['act']]
     ops_mod.head_bwd(v['x'], v['w'], v['draw'], c['n_out'], c['K'], dx=v.get('dx'), relu_mask=act == G.RELU,
-                     dw=v['dw'], db=v['db'], dxsum=v.get('dxsum'), dw2=v.get('dw2'), dw_split=c['split'],
+                     dw=v['dw'], db=v.get('db'), dxsum=v.get('dxsum'), dw2=v.get('dw2'), dw_split=c['split'],
                      dx_cols=c['dx_cols'], dx2=v.get('dx2'), act=act if 'z' in v else G.NONE, z=v.get('z'))
+
+
+def run(ops_mod, c, seed=0):
+  v, bufs = layout(c, 'cuda')
+  init = _fill(c, v, seed)
+  launch(ops_mod, c, v)
   torch.cuda.synchronize()
   return v, bufs, init
 
@@ -214,7 +241,7 @@ def verify(c, v, bufs, init):
   split = c['split'] or c['n_out']
   dw_init = torch.cat([init['dw']] + ([init['dw2']] if 'dw2' in init else []), 1)
   ref = H.head_bwd(v['x'], v['w'], v['draw'], act=ACTS[c['act']], z=v.get('z'), dx_cols=c['dx_cols'],
-                   dw_split=split, dw_init=dw_init, db_init=init['db'], dxsum_init=init.get('dxsum'),
+                   dw_split=split, dw_init=dw_init, db_init=init.get('db'), dxsum_init=init.get('dxsum'),
                    want_dx='dx' in v)
   worst = {}
   for name, (val, bound) in ref.items():
@@ -246,6 +273,17 @@ def test_heads_and_colsum_fp64(ops):
       v, bufs, init = run(ops, c, seed=M + K + n)
       verify(c, v, bufs, init)
   _colsum_case(ops, 5000, 256, False)
+
+
+def fp64_launches(ops_mod):
+  """Every launch test_head_case and test_heads_and_colsum_fp64 check against fp64, made through `launch` on
+  uninitialised CPU buffers of the same layout, for the launch-coverage audit (test_launch_coverage_cpu.py)."""
+  cases = list(CASES) + [c for M, K, n in LEGACY_SHAPES
+                         for c in (case('fwd', M, K, n), case('bwd', M, K, n, act='relu'),
+                                   case('bwd', M, K, n, out='params'))]
+  for c in cases:
+    v, _ = layout(c, 'cpu', fill=False)
+    launch(ops_mod, c, v)
 
 
 # ---------------------------------------------------------------------------------------------- coverage
